@@ -1,14 +1,14 @@
-"""CPU model of the z-binned cell grid of the neighbour search (salva_b200/csrc/sph_kernels.cuh: zbin(), zrun()).
+"""CPU model of the sub-divided cell bins of the neighbour search (salva_b200/csrc/sph_kernels.cuh: abin(), arun()).
 
-The CUDA code splits every cell of width h into `zsub` slices along z and cuts each z-run of the 27-cell stencil down to
-the slices within reach of the particle.  The claim that makes this safe — the contact sets stay EXACTLY the reference's
+Row order splits every cell of width h into `sub` slices along x and y and cuts each row of the 27-cell stencil down to the
+slices within reach of the particle.  The claim that makes this safe — the contact sets stay EXACTLY the reference's
 (contacts.rs:285: `(dx*dx + dy*dy) + dz*dz <= h*h` in f32, candidates from the 3 x 3 x 3 cells floor(x / h) +- 1) — is a
-statement about f32 arithmetic, so it is checked here with numpy's IEEE f32 (same division, same floor, directed rounding
-emulated through f64 + nextafter):
+statement about f32 arithmetic, so it is checked here along one axis with numpy's IEEE f32 (same division, same floor,
+directed rounding emulated through f64 + nextafter):
 
-  * zbin is monotone in z and every bin lies inside ONE reference cell (bin // zsub == floor(z / h));
-  * whenever a pair passes the f32 distance test with dx = dy = 0 (the worst case for z) and sits in adjacent reference cells,
-    the partner's bin lies inside the run [lo, hi] the particle scans.
+  * the bin is monotone in the coordinate and every bin lies inside ONE reference cell (bin // sub == floor(v / h));
+  * whenever a pair passes the f32 distance test with the other two components zero (the worst case for this axis) and sits
+    in adjacent reference cells, the partner's bin lies inside the run [lo, hi] the particle scans.
 """
 import numpy as np
 import pytest
@@ -16,14 +16,11 @@ import pytest
 F = np.float32
 
 
-def zbin(z, h, zsub):
-    q = F(z) / F(h)                      # __fdiv_rn
+def abin(v, h, sub):
+    q = F(v) / F(h)                      # __fdiv_rn
     fl = np.floor(q)
-    cz = int(fl)
-    if zsub == 1:
-        return cz
-    sub = int(F(q - fl) * F(zsub))       # q - floor(q) is exact in f32; the product is rounded, hence the clamp
-    return cz * zsub + min(zsub - 1, sub)
+    s = int(F(q - fl) * F(sub))          # q - floor(q) is exact in f32; the product is rounded, hence the clamp
+    return int(fl) * sub + min(sub - 1, s)
 
 
 def _round_dir(x64, up):
@@ -35,65 +32,63 @@ def _round_dir(x64, up):
     return r
 
 
-def zrun(z, h, zsub):
-    cz = int(np.floor(F(z) / F(h)))
-    if zsub == 1:
-        return cz - 1, cz + 1
+def arun(v, h, sub):
+    c = int(np.floor(F(v) / F(h)))
     h_reach = np.nextafter(F(F(h) * F(1.00001)), F(np.inf))      # fill_static_consts(): Consts::h_reach
-    zlo = _round_dir(float(F(z)) - float(h_reach), up=False)      # __fsub_rd
-    zhi = _round_dir(float(F(z)) + float(h_reach), up=True)       # __fadd_ru
-    lo = max(zbin(zlo, h, zsub), (cz - 1) * zsub)
-    hi = min(zbin(zhi, h, zsub), (cz + 2) * zsub - 1)
+    vlo = _round_dir(float(F(v)) - float(h_reach), up=False)      # __fsub_rd
+    vhi = _round_dir(float(F(v)) + float(h_reach), up=True)       # __fadd_ru
+    lo = max(abin(vlo, h, sub), (c - 1) * sub)
+    hi = min(abin(vhi, h, sub), (c + 2) * sub - 1)
     return lo, hi
 
 
-def accepted(zi, zj, h):
-    dz = F(F(zi) - F(zj))
-    return F(dz * dz) <= F(F(h) * F(h))                           # dist2_exact with dx = dy = 0
+def accepted(vi, vj, h):
+    d = F(F(vi) - F(vj))
+    return F(d * d) <= F(F(h) * F(h))                             # dist2_exact with the other two components zero
 
 
-@pytest.mark.parametrize("zsub", [1, 2, 3, 4, 8])
+@pytest.mark.parametrize("sub", [1, 2, 3, 4, 8])
 @pytest.mark.parametrize("h", [0.1, 0.2, 0.37])
-def test_zbin_is_monotone_and_nested_in_the_reference_cells(zsub, h):
-    rng = np.random.default_rng(zsub * 7 + int(h * 100))
-    z = np.sort(np.concatenate([rng.uniform(-40 * h, 40 * h, 4000), (np.arange(-60, 60) * h).astype(np.float64),
+def test_zbin_is_monotone_and_nested_in_the_reference_cells(sub, h):
+    rng = np.random.default_rng(sub * 7 + int(h * 100))
+    v = np.sort(np.concatenate([rng.uniform(-40 * h, 40 * h, 4000), (np.arange(-60, 60) * h).astype(np.float64),
                                 np.nextafter((np.arange(-60, 60) * F(h)).astype(F), F(-np.inf)).astype(np.float64)]).astype(F))
-    bins = np.array([zbin(v, h, zsub) for v in z])
+    bins = np.array([abin(x, h, sub) for x in v])
     assert np.all(np.diff(bins) >= 0)
-    cells = np.floor(z / F(h)).astype(np.int64)
-    assert np.array_equal(np.floor_divide(bins, zsub), cells)
+    cells = np.floor(v / F(h)).astype(np.int64)
+    assert np.array_equal(np.floor_divide(bins, sub), cells)
 
 
-@pytest.mark.parametrize("zsub", [2, 3, 4, 8])
+@pytest.mark.parametrize("sub", [2, 3, 4, 8])
 @pytest.mark.parametrize("h", [0.1, 0.2, 0.37])
-def test_no_accepted_pair_of_adjacent_cells_is_cut_off(zsub, h):
-    rng = np.random.default_rng(zsub * 13 + int(h * 1000))
+def test_no_accepted_pair_of_adjacent_cells_is_cut_off(sub, h):
+    rng = np.random.default_rng(sub * 13 + int(h * 1000))
     checked = near = 0
-    for scale in (1.0, 30.0, 3000.0):                              # far from the origin the f32 grid of z gets coarse
-        zi_all = rng.uniform(-40 * h * scale, 40 * h * scale, 1500).astype(F)
-        for zi in zi_all:
+    for scale in (1.0, 30.0, 3000.0):                              # far from the origin the f32 grid gets coarse
+        vi_all = rng.uniform(-40 * h * scale, 40 * h * scale, 1500).astype(F)
+        for vi in vi_all:
             # partners right at the cutoff (a few ulps either side) and anywhere within reach
-            cands = [F(zi + s * F(h)) for s in (-1.0, 1.0)]
+            cands = [F(vi + s * F(h)) for s in (-1.0, 1.0)]
             for c in list(cands):
-                v = c
+                x = c
                 for _ in range(4):
-                    v = np.nextafter(v, F(np.inf))
-                    cands.append(v)
-                v = c
+                    x = np.nextafter(x, F(np.inf))
+                    cands.append(x)
+                x = c
                 for _ in range(4):
-                    v = np.nextafter(v, F(-np.inf))
-                    cands.append(v)
-            cands += list((zi + rng.uniform(-1.0, 1.0, 6) * h).astype(F))
-            lo, hi = zrun(zi, h, zsub)
-            czi = int(np.floor(F(zi) / F(h)))
-            assert lo <= zbin(zi, h, zsub) <= hi
-            for zj in cands:
-                if not accepted(zi, zj, h):
+                    x = np.nextafter(x, F(-np.inf))
+                    cands.append(x)
+            cands += list((vi + rng.uniform(-1.0, 1.0, 6) * h).astype(F))
+            lo, hi = arun(vi, h, sub)
+            ci = int(np.floor(F(vi) / F(h)))
+            assert lo <= abin(vi, h, sub) <= hi
+            for vj in cands:
+                if not accepted(vi, vj, h):
                     continue
-                czj = int(np.floor(F(zj) / F(h)))
-                if abs(czj - czi) > 1:
+                cj = int(np.floor(F(vj) / F(h)))
+                if abs(cj - ci) > 1:
                     continue                                       # the reference's stencil does not look there either
                 checked += 1
-                near += abs(abs(float(zi) - float(zj)) - h) < 1e-5 * h
-                assert lo <= zbin(zj, h, zsub) <= hi, (zi, zj, lo, hi, zbin(zj, h, zsub))
+                near += abs(abs(float(vi) - float(vj)) - h) < 1e-5 * h
+                assert lo <= abin(vj, h, sub) <= hi, (vi, vj, lo, hi, abin(vj, h, sub))
     assert checked > 10000 and near > 1000
