@@ -889,16 +889,16 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             TDISPATCH1(k_tile_neighbors, multi, sb, cap, w->pos[c].p, w->vel[c].p, w->cstart.p, cap, w->nbr16.p, w->cnt_f.p, maxcnt);
         } else if (w->hc.xysub > 1) {  // row order
             if (multi)
-                LAUNCH((k_neighbors_xy<true>), N, 128, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+                LAUNCH((k_neighbors_xy<true>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
                        w->cnt_f.p, w->cnt_b.p, maxcnt);
             else
-                LAUNCH((k_neighbors_xy<false>), N, 128, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+                LAUNCH((k_neighbors_xy<false>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
                        w->cnt_f.p, w->cnt_b.p, maxcnt);
         } else if (multi) {
-            LAUNCH((k_neighbors<true>), N, 128, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+            LAUNCH((k_neighbors<true>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
                    w->cnt_f.p, w->cnt_b.p, maxcnt);
         } else {
-            LAUNCH((k_neighbors<false>), N, 128, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+            LAUNCH((k_neighbors<false>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
                    w->cnt_f.p, w->cnt_b.p, maxcnt);
         }
         int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous

@@ -531,20 +531,32 @@ __global__ void k_scanK_add(ScanSet<K> io, uint32_t n, ScanSet<K> block_offsets)
 // candidate loop is executed (predicated off) by the whole warp almost every iteration.  The candidate loop therefore
 // only records hits in a 32-bit mask per chunk of 32 candidates; the (short) emit loop then walks the set bits in
 // ascending order, which keeps every list in the same order as a plain scan.
+// BATCH4 issues the candidate loads four at a time into distinct registers (left to itself, ptxas reuses one register
+// quadruple and every load waits for the previous test).  That pays on h-cell runs (~24 candidates); on the ~6-candidate runs of
+// row order the plain unrolled loop is faster (C2 rows: 0.289 vs 0.304 ms per search, H100 80GB HBM3, 700 W, 1980 MHz).
 // ------------------------------------------------------------------------------------------------
-template <class Accept, class Emit>
+template <bool BATCH4, class Accept, class Emit>
 __device__ __forceinline__ void scan_run(const float4& pi, const float4* __restrict__ P, uint32_t s, uint32_t e, Accept accept, Emit emit) {
+    // d2 <= h*h  <=>  the sign bit of (h*h - d2) is clear (a float difference is zero only for equal operands; NaN positions
+    // never get here, k_bounds rejects them): shift that bit into the mask with one funnel shift
+    const auto test = [&](const float4& pj, uint32_t rej) {
+        const float d2 = dist2_exact(pi.x - pj.x, pi.y - pj.y, pi.z - pj.z);
+        return __funnelshift_l(__float_as_uint(__fsub_rn(C.h2, d2)), rej, 1);
+    };
     for (uint32_t base = s; base < e; base += 32u) {
         const uint32_t n = min(32u, e - base);
         const float4* __restrict__ q = P + base;
+        const float4* const qe = q + n;
         uint32_t rej = 0u;  // candidate t of the chunk ends up in bit n - 1 - t; set = rejected
+        if (BATCH4) {
+            for (; q + 4 <= qe; q += 4) {  // the four loads go out back to back, before the first test waits on one
+                const float4 p0 = __ldg(q), p1 = __ldg(q + 1), p2 = __ldg(q + 2), p3 = __ldg(q + 3);
+                rej = test(p3, test(p2, test(p1, test(p0, rej))));
+            }
+            for (; q < qe; ++q) rej = test(__ldg(q), rej);
+        } else {
 #pragma unroll 4
-        for (uint32_t t = 0; t < n; ++t) {
-            const float4 pj = __ldg(&q[t]);
-            const float d2 = dist2_exact(pi.x - pj.x, pi.y - pj.y, pi.z - pj.z);
-            // d2 <= h*h  <=>  the sign bit of (h*h - d2) is clear (a float difference is zero only for equal operands;
-            // NaN positions never get here, k_bounds rejects them): shift that bit into the mask with one funnel shift
-            rej = __funnelshift_l(__float_as_uint(__fsub_rn(C.h2, d2)), rej, 1);
+            for (; q < qe; ++q) rej = test(__ldg(q), rej);
         }
         uint32_t m = ~rej & (n == 32u ? 0xffffffffu : (1u << n) - 1u);
         while (m) {
@@ -556,66 +568,78 @@ __device__ __forceinline__ void scan_run(const float4& pi, const float4* __restr
     }
 }
 
-#ifndef SPH_NBR_RUNPTR
-#define SPH_NBR_RUNPTR 1  // list entries addressed with a running pointer instead of recomputing ((k >> 2) * stride + i) * 4 + (k & 3)
-#endif
-template <bool MULTI>
-__global__ void __launch_bounds__(128)
-k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
-            const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-            uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
-            uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */) {
+// STAGE: the lists are staged per warp in shared memory and written out once the walk is done.  Storing each hit at its final
+// place (((k >> 2) * stride + i) * 4 + (k & 3)) makes every 16-byte group of a list four partial writes spread over the whole
+// kernel, with the lanes of a warp at different k: the sectors being filled (~29 MB at 10M particles) do not fit H100's L2.
+// Staged, entry k of a lane is one STS at row k, column lane (bank-conflict-free whatever k each lane is at); the write-out
+// then stores group g of 32 consecutive particles as 32 x 16 contiguous bytes, and boundary row k as 32 x 4.
+// Entries past the staging rows go straight to their place in global memory, so any cap_f / cap_b works (list regrow
+// included) while the shared-memory size stays fixed.  The row counts trade the share of staged entries against occupancy:
+// 32 + 8 rows (20 KB per block) leave 10 blocks per SM, as many as the registers allow; at C3 (~33 contacts on average,
+// up to ~51) 48 + 16 rows (6 blocks) made the search 26 % slower, 40 + 8 (9 blocks) 1 % slower (DESIGN.md §4a.11).
+// Row order does not stage: the lanes of a warp are consecutive particles of one line and reach their k-th contact nearly
+// together, so the per-hit stores already coalesce and staging only added cost (C2 rows: 0.300 vs 0.289 ms per search).
+constexpr int NBR_T = 128;                   // threads per block of k_neighbors / k_neighbors_xy
+constexpr uint32_t NBR_SF = 32, NBR_SB = 8;  // staged fluid / boundary rows per lane (multiples of 4)
+
+// The search shared by k_neighbors and k_neighbors_xy; `runs(pi, visit)` calls visit(lo) for every z-run of cells the particle
+// has to scan, lo being the cell id (cstart / bstart index) of the run's first cell; a run is always 3 cells.  STAGE (the
+// h-cell search) also batches the candidate loads: both pay on h-cell runs only.
+template <bool MULTI, bool STAGE, class Runs>
+__device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
+                                               const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
+                                               uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f,
+                                               uint32_t* __restrict__ cnt_b, uint32_t* __restrict__ maxcnt, Runs runs) {
+    __shared__ uint32_t stage[NBR_T / 32][NBR_SF + NBR_SB][32];
+    uint32_t(*const sf)[32] = stage[threadIdx.x >> 5];
+    uint32_t(*const sb)[32] = sf + NBR_SF;
+    const uint32_t lane = threadIdx.x & 31u;
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nf = 0, nb = 0;
     const bool owned = i < C.n_owned;
     i += C.i_begin;
     if (owned) {
-        float4 pi = pos[i];
-        uint32_t fi = MULTI ? fid_of(vel[i]) : 0u;
-        int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
-        uint32_t* wp = nbr_f + (size_t)i * 4;                  // slot 0 of group 0 of this particle's column
-        const size_t gstep = (size_t)C.stride * 4 - 4;         // from behind slot 3 of a group to slot 0 of the next one
-        for (int ax = -1; ax <= 1; ++ax)
-            for (int ay = -1; ay <= 1; ++ay) {
-                const int lo = cell_id(cx + ax, cy + ay, cz - 1), hi = lo + 3;  // the z-run of cells cz-1..cz+1
-                scan_run(
-                    pi, pos, cstart[lo], cstart[hi],
-                    [&](uint32_t j) {
-                        if (!MULTI) return true;
-                        uint32_t fj = fid_of(__ldg(&vel[j]));  // contacts.rs:355-362: different fluids need the groups test
-                        return fi == fj || groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.fluids[fj].memberships, C.fluids[fj].filter);
+        const float4 pi = pos[i];
+        const uint32_t fi = MULTI ? fid_of(vel[i]) : 0u;
+        runs(pi, [&](int lo) {
+            scan_run<STAGE>(
+                pi, pos, cstart[lo], cstart[lo + 3],
+                [&](uint32_t j) {
+                    if (!MULTI) return true;
+                    uint32_t fj = fid_of(__ldg(&vel[j]));  // contacts.rs:355-362: different fluids need the groups test
+                    return fi == fj || groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.fluids[fj].memberships, C.fluids[fj].filter);
+                },
+                [&](uint32_t j) {
+                    if (STAGE && nf < NBR_SF) sf[nf][lane] = j;
+                    else if (nf < C.cap_f) nbr_f[((size_t)(nf >> 2) * C.stride + i) * 4 + (nf & 3)] = j;
+                    ++nf;
+                });
+            if (C.n_bound)
+                scan_run<STAGE>(
+                    pi, bpos, bstart[lo], bstart[lo + 3],
+                    [&](uint32_t j) {  // contacts.rs:347-352
+                        uint32_t bj = fid_of(__ldg(&bvel[j]));
+                        return groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.bounds[bj].memberships, C.bounds[bj].filter);
                     },
                     [&](uint32_t j) {
-                        // (one 4-byte store per hit: collecting four hits in registers and storing 16-byte groups was measured
-                        //  SLOWER, 1.66 -> 1.80 ms at C3 — the shift-in costs more issue slots than the stores save)
-                        //  entry k of particle i lives at ((k >> 2) * stride + i) * 4 + (k & 3): walked with a running pointer)
-#if SPH_NBR_RUNPTR
-                        if (nf < C.cap_f) *wp = j;
-                        ++nf;
-                        ++wp;
-                        if ((nf & 3u) == 0u) wp += gstep;
-#else
-                        if (nf < C.cap_f) nbr_f[((size_t)(nf >> 2) * C.stride + i) * 4 + (nf & 3)] = j;
-                        ++nf;
-#endif
+                        if (STAGE && nb < NBR_SB) sb[nb][lane] = j;
+                        else if (nb < C.cap_b) nbr_b[(size_t)nb * C.stride + i] = j;
+                        ++nb;
                     });
-                if (C.n_bound)
-                    scan_run(
-                        pi, bpos, bstart[lo], bstart[hi],
-                        [&](uint32_t j) {  // contacts.rs:347-352
-                            uint32_t bj = fid_of(__ldg(&bvel[j]));
-                            return groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.bounds[bj].memberships, C.bounds[bj].filter);
-                        },
-                        [&](uint32_t j) {
-                            if (nb < C.cap_b) nbr_b[(size_t)nb * C.stride + i] = j;
-                            ++nb;
-                        });
+        });
+        // write-out: the last group is padded with i; cap_f and NBR_SF are multiples of 4, so a staged group is whole
+        if (STAGE) {
+            const uint32_t sfn = min(nf, min(NBR_SF, C.cap_f));
+            uint4* out = reinterpret_cast<uint4*>(nbr_f) + i;
+            for (uint32_t k = 0; k < sfn; k += 4, out += C.stride) {
+                const uint32_t a = sf[k][lane], b = sf[k + 1][lane], c = sf[k + 2][lane], d = sf[k + 3][lane];
+                *out = make_uint4(a, k + 1 < nf ? b : i, k + 2 < nf ? c : i, k + 3 < nf ? d : i);
             }
-#if SPH_NBR_RUNPTR
-        for (uint32_t t = nf; t < ((nf + 3u) & ~3u) && t < C.cap_f; ++t) *wp++ = i;  // pad the last group
-#else
-        for (uint32_t t = nf; t < ((nf + 3u) & ~3u) && t < C.cap_f; ++t) nbr_f[((size_t)(t >> 2) * C.stride + i) * 4 + (t & 3)] = i;
-#endif
+            const uint32_t sbn = min(nb, min(NBR_SB, C.cap_b));
+            for (uint32_t k = 0; k < sbn; ++k) nbr_b[(size_t)k * C.stride + i] = sb[k][lane];
+        }
+        for (uint32_t t = STAGE ? max(nf, NBR_SF) : nf; t < ((nf + 3u) & ~3u) && t < C.cap_f; ++t)  // pad the last group unless staged
+            nbr_f[((size_t)(t >> 2) * C.stride + i) * 4 + (t & 3)] = i;
         cnt_f[i] = nf;
         cnt_b[i] = nb;
     }
@@ -624,75 +648,43 @@ k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, cons
         mf = max(mf, __shfl_xor_sync(0xffffffffu, mf, o));
         mb = max(mb, __shfl_xor_sync(0xffffffffu, mb, o));
     }
-    if ((threadIdx.x & 31) == 0) {
+    if (lane == 0) {
         if (mf) atomicMax(&maxcnt[0], mf);
         if (mb) atomicMax(&maxcnt[1], mb);
     }
 }
 
-// Row order (Consts::xysub > 1): the same search over the bin rows within reach in x and y (5 x 5 rows of width h / 2 at xysub = 2
-// instead of 3 x 3 of width h; arun() clips them to the reference's cells, so the contact sets are the reference's).  A separate kernel so that
-// the default path above stays byte for byte what was validated.
 template <bool MULTI>
-__global__ void __launch_bounds__(128)
+__global__ void __launch_bounds__(NBR_T)
+k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
+            const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
+            uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
+            uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */) {
+    neighbor_lists<MULTI, true>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, [](const float4& pi, auto&& visit) {
+        const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
+        for (int ax = -1; ax <= 1; ++ax)
+            for (int ay = -1; ay <= 1; ++ay) visit(cell_id(cx + ax, cy + ay, cz - 1));  // the z-run of cells cz-1..cz+1
+    });
+}
+
+// Row order (Consts::xysub > 1): the same search over the bin rows within reach in x and y (5 x 5 rows of width h / 2 at xysub = 2
+// instead of 3 x 3 of width h; arun() clips them to the reference's cells, so the contact sets are the reference's).  Neither
+// staged nor batched: see scan_run and NBR_SF.  No __launch_bounds__: with it ptxas holds the MULTI instantiation to 32
+// registers and spills.
+template <bool MULTI>
+__global__ void
 k_neighbors_xy(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
                uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
                uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t nf = 0, nb = 0;
-    const bool owned = i < C.n_owned;
-    i += C.i_begin;
-    if (owned) {
-        float4 pi = pos[i];
-        uint32_t fi = MULTI ? fid_of(vel[i]) : 0u;
+    neighbor_lists<MULTI, false>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         int xlo, xhi, ylo, yhi;
         arun(pi.x, cx, C.xysub, C.xysub_f, xlo, xhi);
         arun(pi.y, cy, C.xysub, C.xysub_f, ylo, yhi);
-        uint32_t* wp = nbr_f + (size_t)i * 4;
-        const size_t gstep = (size_t)C.stride * 4 - 4;
         for (int bx = xlo; bx <= xhi; ++bx)
-            for (int by = ylo; by <= yhi; ++by) {
-                const int lo = cell_id(bx, by, cz - 1), hi = lo + 3;  // the z-run of cells cz-1..cz+1
-                scan_run(
-                    pi, pos, cstart[lo], cstart[hi],
-                    [&](uint32_t j) {
-                        if (!MULTI) return true;
-                        uint32_t fj = fid_of(__ldg(&vel[j]));
-                        return fi == fj || groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.fluids[fj].memberships, C.fluids[fj].filter);
-                    },
-                    [&](uint32_t j) {
-                        if (nf < C.cap_f) *wp = j;
-                        ++nf;
-                        ++wp;
-                        if ((nf & 3u) == 0u) wp += gstep;
-                    });
-                if (C.n_bound)
-                    scan_run(
-                        pi, bpos, bstart[lo], bstart[hi],
-                        [&](uint32_t j) {
-                            uint32_t bj = fid_of(__ldg(&bvel[j]));
-                            return groups_test(C.fluids[fi].memberships, C.fluids[fi].filter, C.bounds[bj].memberships, C.bounds[bj].filter);
-                        },
-                        [&](uint32_t j) {
-                            if (nb < C.cap_b) nbr_b[(size_t)nb * C.stride + i] = j;
-                            ++nb;
-                        });
-            }
-        for (uint32_t t = nf; t < ((nf + 3u) & ~3u) && t < C.cap_f; ++t) *wp++ = i;  // pad the last group
-        cnt_f[i] = nf;
-        cnt_b[i] = nb;
-    }
-    uint32_t mf = nf, mb = nb;
-    for (int o = 16; o > 0; o >>= 1) {
-        mf = max(mf, __shfl_xor_sync(0xffffffffu, mf, o));
-        mb = max(mb, __shfl_xor_sync(0xffffffffu, mb, o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (mf) atomicMax(&maxcnt[0], mf);
-        if (mb) atomicMax(&maxcnt[1], mb);
-    }
+            for (int by = ylo; by <= yhi; ++by) visit(cell_id(bx, by, cz - 1));
+    });
 }
 // boundary volumes in row order: every bin of the 3 x 3 x 3 reference cells around the particle
 __global__ void __launch_bounds__(128)
