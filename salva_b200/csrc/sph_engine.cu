@@ -235,7 +235,7 @@ struct sph_world {
     DBuf<float> ct_w[2], ct_g[2];
     DBuf<uint32_t> d_ticket;      // last-block ticket of the in-kernel error reduction (kept at 0 between launches)
     bool errsum_ready = false;    // the last evaluation launch already reduced its partials into errsum
-    bool fused_first_div = false;  // the first compute_divergences evaluation rode with the density pass
+    bool fused_first_div = false;  // the neighbour search computed rho, alpha and the first compute_divergences evaluation
     bool xs_valid = false;    // XSPH sums rode with the divergence loop's last evaluation (k_vel_divergence_xsph_u)
     DBuf<float4> xs;
     uint32_t fused_nblk = 0;
@@ -516,7 +516,7 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     if (w->tile) CU(w->nbr16.ensure((size_t)w->cap_f * w->stride));
     else CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
     CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
-    uint32_t nblk = cdiv(std::max<size_t>(N, 1), PASS_T);
+    uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
     CU(w->partial.ensure((size_t)(nblk + 3) * std::max<size_t>(1, w->fluids.size())));  // +3: a slab pass may run as three sub-range launches
     CU(w->errsum.ensure(MAX_FLUIDS));
     return SPH_OK;
@@ -859,13 +859,44 @@ sph_status ensure_tex(sph_world* w, cudaTextureObject_t* tex, const void** cur, 
     return SPH_OK;
 }
 
+// Inputs and outputs of the density sweep that the DFSPH neighbour search runs over its fresh lists (density_alpha_div)
+sph_status density_args(sph_world* w, DensArgs* D) {
+    if (w->unimass) {
+        TRY(ensure_tex(w, &w->tex_vyz, &w->tex_vyz_ptr, w->vyz2.p, w->vyz2.cap));
+        TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
+    } else {
+        TRY(ensure_tex(w, &w->tex_vs, &w->tex_vs_ptr, w->vs.p, w->vs.cap));
+    }
+    TRY(slab_wait(w));  // the sweep gathers v* of ghosts
+    *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx : 0, w->vs.p, w->unimass ? 0 : w->tex_vs, w->vyz2.p,
+                  w->unimass ? w->tex_vyz : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, w->d_scal.p + 7};
+    return SPH_OK;
+}
+
 // `speculative` (optional) enqueues the work that follows the neighbour search and only writes scratch (the density
 // pass): it is launched BEFORE the host learns whether the lists overflowed, so the GPU is busy during that round trip;
 // on overflow the lists are rebuilt with a larger capacity and the speculative work is simply enqueued again.
+// With w->fused_first_div (DFSPH, list backend) the search itself computes rho, alpha and the first divergence evaluation
+// (density_alpha_div); on overflow the relaunched search computes them again.
 sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) = nullptr) {
     size_t N = w->N, B = w->B;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
+    const bool dens = w->fused_first_div, uni = dens && w->unimass;
+    DensArgs D{};
+    if (dens) TRY(density_args(w, &D));
+    using NbrKernel = void (*)(const float4*, const float4*, const uint32_t*, const float4*, const float4*, const uint32_t*, uint32_t*,
+                               uint32_t*, uint32_t*, uint32_t*, uint32_t*, DensArgs);
+    NbrKernel search;
+    if (w->hc.xysub > 1) {  // row order
+        if (multi) search = dens ? k_neighbors_xy<true, true, false> : k_neighbors_xy<true, false, false>;
+        else if (dens) search = uni ? k_neighbors_xy<false, true, true> : k_neighbors_xy<false, true, false>;
+        else search = k_neighbors_xy<false, false, false>;
+    } else {
+        if (multi) search = dens ? k_neighbors<true, true, false> : k_neighbors<true, false, false>;
+        else if (dens) search = uni ? k_neighbors<false, true, true> : k_neighbors<false, true, false>;
+        else search = k_neighbors<false, false, false>;
+    }
     if (B) {  // compute_boundary_volumes dfsph_solver.rs:72-96: the reference recomputes them every substep; they only
               // depend on the boundary positions, so they are reused while the boundaries are unchanged
         if (!w->b_reused) {
@@ -887,19 +918,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             uint32_t sb = multi ? 32u : 16u;
             uint32_t cap = tile_cap(w, sb);
             TDISPATCH1(k_tile_neighbors, multi, sb, cap, w->pos[c].p, w->vel[c].p, w->cstart.p, cap, w->nbr16.p, w->cnt_f.p, maxcnt);
-        } else if (w->hc.xysub > 1) {  // row order
-            if (multi)
-                LAUNCH((k_neighbors_xy<true>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-                       w->cnt_f.p, w->cnt_b.p, maxcnt);
-            else
-                LAUNCH((k_neighbors_xy<false>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-                       w->cnt_f.p, w->cnt_b.p, maxcnt);
-        } else if (multi) {
-            LAUNCH((k_neighbors<true>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-                   w->cnt_f.p, w->cnt_b.p, maxcnt);
         } else {
-            LAUNCH((k_neighbors<false>), N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-                   w->cnt_f.p, w->cnt_b.p, maxcnt);
+            LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+                   w->cnt_f.p, w->cnt_b.p, maxcnt, D);
         }
         int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous
         CU(cudaMemcpyAsync(hs, w->d_scal.p + 7, 4 * sizeof(int), cudaMemcpyDeviceToHost, w->st));
@@ -908,7 +929,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
         const bool early = speculative && !w->tile;  // (tile launches need this read-back's slot count)
         if (early) TRY(speculative(w));
         CU(cudaEventSynchronize(w->ev_lists));
-        if (hs[0]) return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
+        // (a zero density of the search's own density sweep is reported with the other zero densities at the end of the step)
+        if (hs[0] & ~ERR_SEARCH_ZERO_DENSITY)
+            return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
         if (w->tile) {
             if ((uint32_t)hs[3] > 65535u)
                 return w->fail(SPH_ERR_INVALID, "tile halo of %d particles exceeds the 16-bit contact index space", hs[3]);
@@ -928,7 +951,7 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             if (speculative && !early) TRY(speculative(w));
             break;
         }
-        if (early) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded speculative pass
+        if (early) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded density pass or sweep
         if (w->tile) CU(w->nbr16.ensure((size_t)w->cap_f * w->stride));
         else CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
         CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
@@ -943,6 +966,10 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
         k_sum_u32<<<std::min<uint32_t>(cdiv(N, 256), 1184), 256, 0, w->st>>>((uint32_t)N, w->cnt_f.p + w->own_begin, w->cnt_b.p + w->own_begin,
                                                                              w->d_cnt.p + 1);
         w->launches++;
+    }
+    if (dens) {
+        w->fused_nblk = cdiv(N, NBR_T);  // one error partial per block, summed by read_error()
+        w->errsum_ready = false;
     }
     CU(cudaGetLastError());
     w->lists_valid = true;
@@ -1038,7 +1065,6 @@ sph_status post_density_refresh(sph_world* w) {
     }
     return slab_refresh(w, w->dens.p, sizeof(float));  // XSPH / artificial viscosity / Akinci gather rho_j of ghosts
 }
-// DFSPH: densities + alphas + the first divergence evaluation in one sweep (k_density_alpha_div)
 // Launch over a slot range with n = range count (kernels index rg.begin + thread)
 #define LAUNCH_R(kern, rg, ...)                                                                   \
     do {                                                                                          \
@@ -1101,36 +1127,6 @@ sph_status run_parts(sph_world* w, const SlabArray* arrays, int n_arrays, uint32
     }
     if (nblk_total) *nblk_total = off;
     return SPH_OK;
-}
-
-// DFSPH: densities + alphas + the first divergence evaluation in one sweep (k_density_alpha_div)
-sph_status launch_density_alpha_div(sph_world* w, uint32_t* nblk) {
-    int c = w->cur, bc = w->bcur;
-    const bool multi = w->fluids.size() > 1;
-    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-    if (w->unimass) {
-        TRY(ensure_tex(w, &w->tex_vyz, &w->tex_vyz_ptr, w->vyz2.p, w->vyz2.cap));
-        TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
-    } else {
-        TRY(ensure_tex(w, &w->tex_vs, &w->tex_vs_ptr, w->vs.p, w->vs.cap));
-    }
-    const size_t nf = std::max<size_t>(1, w->fluids.size());
-    sph_status rs = run_parts(w, nullptr, 0, nblk, [&](Range rg, uint32_t blk) -> sph_status {
-        float* partial = w->partial.p + (size_t)blk * nf;
-        uint32_t* tk = w->single_launch ? w->d_ticket.p : nullptr;
-        if (w->unimass)
-            LAUNCH_R((k_density_alpha_div<false, true>), rg, w->pvx4.p, w->tex_pvx, w->vs.p, (cudaTextureObject_t)0, w->vyz2.p, w->tex_vyz, w->vel[c].p, w->bpos[bc].p, L,
-                     w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, partial, w->d_scal.p + 7, tk, w->errsum.p);
-        else if (multi)
-            LAUNCH_R((k_density_alpha_div<true, false>), rg, w->pos[c].p, (cudaTextureObject_t)0, w->vs.p, w->tex_vs, w->vyz2.p, (cudaTextureObject_t)0, w->vel[c].p, w->bpos[bc].p,
-                     L, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, partial, w->d_scal.p + 7, tk, w->errsum.p);
-        else
-            LAUNCH_R((k_density_alpha_div<false, false>), rg, w->pos[c].p, (cudaTextureObject_t)0, w->vs.p, w->tex_vs, w->vyz2.p, (cudaTextureObject_t)0, w->vel[c].p, w->bpos[bc].p,
-                     L, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, partial, w->d_scal.p + 7, tk, w->errsum.p);
-        return SPH_OK;
-    });
-    w->errsum_ready = w->single_launch;
-    return rs;
 }
 
 // compute_divergences (predict = false) / compute_predicted_densities (predict = true); returns #partials.
@@ -1487,7 +1483,7 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
     uint32_t maxit = w->force_div >= 0 ? (uint32_t)w->force_div + 1 : w->desc.max_divergence_iter;
     for (uint32_t i = 0; i < maxit; ++i) {
         if (i == 0 && w->fused_first_div) {
-            nblk = w->fused_nblk;  // evaluation 0 was computed by k_density_alpha_div
+            nblk = w->fused_nblk;  // evaluation 0 was computed by the neighbour search
         } else {
             TRY(span_begin(w, SP_DIV_EVAL));
             TRY(launch_vel_divergence(w, false, &nblk));
@@ -1629,18 +1625,12 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
         w->lists_valid = false;
     }
     CU(cudaEventRecord(w->ev[EV_GRID], w->st));
-    // evaluate_kernels + compute_densities (liquid_world.rs:123-134) + compute_alphas (dfsph_solver.rs:679-684), enqueued
+    // evaluate_kernels + compute_densities (liquid_world.rs:123-134) + compute_alphas (dfsph_solver.rs:679-684).  DFSPH with the
+    // list backend: computed by the neighbour search itself, together with the first divergence evaluation; otherwise enqueued
     // speculatively by the neighbour phase (EV_NBR is recorded there, between the two)
+    w->fused_first_div = w->N && w->desc.solver == SPH_SOLVER_DFSPH && !w->tile;
     TRY(phase_neighbors(w, [](sph_world* w) -> sph_status {
-        w->fused_first_div = false;
-        if (w->N) {
-            if (w->desc.solver == SPH_SOLVER_DFSPH && !w->tile) {
-                TRY(launch_density_alpha_div(w, &w->fused_nblk));
-                w->fused_first_div = true;
-            } else {
-                TRY(launch_density_alpha(w));
-            }
-        }
+        if (w->N && !w->fused_first_div) TRY(launch_density_alpha(w));
         return SPH_OK;
     }));
     CU(cudaEventRecord(w->ev[EV_DENS], w->st));

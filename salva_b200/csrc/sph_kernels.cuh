@@ -568,6 +568,150 @@ __device__ __forceinline__ void scan_run(const float4& pi, const float4* __restr
     }
 }
 
+// ------------------------------------------------------------------------------------------------
+// K3 + first K4a (DFSPH), run by the neighbour search over the lists it has just built: densities (dfsph_solver.rs:628-665),
+// alphas (dfsph_solver.rs:165-216) and the first compute_divergences evaluation of divergence_solve (dfsph_solver.rs:474-480).
+// That evaluation reads the same neighbour positions and the step-start v* = vel + vc, and needs alpha_i only for
+// kappa_i = div_i * alpha_i at the very end, so it rides along with the density.  The search holds the first NBR_SF / NBR_SB
+// entries of each list in shared memory and the neighbour positions it has just streamed are still in L2, so the lists do not
+// make a round trip through HBM and the step has one neighbour sweep less.  The sweep runs after the walk, whose registers are
+// then dead (the kernel needs the larger of the two register sets, not their sum).  Per quantity the arithmetic and the order
+// of the terms are those of a separate pass: fluid contacts in list order, then boundary contacts in list order.
+// UNI: uniform-mass packed records (positions from pvx4, v* from pvx4.w + vyz2), else pos4 / vs4.
+// ------------------------------------------------------------------------------------------------
+constexpr int NBR_T = 128;                   // threads per block of k_neighbors / k_neighbors_xy
+struct DensArgs {
+    const float4* posrec;                        // pos4, or pvx4 (UNI)
+    cudaTextureObject_t tposrec;                 // UNI: texture over pvx4
+    const float4* vs;                            // v*
+    cudaTextureObject_t tvs;                     // !UNI: texture over vs
+    const float2* vyz;                           // UNI: v*.yz
+    cudaTextureObject_t tvyz;                    // UNI: texture over vyz
+    float *dens, *alpha, *divv, *kappa;
+    float4* pk4;                                 // UNI: (position, kappa)
+    float* partial;                              // per-block error partials: partial[block * n_fluids + f]
+    int* err;                                    // error word: ERR_SEARCH_ZERO_DENSITY
+};
+// The bit a zero density found by the search's density sweep sets in the error word; the other bits come from the boundary
+// volumes (1, checked right after the search) and the ghost exchange (2), so the host can tell the three apart.
+constexpr int ERR_SEARCH_ZERO_DENSITY = 4;
+struct Vel3 {
+    float x, y, z;
+};
+// `group(q)` returns fluid entries 4q .. 4q+3 of particle i, `bentry(k)` boundary entry k; nf / nb are the contact counts.
+// Every thread of the block calls this; `valid` marks the owned ones.  `arrived` counts the block's finished warps and is 0
+// on entry (the caller zeroes it before the walk).
+template <bool MULTI, bool UNI, class Group, class BEntry>
+__device__ __forceinline__ void density_alpha_div(uint32_t i, bool valid, uint32_t nf, uint32_t nb, const float4* __restrict__ vel,
+                                                  const float4* __restrict__ bpos, const DensArgs& D, uint32_t& arrived, Group group,
+                                                  BEntry bentry) {
+    float e = 0.f;
+    uint32_t fi = 0;
+    if (valid) {
+        const float4 a = D.posrec[i];
+        const float4 pi = make_float4(a.x, a.y, a.z, a.w);
+        fi = MULTI ? fid_of(vel[i]) : 0u;
+        const float rho0 = C.fluids[fi].density0;
+        const float umass = C.fluids[0].mass;
+        Vel3 vi;
+        if (UNI) {
+            float2 b = D.vyz[i];
+            vi = Vel3{a.w, b.x, b.y};
+        } else {
+            float4 s = D.vs[i];
+            vi = Vel3{s.x, s.y, s.z};
+        }
+        float rho = 0.f, sq = 0.f, gx = 0.f, gy = 0.f, gz = 0.f, d = 0.f;
+        const uint32_t n = min(nf, C.cap_f);
+        const uint32_t nq = (n + 3u) >> 2;
+        uint4 J = nq ? group(0u) : make_uint4(i, i, i, i);
+        for (uint32_t q = 0; q < nq; ++q) {
+            uint4 Jn = J;
+            if (q + 1 < nq) Jn = group(q + 1);
+            uint32_t j[4] = {J.x, J.y, J.z, J.w};
+            float4 pj[4];
+            Vel3 vj[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                if (q * 4u + u >= n) j[u] = i;  // tail slots of the last group: self (staged rows past n hold stale entries)
+#pragma unroll
+            for (int u = 0; u < 4; ++u) pj[u] = (UNI && (u & 1)) ? tex1Dfetch<float4>(D.tposrec, (int)j[u]) : __ldg(&D.posrec[j[u]]);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (UNI) {  // even contacts: (record via LSU, velocity via TEX), odd ones the other way round
+                    float2 b = (u & 1) ? __ldg(&D.vyz[j[u]]) : tex1Dfetch<float2>(D.tvyz, (int)j[u]);
+                    vj[u] = Vel3{pj[u].w, b.x, b.y};
+                } else {
+                    float4 s = tex1Dfetch<float4>(D.tvs, (int)j[u]);
+                    vj[u] = Vel3{s.x, s.y, s.z};
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                const bool ok = q * 4u + u < n;
+                Pair p = make_pair<true, true>(pi, pj[u]);
+                if (ok) {
+                    const float mj = UNI ? umass : pj[u].w;
+                    rho = fmaf(mj, p.w, rho);
+                    float s = p.g * mj;  // m_j * gradient
+                    float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
+                    sq += ax * ax + ay * ay + az * az;
+                    gx += ax; gy += ay; gz += az;
+                    float dv = (vi.x - vj[u].x) * p.dx + (vi.y - vj[u].y) * p.dy + (vi.z - vj[u].z) * p.dz;
+                    d = fmaf(dv * p.g, mj, d);
+                }
+            }
+            J = Jn;
+        }
+        const uint32_t m = min(nb, C.cap_b);
+        for (uint32_t k = 0; k < m; ++k) {
+            const float4 pj = __ldg(&bpos[bentry(k)]);
+            const Pair p = make_pair<true, true>(pi, pj);
+            float mb = pj.w * rho0;  // boundary pseudo mass: vol_b * rho0_i
+            rho = fmaf(mb, p.w, rho);
+            float s = p.g * mb;
+            float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
+            sq += ax * ax + ay * ay + az * az;
+            gx += ax; gy += ay; gz += az;
+            float dv = vi.x * p.dx + vi.y * p.dy + vi.z * p.dz;  // boundary velocity ignored (dfsph_solver.rs:336-338)
+            d = fmaf(dv * p.g, mb, d);
+        }
+        if (rho == 0.f) atomicOr(D.err, ERR_SEARCH_ZERO_DENSITY);  // assert!(!density.is_zero()) dfsph_solver.rs:662
+        float den = sq + (gx * gx + gy * gy + gz * gz);
+        float al = den <= 1.0e-5f ? 0.f : 1.0f / den;  // dfsph_solver.rs:209-213
+        D.dens[i] = rho;
+        D.alpha[i] = al;
+        if (nf + nb < 20u) d = 0.f;  // min_neighbors_for_divergence_solve :62,301-314
+        d = fmaxf(d, 0.f);
+        D.divv[i] = d;
+        if (UNI) D.pk4[i] = make_float4(a.x, a.y, a.z, d * al);
+        else D.kappa[i] = d * al;
+        e = d / rho0;
+    }
+    // The block's error partial, with block_sum's tree but no block barrier: the walks of a block's warps end at different
+    // times, and a barrier made the finished warps wait for the slowest one (0.3-0.4 ms of the C3 search).  Each warp leaves
+    // its sums in shared memory; the last warp to arrive adds them up.  read_error() sums the block partials.
+    __shared__ float wsum[NBR_T / 32][MAX_FLUIDS];
+    const uint32_t lane = threadIdx.x & 31u;
+    const int nfl = MULTI ? C.n_fluids : 1;
+    for (int f = 0; f < nfl; ++f) {
+        const float s = warp_sum((valid && (!MULTI || fi == (uint32_t)f)) ? e : 0.f);
+        if (lane == 0) wsum[threadIdx.x >> 5][f] = s;
+    }
+    uint32_t last = 0;
+    if (lane == 0) {
+        __threadfence_block();
+        last = atomicAdd(&arrived, 1u) == NBR_T / 32 - 1;
+    }
+    if (__shfl_sync(0xffffffffu, last, 0)) {
+        __threadfence_block();
+        for (int f = 0; f < nfl; ++f) {
+            const float s = warp_sum(lane < NBR_T / 32 ? *(volatile float*)&wsum[lane][f] : 0.f);
+            if (lane == 0) D.partial[(size_t)blockIdx.x * nfl + f] = s;
+        }
+    }
+}
+
 // STAGE: the lists are staged per warp in shared memory and written out once the walk is done.  Storing each hit at its final
 // place (((k >> 2) * stride + i) * 4 + (k & 3)) makes every 16-byte group of a list four partial writes spread over the whole
 // kernel, with the lanes of a warp at different k: the sectors being filled (~29 MB at 10M particles) do not fit H100's L2.
@@ -579,18 +723,23 @@ __device__ __forceinline__ void scan_run(const float4& pi, const float4* __restr
 // up to ~51) 48 + 16 rows (6 blocks) made the search 26 % slower, 40 + 8 (9 blocks) 1 % slower (DESIGN.md §4a.11).
 // Row order does not stage: the lanes of a warp are consecutive particles of one line and reach their k-th contact nearly
 // together, so the per-hit stores already coalesce and staging only added cost (C2 rows: 0.300 vs 0.289 ms per search).
-constexpr int NBR_T = 128;                   // threads per block of k_neighbors / k_neighbors_xy
 constexpr uint32_t NBR_SF = 32, NBR_SB = 8;  // staged fluid / boundary rows per lane (multiples of 4)
 
 // The search shared by k_neighbors and k_neighbors_xy; `runs(pi, visit)` calls visit(lo) for every z-run of cells the particle
 // has to scan, lo being the cell id (cstart / bstart index) of the run's first cell; a run is always 3 cells.  STAGE (the
-// h-cell search) also batches the candidate loads: both pay on h-cell runs only.
-template <bool MULTI, bool STAGE, class Runs>
+// h-cell search) also batches the candidate loads: both pay on h-cell runs only.  DENS: each particle then sweeps its own
+// list with density_alpha_div, reading the staged entries from shared memory and the later ones back from global memory.
+template <bool MULTI, bool STAGE, bool DENS, bool UNI, class Runs>
 __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                                                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
                                                uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f,
-                                               uint32_t* __restrict__ cnt_b, uint32_t* __restrict__ maxcnt, Runs runs) {
+                                               uint32_t* __restrict__ cnt_b, uint32_t* __restrict__ maxcnt, const DensArgs& D, Runs runs) {
     __shared__ uint32_t stage[NBR_T / 32][NBR_SF + NBR_SB][32];
+    __shared__ uint32_t arrived;  // DENS: warps of the block done with their density sweep
+    if (DENS) {
+        if (threadIdx.x == 0) arrived = 0;
+        __syncthreads();  // (before the walk, while the block's warps are still together)
+    }
     uint32_t(*const sf)[32] = stage[threadIdx.x >> 5];
     uint32_t(*const sb)[32] = sf + NBR_SF;
     const uint32_t lane = threadIdx.x & 31u;
@@ -652,15 +801,28 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
         if (mf) atomicMax(&maxcnt[0], mf);
         if (mb) atomicMax(&maxcnt[1], mb);
     }
+    if constexpr (DENS) {
+        const uint4* const col = reinterpret_cast<const uint4*>(nbr_f) + i;
+        density_alpha_div<MULTI, UNI>(
+            i, owned, nf, nb, vel, bpos, D, arrived,
+            [&](uint32_t q) {
+                const uint32_t k = q * 4u;
+                if (STAGE && k < NBR_SF) return make_uint4(sf[k][lane], sf[k + 1][lane], sf[k + 2][lane], sf[k + 3][lane]);
+                return __ldcs(col + (size_t)q * C.stride);  // this thread's own stores above
+            },
+            [&](uint32_t k) { return STAGE && k < NBR_SB ? sb[k][lane] : nbr_b[(size_t)k * C.stride + i]; });
+    }
 }
 
-template <bool MULTI>
-__global__ void __launch_bounds__(NBR_T)
+// DENS: DFSPH's density sweep runs in the search (density_alpha_div).  One fluid: 56 registers (9 blocks per SM).  Several
+// fluids spill at 56 and get 64 (8 blocks); the generic solver kernels spill at 64 and are not bounded.
+template <bool MULTI, bool DENS = false, bool UNI = false>
+__global__ void __launch_bounds__(NBR_T, !DENS || SPH_GENERIC_KERNELS ? 1 : MULTI ? 8 : 9)
 k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
             const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
             uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
-            uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */) {
-    neighbor_lists<MULTI, true>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, [](const float4& pi, auto&& visit) {
+            uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+    neighbor_lists<MULTI, true, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         for (int ax = -1; ax <= 1; ++ax)
             for (int ay = -1; ay <= 1; ++ay) visit(cell_id(cx + ax, cy + ay, cz - 1));  // the z-run of cells cz-1..cz+1
@@ -669,15 +831,15 @@ k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, cons
 
 // Row order (Consts::xysub > 1): the same search over the bin rows within reach in x and y (5 x 5 rows of width h / 2 at xysub = 2
 // instead of 3 x 3 of width h; arun() clips them to the reference's cells, so the contact sets are the reference's).  Neither
-// staged nor batched: see scan_run and NBR_SF.  No __launch_bounds__: with it ptxas holds the MULTI instantiation to 32
-// registers and spills.
-template <bool MULTI>
+// staged nor batched: see scan_run and NBR_SF, so its density sweep reads the lists back from global memory.  No
+// __launch_bounds__: with it ptxas holds the MULTI instantiation to 32 registers and spills.
+template <bool MULTI, bool DENS = false, bool UNI = false>
 __global__ void
 k_neighbors_xy(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
                uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
-               uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */) {
-    neighbor_lists<MULTI, false>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, [](const float4& pi, auto&& visit) {
+               uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+    neighbor_lists<MULTI, false, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         int xlo, xhi, ylo, yhi;
         arun(pi.x, cx, C.xysub, C.xysub_f, xlo, xhi);

@@ -220,108 +220,6 @@ k_density_alpha(const float4* __restrict__ pos, const float4* __restrict__ vel, 
 }
 
 // ------------------------------------------------------------------------------------------------
-// K3 + first K4a fused (DFSPH): densities, alphas AND the first compute_divergences evaluation in ONE gather pass.
-// The first divergence evaluation of divergence_solve (dfsph_solver.rs:474-480) reads the same neighbour positions
-// and the step-start v* = vel + vc, and needs alpha_i only for kappa_i = div_i * alpha_i at the very end, so it can
-// ride along with the density pass: one full neighbour sweep less per step.  Arithmetic per quantity is unchanged.
-// UNI: uniform-mass packed records (positions from pvx4, v* from pvx4.w + vyz2), else pos4 / vs4.
-// ------------------------------------------------------------------------------------------------
-struct Vel3 {
-    float x, y, z;
-};
-template <bool MULTI, bool UNI>
-__global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
-k_density_alpha_div(const float4* __restrict__ posrec /* pos4 or pvx4 */, cudaTextureObject_t tposrec, const float4* __restrict__ vs, cudaTextureObject_t tvs,
-                    const float2* __restrict__ vyz, cudaTextureObject_t tvyz, const float4* __restrict__ vel, const float4* __restrict__ bpos, Lists L,
-                    float* __restrict__ dens, float* __restrict__ alpha, float* __restrict__ divv, float* __restrict__ kappa,
-                    float4* __restrict__ pk4, float* __restrict__ partial, int* __restrict__ err, uint32_t* __restrict__ ticket,
-                    float* __restrict__ errsum, Range rg) {
-    __shared__ float sm[32];
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    bool valid = i < rg.count;
-    i += rg.begin;
-    float e = 0.f;
-    uint32_t fi = 0;
-    if (valid) {
-        const float4 a = posrec[i];
-        const float4 pi = make_float4(a.x, a.y, a.z, a.w);
-        fi = MULTI ? fid_of(vel[i]) : 0u;
-        const float rho0 = C.fluids[fi].density0;
-        const float umass = C.fluids[0].mass;
-        Vel3 vi;
-        if (UNI) {
-            float2 b = vyz[i];
-            vi = Vel3{a.w, b.x, b.y};
-        } else {
-            float4 s = vs[i];
-            vi = Vel3{s.x, s.y, s.z};
-        }
-        float rho = 0.f, sq = 0.f, gx = 0.f, gy = 0.f, gz = 0.f, d = 0.f;
-        const uint32_t n = min(L.cnt_f[i], C.cap_f);
-        const uint32_t nq = (n + 3u) >> 2;
-        const uint4* col = L.nbr_f + i;
-        uint4 J = nq ? ld_list(col) : make_uint4(i, i, i, i);
-        for (uint32_t q = 0; q < nq; ++q) {
-            uint4 Jn = J;
-            if (q + 1 < nq) Jn = ld_list(col + (size_t)(q + 1) * C.stride);
-            const uint32_t j[4] = {J.x, J.y, J.z, J.w};
-            float4 pj[4];
-            Vel3 vj[4];
-#pragma unroll
-            for (int u = 0; u < 4; ++u) pj[u] = (UNI && (u & 1)) ? tex1Dfetch<float4>(tposrec, (int)j[u]) : __ldg(&posrec[j[u]]);  // tail slots point at i itself
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                if (UNI) {  // even contacts: (record via LSU, velocity via TEX), odd ones the other way round
-                    float2 b = (u & 1) ? __ldg(&vyz[j[u]]) : tex1Dfetch<float2>(tvyz, (int)j[u]);
-                    vj[u] = Vel3{pj[u].w, b.x, b.y};
-                } else {
-                    float4 s = tex1Dfetch<float4>(tvs, (int)j[u]);
-                    vj[u] = Vel3{s.x, s.y, s.z};
-                }
-            }
-#pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const bool ok = q * 4u + u < n;
-                Pair p = make_pair<true, true>(pi, pj[u]);
-                if (ok) {
-                    const float mj = UNI ? umass : pj[u].w;
-                    rho = fmaf(mj, p.w, rho);
-                    float s = p.g * mj;  // m_j * gradient
-                    float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
-                    sq += ax * ax + ay * ay + az * az;
-                    gx += ax; gy += ay; gz += az;
-                    float dv = (vi.x - vj[u].x) * p.dx + (vi.y - vj[u].y) * p.dy + (vi.z - vj[u].z) * p.dz;
-                    d = fmaf(dv * p.g, mj, d);
-                }
-            }
-            J = Jn;
-        }
-        for_boundary_contacts<true, true>(i, pi, L, bpos, [&](uint32_t, const Pair& p, const float4& pj) {
-            float mb = pj.w * rho0;  // boundary pseudo mass: vol_b * rho0_i
-            rho = fmaf(mb, p.w, rho);
-            float s = p.g * mb;
-            float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
-            sq += ax * ax + ay * ay + az * az;
-            gx += ax; gy += ay; gz += az;
-            float dv = vi.x * p.dx + vi.y * p.dy + vi.z * p.dz;  // boundary velocity ignored (dfsph_solver.rs:336-338)
-            d = fmaf(dv * p.g, mb, d);
-        });
-        if (rho == 0.f) atomicOr(err, 1);  // assert!(!density.is_zero()) dfsph_solver.rs:662
-        float den = sq + (gx * gx + gy * gy + gz * gz);
-        float al = den <= 1.0e-5f ? 0.f : 1.0f / den;  // dfsph_solver.rs:209-213
-        dens[i] = rho;
-        alpha[i] = al;
-        if (L.cnt_f[i] + L.cnt_b[i] < 20u) d = 0.f;  // min_neighbors_for_divergence_solve :62,301-314
-        d = fmaxf(d, 0.f);
-        divv[i] = d;
-        if (UNI) pk4[i] = make_float4(a.x, a.y, a.z, d * al);
-        else kappa[i] = d * al;
-        e = d / rho0;
-    }
-    reduce_error<MULTI>(e, fi, valid, partial, sm, ticket, errsum);
-}
-
-// ------------------------------------------------------------------------------------------------
 // K4a / K8a: compute_divergences dfsph_solver.rs:279-356 (PREDICT = false) and compute_predicted_densities
 // dfsph_solver.rs:98-162 (PREDICT = true) share one kernel: sum_j m_j (v*_i - v*_j) . gradW_ij.
 //   PREDICT: out = rho*_i, kappa = max((rho* - rho0) alpha, 0), boundary term uses the boundary velocity (:136-141);
