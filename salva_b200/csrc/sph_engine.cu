@@ -220,7 +220,8 @@ struct sph_world {
     bool unimass = false;
     DBuf<float4> pvx4, pk4;
     DBuf<float2> vyz2;
-    bool nr4_valid = false;  // Akinci normals rode with a divergence evaluation (k_vel_divergence_xsph_u<2>)
+    bool nr4_valid = false;     // Akinci normals nr4 = (n, rho) rode with the divergence loop's first update (k_vel_update_u<.., NORMALS>)
+    bool akinci_valid = false;  // ... and the Akinci fluid force with the evaluation after it (k_vel_divergence_xsph_u<2>), in xs
     cudaTextureObject_t tex_pvx = 0, tex_vyz = 0, tex_pk = 0;
     const void* tex_pvx_ptr = nullptr;
     const void* tex_vyz_ptr = nullptr;
@@ -1140,22 +1141,29 @@ bool xsph_fusable(const sph_world* w) {
     const sph_force_desc& d = w->fluids[0].forces[0].d;
     return d.kind == SPH_FORCE_XSPH_VISCOSITY && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0);
 }
-// ... and Akinci2013 normals (k_vel_divergence_xsph_u<2>, one extra 4-byte gather of rho_j): single uniform-mass fluid
+// ... and an Akinci2013SurfaceTension: its normals ride with the loop's first update (k_vel_update_u<.., NORMALS>) and its fluid
+// term with the evaluation after it (k_vel_divergence_xsph_u<2>), when it is the first force of the single uniform-mass fluid
+// and has no boundary term (no adhesion, or no boundaries) and no boundary wants forces.  Otherwise phase_forces computes it.
 bool akinci_fusable_u(const sph_world* w) {
     if (w->desc.solver != SPH_SOLVER_DFSPH || w->tile || !w->unimass || w->slab.active) return false;
-    if (w->fluids.size() != 1) return false;
-    for (const ForceRec& fr : w->fluids[0].forces)
-        if (fr.d.kind == SPH_FORCE_AKINCI2013_TENSION) return true;
-    return false;
+    if (w->fluids.size() != 1 || w->fluids[0].forces.empty()) return false;
+    const sph_force_desc& d = w->fluids[0].forces[0].d;
+    return d.kind == SPH_FORCE_AKINCI2013_TENSION && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0) && !any_bforce(w);
+}
+// Akinci2013 kernel-normalisation constants of `h` (akinci2013_surface_tension.rs): cohesion, its h^6 / 64 offset, adhesion
+struct AkinciNorms {
+    float coh_norm, h6_64, adh_norm;
+};
+AkinciNorms akinci_norms(float h) {
+    return {32.0f / (3.14159265358979323846f * powf(h, 9.f)), powf(h, 6.f) / 64.0f, 0.007f / powf(h, 3.25f)};
 }
 
 sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
     const bool xsf = !predict && xsph_fusable(w);
-    const bool akf = !predict && !xsf && akinci_fusable_u(w);
-    if (xsf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
-    if (akf) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
+    const bool akf = !predict && w->nr4_valid && !w->akinci_valid;  // the first evaluation after the normals-carrying update
+    if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
     if (w->tile) {
         TileLists L{w->nbr16.p, w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
         uint32_t cap = tile_cap(w, 32);
@@ -1186,12 +1194,13 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
             } else if (xsf) {
                 const float cf = w->fluids[0].forces[0].d.p[0];
                 LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, tk, w->errsum.p, w->xs.p, cf);
+                         w->pk4.p, partial, tk, w->errsum.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
                 w->xs_valid = true;
-            } else if (akf) {  // Akinci normals ride along: nr4 = (n, rho) for k_akinci_force_u
+            } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
+                const AkinciNorms an = akinci_norms(w->h);
                 LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, tk, w->errsum.p, w->normals.p, 0.f);
-                w->nr4_valid = true;
+                         w->pk4.p, partial, tk, w->errsum.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
+                w->akinci_valid = true;
             } else {
                 LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
                          w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
@@ -1205,8 +1214,9 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
     w->errsum_ready = w->single_launch;
     return rs;
 }
-// compute_velocity_changes_for_divergence (pressure = false) / compute_velocity_changes (pressure = true)
-sph_status launch_vel_update(sph_world* w, bool pressure) {
+// compute_velocity_changes_for_divergence (pressure = false) / compute_velocity_changes (pressure = true).
+// normals: the Akinci normals ride along (see akinci_fusable_u).
+sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
     if (w->tile) {
@@ -1222,13 +1232,20 @@ sph_status launch_vel_update(sph_world* w, bool pressure) {
     }
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) TRY(ensure_tex(w, &w->tex_pk, &w->tex_pk_ptr, w->pk4.p, w->pk4.cap));
+    if (normals) {
+        CU(w->normals.ensure(std::max(w->Ntot, w->N)));
+        w->nr4_valid = true;
+    }
     // the following evaluation gathers v*_j of ghosts (vs itself too: the velocity fold reads vel = v* for ghosts)
     SlabArray a[3] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}, {w->vs.p, sizeof(float4)}};
     SlabArray a1[1] = {{w->vs.p, sizeof(float4)}};
     return run_parts(w, w->unimass ? a : a1, w->unimass ? 3 : 1, nullptr, [&](Range rg, uint32_t) -> sph_status {
-        if (w->unimass)
+        if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
+            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
+                     w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
+        else if (w->unimass)
             DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
-                      w->vyz2.p, w->bforce.p, w->inv_dt, rg);
+                      w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr, rg);
         else
             BOOL3(k_vel_update, multi, bf, pressure, rg, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p, w->bforce.p, w->inv_dt);
         return SPH_OK;
@@ -1380,11 +1397,10 @@ sph_status phase_forces(sph_world* w) {
                               w->bforce.p, (uint32_t)f, p[0], p[1], p[2], p[3], p[4]);
                     break;
                 case SPH_FORCE_AKINCI2013_TENSION: {
+                    if (w->akinci_valid && &fr == &w->fluids[0].forces[0]) break;  // in xs, folded in by the fold pass
                     CU(w->normals.ensure(std::max(w->Ntot, w->N)));
-                    float h = w->h;
-                    float coh_norm = 32.0f / (3.14159265358979323846f * powf(h, 9.f));
-                    float h6_64 = powf(h, 6.f) / 64.0f;
-                    float adh_norm = 0.007f / powf(h, 3.25f);
+                    const AkinciNorms an = akinci_norms(w->h);
+                    const float coh_norm = an.coh_norm, h6_64 = an.h6_64, adh_norm = an.adh_norm;
                     if (w->tile) {
                         uint32_t sb1 = multi ? 36u : 20u, sb2 = multi ? 52u : 36u;
                         uint32_t cap1 = tile_cap(w, sb1), cap2 = tile_cap(w, sb2);
@@ -1394,7 +1410,7 @@ sph_status phase_forces(sph_world* w) {
                                    w->normals.p, w->acc.p, w->bforce.p, (uint32_t)f, p[0], p[1], coh_norm, h6_64, adh_norm);
                         break;
                     }
-                    if (w->nr4_valid && f == 0) {  // normals (and rho, in .w) came with a divergence evaluation
+                    if (w->nr4_valid && f == 0) {  // normals (and rho, in .w) came with the first divergence update
                         TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
                         if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
                         else LAUNCH((k_akinci_force_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
@@ -1479,7 +1495,8 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
     // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step)
     w->stats.n_divergence_iter = w->stats.n_divergence_eval = 0;
     w->xs_valid = false;
-    w->nr4_valid = false;
+    w->nr4_valid = w->akinci_valid = false;
+    const bool akf = akinci_fusable_u(w);
     uint32_t maxit = w->force_div >= 0 ? (uint32_t)w->force_div + 1 : w->desc.max_divergence_iter;
     for (uint32_t i = 0; i < maxit; ++i) {
         if (i == 0 && w->fused_first_div) {
@@ -1505,7 +1522,7 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
         }
         if (!(i == 0 && w->fused_first_div)) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts
         TRY(span_begin(w, SP_DIV_UPD));
-        TRY(launch_vel_update(w, false));
+        TRY(launch_vel_update(w, false, akf && i == 0));
         TRY(span_end(w));
         w->xs_valid = false;  // v* moved on: XSPH sums of the evaluation above are stale unless another evaluation follows
         w->stats.n_divergence_iter++;
@@ -1513,23 +1530,24 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
     CU(cudaEventRecord(w->ev[EV_DIV], w->st));
     // update_velocities :422-430, zero vc :689-691, acc += gravity :574-578
     TRY(slab_wait(w));
-    // nothing to launch in the force phase (no plugin at all, or only the XSPH whose sums rode with the divergence loop)?  Then
-    // fold, acceleration and integration are one streaming pass
+    // the first force of fluid 0 may already sit in xs: the XSPH sums of the loop's last evaluation (acc = g + xs * inv_dt) or
+    // the Akinci fluid force (acc = g + xs; a scale of 1 leaves the product exact)
+    const bool folded = w->xs_valid || w->akinci_valid;
+    const float4* xs = folded ? w->xs.p : nullptr;
+    const float xs_scale = w->akinci_valid ? 1.0f : w->inv_dt;
+    // nothing (else) to launch in the force phase?  Then fold, acceleration and integration are one streaming pass
     bool quiet_forces = true;
     for (size_t f = 0; f < w->fluids.size() && quiet_forces; ++f)
         for (const ForceRec& fr : w->fluids[f].forces)
-            if (!(w->xs_valid && f == 0 && &fr == &w->fluids[0].forces[0] && fr.d.kind == SPH_FORCE_XSPH_VISCOSITY)) quiet_forces = false;
+            if (!(folded && f == 0 && &fr == &w->fluids[0].forces[0])) quiet_forces = false;
     if (quiet_forces) {
-        const float inv_dt_old = w->inv_dt;
         CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
         CU(cudaEventRecord(w->ev[EV_FORCES], w->st));
         timestep_advance(w, dt_total);  // :702
-        LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2],
-               w->xs_valid ? (const float4*)w->xs.p : (const float4*)nullptr, inv_dt_old, w->dt, w->unimass ? w->pvx4.p : nullptr,
-               w->unimass ? w->vyz2.p : nullptr);
+        LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale, w->dt,
+               w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
     } else {
-        LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2],  // ghosts too (vel = v*)
-               w->xs_valid ? (const float4*)w->xs.p : (const float4*)nullptr, w->inv_dt);
+        LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale);  // ghosts too (vel = v*)
         CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
         TRY(phase_forces(w));
         CU(cudaEventRecord(w->ev[EV_FORCES], w->st));

@@ -988,10 +988,11 @@ __global__ void k_make_vstar(const float4* __restrict__ vel, const float4* __res
 // a10: update_velocities dfsph_solver.rs:422-430 + zero vc :689-691 + acc = gravity (predict_advection :574-578).
 // vel += vc is written as vel = v*: v* was materialised as vel + vc by the producer, so the result is bitwise the
 // same for owned particles, and ghost particles (multi-GPU) only carry an up-to-date v*.
-// xs (optional): XSPH sums of the divergence loop's last evaluation (k_vel_divergence_xsph_u): acc = g + xs * inv_dt,
-// rounded like k_force_xsph's `acc += f * inv_dt` on top of the gravity written here.
+// xs (optional): a force sum of the divergence loop (k_vel_divergence_xsph_u): acc = g + xs * scale, rounded like the force
+// pass's `acc += f * scale` on top of the gravity written here.  XSPH sums: scale = inv_dt; the Akinci force: scale = 1, so
+// acc = g + f exactly as `acc = g; acc += f`.
 __global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__ vc, const float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
-                                  float gz, const float4* __restrict__ xs, float inv_dt) {
+                                  float gz, const float4* __restrict__ xs, float scale) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
     float4 v = vel[i], s = vs[i];
@@ -1000,17 +1001,17 @@ __global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__
     float ax = gx, ay = gy, az = gz;
     if (xs) {
         float4 f = xs[i];
-        ax = __fadd_rn(gx, __fmul_rn(f.x, inv_dt));
-        ay = __fadd_rn(gy, __fmul_rn(f.y, inv_dt));
-        az = __fadd_rn(gz, __fmul_rn(f.z, inv_dt));
+        ax = __fadd_rn(gx, __fmul_rn(f.x, scale));
+        ay = __fadd_rn(gy, __fmul_rn(f.y, scale));
+        az = __fadd_rn(gz, __fmul_rn(f.z, scale));
     }
     acc[i] = make_float4(ax, ay, az, 0.f);
 }
-// update_velocities + the gravity / folded-XSPH acceleration + integrate_and_clear_accelerations in ONE pass, for steps whose force
-// phase launches nothing (no plugin, or only the XSPH whose sums rode with the divergence loop): same arithmetic, in the same
+// update_velocities + the gravity / folded-force acceleration + integrate_and_clear_accelerations in ONE pass, for steps whose force
+// phase launches nothing (no plugin, or only the force whose sum rode with the divergence loop): same arithmetic, in the same
 // order, as k_fold_velocities followed by k_integrate_acc.  Ghost slots (multi-GPU) only take the fold part.
 __global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ vc, float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
-                                 float gz, const float4* __restrict__ xs, float inv_dt_old, float dt_new, float4* __restrict__ pvx, float2* __restrict__ vyz) {
+                                 float gz, const float4* __restrict__ xs, float scale, float dt_new, float4* __restrict__ pvx, float2* __restrict__ vyz) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
     const float4 v = vel[i], s = vs[i];
@@ -1020,9 +1021,9 @@ __global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ 
     float ax = gx, ay = gy, az = gz;
     if (xs) {
         const float4 f = xs[i];
-        ax = __fadd_rn(gx, __fmul_rn(f.x, inv_dt_old));
-        ay = __fadd_rn(gy, __fmul_rn(f.y, inv_dt_old));
-        az = __fadd_rn(gz, __fmul_rn(f.z, inv_dt_old));
+        ax = __fadd_rn(gx, __fmul_rn(f.x, scale));
+        ay = __fadd_rn(gy, __fmul_rn(f.y, scale));
+        az = __fadd_rn(gz, __fmul_rn(f.z, scale));
     }
     acc[i] = make_float4(ax, ay, az, 0.f);
     if (!owned) {

@@ -82,8 +82,11 @@ __device__ __forceinline__ void for_fluid_contacts_g(uint32_t i, const float4& p
 // (A deeper software pipeline — gathers one group ahead — needs 80-96 registers, which halves the occupancy.)
 // The gradient scalar g_ij = W'(|x_ij|)/|x_ij| is recomputed from the positions in every pass.
 // No tail masking: padded slots are (j = i, g = 0) and a self contact has zero gradient either way.
-template <bool NEED_W = false, class LP, class LD, class FF>
+// BATCH = 2: a group's gathers are issued two contacts at a time, for passes whose per-contact records do not fit 64 registers
+// four at a time.
+template <bool NEED_W = false, int BATCH = 4, class LP, class LD, class FF>
 __device__ __forceinline__ void for_fluid_grads(uint32_t i, const float4& pi, const Lists& L, LP ldpos, LD ld, FF ff) {
+    static_assert(BATCH == 2 || BATCH == 4, "a group of four contacts is split into whole batches");
     const uint32_t n = min(L.cnt_f[i], C.cap_f);
     const uint32_t nq = (n + 3u) >> 2;
     if (nq == 0) return;
@@ -93,16 +96,19 @@ __device__ __forceinline__ void for_fluid_grads(uint32_t i, const float4& pi, co
         uint4 Jn = J;
         if (q + 1 < nq) Jn = ld_list(col + (size_t)(q + 1) * C.stride);  // fetch the next group early
         const uint32_t j[4] = {J.x, J.y, J.z, J.w};
-        float4 pj[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) pj[u] = call_gather(ldpos, j[u], u);
-        decltype(call_gather(ld, 0u, 0)) aux[4];
+        for (int u0 = 0; u0 < 4; u0 += BATCH) {
+            float4 pj[BATCH];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) aux[u] = call_gather(ld, j[u], u);
+            for (int u = 0; u < BATCH; ++u) pj[u] = call_gather(ldpos, j[u0 + u], u0 + u);
+            decltype(call_gather(ld, 0u, 0)) aux[BATCH];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            Pair p = make_pair<NEED_W, true>(pi, pj[u]);
-            ff(j[u], p, pj[u], aux[u]);
+            for (int u = 0; u < BATCH; ++u) aux[u] = call_gather(ld, j[u0 + u], u0 + u);
+#pragma unroll
+            for (int u = 0; u < BATCH; ++u) {
+                Pair p = make_pair<NEED_W, true>(pi, pj[u]);
+                ff(j[u0 + u], p, pj[u], aux[u]);
+            }
         }
         J = Jn;
     }
@@ -385,26 +391,52 @@ k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, con
     reduce_error<false>(e, 0u, valid, partial, sm, ticket, errsum);
 }
 
-// compute_divergences (a7) + the fluid term of XSPHViscosity::solve (a12, xsph_viscosity.rs:52-69) in ONE sweep.
-// XSPH is evaluated on `fluid.velocities` right after update_velocities folded vc into them (dfsph_solver.rs:688-697),
-// i.e. on exactly the v* the divergence loop's LAST evaluation gathers; so every stand-alone evaluation also accumulates
-// the XSPH sums (one extra 4-byte gather of rho_j and the kernel value per contact) and the last one's are used:
-// k_fold_velocities adds xs * inv_dt to the gravity it writes and the separate XSPH pass is skipped.  Same per-contact
-// arithmetic and summation order as k_force_xsph; padded self slots contribute c * (v_i - v_i) = 0.
-struct VyzRho {
+// One fluid-fluid contact of Akinci2013SurfaceTension::solve (akinci2013_surface_tension.rs:113-192): the cohesion and
+// curvature terms of neighbour j (mass mj, normal nj, density rho_j) added to a.  Every list-backend Akinci force pass goes
+// through it, so the separate passes and the one fused with a divergence evaluation round alike.
+__device__ __forceinline__ void akinci_contact(const Pair& p, const float4& ni, float rho_i, const float4& nj, float rho_j, float mj, float gamma,
+                                               float rho0, float coh_norm, float h6_64, float& ax, float& ay, float& az) {
+    // cohesion_vec = dir * C(dist) if |dpos|^2 > eps^2 (Unit::try_new_and_get)
+    float coh = p.d2 > F32_EPS * F32_EPS ? cohesion_kernel(p.r, coh_norm, h6_64) / p.r : 0.f;
+    float cm = coh * (-gamma * mj);
+    float kij = 2.0f * rho0 / (rho_i + rho_j);
+    ax += (-gamma * (ni.x - nj.x) + cm * p.dx) * kij;
+    ay += (-gamma * (ni.y - nj.y) + cm * p.dy) * kij;
+    az += (-gamma * (ni.z - nj.z) + cm * p.dz) * kij;
+}
+
+// compute_divergences (a7) + the fluid term of a force in ONE sweep.
+// EXTRA = 1: XSPHViscosity::solve (a12, xsph_viscosity.rs:52-69).  XSPH is evaluated on `fluid.velocities` right after
+// update_velocities folded vc into them (dfsph_solver.rs:688-697), i.e. on exactly the v* the divergence loop's LAST
+// evaluation gathers; so every stand-alone evaluation also accumulates the XSPH sums (one extra 4-byte gather of rho_j and
+// the kernel value per contact) into xs and the last one's are used: k_fold_velocities adds xs * inv_dt to the gravity it
+// writes and the separate XSPH pass is skipped.  Same per-contact arithmetic and summation order as k_force_xsph; padded self
+// slots contribute c * (v_i - v_i) = 0.
+// EXTRA = 2: the fluid term of Akinci2013SurfaceTension::solve.  It needs positions, densities and the normals only, none of
+// which the divergence loop changes, so the first stand-alone evaluation after k_vel_update_u<.., NORMALS> wrote
+// nr4 = (n, rho) computes it (one 16-byte gather of nr4_j per contact instead of rho_j) and it stays valid whatever follows:
+// xs = the force sum, which the fold adds to the gravity.  Same per-contact arithmetic (akinci_contact) and order as
+// k_akinci_force_u.  The padded self slots of the last group are not masked here, but their term is exactly +0: d2 = 0 gives
+// no cohesion and n_i - n_i = 0.
+template <int EXTRA>
+struct EvalAux;
+template <>
+struct EvalAux<1> {
     float2 v;
     float rho;
 };
-// EXTRA = 1: XSPH sums (above) -> xs.   EXTRA = 2: Akinci2013 compute_normals (akinci2013_surface_tension.rs:43-68) rides along
-// instead: n_i = h sum_j (m_j / rho_j) grad W_ij needs positions and densities only, so ANY stand-alone evaluation of the
-// step may produce it; the output record nr4 = (n_x, n_y, n_z, rho_i) is what k_akinci_force_u gathers (one float4 instead
-// of a normal and a density), and the separate normals pass is skipped.
+template <>
+struct EvalAux<2> {
+    float2 v;
+    float4 n;
+};
 template <int EXTRA>
 __global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)  // 64 registers: the extra sums spill at 56
 k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float2* __restrict__ vyz, cudaTextureObject_t tvyz,
                         const float4* __restrict__ bpos, Lists L, const float* __restrict__ dens, const float* __restrict__ alpha,
                         float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, uint32_t* __restrict__ ticket,
-                        float* __restrict__ errsum, float4* __restrict__ xs, float cf, Range rg) {
+                        float* __restrict__ errsum, float4* __restrict__ xs, float cf, const float4* __restrict__ nr4, float coh_norm,
+                        float h6_64, Range rg) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     bool valid = i < rg.count;
@@ -417,19 +449,25 @@ k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx
         const float vix = a.w, viy = b.x, viz = b.y;
         const float rho0 = C.fluids[0].density0, mass = C.fluids[0].mass;
         const bool gated = L.cnt_f[i] + L.cnt_b[i] < 20u;  // dfsph_solver.rs:301-314
+        float4 ni;
+        if (EXTRA == 2) ni = nr4[i];
         float d = 0.f, fx = 0.f, fy = 0.f, fz = 0.f;
-        for_fluid_grads<EXTRA == 1>(
+        // EXTRA = 2 holds 40 bytes of records per contact: gathered four contacts at a time they spill at 64 registers
+        for_fluid_grads<EXTRA == 1, EXTRA == 1 ? 4 : 2>(
             i, pi, L, [&](uint32_t j, int u) { return !(u & 1) ? tex1Dfetch<float4>(tpvx, (int)j) : __ldg(&pvx[j]); },
-            [&](uint32_t j, int u) { return VyzRho{!(u & 1) ? __ldg(&vyz[j]) : tex1Dfetch<float2>(tvyz, (int)j), __ldg(&dens[j])}; },
-            [&](uint32_t, const Pair& p, const float4& pj, const VyzRho& wj) {
+            [&](uint32_t j, int u) {
+                const float2 v = !(u & 1) ? __ldg(&vyz[j]) : tex1Dfetch<float2>(tvyz, (int)j);
+                if constexpr (EXTRA == 1) return EvalAux<1>{v, __ldg(&dens[j])};
+                else return EvalAux<2>{v, __ldg(&nr4[j])};
+            },
+            [&](uint32_t, const Pair& p, const float4& pj, const EvalAux<EXTRA>& wj) {
                 float dv = (vix - pj.w) * p.dx + (viy - wj.v.x) * p.dy + (viz - wj.v.y) * p.dz;
                 d = fmaf(dv * p.g, mass, d);
-                if (EXTRA == 1) {
+                if constexpr (EXTRA == 1) {
                     float c = cf * p.w * mass / wj.rho;  // coeff * W * (vol_j * rho0) / rho_j
                     fx = fmaf(c, pj.w - vix, fx); fy = fmaf(c, wj.v.x - viy, fy); fz = fmaf(c, wj.v.y - viz, fz);
                 } else {
-                    float c = p.g * (mass / wj.rho);
-                    fx = fmaf(c, p.dx, fx); fy = fmaf(c, p.dy, fy); fz = fmaf(c, p.dz, fz);
+                    akinci_contact(p, ni, ni.w, wj.n, wj.n.w, mass, cf, rho0, coh_norm, h6_64, fx, fy, fz);
                 }
             });
         if (gated) {
@@ -444,15 +482,15 @@ k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx
         out[i] = d;
         e = d / rho0;
         pk4[i] = make_float4(a.x, a.y, a.z, d * alpha[i]);
-        if (EXTRA == 1) xs[i] = make_float4(fx, fy, fz, 0.f);
-        else xs[i] = make_float4(fx * C.h, fy * C.h, fz * C.h, dens[i]);
+        xs[i] = make_float4(fx, fy, fz, 0.f);
     }
     reduce_error<false>(e, 0u, valid, partial, sm, ticket, errsum);
 }
 
-// a14 pass 2 for a single uniform-mass fluid on the records of the fused pass: positions from pvx4 (texture pipe) and
-// nr4 = (n_x, n_y, n_z, rho) (LSU pipe): two gathers per contact instead of three.  Akinci2013SurfaceTension::solve
-// akinci2013_surface_tension.rs:113-192.
+// a14 pass 2 for a single uniform-mass fluid on the normals record of k_vel_update_u<.., NORMALS>: positions from pvx4
+// (texture pipe) and nr4 = (n_x, n_y, n_z, rho) (LSU pipe): two gathers per contact instead of three.  Runs when no
+// evaluation followed that update, or when the boundary term or boundary forces keep the force out of the evaluation.
+// Akinci2013SurfaceTension::solve akinci2013_surface_tension.rs:113-192.
 template <bool BFORCE>
 __global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)
 k_akinci_force_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float4* __restrict__ nr4, const float4* __restrict__ bpos, Lists L,
@@ -468,13 +506,7 @@ k_akinci_force_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const
         for_fluid_contacts_g<false, false>(
             i, pi, L, [&](uint32_t j) { return tex1Dfetch<float4>(tpvx, (int)j); }, [&](uint32_t j) { return __ldg(&nr4[j]); },
             [&](uint32_t, const Pair& p, const float4&, const float4& nj) {
-                // cohesion_vec = dir * C(dist) if |dpos|^2 > eps^2 (Unit::try_new_and_get)
-                float coh = p.d2 > F32_EPS * F32_EPS ? cohesion_kernel(p.r, coh_norm, h6_64) / p.r : 0.f;
-                float cm = coh * (-gamma * mass);
-                float kij = 2.0f * rho0 / (rho_i + nj.w);
-                ax += (-gamma * (ni.x - nj.x) + cm * p.dx) * kij;
-                ay += (-gamma * (ni.y - nj.y) + cm * p.dy) * kij;
-                az += (-gamma * (ni.z - nj.z) + cm * p.dz) * kij;
+                akinci_contact(p, ni, rho_i, nj, nj.w, mass, gamma, rho0, coh_norm, h6_64, ax, ay, az);
             });
     if (adh != 0.f)
         for_boundary_contacts<false, false>(i, pi, L, bpos, [&](uint32_t j, const Pair& p, const float4& pj) {
@@ -494,11 +526,15 @@ k_akinci_force_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const
 
 // The (x, y, z, kappa) gathers of every group of four contacts: contacts 0 and 2 through the texture pipe, 1 and 3 through the
 // LSU pipe, so both L1TEX front ends carry half the wavefronts.
-template <bool BFORCE, bool PRESSURE>
-__global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
+// NORMALS: Akinci2013 compute_normals (akinci2013_surface_tension.rs:43-68) rides along: n_i = h sum_j (m_j / rho_j) grad W_ij
+// needs positions and this step's final densities only, so the divergence loop's first update gathers rho_j too (4 bytes per
+// contact) and writes nr4 = (n_x, n_y, n_z, rho_i), the record the Akinci force passes gather (one float4 instead of a normal
+// and a density).  Same arithmetic and order as k_akinci_normals; self slots have zero gradient.
+template <bool BFORCE, bool PRESSURE, bool NORMALS = false>
+__global__ void __launch_bounds__(PASS_T, NORMALS && SPH_GENERIC_KERNELS ? SPH_FORCE_MINB : SPH_PASS_MINB)  // generic kernels: spills at 56
 k_vel_update_u(const float4* __restrict__ pk4, cudaTextureObject_t tpk, const float4* __restrict__ vel, const float4* __restrict__ bpos, Lists L,
                float4* __restrict__ vc, float4* __restrict__ vs, float4* __restrict__ pvx, float2* __restrict__ vyz, float* __restrict__ bforce,
-               float inv_dt, Range rg) {
+               float inv_dt, const float* __restrict__ dens, float4* __restrict__ nr4, Range rg) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rg.count) return;
     i += rg.begin;
@@ -508,13 +544,22 @@ k_vel_update_u(const float4* __restrict__ pk4, cudaTextureObject_t tpk, const fl
     const float4 v = vel[i];
     const float rho0 = C.fluids[0].density0, mass = C.fluids[0].mass;
     const float scale = (PRESSURE ? inv_dt : 1.0f) * mass;
-    float ax = 0.f, ay = 0.f, az = 0.f;
+    float ax = 0.f, ay = 0.f, az = 0.f, nx = 0.f, ny = 0.f, nz = 0.f;
     for_fluid_grads(
-        i, pi, L, [&](uint32_t j, int u) { return !(u & 1) ? tex1Dfetch<float4>(tpk, (int)j) : __ldg(&pk4[j]); }, [](uint32_t) { return NoAux{}; },
-        [&](uint32_t, const Pair& p, const float4& pj, NoAux) {
+        i, pi, L, [&](uint32_t j, int u) { return !(u & 1) ? tex1Dfetch<float4>(tpk, (int)j) : __ldg(&pk4[j]); },
+        [&](uint32_t j) {
+            if constexpr (NORMALS) return __ldg(&dens[j]);
+            else return NoAux{};
+        },
+        [&](uint32_t, const Pair& p, const float4& pj, auto rho_j) {
             float c = (ki + pj.w) * scale * p.g;
             ax = fmaf(c, p.dx, ax); ay = fmaf(c, p.dy, ay); az = fmaf(c, p.dz, az);
+            if constexpr (NORMALS) {
+                float cn = p.g * (mass / rho_j);
+                nx = fmaf(cn, p.dx, nx); ny = fmaf(cn, p.dy, ny); nz = fmaf(cn, p.dz, nz);
+            }
         });
+    if (NORMALS) nr4[i] = make_float4(nx * C.h, ny * C.h, nz * C.h, dens[i]);
     if (!PRESSURE || ki > 0.f) {
         const float bscale = PRESSURE ? inv_dt : 1.0f;
         for_boundary_contacts<false, true>(i, pi, L, bpos, [&](uint32_t j, const Pair& p, const float4& pj) {
@@ -677,13 +722,7 @@ k_akinci_force(const float4* __restrict__ pos, const float4* __restrict__ vel, c
             i, pi, L, pos, [&](uint32_t j) { return NrmRho{__ldg(&normals[j]), __ldg(&dens[j]), MULTI ? fid_of(__ldg(&vel[j])) : 0u}; },
             [&](uint32_t, const Pair& p, const float4& pj, const NrmRho& a) {
                 if (MULTI && a.fid != which) return;
-                // cohesion_vec = dir * C(dist) if |dpos|^2 > eps^2 (Unit::try_new_and_get)
-                float coh = p.d2 > F32_EPS * F32_EPS ? cohesion_kernel(p.r, coh_norm, h6_64) / p.r : 0.f;
-                float cm = coh * (-gamma * pj.w);
-                float kij = 2.0f * rho0 / (rho_i + a.rho);
-                ax += (-gamma * (ni.x - a.n.x) + cm * p.dx) * kij;
-                ay += (-gamma * (ni.y - a.n.y) + cm * p.dy) * kij;
-                az += (-gamma * (ni.z - a.n.z) + cm * p.dz) * kij;
+                akinci_contact(p, ni, rho_i, a.n, a.rho, pj.w, gamma, rho0, coh_norm, h6_64, ax, ay, az);
             });
     if (adh != 0.f)
         for_boundary_contacts<false, false>(i, pi, L, bpos, [&](uint32_t j, const Pair& p, const float4& pj) {
