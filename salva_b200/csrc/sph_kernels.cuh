@@ -117,7 +117,7 @@ __device__ __forceinline__ float kernel_gfac(float d2, float r, float inv_r) {
 #define SPH_FAST_PAIR 1
 #endif
 // MUFU.RSQ without the denormal-rescue sequence rsqrtf() compiles to (3 extra instructions per contact): operands
-// here are squared distances >= g_t2 ~ 1e-14 or exactly 0 (self contact: +inf, masked by the d2 > g_t2 select).
+// here are squared distances floored at 1e-30, far above the denormals.
 __device__ __forceinline__ float rsqrt_ftz(float x) {
     float y;
     asm("rsqrt.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -204,11 +204,13 @@ __device__ __forceinline__ Pair make_pair(const float4& pi, const float4& pj) {
 #if SPH_FAST_PAIR
     // Lean evaluation (about half the instructions of the guarded one below): contacts come from lists built with
     // d^2 <= h^2, so q <= 1 up to rounding (where (1 - q)^2 ~ 1e-14 anyway), and the two "zero gradient" guards of the
-    // reference (|x_ij|^2 > eps^2, q > 1e-5) collapse into one select on d2.  d2 == 0 gives inv_r = +inf and NaNs in
-    // r / q, all discarded by the selects (never multiplied).
-    const float inv_r = rsqrt_ftz(p.d2);
+    // reference (|x_ij|^2 > eps^2, q > 1e-5) collapse into one select on d2.  r itself is the distance down to d2 = 0
+    // (the floor keeps rsqrt finite, so 0 * inv_r = 0): Akinci2013's cohesion and adhesion act on every pair with
+    // |x_ij|^2 > eps^2, below the gradient's threshold too, and divide by r.  W takes the true r as well; at q <= 1e-5,
+    // 1 - 6 q^2 rounds to 1 as it did with r = 0.
+    const float inv_r = rsqrt_ftz(fmaxf(p.d2, 1.0e-30f));
     const bool nz = p.d2 > C.g_t2;
-    p.r = nz ? p.d2 * inv_r : 0.f;
+    p.r = p.d2 * inv_r;
     const float q = p.r * C.inv_h;
     const float t = 1.0f - q;
     const bool inner = q <= 0.5f;
