@@ -147,7 +147,11 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        SPH_DBG_NUM_FLUID_CONTACTS = 5, /* len(ff list) as float, self included contacts.rs:83-87 */
        SPH_DBG_NUM_BOUNDARY_CONTACTS = 6,
        SPH_DBG_PRESSURE = 7,           /* IISPH pressures      iisph_solver.rs:37  */
-       SPH_DBG_ACCELERATION = 8        /* fluid.accelerations (3 floats/particle), after forces, before integrate */ };
+       SPH_DBG_ACCELERATION = 8,       /* fluid.accelerations (3 floats/particle), after forces, before integrate */
+       /* IISPH scratch (SPH_ERR_INVALID for DFSPH, and before the first IISPH step) */
+       SPH_DBG_IISPH_DII = 9,          /* dii (3 floats/particle)                      iisph_solver.rs:32 */
+       SPH_DBG_IISPH_AII = 10,         /* aii                                          iisph_solver.rs:33 */
+       SPH_DBG_IISPH_DIJ_PJL = 11      /* dij_pjl of the last pressure iteration (3)   iisph_solver.rs:34 */ };
 
 /* LiquidWorld::new  liquid_world.rs:39-57 */
 void       sph_world_desc_default(sph_world_desc* desc);

@@ -495,7 +495,8 @@ class NumpyDFSPH:
             o += n
 
     def step_iisph(self, dt, gravity=(0.0, -9.81, 0.0), omega=F(0.5)):
-        """liquid_world.rs:67-158 + iisph_solver.rs:643-711 (dense restatement)."""
+        """liquid_world.rs:67-158 + iisph_solver.rs:643-711 (dense restatement).  Keeps dii, aii and the last iteration's
+        dij_pjl (dijpj) as attributes."""
         self.contacts()
         self.densities_alphas()
         if not hasattr(self, "press") or len(self.press) != len(self.P):
@@ -517,11 +518,13 @@ class NumpyDFSPH:
         aii = ((((dii[:, None, :] - dji) * self.Gff).sum(axis=2, dtype=F) * self.mass[None, :]).sum(axis=1, dtype=F))
         djib = (self.Gfb * fac2[:, None, None]).astype(F)
         aii = (aii + (((dii[:, None, :] - djib) * self.Gfb).sum(axis=2, dtype=F) * self.mb).sum(axis=1, dtype=F)).astype(F)
+        self.dii, self.aii = dii, aii
         self.n_press_iter = 0
         nmax = self.force_press if self.force_press >= 0 else self.max_p_iter
         for i in range(nmax):
             p = self.press
             dijpj = ((self.Gff * (-self.mass * p / (rho * rho))[None, :, None]).sum(axis=1, dtype=F) * (dt * dt)).astype(F)
+            self.dijpj = dijpj   # the last iteration's, as the solver keeps it
             fct = (dijpj[:, None, :] - dii[None, :, :] * p[None, :, None] - (dijpj[None, :, :] - dji * p[:, None, None])).astype(F)
             ssum = ((fct * self.Gff).sum(axis=2, dtype=F) * self.mass[None, :]).sum(axis=1, dtype=F)
             ssum = (ssum + ((dijpj[:, None, :] * self.Gfb).sum(axis=2, dtype=F) * self.mb).sum(axis=1, dtype=F)).astype(F)

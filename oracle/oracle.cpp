@@ -1876,6 +1876,9 @@ int orc_debug_read(void* p, uint32_t fluid, int what, float* out) {
         case 6: for (size_t i = 0; i < n; ++i) out[i] = fluid < w.fb.size() && i < w.fb[fluid].lists.size() ? (float)w.fb[fluid].lists[i].size() : 0.f; break;
         case 7: cpf(w.pressures); break;
         case 8: cpv(w.dbg_acc); break;
+        case 9: cpv(w.dii); break;
+        case 10: cpf(w.aii); break;
+        case 11: cpv(w.dij_pjl); break;
         default: return 1;
     }
     return 0;

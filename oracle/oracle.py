@@ -100,8 +100,8 @@ def _f32(a, shape=None):
 
 
 DBG = dict(density=0, alpha=1, divergence=2, predicted_density=3, velocity_change=4, num_fluid_contacts=5,
-           num_boundary_contacts=6, pressure=7, acceleration=8)
-_VEC = {4, 8}
+           num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11)
+_VEC = {4, 8, 9, 11}
 
 
 class OracleWorld:

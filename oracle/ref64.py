@@ -1,4 +1,5 @@
-"""Float64 restatement of single DFSPH gather passes, each with the scale its float32 evaluation's error is measured against.
+"""Float64 restatement of single DFSPH and IISPH gather passes, each with the scale its float32 evaluation's error is measured
+against.
 
 TEST INFRASTRUCTURE ONLY.  `numpy_ref.py` restates the whole step densely in float32; this module restates ONE pass at a time,
 sparsely (contacts from a k-d tree, no grid, no lists), in float64 from the pass's own float32 inputs, so that a kernel's output
@@ -26,7 +27,7 @@ error of the kernel where (1 - q) cancels near q = 1, with no derivative involve
 support's edge.  The kernels' normalisation constants (sigma: pi and h^3, 4.5u, dsigma6 two more; poly6: h^9 by repeated
 products, 10.5u) are a relative error of every term and are counted in each pass's c_pass as C_NORM = 11.
 
-Cites (reference src/): kernel/*.rs, solver/pressure/dfsph_solver.rs, solver/viscosity/xsph_viscosity.rs,
+Cites (reference src/): kernel/*.rs, solver/pressure/dfsph_solver.rs, solver/pressure/iisph_solver.rs, solver/viscosity/xsph_viscosity.rs,
 solver/surface_tension/akinci2013_surface_tension.rs, as restated in SURVEY.md Appendix A.
 """
 from dataclasses import dataclass
@@ -60,7 +61,24 @@ C_PASS = dict(
     # c inv_dt m_i (2) and * dx (1 + 1), margin 2; adhesion: A(r) / r (r 2, / 1), * adh * vol_b * rho0 (3), * dx * m_i (2 + 1);
     # XSPH: c = cb W vol_b rho0 / rho_i (4), * (v_b - v_i) (1 + 1), * (-m_i inv_dt) (2), margin 2
     boundary_force=C_NORM + 16,
+    # IISPH (iisph_solver.rs).  A pass whose term carries the gradient twice (g^2 |x|^2) counts its normalisation and its
+    # 6.2 + dx twice.
+    # dii: factor -dt dt / (rho rho) 3, m_j factor 1 (boundary vol_b rho0 factor 2), g x 1, fma with x 1 + dx 1, g 6.2, margin 1
+    iisph_dii=C_NORM + 14,
+    # aii: g and dx twice 14.4, factor dt dt m_i / (rho rho) 4, g dx 1, dii - g dx factor 2, * g dx 1, dot sums 2,
+    # fma with m_j (boundary vol_b rho0: 1 more) 2, margin 3.6
+    iisph_aii=2 * C_NORM + 30,
+    # dij_pjl: prho = p / (rho rho) 2, -m_j prho_j 1, g x 1, fma with x 1 + dx 1, g 6.2, dt dt 1, * dt^2 1, margin 1.8
+    iisph_dij_pjl=C_NORM + 16,
+    # next pressure: the sum's term as aii's 14.4 + 2 + 2 + 1 + 2, dji_f = dt dt m_i / (rho rho) p_i 5, dij_i - s_j 1, s_j's
+    # own fma 1 (carried in A through |dii_j p_j| + |dij_pjl_j|); then rho0 - pred 1, - sum 1, / aii 1, omega * 1,
+    # (1 - omega) * p 2, + 1; margin 3.6
+    iisph_pressure=2 * C_NORM + 38,
+    # velocity: prho 2, prho_i + prho_j 1, dt m_j 1, * 1, g x 1, fma with x 1 + dx 1, g 6.2, vc - sum 1, v + vc 1, boundary
+    # c dt 1; margin 1.8
+    iisph_velocity=C_NORM + 18,
 )
+IISPH_AII_GATE = 1.0e-9  # iisph_solver.rs:303: no pressure where |aii| <= 1e-9
 
 
 # ---- kernels: value f and absolute evaluation fa, both float64, for r >= 0 -------------------------------------------------
@@ -546,6 +564,161 @@ class Passes:
             K += _sum(N, fb.i, (np.abs(cbv) * wbe)[:, None] * np.abs(dvb))
             n += self._n(fb)
         return Ref(val * s, A * s, K * s, n)
+
+    # ---- IISPH (iisph_solver.rs) ----------------------------------------------------------------------------------------
+    # Every input is the float32 array the kernel reads (densities, pressures, dii, aii, dij_pjl read back), so the kernels'
+    # pre-combined quantities (prho = p / rho^2, s_j = dii_j p_j + dij_pjl_j, dji_f = dt^2 m_i / rho_i^2 p_i) are restated
+    # from their parts here and their roundings are counted in C_PASS.
+    def _pseudo_mass(self, fb, bvol, rho0_b):
+        return _f64(bvol)[fb.j] * (self.rho0 if rho0_b is None else rho0_b)[fb.i]
+
+    def iisph_dii(self, dens, bvol, dt, rho0_b=None, ff=None, fb=None):
+        """dii_i = -dt^2 / rho_i^2 [sum_j m_j grad W_ij + sum_b vol_b rho0_i grad W_ib] (iisph_solver.rs:144-186)."""
+        ff = self.ff if ff is None else ff
+        fb = self.fb if fb is None else fb
+        rho, dt = _f64(dens), float(F(dt))
+        fac = -dt * dt / (rho * rho)
+        a, aA, aK = self._grad_terms(ff, self.mass[ff.j] * fac[ff.i])
+        b, bA, bK = self._grad_terms(fb, self._pseudo_mass(fb, bvol, rho0_b) * fac[fb.i])
+        N = self.N
+        return Ref(_sum(N, ff.i, a) + _sum(N, fb.i, b), _sum(N, ff.i, aA) + _sum(N, fb.i, bA),
+                   _sum(N, ff.i, aK) + _sum(N, fb.i, bK), (self._n(ff) + self._n(fb)).astype(np.float64))
+
+    def _quadratic(self, pr, w, u, uA, cf):
+        """Per contact w [g (u . x) + cf g^2 |x|^2] (aii's and the pressure sum's term; cf: d_ji's factor), its absolute
+        evaluation and its kernel part (g enters twice)."""
+        g, _, ge = self._g(pr)
+        ux, uxA = (u * pr.x).sum(1), (uA * np.abs(pr.x)).sum(1)
+        wa, ca = np.abs(w), np.abs(cf)
+        t = w * (g * ux + cf * g * g * pr.d2)
+        tA = wa * (np.abs(g) * uxA + ca * g * g * pr.d2)
+        tK = wa * (uxA + ca * (2 * np.abs(g) + ge) * pr.d2) * ge
+        return t, tA, tK
+
+    def iisph_aii(self, dens, dii, bvol, dt, rho0_b=None, dji_mass=None, ff=None, fb=None):
+        """aii = sum_j m_j (dii_i - d_ji) . grad W_ij + sum_b vol_b rho0_i (dii_i - d_ji) . grad W_ib with d_ji = dt^2 m_i /
+        rho_i^2 grad W_ij (iisph_solver.rs:188-233).  dii: the float32 dii the kernel read.  dji_mass: per fluid contact, the
+        mass d_ji uses (default m_i)."""
+        ff = self.ff if ff is None else ff
+        fb = self.fb if fb is None else fb
+        rho, d, dt = _f64(dens), _f64(dii), float(F(dt))
+        fac = dt * dt / (rho * rho)
+        mi = self.mass[ff.i] if dji_mass is None else dji_mass
+        N = self.N
+        val, A, K = np.zeros(N), np.zeros(N), np.zeros(N)
+        for pr, w, cf in ((ff, self.mass[ff.j], -fac[ff.i] * mi),
+                          (fb, self._pseudo_mass(fb, bvol, rho0_b), -fac[fb.i] * self.mass[fb.i])):
+            t, tA, tK = self._quadratic(pr, w, d[pr.i], np.abs(d[pr.i]), cf)
+            val += _sum(N, pr.i, t)
+            A += _sum(N, pr.i, tA)
+            K += _sum(N, pr.i, tK)
+        return Ref(val, A, K, (self._n(ff) + self._n(fb)).astype(np.float64))
+
+    def iisph_dij_pjl(self, dens, press, dt, prho_i=False, ff=None):
+        """dij_pjl_i = dt^2 sum_j -m_j p_j / rho_j^2 grad W_ij over fluid contacts (iisph_solver.rs:235-268).  press: the
+        pressures of the previous iteration.  prho_i: p_i / rho_i^2 in place of p_j / rho_j^2."""
+        ff = self.ff if ff is None else ff
+        rho, p, dt = _f64(dens), _f64(press), float(F(dt))
+        prho = p / (rho * rho)
+        a, aA, aK = self._grad_terms(ff, -dt * dt * self.mass[ff.j] * prho[ff.i if prho_i else ff.j])
+        N = self.N
+        return Ref(_sum(N, ff.i, a), _sum(N, ff.i, aA), _sum(N, ff.i, aK), self._n(ff).astype(np.float64))
+
+    def _pressure_sum(self, dens, press, dii, dij, bvol, dt, rho0_b=None, dji_mass=None, s_dii_p=True, boundary=True,
+                      ff=None, fb=None):
+        """sum_i = sum_j m_j (dij_pjl_i - s_j + d_ji p_i) . grad W_ij + sum_b vol_b rho0_i dij_pjl_i . grad W_ib, with
+        s_j = dii_j p_j + dij_pjl_j (iisph_solver.rs:296-322): (value, A, K, n)."""
+        ff = self.ff if ff is None else ff
+        fb = self.fb if fb is None else fb
+        rho, p, d, dj, dt = _f64(dens), _f64(press), _f64(dii), _f64(dij), float(F(dt))
+        s = dj + (d * p[:, None] if s_dii_p else 0.0)
+        sA = np.abs(dj) + (np.abs(d) * np.abs(p)[:, None] if s_dii_p else 0.0)
+        mi = self.mass[ff.i] if dji_mass is None else dji_mass
+        cf = dt * dt * mi / (rho[ff.i] * rho[ff.i]) * p[ff.i]
+        N = self.N
+        t, tA, tK = self._quadratic(ff, self.mass[ff.j], dj[ff.i] - s[ff.j], np.abs(dj[ff.i]) + sA[ff.j], cf)
+        val, A, K = _sum(N, ff.i, t), _sum(N, ff.i, tA), _sum(N, ff.i, tK)
+        if boundary:
+            b, bA, bK = self._grad_terms(fb, self._pseudo_mass(fb, bvol, rho0_b))
+            val += (_sum(N, fb.i, b) * dj).sum(1)
+            A += (_sum(N, fb.i, bA) * np.abs(dj)).sum(1)
+            K += (_sum(N, fb.i, bK) * np.abs(dj)).sum(1)
+        return val, A, K, (self._n(ff) + self._n(fb)).astype(np.float64)
+
+    def iisph_next_pressure(self, dens, pred, press, aii, dii, dij, bvol, dt, omega, pred_err=None, relax=True, **kw):
+        """p_i' = (1 - omega) p_i + omega (rho0_i - pred_i - sum_i) / aii_i, 0 where |aii_i| <= 1e-9 or p_i' <= 0
+        (iisph_solver.rs:270-353).  Returns (Ref, unclamped): the clamp is a float decision, so the caller excludes particles
+        whose unclamped value lies within its bound of 0.  pred_err: an absolute error of pred (when pred is itself a
+        reference value rather than the float32 array the kernel read).  relax = False drops (1 - omega) p_i.
+        The error of (rho0 - pred) - sum is carried through A rather than taken relative to the result: the two cancel."""
+        S, SA, SK, n = self._pressure_sum(dens, press, dii, dij, bvol, dt, **kw)
+        p, a, pr = _f64(press), _f64(aii), np.asarray(pred, np.float64)
+        om = float(F(omega))
+        on = np.abs(a) > IISPH_AII_GATE   # an exact decision on the float32 input
+        sa = np.where(on, np.abs(a), 1.0)
+        raw = (1.0 - om) * p * relax + om * (self.rho0 - pr - S) / np.where(on, a, 1.0)
+        A = (1.0 - om) * np.abs(p) * relax + om * (self.rho0 + np.abs(pr) + SA) / sa
+        K = om * (SK + (0.0 if pred_err is None else pred_err)) / sa
+        val = np.where(on, np.maximum(raw, 0.0), 0.0)
+        return Ref(val, np.where(on, A, 0.0), np.where(on, K, 0.0), n), np.where(on, raw, np.nan)
+
+    def iisph_density_error(self, dens, pred, press, aii, dii, dij, bvol, dt, omega, c_pass, count_clamped=False, relax=True,
+                            **kw):
+        """The pressure iteration's density error: per fluid, the sum over its particles with p_i' > 0 of
+        (-sum_i - aii_i p_i') / rho0, divided by the fluid's particle count, then the maximum over fluids and 0 (the
+        kernel's block partials and read_error).  Returns (value, bound, ambiguous): the bound carries the errors of sum_i and
+        p_i', and for particles whose p_i' lies within its bound of 0 (either side of the clamp) the whole term.
+        count_clamped: clamped particles add -sum_i / rho0 too."""
+        S, SA, SK, n = self._pressure_sum(dens, press, dii, dij, bvol, dt, **kw)
+        ref, raw = self.iisph_next_pressure(dens, pred, press, aii, dii, dij, bvol, dt, omega, relax=relax, **kw)
+        a = _f64(aii)
+        on = np.abs(a) > IISPH_AII_GATE
+        bp = ref.bound(c_pass)
+        amb = on & (np.abs(np.nan_to_num(raw)) <= bp)
+        pos = on & (np.nan_to_num(raw) > 0)
+        e = (-S - a * ref.value) / self.rho0
+        eS = (n + c_pass) * U * SA + SK
+        ee = (eS + np.abs(a) * bp + 3 * U * (np.abs(S) + np.abs(a * ref.value))) / self.rho0
+        take = pos | (count_clamped & on)
+        val, bound = 0.0, 0.0
+        for f in np.unique(self.fid):
+            sel = self.fid == f
+            nf = sel.sum()
+            ef = np.where(take & sel & ~amb, e, 0.0)
+            slack = np.where(sel & take & ~amb, ee, 0.0) + np.where(sel & amb, np.abs(e) + ee, 0.0)
+            v = ef.sum() / nf
+            b = (slack.sum() + (nf + 2) * U * np.abs(np.where(sel & (take | amb), e, 0.0)).sum()) / nf
+            # max over fluids is 1-Lipschitz in each: the bound of the maximum is the largest bound
+            val, bound = max(val, v), max(bound, b)
+        return val, bound, int(amb.sum())
+
+    def iisph_velocity(self, dens, press, v0, bvol, dt, rho0_b=None, prho_i_twice=False, ff=None, fb=None):
+        """v0 - dt sum_j m_j (p_i / rho_i^2 + p_j / rho_j^2) grad W_ij - dt sum_b vol_b rho0_i p_i / rho_i^2 grad W_ib
+        (iisph_solver.rs:355-420: the velocity change added to the velocity).  prho_i_twice: p_i / rho_i^2 for both."""
+        ff = self.ff if ff is None else ff
+        fb = self.fb if fb is None else fb
+        rho, p, dt = _f64(dens), _f64(press), float(F(dt))
+        prho = p / (rho * rho)
+        pj = prho[ff.i] if prho_i_twice else prho[ff.j]
+        a, aA, aK = self._grad_terms(ff, dt * self.mass[ff.j] * (prho[ff.i] + pj),
+                                     dt * self.mass[ff.j] * (np.abs(prho[ff.i]) + np.abs(pj)))
+        b, bA, bK = self._grad_terms(fb, dt * self._pseudo_mass(fb, bvol, rho0_b) * prho[fb.i])
+        v0 = _f64(v0)
+        N = self.N
+        return Ref(v0 - _sum(N, ff.i, a) - _sum(N, fb.i, b), np.abs(v0) + _sum(N, ff.i, aA) + _sum(N, fb.i, bA),
+                   _sum(N, ff.i, aK) + _sum(N, fb.i, bK), (self._n(ff) + self._n(fb) + 1).astype(np.float64))
+
+    def iisph_boundary_force(self, dens, press, bvol, rho0_b=None, with_mass=True):
+        """The force the pressure puts on boundary particles (iisph_solver.rs:399-401): per boundary particle,
+        sum_i m_i vol_b rho0_i p_i / rho_i^2 grad W_ib.  with_mass = False drops m_i."""
+        fb = self.fb
+        rho, p = _f64(dens), _f64(press)
+        w = self._pseudo_mass(fb, bvol, rho0_b) * (p / (rho * rho))[fb.i] * (self.mass[fb.i] if with_mass else 1.0)
+        return self._on_boundary(fb, *self._grad_terms(fb, w))
+
+
+def _f64(a):
+    return np.asarray(a, F).astype(np.float64)
 
 
 def _cohesion(r, h):

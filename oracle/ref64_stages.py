@@ -1,4 +1,5 @@
-"""Feed each DFSPH gather pass its own inputs and check its output against oracle/ref64.py, particle by particle.
+"""Feed each DFSPH gather pass its own inputs and check its output against oracle/ref64.py, particle by particle (the IISPH
+passes: Checks.iisph_stages).
 
 TEST INFRASTRUCTURE ONLY.  A world (salva_b200.LiquidWorld or oracle.OracleWorld: the same driving code checks both) is
 replayed from scratch once per stage, with the loop shapes pinned by force_iterations(n_div, n_press) and gravity 0:
@@ -195,10 +196,13 @@ def populate(world, scene, forces=()):
     return fh, bh
 
 
-def _read(world, fh, bh):
+IISPH_SCRATCH = ("pressure", "dii", "aii", "dij_pjl")
+
+
+def _read(world, fh, bh, extra=()):
     cat = lambda what: np.concatenate([world.debug(f, what) for f in fh])  # noqa: E731
     out = {w: cat(w) for w in ("density", "alpha", "divergence", "predicted_density", "velocity_change", "acceleration",
-                               "num_fluid_contacts", "num_boundary_contacts")}
+                               "num_fluid_contacts", "num_boundary_contacts") + tuple(extra)}
     pv = [world.read_fluid(f) for f in fh]
     out["P"] = np.concatenate([p for p, _ in pv])
     out["V"] = np.concatenate([v for _, v in pv])
@@ -209,21 +213,22 @@ def _read(world, fh, bh):
     return out
 
 
-def run(make_world, scene, iters, forces=(), first=None, **world_kw):
+def run(make_world, scene, iters, forces=(), first=None, extra=(), **world_kw):
     """Step a fresh world once with force_iterations(*iters) (iters None: the solver's own loop), or twice when `first`
     gives the first step's iterations.  Returns the observables after the last step and, for two steps, those after the
-    first.  world_kw goes to make_world (max_divergence_iter)."""
+    first.  extra: further debug selectors to read (IISPH_SCRATCH); world_kw goes to make_world (max_divergence_iter,
+    min_pressure_iter, max_pressure_iter)."""
     w = make_world(**world_kw)
     fh, bh = populate(w, scene, forces)
     before = None
     if first is not None:
         w.force_iterations(*first)
         w.step(DT, ZERO_G)
-        before = _read(w, fh, bh)
+        before = _read(w, fh, bh, extra)
     if iters is not None:
         w.force_iterations(*iters)
     w.step(DT, ZERO_G)
-    out = _read(w, fh, bh)
+    out = _read(w, fh, bh, extra)
     if hasattr(w, "close"):
         w.close()
     return out, before
@@ -268,7 +273,10 @@ def passes_for(scene, P=None, kw=0, kg=0):
 
 # ---- the checks ----------------------------------------------------------------------------------------------------------------
 MUTANTS = ("drop_entries_32_35", "swap_vy_vz_odd", "gate_at_21", "normals_rho_i", "boundary_mass_fluid0_rho0",
-           "no_kappa_gate", "drop_last_boundary", "bforce_no_inv_dt", "artificial_no_vr_gate")
+           "no_kappa_gate", "drop_last_boundary", "bforce_no_inv_dt", "artificial_no_vr_gate",
+           # IISPH
+           "dji_mass_j", "s_without_dii_p", "dij_prho_i", "next_p_no_boundary", "no_relaxation", "velocity_prho_i_twice",
+           "no_warm_start", "error_counts_clamped", "iisph_bforce_no_mass")
 
 
 class Checks:
@@ -278,7 +286,7 @@ class Checks:
     def __init__(self, make_world, scene, kw=0, kg=0, mutant=None):
         self.make_world, self.scene, self.mutant = make_world, scene, mutant
         self.ps = passes_for(scene, kw=kw, kg=kg)
-        self.worst, self.excluded = {}, {}
+        self.worst, self.excluded, self.clamp = {}, {}, {}
         ps = self.ps
         self.ff, self.fb = ps.ff, ps.fb
         if mutant == "drop_entries_32_35":
@@ -306,11 +314,12 @@ class Checks:
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()))
         self.excluded[name] = self.excluded.get(name, 0) + int((ex & self.want).sum())
 
-    def record(self, name, gpu, ref, c_pass, exclude=None):
+    def record(self, name, gpu, ref, c_pass, exclude=None, ps=None):
+        ps = ps or self.ps
         r = ref64.ratio(gpu, ref, c_pass)
         if r.ndim == 2:
             r = r.max(axis=1)
-        ex = self.ps.ambiguous() if exclude is None else exclude | self.ps.ambiguous()
+        ex = ps.ambiguous() if exclude is None else exclude | ps.ambiguous()
         r = np.where(ex, 0.0, r)
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()) if len(r) else 0.0)
         self.excluded[name] = self.excluded.get(name, 0) + int(ex.sum())
@@ -323,9 +332,9 @@ class Checks:
             vj[odd] = vj[odd][:, [0, 2, 1]]
         return vj
 
-    def stages(self):
-        ps, sc = self.ps, self.scene
-        o00, _ = run(self.make_world, sc, (0, 0))
+    def _first_step_lists(self, o00, alpha=True):
+        """Counts, boundary volumes, rho and (alpha) alpha of a first step (the neighbour search and the density pass)."""
+        ps = self.ps
         nf, nb = o00["num_fluid_contacts"].astype(np.int64), o00["num_boundary_contacts"].astype(np.int64)
         self.nf, self.nb = nf, nb
         cnt = np.where((nf == np.bincount(self.ff.i, minlength=ps.N)) & (nb == np.bincount(self.fb.i, minlength=ps.N)), 0.0, np.inf)
@@ -337,7 +346,14 @@ class Checks:
             self.worst["boundary_volume"] = float(r.max())
         kw = dict(ff=self.ff, fb=self.fb, rho0_b=self.rho0_b)
         self.record("density", o00["density"], ps.density(bvol, **kw), C_PASS["density"])
-        self._alpha(o00["alpha"], bvol)
+        if alpha:
+            self._alpha(o00["alpha"], bvol)
+        return bvol, kw
+
+    def stages(self):
+        ps, sc = self.ps, self.scene
+        o00, _ = run(self.make_world, sc, (0, 0))
+        bvol, kw = self._first_step_lists(o00)
         V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
         self.record("divergence_sweep", o00["divergence"],
                     ps.divergence(V0, bvol, vj=self._vj(V0, self.ff), min_neighbors=self.min_nb, **kw), C_PASS["divergence"])
@@ -369,6 +385,87 @@ class Checks:
         self.record_boundary("boundary_force_pressure", o11["bforce"],
                              ps.pressure_boundary_force(kp, bvol, inv_dt, scale_m_inv_dt=self.mutant != "bforce_no_inv_dt"))
         return o00
+
+    def iisph_stages(self, omega=0.5, alpha=True):
+        """The IISPH passes, on a world made with the IISPH solver (make_world takes min_pressure_iter and
+        max_pressure_iter).  Gravity 0 and no forces: acc = 0, so v* = V0.  alpha: the world computes alpha under IISPH too
+        (the engine's density pass does; the CPU oracle's IISPH, like the reference's, does not).
+          (0, 0)  counts, boundary volumes, rho and alpha (the density pass), dii, aii (fed dii as read back), the
+                  predicted density, p = 0 and V = V0;
+          (0, 1)  p_1 (dij_pjl = 0 and s = 0 here; fed the reference's predicted density, so it sees that pass's
+                  boundary term too), then V and the boundary forces on p_1;
+          (0, 2)  dij_pjl fed p_1, and p_2 fed p_1 and this run's aii, dii, dij_pjl: s_j, d_ji p_i and the boundary term;
+          error   the free-running loop held to k = 1, 2 iterations: last_density_error;
+          warm    step 1 with (0, 2), step 2 with (0, 1) on contacts re-derived on P1: dij_pjl and p fed 0.5 p_2 of each
+                  particle, which checks that pressures ride the step's counting sort.
+        The |aii| > 1e-9 gate is an exact decision on the float32 aii the kernel reads, so it needs no exclusion.  A
+        nonzero |aii| <= 1e-9 needs a particle with a few contacts near the support's edge, whose density is about a
+        quarter of rho0 and whose pressure is clamped to 0 whether or not the gate fires; so the gate shows only at
+        aii = 0, which the lone particle of tail1 reaches."""
+        ps, sc, m = self.ps, self.scene, self.mutant
+        X = IISPH_SCRATCH
+        o0, _ = run(self.make_world, sc, (0, 0), extra=X)
+        bvol, kw = self._first_step_lists(o0, alpha)
+        dens = o0["density"]
+        V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
+        bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
+        pred = ps.divergence(V0, bvol, predicted=True, bvel=bvel, dens=dens, dt=DT, **kw)
+        self.record("predicted", o0["predicted_density"], pred, C_PASS["predicted"])
+        self.record("dii", o0["dii"], ps.iisph_dii(dens, bvol, DT, **kw), C_PASS["iisph_dii"])
+        dji_mass = ps.mass[self.ff.j] if m == "dji_mass_j" else None
+        self.record("aii", o0["aii"], ps.iisph_aii(dens, o0["dii"], bvol, DT, dji_mass=dji_mass, **kw), C_PASS["iisph_aii"])
+        self.worst["pressure_0"] = 0.0 if not o0["pressure"].any() and np.array_equal(o0["V"], V0) else np.inf
+
+        pk = dict(dji_mass=dji_mass, s_dii_p=m != "s_without_dii_p", boundary=m != "next_p_no_boundary", **kw)
+        relax = m != "no_relaxation"
+        o1, _ = run(self.make_world, sc, (0, 1), extra=X)
+        ref, raw = ps.iisph_next_pressure(o1["density"], pred.value, o0["pressure"], o1["aii"], o1["dii"], o1["dij_pjl"], bvol,
+                                          DT, omega, pred_err=pred.bound(C_PASS["predicted"]), relax=relax, **pk)
+        self._pressure("pressure_1", o1["pressure"], ref, raw)
+        p1 = o1["pressure"]
+        self.record("velocity", o1["V"], ps.iisph_velocity(dens, p1, V0, bvol, DT, prho_i_twice=m == "velocity_prho_i_twice", **kw),
+                    C_PASS["iisph_velocity"])
+        self.record_boundary("boundary_force_iisph", o1["bforce"],
+                             ps.iisph_boundary_force(dens, p1, bvol, rho0_b=self.rho0_b, with_mass=m != "iisph_bforce_no_mass"))
+
+        o2, _ = run(self.make_world, sc, (0, 2), extra=X)
+        self.record("dij_pjl", o2["dij_pjl"], ps.iisph_dij_pjl(dens, p1, DT, prho_i=m == "dij_prho_i", ff=self.ff),
+                    C_PASS["iisph_dij_pjl"])
+        ref, raw = ps.iisph_next_pressure(dens, o2["predicted_density"], p1, o2["aii"], o2["dii"], o2["dij_pjl"], bvol, DT, omega,
+                                          relax=relax, **pk)
+        self._pressure("pressure_2", o2["pressure"], ref, raw)
+
+        for k, p_prev in ((1, o0["pressure"]), (2, p1)):
+            o, _ = run(self.make_world, sc, None, extra=X, min_pressure_iter=k, max_pressure_iter=k)
+            assert o["stats"]["n_pressure_iter"] == k, o["stats"]
+            v, b, amb = ps.iisph_density_error(o["density"], o["predicted_density"], p_prev, o["aii"], o["dii"], o["dij_pjl"],
+                                               o["bvol"], DT, omega, C_PASS["iisph_pressure"],
+                                               count_clamped=m == "error_counts_clamped", relax=relax, **pk)
+            err = abs(float(o["stats"]["last_density_error"]) - v)
+            self.worst["density_error"] = max(self.worst.get("density_error", 0.0), err / b if b > 0 else (0.0 if err == 0 else np.inf))
+            self.excluded["density_error"] = self.excluded.get("density_error", 0) + amb
+
+        o2w, o1w = run(self.make_world, sc, (0, 1), first=(0, 2), extra=X)
+        ps1 = passes_for(sc, P=o1w["P"], kw=ps.kw, kg=ps.kg)
+        assert np.array_equal(o2w["num_fluid_contacts"], ps1.nf) and np.array_equal(o2w["num_boundary_contacts"], ps1.nb)
+        p_ws = o1w["pressure"] if m == "no_warm_start" else (o1w["pressure"] * F(0.5)).astype(F)
+        self.record("dij_pjl_warm", o2w["dij_pjl"], ps1.iisph_dij_pjl(o2w["density"], p_ws, DT), C_PASS["iisph_dij_pjl"], ps=ps1)
+        ref, raw = ps1.iisph_next_pressure(o2w["density"], o2w["predicted_density"], p_ws, o2w["aii"], o2w["dii"], o2w["dij_pjl"],
+                                           o2w["bvol"], DT, omega)
+        self._pressure("pressure_warm", o2w["pressure"], ref, raw, ps=ps1)
+        self.moved_cells = int((np.floor(o1w["P"] / ps.h) != np.floor(ps.P / ps.h)).any(axis=1).sum())
+        return o0
+
+    def _pressure(self, name, gpu, ref, raw, ps=None):
+        """A pressure pass: particles whose unclamped value lies within its bound of 0 are excluded (the clamp may go either
+        way); the others are counted on each side of the clamp."""
+        b = ref.bound(C_PASS["iisph_pressure"])
+        amb = np.abs(np.nan_to_num(raw)) <= b
+        amb &= ~np.isnan(raw)
+        self.record(name, gpu, ref, C_PASS["iisph_pressure"], exclude=amb, ps=ps)
+        side = self.clamp.setdefault(name, [0, 0])
+        side[0] += int((np.nan_to_num(raw) < -b).sum())
+        side[1] += int((np.nan_to_num(raw) > b).sum())
 
     def _alpha(self, alpha, bvol):
         ref = self.ps.den(bvol, rho0_b=self.rho0_b)

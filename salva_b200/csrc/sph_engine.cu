@@ -2259,9 +2259,12 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     FLUID_OR_FAIL(fluid, fluid_h)
     FluidRec& f = w->fluids[fluid];
-    bool vec = what == SPH_DBG_VELOCITY_CHANGE || what == SPH_DBG_ACCELERATION;
+    bool vec = what == SPH_DBG_VELOCITY_CHANGE || what == SPH_DBG_ACCELERATION || what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_DIJ_PJL;
     size_t width = vec ? 3 : 1;
     if (cap < f.n) return w->fail(SPH_ERR_INVALID, "sph_debug_read: capacity %zu < particle count %zu", cap, f.n);
+    const bool iisph_sel = what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_AII || what == SPH_DBG_IISPH_DIJ_PJL;
+    if (iisph_sel && (w->desc.solver != SPH_SOLVER_IISPH || !w->iisph.dii || w->own_begin + w->N > w->iisph.cap))
+        return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs an IISPH world that has stepped with its current particles", what);
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
         if (what == SPH_DBG_VELOCITY_CHANGE) memcpy(out, w->h_vc.data() + 3 * f.offset, 3 * f.n * sizeof(float));
@@ -2279,6 +2282,7 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         case SPH_DBG_DIVERGENCE: s1 = w->divv.p; break;
         case SPH_DBG_PREDICTED_DENSITY: s1 = w->desc.solver == SPH_SOLVER_IISPH ? iisph_pred(w) : w->pred.p; break;
         case SPH_DBG_PRESSURE: s1 = w->press[c].p; break;
+        case SPH_DBG_IISPH_AII: s1 = w->iisph.aii; break;
         default: break;
     }
     const uint32_t ob = w->own_begin;
@@ -2286,6 +2290,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     if (s1) LAUNCH(k_export1, N, 256, (uint32_t)N, og, s1 + ob, w->o_c.p);
     else if (what == SPH_DBG_VELOCITY_CHANGE) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->vc[c].p + ob, w->o_c.p);
     else if (what == SPH_DBG_ACCELERATION) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->acc.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_IISPH_DII) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dii + ob, w->o_c.p);
+    else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_f.p + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_b.p + ob, w->o_c.p);
     else return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);

@@ -42,6 +42,98 @@ def test_ref64_agrees_with_the_dense_float32_restatement(kd, kg):
     assert (div.value > 0).sum() >= 10
 
 
+@pytest.mark.parametrize("kd,kg", [(0, 0), (1, 2), (3, 1)], ids=["cubic", "poly6+spiky", "viscosity+poly6"])
+def test_iisph_passes_agree_with_the_dense_float32_restatement(kd, kg):
+    """dii, aii, dij_pjl (fed p_1), p_2 and the velocity of numpy_ref.py's step_iisph, two pressure iterations, against the
+    IISPH passes fed the dense restatement's own float32 values."""
+    sc = S.scene_tail(129)
+    ps = S.passes_for(sc, kw=kd, kg=kg)
+    f = sc["fluids"][0]
+    nds = []
+    for k in (1, 2):
+        nd = NumpyDFSPH(S.R, 2.0, kernel_density=kd, kernel_gradient=kg)
+        nd.add_fluid(f["positions"], f["density0"], velocities=f["velocities"])
+        nd.add_boundary(sc["boundaries"][0]["positions"], velocities=sc["boundaries"][0]["velocities"])
+        nd.force_press = k
+        nd.step_iisph(S.DT, S.ZERO_G)
+        nds.append(nd)
+    n1, n2 = nds
+    C = ref64.C_PASS
+    assert ref64.ratio(n2.dii, ps.iisph_dii(n2.dens, n2.bvol, S.DT), C["iisph_dii"]).max() <= 1
+    assert ref64.ratio(n2.aii, ps.iisph_aii(n2.dens, n2.dii, n2.bvol, S.DT), C["iisph_aii"]).max() <= 1
+    assert ref64.ratio(n2.dijpj, ps.iisph_dij_pjl(n2.dens, n1.press, S.DT), C["iisph_dij_pjl"]).max() <= 1
+    ref, raw = ps.iisph_next_pressure(n2.dens, n2.pred, n1.press, n2.aii, n2.dii, n2.dijpj, n2.bvol, S.DT, 0.5)
+    b = ref.bound(C["iisph_pressure"])
+    clear = np.abs(np.nan_to_num(raw)) > b
+    assert ref64.ratio(n2.press, ref, C["iisph_pressure"])[clear].max() <= 1
+    assert (raw[clear] > 0).sum() >= 50 and (raw[clear] < 0).sum() >= 1     # both sides of the clamp
+    v = ps.iisph_velocity(n2.dens, n2.press, f["velocities"], n2.bvol, S.DT)
+    assert ref64.ratio(n2.V, v, C["iisph_velocity"]).max() <= 1
+    assert (np.abs(v.value - f["velocities"]) > 100 * v.bound(C["iisph_velocity"])).any()
+
+
+def _iisph(kd=0, kg=0):
+    return lambda **kw: OracleWorld(S.R, 2.0, solver=1, kernel_density=kd, kernel_gradient=kg, **kw)
+
+
+def _iisph_checks(name, kd=0, kg=0, mutant=None):
+    c = S.Checks(_iisph(kd, kg), S.SCENES[name](), kw=kd, kg=kg, mutant=mutant)
+    c.iisph_stages(alpha=False)   # the oracle's IISPH, like the reference's, computes no alpha
+    return c
+
+
+IISPH_PASSES = {"counts", "density", "predicted", "dii", "aii", "pressure_0", "pressure_1", "velocity", "dij_pjl", "pressure_2",
+                "density_error", "dij_pjl_warm", "pressure_warm"}
+
+
+@pytest.mark.parametrize("name", sorted(S.SCENES))
+def test_the_cpu_oracle_meets_every_iisph_bound(name):
+    c = _iisph_checks(name)
+    assert not c.flagged(), c.worst
+    assert IISPH_PASSES <= set(c.worst)
+    assert c.worst["counts"] == 0
+    if name == "two_fluids":
+        assert "boundary_force_iisph" in c.worst
+    if name == "block":   # the warm start is checked after most particles moved, many of them across cells
+        assert c.moved_cells >= 300, c.moved_cells
+
+
+@pytest.mark.parametrize("kd,kg", [(1, 2), (3, 1)], ids=["poly6+spiky", "viscosity+poly6"])
+def test_the_cpu_oracle_meets_every_iisph_bound_with_generic_kernels(kd, kg):
+    c = _iisph_checks("two_fluids", kd, kg)
+    assert not c.flagged(), c.worst
+
+
+def test_the_iisph_pressure_clamp_is_reached_on_both_sides():
+    """Particles whose unclamped pressure lies clear of 0 on each side, counted outside the excluded band."""
+    c = _iisph_checks("block")
+    for stage in ("pressure_1", "pressure_2", "pressure_warm"):
+        below, above = c.clamp[stage]
+        assert below >= 1 and above >= 1000, (stage, c.clamp)
+    assert _iisph_checks("gate").clamp["pressure_2"][0] >= 1000   # almost every particle clamped
+
+
+IISPH_MUTANTS = {
+    "dji_mass_j": ("volumes", {"aii", "pressure_2"}),
+    "s_without_dii_p": ("block", {"pressure_2"}),
+    "dij_prho_i": ("block", {"dij_pjl"}),
+    "next_p_no_boundary": ("block", {"pressure_2"}),
+    "no_relaxation": ("block", {"pressure_2"}),
+    "boundary_mass_fluid0_rho0": ("two_fluids", {"dii", "aii", "pressure_1", "velocity"}),
+    "velocity_prho_i_twice": ("block", {"velocity"}),
+    "no_warm_start": ("block", {"dij_pjl_warm", "pressure_warm"}),
+    "error_counts_clamped": ("block", {"density_error"}),
+    "iisph_bforce_no_mass": ("two_fluids", {"boundary_force_iisph"}),
+}
+
+
+@pytest.mark.parametrize("mutant", sorted(IISPH_MUTANTS))
+def test_plausible_iisph_kernel_bugs_are_caught(mutant):
+    scene, must = IISPH_MUTANTS[mutant]
+    flagged = set(_iisph_checks(scene, mutant=mutant).flagged())
+    assert must <= flagged, flagged
+
+
 @pytest.mark.parametrize("name", sorted(S.SCENES))
 def test_the_cpu_oracle_meets_every_bound(name):
     c = _checks(name)
