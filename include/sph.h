@@ -151,7 +151,17 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        /* IISPH scratch (SPH_ERR_INVALID for DFSPH, and before the first IISPH step) */
        SPH_DBG_IISPH_DII = 9,          /* dii (3 floats/particle)                      iisph_solver.rs:32 */
        SPH_DBG_IISPH_AII = 10,         /* aii                                          iisph_solver.rs:33 */
-       SPH_DBG_IISPH_DIJ_PJL = 11      /* dij_pjl of the last pressure iteration (3)   iisph_solver.rs:34 */ };
+       SPH_DBG_IISPH_DIJ_PJL = 11,     /* dij_pjl of the last pressure iteration (3)   iisph_solver.rs:34 */
+       /* Plugin scratch of the fluid's last force of the kind (SPH_ERR_INVALID unless that force has been solved since
+        * particles were last added or deleted; after sph_fluid_write it holds the last solve's values).  `out` holds width * cap floats, width as noted (1 if not). */
+       SPH_DBG_HE2014_COLOR = 12,      /* He2014 colours                               he2014_surface_tension.rs:16 */
+       SPH_DBG_HE2014_GRADC = 13,      /* He2014 squared colour-gradient norms         he2014_surface_tension.rs:17 */
+       SPH_DBG_VISC_BETA = 14,         /* DFSPHViscosity beta (36, row-major 6x6)      dfsph_viscosity.rs:99 */
+       SPH_DBG_VISC_TARGET = 15,       /* DFSPHViscosity strain-rate target (6)        dfsph_viscosity.rs:100 */
+       SPH_DBG_EL_VOLUME0 = 16,        /* Becker2009 rest volumes                      becker2009_elasticity.rs:48-58 */
+       SPH_DBG_EL_ROTATION = 17,       /* Becker2009 rotation (9, row-major)           becker2009_elasticity.rs:48-58 */
+       SPH_DBG_EL_GRAD_TR = 18,        /* Becker2009 deformation_gradient_tr (9, row-major) becker2009_elasticity.rs:48-58 */
+       SPH_DBG_EL_STRESS = 19          /* Becker2009 stress (6: x y z w a b)           becker2009_elasticity.rs:48-58 */ };
 
 /* LiquidWorld::new  liquid_world.rs:39-57 */
 void       sph_world_desc_default(sph_world_desc* desc);

@@ -332,6 +332,7 @@ struct World {
 
     uint32_t n_div_iter = 0, n_press_iter = 0, n_div_eval = 0, n_press_eval = 0;
     float last_div_err = 0, last_dens_err = 0;
+    bool edited = true;  // particles appended or deleted since the last step (the plugin scratch no longer fits them)
     Timings tm;
     std::string err;
 };
@@ -1746,6 +1747,7 @@ int orc_fluid_push_host_force(void* p, uint32_t fluid, host_force_fn fn, void* u
 int orc_fluid_append(void* p, uint32_t fluid, const float* pos, const float* vel, size_t n) {
     World& w = *(World*)p;
     if (fluid >= w.fluids.size()) return 1;
+    w.edited = true;
     Fluid& f = w.fluids[fluid];
     float pv = f.particle_radius * f.particle_radius * f.particle_radius * (float)(8.0 * 0.8);
     for (size_t i = 0; i < n; ++i) {
@@ -1761,6 +1763,7 @@ int orc_fluid_append(void* p, uint32_t fluid, const float* pos, const float* vel
 int orc_fluid_delete(void* p, uint32_t fluid, const uint8_t* mask, size_t n) {
     World& w = *(World*)p;
     if (fluid >= w.fluids.size() || n != w.fluids[fluid].n()) return 1;
+    w.edited = true;
     Fluid& f = w.fluids[fluid];
     for (size_t i = 0; i < n; ++i)
         if (mask[i] && !f.deleted[i]) {
@@ -1819,7 +1822,9 @@ int orc_boundary_read(void* p, uint32_t b, float* volumes, float* forces) {
 }
 int orc_world_step(void* p, float dt, const float* g) {
     World& w = *(World*)p;
-    return world_step(w, dt, {g[0], g[1], g[2]});
+    int rc = world_step(w, dt, {g[0], g[1], g[2]});
+    if (rc == 0) w.edited = false;
+    return rc;
 }
 void orc_world_force_iterations(void* p, int n_div, int n_press) {
     World& w = *(World*)p;
@@ -1879,6 +1884,28 @@ int orc_debug_read(void* p, uint32_t fluid, int what, float* out) {
         case 9: cpv(w.dii); break;
         case 10: cpf(w.aii); break;
         case 11: cpv(w.dij_pjl); break;
+        case 12: case 13: case 14: case 15: case 16: case 17: case 18: case 19: {
+            // plugin scratch of the fluid's last force of the kind; refused, as by the engine, unless that force has been
+            // solved and no particle has been appended or deleted since (a write keeps the last solve's values)
+            const int kind = what <= 13 ? F_HE2014 : what <= 15 ? F_DFSPH_VISC : F_BECKER;
+            const Force* fc = nullptr;
+            for (const Force& x : w.fluids[fluid].forces)
+                if (x.kind == kind) fc = &x;
+            if (!fc || w.edited) return 1;
+            const size_t solved = kind == F_HE2014 ? fc->colors.size() : kind == F_DFSPH_VISC ? fc->betas.size() : fc->positions0.size();
+            if (solved != n || (kind == F_DFSPH_VISC && fc->sr_target.size() != n)) return 1;
+            for (size_t i = 0; i < n; ++i) switch (what) {
+                case 12: out[i] = fc->colors[i]; break;
+                case 13: out[i] = fc->gradcs[i]; break;
+                case 14: std::memcpy(out + 36 * i, fc->betas[i].data(), 36 * sizeof(float)); break;
+                case 15: std::memcpy(out + 6 * i, fc->sr_target[i].data(), 6 * sizeof(float)); break;
+                case 16: out[i] = fc->volumes0[i]; break;
+                case 17: std::memcpy(out + 9 * i, &fc->rotations[i].m[0][0], 9 * sizeof(float)); break;
+                case 18: std::memcpy(out + 9 * i, &fc->grad_tr[i].m[0][0], 9 * sizeof(float)); break;
+                default: std::memcpy(out + 6 * i, &fc->stress[6 * i], 6 * sizeof(float)); break;
+            }
+            break;
+        }
         default: return 1;
     }
     return 0;

@@ -1,5 +1,5 @@
-"""Float64 restatement of single DFSPH and IISPH gather passes, each with the scale its float32 evaluation's error is measured
-against.
+"""Float64 restatement of single DFSPH and IISPH gather passes and of the WCSPH, He2014, DFSPHViscosity and Becker2009
+plugins' passes, each with the scale its float32 evaluation's error is measured against.
 
 TEST INFRASTRUCTURE ONLY.  `numpy_ref.py` restates the whole step densely in float32; this module restates ONE pass at a time,
 sparsely (contacts from a k-d tree, no grid, no lists), in float64 from the pass's own float32 inputs, so that a kernel's output
@@ -28,7 +28,7 @@ support's edge.  The kernels' normalisation constants (sigma: pi and h^3, 4.5u, 
 products, 10.5u) are a relative error of every term and are counted in each pass's c_pass as C_NORM = 11.
 
 Cites (reference src/): kernel/*.rs, solver/pressure/dfsph_solver.rs, solver/pressure/iisph_solver.rs, solver/viscosity/xsph_viscosity.rs,
-solver/surface_tension/akinci2013_surface_tension.rs, as restated in SURVEY.md Appendix A.
+solver/surface_tension/{akinci2013,he2014,wcsph}_surface_tension.rs, solver/elasticity/becker2009_elasticity.rs, as restated in SURVEY.md Appendix A.
 """
 from dataclasses import dataclass
 
@@ -77,7 +77,42 @@ C_PASS = dict(
     # velocity: prho 2, prho_i + prho_j 1, dt m_j 1, * 1, g x 1, fma with x 1 + dx 1, g 6.2, vc - sum 1, v + vc 1, boundary
     # c dt 1; margin 1.8
     iisph_velocity=C_NORM + 18,
+    # Surface tension plugins (surface_tension/*.rs), over same-fluid contacts.
+    # WCSPH: c = -cf W m_j / m_i: -cf W 1, * m_j 1, / m_i 1; fma with x 1 + dx 1; margin 3
+    wcsph=C_NORM + 8,
+    # He2014 colours: W m_j 1, / rho_j 1 (boundary: W vol_b 1); margin 2
+    he2014_color=C_NORM + 4,
+    # He2014 gradc, per component before the square: c = g c_j m_j / rho_j 3, g 6.2, fma with x 1 + dx 1; margin 1.8.  The
+    # division by c_i and the square are carried explicitly (Passes.he2014_gradc)
+    he2014_gradc=C_NORM + 13,
+    # He2014 force: fluid m_i / rho_i 1, * m_j 1, / rho_j 1, g_i + g_j 1, * 1, g * 1, g 6.2, * x 1 + dx 1, * k 1, k = cf / (2 m_i)
+    # 1; boundary vol_b rho0 1, / rho0 1, * g_i 1, * cb 1, s * x 1, / m_i 1, acc + 1; margin 2.8
+    he2014_force=C_NORM + 18,
+    # DFSPHViscosity.  G = grad W m_j / (2 rho_i): g 6.2, * x 1 + dx 1, s = m_j / (2 rho_i) 1, * s 1, margin 1.8; the
+    # matrix entries (products of two G, / rho, sums) are bounded from it in Passes.visc_matrix
+    visc_matrix=C_NORM + 12,
+    # strain rate: G as above 11 + vv = fma(a, dt, v) 1, vv_j - vv_i 1, products and the pair sum 2, margin 2
+    visc_rate=C_NORM + 16,
+    # acceleration: g 6.2 + dx 1, u_i + u_j 1, * m_j / 2 1, gradient^T products and sums 3, * m_i inv_dt 2, acc + 1,
+    # margin 2.8 (u's own error is carried in K)
+    visc_accel=C_NORM + 18,
+    # Becker2009 elasticity (becker2009_elasticity.rs), over the rest contacts, always with the cubic spline.
+    # rest volume, checked as m_i / vol0 against the sum: 2 m_j W 1 (2 exact), m_i / sum 1, its inverse read back 1; margin 2
+    el_volume=C_NORM + 5,
+    # A_pq entry: p = x_j - x_i 1, q = x0_j - x0_i 1, coeff = W m_j 1, q coeff 1, p q 1; margin 2
+    el_apq=C_NORM + 7,
+    # grad_tr entry: a = g vol0_j x0 (g 6.2, * vol0 1, * x0 1 + dx 1), u = R^T p - q (p 1, three products and two sums 3,
+    # q 1, - 1: carried in A through |R|^T |p| + |q|), a u 1; margin 2.8
+    el_grad_tr=C_NORM + 18,
+    # force term: grad 6.2 + dx 1, * vol0 1, S d (products and sums) 3, G (S d) 3 + 1, * vol0 1, R f 3, R_j f_ij - R_i f_ji 1,
+    # * 0.5 / m_i 1; margin 2.8
+    el_force=C_NORM + 24,
 )
+# stress from grad_tr read back, no sum: J = G + I 1, J J^T 3, - 1 1, d0 ex + d1 ey + d1 ez 3, * k 1, * d2 1; margin 2
+C_EL_STRESS = 12
+# orthonormality of the float32 rotation: each of at most 20 iterations multiplies by an axis-angle rotation built from
+# sin / cos and products (<= 8u per entry) in a 3-term product (3u)
+C_EL_ORTHO = 20 * 11 + 20
 IISPH_AII_GATE = 1.0e-9  # iisph_solver.rs:303: no pressure where |aii| <= 1e-9
 
 
@@ -715,6 +750,389 @@ class Passes:
         rho, p = _f64(dens), _f64(press)
         w = self._pseudo_mass(fb, bvol, rho0_b) * (p / (rho * rho))[fb.i] * (self.mass[fb.i] if with_mass else 1.0)
         return self._on_boundary(fb, *self._grad_terms(fb, w))
+
+    # ---- surface tension plugins (surface_tension/*.rs) -----------------------------------------------------------------
+    # Fluid sums run over contacts of the particle's own fluid (self included: x_ii = 0); every input is the float32 array
+    # the kernel read (densities, and the colours and gradc read back).
+    def _same(self):
+        return self.ff.subset(self.fid[self.ff.i] == self.fid[self.ff.j])
+
+    def _vec_sum(self, pr, t, tA, tK, n=None):
+        N = self.N
+        return Ref(_sum(N, pr.i, t), _sum(N, pr.i, tA), _sum(N, pr.i, tK), self._n(pr).astype(np.float64) if n is None else n)
+
+    def wcsph(self, cf, inverted_mass_ratio=False):
+        """WCSPHSurfaceTension's fluid term (wcsph_surface_tension.rs:45-63): sum_j -cf W_ij m_j / m_i x_ij.
+        inverted_mass_ratio: m_i / m_j."""
+        sf = self._same()
+        w, _, we = self._w(sf)
+        ratio = self.mass[sf.i] / self.mass[sf.j] if inverted_mass_ratio else self.mass[sf.j] / self.mass[sf.i]
+        c = -float(F(cf)) * ratio
+        return self._vec_sum(sf, (c * w)[:, None] * sf.x, np.abs(c * w)[:, None] * np.abs(sf.x), (np.abs(c) * we)[:, None] * np.abs(sf.x))
+
+    def he2014_colors(self, dens, bvol, boundary=True):
+        """He2014's colours (he2014_surface_tension.rs:40-75): sum_j W_ij m_j / rho_j + sum_b W_ib vol_b."""
+        sf, fb, N = self._same(), self.fb, self.N
+        w, _, we = self._w(sf)
+        c = self.mass[sf.j] / _f64(dens)[sf.j]
+        val, A, K = _sum(N, sf.i, c * w), _sum(N, sf.i, np.abs(c * w)), _sum(N, sf.i, c * we)
+        n = self._n(sf)
+        if boundary:
+            wb, _, wbe = self._w(fb)
+            vb = _f64(bvol)[fb.j]
+            val, A, K = val + _sum(N, fb.i, vb * wb), A + _sum(N, fb.i, np.abs(vb * wb)), K + _sum(N, fb.i, vb * wbe)
+            n = n + self._n(fb)
+        return Ref(val, A, K, n.astype(np.float64))
+
+    def he2014_gradc(self, dens, colors, c_pass, divide_by_cj=False):
+        """He2014's squared colour-gradient norm (he2014_surface_tension.rs:77-105): |sum_j grad W_ij c_j m_j / rho_j / c_i|^2.
+        The vector sum cancels in the interior, so its error is bounded per component and carried through the division
+        and the square explicitly (as in den); the Ref's A is 0 and K the whole bound.  divide_by_cj: each term divided by
+        its own c_j instead of the sum by c_i."""
+        sf, N = self._same(), self.N
+        c = _f64(colors)
+        wt = self.mass[sf.j] / _f64(dens)[sf.j] * (1.0 if divide_by_cj else c[sf.j])
+        a, aA, aK = self._grad_terms(sf, wt)
+        n = self._n(sf).astype(np.float64)
+        gs = _sum(N, sf.i, a)
+        e_gs = (n + c_pass)[:, None] * U * _sum(N, sf.i, aA) + _sum(N, sf.i, aK)
+        ci = np.ones(N) if divide_by_cj else np.abs(c)
+        q = gs / ci[:, None]
+        e_q = e_gs / ci[:, None] + U * np.abs(q)
+        val = (q * q).sum(1)
+        e = (2 * np.abs(q) * e_q + e_q * e_q).sum(1) + 4 * U * val
+        return Ref(val, np.zeros(N), e, n)
+
+    def _he2014_boundary_terms(self, dens, gradc, cb, bvol):
+        """Per fluid-boundary contact f = cb / 4 grad W_ib m_i / rho_i vol_b g_i (the boundary loop of he2014_surface_tension.rs:131-178)."""
+        fb = self.fb
+        w = float(F(cb)) * 0.25 * self.mass[fb.i] / _f64(dens)[fb.i] * _f64(bvol)[fb.j] * _f64(gradc)[fb.i]
+        return fb, self._grad_terms(fb, w)
+
+    def he2014_force(self, dens, gradc, cf, cb, bvol, gradc_i_twice=False):
+        """He2014's acceleration (he2014_surface_tension.rs:131-178): cf / (2 m_i) sum_j grad W_ij m_i / rho_i m_j / rho_j
+        (g_i + g_j) / 2 over the same fluid, plus the boundary term f / m_i.  gradc_i_twice: g_i + g_i."""
+        sf, N = self._same(), self.N
+        g, rho = _f64(gradc), _f64(dens)
+        gj = g[sf.i] if gradc_i_twice else g[sf.j]
+        base = float(F(cf)) / (2.0 * self.mass[sf.i]) * self.mass[sf.i] / rho[sf.i] * self.mass[sf.j] / rho[sf.j] * 0.5
+        a, aA, aK = self._grad_terms(sf, base * (g[sf.i] + gj), np.abs(base) * (np.abs(g[sf.i]) + np.abs(gj)))
+        ref = self._vec_sum(sf, a, aA, aK)
+        if cb != 0:
+            fb, (b, bA, bK) = self._he2014_boundary_terms(dens, gradc, cb, bvol)
+            mi = self.mass[fb.i][:, None]
+            ref = Ref(ref.value + _sum(N, fb.i, b / mi), ref.A + _sum(N, fb.i, bA / mi), ref.K + _sum(N, fb.i, bK / mi),
+                      ref.n + self._n(fb))
+        return ref
+
+    # ---- DFSPHViscosity (viscosity/dfsph_viscosity.rs) -----------------------------------------------------------------
+    def _visc_grads(self, dens):
+        """Same-fluid contacts and, per contact, G = grad W_ij m_j / (2 rho_i), its absolute evaluation and kernel part."""
+        sf = self._same()
+        g, _, ge = self._g(sf)
+        s = self.mass[sf.j] / (2.0 * _f64(dens)[sf.i])
+        return sf, (g * s)[:, None] * sf.x, (np.abs(g) * s)[:, None] * np.abs(sf.x), (ge * s)[:, None] * np.abs(sf.x)
+
+    @staticmethod
+    def _mat6(G):
+        """compute_gradient_matrix (dfsph_viscosity.rs:59-82): rows (2gx,0,0) (0,2gy,0) (0,0,2gz) (gy,gx,0) (gz,0,gx)
+        (0,gz,gy), (..., 6, 3)."""
+        x, y, z = G[..., 0], G[..., 1], G[..., 2]
+        o = np.zeros_like(x)
+        return np.stack([np.stack(r, -1) for r in ((2 * x, o, o), (o, 2 * y, o), (o, o, 2 * z), (y, x, o), (z, o, x),
+                                                    (o, z, y))], -2)
+
+    def visc_matrix(self, dens, c_pass, by_column=False):
+        """The preconditioned 6x6 matrix whose inverse is beta (dfsph_viscosity.rs:133-201), in float64: D = sum_j M_j M_j^T
+        / rho_i + M(sum_j G_j) M(sum_j G_j)^T / rho_i with M_j = M(G_j); then column c < 3 of row r scaled by p_r = 1 / D_rr
+        (1 where |D_rr| < 1e-6).  Returns (Dt, dDt, p, dp, ambiguous): the bound of each entry of the kernel's float32
+        Dt (D's own error plus the float32 p's), p and its relative error, and the particles whose preconditioner switch
+        |D_rr| < 1e-6 lies within D_rr's bound.  by_column: column c scaled by p_c instead."""
+        sf, G, GA, GK = self._visc_grads(dens)
+        N, rho = self.N, _f64(dens)
+        n = self._n(sf).astype(np.float64)
+        M, MA, MK = self._mat6(G), self._mat6(GA), self._mat6(GK)
+        outer = lambda a, b: np.einsum("nrk,nck->nrc", a, b) / rho[sf.i][:, None, None]  # noqa: E731
+        sq = lambda t: np.stack([_sum(N, sf.i, t[:, r, :]) for r in range(6)], axis=1)  # noqa: E731
+        D1, D1A = sq(outer(M, M)), sq(outer(MA, MA))
+        D1K = sq(outer(MA, MK) + outer(MK, MA))
+        gs, gsA, gsK = _sum(N, sf.i, G), _sum(N, sf.i, GA), _sum(N, sf.i, GK)
+        e_gs = (n + c_pass)[:, None] * U * gsA + gsK
+        Ms, MsA, Me = self._mat6(gs), self._mat6(np.abs(gs)), self._mat6(e_gs)
+        op = lambda a, b: np.einsum("nrk,nck->nrc", a, b) / rho[:, None, None]  # noqa: E731
+        D = D1 + op(Ms, Ms)
+        dD = (n + 2 * c_pass + 4)[:, None, None] * U * D1A + D1K + op(MsA, Me) + op(Me, MsA) + op(Me, Me) + \
+            8 * U * op(MsA, MsA) + 2 * U * np.abs(D)
+        dg = np.diagonal(D, axis1=1, axis2=2)
+        ddg = np.diagonal(dD, axis1=1, axis2=2)
+        small = np.abs(dg) < 1e-6
+        ambiguous = (np.abs(np.abs(dg) - 1e-6) <= ddg).any(axis=1)
+        p = np.where(small, 1.0, 1.0 / np.where(small, 1.0, dg))
+        dp = np.where(small, 0.0, ddg / np.where(small, 1.0, np.abs(dg)) + 2 * U)
+        scale = np.ones((N, 6, 6))
+        if by_column:
+            scale[:, :, :3] = p[:, None, :3]
+            rel = np.zeros((N, 6, 6)) + dp[:, None, :]
+        else:
+            scale[:, :, :3] = p[:, :, None]
+            rel = np.zeros((N, 6, 6)) + dp[:, :, None]
+        rel[:, :, 3:] = 0.0
+        Dt = D * scale
+        return Dt, dD * np.abs(scale) + rel * np.abs(Dt) + U * np.abs(Dt), p, dp, ambiguous
+
+    def visc_beta(self, dens, beta, c_pass, by_column=False):
+        """beta (N, 36 row-major) read back against the LU backward-error bound (Higham 9, 14.3), not against a float64
+        inverse: with the column scaling undone (x_k = beta_k / p_k, k < 3), |Dt x_k - e_k| <= (|dDt| + 2 gamma_18
+        |L||U|) |x_k| (+ the scaling's own error), |L||U| from a float64 partial-pivoting LU of Dt.  The gate: beta = 0
+        exactly when |det| < 1e-6 (on the float32 LU) or a pivot is 0.  Returns (ratio, gate_violations, excluded, zero):
+        excluded where the preconditioner switch or |det| lies within its bound of 1e-6; zero: beta = 0."""
+        import scipy.linalg
+        Dt, dDt, p, dp, amb = self.visc_matrix(dens, c_pass, by_column)
+        N = self.N
+        B = np.asarray(beta, np.float64).reshape(N, 6, 6)
+        zero = ~B.any(axis=(1, 2))
+        X = B.copy()
+        X[:, :, :3] /= p[:, None, :3]
+        gam = 18 * U / (1 - 18 * U)
+        LU = np.zeros((N, 6, 6))
+        det = np.zeros(N)
+        det_b = np.full(N, np.inf)
+        for k in range(N):
+            P_, L_, U_ = scipy.linalg.lu(Dt[k])
+            LU[k] = P_ @ (np.abs(L_) @ np.abs(U_))
+            det[k] = np.linalg.det(Dt[k])
+            if not Dt[k].any() and not dDt[k].any():   # no contact but itself: exactly singular
+                det_b[k] = 0.0
+            elif np.all(np.abs(np.diag(U_)) > 0):
+                inv = np.linalg.inv(Dt[k])
+                det_b[k] = 2 * abs(det[k]) * (np.abs(inv.T) * (dDt[k] + 2 * gam * LU[k])).sum()
+        E = dDt + 2 * gam * LU
+        res = np.abs(np.einsum("nrc,nck->nrk", Dt, X) - np.eye(6))
+        bnd = np.einsum("nrc,nck->nrk", E, np.abs(X)) + \
+            np.einsum("nrc,nck->nrk", np.abs(Dt), np.abs(X) * np.concatenate([dp[:, :3], np.zeros((N, 3))], 1)[:, None, :])
+        with np.errstate(divide="ignore", invalid="ignore"):
+            ratio = np.where(bnd > 0, res / bnd, np.where(res == 0, 0.0, np.inf)).max(axis=(1, 2))
+        amb = amb | (np.abs(np.abs(det) - 1e-6) <= det_b)
+        below = np.abs(det) + det_b < 1e-6
+        violations = (zero & ~below & ~amb) | (~zero & below & ~amb)
+        ratio = np.where(zero | amb, 0.0, ratio)
+        return ratio, int(violations.sum()), amb, zero
+
+    def visc_rates(self, dens, vel, acc, dt, scale, skip_adt=False):
+        """The strain rate scale * sum_j m_j / (2 rho_i) S(grad W_ij, vv_j - vv_i) over the same fluid, vv = v + a dt as
+        k_visc_vv forms it (dfsph_viscosity.rs:203-252): a Ref (N, 6).  scale: (1 - visc) for the target, 1 for the
+        error.  skip_adt: vv = v."""
+        sf, G, GA, GK = self._visc_grads(dens)
+        v, a, dt = _f64(vel), _f64(acc), float(F(dt))
+        vv = v + (0.0 if skip_adt else a * dt)
+        vvA = np.abs(v) + (0.0 if skip_adt else np.abs(a) * dt)
+        dv, dvA = vv[sf.j] - vv[sf.i], vvA[sf.j] + vvA[sf.i]
+
+        def rate(g, d):
+            x, y, z = g[:, 0], g[:, 1], g[:, 2]
+            return np.stack([2 * d[:, 0] * x, 2 * d[:, 1] * y, 2 * d[:, 2] * z, d[:, 0] * y + d[:, 1] * x,
+                             d[:, 0] * z + d[:, 2] * x, d[:, 1] * z + d[:, 2] * y], 1)
+        N, s = self.N, abs(scale)
+        return Ref(scale * _sum(N, sf.i, rate(G, dv)), s * _sum(N, sf.i, rate(GA, dvA)), s * _sum(N, sf.i, rate(GK, dvA)),
+                   self._n(sf).astype(np.float64))
+
+    def visc_accel(self, dens, beta, rate, rate_err, target, acc0, inv_dt, beta_i_for_j=False):
+        """acc0 + sum_j G(grad W_ij)^T (u_i + u_j) m_j / 2 * m_i inv_dt over the same fluid (dfsph_viscosity.rs:254-289),
+        u = beta (rate - target) / rho^2 with beta and target read back; rate: the float64 strain rate and rate_err its
+        bound, carried through |beta|.  beta_i_for_j: u_j formed with beta_i."""
+        sf, G, GA, GK = self._visc_grads(dens)
+        N, rho = self.N, _f64(dens)
+        B = np.asarray(beta, np.float64).reshape(N, 6, 6)
+        err = rate - _f64(target)
+        errA = np.abs(rate) + np.abs(_f64(target))
+        u = np.einsum("nrk,nk->nr", B, err) / (rho * rho)[:, None]
+        e_u = (np.einsum("nrk,nk->nr", np.abs(B), rate_err + 10 * U * errA)) / (rho * rho)[:, None]
+        uA = np.einsum("nrk,nk->nr", np.abs(B), errA) / (rho * rho)[:, None]
+        if beta_i_for_j:
+            uj = np.einsum("nrk,nk->nr", B[sf.i], err[sf.j]) / (rho * rho)[sf.j][:, None]
+        else:
+            uj = u[sf.j]
+        hm = self.mass[sf.j] / 2.0 * self.mass[sf.i] * float(F(inv_dt))
+        c, cA, cE = (u[sf.i] + uj) * hm[:, None], (uA[sf.i] + uA[sf.j]) * hm[:, None], (e_u[sf.i] + e_u[sf.j]) * hm[:, None]
+        tr = lambda m, w: np.einsum("nrk,nr->nk", m, w)  # noqa: E731
+        Mt, MA, MK = self._mat6(G / (self.mass[sf.j] / (2.0 * rho[sf.i]))[:, None]), \
+            self._mat6(GA / (self.mass[sf.j] / (2.0 * rho[sf.i]))[:, None]), self._mat6(GK / (self.mass[sf.j] / (2.0 * rho[sf.i]))[:, None])
+        a0 = _f64(acc0)
+        return Ref(a0 + _sum(N, sf.i, tr(Mt, c)), np.abs(a0) + _sum(N, sf.i, tr(MA, cA)),
+                   _sum(N, sf.i, tr(MK, cA) + tr(MA, cE)), self._n(sf).astype(np.float64))
+
+    def he2014_boundary_force(self, dens, gradc, cb, bvol, sign=-1.0):
+        """He2014's reaction on boundary particles (he2014_surface_tension.rs:175): -f per contact.  sign: the sign of f."""
+        fb, (b, bA, bK) = self._he2014_boundary_terms(dens, gradc, cb, bvol)
+        return self._on_boundary(fb, sign * b, bA, bK)
+
+
+class Becker:
+    """Becker2009Elasticity's passes (becker2009_elasticity.rs:84-334) over the rest contacts: the same-fluid contacts of
+    the rest positions Q (self included), always with the cubic spline.  Particles are in the fluids' original order, fluids
+    concatenated; fid: the fluid of each, mass: float32 masses.  rest: other contacts to use (a kernel that recaptures its
+    lists)."""
+
+    def __init__(self, h, Q, fid, mass, young, poisson, nonlinear, rest=None):
+        self.h = float(F(h))
+        self.N, self.mass, self.nonlinear, self.fid = len(Q), _f64(mass), nonlinear, np.asarray(fid)
+        same = lambda i, j: fid[i] == fid[j]  # noqa: E731
+        self.rest = contacts(Q, Q, self.h, same, same=True) if rest is None else rest
+        r = self.rest
+        E, nu, one, two = F(young), F(poisson), F(1.0), F(2.0)   # elasticity_coefficients :15-25, in float32 as solved
+        self.d0 = float(F((E * (one - nu)) / ((one + nu) * (one - two * nu))))
+        self.d1 = float(F((E * nu) / ((one + nu) * (one - two * nu))))
+        self.d2 = float(F((E * (one - two * nu)) / (two * (one + nu) * (one - two * nu))))
+        self.w, _, self.we = kernel(0, "w", r.r, self.h)
+        g, _, ge = kernel(0, "g", r.r, self.h)
+        z = r.d2 <= grad_threshold(0, self.h)
+        self.g, self.ge = np.where(z, 0.0, g), np.where(z, 0.0, ge)
+        self.n = np.bincount(r.i, minlength=self.N).astype(np.float64)
+
+    def volume_sum(self, per_contact=2.0, old=None):
+        """old_i + sum_j 2 m_j W0_ij: the rest volume is m_i over it (:89-111; each contact adds to both ends, the self
+        contact included).  per_contact: the factor (1: each contact counted once).  old: the rest volumes a re-capture
+        starts from (Vec::resize keeps the leading old values; 0 for new particles)."""
+        r, N = self.rest, self.N
+        t = per_contact * self.mass[r.j] * self.w
+        o = np.zeros(N) if old is None else _f64(old)
+        return Ref(o + _sum(N, r.i, t), np.abs(o) + _sum(N, r.i, np.abs(t)), _sum(N, r.i, per_contact * self.mass[r.j] * self.we),
+                   self.n + (old is not None))
+
+    def _pq(self, P):
+        """Per rest contact p = x_j - x_i (current, float64 of float32) and q = x0_j - x0_i."""
+        P = _f64(P)
+        return P[self.rest.j] - P[self.rest.i], -self.rest.x
+
+    def apq(self, P, c_pass):
+        """A_pq = sum_j p_j q_j^T W0_ij m_j (:115-137) in float64 at the current positions P, and the bound of each entry
+        of its float32 evaluation: (N, 3, 3) each."""
+        r, N = self.rest, self.N
+        p, q = self._pq(P)
+        cw = self.w * self.mass[r.j]
+        pq = p[:, :, None] * q[:, None, :]
+        A = np.stack([_sum(N, r.i, pq[:, a, :] * cw[:, None]) for a in range(3)], axis=1)
+        dA = np.stack([(self.n + c_pass)[:, None] * U * _sum(N, r.i, np.abs(pq[:, a, :]) * cw[:, None]) +
+                       _sum(N, r.i, np.abs(pq[:, a, :]) * (self.mass[r.j] * self.we)[:, None]) for a in range(3)], axis=1)
+        return A, dA
+
+    def rotation(self, P, R_hat, R_prev, c_pass):
+        """(ratio, orthonormality ratio, excluded, reference, iterations) of the float32 rotations R_hat (N, 3, 3) at the
+        current positions P.  The reference is from_matrix_eps (rotation_from_matrix_eps) restated in float64 and run from
+        the same warm start R_prev (the previous step's float32 rotations) on A_pq formed in float64.  The bound is the polar
+        factor's perturbation bound 2 |dA|_F / (s2 + s3) (s3 negative when det A < 0), dA the float32 A_pq's error, plus
+        the iteration's stopping test |axis / denom| <= eps (a residual angle of about eps (s1 + s2 + s3) / (s2 + s3)) and
+        R_hat's own departure from orthonormality.  Excluded: particles where that bound exceeds 0.05 (s2 + s3 too small for
+        the rotation to be determined), and those whose float64 run needs all 20 iterations."""
+        A, dA = self.apq(P, c_pass)
+        R, iters = from_matrix_eps(A, np.asarray(R_prev, np.float64))
+        s = np.linalg.svd(A, compute_uv=False)
+        d = np.sign(np.linalg.det(A))
+        gap = s[:, 1] + d * s[:, 2]
+        gs = np.where(gap > 0, gap, 1.0)
+        ortho = np.abs(np.einsum("nki,nkj->nij", R_hat, R_hat) - np.eye(3)).max(axis=(1, 2))
+        bound = 2 * np.sqrt((dA * dA).sum(axis=(1, 2))) / gs + (EPS32 + 8 * U) * (s[:, 0] + s[:, 1] + d * s[:, 2]) / gs + \
+            C_EL_ORTHO * U
+        excluded = (gap <= 0) | (bound > 0.05) | (iters >= 20)
+        err = np.abs(np.asarray(R_hat, np.float64) - R).max(axis=(1, 2))
+        return np.where(excluded, 0.0, err / bound), ortho / (C_EL_ORTHO * U), excluded, R, iters
+
+    @staticmethod
+    def polar(A):
+        """The rotation of A's polar decomposition (SVD, det-corrected): the maximiser of tr(R^T A)."""
+        u, _, vt = np.linalg.svd(A)
+        d = np.sign(np.linalg.det(u @ vt))
+        return (u * np.stack([np.ones(len(A)), np.ones(len(A)), d], axis=1)[:, None, :]) @ vt
+
+    def grad_tr(self, P, R_hat, vol0):
+        """deformation_gradient_tr_i = sum_j (vol0_j grad W0_ij) (R_i^T p_j - q_j)^T (:139-180), fed R_hat and vol0 read back
+        (N, 3, 3), row-major.  R^T p - q cancels, so its absolute evaluation |R|^T |p| + |q| is carried in A."""
+        r, N = self.rest, self.N
+        R = np.asarray(R_hat, np.float64)
+        v0 = _f64(vol0)
+        p, q = self._pq(P)
+        uu = np.einsum("nki,nk->ni", R[r.i], p) - q
+        uA = np.einsum("nki,nk->ni", np.abs(R[r.i]), np.abs(p)) + np.abs(q)
+        a = (self.g * v0[r.j])[:, None] * r.x
+        aA = np.abs(a)
+        aK = (self.ge * np.abs(v0[r.j]))[:, None] * np.abs(r.x)
+        t = lambda x, y: np.stack([_sum(N, r.i, x[:, k, None] * y).reshape(N, 3) for k in range(3)], axis=1).reshape(N, 9)  # noqa: E731
+        return Ref(t(a, uu), t(aA, uA), t(aK, uA), self.n)
+
+    def stress(self, G):
+        """Stress (x y z w a b) from deformation_gradient_tr G (N, 3, 3) read back (:182-262): linear, with the diagonal of G
+        as the strain, or nonlinear, with J J^T - I, J = G + I; k = 0.564.  Ref with A the absolute evaluation (no sum)."""
+        G = np.asarray(G, np.float64)
+        k, d0, d1, d2 = float(F(0.564)), self.d0, self.d1, self.d2
+        I = np.eye(3)
+        if self.nonlinear:
+            J, JA = G + I, np.abs(G) + I
+            M, MA = J @ J.transpose(0, 2, 1), JA @ JA.transpose(0, 2, 1)
+            e, eA = np.diagonal(M, axis1=1, axis2=2) - 1.0, np.diagonal(MA, axis1=1, axis2=2) + 1.0
+            off, offA, ks = (M[:, 1, 0], M[:, 2, 0], M[:, 2, 1]), (MA[:, 1, 0], MA[:, 2, 0], MA[:, 2, 1]), k
+        else:
+            e, eA = np.diagonal(G, axis1=1, axis2=2), np.abs(np.diagonal(G, axis1=1, axis2=2))
+            off = (G[:, 1, 0] + G[:, 0, 1], G[:, 2, 0] + G[:, 0, 2], G[:, 1, 2] + G[:, 2, 1])
+            offA = (np.abs(G[:, 1, 0]) + np.abs(G[:, 0, 1]), np.abs(G[:, 2, 0]) + np.abs(G[:, 0, 2]),
+                    np.abs(G[:, 1, 2]) + np.abs(G[:, 2, 1]))
+            ks = 1.0
+        D = np.array([[d0, d1, d1], [d1, d0, d1], [d1, d1, d0]])
+        val = np.concatenate([(e @ D.T) * ks, np.stack(off, 1) * k * d2], axis=1)
+        A = np.concatenate([(eA @ np.abs(D).T) * ks, np.stack(offA, 1) * k * abs(d2)], axis=1)
+        N = len(G)
+        return Ref(val, A, np.zeros_like(A), np.zeros(N))
+
+    def force(self, S, G, R_hat, vol0, r_i_for_r_j=False, g_i_for_g_j=False):
+        """The acceleration sum_j 0.5 (R_j f_ij - R_i f_ji) / m_i (:268-334), fed the stress S (N, 6), G, R_hat (N, 3, 3) and
+        vol0 read back; f_ji = (s_i d_ij [+ G_i s_i d_ij]) (-vol0_i) with d_ij = grad W0_ij vol0_j, and f_ij likewise with
+        j's stress, G and d_ji = -grad W0_ij vol0_i.  r_i_for_r_j / g_i_for_g_j: R_i / G_i in place of R_j / G_j."""
+        r, N = self.rest, self.N
+        S, G, R, v0 = np.asarray(S, np.float64), np.asarray(G, np.float64), np.asarray(R_hat, np.float64), _f64(vol0)
+        sym = S[:, [0, 3, 4, 3, 1, 5, 4, 5, 2]].reshape(N, 3, 3)
+        Rj = R[r.i] if r_i_for_r_j else R[r.j]
+        Gj = G[r.i] if g_i_for_g_j else G[r.j]
+
+        def terms(gk, absolute):
+            ab = np.abs if absolute else (lambda x: x)
+            grad = gk[:, None] * (np.abs(r.x) if absolute else r.x)
+            d_ij, d_ji = grad * ab(v0[r.j])[:, None], grad * (ab(v0[r.i]) if absolute else -v0[r.i])[:, None]
+            sd_ij = np.einsum("nab,nb->na", ab(sym[r.i]), d_ij)
+            sd_ji = np.einsum("nab,nb->na", ab(sym[r.j]), d_ji)
+            if self.nonlinear:
+                sd_ij = sd_ij + np.einsum("nab,nb->na", ab(G[r.i]), sd_ij)
+                sd_ji = sd_ji + np.einsum("nab,nb->na", ab(Gj), sd_ji)
+            f_ji = sd_ij * (ab(v0[r.i]) if absolute else -v0[r.i])[:, None]
+            f_ij = sd_ji * (ab(v0[r.j]) if absolute else -v0[r.j])[:, None]
+            a, b = np.einsum("nab,nb->na", ab(Rj), f_ij), np.einsum("nab,nb->na", ab(R[r.i]), f_ji)
+            return ((a + b) if absolute else (a - b)) * (0.5 / self.mass[r.i])[:, None]
+
+        t, tA, tK = terms(self.g, False), terms(np.abs(self.g), True), terms(self.ge, True)
+        return Ref(_sum(N, r.i, t), _sum(N, r.i, tA), _sum(N, r.i, tK), self.n)
+
+
+def from_matrix_eps(A, R0, eps=EPS32, max_iter=20):
+    """nalgebra 0.33 Rotation3::from_matrix_eps (Mueller et al. 2016) in float64, vectorised over (N, 3, 3): from R0, while
+    |aa| > eps with aa = sum_k r_k x a_k / (|sum_k r_k . a_k| + eps) (columns), R <- rot(aa) R.  Returns (R, iterations),
+    iterations = 20 where the loop did not stop by itself."""
+    R = R0.copy()
+    iters = np.zeros(len(A), np.int64)
+    active = np.ones(len(A), bool)
+    for _ in range(max_iter):
+        axis = sum(np.cross(R[:, :, k], A[:, :, k]) for k in range(3))
+        denom = sum((R[:, :, k] * A[:, :, k]).sum(1) for k in range(3))
+        aa = axis / (np.abs(denom) + eps)[:, None]
+        active &= (aa * aa).sum(1) > eps * eps
+        if not active.any():
+            break
+        ang = np.linalg.norm(aa, axis=1)
+        u = aa / np.where(ang > 0, ang, 1.0)[:, None]
+        K = np.zeros((len(A), 3, 3))
+        K[:, 0, 1], K[:, 0, 2], K[:, 1, 2] = -u[:, 2], u[:, 1], -u[:, 0]
+        K[:, 1, 0], K[:, 2, 0], K[:, 2, 1] = u[:, 2], -u[:, 1], u[:, 0]
+        D = np.eye(3) + np.sin(ang)[:, None, None] * K + (1 - np.cos(ang))[:, None, None] * (K @ K)
+        R[active] = (D @ R)[active]
+        iters[active] += 1
+    return R, iters
 
 
 def _f64(a):

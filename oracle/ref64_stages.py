@@ -1,5 +1,6 @@
 """Feed each DFSPH gather pass its own inputs and check its output against oracle/ref64.py, particle by particle (the IISPH
-passes: Checks.iisph_stages).
+passes: Checks.iisph_stages; the WCSPH, He2014, DFSPHViscosity and Becker2009 plugins: Checks.wcsph, .he2014, .viscosity,
+.becker).
 
 TEST INFRASTRUCTURE ONLY.  A world (salva_b200.LiquidWorld or oracle.OracleWorld: the same driving code checks both) is
 replayed from scratch once per stage, with the loop shapes pinned by force_iterations(n_div, n_press) and gravity 0:
@@ -177,6 +178,13 @@ def scene_two_fluids():
                                  filter=1, want_forces=True)])
 
 
+def light(scene):
+    """The scene with every rest density divided by 1000.  DFSPHViscosity's matrix scales as 1 / rho0: at water's density
+    its determinant lies below the 1e-6 gate almost everywhere and beta is 0; here it lies above."""
+    out = dict(scene, fluids=[dict(f, density0=f["density0"] / 1000.0) for f in scene["fluids"]])
+    return out
+
+
 SCENES = dict(block=scene_block, far=scene_far, gate=scene_gate, pairs=scene_pairs, volumes=scene_volumes,
               two_fluids=scene_two_fluids, **{"tail%d" % n: (lambda n=n: scene_tail(n)) for n in TAILS})
 
@@ -197,6 +205,26 @@ def populate(world, scene, forces=()):
 
 
 IISPH_SCRATCH = ("pressure", "dii", "aii", "dij_pjl")
+HE2014_SCRATCH = ("he2014_color", "he2014_gradc")
+VISC_SCRATCH = ("visc_beta", "visc_target")
+EL_SCRATCH = ("el_volume0", "el_rotation", "el_grad_tr", "el_stress")
+
+
+def deform(P, fid, angle, seed):
+    """Each fluid's positions rotated by `angle` degrees about a tilted axis through its centre, stretched by a few percent
+    along x and compressed along y, plus jitter of 0.2 % of the particle radius."""
+    rng = np.random.default_rng(seed)
+    ax = np.array([0.3, 1.0, 0.2]) / np.linalg.norm([0.3, 1.0, 0.2])
+    t = np.radians(angle)
+    K = np.array([[0, -ax[2], ax[1]], [ax[2], 0, -ax[0]], [-ax[1], ax[0], 0]])
+    rot = np.eye(3) + np.sin(t) * K + (1 - np.cos(t)) * K @ K
+    M = rot @ np.diag([1.03, 0.98, 1.01])
+    out = np.asarray(P, np.float64).copy()
+    for k in np.unique(fid):
+        sel = fid == k
+        c = out[sel].mean(axis=0)
+        out[sel] = c + (out[sel] - c) @ M.T
+    return (out + rng.normal(0, 0.002 * R, out.shape)).astype(F)
 
 
 def _read(world, fh, bh, extra=()):
@@ -276,7 +304,15 @@ MUTANTS = ("drop_entries_32_35", "swap_vy_vz_odd", "gate_at_21", "normals_rho_i"
            "no_kappa_gate", "drop_last_boundary", "bforce_no_inv_dt", "artificial_no_vr_gate",
            # IISPH
            "dji_mass_j", "s_without_dii_p", "dij_prho_i", "next_p_no_boundary", "no_relaxation", "velocity_prho_i_twice",
-           "no_warm_start", "error_counts_clamped", "iisph_bforce_no_mass")
+           "no_warm_start", "error_counts_clamped", "iisph_bforce_no_mass",
+           # surface tension plugins
+           "wcsph_inverted_mass_ratio", "he2014_colors_no_boundary", "he2014_gradc_by_cj", "he2014_gradc_i_twice",
+           "he2014_reaction_sign",
+           # Becker2009 elasticity
+           "el_volume_once", "el_r_i_for_r_j", "el_g_i_for_g_j", "el_rest_lists_recaptured",
+           "el_recapture_no_old_volumes", "el_second_fluid_no_offset",
+           # DFSPHViscosity
+           "visc_precondition_columns", "visc_target_no_scale", "visc_vv_no_adt", "visc_u_j_beta_i")
 
 
 class Checks:
@@ -314,12 +350,15 @@ class Checks:
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()))
         self.excluded[name] = self.excluded.get(name, 0) + int((ex & self.want).sum())
 
-    def record(self, name, gpu, ref, c_pass, exclude=None, ps=None):
+    def record(self, name, gpu, ref, c_pass, exclude=None, ps=None, ambiguous=True):
+        """ambiguous = False: the pass does not run on ps's contacts (Becker's rest contacts), so ps's pairs at the
+        gradient's zero threshold do not exclude anything."""
         ps = ps or self.ps
         r = ref64.ratio(gpu, ref, c_pass)
         if r.ndim == 2:
             r = r.max(axis=1)
-        ex = ps.ambiguous() if exclude is None else exclude | ps.ambiguous()
+        amb = ps.ambiguous() if ambiguous else np.zeros(len(r), bool)
+        ex = amb if exclude is None else exclude | amb
         r = np.where(ex, 0.0, r)
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()) if len(r) else 0.0)
         self.excluded[name] = self.excluded.get(name, 0) + int(ex.sum())
@@ -534,6 +573,168 @@ class Checks:
                                           vr_gate=self.mutant != "artificial_no_vr_gate")
             assert amb.mean() <= 0.02, "%s: %d of %d particles at the v_r < 0 decision" % (name, amb.sum(), len(amb))
             self.record(name, o["acceleration"], ref, C_PASS["artificial"], exclude=amb)
+
+    def wcsph(self, cf=0.5):
+        """WCSPHSurfaceTension on the first step with no update (0, 0): the acceleration is its fluid term.  Its boundary
+        coefficient must be 0 (include/sph.h), so there is no boundary term."""
+        from salva_b200 import scenes
+        o, _ = run(self.make_world, self.scene, (0, 0), [scenes.wcsph_surface_tension(cf)])
+        ref = self.ps.wcsph(cf, inverted_mass_ratio=self.mutant == "wcsph_inverted_mass_ratio")
+        self.record("wcsph", o["acceleration"], ref, C_PASS["wcsph"])
+
+    def he2014(self, cf=0.5, cb=0.3):
+        """He2014SurfaceTension on the first step with no update (0, 0), each pass fed what its kernel read: the colours on
+        the step's densities, gradc on the colours read back, the acceleration (the force: gravity 0) and the boundary
+        reaction on gradc read back.  With cb = 0 the boundaries that want forces get none."""
+        from salva_b200 import scenes
+        ps, m = self.ps, self.mutant
+        o, _ = run(self.make_world, self.scene, (0, 0), [scenes.he2014_surface_tension(cf, cb)], extra=HE2014_SCRATCH)
+        dens, bvol = o["density"], o["bvol"]
+        self.record("he2014_color", o["he2014_color"], ps.he2014_colors(dens, bvol, boundary=m != "he2014_colors_no_boundary"),
+                    C_PASS["he2014_color"])
+        self.record("he2014_gradc", o["he2014_gradc"],
+                    ps.he2014_gradc(dens, o["he2014_color"], C_PASS["he2014_gradc"], divide_by_cj=m == "he2014_gradc_by_cj"), 0)
+        tag = "fluid" if cb == 0 else "boundary" if cf == 0 else "both"
+        self.record("he2014_force_" + tag, o["acceleration"],
+                    ps.he2014_force(dens, o["he2014_gradc"], cf, cb, bvol, gradc_i_twice=m == "he2014_gradc_i_twice"), C_PASS["he2014_force"])
+        if cb != 0:
+            ref = ps.he2014_boundary_force(dens, o["he2014_gradc"], cb, bvol, sign=1.0 if m == "he2014_reaction_sign" else -1.0)
+        else:
+            nb = len(self.want)
+            ref = ref64.Ref(np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros(nb))
+        self.record_boundary("boundary_force_he2014", o["bforce"], ref)
+
+    def viscosity(self, visc=0.5, wcsph=0.0):
+        """DFSPHViscosity.  Forces see the previous step's dt, 0 on the first step, so (as for XSPH) step 1 with (1, 0),
+        then step 2 with (0, 0) on positions P1, the velocities V2 and the densities of step 2, once with
+        max_viscosity_iter = 1 and once with 2 (max_viscosity_error = 0: no early break).  Each pass fed what its kernel
+        read: beta (residual check), the target on vv = v + a dt, the acceleration after one update (rate on the same vv,
+        beta and target read back) and after two (vv on the acceleration read back from the one-update run).  wcsph: a
+        WCSPHSurfaceTension coefficient pushed before the viscosity, so that a != 0 in vv; its acceleration comes from a
+        run with WCSPH alone."""
+        from salva_b200 import scenes
+        sc, m, kw = self.scene, self.mutant, dict(kw=self.ps.kw, kg=self.ps.kg)
+        tag = "_after_wcsph" if wcsph else ""
+        pre = [scenes.wcsph_surface_tension(wcsph)] if wcsph else []
+        runs = {k: run(self.make_world, sc, (0, 0), pre + [scenes.dfsph_viscosity(visc, 1, k, 0.0)], first=(1, 0), extra=VISC_SCRATCH)
+                for k in (1, 2)}
+        o2, o1 = runs[1]
+        ps1 = passes_for(sc, P=o1["P"], **kw)
+        dens, V = o2["density"], o2["V"]
+        a0 = run(self.make_world, sc, (0, 0), pre, first=(1, 0))[0]["acceleration"] if wcsph else np.zeros_like(V)
+        ratio, viol, amb, zero = ps1.visc_beta(dens, o2["visc_beta"], C_PASS["visc_matrix"], by_column=m == "visc_precondition_columns")
+        amb = amb | ps1.ambiguous()
+        self.worst["visc_beta" + tag] = max(self.worst.get("visc_beta" + tag, 0.0), float(np.where(amb, 0.0, ratio).max()))
+        self.worst["visc_beta_gate" + tag] = np.inf if viol else 0.0
+        self.excluded["visc_beta" + tag] = self.excluded.get("visc_beta" + tag, 0) + int(amb.sum())
+        self.visc_zero = getattr(self, "visc_zero", 0) + int(zero.sum())
+        skip = m == "visc_vv_no_adt"
+        scale = 1.0 if m == "visc_target_no_scale" else float(F(1.0) - F(visc))
+        self.record("visc_target" + tag, o2["visc_target"], ps1.visc_rates(dens, V, a0, DT, scale, skip_adt=skip),
+                    C_PASS["visc_rate"] + 1, ps=ps1)
+        inv_dt = F(1.0) / F(DT)
+        acc = a0
+        for k in (1, 2):
+            ok = runs[k][0]
+            rate = ps1.visc_rates(dens, V, acc, DT, 1.0, skip_adt=skip)
+            ref = ps1.visc_accel(dens, ok["visc_beta"], rate.value, rate.bound(C_PASS["visc_rate"]), ok["visc_target"], acc, inv_dt,
+                                 beta_i_for_j=m == "visc_u_j_beta_i")
+            self.record("visc_accel_%d%s" % (k, tag), ok["acceleration"], ref, C_PASS["visc_accel"], ps=ps1)
+            acc = runs[1][0]["acceleration"]
+
+    def becker(self, young=2.0e5, poisson=0.3, nonlinear=True, angle=40.0):
+        """Becker2009Elasticity, every pass fed what its kernel read (rest volumes, rotations, grad_tr and stress read
+        back), with no update (0, 0) so that the acceleration is the force:
+          step 1  captures the rest pose (the step's positions and same-fluid contacts): the rest volumes; the rotation
+                  within its bound of the polar rotation, which is I here; grad_tr, stress and force near 0;
+          step 2  after write_fluid imposed a deformation of each fluid about its centre (a rotation by `angle` degrees
+                  about a tilted axis, a few percent of strain and jitter): the current contacts differ from the rest
+                  contacts, and rotation, grad_tr, stress and force are checked on the rest contacts;
+          step 3  a further deformation (25 degrees): the rotation warm-started from step 2's;
+          step 4  after appending particles to every fluid: the rest pose is captured again, with the old rest volumes
+                  added to the new sums and the old rotations kept as warm starts (identity for the new particles)
+                  (becker2009_elasticity.rs:84-113, Vec::resize)."""
+        from salva_b200 import scenes
+        sc, ps, m = self.scene, self.ps, self.mutant
+        w = self.make_world()
+        fh, bh = populate(w, sc, [scenes.becker2009_elasticity(young, poisson, nonlinear)])
+        w.force_iterations(0, 0)
+        Q = np.concatenate([f["positions"] for f in sc["fluids"]]).astype(F)
+        same = lambda fid: (lambda i, j: fid[i] == fid[j])  # noqa: E731
+        bk = ref64.Becker(ps.h, Q, ps.fid, ps.mass, young, poisson, nonlinear)
+        tag = "nonlinear" if nonlinear else "linear"
+        w.step(DT, ZERO_G)
+        o = _read(w, fh, bh, EL_SCRATCH)
+        self.record("el_volume", ps.mass / o["el_volume0"].astype(np.float64), bk.volume_sum(1.0 if m == "el_volume_once" else 2.0),
+                    C_PASS["el_volume"], exclude=np.zeros(ps.N, bool), ambiguous=False)
+        self._becker_step(bk, Q, o, np.tile(np.eye(3), (ps.N, 1, 1)), "el_rest_" + tag)
+        R_prev = o["el_rotation"].reshape(ps.N, 3, 3).astype(np.float64)
+        if m == "el_rest_lists_recaptured":
+            P2 = deform(o["P"], ps.fid, angle, seed=29)
+            bk = ref64.Becker(ps.h, Q, ps.fid, ps.mass, young, poisson, nonlinear, rest=ref64.contacts(P2, P2, ps.h, same(ps.fid), same=True))
+        for name, ang, seed in (("el_deformed_", angle, 29), ("el_warm_", 25.0, 31)):
+            P = deform(o["P"], ps.fid, ang, seed=seed)
+            for k, f in enumerate(fh):
+                w.write_fluid(f, positions=P[ps.fid == k])
+            w.step(DT, ZERO_G)
+            o = _read(w, fh, bh, EL_SCRATCH)
+            self._becker_step(bk, P, o, R_prev, name + tag)
+            R_prev = o["el_rotation"].reshape(ps.N, 3, 3).astype(np.float64)
+            if name == "el_deformed_":   # rest contacts against the same-fluid contacts at P
+                cur = ref64.contacts(P, P, ps.h, same(ps.fid), same=True)
+                self.rest_differs = int((np.bincount(bk.rest.i, minlength=ps.N) != np.bincount(cur.i, minlength=ps.N)).sum())
+        # re-capture: 7 particles appended to every fluid, near particles of it
+        P, vol0 = o["P"], o["el_volume0"]
+        vdef = F(R) * F(R) * F(R) * F(8.0 * 0.8)
+        pos, fid, mass, old_vol, old_rot = [], [], [], [], []
+        for k, f in enumerate(fh):
+            sel = np.nonzero(ps.fid == k)[0]
+            new = (P[sel[5:68:9]] + np.array([0.4, 0.1, 0.2], F) * F(R)).astype(F)
+            w.append_particles(f, new)
+            pos += [P[sel], new]
+            fid += [np.full(len(sel) + len(new), k)]
+            mass += [ps.mass[sel], np.full(len(new), F(vdef * F(sc["fluids"][k]["density0"])), F)]   # appended: default volume
+            old_vol += [vol0[sel], np.zeros(len(new))]
+            old_rot += [R_prev[sel], np.tile(np.eye(3), (len(new), 1, 1))]
+        Q4, fid4, mass4 = np.concatenate(pos).astype(F), np.concatenate(fid), np.concatenate(mass).astype(F)
+        w.step(DT, ZERO_G)
+        o = _read(w, fh, bh, EL_SCRATCH)
+        bk4 = ref64.Becker(ps.h, Q4, fid4, mass4, young, poisson, nonlinear)
+        old = np.zeros(len(Q4)) if m == "el_recapture_no_old_volumes" else np.concatenate(old_vol)
+        self.record("el_recaptured_volume", mass4 / o["el_volume0"].astype(np.float64),
+                    bk4.volume_sum(2.0, old=old), C_PASS["el_volume"],
+                    exclude=np.zeros(len(Q4), bool), ambiguous=False)
+        self._becker_step(bk4, Q4, o, np.concatenate(old_rot), "el_recaptured_" + tag)
+        if hasattr(w, "close"):
+            w.close()
+
+    def _becker_step(self, bk, P, o, R_prev, name):
+        N, m = bk.N, self.mutant
+        R = o["el_rotation"].reshape(N, 3, 3).astype(np.float64)
+        G = o["el_grad_tr"].reshape(N, 3, 3)
+        if m == "el_second_fluid_no_offset" and bk.fid.max() > 0:   # the second fluid reads the first one's positions
+            P = np.asarray(P, F).copy()
+            sel = np.nonzero(bk.fid == 1)[0]
+            P[sel] = P[np.nonzero(bk.fid == 0)[0][:len(sel)]]
+        none = np.zeros(N, bool)
+        r, ortho, ex, Rref, iters = bk.rotation(P, R, R_prev, C_PASS["el_apq"])
+        # the scenes' edges: how far the float64 run turned from its warm start, in how many iterations, and that it ends
+        # on the polar rotation (no other stationary point of the iteration)
+        ok = ~ex
+        turn = np.degrees(np.arccos(np.clip((np.einsum("nij,nij->n", R_prev, Rref) - 1) / 2, -1, 1)))
+        self.el_turn = max(getattr(self, "el_turn", 0.0), float(turn[ok].min()) if ok.any() else 0.0)
+        self.el_iterations = max(getattr(self, "el_iterations", 0), int(iters[ok].max()) if ok.any() else 0)
+        gap = np.abs(Rref - bk.polar(bk.apq(P, C_PASS["el_apq"])[0])).max(axis=(1, 2))
+        self.el_polar_gap = max(getattr(self, "el_polar_gap", 0.0), float(gap[ok].max()) if ok.any() else 0.0)
+        self.worst[name + "_rotation"] = max(self.worst.get(name + "_rotation", 0.0), float(r.max()))
+        self.excluded[name + "_rotation"] = self.excluded.get(name + "_rotation", 0) + int(ex.sum())
+        self.worst[name + "_orthonormal"] = max(self.worst.get(name + "_orthonormal", 0.0), float(ortho.max()))
+        kw = dict(exclude=none, ambiguous=False)
+        self.record(name + "_grad_tr", G.reshape(N, 9), bk.grad_tr(P, R, o["el_volume0"]), C_PASS["el_grad_tr"], **kw)
+        self.record(name + "_stress", o["el_stress"], bk.stress(G), ref64.C_EL_STRESS, **kw)
+        self.record(name + "_force", o["acceleration"],
+                    bk.force(o["el_stress"], G, R, o["el_volume0"], r_i_for_r_j=m == "el_r_i_for_r_j",
+                             g_i_for_g_j=m == "el_g_i_for_g_j"), C_PASS["el_force"], **kw)
 
     def flagged(self):
         return {k: v for k, v in self.worst.items() if not v <= 1.0}

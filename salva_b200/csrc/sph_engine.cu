@@ -79,6 +79,7 @@ struct ForceRec {
     ElasticityState* elastic = nullptr;  // Becker2009 rest-pose state (sph_elasticity.cuh)
     uint32_t visc_iters = 0;             // DFSPHViscosity: acceleration updates of the last solve
     float visc_err = 0.f;                // ... and its last strain-rate error
+    bool solved = false;                 // has run in a step (sph_debug_read's plugin scratch is valid until particles change)
 };
 struct FluidRec {
     size_t n = 0, offset = 0;
@@ -1474,6 +1475,7 @@ sph_status phase_forces(sph_world* w) {
                 default:
                     return w->fail(SPH_ERR_INVALID, "unknown force kind %d", fr.d.kind);
             }
+            fr.solved = true;
         }
     CU(cudaGetLastError());
     return SPH_OK;
@@ -2265,6 +2267,19 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     const bool iisph_sel = what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_AII || what == SPH_DBG_IISPH_DIJ_PJL;
     if (iisph_sel && (w->desc.solver != SPH_SOLVER_IISPH || !w->iisph.dii || w->own_begin + w->N > w->iisph.cap))
         return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs an IISPH world that has stepped with its current particles", what);
+    // plugin scratch: that of the fluid's last force of the selector's kind, solved since its particles last changed
+    const ForceRec* pf = nullptr;
+    if (what >= SPH_DBG_HE2014_COLOR && what <= SPH_DBG_EL_STRESS) {
+        static const uint32_t widths[] = {1, 1, 36, 6, 1, 9, 9, 6};
+        width = widths[what - SPH_DBG_HE2014_COLOR];
+        const int kind = what <= SPH_DBG_HE2014_GRADC ? SPH_FORCE_HE2014_TENSION
+                         : what <= SPH_DBG_VISC_TARGET ? SPH_FORCE_DFSPH_VISCOSITY : SPH_FORCE_BECKER2009_ELASTICITY;
+        for (const ForceRec& fr : f.forces)
+            if (fr.d.kind == kind) pf = &fr;
+        const bool el = kind == SPH_FORCE_BECKER2009_ELASTICITY;
+        if (!pf || w->staged || !pf->solved || (el && (!pf->elastic || pf->elastic->n != f.n)))
+            return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs a force of kind %d solved with the fluid's current particles", what, kind);
+    }
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
         if (what == SPH_DBG_VELOCITY_CHANGE) memcpy(out, w->h_vc.data() + 3 * f.offset, 3 * f.n * sizeof(float));
@@ -2274,7 +2289,18 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     TRY(enter(w));
     size_t N = w->N;
     int c = w->cur;
-    CU(w->o_c.ensure(3 * std::max(N, w->B)));
+    CU(w->o_c.ensure(std::max(width * N, 3 * std::max(N, w->B))));
+    if (pf && pf->elastic) {  // the rest pose is kept in the fluid's original order already
+        const ElasticityState& E = *pf->elastic;
+        const float* src = what == SPH_DBG_EL_ROTATION ? E.rot : what == SPH_DBG_EL_GRAD_TR ? E.grad_tr : E.stress;
+        if (what == SPH_DBG_EL_VOLUME0) {
+            LAUNCH(k_export_w_plain, f.n, 256, (uint32_t)f.n, E.pos0, w->o_c.p);
+            src = w->o_c.p;
+        }
+        CU(cudaMemcpyAsync(out, src, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+        CU(cudaStreamSynchronize(w->st));
+        return SPH_OK;
+    }
     const float* s1 = nullptr;
     switch (what) {
         case SPH_DBG_DENSITY: s1 = w->dens.p; break;
@@ -2283,6 +2309,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         case SPH_DBG_PREDICTED_DENSITY: s1 = w->desc.solver == SPH_SOLVER_IISPH ? iisph_pred(w) : w->pred.p; break;
         case SPH_DBG_PRESSURE: s1 = w->press[c].p; break;
         case SPH_DBG_IISPH_AII: s1 = w->iisph.aii; break;
+        case SPH_DBG_HE2014_COLOR: s1 = w->he_colors.p; break;
+        case SPH_DBG_HE2014_GRADC: s1 = w->he_gradc.p; break;
         default: break;
     }
     const uint32_t ob = w->own_begin;
@@ -2292,6 +2320,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     else if (what == SPH_DBG_ACCELERATION) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->acc.p + ob, w->o_c.p);
     else if (what == SPH_DBG_IISPH_DII) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dii + ob, w->o_c.p);
     else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl + ob, w->o_c.p);
+    else if (what == SPH_DBG_VISC_BETA) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 36u, w->stride, og, w->visc.beta + ob, w->o_c.p);
+    else if (what == SPH_DBG_VISC_TARGET) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 6u, w->stride, og, w->visc.target + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_f.p + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_b.p + ob, w->o_c.p);
     else return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);

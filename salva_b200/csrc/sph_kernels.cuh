@@ -1201,6 +1201,14 @@ __global__ void k_export1u(uint32_t n, const uint32_t* __restrict__ orig, const 
     if (s >= n) return;
     dst[orig[s]] = (float)src[s];
 }
+// `width` planes src[k * stride + s] indexed by sorted index -> original order, packed width floats per particle
+__global__ void k_export_planes(uint32_t n, uint32_t width, uint32_t stride, const uint32_t* __restrict__ orig, const float* __restrict__ src,
+                                float* __restrict__ dst) {
+    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= n) return;
+    uint32_t g = orig[s];
+    for (uint32_t k = 0; k < width; ++k) dst[(size_t)width * g + k] = src[(size_t)k * stride + s];
+}
 // accelerations back from a host force callback: acc[s].xyz = src[orig[s]] for the particles of one fluid
 __global__ void k_import_acc(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ src, uint32_t lo, uint32_t hi, float4* __restrict__ acc) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;

@@ -18,8 +18,10 @@ from . import _lib
 from ._lib import ForceDesc, StepStats, WorldDesc
 
 DBG = dict(density=0, alpha=1, divergence=2, predicted_density=3, velocity_change=4, num_fluid_contacts=5,
-           num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11)
-_VEC = {4, 8, 9, 11}
+           num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11, he2014_color=12, he2014_gradc=13,
+           visc_beta=14, visc_target=15, el_volume0=16, el_rotation=17, el_grad_tr=18, el_stress=19)
+# floats per particle of the selectors that are not scalars (include/sph.h)
+WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6}
 
 
 class SphError(RuntimeError):
@@ -559,6 +561,6 @@ class LiquidWorld:
     def debug(self, fluid, what):
         code = DBG[what] if isinstance(what, str) else what
         n = self.num_particles(fluid)
-        out = np.zeros((n, 3) if code in _VEC else (n,), np.float32)
+        out = np.zeros((n, WIDTH[code]) if code in WIDTH else (n,), np.float32)
         self._ck(self._L.sph_debug_read(self._w, fluid, code, _fp(out), n))
         return out

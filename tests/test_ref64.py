@@ -186,6 +186,188 @@ def test_plausible_kernel_bugs_are_caught(mutant):
     assert must <= flagged, (flagged, c.worst)
 
 
+TENSION_SCENES = ("block", "pairs", "two_fluids", "volumes", "tail1", "tail33")
+
+
+def _tension(c):
+    c.wcsph(0.5)
+    for cf, cb in ((0.5, 0.0), (0.0, 0.3), (0.5, 0.3)):
+        c.he2014(cf, cb)
+    return c
+
+
+@pytest.mark.parametrize("name", TENSION_SCENES)
+def test_the_cpu_oracle_meets_every_surface_tension_bound(name):
+    c = _tension(S.Checks(_oracle(), S.SCENES[name]()))
+    assert not c.flagged(), c.worst
+    assert {"wcsph", "he2014_color", "he2014_gradc", "he2014_force_fluid", "he2014_force_boundary", "he2014_force_both"} <= set(c.worst)
+    if name == "two_fluids":   # the walls want their forces: He2014's reaction is checked
+        assert "boundary_force_he2014" in c.worst
+
+
+@pytest.mark.parametrize("kd,kg", [(1, 2), (3, 1)], ids=["poly6+spiky", "viscosity+poly6"])
+def test_the_cpu_oracle_meets_every_surface_tension_bound_with_generic_kernels(kd, kg):
+    c = _tension(S.Checks(_oracle(kd, kg), S.SCENES["two_fluids"](), kw=kd, kg=kg))
+    assert not c.flagged(), c.worst
+
+
+def test_the_he2014_gradc_bound_is_not_vacuous():
+    """gradc's bound is carried through the cancelling vector sum explicitly; it stays far below gradc where the colour
+    gradient does not cancel (the free surface), so a relative error of a few percent there is caught."""
+    from salva_b200 import scenes
+    sc = S.scene_block()
+    w = _oracle()()
+    fh, _ = S.populate(w, sc, [scenes.he2014_surface_tension(0.5, 0.0)])
+    w.force_iterations(0, 0)
+    w.step(S.DT, S.ZERO_G)
+    ps = S.passes_for(sc)
+    ref = ps.he2014_gradc(w.debug(fh[0], "density"), w.debug(fh[0], "he2014_color"), ref64.C_PASS["he2014_gradc"])
+    surface = ref.value > np.quantile(ref.value, 0.9)
+    assert (ref.bound(0)[surface] < 1e-3 * ref.value[surface]).all()
+
+
+# mutant -> (scene, the passes that must flag it)
+TENSION_MUTANTS = {
+    "wcsph_inverted_mass_ratio": ("volumes", {"wcsph"}),
+    "he2014_colors_no_boundary": ("block", {"he2014_color"}),
+    "he2014_gradc_by_cj": ("block", {"he2014_gradc"}),
+    "he2014_gradc_i_twice": ("block", {"he2014_force_fluid", "he2014_force_both"}),
+    "he2014_reaction_sign": ("two_fluids", {"boundary_force_he2014"}),
+}
+
+
+@pytest.mark.parametrize("mutant", sorted(TENSION_MUTANTS))
+def test_plausible_surface_tension_kernel_bugs_are_caught(mutant):
+    scene, must = TENSION_MUTANTS[mutant]
+    flagged = set(_tension(S.Checks(_oracle(), S.SCENES[scene](), mutant=mutant)).flagged())
+    assert must <= flagged, flagged
+
+
+BECKER_SCENES = ("block", "two_fluids", "volumes")
+
+
+def _becker(c):
+    c.becker(nonlinear=True)
+    c.becker(nonlinear=False)
+    return c
+
+
+@pytest.mark.parametrize("name", BECKER_SCENES)
+def test_the_cpu_oracle_meets_every_becker_bound(name):
+    c = _becker(S.Checks(_oracle(), S.SCENES[name]()))
+    assert not c.flagged(), c.worst
+    for stage in ("el_rest", "el_deformed", "el_warm", "el_recaptured"):
+        for kind in ("nonlinear", "linear"):
+            assert {"%s_%s_%s" % (stage, kind, p) for p in ("rotation", "orthonormal", "grad_tr", "stress", "force")} <= set(c.worst)
+    # the deformation turned every checked particle by more than 20 degrees, some over many iterations; the float64 run
+    # ends on the polar rotation; the current contacts differ from the rest contacts for many particles
+    assert c.el_turn >= 20 and c.el_iterations >= 5, (c.el_turn, c.el_iterations)
+    assert c.el_polar_gap <= 1e-6, c.el_polar_gap
+    assert c.rest_differs >= 100, c.rest_differs
+    assert "el_recaptured_volume" in c.worst
+
+
+def test_the_cpu_oracle_meets_every_becker_bound_under_iisph():
+    """Becker runs under IISPH in the C5 configuration."""
+    c = _becker(S.Checks(_iisph(), S.SCENES["two_fluids"]()))
+    assert not c.flagged(), c.worst
+    assert max(v for k, v in c.excluded.items() if k.endswith("rotation")) <= 0.05 * c.ps.N, c.excluded   # per stage
+
+
+def test_the_becker_rest_lists_exceed_the_initial_capacity():
+    sc = S.scene_block()
+    ps = S.passes_for(sc)
+    bk = ref64.Becker(ps.h, ps.P, ps.fid, ps.mass, 2e5, 0.3, True)
+    assert bk.n.max() > 64
+
+
+BECKER_MUTANTS = {
+    "el_volume_once": ("block", {"el_volume"}),
+    "el_r_i_for_r_j": ("block", {"el_deformed_nonlinear_force", "el_deformed_linear_force"}),
+    "el_g_i_for_g_j": ("block", {"el_deformed_nonlinear_force"}),
+    "el_rest_lists_recaptured": ("two_fluids", {"el_deformed_nonlinear_rotation", "el_deformed_nonlinear_grad_tr",
+                                                "el_deformed_nonlinear_force"}),
+    "el_second_fluid_no_offset": ("two_fluids", {"el_deformed_nonlinear_rotation", "el_deformed_nonlinear_grad_tr"}),
+    # the old rest volumes are about 1e-7 of the sum at water's density, below float32's resolution: a light fluid
+    "el_recapture_no_old_volumes": ("light_two_fluids", {"el_recaptured_volume"}),
+}
+
+
+def _scene(name):
+    return S.light(S.SCENES[name[6:]]()) if name.startswith("light_") else S.SCENES[name]()
+
+
+@pytest.mark.parametrize("mutant", sorted(BECKER_MUTANTS))
+def test_plausible_becker_kernel_bugs_are_caught(mutant):
+    scene, must = BECKER_MUTANTS[mutant]
+    flagged = set(_becker(S.Checks(_oracle(), _scene(scene), mutant=mutant)).flagged())
+    assert must <= flagged, flagged
+
+
+# DFSPHViscosity: on light fluids beta is non-zero everywhere; at water's density (block) and for a lone particle (tail1)
+# the determinant gate sets it to 0
+VISC_SCENES = ("light_block", "light_two_fluids", "light_volumes", "block", "tail1")
+
+
+def _visc(c):
+    c.viscosity(0.5)
+    c.viscosity(0.5, wcsph=2.0)
+    return c
+
+
+@pytest.mark.parametrize("name", VISC_SCENES)
+def test_the_cpu_oracle_meets_every_viscosity_bound(name):
+    c = _visc(S.Checks(_oracle(), _scene(name)))
+    assert not c.flagged(), c.worst
+    assert {"visc_beta", "visc_beta_gate", "visc_target", "visc_accel_1", "visc_accel_2", "visc_target_after_wcsph",
+            "visc_accel_2_after_wcsph"} <= set(c.worst)
+    if name.startswith("light_"):
+        assert c.visc_zero == 0 and sum(c.excluded.values()) <= 4, (c.visc_zero, c.excluded)
+    else:   # most particles on the beta = 0 path, the gate checked for each
+        assert c.visc_zero >= c.ps.N, c.visc_zero
+
+
+VISC_MUTANTS = {
+    "visc_precondition_columns": ("light_block", {"visc_beta"}),
+    "visc_target_no_scale": ("light_block", {"visc_target"}),
+    "visc_vv_no_adt": ("light_block", {"visc_target_after_wcsph", "visc_accel_1_after_wcsph", "visc_accel_2"}),
+    "visc_u_j_beta_i": ("light_block", {"visc_accel_1", "visc_accel_2"}),
+}
+
+
+@pytest.mark.parametrize("mutant", sorted(VISC_MUTANTS))
+def test_plausible_viscosity_kernel_bugs_are_caught(mutant):
+    scene, must = VISC_MUTANTS[mutant]
+    flagged = set(_visc(S.Checks(_oracle(), _scene(scene), mutant=mutant)).flagged())
+    assert must <= flagged, flagged
+
+
+def test_the_plugin_scratch_is_refused_without_its_force():
+    """The CPU oracle's selectors 12-19 refuse a fluid without the force, or before it has been solved; with it they have
+    one row of the selector's width per particle."""
+    from salva_b200 import scenes
+    sc = S.scene_tail(33)
+    kinds = {"he2014": scenes.he2014_surface_tension(0.5, 0.3), "visc": scenes.dfsph_viscosity(0.1),
+             "el": scenes.becker2009_elasticity(1e5, 0.3)}
+    sel = {"he2014_color": ("he2014", ()), "he2014_gradc": ("he2014", ()), "visc_beta": ("visc", (36,)),
+           "visc_target": ("visc", (6,)), "el_volume0": ("el", ()), "el_rotation": ("el", (9,)), "el_grad_tr": ("el", (9,)),
+           "el_stress": ("el", (6,))}
+    for kind, force in kinds.items():
+        for stage in ("pushed", "stepped", "written"):
+            w = _oracle()()
+            (fh,), _ = S.populate(w, sc, [force])
+            if stage != "pushed":
+                w.step(S.DT, S.ZERO_G)
+            if stage == "written":   # same particles, new positions: the last solve's scratch stays readable
+                w.write_fluid(fh, positions=w.read_fluid(fh)[0])
+            for what, (k, shape) in sel.items():
+                if k == kind and stage in ("stepped", "written"):
+                    assert w.debug(fh, what).shape == (33,) + shape
+                else:
+                    with pytest.raises(AssertionError):
+                        w.debug(fh, what)
+
+
 def test_the_list_layout_scene_reaches_its_counts():
     for name in ("block", "far"):
         ps = S.passes_for(S.SCENES[name]())
