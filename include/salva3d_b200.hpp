@@ -13,6 +13,8 @@
 //   LiquidWorld::{remove_fluid, remove_boundary, step_with_coupling, particles_intersecting_shape}          liquid_world.rs:67-178,246-281
 //   trait CouplingManager                                                                                    coupling/coupling_manager.rs:9-28
 //   NonPressureForce::solve with contacts and boundaries (CustomNonPressureForceWithContacts)                nonpressure_force.rs:15-27
+//   ColliderCouplingSet::{register_coupling, unregister_coupling} + ColliderSampling::StaticSampling, run on the device
+//   (the rigid bodies stay with the caller: set_collider_state before a step, collider_impulse after it)   fluids_pipeline.rs:64-287
 // Every call goes to libsalva_b200.so (CUDA); there is no CPU path.
 #pragma once
 #include <cstdint>
@@ -157,6 +159,12 @@ struct Isometry3 {
 struct Ball { Real radius; };
 struct Cuboid { Vector3 half_extents; };
 struct Capsule { Real half_height, radius; };  // segment along local y
+// ColliderSampling (fluids_pipeline.rs:64-72); StaticSampling is the sampling the device path implements
+struct ColliderSampling {
+    std::vector<Point3> points;  // in the collider's local frame
+    static ColliderSampling StaticSampling(std::vector<Point3> points) { return ColliderSampling{std::move(points)}; }
+};
+using ColliderHandle = uint32_t;
 
 class LiquidWorld;
 // trait CouplingManager (coupling/coupling_manager.rs:9-28)
@@ -232,6 +240,7 @@ private:
     bool want_forces_;
     uint32_t handle_ = 0;
     bool alive_ = true;
+    bool coupled_ = false;             // a collider owns the particles: they are read back, never written
     std::vector<Point3> synced_pos_;   // last upload: the engine caches the boundary sort / volumes while they are unchanged
     std::vector<Vector3> synced_vel_;
 };
@@ -357,7 +366,7 @@ public:
             }
         }
         for (Boundary& b : boundaries_) {
-            if (!b.alive_) continue;
+            if (!b.alive_ || b.coupled_) continue;
             if (b.velocities.size() != b.positions.size()) b.velocities.resize(b.positions.size());
             if (b.positions.size() != b.synced_pos_.size()) {
                 check(sph_boundary_set_particles(raw_, b.handle_, fp(b.positions), fp(b.velocities), b.positions.size()));
@@ -387,9 +396,22 @@ public:
             f.synced_vel_ = f.velocities;
         }
         for (Boundary& b : boundaries_) {
-            if (!b.alive_ || !b.num_particles()) continue;
+            if (!b.alive_) continue;
+            if (b.coupled_) {  // boundary.positions / velocities as the collider posed them
+                size_t n = 0;
+                check(sph_boundary_read(raw_, b.handle_, nullptr, nullptr, 0, &n));
+                b.positions.resize(n);
+                b.velocities.resize(n);
+                b.volumes.resize(n);
+                b.forces.resize(n);
+                if (n) check(sph_boundary_read(raw_, b.handle_, reinterpret_cast<float*>(b.positions.data()), reinterpret_cast<float*>(b.velocities.data()), n, &n));
+                b.synced_pos_ = b.positions;
+                b.synced_vel_ = b.velocities;
+            }
+            if (!b.num_particles()) continue;
             check(sph_boundary_read_volumes(raw_, b.handle_, b.volumes.data(), b.volumes.size()));
-            if (b.want_forces_) check(sph_boundary_read_forces(raw_, b.handle_, reinterpret_cast<float*>(b.forces.data()), b.forces.size()));
+            if (b.coupled_) check(sph_boundary_read_forces(raw_, b.handle_, reinterpret_cast<float*>(b.forces.data()), b.forces.size()));
+            else if (b.want_forces_) check(sph_boundary_read_forces(raw_, b.handle_, reinterpret_cast<float*>(b.forces.data()), b.forces.size()));
         }
     }
     // Snapshot / restore of the state the solver carries across steps (include/sph.h sph_world_snapshot_*).
@@ -431,6 +453,38 @@ public:
     }
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Capsule& s) {
         return shape_query(pos, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}});
+    }
+    // ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114: the boundary's particles become the collider's samples
+    ColliderHandle register_coupling(BoundaryHandle boundary, const ColliderSampling& sampling) {
+        Boundary& b = boundaries_.at(boundary);
+        uint32_t c = 0;
+        check(sph_collider_register(raw_, b.handle_, SPH_SAMPLING_STATIC, nullptr, fp(sampling.points), sampling.points.size(), &c));
+        b.coupled_ = true;
+        pull_results();
+        return c;
+    }
+    // collider.position() and its parent body for the next steps (SPH_BODY_NONE / _FIXED / _DYNAMIC)
+    void set_collider_state(ColliderHandle c, const Isometry3& pos, int body, const Vector3& linvel = Vector3(), const Vector3& angvel = Vector3(),
+                            const Point3& world_com = Point3()) {
+        sph_collider_state s;
+        s.translation[0] = pos.translation.x; s.translation[1] = pos.translation.y; s.translation[2] = pos.translation.z;
+        std::memcpy(s.rotation_rowmajor, pos.rotation, sizeof s.rotation_rowmajor);
+        s.body = body;
+        s.linvel[0] = linvel.x; s.linvel[1] = linvel.y; s.linvel[2] = linvel.z;
+        s.angvel[0] = angvel.x; s.angvel[1] = angvel.y; s.angvel[2] = angvel.z;
+        s.world_com[0] = world_com.x; s.world_com[1] = world_com.y; s.world_com[2] = world_com.z;
+        check(sph_collider_set_state(raw_, c, &s));
+    }
+    // transmit_forces fluids_pipeline.rs:263-287: (linear, angular) impulse of the last step
+    std::pair<Vector3, Vector3> collider_impulse(ColliderHandle c) {
+        float lin[3], ang[3];
+        check(sph_collider_read_impulse(raw_, c, lin, ang));
+        return {Vector3{lin[0], lin[1], lin[2]}, Vector3{ang[0], ang[1], ang[2]}};
+    }
+    // ColliderCouplingSet::unregister_coupling fluids_pipeline.rs:119-122: the boundary stays with its last particles
+    void unregister_coupling(ColliderHandle c, BoundaryHandle boundary) {
+        check(sph_collider_unregister(raw_, c));
+        boundaries_.at(boundary).coupled_ = false;
     }
     sph_step_stats counters() const {  // world.counters (counters/mod.rs:17-30)
         sph_step_stats s;

@@ -302,6 +302,45 @@ typedef struct {
 } sph_coupling_manager;
 sph_status sph_world_step_with_coupling(sph_world* w, float dt, const float gravity[3], const sph_coupling_manager* coupling);
 
+/* Collider coupling on the device: the rapier integration's ColliderCouplingSet / ColliderCouplingManager
+ * (integrations/rapier/fluids_pipeline.rs:72-287) run inside sph_world_step, where update_boundaries runs
+ * (liquid_world.rs:86-103).  The rigid-body engine stays with the caller: before each step it hands over each collider's
+ * pose and body velocities (sph_collider_set_state), after it reads the impulse the fluid applied (sph_collider_read_impulse).
+ * Colliders cannot be combined with a host sph_coupling_manager in one step, nor used in slab-decomposed worlds; a collider
+ * whose boundary was removed is inert and no longer counts.  ColliderSampling::DynamicContactSampling (fluids_pipeline.rs:71,
+ * 192-255) has no device path: contact-sample through sph_world_step_with_coupling (examples/coupling3.cpp). */
+enum { SPH_SAMPLING_STATIC = 0 };  /* ColliderSampling::StaticSampling(points)  fluids_pipeline.rs:69,180-191 */
+enum { SPH_BODY_NONE = 0,     /* collider.parent() == None: velocity 0, boundary.forces left as it is (fluids_pipeline.rs:163-171),
+                                 no impulse (transmit_forces needs the parent body, :273-276) */
+       SPH_BODY_FIXED = 1,    /* !body.is_dynamic(): boundary.forces = None, no impulse */
+       SPH_BODY_DYNAMIC = 2 };/* boundary.forces = Some, cleared every step */
+typedef struct {
+    float   translation[3];        /* collider.position(): world = rotation * local + translation */
+    float   rotation_rowmajor[9];
+    int32_t body;                  /* SPH_BODY_* */
+    float   linvel[3], angvel[3], world_com[3];  /* RigidBody::velocity_at_point(p) = linvel + angvel x (p - world_com) */
+} sph_collider_state;
+/* ColliderCouplingSet::register_coupling(boundary, collider, sampling)  fluids_pipeline.rs:98-114.  StaticSampling: the n_points
+ * local points (packed xyz) become the boundary's particles; every step they are posed by the collider's state, with the
+ * velocity velocity_at_point(pt) evaluated at the LOCAL point pt, as fluids_pipeline.rs:183 does (a quirk of the reference,
+ * reproduced).  `shape` may be NULL for StaticSampling.  The engine owns the boundary's particle set from then on:
+ * sph_boundary_write / _set_particles refuse it.  A boundary can be coupled to one collider at a time.  The initial state
+ * is the identity pose with SPH_BODY_NONE.  Handles are slot | generation << 16. */
+sph_status sph_collider_register(sph_world* w, uint32_t boundary, int32_t sampling, const sph_shape* shape, const float* local_points_xyz,
+                                 size_t n_points, uint32_t* collider);
+/* The collider's pose and body for the next steps (the reference reads collider.position() and the parent body each
+ * update_boundaries, fluids_pipeline.rs:159-186).  A StaticSampling collider whose state is bit-equal to the one of its
+ * last step leaves its boundary unchanged, so the boundary's sort and volumes are reused as for a static boundary. */
+sph_status sph_collider_set_state(sph_world* w, uint32_t collider, const sph_collider_state* state);
+/* ColliderCouplingManager::transmit_forces fluids_pipeline.rs:263-287 of the last step: linear = sum of force * dt,
+ * angular = sum of (p - world_com) x force * dt over the boundary's particles, with the step's dt.  Zero when the body is
+ * not SPH_BODY_DYNAMIC, when the boundary is empty or was removed, and before the first step. */
+sph_status sph_collider_read_impulse(sph_world* w, uint32_t collider, float linear[3], float angular[3]);
+/* ColliderCouplingSet::unregister_coupling fluids_pipeline.rs:119-122: the boundary stays, with its last particle set. */
+sph_status sph_collider_unregister(sph_world* w, uint32_t collider);
+/* boundary.positions / velocities (boundary.rs:13-15) in ORIGINAL index order.  NULL = skip; *n = particle count. */
+sph_status sph_boundary_read(sph_world* w, uint32_t boundary, float* pos_xyz, float* vel_xyz, size_t cap, size_t* n);
+
 /* Snapshot / restore of everything the solver carries ACROSS steps: positions, velocities, velocity_changes
  * (dfsph_solver.rs:44, carried :704-706), the lagging dt / inv_dt (timestep_manager.rs:29-30), IISPH warm-start pressures
  * (iisph_solver.rs:673-677), Becker-2009 rest pose and rotations (becker2009_elasticity.rs:84-135), volumes, particle ids,

@@ -68,6 +68,11 @@ class Shape(C.Structure):
     _fields_ = [("kind", C.c_int32), ("p", C.c_float * 4)]
 
 
+class ColliderState(C.Structure):
+    _fields_ = [("translation", C.c_float * 3), ("rotation_rowmajor", C.c_float * 9), ("body", C.c_int32),
+                ("linvel", C.c_float * 3), ("angvel", C.c_float * 3), ("world_com", C.c_float * 3)]
+
+
 HOST_FORCE_FN2 = C.CFUNCTYPE(None, C.c_void_p, C.POINTER(HostForceCtx))
 COUPLING_UPDATE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_float, C.c_float)
 COUPLING_TRANSMIT_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_void_p, C.c_float, C.c_float)
@@ -126,6 +131,11 @@ SYMBOLS = {
     "sph_world_snapshot_save": (C.c_int, [_vp, _vp, C.c_size_t, C.POINTER(C.c_size_t)]),
     "sph_world_snapshot_load": (C.c_int, [_vp, _vp, C.c_size_t]),
     "sph_fluid_read_ids": (C.c_int, [_vp, C.c_uint32, C.POINTER(C.c_uint32), C.c_size_t]),
+    "sph_collider_register": (C.c_int, [_vp, C.c_uint32, C.c_int32, C.POINTER(Shape), _fp, C.c_size_t, C.POINTER(C.c_uint32)]),
+    "sph_collider_set_state": (C.c_int, [_vp, C.c_uint32, C.POINTER(ColliderState)]),
+    "sph_collider_read_impulse": (C.c_int, [_vp, C.c_uint32, _fp, _fp]),
+    "sph_collider_unregister": (C.c_int, [_vp, C.c_uint32]),
+    "sph_boundary_read": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
 }
 
 

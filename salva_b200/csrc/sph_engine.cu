@@ -99,6 +99,19 @@ struct BoundaryRec {
     bool alive = true;
     uint32_t gen = 0;
 };
+// ColliderCouplingEntry (fluids_pipeline.rs:76-80) of a StaticSampling collider
+struct ColliderRec {
+    uint32_t boundary = 0;          // boundary handle; a removed boundary leaves the collider inert
+    size_t n = 0;                   // sample points
+    DBuf<float4> local;             // the points in the collider's frame
+    sph_collider_state state{};     // for the next step
+    sph_collider_state applied{};   // what the boundary's particles on the device were posed with
+    bool applied_valid = false;
+    float impulse[6] = {};          // of the last step: linear, angular
+    bool impulse_pending = false;   // this step's reduction is in flight to sph_world::h_imp
+    bool alive = true;
+    uint32_t gen = 0;
+};
 
 sph_status iisph_step(sph_world* w, float dt_total, const float g[3]);
 sph_status slab_begin_step(sph_world* w);
@@ -199,6 +212,11 @@ struct sph_world {
     unsigned long long bb_contacts = 0;
     int b_sorted_grid[6] = {0, 0, 0, 0, 0, 0};
     std::vector<float> hb_pos, hb_vel;
+    bool hb_stale = false;  // colliders posed boundary particles on the device: hb_pos / hb_vel lag behind (pull_boundaries)
+    std::vector<ColliderRec> colliders;
+    DBuf<int> d_cb;         // boundary cell AABB + bad flag after colliders moved (as k_bounds writes it)
+    DBuf<float> d_imp;      // 6 floats per collider slot: the impulses of the step
+    float* h_imp = nullptr;  // pinned copy, read back with the step's final read-back
 
     // sorted device state (double buffered for the counting sort)
     int cur = 0, bcur = 0;
@@ -629,6 +647,107 @@ sph_status upload_boundaries(sph_world* w) {
     return SPH_OK;
 }
 
+// Colliders keep their boundaries on the device; before the host copy is edited or handed out, bring it up to date.
+sph_status pull_boundaries(sph_world* w) {
+    if (!w->hb_stale) return SPH_OK;
+    TRY(enter(w));
+    const size_t B = w->B;
+    const int bc = w->bcur;
+    CU(w->o_b.ensure(3 * B));
+    CU(w->o_c.ensure(3 * B));
+    LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bpos[bc].p, w->o_b.p);
+    LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bvel[bc].p, w->o_c.p);
+    CU(cudaMemcpyAsync(w->hb_pos.data(), w->o_b.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaMemcpyAsync(w->hb_vel.data(), w->o_c.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaStreamSynchronize(w->st));
+    w->hb_stale = false;
+    return SPH_OK;
+}
+
+inline int collider_slot(const sph_world* w, uint32_t handle) {
+    const uint32_t slot = handle & 0xFFFFu;
+    if (slot >= w->colliders.size() || !w->colliders[slot].alive || (w->colliders[slot].gen & 0xFFFFu) != (handle >> 16)) return -1;
+    return (int)slot;
+}
+// a live collider whose boundary exists (a removed boundary leaves its collider inert)
+bool any_collider(const sph_world* w) {
+    for (const ColliderRec& c : w->colliders)
+        if (c.alive && boundary_slot(w, c.boundary) >= 0) return true;
+    return false;
+}
+bool boundary_coupled(const sph_world* w, uint32_t boundary) {
+    for (const ColliderRec& c : w->colliders)
+        if (c.alive && boundary_slot(w, c.boundary) == (int)boundary) return true;
+    return false;
+}
+
+// ColliderCouplingManager::update_boundaries (fluids_pipeline.rs:151-261) for StaticSampling colliders.  Their samples do not
+// depend on the fluid, so they are posed before the step's grid is sized: the grid then covers them.  `reposed_all`: the
+// boundaries were just uploaded from the host copy, which holds the points of registration, not the posed ones.
+sph_status colliders_update(sph_world* w, bool reposed_all) {
+    const size_t B = w->B;
+    bool moved = false;
+    for (ColliderRec& c : w->colliders) {
+        if (!c.alive) continue;
+        const int bs = boundary_slot(w, c.boundary);
+        if (bs < 0) continue;  // boundaries.get_mut finds nothing (:159-162)
+        BoundaryRec& b = w->bounds[bs];
+        if (c.state.body == SPH_BODY_FIXED) b.want_forces = false;  // :163-171
+        else if (c.state.body == SPH_BODY_DYNAMIC) b.want_forces = true;
+        if (!reposed_all && c.applied_valid && memcmp(&c.state, &c.applied, sizeof c.state) == 0) continue;
+        ColliderPose P;
+        memcpy(P.rot, c.state.rotation_rowmajor, sizeof P.rot);
+        memcpy(P.t, c.state.translation, sizeof P.t);
+        memcpy(P.linvel, c.state.linvel, sizeof P.linvel);
+        memcpy(P.angvel, c.state.angvel, sizeof P.angvel);
+        memcpy(P.com, c.state.world_com, sizeof P.com);
+        P.moving = c.state.body != SPH_BODY_NONE;
+        const int bc = w->bcur;
+        if (c.n) LAUNCH(k_collider_static, B, 256, (uint32_t)B, w->borig[bc].p, (uint32_t)b.offset, (uint32_t)c.n, c.local.p, P, w->bpos[bc].p, w->bvel[bc].p);
+        c.applied = c.state;
+        c.applied_valid = true;
+        moved = moved || c.n;
+    }
+    if (!moved) return SPH_OK;
+    // the boundary AABB sizes the grid (phase_grid): recompute it from the device particles, the step's one collider sync
+    static const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+    CU(w->d_cb.ensure(8));
+    CU(cudaMemcpyAsync(w->d_cb.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
+    k_bounds<<<std::min<uint32_t>(cdiv(B, 256), 296), 256, 0, w->st>>>(w->bpos[w->bcur].p, (uint32_t)B, w->d_cb.p);
+    w->launches++;
+    int hb[7];
+    CU(cudaMemcpyAsync(hb, w->d_cb.p, sizeof hb, cudaMemcpyDeviceToHost, w->st));
+    CU(cudaStreamSynchronize(w->st));
+    memcpy(w->b_aabb, hb, sizeof w->b_aabb);
+    w->b_bad = hb[6] != 0;
+    w->b_sorted_valid = false;  // re-sort the boundaries and recompute their volumes
+    w->hb_stale = true;
+    return SPH_OK;
+}
+
+// transmit_forces (fluids_pipeline.rs:263-287): enqueued after the solve; the impulses come back with the step's final read-back
+sph_status colliders_impulse(sph_world* w) {
+    ImpulseTable T;
+    for (int b = 0; b < MAX_BOUNDARIES; ++b) T.collider[b] = -1;
+    bool any = false;
+    for (size_t k = 0; k < w->colliders.size(); ++k) {
+        ColliderRec& c = w->colliders[k];
+        const int bs = c.alive ? boundary_slot(w, c.boundary) : -1;
+        if (bs < 0 || c.state.body != SPH_BODY_DYNAMIC || !w->bounds[bs].want_forces || w->bounds[bs].n == 0) continue;
+        T.collider[bs] = (int)k;
+        memcpy(T.com[k], c.state.world_com, sizeof T.com[k]);
+        c.impulse_pending = any = true;
+    }
+    if (!any) return SPH_OK;
+    const size_t bytes = 6 * w->colliders.size() * sizeof(float);
+    CU(cudaMemsetAsync(w->d_imp.p, 0, bytes, w->st));
+    k_collider_impulse<<<std::min<uint32_t>(cdiv(w->B, 256), 264), 256, 0, w->st>>>((uint32_t)w->B, w->bpos[w->bcur].p, w->bvel[w->bcur].p, w->bforce.p,
+                                                                                   w->dt, T, w->d_imp.p);
+    w->launches++;
+    CU(cudaMemcpyAsync(w->h_imp, w->d_imp.p, bytes, cudaMemcpyDeviceToHost, w->st));
+    return SPH_OK;
+}
+
 // fluid.rs:88-98 apply_particles_removal (+ solver scratch filtering dfsph_solver.rs:550-559)
 sph_status apply_pending_deletes(sph_world* w) {
     bool any = false;
@@ -764,7 +883,10 @@ sph_status phase_grid(sph_world* w) {
         else LAUNCH(k_cell_hist, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, (const uint32_t*)nullptr, 0u);
         TRY(scan_exclusive(w, w->bstart.p, ncell + 1));
         LAUNCH(k_cell_scatter, B, 256, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, w->bperm.p);
-        if (w->desc.deterministic) LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, (const uint32_t*)nullptr, (const float4*)nullptr);
+        // in-cell order by original index: the same whether the input is a fresh upload or the last sort of boundaries that
+        // colliders moved on the device
+        if (w->desc.deterministic)
+            LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, (const uint32_t*)w->borig[bc].p, (const float4*)nullptr);
         GatherSet g;
         memset(&g, 0, sizeof g);
         g.in4[0] = w->bpos[bc].p; g.out4[0] = w->bpos[bc ^ 1].p;
@@ -1350,6 +1472,7 @@ sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<
             CU(cudaMemcpyAsync(bvol.data(), w->o_c.p, w->B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
             CU(cudaStreamSynchronize(w->st));
         }
+        TRY(pull_boundaries(w));
         views.resize(w->bounds.size());
         for (size_t b = 0; b < w->bounds.size(); ++b) {
             const BoundaryRec& br = w->bounds[b];
@@ -1603,8 +1726,16 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     w->n_spans = 0;
     w->nb_pending = false;
     memset(&w->stats, 0, sizeof w->stats);
+    const bool colliders = any_collider(w);  // refused before anything of the step is applied
+    if (colliders && coupling) return w->fail(SPH_ERR_INVALID, "registered colliders and a host coupling manager cannot run in one step");
+    if (colliders && w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
     TRY(apply_pending_deletes(w));  // liquid_world.rs:79-81
     TRY(stage_up(w));
+    for (ColliderRec& c : w->colliders) {
+        memset(c.impulse, 0, sizeof c.impulse);
+        c.impulse_pending = false;
+    }
+    const bool b_uploaded = w->b_dirty;
     TRY(upload_boundaries(w));
     size_t N = w->N;
     w->stats.n_fluid_particles = N;
@@ -1622,6 +1753,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
         w->own_begin = 0;
     }
     if (w->Ntot + w->B == 0) return SPH_OK;
+    if (colliders) TRY(colliders_update(w, b_uploaded));
     TRY(phase_grid(w));
     w->grid_ready = true;
     w->ever_stepped = true;
@@ -1658,6 +1790,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
         if (w->desc.solver == SPH_SOLVER_DFSPH) TRY(dfsph_step(w, dt, g));
         else TRY(iisph_step(w, dt, g));
     }
+    if (colliders && N) TRY(colliders_impulse(w));  // without fluid particles no force reaches a boundary (and dt did not advance)
     CU(cudaEventRecord(w->ev[EV_END], w->st));
     int flag = 0;
     unsigned long long cnts[2] = {0, 0};
@@ -1668,6 +1801,8 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     w->nb_valid = w->nb_pending;
     w->nb_pending = false;
     CU(cudaGetLastError());
+    for (size_t k = 0; k < w->colliders.size(); ++k)
+        if (w->colliders[k].impulse_pending) memcpy(w->colliders[k].impulse, w->h_imp + 6 * k, sizeof w->colliders[k].impulse);
     if (!w->b_reused) w->bb_contacts = cnts[0];
     w->stats.n_contacts = w->bb_contacts + cnts[1];
     w->stats.kernel_launches = w->launches;
@@ -1811,6 +1946,10 @@ void sph_world_destroy(sph_world* w) {
         cudaEventDestroy(s.b);
     }
     if (w->h_pinned) cudaFreeHost(w->h_pinned);
+    for (auto& c : w->colliders) c.local.release();
+    w->d_cb.release();
+    w->d_imp.release();
+    if (w->h_imp) cudaFreeHost(w->h_imp);
     w->d_ticket.release();
     w->d_nb.release();
     w->xs.release(); w->he_colors.release(); w->he_gradc.release(); w->q_out.release(); w->q_count.release();
@@ -2017,6 +2156,7 @@ sph_status sph_boundary_add(sph_world* w, const float* pos, const float* vel, si
     if (!w) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     if (n && !pos) return w->fail(SPH_ERR_INVALID, "sph_boundary_add: null positions");
+    TRY(pull_boundaries(w));
     size_t slot = w->bounds.size();
     for (size_t k = 0; k < w->bounds.size(); ++k)
         if (!w->bounds[k].alive) { slot = k; break; }
@@ -2047,6 +2187,8 @@ sph_status sph_boundary_write(sph_world* w, uint32_t boundary_h, const float* po
     BOUNDARY_OR_FAIL(boundary, boundary_h)
     BoundaryRec& b = w->bounds[boundary];
     if (n != b.n) return w->fail(SPH_ERR_INVALID, "sph_boundary_write: length %zu != particle count %zu", n, b.n);
+    if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "sph_boundary_write: the boundary is coupled to a collider");
+    TRY(pull_boundaries(w));
     if (pos) memcpy(w->hb_pos.data() + 3 * b.offset, pos, 3 * n * sizeof(float));
     if (vel) memcpy(w->hb_vel.data() + 3 * b.offset, vel, 3 * n * sizeof(float));
     w->b_dirty = true;
@@ -2489,6 +2631,7 @@ sph_status sph_boundary_remove(sph_world* w, uint32_t boundary_h) {
     if (!w) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     BOUNDARY_OR_FAIL(boundary, boundary_h)
+    TRY(pull_boundaries(w));
     BoundaryRec& b = w->bounds[boundary];
     w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
     w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
@@ -2506,6 +2649,8 @@ sph_status sph_boundary_set_particles(sph_world* w, uint32_t boundary_h, const f
     if (!w || (n && !pos)) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     BOUNDARY_OR_FAIL(boundary, boundary_h)
+    if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "sph_boundary_set_particles: the boundary is coupled to a collider");
+    TRY(pull_boundaries(w));
     BoundaryRec& b = w->bounds[boundary];
     w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
     w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
@@ -2523,6 +2668,114 @@ sph_status sph_boundary_count(sph_world* w, uint32_t boundary_h, size_t* n) {
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     BOUNDARY_OR_FAIL(boundary, boundary_h)
     *n = w->bounds[boundary].n;
+    return SPH_OK;
+}
+
+// boundary.positions / velocities boundary.rs:13-15
+sph_status sph_boundary_read(sph_world* w, uint32_t boundary_h, float* pos, float* vel, size_t cap, size_t* n) {
+    if (!w || !n) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    BOUNDARY_OR_FAIL(boundary, boundary_h)
+    const BoundaryRec& b = w->bounds[boundary];
+    *n = b.n;
+    if ((pos || vel) && cap < b.n) return w->fail(SPH_ERR_INVALID, "sph_boundary_read: capacity %zu < particle count %zu", cap, b.n);
+    TRY(pull_boundaries(w));
+    if (pos) memcpy(pos, w->hb_pos.data() + 3 * b.offset, 3 * b.n * sizeof(float));
+    if (vel) memcpy(vel, w->hb_vel.data() + 3 * b.offset, 3 * b.n * sizeof(float));
+    return SPH_OK;
+}
+
+// ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114
+sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t sampling, const sph_shape* shape, const float* pts, size_t n,
+                                 uint32_t* collider) {
+    if (!w || !collider || (n && !pts)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "colliders cannot be registered from inside a coupling callback");
+    if (w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
+    BOUNDARY_OR_FAIL(boundary, boundary_h)
+    if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "boundary %u is already coupled to a collider", (unsigned)boundary_h);
+    if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE)) return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
+    if (sampling != SPH_SAMPLING_STATIC) return w->fail(SPH_ERR_INVALID, "unknown sampling %d (StaticSampling is the only one)", sampling);
+    if (n >= (size_t)UINT32_MAX) return w->fail(SPH_ERR_INVALID, "too many sample points");
+    for (size_t k = 0; k < 3 * n; ++k)
+        if (!std::isfinite(pts[k])) return w->fail(SPH_ERR_INVALID, "non-finite sample point");
+    size_t slot = w->colliders.size();
+    for (size_t k = 0; k < w->colliders.size(); ++k)
+        if (!w->colliders[k].alive) { slot = k; break; }
+    if (slot >= (size_t)MAX_BOUNDARIES) return w->fail(SPH_ERR_INVALID, "too many colliders (max %d)", MAX_BOUNDARIES);
+    TRY(enter(w));
+    if (!w->h_imp) CU(cudaMallocHost(&w->h_imp, 6 * MAX_BOUNDARIES * sizeof(float)));
+    CU(w->d_imp.ensure(6 * MAX_BOUNDARIES));
+    ColliderRec c;
+    if (slot < w->colliders.size()) c.gen = w->colliders[slot].gen + 1;
+    c.boundary = boundary_h;
+    c.n = n;
+    c.state.rotation_rowmajor[0] = c.state.rotation_rowmajor[4] = c.state.rotation_rowmajor[8] = 1.f;
+    c.state.body = SPH_BODY_NONE;
+    if (n) {
+        std::vector<float4> l(n);
+        for (size_t k = 0; k < n; ++k) l[k] = make_float4(pts[3 * k], pts[3 * k + 1], pts[3 * k + 2], 0.f);
+        CU(c.local.ensure(n));
+        CU(cudaMemcpyAsync(c.local.p, l.data(), n * sizeof(float4), cudaMemcpyHostToDevice, w->st));
+        CU(cudaStreamSynchronize(w->st));
+    }
+    // the points become the boundary's particle set; the next step poses them
+    TRY(pull_boundaries(w));
+    BoundaryRec& b = w->bounds[boundary];
+    w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
+    w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
+    w->hb_pos.insert(w->hb_pos.begin() + 3 * b.offset, pts, pts + 3 * n);
+    w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, 3 * n, 0.f);
+    b.n = n;
+    recompute_offsets(w);
+    w->b_dirty = true;
+    if (slot == w->colliders.size()) w->colliders.push_back(c);
+    else w->colliders[slot] = c;
+    *collider = make_handle(slot, c.gen);
+    return SPH_OK;
+}
+
+#define COLLIDER_OR_FAIL(var, handle)                                                                   \
+    const int var##_slot_ = collider_slot(w, handle);                                                   \
+    if (var##_slot_ < 0) return w->fail(SPH_ERR_INVALID, "bad collider handle %u", (unsigned)(handle)); \
+    ColliderRec& var = w->colliders[var##_slot_];
+
+sph_status sph_collider_set_state(sph_world* w, uint32_t collider_h, const sph_collider_state* state) {
+    if (!w || !state) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    COLLIDER_OR_FAIL(c, collider_h)
+    if (state->body < SPH_BODY_NONE || state->body > SPH_BODY_DYNAMIC) return w->fail(SPH_ERR_INVALID, "unknown body kind %d", state->body);
+    const float* f[5] = {state->translation, state->rotation_rowmajor, state->linvel, state->angvel, state->world_com};
+    const int len[5] = {3, 9, 3, 3, 3};
+    for (int a = 0; a < 5; ++a)
+        for (int k = 0; k < len[a]; ++k)
+            if (!std::isfinite(f[a][k])) return w->fail(SPH_ERR_INVALID, "non-finite collider state");
+    c.state = *state;
+    return SPH_OK;
+}
+
+// transmit_forces fluids_pipeline.rs:263-287 of the last step
+sph_status sph_collider_read_impulse(sph_world* w, uint32_t collider_h, float linear[3], float angular[3]) {
+    if (!w || !linear || !angular) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    COLLIDER_OR_FAIL(c, collider_h)
+    const bool inert = boundary_slot(w, c.boundary) < 0;
+    for (int a = 0; a < 3; ++a) {
+        linear[a] = inert ? 0.f : c.impulse[a];
+        angular[a] = inert ? 0.f : c.impulse[3 + a];
+    }
+    return SPH_OK;
+}
+
+// ColliderCouplingSet::unregister_coupling fluids_pipeline.rs:119-122
+sph_status sph_collider_unregister(sph_world* w, uint32_t collider_h) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "colliders cannot be unregistered from inside a coupling callback");
+    COLLIDER_OR_FAIL(c, collider_h)
+    TRY(enter(w));
+    c.local.release();
+    c.alive = false;
     return SPH_OK;
 }
 

@@ -369,7 +369,9 @@ __global__ void k_cell_scatter(uint32_t n, const uint32_t* __restrict__ cid, con
 // order (and every f32 summation order downstream) is reproducible.  The in-cell order is CANONICAL — ascending
 // (fluid, particle id), a pure function of the particle set — so a world restored from a snapshot, a world whose state
 // went through the host, and the ranks of a slab decomposition (ghost columns!) all see the same order and produce
-// bit-identical sums.  key == nullptr (boundaries): ascending previous slot, i.e. insertion order.
+// bit-identical sums.  Boundaries pass their original indices (borig) as the key, so their in-cell order is insertion
+// order whether the input is a fresh upload or a sort of boundaries that colliders moved on the device.  key == nullptr:
+// ascending previous slot.
 __device__ __forceinline__ unsigned long long sort_key(uint32_t src, const uint32_t* __restrict__ gid, const float4* __restrict__ vel) {
     if (!gid) return src;
     const uint32_t f = vel ? fid_of(vel[src]) : 0u;
@@ -1457,7 +1459,73 @@ __device__ __forceinline__ bool query_near(const AabbQuery& q, const float4& p) 
     }
     return d <= q.radius;
 }
-__global__ void k_aabb_query(AabbQuery q, const float4* __restrict__ pos, const uint32_t* __restrict__ cstart, const uint32_t* __restrict__ orig,
+// ColliderCouplingManager::update_boundaries, StaticSampling (fluids_pipeline.rs:180-191): the coupled boundary's particles
+// are the collider's local sample points under its pose, world = rot * local + t (the convention of AabbQuery), with the
+// body's velocity_at_point(pt) = linvel + angvel x (pt - world_com) evaluated at the LOCAL point, as :183 does.  Explicit
+// round-to-nearest operations (no contraction into FMAs) keep the result a fixed float32 expression a host can restate.
+struct ColliderPose {
+    float rot[9], t[3];
+    float linvel[3], angvel[3], com[3];
+    int moving;  // 0: no parent body, velocity 0 (:184-186)
+};
+__device__ __forceinline__ float dot3_rn(float a0, float a1, float a2, float b0, float b1, float b2) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
+}
+// One thread per SORTED boundary slot; the slots whose original index lies in [first, first + n) belong to the collider.
+__global__ void k_collider_static(uint32_t nb, const uint32_t* __restrict__ borig, uint32_t first, uint32_t n, const float4* __restrict__ local,
+                                  ColliderPose P, float4* __restrict__ bpos, float4* __restrict__ bvel) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nb) return;
+    const uint32_t k = borig[s] - first;
+    if (k >= n) return;
+    const float4 l = local[k];
+    bpos[s] = make_float4(__fadd_rn(dot3_rn(P.rot[0], P.rot[1], P.rot[2], l.x, l.y, l.z), P.t[0]),
+                          __fadd_rn(dot3_rn(P.rot[3], P.rot[4], P.rot[5], l.x, l.y, l.z), P.t[1]),
+                          __fadd_rn(dot3_rn(P.rot[6], P.rot[7], P.rot[8], l.x, l.y, l.z), P.t[2]), 0.f);
+    float4 v = bvel[s];  // .w carries the boundary slot
+    v.x = v.y = v.z = 0.f;
+    if (P.moving) {
+        const float dx = __fsub_rn(l.x, P.com[0]), dy = __fsub_rn(l.y, P.com[1]), dz = __fsub_rn(l.z, P.com[2]);
+        v.x = __fadd_rn(P.linvel[0], __fsub_rn(__fmul_rn(P.angvel[1], dz), __fmul_rn(P.angvel[2], dy)));
+        v.y = __fadd_rn(P.linvel[1], __fsub_rn(__fmul_rn(P.angvel[2], dx), __fmul_rn(P.angvel[0], dz)));
+        v.z = __fadd_rn(P.linvel[2], __fsub_rn(__fmul_rn(P.angvel[0], dy), __fmul_rn(P.angvel[1], dx)));
+    }
+    bvel[s] = v;
+}
+// transmit_forces (fluids_pipeline.rs:263-287): the impulse body.apply_impulse_at_point(force * dt, pos) gives the body,
+// summed over the collider's boundary particles: out[6k..] = (sum f dt, sum (p - com) x f dt) of collider slot k.  One
+// launch for all colliders, each boundary slot read once: a block sums its slots per collider in shared memory and adds
+// the non-zero sums to `out` (zeroed before).  The float atomics make the last bits depend on timing.
+struct ImpulseTable {
+    int collider[MAX_BOUNDARIES];   // boundary slot -> collider slot whose impulse it feeds, or -1
+    float com[MAX_BOUNDARIES][3];   // per collider slot: the body's world centre of mass
+};
+__global__ void k_collider_impulse(uint32_t nb, const float4* __restrict__ bpos, const float4* __restrict__ bvel, const float* __restrict__ bforce,
+                                   float dt, ImpulseTable T, float* __restrict__ out) {
+    __shared__ float acc[MAX_BOUNDARIES][6];
+    for (int k = threadIdx.x; k < MAX_BOUNDARIES * 6; k += blockDim.x) (&acc[0][0])[k] = 0.f;
+    __syncthreads();
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < nb; s += gridDim.x * blockDim.x) {
+        const int k = T.collider[fid_of(bvel[s])];
+        if (k < 0) continue;
+        const float fx = bforce[3 * (size_t)s] * dt, fy = bforce[3 * (size_t)s + 1] * dt, fz = bforce[3 * (size_t)s + 2] * dt;
+        const float4 p = bpos[s];
+        const float rx = p.x - T.com[k][0], ry = p.y - T.com[k][1], rz = p.z - T.com[k][2];
+        atomicAdd(&acc[k][0], fx);
+        atomicAdd(&acc[k][1], fy);
+        atomicAdd(&acc[k][2], fz);
+        atomicAdd(&acc[k][3], ry * fz - rz * fy);
+        atomicAdd(&acc[k][4], rz * fx - rx * fz);
+        atomicAdd(&acc[k][5], rx * fy - ry * fx);
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < MAX_BOUNDARIES * 6; k += blockDim.x) {
+        const float v = (&acc[0][0])[k];
+        if (v != 0.f) atomicAdd(&out[k], v);
+    }
+}
+
+__global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const uint32_t* __restrict__ cstart, const uint32_t* __restrict__ orig,
                              const float4* __restrict__ bpos, const uint32_t* __restrict__ bstart, const uint32_t* __restrict__ borig,
                              uint32_t* __restrict__ out, uint32_t cap, uint32_t* __restrict__ count) {
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;

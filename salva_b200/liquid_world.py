@@ -164,6 +164,19 @@ class Capsule:
         self.params = [half_height, radius]
 
 
+class StaticSampling:
+    """ColliderSampling::StaticSampling(points) (fluids_pipeline.rs:64-69): the collider approximated by sample points given
+    in its local frame."""
+    kind = 0
+
+    def __init__(self, points):
+        self.points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
+
+
+# the rigid body a collider is attached to (include/sph.h SPH_BODY_*)
+BODY_NONE, BODY_FIXED, BODY_DYNAMIC = 0, 1, 2
+
+
 class CouplingManager:
     """trait CouplingManager (coupling/coupling_manager.rs:9-28).  Subclass and override; `world` is the LiquidWorld being
     stepped (queries issued from update_boundaries see fluid particles only, liquid_world.rs:86-103)."""
@@ -387,6 +400,55 @@ class LiquidWorld:
         tr = _lib.COUPLING_TRANSMIT_FN(lambda _u, _w, dt_, inv_dt: coupling.transmit_forces(self, dt_, inv_dt))
         cm = _lib.CouplingManagerC(upd, tr, None)
         self._ck(self._L.sph_world_step_with_coupling(self._w, dt, _fp(g), C.byref(cm)))
+
+    # -- collider coupling on the device (ColliderCouplingSet, fluids_pipeline.rs:72-287) ------------------------
+    def register_coupling(self, boundary, sampling):
+        """ColliderCouplingSet::register_coupling (fluids_pipeline.rs:98-114): couples `boundary` to a new collider and
+        returns the collider's handle.  The engine owns the boundary's particles from then on."""
+        pts = getattr(sampling, "points", np.zeros((0, 3), np.float32))
+        sh = None
+        if getattr(sampling, "shape", None) is not None:
+            sh = _lib.Shape()
+            sh.kind = sampling.shape.kind
+            for i, x in enumerate(sampling.shape.params):
+                sh.p[i] = x
+        h = C.c_uint32()
+        self._ck(self._L.sph_collider_register(self._w, boundary, sampling.kind, C.byref(sh) if sh is not None else None, _fp(pts),
+                                               len(pts), C.byref(h)))
+        self._nb[boundary] = len(pts)
+        return h.value
+
+    def set_collider_state(self, collider, translation=(0.0, 0.0, 0.0), rotation=None, body=BODY_NONE, linvel=(0.0, 0.0, 0.0),
+                           angvel=(0.0, 0.0, 0.0), world_com=(0.0, 0.0, 0.0)):
+        """The collider's pose (world = rotation @ local + translation, rotation 3x3) and its body for the next steps;
+        a body's velocity at p is linvel + angvel x (p - world_com)."""
+        s = _lib.ColliderState()
+        s.translation[:] = [float(x) for x in translation]
+        s.rotation_rowmajor[:] = [float(x) for x in (np.eye(3) if rotation is None else np.asarray(rotation)).reshape(9)]
+        s.body = body
+        s.linvel[:] = [float(x) for x in linvel]
+        s.angvel[:] = [float(x) for x in angvel]
+        s.world_com[:] = [float(x) for x in world_com]
+        self._ck(self._L.sph_collider_set_state(self._w, collider, C.byref(s)))
+
+    def collider_impulse(self, collider):
+        """(linear, angular) impulse the fluid applied to the collider's body in the last step (transmit_forces,
+        fluids_pipeline.rs:263-287)."""
+        lin, ang = np.zeros(3, np.float32), np.zeros(3, np.float32)
+        self._ck(self._L.sph_collider_read_impulse(self._w, collider, _fp(lin), _fp(ang)))
+        return lin, ang
+
+    def unregister_coupling(self, collider):
+        """ColliderCouplingSet::unregister_coupling (fluids_pipeline.rs:119-122): the boundary stays."""
+        self._ck(self._L.sph_collider_unregister(self._w, collider))
+
+    def read_boundary_particles(self, b):
+        """boundary.positions / velocities (boundary.rs:13-15) in original index order."""
+        n = C.c_size_t()
+        self._ck(self._L.sph_boundary_read(self._w, b, None, None, 0, C.byref(n)))
+        p, v = np.empty((n.value, 3), np.float32), np.empty((n.value, 3), np.float32)
+        self._ck(self._L.sph_boundary_read(self._w, b, _fp(p), _fp(v), n.value, C.byref(n)))
+        return p, v
 
     def particles_intersecting_shape(self, shape, translation=(0.0, 0.0, 0.0), rotation=None):
         """liquid_world.rs:246-281 for Ball / Cuboid / Capsule under the isometry (rotation 3x3 row-major, translation)."""
