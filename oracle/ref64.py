@@ -114,6 +114,11 @@ C_EL_STRESS = 12
 # sin / cos and products (<= 8u per entry) in a 3-term product (3u)
 C_EL_ORTHO = 20 * 11 + 20
 IISPH_AII_GATE = 1.0e-9  # iisph_solver.rs:303: no pressure where |aii| <= 1e-9
+# the loop errors: the term's division by rho0 (1), the mean's division by n (1), margin 2; the sum's depth is n
+C_ERR = 4
+# integration: vc = acc dt (1), margin 1; positions: v + vc, * dt, + P (3), margin 1
+C_INTEGRATE = 2
+C_POSITIONS = 4
 
 
 # ---- kernels: value f and absolute evaluation fa, both float64, for r >= 0 -------------------------------------------------
@@ -506,12 +511,66 @@ class Passes:
     def pressure_boundary_force(self, kappa, bvol, inv_dt, scale_m_inv_dt=True):
         """The force a pressure update puts on boundary particles (dfsph_solver.rs:267-272): for every contact with
         k_i > 0, (k_i vol_b rho0_i inv_dt g_ib) inv_dt m_i x_ib.  scale_m_inv_dt = False drops the second inv_dt m_i."""
+        return self.update_boundary_force(kappa, bvol, inv_dt, pressure=True, scale_m_inv_dt=scale_m_inv_dt)
+
+    def update_boundary_force(self, kappa, bvol, inv_dt, pressure=True, scale_m_inv_dt=True):
+        """The force an update puts on boundary particles, per boundary particle.  Pressure update (dfsph_solver.rs:267-272):
+        (k_i vol_b rho0_i inv_dt g_ib) inv_dt m_i x_ib over contacts with k_i > 0.  Divergence update (:400-406):
+        (k_i vol_b rho0_i g_ib) inv_dt m_i x_ib, where inv_dt is the previous step's (0 on the first step) and k_i =
+        div_i alpha_i >= 0.  scale_m_inv_dt = False drops the outer inv_dt m_i."""
         fb = self.fb
         k = np.asarray(kappa, F).astype(np.float64)[fb.i]
         s = float(F(inv_dt))
         mb = np.asarray(bvol, F).astype(np.float64)[fb.j] * self.rho0[fb.i]
-        w = np.where(k > 0, k * mb * s, 0.0) * ((s * self.mass[fb.i]) if scale_m_inv_dt else 1.0)
+        inner = np.where(k > 0, k * mb * s, 0.0) if pressure else k * mb
+        w = inner * ((s * self.mass[fb.i]) if scale_m_inv_dt else 1.0)
         return self._on_boundary(fb, *self._grad_terms(fb, w))
+
+    def loop_error(self, kind, x, c_pass=0, mutant=None, block=128):
+        """The error a DFSPH Jacobi loop breaks on (dfsph_solver.rs:153-158, 347-352): per particle e_i = max(div_i, 0) / rho0
+        (kind "divergence"; 0 under the 20-contact gate, still counted) or pred_i < rho0 ? 0 : pred_i / rho0 - 1 (kind
+        "density"); per fluid the mean over its particles; over fluids the maximum, empty fluids skipped, and 0.  Returns
+        (value, bound).
+        x: the float32 values read back (the reduction fed its own inputs), or a Ref of the pass (end to end: the pass
+        bound, at c_pass, is carried through the sum; both terms are 1 / rho0-Lipschitz in their input and continuous at
+        their gates, so no particle needs excluding).
+        The float32 reduction: each term rounds once or twice (x / rho0, then - 1, which cancels: its rounding is relative
+        to q = x / rho0), the sum of n terms in any order (n - 1) u sum |e|, and the division by n.
+        mutant: error_mean_over_all_fluids, error_drops_last_block (of `block` particles), error_unclamped (density)."""
+        end = isinstance(x, Ref)
+        v = x.value if end else _f64(x)
+        b = (x.bound(c_pass) if end else np.zeros(self.N)) / self.rho0
+        if kind == "divergence":
+            e = np.maximum(v, 0.0) / self.rho0
+            a = e
+        else:
+            q = v / self.rho0
+            on = (v >= self.rho0) | (mutant == "error_unclamped")
+            e = np.where(on, q - 1.0, 0.0)
+            a = np.where(on, np.abs(q) + np.abs(e), 0.0)
+        keep = np.ones(self.N, bool)
+        if mutant == "error_drops_last_block" and self.N:
+            keep[(self.N - 1) // block * block:] = False
+        groups = [np.arange(self.N)] if mutant == "error_mean_over_all_fluids" else \
+            [np.nonzero(self.fid == f)[0] for f in np.unique(self.fid)]
+        val, bound = 0.0, 0.0
+        for sel in groups:
+            n = len(sel)
+            val = max(val, e[sel[keep[sel]]].sum() / n)
+            # the maximum over fluids is 1-Lipschitz in each: the bound of the maximum is the largest bound
+            bound = max(bound, ((n + C_ERR) * U * np.abs(e[sel]).sum() + U * a[sel].sum() + b[sel].sum()) / n)
+        return val, bound
+
+    def integrate(self, acc, dt):
+        """The velocity change of the integration (dfsph_solver.rs:505-518): vc = acc dt, one float32 rounding."""
+        a = _f64(acc) * float(F(dt))
+        return Ref(a, np.abs(a), np.zeros_like(a), np.zeros(self.N))
+
+    def positions(self, P, V, vc, dt):
+        """update_positions (dfsph_solver.rs:411-420): P' = P + (v + vc) dt, fed the float32 P, v and vc; three float32
+        roundings (v + vc, * dt, + P), each relative to its operands."""
+        P, s, dt = _f64(P), _f64(V) + _f64(vc), float(F(dt))
+        return Ref(P + s * dt, np.abs(P) + (np.abs(_f64(V)) + np.abs(_f64(vc))) * abs(dt), np.zeros_like(P), np.zeros(self.N))
 
     def adhesion_boundary_force(self, adhesion, bvol):
         """Akinci2013's adhesion on boundary particles (akinci2013_surface_tension.rs:188): adh vol_b rho0_i A(r) / r x_ib m_i."""

@@ -188,13 +188,70 @@ def light(scene):
 SCENES = dict(block=scene_block, far=scene_far, gate=scene_gate, pairs=scene_pairs, volumes=scene_volumes,
               two_fluids=scene_two_fluids, **{"tail%d" % n: (lambda n=n: scene_tail(n)) for n in TAILS})
 
+SIXTEEN_SIZES = (1, 2, 7, 31, 33, 64, 96, 127, 128, 129, 290, 0, 100, 120, 90)   # the sixteenth takes the rest (41)
+SIXTEEN_EMPTIED = 11
+
+
+def scene_sixteen():
+    """The block's particles dealt at random to 16 fluids (MAX_FLUIDS): rest densities 500 to 2000, 1 to 290 particles
+    each, so the per-fluid means run over every partial slot.  The fluids of 1, 2 and 7 particles sit on the top face
+    moving down at 10 m/s, so that each keeps a positive divergence through the first step's loop.  Interaction groups cut the pairs of fluids 3, 7 and 13 with
+    the fluids of the next membership bit.  Fluid 11 had 20 particles, all deleted before the first step: it is empty,
+    and the error maximum skips it."""
+    sc = scene_block()
+    pts, vel = sc["fluids"][0]["positions"], sc["fluids"][0]["velocities"]
+    perm = np.random.default_rng(61).permutation(len(pts))
+    top = np.argsort(-pts[:, 1], kind="stable")[:10]   # the fluids of 1, 2 and 7 particles: on the top face, moving down
+    perm = np.r_[top, perm[~np.isin(perm, top)]]
+    vel = vel.copy()
+    vel[top] = (0.0, -10.0, 0.0)
+    cuts = np.cumsum(SIXTEEN_SIZES)
+    fluids = []
+    for k, sel in enumerate(np.split(perm, cuts)):
+        sel = np.sort(sel)
+        f = dict(positions=pts[sel], velocities=vel[sel], density0=float(F(500.0 + 100.0 * k)), memberships=1 << (k % 8),
+                 filter=(0xFFFFFFFF & ~(1 << ((k + 1) % 8))) if k in (3, 7, 13) else 0xFFFFFFFF)
+        if k == SIXTEEN_EMPTIED:
+            f["deleted"] = pts[:20] + np.array([0.0, 0.5, 0.0], F)
+        fluids.append(f)
+    b = sc["boundaries"][0]
+    return dict(fluids=fluids, boundaries=[dict(b, memberships=1 << 8, want_forces=True)])
+
+
+def scene_block_forces():
+    """The block with its tank wanting its forces: the boundary reactions of both updates are read back."""
+    sc = scene_block()
+    return dict(sc, boundaries=[dict(b, want_forces=True) for b in sc["boundaries"]])
+
+
+def scene_burst():
+    """The block's two halves flying apart along x at 60 m/s on top of their velocities: 0.24 m per DT, more than a cell
+    (h = 0.2) beyond the first step's grid, which the next step must size from the bounds the first one left."""
+    sc = scene_block()
+    f = sc["fluids"][0]
+    side = np.where(f["positions"][:, 0] < np.median(f["positions"][:, 0]), -60.0, 60.0)
+    v = (f["velocities"] + np.stack([side, np.zeros_like(side), np.zeros_like(side)], 1)).astype(F)
+    return dict(sc, fluids=[dict(f, velocities=v)])
+
+
+LOOP_SCENES = dict(block=scene_block_forces, gate=scene_gate, two_fluids=scene_two_fluids, sixteen=scene_sixteen,
+                   tail33=lambda: scene_tail(33))
+
 
 # ---- driving a world ---------------------------------------------------------------------------------------------------------
 def populate(world, scene, forces=()):
     fh = []
     for f in scene["fluids"]:
-        h = world.add_fluid(f["positions"], density0=f["density0"], velocities=f.get("velocities"), volumes=f.get("volumes"),
+        pos, vel, gone = f["positions"], f.get("velocities"), None
+        if "deleted" in f:   # added, then deleted before the first step: the fluid the scene describes is what is left
+            d = np.asarray(f["deleted"], F)
+            pos = np.concatenate([pos, d]).astype(F)
+            vel = None if vel is None else np.concatenate([vel, np.zeros_like(d)]).astype(F)
+            gone = np.r_[np.zeros(len(f["positions"]), np.uint8), np.ones(len(d), np.uint8)]
+        h = world.add_fluid(pos, density0=f["density0"], velocities=vel, volumes=f.get("volumes"),
                             memberships=f.get("memberships", 1), filter=f.get("filter", 0xFFFFFFFF))
+        if gone is not None:
+            world.delete_particles(h, gone)
         for kind, params in forces:
             world.push_force(h, kind, params)
         fh.append(h)
@@ -241,25 +298,28 @@ def _read(world, fh, bh, extra=()):
     return out
 
 
-def run(make_world, scene, iters, forces=(), first=None, extra=(), **world_kw):
-    """Step a fresh world once with force_iterations(*iters) (iters None: the solver's own loop), or twice when `first`
-    gives the first step's iterations.  Returns the observables after the last step and, for two steps, those after the
-    first.  extra: further debug selectors to read (IISPH_SCRATCH); world_kw goes to make_world (max_divergence_iter,
-    min_pressure_iter, max_pressure_iter)."""
+def run(make_world, scene, iters=None, forces=(), first=None, extra=(), steps=None, **world_kw):
+    """Step a fresh world once at DT with force_iterations(*iters) (iters None: the solver's own loops), or twice when
+    `first` gives the first step's iterations; gravity 0.  Returns the observables after the last step and, for two steps,
+    those after the first.
+    steps: a list of (dt, iters, gravity) instead, one per step (an entry of iters may be None: that loop runs free);
+    returns the list of observables after every step.
+    extra: further debug selectors to read (IISPH_SCRATCH); world_kw goes to make_world (min / max_divergence_iter,
+    max_divergence_error, min / max_pressure_iter, max_density_error)."""
+    seq = steps if steps is not None else ([(DT, first, ZERO_G)] if first is not None else []) + [(DT, iters, ZERO_G)]
     w = make_world(**world_kw)
     fh, bh = populate(w, scene, forces)
-    before = None
-    if first is not None:
-        w.force_iterations(*first)
-        w.step(DT, ZERO_G)
-        before = _read(w, fh, bh, extra)
-    if iters is not None:
-        w.force_iterations(*iters)
-    w.step(DT, ZERO_G)
-    out = _read(w, fh, bh, extra)
+    outs = []
+    for dt, it, g in seq:
+        it = (None, None) if it is None else it
+        w.force_iterations(*(-1 if k is None else k for k in it))
+        w.step(dt, g)
+        outs.append(_read(w, fh, bh, extra))
     if hasattr(w, "close"):
         w.close()
-    return out, before
+    if steps is not None:
+        return outs
+    return outs[-1], (outs[0] if first is not None else None)
 
 
 def passes_for(scene, P=None, kw=0, kg=0):
@@ -312,7 +372,11 @@ MUTANTS = ("drop_entries_32_35", "swap_vy_vz_odd", "gate_at_21", "normals_rho_i"
            "el_volume_once", "el_r_i_for_r_j", "el_g_i_for_g_j", "el_rest_lists_recaptured",
            "el_recapture_no_old_volumes", "el_second_fluid_no_offset",
            # DFSPHViscosity
-           "visc_precondition_columns", "visc_target_no_scale", "visc_vv_no_adt", "visc_u_j_beta_i")
+           "visc_precondition_columns", "visc_target_no_scale", "visc_vv_no_adt", "visc_u_j_beta_i",
+           # the loop errors, the lagging dt and the carried state
+           "error_mean_over_all_fluids", "error_drops_last_block", "error_counts_gated", "error_unclamped",
+           "div_threshold_current_inv_dt", "div_bforce_current_inv_dt", "xsph_current_inv_dt", "visc_current_dt",
+           "positions_previous_dt", "vc_not_carried", "vc_carried_unsorted", "fluid15_rho0_of_fluid0", "iisph_previous_dt")
 
 
 class Checks:
@@ -322,7 +386,7 @@ class Checks:
     def __init__(self, make_world, scene, kw=0, kg=0, mutant=None):
         self.make_world, self.scene, self.mutant = make_world, scene, mutant
         self.ps = passes_for(scene, kw=kw, kg=kg)
-        self.worst, self.excluded, self.clamp = {}, {}, {}
+        self.worst, self.excluded, self.clamp, self.errors, self.nonzero = {}, {}, {}, {}, {}
         ps = self.ps
         self.ff, self.fb = ps.ff, ps.fb
         if mutant == "drop_entries_32_35":
@@ -332,6 +396,8 @@ class Checks:
             last = np.r_[ps.fb.i[1:] != ps.fb.i[:-1], True] if len(ps.fb.i) else np.zeros(0, bool)
             self.fb = ps.fb.subset(~last)
         self.rho0_b = np.full(ps.N, ps.rho0[0]) if mutant == "boundary_mass_fluid0_rho0" else None
+        if mutant == "fluid15_rho0_of_fluid0":   # the last fluid slot reads the first one's rest density
+            self.rho0_b = np.where(ps.fid == 15, ps.rho0[0], ps.rho0)
         self.min_nb = 21 if mutant == "gate_at_21" else ref64.MIN_NEIGHBORS
         bd = scene["boundaries"]
         self.want = np.concatenate([np.full(len(b["positions"]), bool(b.get("want_forces", False))) for b in bd]) if bd else np.zeros(0, bool)
@@ -484,16 +550,31 @@ class Checks:
             self.worst["density_error"] = max(self.worst.get("density_error", 0.0), err / b if b > 0 else (0.0 if err == 0 else np.inf))
             self.excluded["density_error"] = self.excluded.get("density_error", 0) + amb
 
-        o2w, o1w = run(self.make_world, sc, (0, 1), first=(0, 2), extra=X)
+        self.iisph_warm(omega=omega)
+        return o0
+
+    def iisph_warm(self, dts=(DT, DT), omega=0.5):
+        """The warm-started IISPH step: step 1 at dts[0] with (0, 2), step 2 at dts[1] with (0, 1) on contacts re-derived on
+        P1.  dii, aii (fed dii read back), dij_pjl and p (fed 0.5 p_2 of each particle, which checks that pressures ride
+        the step's counting sort) all use the current step's dt: IISPH advances the timestep before its passes
+        (iisph_solver.rs)."""
+        sc, ps, m = self.scene, self.ps, self.mutant
+        tag = "" if dts[0] == dts[1] else "_dt_change"
+        dt = dts[0] if m == "iisph_previous_dt" else dts[1]
+        o1w, o2w = run(self.make_world, sc, steps=[(dts[0], (0, 2), ZERO_G), (dts[1], (0, 1), ZERO_G)], extra=IISPH_SCRATCH)
         ps1 = passes_for(sc, P=o1w["P"], kw=ps.kw, kg=ps.kg)
         assert np.array_equal(o2w["num_fluid_contacts"], ps1.nf) and np.array_equal(o2w["num_boundary_contacts"], ps1.nb)
+        dens, bvol = o2w["density"], o2w["bvol"]
+        self.record("dii_warm" + tag, o2w["dii"], ps1.iisph_dii(dens, bvol, dt, rho0_b=self.rho0_b), C_PASS["iisph_dii"], ps=ps1)
+        self.record("aii_warm" + tag, o2w["aii"], ps1.iisph_aii(dens, o2w["dii"], bvol, dt, rho0_b=self.rho0_b), C_PASS["iisph_aii"],
+                    ps=ps1)
         p_ws = o1w["pressure"] if m == "no_warm_start" else (o1w["pressure"] * F(0.5)).astype(F)
-        self.record("dij_pjl_warm", o2w["dij_pjl"], ps1.iisph_dij_pjl(o2w["density"], p_ws, DT), C_PASS["iisph_dij_pjl"], ps=ps1)
-        ref, raw = ps1.iisph_next_pressure(o2w["density"], o2w["predicted_density"], p_ws, o2w["aii"], o2w["dii"], o2w["dij_pjl"],
-                                           o2w["bvol"], DT, omega)
-        self._pressure("pressure_warm", o2w["pressure"], ref, raw, ps=ps1)
-        self.moved_cells = int((np.floor(o1w["P"] / ps.h) != np.floor(ps.P / ps.h)).any(axis=1).sum())
-        return o0
+        self.record("dij_pjl_warm" + tag, o2w["dij_pjl"], ps1.iisph_dij_pjl(dens, p_ws, dt), C_PASS["iisph_dij_pjl"], ps=ps1)
+        ref, raw = ps1.iisph_next_pressure(dens, o2w["predicted_density"], p_ws, o2w["aii"], o2w["dii"], o2w["dij_pjl"],
+                                           bvol, dt, omega)
+        self._pressure("pressure_warm" + tag, o2w["pressure"], ref, raw, ps=ps1)
+        if not tag:
+            self.moved_cells = int((np.floor(o1w["P"] / ps.h) != np.floor(ps.P / ps.h)).any(axis=1).sum())
 
     def _pressure(self, name, gpu, ref, raw, ps=None):
         """A pressure pass: particles whose unclamped value lies within its bound of 0 are excluded (the clamp may go either
@@ -540,23 +621,26 @@ class Checks:
             assert np.isfinite(acc).all(), "%s: non-finite accelerations at %s" % (name, np.nonzero(~np.isfinite(acc).all(1))[0][:8])
             self.record(name, acc, ref, C_PASS["akinci"])
 
-    def xsph(self, cf=0.5, cb=0.0):
+    def xsph(self, cf=0.5, cb=0.0, dts=(DT, DT)):
+        """dts: the two steps' dt; step 2's XSPH sees the first one's inv_dt."""
         from salva_b200 import scenes
         sc = self.scene
         forces = [scenes.xsph_viscosity(cf, cb)]
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
-        for it, name in (((1, 0), "xsph_after_update"), ((0, 0), "xsph_separate")):
-            o2, o1 = run(self.make_world, sc, it, forces, first=(1, 0))
+        tag = "" if dts[0] == dts[1] else "_dt_change"
+        inv_dt = F(1.0) / F(dts[1] if self.mutant == "xsph_current_inv_dt" else dts[0])
+        for it, name in (((1, 0), "xsph_after_update" + tag), ((0, 0), "xsph_separate" + tag)):
+            o1, o2 = run(self.make_world, sc, forces=forces, steps=[(dts[0], (1, 0), ZERO_G), (dts[1], it, ZERO_G)])
             ps1 = passes_for(sc, P=o1["P"], kw=self.ps.kw, kg=self.ps.kg)
             assert np.array_equal(o2["num_fluid_contacts"], np.bincount(ps1.ff.i, minlength=ps1.N))
-            ref = ps1.xsph(o2["V"], o2["density"], cf, cb, F(1.0) / F(DT), bvel, o2["bvol"])
+            ref = ps1.xsph(o2["V"], o2["density"], cf, cb, inv_dt, bvel, o2["bvol"])
             r = ref64.ratio(o2["acceleration"], ref, C_PASS["xsph"]).max(axis=1)
             r = np.where(ps1.ambiguous(), 0.0, r)
             self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()))
             self.excluded[name] = self.excluded.get(name, 0) + int(ps1.ambiguous().sum())
             if it == (0, 0) and cb != 0:   # no update on step 2: the forces are XSPH's alone
-                self.record_boundary("boundary_force_xsph", o2["bforce"],
-                                     ps1.xsph_boundary_force(o2["V"], o2["density"], cb, F(1.0) / F(DT), bvel, o2["bvol"]), ps=ps1)
+                self.record_boundary("boundary_force_xsph" + tag, o2["bforce"],
+                                     ps1.xsph_boundary_force(o2["V"], o2["density"], cb, inv_dt, bvel, o2["bvol"]), ps=ps1)
 
     def artificial(self, cf=1.0, cb=0.0, alpha=1.0, beta=0.0, cs=10.0):
         """ArtificialViscosity on the first step, with no update (0, 0) and after one (1, 0): it does not depend on dt, so
@@ -604,24 +688,26 @@ class Checks:
             ref = ref64.Ref(np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros(nb))
         self.record_boundary("boundary_force_he2014", o["bforce"], ref)
 
-    def viscosity(self, visc=0.5, wcsph=0.0):
+    def viscosity(self, visc=0.5, wcsph=0.0, dts=(DT, DT)):
         """DFSPHViscosity.  Forces see the previous step's dt, 0 on the first step, so (as for XSPH) step 1 with (1, 0),
         then step 2 with (0, 0) on positions P1, the velocities V2 and the densities of step 2, once with
         max_viscosity_iter = 1 and once with 2 (max_viscosity_error = 0: no early break).  Each pass fed what its kernel
         read: beta (residual check), the target on vv = v + a dt, the acceleration after one update (rate on the same vv,
         beta and target read back) and after two (vv on the acceleration read back from the one-update run).  wcsph: a
         WCSPHSurfaceTension coefficient pushed before the viscosity, so that a != 0 in vv; its acceleration comes from a
-        run with WCSPH alone."""
+        run with WCSPH alone.  dts: the two steps' dt; step 2's viscosity sees the first one's dt and inv_dt."""
         from salva_b200 import scenes
         sc, m, kw = self.scene, self.mutant, dict(kw=self.ps.kw, kg=self.ps.kg)
-        tag = "_after_wcsph" if wcsph else ""
+        tag = ("_after_wcsph" if wcsph else "") + ("" if dts[0] == dts[1] else "_dt_change")
         pre = [scenes.wcsph_surface_tension(wcsph)] if wcsph else []
-        runs = {k: run(self.make_world, sc, (0, 0), pre + [scenes.dfsph_viscosity(visc, 1, k, 0.0)], first=(1, 0), extra=VISC_SCRATCH)
+        steps = [(dts[0], (1, 0), ZERO_G), (dts[1], (0, 0), ZERO_G)]
+        runs = {k: run(self.make_world, sc, forces=pre + [scenes.dfsph_viscosity(visc, 1, k, 0.0)], steps=steps, extra=VISC_SCRATCH)[::-1]
                 for k in (1, 2)}
         o2, o1 = runs[1]
         ps1 = passes_for(sc, P=o1["P"], **kw)
         dens, V = o2["density"], o2["V"]
-        a0 = run(self.make_world, sc, (0, 0), pre, first=(1, 0))[0]["acceleration"] if wcsph else np.zeros_like(V)
+        a0 = run(self.make_world, sc, forces=pre, steps=steps)[-1]["acceleration"] if wcsph else np.zeros_like(V)
+        dt = dts[1] if m == "visc_current_dt" else dts[0]   # the viscosity's dt: the previous step's
         ratio, viol, amb, zero = ps1.visc_beta(dens, o2["visc_beta"], C_PASS["visc_matrix"], by_column=m == "visc_precondition_columns")
         amb = amb | ps1.ambiguous()
         self.worst["visc_beta" + tag] = max(self.worst.get("visc_beta" + tag, 0.0), float(np.where(amb, 0.0, ratio).max()))
@@ -630,13 +716,13 @@ class Checks:
         self.visc_zero = getattr(self, "visc_zero", 0) + int(zero.sum())
         skip = m == "visc_vv_no_adt"
         scale = 1.0 if m == "visc_target_no_scale" else float(F(1.0) - F(visc))
-        self.record("visc_target" + tag, o2["visc_target"], ps1.visc_rates(dens, V, a0, DT, scale, skip_adt=skip),
+        self.record("visc_target" + tag, o2["visc_target"], ps1.visc_rates(dens, V, a0, dt, scale, skip_adt=skip),
                     C_PASS["visc_rate"] + 1, ps=ps1)
-        inv_dt = F(1.0) / F(DT)
+        inv_dt = F(1.0) / F(dt)
         acc = a0
         for k in (1, 2):
             ok = runs[k][0]
-            rate = ps1.visc_rates(dens, V, acc, DT, 1.0, skip_adt=skip)
+            rate = ps1.visc_rates(dens, V, acc, dt, 1.0, skip_adt=skip)
             ref = ps1.visc_accel(dens, ok["visc_beta"], rate.value, rate.bound(C_PASS["visc_rate"]), ok["visc_target"], acc, inv_dt,
                                  beta_i_for_j=m == "visc_u_j_beta_i")
             self.record("visc_accel_%d%s" % (k, tag), ok["acceleration"], ref, C_PASS["visc_accel"], ps=ps1)
@@ -735,6 +821,183 @@ class Checks:
         self.record(name + "_force", o["acceleration"],
                     bk.force(o["el_stress"], G, R, o["el_volume0"], r_i_for_r_j=m == "el_r_i_for_r_j",
                              g_i_for_g_j=m == "el_g_i_for_g_j"), C_PASS["el_force"], **kw)
+
+    # ---- the loop errors, the loops' exits, the lagging dt and the state a step carries into the next ---------------------
+    def _error(self, name, gpu, value, bound):
+        err = abs(float(gpu) - value)
+        r = err / bound if bound > 0 else (0.0 if err == 0 else np.inf)
+        self.worst[name] = max(self.worst.get(name, 0.0), r)
+        self.errors.setdefault(name, []).append(value)
+
+    def _nonzero(self, kind, ps, on):
+        fewest = min(int(on[ps.fid == f].sum()) for f in np.unique(ps.fid))
+        self.nonzero[kind] = min(self.nonzero.get(kind, fewest), fewest)
+
+    def _vstar(self, o):
+        """v + vc a step leaves, as the next step's first evaluation sweeps it (both read back by particle)."""
+        vc = o["velocity_change"]
+        if self.mutant == "vc_not_carried":
+            vc = np.zeros_like(vc)
+        return (o["V"] + vc).astype(F)
+
+    def loop_errors(self, dts=(DT,), forces=()):
+        """The errors the DFSPH loops break on (stats last_divergence_error, last_density_error), on the last of the steps
+        `dts` (the ones before it pinned at (1, 1), so that it starts from a carried vc and a different dt_prev), with the
+        loop free-running but held to min = max = k: the engine reads the error back only where the loop may break.
+          divergence  k = 1: evaluation 0, the neighbour search's partials; k = 2: evaluation 1, reduce_error;
+          pressure    k = 1, 2, the divergence loop pinned to one update.
+        Each error is checked fed the values the loop read back (the reduction alone) and end to end, against the float64
+        pass on the evaluation's inputs, read back from a run pinned to stop at that evaluation.  forces: pushed on every
+        fluid (XSPH and Akinci2013 fuse into the divergence evaluations of a single uniform-mass fluid).
+        nonzero: on a first step, per loop, the fewest nonzero error terms of any non-empty fluid, so that a dropped
+        partial shows (after a step the expanding scenes leave some small fluids with no compressing particle)."""
+        sc, m = self.scene, self.mutant
+        pre = [(dt, (1, 1), ZERO_G) for dt in dts[:-1]]
+        dt = dts[-1]
+        tag = "" if len(dts) == 1 else "_after_dt_change"
+        for k in (1, 2):
+            outs = run(self.make_world, sc, forces=forces, steps=pre + [(dt, (None, 0), ZERO_G)], min_divergence_iter=k,
+                       max_divergence_iter=k)
+            o = outs[-1]
+            assert o["stats"]["n_divergence_eval"] == k and o["stats"]["n_divergence_iter"] == k, o["stats"]
+            prev = outs[-2] if pre else None
+            ps = self.ps if prev is None else passes_for(sc, P=prev["P"], kw=self.ps.kw, kg=self.ps.kg)
+            gpu = o["stats"]["last_divergence_error"]
+            self._error("divergence_error_read%s" % tag, gpu, *ps.loop_error("divergence", o["divergence"], mutant=m))
+            if not pre:
+                self._nonzero("divergence", ps, o["divergence"] > 0)
+            # end to end: the evaluation's velocities are those a run pinned to k - 1 updates leaves
+            p = run(self.make_world, sc, forces=forces, steps=pre + [(dt, (k - 1, 0), ZERO_G)])[-1]
+            assert np.array_equal(p["divergence"], o["divergence"])
+            bvol = p["bvol"]
+            ref = ps.divergence(p["V"], bvol, gate=m != "error_counts_gated")
+            self._error("divergence_error%s" % tag, gpu, *ps.loop_error("divergence", ref, C_PASS["divergence"], mutant=m))
+            self.record("divergence_eval_%d%s" % (k - 1, tag), p["divergence"], ps.divergence(p["V"], bvol), C_PASS["divergence"], ps=ps)
+        bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
+        for k in (1, 2):
+            outs = run(self.make_world, sc, forces=forces, steps=pre + [(dt, (1, None), ZERO_G)], min_pressure_iter=k,
+                       max_pressure_iter=k)
+            o = outs[-1]
+            assert o["stats"]["n_pressure_eval"] == k and o["stats"]["n_pressure_iter"] == k, o["stats"]
+            ps = self.ps if not pre else passes_for(sc, P=outs[-2]["P"], kw=self.ps.kw, kg=self.ps.kg)
+            gpu = o["stats"]["last_density_error"]
+            self._error("density_error_read%s" % tag, gpu, *ps.loop_error("density", o["predicted_density"], mutant=m))
+            if not pre:
+                self._nonzero("density", ps, o["predicted_density"] > ps.rho0)
+            p = run(self.make_world, sc, forces=forces, steps=pre + [(dt, (1, k - 1), ZERO_G)])[-1]
+            assert np.array_equal(p["predicted_density"], o["predicted_density"])
+            vs = (p["V"] + p["velocity_change"]).astype(F)
+            ref = ps.divergence(vs, p["bvol"], predicted=True, bvel=bvel, dens=p["density"], dt=dt)
+            self._error("density_error%s" % tag, gpu, *ps.loop_error("density", ref, C_PASS["predicted"], mutant=m))
+
+    def loop_exits(self, factor, margin=0.25):
+        """min_divergence_iter = 0, so evaluation 0 may end the divergence loop.  Step 1 at DT pinned (1, 1); step 2 at
+        dt = factor DT runs free, with max_divergence_error set so that the threshold max_err * inv_dt * 0.01 (float32, in
+        the reference's order) lies `margin` above the float64 error e0 of step 2's evaluation 0 under inv_dt_prev = 1 / DT
+        (margin > 0) or below it (margin < 0).  With factor = 2 and margin 0.25, the threshold under inv_dt_cur lies 37.5 %
+        below e0; with factor = 1/2 and margin -0.25, 50 % above.  The loop must end on evaluation 0 exactly when the
+        threshold under inv_dt_prev lies above e0.  Likewise max_density_error, `margin` off the density error of step
+        2's evaluation 0, whose predicted densities use dt_cur."""
+        sc, m = self.scene, self.mutant
+        dt = DT * factor
+        first = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G)])[-1]
+        ps = passes_for(sc, P=first["P"], kw=self.ps.kw, kg=self.ps.kg)
+        e0, b0 = ps.loop_error("divergence", ps.divergence(self._vstar(first), first["bvol"]), C_PASS["divergence"])
+        inv_prev, inv_cur = F(1.0) / F(DT), F(1.0) / F(dt)
+        mde = F(e0 * (1.0 + margin) / (float(inv_prev) * 0.01))
+        thr = lambda inv: float(F(F(mde * inv) * F(0.01)))  # noqa: E731
+        o = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (None, 0), ZERO_G)], min_divergence_iter=0,
+                max_divergence_error=float(mde))[-1]["stats"]
+        inv = inv_cur if m == "div_threshold_current_inv_dt" else inv_prev
+        ends = e0 <= thr(inv)
+        ok = (o["n_divergence_iter"] == 0) if ends else (o["n_divergence_iter"] >= 1)
+        name = "exit_%s" % ("ends" if margin > 0 else "iterates")
+        self.worst["divergence_" + name] = 0.0 if ok else np.inf
+        # the pressure loop, the divergence loop pinned to one update: the density error of evaluation 0 with dt_cur (a
+        # run pinned to stop there gives its inputs)
+        p = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (1, 0), ZERO_G)])[-1]
+        bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
+        vs = (p["V"] + p["velocity_change"]).astype(F)
+        d0, db0 = ps.loop_error("density", ps.divergence(vs, p["bvol"], predicted=True, bvel=bvel, dens=p["density"], dt=dt),
+                                C_PASS["predicted"])
+        mxd = F(d0 * (1.0 + margin))
+        q = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (1, None), ZERO_G)], min_pressure_iter=0,
+                max_density_error=float(mxd))[-1]["stats"]
+        pok = (q["n_pressure_iter"] == 0) if d0 <= float(mxd) else (q["n_pressure_iter"] >= 1)
+        self.worst["density_" + name] = 0.0 if pok else np.inf
+        # how far the decisions lie from the rounding: |threshold - e0| in units of e0's bound
+        self.exit_margin = min(getattr(self, "exit_margin", np.inf), abs(thr(inv_prev) - e0) / b0, abs(float(mxd) - d0) / db0)
+
+    def lagging_dt(self, dts=(DT, 2 * DT, DT / 3), gravity=(0.0, -9.81, 0.0)):
+        """Steps of varying length under gravity, each checked step pinned at (0, 0), (1, 0) and (1, 1) after the steps
+        before it at (1, 1).  The divergence loop and the forces run before timestep.advance and see the previous step's dt
+        (dfsph_solver.rs:686-702); the pressure loop, the integration and the positions see the current one.  Per particle:
+          carried     evaluation 0 fed the positions P1 and v + vc of the step before, both read back (vc survives the
+                      step, dfsph_solver.rs:704-706, and rides the counting sort);
+          update      the divergence update, and its boundary reaction with inv_dt_prev;
+          integrate   vc = acc dt_cur;
+          predicted   the predicted density with dt_cur;
+          pressure    the pressure update and the sum of both updates' boundary reactions, with inv_dt_cur;
+          positions   P1 + (v + vc) dt_cur.
+        moved_cells: the largest number of particles whose cell of side h, counted from the world origin, changed in one
+        checked step's predecessor.  The engine's grid has its own origin and cell order, so this is a proxy for how many
+        particles the counting sort moved, not the engine's count; likewise the vc_carried_unsorted mutant permutes vc
+        by a lexicographic order of those cells, a stand-in for the engine's previous sort."""
+        sc, m = self.scene, self.mutant
+        bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
+        rho0 = self.ps.rho0.astype(F)
+        P_before = self.ps.P
+        for s in range(1, len(dts)):
+            pre = [(d, (1, 1), gravity) for d in dts[:s]]
+            dt, dt_prev = dts[s], dts[s - 1]
+            o = {it: run(self.make_world, sc, steps=pre + [(dt, it, gravity)]) for it in ((0, 0), (1, 0), (1, 1))}
+            o1 = o[(1, 1)][-2]
+            o00, o10, o11 = o[(0, 0)][-1], o[(1, 0)][-1], o[(1, 1)][-1]
+            ps = passes_for(sc, P=o1["P"], kw=self.ps.kw, kg=self.ps.kg)
+            assert np.array_equal(o00["num_fluid_contacts"], ps.nf) and np.array_equal(o00["num_boundary_contacts"], ps.nb)
+            cell = lambda P: np.floor(np.asarray(P, np.float64) / ps.h)  # noqa: E731
+            self.moved_cells = max(getattr(self, "moved_cells", 0), int((cell(o1["P"]) != cell(P_before)).any(axis=1).sum()))
+            inv_prev, inv_cur = F(1.0) / F(dt_prev), F(1.0) / F(dt)
+            bvol = o00["bvol"]
+            vstar = self._vstar(o1)
+            if m == "vc_carried_unsorted":   # vc kept in the order of the previous sort: particles that changed cell swap
+                vc = o1["velocity_change"]
+                key = lambda P: np.lexsort(cell(P).T[::-1])  # noqa: E731
+                moved = np.empty_like(vc)
+                moved[key(o1["P"])] = vc[key(P_before)]
+                vstar = (o1["V"] + moved).astype(F)
+            self.record("carried_divergence", o00["divergence"], ps.divergence(vstar, bvol), C_PASS["divergence"], ps=ps)
+            kappa = (o00["divergence"] * o00["alpha"]).astype(F)
+            self.record("lagging_update", o10["V"], ps.update(kappa, bvol, vstar), C_PASS["update"], ps=ps)
+            sd = inv_cur if m == "div_bforce_current_inv_dt" else inv_prev
+            rdiv = ps.update_boundary_force(kappa, bvol, sd, pressure=False)
+            self.record_boundary("lagging_boundary_force_divergence", o10["bforce"], rdiv, ps=ps)
+            vc0 = o10["velocity_change"]
+            self.record("lagging_integrate", vc0, ps.integrate(o10["acceleration"], dt), ref64.C_INTEGRATE,
+                        exclude=np.zeros(ps.N, bool), ambiguous=False)
+            vs = (o10["V"] + vc0).astype(F)
+            self.record("lagging_predicted", o10["predicted_density"],
+                        ps.divergence(vs, bvol, predicted=True, bvel=bvel, dens=o10["density"], dt=dt), C_PASS["predicted"], ps=ps)
+            kp = np.maximum(((o10["predicted_density"] - rho0).astype(F) * o10["alpha"]).astype(F), F(0))
+            self.record("lagging_pressure_update", o11["velocity_change"], ps.update(kp, bvol, vc0, pressure=True, inv_dt=inv_cur),
+                        C_PASS["update"], ps=ps)
+            rp = ps.update_boundary_force(kp, bvol, inv_cur)
+            both = ref64.Ref(rdiv.value + rp.value, rdiv.A + rp.A, rdiv.K + rp.K, rdiv.n + rp.n)
+            self.record_boundary("lagging_boundary_force_both", o11["bforce"], both, ps=ps)
+            dtp = dt_prev if m == "positions_previous_dt" else dt
+            self.record("lagging_positions", o11["P"], ps.positions(o1["P"], o11["V"], o11["velocity_change"], dtp),
+                        ref64.C_POSITIONS, exclude=np.zeros(ps.N, bool), ambiguous=False)
+            P_before = o1["P"]
+
+    def grid_growth(self):
+        """Two steps pinned at (0, 0): the second step's per-particle contact counts on the positions the first left.
+        grown: how far (in cells) those positions reach beyond the first step's bounding box."""
+        o = run(self.make_world, self.scene, steps=[(DT, (0, 0), ZERO_G)] * 2)
+        ps1 = passes_for(self.scene, P=o[0]["P"], kw=self.ps.kw, kg=self.ps.kg)
+        same = np.array_equal(o[1]["num_fluid_contacts"], ps1.nf) and np.array_equal(o[1]["num_boundary_contacts"], ps1.nb)
+        self.worst["grown_counts"] = 0.0 if same else np.inf
+        P0, P1 = self.ps.P.astype(np.float64), o[0]["P"].astype(np.float64)
+        self.grown = float(max((P0.min(0) - P1.min(0)).max(), (P1.max(0) - P0.max(0)).max()) / self.ps.h)
 
     def flagged(self):
         return {k: v for k, v in self.worst.items() if not v <= 1.0}
