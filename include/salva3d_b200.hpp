@@ -13,7 +13,8 @@
 //   LiquidWorld::{remove_fluid, remove_boundary, step_with_coupling, particles_intersecting_shape}          liquid_world.rs:67-178,246-281
 //   trait CouplingManager                                                                                    coupling/coupling_manager.rs:9-28
 //   NonPressureForce::solve with contacts and boundaries (CustomNonPressureForceWithContacts)                nonpressure_force.rs:15-27
-//   ColliderCouplingSet::{register_coupling, unregister_coupling} + ColliderSampling::StaticSampling, run on the device
+//   ColliderCouplingSet::{register_coupling, unregister_coupling} + ColliderSampling::{StaticSampling, DynamicContactSampling},
+//   run on the device
 //   (the rigid bodies stay with the caller: set_collider_state before a step, collider_impulse after it)   fluids_pipeline.rs:64-287
 // Every call goes to libsalva_b200.so (CUDA); there is no CPU path.
 #pragma once
@@ -159,10 +160,25 @@ struct Isometry3 {
 struct Ball { Real radius; };
 struct Cuboid { Vector3 half_extents; };
 struct Capsule { Real half_height, radius; };  // segment along local y
-// ColliderSampling (fluids_pipeline.rs:64-72); StaticSampling is the sampling the device path implements
+// ColliderSampling (fluids_pipeline.rs:64-72): both samplings run on the device
 struct ColliderSampling {
-    std::vector<Point3> points;  // in the collider's local frame
+    std::vector<Point3> points;  // StaticSampling: in the collider's local frame
+    int32_t kind = SPH_SAMPLING_STATIC;
+    sph_shape shape{};           // DynamicContactSampling: the collider's shape
     static ColliderSampling StaticSampling(std::vector<Point3> points) { return ColliderSampling{std::move(points)}; }
+    static ColliderSampling DynamicContactSampling(const Ball& s) { return contact(sph_shape{SPH_SHAPE_BALL, {s.radius}}); }
+    static ColliderSampling DynamicContactSampling(const Cuboid& s) {
+        return contact(sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}});
+    }
+    static ColliderSampling DynamicContactSampling(const Capsule& s) { return contact(sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}); }
+
+private:
+    static ColliderSampling contact(sph_shape shape) {
+        ColliderSampling c;
+        c.kind = SPH_SAMPLING_CONTACT;
+        c.shape = shape;
+        return c;
+    }
 };
 using ColliderHandle = uint32_t;
 
@@ -455,10 +471,12 @@ public:
         return shape_query(pos, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}});
     }
     // ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114: the boundary's particles become the collider's samples
+    // (DynamicContactSampling: from the next step on, its size changes every step)
     ColliderHandle register_coupling(BoundaryHandle boundary, const ColliderSampling& sampling) {
         Boundary& b = boundaries_.at(boundary);
         uint32_t c = 0;
-        check(sph_collider_register(raw_, b.handle_, SPH_SAMPLING_STATIC, nullptr, fp(sampling.points), sampling.points.size(), &c));
+        check(sph_collider_register(raw_, b.handle_, sampling.kind, sampling.kind == SPH_SAMPLING_CONTACT ? &sampling.shape : nullptr,
+                                    fp(sampling.points), sampling.points.size(), &c));
         b.coupled_ = true;
         pull_results();
         return c;

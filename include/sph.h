@@ -307,9 +307,15 @@ sph_status sph_world_step_with_coupling(sph_world* w, float dt, const float grav
  * (liquid_world.rs:86-103).  The rigid-body engine stays with the caller: before each step it hands over each collider's
  * pose and body velocities (sph_collider_set_state), after it reads the impulse the fluid applied (sph_collider_read_impulse).
  * Colliders cannot be combined with a host sph_coupling_manager in one step, nor used in slab-decomposed worlds; a collider
- * whose boundary was removed is inert and no longer counts.  ColliderSampling::DynamicContactSampling (fluids_pipeline.rs:71,
- * 192-255) has no device path: contact-sample through sph_world_step_with_coupling (examples/coupling3.cpp). */
-enum { SPH_SAMPLING_STATIC = 0 };  /* ColliderSampling::StaticSampling(points)  fluids_pipeline.rs:69,180-191 */
+ * whose boundary was removed is inert and no longer counts. */
+enum { SPH_SAMPLING_STATIC = 0,    /* ColliderSampling::StaticSampling(points)  fluids_pipeline.rs:69,180-191 */
+       SPH_SAMPLING_CONTACT = 1 }; /* ColliderSampling::DynamicContactSampling  fluids_pipeline.rs:71,192-255: every step, after the
+   fluids are in the cell grid, each fluid particle in the cells of the posed shape's AABB loosened by 1.5 h whose predicted
+   position p = pos + vel * dt (the lagging dt) lies in that AABB is projected onto the shape's surface; a particle inside is
+   pushed out along the projection normal by depth + 0.1 particle_radius and loses its velocity into the shape; the projection
+   becomes a boundary particle with the body's velocity at that WORLD point, unless p lies more than 1.5 h outside.  Colliders
+   run in slot order; the boundary holds its samples ordered by the sampled particle's fluid slot, then index.  A ball's
+   centre yields no sample; a point on a capsule's axis projects along local +x.  See DESIGN.md section 10. */
 enum { SPH_BODY_NONE = 0,     /* collider.parent() == None: velocity 0, boundary.forces left as it is (fluids_pipeline.rs:163-171),
                                  no impulse (transmit_forces needs the parent body, :273-276) */
        SPH_BODY_FIXED = 1,    /* !body.is_dynamic(): boundary.forces = None, no impulse */
@@ -323,7 +329,9 @@ typedef struct {
 /* ColliderCouplingSet::register_coupling(boundary, collider, sampling)  fluids_pipeline.rs:98-114.  StaticSampling: the n_points
  * local points (packed xyz) become the boundary's particles; every step they are posed by the collider's state, with the
  * velocity velocity_at_point(pt) evaluated at the LOCAL point pt, as fluids_pipeline.rs:183 does (a quirk of the reference,
- * reproduced).  `shape` may be NULL for StaticSampling.  The engine owns the boundary's particle set from then on:
+ * reproduced).  `shape` may be NULL for StaticSampling.  SPH_SAMPLING_CONTACT needs a ball, cuboid or capsule `shape` with
+ * finite, non-negative parameters and n_points == 0; the boundary keeps its particles until the next step refills it, and its
+ * particle count changes every step (sph_boundary_count).  The engine owns the boundary's particle set from then on:
  * sph_boundary_write / _set_particles refuse it.  A boundary can be coupled to one collider at a time.  The initial state
  * is the identity pose with SPH_BODY_NONE.  Handles are slot | generation << 16. */
 sph_status sph_collider_register(sph_world* w, uint32_t boundary, int32_t sampling, const sph_shape* shape, const float* local_points_xyz,

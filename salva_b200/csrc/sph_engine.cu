@@ -5,6 +5,7 @@
 //
 // There is no CPU fallback: every entry point needs a CUDA device.
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
 #include <climits>
@@ -99,10 +100,12 @@ struct BoundaryRec {
     bool alive = true;
     uint32_t gen = 0;
 };
-// ColliderCouplingEntry (fluids_pipeline.rs:76-80) of a StaticSampling collider
+// ColliderCouplingEntry (fluids_pipeline.rs:76-80)
 struct ColliderRec {
     uint32_t boundary = 0;          // boundary handle; a removed boundary leaves the collider inert
-    size_t n = 0;                   // sample points
+    int32_t sampling = SPH_SAMPLING_STATIC;
+    sph_shape shape{};              // SPH_SAMPLING_CONTACT: the collider's shape
+    size_t n = 0;                   // StaticSampling: sample points
     DBuf<float4> local;             // the points in the collider's frame
     sph_collider_state state{};     // for the next step
     sph_collider_state applied{};   // what the boundary's particles on the device were posed with
@@ -217,6 +220,14 @@ struct sph_world {
     DBuf<int> d_cb;         // boundary cell AABB + bad flag after colliders moved (as k_bounds writes it)
     DBuf<float> d_imp;      // 6 floats per collider slot: the impulses of the step
     float* h_imp = nullptr;  // pinned copy, read back with the step's final read-back
+    // DynamicContactSampling (colliders_contact): collider table, result ints, growing sample / push records, sort buffers
+    DBuf<ContactCollider> d_ccol;
+    DBuf<int> d_cres;
+    DBuf<float4> cs_s4, cs_p4;
+    DBuf<unsigned long long> cs_key[2];
+    DBuf<uint32_t> cs_val[2];
+    DBuf<char> cs_tmp;
+    uint32_t cap_s = 4096, cap_p = 4096;
 
     // sorted device state (double buffered for the counting sort)
     int cur = 0, bcur = 0;
@@ -746,6 +757,186 @@ sph_status colliders_impulse(sph_world* w) {
     w->launches++;
     CU(cudaMemcpyAsync(w->h_imp, w->d_imp.p, bytes, cudaMemcpyDeviceToHost, w->st));
     return SPH_OK;
+}
+
+// Half extents of the AABB of a ball / cuboid / capsule (segment along local y) under the rotation R: the box parry's
+// compute_aabb(pos) centres on the translation.
+void posed_aabb_ext(const sph_shape& s, const float R[9], float ext[3]) {
+    for (int a = 0; a < 3; ++a) {
+        if (s.kind == SPH_SHAPE_BALL) ext[a] = s.p[0];
+        else if (s.kind == SPH_SHAPE_CUBOID) ext[a] = std::fabs(R[3 * a]) * s.p[0] + std::fabs(R[3 * a + 1]) * s.p[1] + std::fabs(R[3 * a + 2]) * s.p[2];
+        else ext[a] = std::fabs(R[3 * a + 1]) * s.p[0] + s.p[1];  // the segment, swept by the radius
+    }
+}
+
+sph_status phase_grid(sph_world* w);
+
+bool any_contact(const sph_world* w) {
+    for (const ColliderRec& c : w->colliders)
+        if (c.alive && c.sampling == SPH_SAMPLING_CONTACT && boundary_slot(w, c.boundary) >= 0) return true;
+    return false;
+}
+
+// ColliderCouplingManager::update_boundaries (fluids_pipeline.rs:192-255) for DynamicContactSampling colliders.  Runs after
+// the fluid sort of phase_grid, where a host CouplingManager runs (liquid_world.rs:90-103): k_contact_sample finds the
+// candidates in each collider's cell box and appends sample and push records; the pushes are applied and the cell bounds of
+// the fluid and of the new boundary set reduced, and ONE read-back brings the counts and bounds to the host.  Then, with
+// nothing more read back, the samples are radix-sorted by (collider slot, original fluid index), the boundary arrays are
+// rebuilt in original order (the other boundaries un-sorted through borig to their new offsets) and the grid is rebuilt
+// from the bounds already read back: the pushes moved particles, and the re-sort also refreshes v* = vel + vc.
+sph_status colliders_contact(sph_world* w) {
+    const size_t N = w->N, B = w->B;
+    const Consts& hc = w->hc;
+    const int xs = hc.xysub > 0 ? hc.xysub : 1;  // the grid counts x and y in bins of h / xysub
+    const int go[3] = {hc.ox / xs, hc.oy / xs, hc.oz}, gn[3] = {hc.nx / xs, hc.ny / xs, hc.nz};
+    const float h = w->h, prediction = h * 0.5f, cut = h + prediction, margin = w->desc.particle_radius * 0.1f;
+    std::vector<ContactCollider> cc;
+    unsigned long long skip = 0;
+    size_t bins = 0;
+    for (size_t k = 0; k < w->colliders.size(); ++k) {
+        const ColliderRec& c = w->colliders[k];
+        if (!c.alive || c.sampling != SPH_SAMPLING_CONTACT) continue;
+        const int bs = boundary_slot(w, c.boundary);
+        if (bs < 0) continue;
+        skip |= 1ull << bs;
+        ContactCollider K;
+        memset(&K, 0, sizeof K);
+        K.kind = c.shape.kind;
+        K.slot = (uint32_t)k;
+        memcpy(K.rot, c.state.rotation_rowmajor, sizeof K.rot);
+        memcpy(K.t, c.state.translation, sizeof K.t);
+        for (int a = 0; a < 3; ++a) K.sp[a] = c.shape.p[a];
+        memcpy(K.linvel, c.state.linvel, sizeof K.linvel);
+        memcpy(K.angvel, c.state.angvel, sizeof K.angvel);
+        memcpy(K.com, c.state.world_com, sizeof K.com);
+        K.moving = c.state.body != SPH_BODY_NONE;
+        float ext[3];
+        posed_aabb_ext(c.shape, K.rot, ext);
+        size_t nbin = 1;
+        for (int a = 0; a < 3; ++a) {
+            K.mins[a] = (K.t[a] - ext[a]) - cut;  // compute_aabb(pos).loosened(h + prediction)
+            K.maxs[a] = (K.t[a] + ext[a]) + cut;
+            // hgrid.rs:41-52 keys; clamped where no particle can be (k_bounds refuses |cell| >= 1e9)
+            const float flo = std::fmin(std::fmax(std::floor(K.mins[a] / h), -1.5e9f), 1.5e9f);
+            const float fhi = std::fmin(std::fmax(std::floor(K.maxs[a] / h), -1.5e9f), 1.5e9f);
+            K.clo[a] = (int)flo;
+            K.chi[a] = (int)fhi;
+            const int lo = std::max(K.clo[a], go[a]), hi = std::min(K.chi[a], go[a] + gn[a] - 1);
+            const int sub = a < 2 ? xs : 1;
+            K.bl[a] = lo * sub;
+            K.bd[a] = hi < lo ? 0 : (hi - lo + 1) * sub;
+            nbin *= (size_t)K.bd[a];
+        }
+        K.first_bin = (uint32_t)bins;
+        bins += nbin;
+        if (bins > (size_t)(UINT32_MAX / 64)) return w->fail(SPH_ERR_OOM, "contact sampling: collider cell boxes too large");
+        cc.push_back(K);
+    }
+    const int nc = (int)cc.size();
+    CU(w->d_ccol.ensure(nc));
+    CU(cudaMemcpyAsync(w->d_ccol.p, cc.data(), nc * sizeof(ContactCollider), cudaMemcpyHostToDevice, w->st));
+    constexpr int NRES = CS_PER_COLLIDER + MAX_BOUNDARIES;
+    int init[NRES] = {};
+    for (int base : {CS_FLUID_BOUNDS, CS_BOUND_BOUNDS})
+        for (int a = 0; a < 3; ++a) {
+            init[base + a] = INT_MAX;
+            init[base + 3 + a] = INT_MIN;
+        }
+    int res[NRES];
+    CU(w->d_cres.ensure(NRES));
+    const int c = w->cur, bc = w->bcur;
+    for (;;) {
+        CU(w->cs_s4.ensure(2 * (size_t)w->cap_s));
+        CU(w->cs_key[0].ensure(w->cap_s));
+        CU(w->cs_val[0].ensure(w->cap_s));
+        CU(w->cs_p4.ensure(2 * (size_t)w->cap_p));
+        CU(cudaMemcpyAsync(w->d_cres.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
+        if (N && bins) {
+            ContactParams P{w->d_ccol.p, nc, (uint32_t)bins, w->dt, cut, margin, w->cap_s, w->cap_p};
+            LAUNCH(k_contact_sample, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p, w->cs_key[0].p,
+                   w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
+            k_contact_apply<<<std::min<uint32_t>(cdiv(w->cap_p, 256), 264), 256, 0, w->st>>>(w->cs_p4.p, w->d_cres.p, w->cap_s, w->cap_p, w->pos[c].p,
+                                                                                         w->vel[c].p);
+            w->launches++;
+        }
+        if (N) {
+            k_bounds<<<std::min<uint32_t>(cdiv(N, 256), 296), 256, 0, w->st>>>(w->pos[c].p, (uint32_t)N, w->d_cres.p + CS_FLUID_BOUNDS);
+            w->launches++;
+        }
+        if (B) {
+            k_bounds_kept<<<std::min<uint32_t>(cdiv(B, 256), 296), 256, 0, w->st>>>(w->bpos[bc].p, w->bvel[bc].p, (uint32_t)B, skip,
+                                                                                   w->d_cres.p + CS_BOUND_BOUNDS);
+            w->launches++;
+        }
+        CU(cudaMemcpyAsync(res, w->d_cres.p, sizeof res, cudaMemcpyDeviceToHost, w->st));
+        CU(cudaStreamSynchronize(w->st));  // the step's one contact-sampling round trip
+        const uint32_t ns = (uint32_t)res[CS_SAMPLES], np = (uint32_t)res[CS_PUSHES];
+        if (ns <= w->cap_s && np <= w->cap_p) break;
+        // nothing was written to the fluid: re-run with room for every record
+        w->cap_s = std::max(w->cap_s, ns + ns / 4);
+        w->cap_p = std::max(w->cap_p, np + np / 4);
+    }
+    const uint32_t M = (uint32_t)res[CS_SAMPLES];
+    // the coupled boundaries' new sizes and everyone's new offsets
+    ContactRebuild T;
+    memset(&T, 0, sizeof T);
+    T.skip = skip;
+    for (size_t b = 0; b < w->bounds.size(); ++b) T.old_off[b] = (uint32_t)w->bounds[b].offset;
+    for (size_t k = 0; k < w->colliders.size(); ++k) {
+        const ColliderRec& cr = w->colliders[k];
+        const int bs = cr.alive && cr.sampling == SPH_SAMPLING_CONTACT ? boundary_slot(w, cr.boundary) : -1;
+        if (bs >= 0) w->bounds[bs].n = (size_t)res[CS_PER_COLLIDER + k];
+    }
+    recompute_offsets(w);
+    for (size_t b = 0; b < w->bounds.size(); ++b) T.new_off[b] = (uint32_t)w->bounds[b].offset;
+    uint32_t first = 0;
+    for (size_t k = 0; k < w->colliders.size(); ++k) {
+        const ColliderRec& cr = w->colliders[k];
+        const int bs = cr.alive && cr.sampling == SPH_SAMPLING_CONTACT ? boundary_slot(w, cr.boundary) : -1;
+        if (bs < 0) continue;
+        T.col_first[k] = first;
+        T.col_dst[k] = (uint32_t)w->bounds[bs].offset;
+        T.col_bslot[k] = (uint32_t)bs;
+        first += (uint32_t)res[CS_PER_COLLIDER + k];
+    }
+    const size_t NB = w->B;
+    const int nbc = bc ^ 1;
+    CU(w->bpos[bc].ensure(NB, true, w->st));  // the source of the rebuild, the target of the next boundary sort
+    CU(w->bvel[bc].ensure(NB, true, w->st));
+    CU(w->borig[bc].ensure(NB, true, w->st));
+    CU(w->bpos[nbc].ensure(NB));
+    CU(w->bvel[nbc].ensure(NB));
+    CU(w->borig[nbc].ensure(NB));
+    CU(w->bvol.ensure(NB));
+    CU(w->bcid.ensure(NB));
+    CU(w->brank.ensure(NB));
+    CU(w->bperm.ensure(NB));
+    CU(w->bforce.ensure(3 * NB));
+    if (M) {
+        CU(w->cs_key[1].ensure(M));
+        CU(w->cs_val[1].ensure(M));
+        const int end_bit = 32 + 6;  // collider slots < MAX_BOUNDARIES = 64
+        size_t tmp = 0;
+        CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, w->cs_key[0].p, w->cs_key[1].p, w->cs_val[0].p, w->cs_val[1].p, (int)M, 0, end_bit, w->st));
+        CU(w->cs_tmp.ensure(tmp));
+        CU(cub::DeviceRadixSort::SortPairs(w->cs_tmp.p, tmp, w->cs_key[0].p, w->cs_key[1].p, w->cs_val[0].p, w->cs_val[1].p, (int)M, 0, end_bit,
+                                           w->st));
+        w->launches++;  // (CUB's passes count as one)
+    }
+    LAUNCH(k_contact_keep, B, 256, (uint32_t)B, w->bpos[bc].p, w->bvel[bc].p, w->borig[bc].p, T, w->bpos[nbc].p, w->bvel[nbc].p, w->borig[nbc].p);
+    LAUNCH(k_contact_write, M, 256, M, w->cs_key[1].p, w->cs_val[1].p, w->cs_s4.p, T, w->bpos[nbc].p, w->bvel[nbc].p, w->borig[nbc].p);
+    w->bcur = nbc;
+    memcpy(w->b_aabb, res + CS_BOUND_BOUNDS, sizeof w->b_aabb);
+    w->b_bad = res[CS_BOUND_BOUNDS + 6] != 0;
+    memcpy(w->nb, res + CS_FLUID_BOUNDS, sizeof w->nb);
+    w->nb_valid = N > 0;  // phase_grid sizes the grid from these bounds, without a bounds pass of its own
+    w->b_sorted_valid = false;
+    w->lists_valid = false;
+    w->hb_pos.resize(3 * NB);
+    w->hb_vel.resize(3 * NB);
+    w->hb_stale = true;
+    w->stats.n_boundary_particles = NB;
+    return phase_grid(w);
 }
 
 // fluid.rs:88-98 apply_particles_removal (+ solver scratch filtering dfsph_solver.rs:550-559)
@@ -1757,6 +1948,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     TRY(phase_grid(w));
     w->grid_ready = true;
     w->ever_stepped = true;
+    if (colliders && any_contact(w)) TRY(colliders_contact(w));
     if (coupling && coupling->update_boundaries) {
         // CouplingManager::update_boundaries runs after the FLUIDS of this substep are in the grid and before the boundaries
         // are (liquid_world.rs:86-103): queries issued by the callback see the fluid particles only.  The callback may rewrite
@@ -2331,28 +2523,26 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
     const float* R = rotation_rowmajor ? rotation_rowmajor : ident;
     for (int k = 0; k < 9; ++k) q.rot[k] = R[k];
     for (int a = 0; a < 3; ++a) q.t[a] = translation[a];
-    float ext[3];  // half extents of the posed shape's AABB
     switch (shape->kind) {
         case SPH_SHAPE_BALL:
             if (!(shape->p[0] >= 0.f)) return w->fail(SPH_ERR_INVALID, "ball radius must be >= 0");
             q.kind = 1;
             q.sp[0] = shape->p[0];
-            ext[0] = ext[1] = ext[2] = shape->p[0];
             break;
         case SPH_SHAPE_CUBOID:
             q.kind = 2;
             for (int a = 0; a < 3; ++a) q.sp[a] = shape->p[a];
-            for (int a = 0; a < 3; ++a) ext[a] = std::fabs(R[3 * a]) * shape->p[0] + std::fabs(R[3 * a + 1]) * shape->p[1] + std::fabs(R[3 * a + 2]) * shape->p[2];
             break;
         case SPH_SHAPE_CAPSULE:
             q.kind = 3;
             q.sp[0] = shape->p[0];
             q.sp[1] = shape->p[1];
-            for (int a = 0; a < 3; ++a) ext[a] = std::fabs(R[3 * a + 1]) * shape->p[0] + shape->p[1];  // segment along local y, swept by the radius
             break;
         default:
             return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
     }
+    float ext[3];  // half extents of the posed shape's AABB
+    posed_aabb_ext(*shape, R, ext);
     float mins[3], maxs[3];
     for (int a = 0; a < 3; ++a) {
         mins[a] = translation[a] - ext[a];
@@ -2695,7 +2885,14 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     BOUNDARY_OR_FAIL(boundary, boundary_h)
     if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "boundary %u is already coupled to a collider", (unsigned)boundary_h);
     if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE)) return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
-    if (sampling != SPH_SAMPLING_STATIC) return w->fail(SPH_ERR_INVALID, "unknown sampling %d (StaticSampling is the only one)", sampling);
+    if (sampling != SPH_SAMPLING_STATIC && sampling != SPH_SAMPLING_CONTACT) return w->fail(SPH_ERR_INVALID, "unknown sampling %d", sampling);
+    if (sampling == SPH_SAMPLING_CONTACT) {
+        if (!shape) return w->fail(SPH_ERR_INVALID, "DynamicContactSampling needs the collider's shape");
+        if (n) return w->fail(SPH_ERR_INVALID, "DynamicContactSampling takes no sample points");
+        const int np = shape->kind == SPH_SHAPE_BALL ? 1 : shape->kind == SPH_SHAPE_CUBOID ? 3 : 2;
+        for (int a = 0; a < np; ++a)
+            if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f)) return w->fail(SPH_ERR_INVALID, "shape parameters must be finite and >= 0");
+    }
     if (n >= (size_t)UINT32_MAX) return w->fail(SPH_ERR_INVALID, "too many sample points");
     for (size_t k = 0; k < 3 * n; ++k)
         if (!std::isfinite(pts[k])) return w->fail(SPH_ERR_INVALID, "non-finite sample point");
@@ -2709,6 +2906,8 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     ColliderRec c;
     if (slot < w->colliders.size()) c.gen = w->colliders[slot].gen + 1;
     c.boundary = boundary_h;
+    c.sampling = sampling;
+    if (shape) c.shape = *shape;
     c.n = n;
     c.state.rotation_rowmajor[0] = c.state.rotation_rowmajor[4] = c.state.rotation_rowmajor[8] = 1.f;
     c.state.body = SPH_BODY_NONE;
@@ -2718,6 +2917,12 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
         CU(c.local.ensure(n));
         CU(cudaMemcpyAsync(c.local.p, l.data(), n * sizeof(float4), cudaMemcpyHostToDevice, w->st));
         CU(cudaStreamSynchronize(w->st));
+    }
+    if (sampling == SPH_SAMPLING_CONTACT) {  // the boundary keeps its particles until the next step samples it
+        if (slot == w->colliders.size()) w->colliders.push_back(c);
+        else w->colliders[slot] = c;
+        *collider = make_handle(slot, c.gen);
+        return SPH_OK;
     }
     // the points become the boundary's particle set; the next step poses them
     TRY(pull_boundaries(w));

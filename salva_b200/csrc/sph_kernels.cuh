@@ -1525,6 +1525,277 @@ __global__ void k_collider_impulse(uint32_t nb, const float4* __restrict__ bpos,
     }
 }
 
+// ColliderCouplingManager::update_boundaries, DynamicContactSampling (fluids_pipeline.rs:192-255).  Each candidate fluid
+// particle is handled by one thread, which runs every contact collider whose cell box holds the particle's cell (of its
+// position at the start of the substep), in collider-slot order: a particle's pushes depend only on its own state and on
+// earlier colliders, so this is the reference's collider-major loop with slot order standing in for hash-map order.  The
+// pass does not write the fluid: it appends sample and push records (k_contact_apply writes the pushes), so it can be
+// re-run with larger buffers when they overflow.  Every operation is an explicit round-to-nearest one, a fixed float32
+// expression a host can restate.
+struct ContactCollider {
+    int kind;                       // 1 ball (sp[0] radius), 2 cuboid (sp half extents), 3 capsule along local y (sp[0] half height, sp[1] radius)
+    uint32_t slot;                  // collider slot: the samples' sort key
+    float rot[9], t[3], sp[3];      // world = rot * local + t
+    float mins[3], maxs[3];         // the posed shape's AABB loosened by h + prediction
+    int clo[3], chi[3];             // its cell box [key(mins), key(maxs)]
+    float linvel[3], angvel[3], com[3];
+    int moving;                     // 0: no parent body, sample velocity 0
+    uint32_t first_bin;             // first enumeration index of this collider's (grid-clipped) bin box
+    int bl[3], bd[3];               // that bin box: first bin and extent per axis
+};
+constexpr int CS_SAMPLES = 0, CS_PUSHES = 1, CS_FLUID_BOUNDS = 2, CS_BOUND_BOUNDS = 9, CS_PER_COLLIDER = 16;  // layout of the result ints
+struct ContactParams {
+    const ContactCollider* col;
+    int nc;                         // contact colliders, ascending slot
+    uint32_t total_bins;
+    float dt, cut, margin;          // lagging dt, h + prediction, 0.1 particle_radius
+    uint32_t cap_s, cap_p;
+};
+__device__ __forceinline__ bool contact_in_box(const ContactCollider& c, int cx, int cy, int cz) {
+    return cx >= c.clo[0] && cx <= c.chi[0] && cy >= c.clo[1] && cy <= c.chi[1] && cz >= c.clo[2] && cz <= c.chi[2];
+}
+// project_point_and_get_feature, non-solid, in the shape's local frame: false when the projection is undefined (ball centre)
+__device__ __forceinline__ bool contact_project_local(const ContactCollider& c, float lx, float ly, float lz, float* q, bool* inside) {
+    if (c.kind == 1) {  // parry Ball::project_local_point
+        const float n2 = dot3_rn(lx, ly, lz, lx, ly, lz);
+        if (n2 == 0.f) return false;  // parry divides by zero here (NaN): no sample, no push
+        *inside = n2 <= __fmul_rn(c.sp[0], c.sp[0]);
+        const float s = __fdiv_rn(c.sp[0], __fsqrt_rn(n2));
+        q[0] = __fmul_rn(lx, s); q[1] = __fmul_rn(ly, s); q[2] = __fmul_rn(lz, s);
+    } else if (c.kind == 2) {  // parry Aabb::project_local_point over [-e, e]
+        const float l[3] = {lx, ly, lz};
+        float mp[3], pm[3], sh[3];
+        bool in = true;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            mp[a] = __fsub_rn(-c.sp[a], l[a]);
+            pm[a] = __fsub_rn(l[a], c.sp[a]);
+            sh[a] = __fsub_rn(fmaxf(mp[a], 0.f), fmaxf(pm[a], 0.f));
+            in = in && sh[a] == 0.f;
+        }
+        if (in) {  // nearest face; a tie goes to the mins face, a tie across axes keeps the lowest axis
+            float best = -3.402823466e38f;
+            int id = 0;
+            bool is_mins = false;
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                if (mp[a] < pm[a]) {
+                    if (pm[a] > best) { id = a; is_mins = false; best = pm[a]; }
+                } else if (mp[a] > best) { id = a; is_mins = true; best = mp[a]; }
+            }
+#pragma unroll
+            for (int a = 0; a < 3; ++a) sh[a] = a == id ? (is_mins ? best : -best) : 0.f;
+        }
+        *inside = in;
+#pragma unroll
+        for (int a = 0; a < 3; ++a) q[a] = __fadd_rn(l[a], sh[a]);
+    } else {  // capsule: closest segment point, then out along (l - c) by the radius; on the axis along local +x
+        const float cy = fminf(fmaxf(ly, -c.sp[0]), c.sp[0]);
+        const float dy = __fsub_rn(ly, cy);
+        const float dn = __fsqrt_rn(dot3_rn(lx, dy, lz, lx, dy, lz));
+        *inside = dn <= c.sp[1];
+        if (dn == 0.f) {
+            q[0] = c.sp[1]; q[1] = cy; q[2] = 0.f;
+        } else {
+            const float s = __fdiv_rn(c.sp[1], dn);
+            q[0] = __fmul_rn(lx, s); q[1] = __fadd_rn(cy, __fmul_rn(dy, s)); q[2] = __fmul_rn(lz, s);
+        }
+    }
+    return true;
+}
+__device__ __forceinline__ void cell_bounds_add(float x, float y, float z, int* mn, int* mx, int* bad) {
+    const float c[3] = {floorf(__fdiv_rn(x, C.h)), floorf(__fdiv_rn(y, C.h)), floorf(__fdiv_rn(z, C.h))};
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        if (!(fabsf(c[a]) < 1.0e9f)) { *bad = 1; continue; }
+        mn[a] = min(mn[a], (int)c[a]);
+        mx[a] = max(mx[a], (int)c[a]);
+    }
+}
+__device__ __forceinline__ void warp_bounds_commit(int* mn, int* mx, int bad, int* out) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+        for (int o = 16; o > 0; o >>= 1) {
+            mn[a] = min(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
+            mx[a] = max(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
+        }
+    bad = __any_sync(0xffffffffu, bad);
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            if (mn[a] != INT_MAX) atomicMin(&out[a], mn[a]);
+            if (mx[a] != INT_MIN) atomicMax(&out[3 + a], mx[a]);
+        }
+        if (bad) atomicOr(&out[6], 1);
+    }
+}
+// One warp per enumerated bin (the bins of each collider's cell box, clipped to the grid); its lanes take the bin's particles.
+// A particle is processed by the enumeration of the lowest-slot collider whose box holds its cell.  Records:
+// samples  s4[2r] = (proj, orig), s4[2r+1] = (velocity, 0), key[r] = slot << 32 | orig, val[r] = r;
+// pushes   p4[2r] = (new position, sorted slot), p4[2r+1] = (new velocity, 0).
+__global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
+                                 const uint32_t* __restrict__ orig, float4* __restrict__ s4, unsigned long long* __restrict__ key, uint32_t* __restrict__ val,
+                                 float4* __restrict__ p4, int* __restrict__ res) {
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+    if (warp >= P.total_bins) return;  // warp-uniform
+    int e = 0;
+    while (e + 1 < P.nc && P.col[e + 1].first_bin <= warp) ++e;
+    const ContactCollider& E = P.col[e];
+    const uint32_t t = warp - E.first_bin;
+    const int bz = E.bl[2] + (int)(t % (uint32_t)E.bd[2]);
+    const int by = E.bl[1] + (int)((t / (uint32_t)E.bd[2]) % (uint32_t)E.bd[1]);
+    const int bx = E.bl[0] + (int)(t / (uint32_t)(E.bd[2] * E.bd[1]));
+    const int cell = cell_id(bx, by, bz);
+    const uint32_t start = cstart[cell], end = cstart[cell + 1];
+    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN}, bad = 0;
+    for (uint32_t base = start; base < end; base += 32) {
+        const uint32_t j = base + lane;
+        bool mine = j < end;
+        float4 p = make_float4(0.f, 0.f, 0.f, 0.f), v = p;
+        int cx = 0, cy = 0, cz = 0;
+        if (mine) {
+            p = pos[j];
+            v = vel[j];
+            cx = cell_coord(p.x); cy = cell_coord(p.y); cz = cell_coord(p.z);
+            mine = contact_in_box(E, cx, cy, cz);
+            for (int k = 0; k < e && mine; ++k) mine = !contact_in_box(P.col[k], cx, cy, cz);
+        }
+        bool pushed = false;
+        for (int k = e; k < P.nc; ++k) {  // warp-uniform loop: every lane reaches the ballots
+            const ContactCollider& K = P.col[k];
+            bool emit = false;
+            float q[3] = {0.f, 0.f, 0.f}, sv[3] = {0.f, 0.f, 0.f};
+            if (mine && contact_in_box(K, cx, cy, cz)) {
+                const float pr[3] = {__fadd_rn(p.x, __fmul_rn(v.x, P.dt)), __fadd_rn(p.y, __fmul_rn(v.y, P.dt)), __fadd_rn(p.z, __fmul_rn(v.z, P.dt))};
+                emit = pr[0] >= K.mins[0] && pr[0] <= K.maxs[0] && pr[1] >= K.mins[1] && pr[1] <= K.maxs[1] && pr[2] >= K.mins[2] &&
+                       pr[2] <= K.maxs[2];
+                float lq[3];
+                bool inside = false;
+                if (emit) {
+                    const float wx = __fsub_rn(pr[0], K.t[0]), wy = __fsub_rn(pr[1], K.t[1]), wz = __fsub_rn(pr[2], K.t[2]);
+                    emit = contact_project_local(K, dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
+                                                 dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &inside);
+                }
+                if (emit) {
+#pragma unroll
+                    for (int a = 0; a < 3; ++a) q[a] = __fadd_rn(dot3_rn(K.rot[3 * a], K.rot[3 * a + 1], K.rot[3 * a + 2], lq[0], lq[1], lq[2]), K.t[a]);
+                    const float d[3] = {__fsub_rn(pr[0], q[0]), __fsub_rn(pr[1], q[1]), __fsub_rn(pr[2], q[2])};
+                    const float depth = __fsqrt_rn(dot3_rn(d[0], d[1], d[2], d[0], d[1], d[2]));
+                    if (depth > F32_EPS) {  // Unit::try_new_and_get(dpt, f32::EPSILON)
+                        const float n[3] = {__fdiv_rn(d[0], depth), __fdiv_rn(d[1], depth), __fdiv_rn(d[2], depth)};
+                        if (inside) {
+                            const float s = __fadd_rn(depth, P.margin);
+                            p.x = __fsub_rn(p.x, __fmul_rn(n[0], s));
+                            p.y = __fsub_rn(p.y, __fmul_rn(n[1], s));
+                            p.z = __fsub_rn(p.z, __fmul_rn(n[2], s));
+                            const float ve = dot3_rn(n[0], n[1], n[2], v.x, v.y, v.z);
+                            if (ve > 0.f) {
+                                v.x = __fsub_rn(v.x, __fmul_rn(n[0], ve));
+                                v.y = __fsub_rn(v.y, __fmul_rn(n[1], ve));
+                                v.z = __fsub_rn(v.z, __fmul_rn(n[2], ve));
+                            }
+                            pushed = true;
+                        } else if (depth > P.cut) {
+                            emit = false;
+                        }
+                    }
+                }
+                if (emit && K.moving) {  // body.velocity_at_point(proj) at the WORLD point
+                    const float dx = __fsub_rn(q[0], K.com[0]), dy = __fsub_rn(q[1], K.com[1]), dz = __fsub_rn(q[2], K.com[2]);
+                    sv[0] = __fadd_rn(K.linvel[0], __fsub_rn(__fmul_rn(K.angvel[1], dz), __fmul_rn(K.angvel[2], dy)));
+                    sv[1] = __fadd_rn(K.linvel[1], __fsub_rn(__fmul_rn(K.angvel[2], dx), __fmul_rn(K.angvel[0], dz)));
+                    sv[2] = __fadd_rn(K.linvel[2], __fsub_rn(__fmul_rn(K.angvel[0], dy), __fmul_rn(K.angvel[1], dx)));
+                }
+            }
+            const unsigned m = __ballot_sync(0xffffffffu, emit);
+            if (!m) continue;
+            uint32_t r0 = 0;
+            if (lane == 0) {
+                r0 = atomicAdd((uint32_t*)&res[CS_SAMPLES], (uint32_t)__popc(m));
+                atomicAdd(&res[CS_PER_COLLIDER + K.slot], __popc(m));
+            }
+            r0 = __shfl_sync(0xffffffffu, r0, 0);
+            if (emit) {
+                const uint32_t r = r0 + __popc(m & ((1u << lane) - 1u));
+                const uint32_t o = orig[j];
+                cell_bounds_add(q[0], q[1], q[2], mn, mx, &bad);
+                if (r < P.cap_s) {
+                    s4[2 * (size_t)r] = make_float4(q[0], q[1], q[2], __uint_as_float(o));
+                    s4[2 * (size_t)r + 1] = make_float4(sv[0], sv[1], sv[2], 0.f);
+                    key[r] = (unsigned long long)K.slot << 32 | o;
+                    val[r] = r;
+                }
+            }
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, pushed);
+        if (m) {
+            uint32_t r0 = 0;
+            if (lane == 0) r0 = atomicAdd((uint32_t*)&res[CS_PUSHES], (uint32_t)__popc(m));
+            r0 = __shfl_sync(0xffffffffu, r0, 0);
+            const uint32_t r = r0 + __popc(m & ((1u << lane) - 1u));
+            if (pushed && r < P.cap_p) {
+                p4[2 * (size_t)r] = make_float4(p.x, p.y, p.z, __uint_as_float(j));
+                p4[2 * (size_t)r + 1] = make_float4(v.x, v.y, v.z, 0.f);
+            }
+        }
+    }
+    warp_bounds_commit(mn, mx, bad, res + CS_BOUND_BOUNDS);
+}
+// The pushes of k_contact_sample, written only when neither record buffer overflowed (the pass is then re-run unchanged).
+__global__ void k_contact_apply(const float4* __restrict__ p4, const int* __restrict__ res, uint32_t cap_s, uint32_t cap_p, float4* __restrict__ pos,
+                                float4* __restrict__ vel) {
+    const uint32_t ns = (uint32_t)res[CS_SAMPLES], np = (uint32_t)res[CS_PUSHES];
+    if (ns > cap_s || np > cap_p) return;
+    for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < np; r += gridDim.x * blockDim.x) {
+        const float4 a = p4[2 * (size_t)r], b = p4[2 * (size_t)r + 1];
+        const uint32_t s = __float_as_uint(a.w);
+        pos[s] = make_float4(a.x, a.y, a.z, pos[s].w);
+        vel[s] = make_float4(b.x, b.y, b.z, vel[s].w);
+    }
+}
+// Cell bounds of the boundary particles that stay (boundaries not coupled by contact sampling: skip bit set).
+__global__ void k_bounds_kept(const float4* __restrict__ bpos, const float4* __restrict__ bvel, uint32_t n, unsigned long long skip, int* __restrict__ out) {
+    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN}, bad = 0;
+    for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) {
+        if ((skip >> fid_of(bvel[s])) & 1ull) continue;
+        const float4 p = bpos[s];
+        cell_bounds_add(p.x, p.y, p.z, mn, mx, &bad);
+    }
+    warp_bounds_commit(mn, mx, bad, out);
+}
+// Rebuild of the boundary arrays in ORIGINAL order: the boundaries that stay move to their new offsets...
+struct ContactRebuild {
+    uint32_t old_off[MAX_BOUNDARIES], new_off[MAX_BOUNDARIES];
+    unsigned long long skip;             // boundary slots refilled from samples
+    uint32_t col_first[MAX_BOUNDARIES];  // per collider slot: its first record in the sorted samples
+    uint32_t col_dst[MAX_BOUNDARIES];    // ... the new offset of its boundary
+    uint32_t col_bslot[MAX_BOUNDARIES];  // ... and that boundary's slot
+};
+__global__ void k_contact_keep(uint32_t nb, const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ borig,
+                               const ContactRebuild T, float4* __restrict__ opos, float4* __restrict__ ovel, uint32_t* __restrict__ oorig) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s >= nb) return;
+    const float4 v = bvel[s];
+    const uint32_t b = fid_of(v);
+    if ((T.skip >> b) & 1ull) return;
+    const uint32_t d = T.new_off[b] + (borig[s] - T.old_off[b]);
+    opos[d] = bpos[s];
+    ovel[d] = v;
+    oorig[d] = d;
+}
+// ... and the sorted samples (by collider slot, then original fluid index) fill the contact-coupled boundaries.
+__global__ void k_contact_write(uint32_t n, const unsigned long long* __restrict__ key, const uint32_t* __restrict__ val, const float4* __restrict__ s4,
+                                const ContactRebuild T, float4* __restrict__ opos, float4* __restrict__ ovel, uint32_t* __restrict__ oorig) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const uint32_t k = (uint32_t)(key[r] >> 32), src = val[r];
+    const uint32_t d = T.col_dst[k] + (r - T.col_first[k]);
+    const float4 a = s4[2 * (size_t)src], b = s4[2 * (size_t)src + 1];
+    opos[d] = make_float4(a.x, a.y, a.z, 0.f);
+    ovel[d] = make_float4(b.x, b.y, b.z, __uint_as_float(T.col_bslot[k]));
+    oorig[d] = d;
+}
+
 __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const uint32_t* __restrict__ cstart, const uint32_t* __restrict__ orig,
                              const float4* __restrict__ bpos, const uint32_t* __restrict__ bstart, const uint32_t* __restrict__ borig,
                              uint32_t* __restrict__ out, uint32_t cap, uint32_t* __restrict__ count) {

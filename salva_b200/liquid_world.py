@@ -173,6 +173,15 @@ class StaticSampling:
         self.points = np.ascontiguousarray(points, np.float32).reshape(-1, 3)
 
 
+class DynamicContactSampling:
+    """ColliderSampling::DynamicContactSampling (fluids_pipeline.rs:71, 192-255): every step the collider's shape (Ball,
+    Cuboid or Capsule) is sampled where the fluid is about to touch it, and penetrating fluid particles are pushed out."""
+    kind = 1
+
+    def __init__(self, shape):
+        self.shape = shape
+
+
 # the rigid body a collider is attached to (include/sph.h SPH_BODY_*)
 BODY_NONE, BODY_FIXED, BODY_DYNAMIC = 0, 1, 2
 
@@ -415,7 +424,10 @@ class LiquidWorld:
         h = C.c_uint32()
         self._ck(self._L.sph_collider_register(self._w, boundary, sampling.kind, C.byref(sh) if sh is not None else None, _fp(pts),
                                                len(pts), C.byref(h)))
-        self._nb[boundary] = len(pts)
+        if sampling.kind == DynamicContactSampling.kind:
+            self._nb.pop(boundary, None)  # resampled every step: its size comes from sph_boundary_count
+        else:
+            self._nb[boundary] = len(pts)
         return h.value
 
     def set_collider_state(self, collider, translation=(0.0, 0.0, 0.0), rotation=None, body=BODY_NONE, linvel=(0.0, 0.0, 0.0),
@@ -551,10 +563,18 @@ class LiquidWorld:
     def write_boundary(self, b, positions=None, velocities=None):
         p = _f32(positions, (-1, 3))
         v = _f32(velocities, (-1, 3))
-        self._ck(self._L.sph_boundary_write(self._w, b, _fp(p), _fp(v), self._nb[b]))
+        n = len(p) if p is not None else len(v) if v is not None else self._boundary_count(b)  # the library refuses a wrong length
+        self._ck(self._L.sph_boundary_write(self._w, b, _fp(p), _fp(v), n))
+
+    def _boundary_count(self, b):
+        if b in self._nb:
+            return self._nb[b]
+        n = C.c_size_t()
+        self._ck(self._L.sph_boundary_count(self._w, b, C.byref(n)))
+        return n.value
 
     def read_boundary(self, b):
-        n = self._nb[b]
+        n = self._boundary_count(b)
         vol = np.empty(n, np.float32)
         f = np.zeros((n, 3), np.float32)
         self._ck(self._L.sph_boundary_read_volumes(self._w, b, _fp(vol), n))
