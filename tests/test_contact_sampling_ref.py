@@ -1,10 +1,12 @@
 """CPU checks of DynamicContactSampling: the float32 numpy restatement the GPU tests hold the device to
-(salva_b200.contact_sampling) against an independent float64 restatement of the contract, and the ABI value."""
+(salva_b200.contact_sampling) against the float64 projections and the float64 reference (oracle/ref64_colliders.py) on one
+cuboid, and the ABI value."""
 import os
 import subprocess
 
 import numpy as np
 
+from oracle import ref64_colliders as C64
 from salva_b200 import BODY_DYNAMIC, DynamicContactSampling
 from salva_b200.contact_sampling import BALL, CAPSULE, CUBOID, contact_sample, project_local
 
@@ -87,61 +89,20 @@ def _scene():
     return pos, vel, col
 
 
-def ref64(pos, vel, col, dt, h, r, use_pred=True, lag_dt=None, local_vel=False, err_sign=1.0, margin=True, cut=True, loosen=True):
-    """The contract in float64, one particle at a time, with switches for the mutants."""
-    pos, vel = pos.astype(np.float64), vel.astype(np.float64)
-    e = np.asarray(col["params"], np.float64)
-    t = col["translation"].astype(np.float64)
-    L = 1.5 * h if loosen else 0.0
-    mins, maxs = t - e - L, t + e + L
-    lo, hi = np.floor(mins / h), np.floor(maxs / h)
-    out_p, out_v, samples = pos.copy(), vel.copy(), []
-    d_t = dt if lag_dt is None else lag_dt
-    for i in range(len(pos)):
-        c = np.floor(pos[i] / h)
-        if np.any(c < lo) or np.any(c > hi):
-            continue
-        p = pos[i] + vel[i] * d_t if use_pred else pos[i].copy()
-        if np.any(p < mins) or np.any(p > maxs):
-            continue
-        q, ins = proj64(CUBOID, e, (p - t)[None])
-        q = q[0] + t
-        d = p - q
-        depth = np.linalg.norm(d)
-        if depth > np.finfo(np.float32).eps:
-            n = d / depth
-            if ins[0]:
-                out_p[i] -= n * (depth + (0.1 * r if margin else 0.0))
-                ve = err_sign * n.dot(vel[i])
-                if ve > 0:
-                    out_v[i] -= n * n.dot(vel[i])
-            elif cut and depth > 1.5 * h:
-                continue
-        at = (q - t) if local_vel else q
-        samples.append((q, col["linvel"] + np.cross(col["angvel"], at - col["world_com"])))
-    sp = np.array([s[0] for s in samples]).reshape(-1, 3)
-    sv = np.array([s[1] for s in samples]).reshape(-1, 3)
-    return out_p, out_v, sp, sv
-
-
-def _close(a, b, tol):
-    return a.shape == b.shape and (a.size == 0 or np.abs(a - b).max() <= tol)
-
-
 def test_restatement_matches_float64_and_every_mutant_is_flagged():
+    """One cuboid on a dynamic body against the float64 reference (oracle/ref64_colliders.py); the scenes of several
+    colliders of every shape are in test_ref64_colliders.py."""
     pos, vel, col = _scene()
     dt, h, r = 0.02, 0.1, 0.025
     p32, v32, s32 = contact_sample(pos, vel, [col], dt, h, r)
-    p, v, sp, sv = ref64(pos, vel, col, dt, h, r)
     assert np.any(p32 != pos), "the scene pushes"
-
-    def agrees(res):
-        return _close(p32, res[0], 1e-5) and _close(v32, res[1], 1e-5) and _close(s32[0][0], res[2], 1e-5) and _close(s32[0][1], res[3], 1e-5)
-    assert agrees((p, v, sp, sv))
-    mutants = dict(current_position=dict(use_pred=False), current_dt=dict(lag_dt=0.5 * dt), local_point_velocity=dict(local_vel=True),
-                   vel_err_sign=dict(err_sign=-1.0), no_margin=dict(margin=False), no_cut=dict(cut=False), aabb_not_loosened=dict(loosen=False))
-    for name, kw in mutants.items():
-        assert not agrees(ref64(pos, vel, col, dt, h, r, **kw)), name
+    res = C64.contact64(pos, vel, [col], dt, h, r)
+    worst = C64.check_restatement(res, p32, v32, s32)
+    assert max(worst.values()) <= 1.0, worst
+    assert res.excluded.sum() <= 0.01 * res.candidates
+    for m in ("current_position", "current_dt", "local_point_velocity", "no_vn_gate", "no_margin", "no_cut", "aabb_not_loosened"):
+        res = C64.contact64(pos, vel, [col], dt, h, r, dt_step=0.5 * dt, mutant=m)
+        assert max(C64.check_restatement(res, p32, v32, s32).values()) > 1.0, m
 
 
 def test_points_on_the_surface_are_sampled_without_a_push():
@@ -155,8 +116,9 @@ def test_points_on_the_surface_are_sampled_without_a_push():
     assert np.array_equal(p2, pos) and np.array_equal(v2, vel)
     assert np.array_equal(s[0][0], pos)
     assert branches["on_surface"] == 3 and branches["pushed"] == 0
-    p, v, sp, _ = ref64(pos, vel, col, 0.01, 0.1, 0.025)
-    assert np.abs(p - pos).max() <= 1e-7 and np.abs(sp - pos).max() <= 1e-7
+    res = C64.contact64(pos, vel, [col], 0.01, 0.1, 0.025)
+    assert not res.excluded.any() and res.branches[CUBOID]["on_surface"] == 3
+    assert np.array_equal(res.pos, pos) and np.array_equal(res.samples[0]["q"], pos)
 
 
 def test_sampling_kind_matches_the_c_header(tmp_path):
