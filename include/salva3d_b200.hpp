@@ -160,6 +160,13 @@ struct Isometry3 {
 struct Ball { Real radius; };
 struct Cuboid { Vector3 half_extents; };
 struct Capsule { Real half_height, radius; };  // segment along local y
+// parry HeightField(heights, scale) for ray sampling: nrows x ncols row-major heights, rows along z, columns along x,
+// centred on [-0.5, 0.5] * scale in x and z, cells split along their (x0, z1)-(x1, z0) diagonal (DESIGN.md section 11)
+struct HeightField {
+    uint32_t nrows = 0, ncols = 0;
+    std::vector<Real> heights;
+    Vector3 scale{1, 1, 1};
+};
 // ColliderSampling (fluids_pipeline.rs:64-72): both samplings run on the device
 struct ColliderSampling {
     std::vector<Point3> points;  // StaticSampling: in the collider's local frame
@@ -463,6 +470,18 @@ public:
         return out;
     }
     // liquid_world.rs:246-281 for Ball / Cuboid / Capsule
+    // ray_sampling.rs:9-24 on this world's device (salva3d::sampling below): points in ascending quantised-key order
+    std::vector<Point3> ray_sample(int32_t method, const sph_shape& shape, const sph_heightfield* hf, Real particle_rad) {
+        std::vector<Point3> out(4096);
+        size_t n = 0;
+        for (;;) {
+            check(sph_world_sample_shape(raw_, method, &shape, hf, particle_rad, reinterpret_cast<float*>(out.data()), out.size(), &n));
+            if (n <= out.size()) break;
+            out.resize(n);
+        }
+        out.resize(n);
+        return out;
+    }
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Ball& s) { return shape_query(pos, sph_shape{SPH_SHAPE_BALL, {s.radius}}); }
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Cuboid& s) {
         return shape_query(pos, sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}});
@@ -563,5 +582,34 @@ private:
     std::vector<Fluid> fluids_;
     std::vector<Boundary> boundaries_;
 };
+
+// salva3d::sampling (sampling/ray_sampling.rs:9-24).  The world is the one extra argument: its device runs the sampler.
+namespace sampling {
+namespace detail {
+inline sph_heightfield view(const HeightField& s) {
+    if (s.heights.size() != (size_t)s.nrows * s.ncols) throw std::runtime_error("salva_b200: HeightField heights must hold nrows * ncols values");
+    return sph_heightfield{s.nrows, s.ncols, s.heights.data(), {s.scale.x, s.scale.y, s.scale.z}};
+}
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Ball& s, Real r) { return w.ray_sample(m, sph_shape{SPH_SHAPE_BALL, {s.radius}}, nullptr, r); }
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Cuboid& s, Real r) {
+    return w.ray_sample(m, sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}}, nullptr, r);
+}
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Capsule& s, Real r) {
+    return w.ray_sample(m, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}, nullptr, r);
+}
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const HeightField& s, Real r) {
+    const sph_heightfield hf = view(s);
+    return w.ray_sample(m, sph_shape{SPH_SHAPE_HEIGHTFIELD, {}}, &hf, r);
+}
+}  // namespace detail
+template <class S>
+std::vector<Point3> shape_surface_ray_sample(LiquidWorld& world, const S& shape, Real particle_rad) {
+    return detail::run(world, SPH_SAMPLE_SURFACE, shape, particle_rad);
+}
+template <class S>
+std::vector<Point3> shape_volume_ray_sample(LiquidWorld& world, const S& shape, Real particle_rad) {
+    return detail::run(world, SPH_SAMPLE_VOLUME, shape, particle_rad);
+}
+}  // namespace sampling
 
 }  // namespace salva3d

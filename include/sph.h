@@ -286,6 +286,27 @@ typedef struct {
 sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, const float translation[3], const float rotation_rowmajor[9],
                                         uint32_t* kinds, uint32_t* handles, uint32_t* indices, size_t cap, size_t* n);
 
+/* salva3d::sampling::shape_surface_ray_sample / shape_volume_ray_sample  sampling/ray_sampling.rs:9-24 (the 3-D branch of
+ * :27-231) on the device.  The shape is in its local frame.  SPH_SHAPE_HEIGHTFIELD is parry's HeightField: rows of the
+ * height matrix run along z and columns along x, x and z span [-0.5, 0.5] * scale, heights are multiplied by scale[1], and
+ * cell (row i, column j) is split along its (x0, z1)-(x1, z0) diagonal; its triangles are hit from both sides.  Only the
+ * sampler takes it: sph_world_particles_in_shape and sph_collider_register refuse it.  The world supplies the device, the
+ * stream and the scratch memory; the world's particles are not touched.  Output: *n points (packed xyz) in ascending
+ * order of their quantised (x, y, z) keys, where the reference's order is HashSet order; *n may exceed cap, only cap points are
+ * written.  SPH_ERR_INVALID (nothing written) for a particle_radius that is not finite and positive, a shape parameter
+ * that is negative or not finite, a heightfield with nrows or ncols below 2, a non-finite height or a scale component that
+ * is not finite and positive, and when a quantised coordinate reaches 2^21 (or an axis needs more than 2^21 rays).
+ * SPH_ERR_OOM when the candidate buffers cannot be allocated.  See DESIGN.md section 11. */
+enum { SPH_SHAPE_HEIGHTFIELD = 4 };  /* sph_shape.p unused; the field is the sph_heightfield argument */
+enum { SPH_SAMPLE_SURFACE = 0, SPH_SAMPLE_VOLUME = 1 };
+typedef struct {
+    uint32_t     nrows, ncols;
+    const float* heights;  /* nrows * ncols, row-major */
+    float        scale[3];
+} sph_heightfield;
+sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape* shape, const sph_heightfield* heightfield,
+                                  float particle_radius, float* xyz, size_t cap, size_t* n);
+
 /* LiquidWorld::step  liquid_world.rs:62-158 */
 sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]);
 

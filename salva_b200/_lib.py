@@ -68,6 +68,10 @@ class Shape(C.Structure):
     _fields_ = [("kind", C.c_int32), ("p", C.c_float * 4)]
 
 
+class HeightFieldC(C.Structure):
+    _fields_ = [("nrows", C.c_uint32), ("ncols", C.c_uint32), ("heights", C.POINTER(C.c_float)), ("scale", C.c_float * 3)]
+
+
 class ColliderState(C.Structure):
     _fields_ = [("translation", C.c_float * 3), ("rotation_rowmajor", C.c_float * 9), ("body", C.c_int32),
                 ("linvel", C.c_float * 3), ("angvel", C.c_float * 3), ("world_com", C.c_float * 3)]
@@ -136,6 +140,8 @@ SYMBOLS = {
     "sph_collider_read_impulse": (C.c_int, [_vp, C.c_uint32, _fp, _fp]),
     "sph_collider_unregister": (C.c_int, [_vp, C.c_uint32]),
     "sph_boundary_read": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "sph_world_sample_shape": (C.c_int, [_vp, C.c_int32, C.POINTER(Shape), C.POINTER(HeightFieldC), C.c_float, _fp, C.c_size_t,
+                                         C.POINTER(C.c_size_t)]),
 }
 
 

@@ -25,6 +25,9 @@
 #include "sph_iisph.cuh"
 #include "sph_elasticity.cuh"
 #include "sph_viscosity.cuh"
+#include "sph_sampling.cuh"
+#include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 using namespace sphk;
 
@@ -228,6 +231,10 @@ struct sph_world {
     DBuf<uint32_t> cs_val[2];
     DBuf<char> cs_tmp;
     uint32_t cap_s = 4096, cap_p = 4096;
+    // sph_world_sample_shape: ray tables + heights, per-ray counts / offsets, candidate keys, points, flags
+    DBuf<float> smp_f, smp_xyz;
+    DBuf<unsigned long long> smp_cnt, smp_off, smp_key[2];
+    DBuf<int> smp_flag;
 
     // sorted device state (double buffered for the counting sort)
     int cur = 0, bcur = 0;
@@ -2139,6 +2146,8 @@ void sph_world_destroy(sph_world* w) {
     }
     if (w->h_pinned) cudaFreeHost(w->h_pinned);
     for (auto& c : w->colliders) c.local.release();
+    w->smp_f.release(); w->smp_xyz.release(); w->smp_cnt.release(); w->smp_off.release(); w->smp_flag.release();
+    w->smp_key[0].release(); w->smp_key[1].release();
     w->d_cb.release();
     w->d_imp.release();
     if (w->h_imp) cudaFreeHost(w->h_imp);
@@ -2549,6 +2558,155 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
         maxs[a] = translation[a] + ext[a];
     }
     return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
+}
+
+// salva3d::sampling::shape_{surface,volume}_ray_sample ray_sampling.rs:9-231 (sph_sampling.cuh, DESIGN.md section 11)
+sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape* shape, const sph_heightfield* hf, float particle_radius,
+                                  float* xyz, size_t cap, size_t* n) {
+    if (!w || !shape || !n || (cap && !xyz)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    if (method != SPH_SAMPLE_SURFACE && method != SPH_SAMPLE_VOLUME) return w->fail(SPH_ERR_INVALID, "unknown sampling method %d", method);
+    if (!(std::isfinite(particle_radius) && particle_radius > 0.f))
+        return w->fail(SPH_ERR_INVALID, "particle radius must be finite and > 0 (got %g)", (double)particle_radius);
+    SampleRays P;
+    memset(&P, 0, sizeof P);
+    P.kind = shape->kind;
+    P.volume = method == SPH_SAMPLE_VOLUME;
+    float mins[3], maxs[3];
+    std::vector<float> heights;
+    const int np = shape->kind == SPH_SHAPE_BALL ? 1 : shape->kind == SPH_SHAPE_CUBOID ? 3 : shape->kind == SPH_SHAPE_CAPSULE ? 2 : 0;
+    for (int a = 0; a < np; ++a) {
+        if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f))
+            return w->fail(SPH_ERR_INVALID, "shape parameter %d must be finite and >= 0 (got %g)", a, (double)shape->p[a]);
+        P.p[a] = shape->p[a];
+    }
+    // shape.compute_aabb(&Isometry::identity())
+    switch (shape->kind) {
+        case SPH_SHAPE_BALL:
+            for (int a = 0; a < 3; ++a) { mins[a] = 0.f - P.p[0]; maxs[a] = 0.f + P.p[0]; }
+            break;
+        case SPH_SHAPE_CUBOID:
+            for (int a = 0; a < 3; ++a) { mins[a] = 0.f - P.p[a]; maxs[a] = 0.f + P.p[a]; }
+            break;
+        case SPH_SHAPE_CAPSULE:  // segment a = (0, -hh, 0), b = (0, hh, 0): inf(a, b) - radius, sup(a, b) + radius
+            mins[0] = mins[2] = 0.f - P.p[1];
+            maxs[0] = maxs[2] = 0.f + P.p[1];
+            mins[1] = -P.p[0] - P.p[1];
+            maxs[1] = P.p[0] + P.p[1];
+            break;
+        case SPH_SHAPE_HEIGHTFIELD: {
+            if (!hf || !hf->heights) return w->fail(SPH_ERR_INVALID, "a heightfield shape needs its sph_heightfield");
+            if (hf->nrows < 2 || hf->ncols < 2)
+                return w->fail(SPH_ERR_INVALID, "heightfield needs at least 2 rows and 2 columns (got %u x %u)", hf->nrows, hf->ncols);
+            for (int a = 0; a < 3; ++a)
+                if (!(std::isfinite(hf->scale[a]) && hf->scale[a] > 0.f))
+                    return w->fail(SPH_ERR_INVALID, "heightfield scale[%d] must be finite and > 0 (got %g)", a, (double)hf->scale[a]);
+            const size_t cnt = (size_t)hf->nrows * hf->ncols;
+            heights.assign(hf->heights, hf->heights + cnt);
+            float lo = heights[0], hi = heights[0];
+            for (size_t q = 0; q < cnt; ++q) {
+                if (!std::isfinite(heights[q])) return w->fail(SPH_ERR_INVALID, "heightfield height %zu is not finite", q);
+                lo = std::min(lo, heights[q]);
+                hi = std::max(hi, heights[q]);
+            }
+            P.nrows = (int)hf->nrows;
+            P.ncols = (int)hf->ncols;
+            P.hx = hf->scale[0] * 0.5f;
+            P.hz = hf->scale[2] * 0.5f;
+            P.sy = hf->scale[1];
+            P.dx = hf->scale[0] / (float)(hf->ncols - 1);
+            P.dz = hf->scale[2] / (float)(hf->nrows - 1);
+            mins[0] = -P.hx; maxs[0] = P.hx;
+            mins[1] = lo * P.sy; maxs[1] = hi * P.sy;
+            mins[2] = -P.hz; maxs[2] = P.hz;
+            if (!std::isfinite(mins[1]) || !std::isfinite(maxs[1])) return w->fail(SPH_ERR_INVALID, "heightfield heights overflow once scaled");
+            break;
+        }
+        default:
+            return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
+    }
+    // surface_ray_sample / volume_ray_sample :32-38 and the running sums of the traversal :55-72
+    const float sub = particle_radius * 2.f;
+    P.sub = sub;
+    P.sub10 = sub / 10.f;
+    std::vector<float> tab[3];
+    for (int a = 0; a < 3; ++a) {
+        const float lo = mins[a] - sub, hi = maxs[a] + sub;  // aabb.loosened(sub)
+        P.origin[a] = lo + sub / 2.f;
+        if (!std::isfinite(P.origin[a]) || !std::isfinite(hi)) return w->fail(SPH_ERR_INVALID, "the shape's AABB is not finite once loosened");
+        for (float c = P.origin[a]; c < hi; c += sub) {
+            if (tab[a].size() > SMP_KEY_LIM)
+                return w->fail(SPH_ERR_INVALID, "axis %d needs more than 2^21 rays of spacing %g: quantised coordinates would reach 2^21", a, (double)sub);
+            tab[a].push_back(c);
+        }
+        P.n[a] = (uint32_t)tab[a].size();
+    }
+    unsigned long long R = 0;
+    for (int i = 0; i < 3; ++i) {
+        R += (unsigned long long)P.n[(i + 1) % 3] * P.n[(i + 2) % 3];
+        P.fam_end[i] = R;
+    }
+    if (R >= (1ull << 31) - 1) return w->fail(SPH_ERR_OOM, "%llu rays exceed the sampler's limit of 2^31 - 2", R);
+    CU(cudaSetDevice(w->desc.device));
+    const size_t nt = (size_t)P.n[0] + P.n[1] + P.n[2];
+    CU(w->smp_f.ensure(nt + heights.size()));
+    std::vector<float> up(nt + heights.size());
+    std::copy(tab[0].begin(), tab[0].end(), up.begin());
+    std::copy(tab[1].begin(), tab[1].end(), up.begin() + P.n[0]);
+    std::copy(tab[2].begin(), tab[2].end(), up.begin() + P.n[0] + P.n[1]);
+    std::copy(heights.begin(), heights.end(), up.begin() + nt);
+    CU(cudaMemcpyAsync(w->smp_f.p, up.data(), up.size() * sizeof(float), cudaMemcpyHostToDevice, w->st));
+    P.tab[0] = w->smp_f.p;
+    P.tab[1] = w->smp_f.p + P.n[0];
+    P.tab[2] = w->smp_f.p + P.n[0] + P.n[1];
+    P.hgt = heights.empty() ? nullptr : w->smp_f.p + nt;
+    // count, scan, fill
+    CU(w->smp_cnt.ensure(R + 1));
+    CU(w->smp_off.ensure(R + 1));
+    CU(w->smp_flag.ensure(1));
+    CU(cudaMemsetAsync(w->smp_flag.p, 0, sizeof(int), w->st));
+    CU(cudaMemsetAsync(w->smp_cnt.p + R, 0, sizeof(unsigned long long), w->st));
+    LAUNCH(k_sample_rays<false>, R, 256, P, w->smp_cnt.p, nullptr, nullptr, w->smp_flag.p);
+    CU(cudaGetLastError());
+    size_t tmp = 0;
+    CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp, w->smp_cnt.p, w->smp_off.p, (int)(R + 1), w->st));
+    CU(w->cs_tmp.ensure(tmp));
+    CU(cub::DeviceScan::ExclusiveSum(w->cs_tmp.p, tmp, w->smp_cnt.p, w->smp_off.p, (int)(R + 1), w->st));
+    unsigned long long total = 0;
+    int overflow = 0;
+    CU(cudaMemcpyAsync(&total, w->smp_off.p + R, sizeof total, cudaMemcpyDeviceToHost, w->st));
+    CU(cudaMemcpyAsync(&overflow, w->smp_flag.p, sizeof overflow, cudaMemcpyDeviceToHost, w->st));
+    CU(cudaStreamSynchronize(w->st));
+    if (overflow) return w->fail(SPH_ERR_INVALID, "a quantised coordinate reaches 2^21 (particle radius %g is too small for the shape)", (double)particle_radius);
+    if (total > (1ull << 31) - 1) return w->fail(SPH_ERR_OOM, "%llu candidate keys exceed the sampler's limit of 2^31", total);
+    unsigned long long m = 0;
+    if (total) {
+        CU(w->smp_key[0].ensure(total));
+        CU(w->smp_key[1].ensure(total));
+        LAUNCH(k_sample_rays<true>, R, 256, P, nullptr, w->smp_off.p, w->smp_key[0].p, w->smp_flag.p);
+        CU(cudaGetLastError());
+        // ascending keys, then the unique ones (the reference's HashSet)
+        size_t t1 = 0, t2 = 0;
+        CU(cub::DeviceRadixSort::SortKeys(nullptr, t1, w->smp_key[0].p, w->smp_key[1].p, (int)total, 0, 3 * SMP_KEY_BITS, w->st));
+        CU(cub::DeviceSelect::Unique(nullptr, t2, w->smp_key[1].p, w->smp_key[0].p, w->smp_cnt.p, (int)total, w->st));
+        CU(w->cs_tmp.ensure(std::max(t1, t2)));
+        t1 = t2 = w->cs_tmp.cap;
+        CU(cub::DeviceRadixSort::SortKeys(w->cs_tmp.p, t1, w->smp_key[0].p, w->smp_key[1].p, (int)total, 0, 3 * SMP_KEY_BITS, w->st));
+        CU(cub::DeviceSelect::Unique(w->cs_tmp.p, t2, w->smp_key[1].p, w->smp_key[0].p, w->smp_cnt.p, (int)total, w->st));
+        w->launches += 2;
+        CU(cudaMemcpyAsync(&m, w->smp_cnt.p, sizeof m, cudaMemcpyDeviceToHost, w->st));
+        CU(cudaStreamSynchronize(w->st));
+        const size_t out = std::min<size_t>(m, cap);
+        if (out) {
+            CU(w->smp_xyz.ensure(3 * out));
+            LAUNCH(k_sample_unquantize, out, 256, w->smp_key[0].p, (unsigned long long)out, P.origin[0], P.origin[1], P.origin[2], sub, w->smp_xyz.p);
+            CU(cudaGetLastError());
+            CU(cudaMemcpyAsync(xyz, w->smp_xyz.p, 3 * out * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+            CU(cudaStreamSynchronize(w->st));
+        }
+    }
+    *n = (size_t)m;
+    return SPH_OK;
 }
 
 sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]) {
