@@ -167,17 +167,29 @@ struct HeightField {
     std::vector<Real> heights;
     Vector3 scale{1, 1, 1};
 };
+// the sph_heightfield of a HeightField; it points into s.heights
+inline sph_heightfield heightfield_view(const HeightField& s) {
+    if (s.heights.size() != (size_t)s.nrows * s.ncols) throw std::runtime_error("salva_b200: HeightField heights must hold nrows * ncols values");
+    return sph_heightfield{s.nrows, s.ncols, s.heights.data(), {s.scale.x, s.scale.y, s.scale.z}};
+}
 // ColliderSampling (fluids_pipeline.rs:64-72): both samplings run on the device
 struct ColliderSampling {
     std::vector<Point3> points;  // StaticSampling: in the collider's local frame
     int32_t kind = SPH_SAMPLING_STATIC;
     sph_shape shape{};           // DynamicContactSampling: the collider's shape
+    HeightField heightfield;     // ... when shape.kind == SPH_SHAPE_HEIGHTFIELD
     static ColliderSampling StaticSampling(std::vector<Point3> points) { return ColliderSampling{std::move(points)}; }
     static ColliderSampling DynamicContactSampling(const Ball& s) { return contact(sph_shape{SPH_SHAPE_BALL, {s.radius}}); }
     static ColliderSampling DynamicContactSampling(const Cuboid& s) {
         return contact(sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}});
     }
     static ColliderSampling DynamicContactSampling(const Capsule& s) { return contact(sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}); }
+    // a heightfield only samples, it never pushes fluid (parry's heightfield point query has is_inside always false)
+    static ColliderSampling DynamicContactSampling(const HeightField& s) {
+        ColliderSampling c = contact(sph_shape{SPH_SHAPE_HEIGHTFIELD, {}});
+        c.heightfield = s;
+        return c;
+    }
 
 private:
     static ColliderSampling contact(sph_shape shape) {
@@ -469,7 +481,7 @@ public:
         for (size_t t = 0; t < n; ++t) out[t] = ParticleId{k[t] != 0, h[t], i[t]};
         return out;
     }
-    // liquid_world.rs:246-281 for Ball / Cuboid / Capsule
+    // liquid_world.rs:246-281 for Ball / Cuboid / Capsule / HeightField
     // ray_sampling.rs:9-24 on this world's device (salva3d::sampling below): points in ascending quantised-key order
     std::vector<Point3> ray_sample(int32_t method, const sph_shape& shape, const sph_heightfield* hf, Real particle_rad) {
         std::vector<Point3> out(4096);
@@ -489,13 +501,24 @@ public:
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Capsule& s) {
         return shape_query(pos, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}});
     }
+    std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const HeightField& s) {
+        const sph_heightfield hf = heightfield_view(s);
+        return shape_query(pos, [&](const float* t, uint32_t* k, uint32_t* h, uint32_t* i, size_t cap, size_t* n) {
+            return sph_world_particles_in_heightfield(raw_, &hf, t, pos.rotation, k, h, i, cap, n);
+        });
+    }
     // ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114: the boundary's particles become the collider's samples
     // (DynamicContactSampling: from the next step on, its size changes every step)
     ColliderHandle register_coupling(BoundaryHandle boundary, const ColliderSampling& sampling) {
         Boundary& b = boundaries_.at(boundary);
         uint32_t c = 0;
-        check(sph_collider_register(raw_, b.handle_, sampling.kind, sampling.kind == SPH_SAMPLING_CONTACT ? &sampling.shape : nullptr,
-                                    fp(sampling.points), sampling.points.size(), &c));
+        if (sampling.kind == SPH_SAMPLING_CONTACT && sampling.shape.kind == SPH_SHAPE_HEIGHTFIELD) {
+            const sph_heightfield hf = heightfield_view(sampling.heightfield);
+            check(sph_collider_register_heightfield(raw_, b.handle_, &hf, &c));
+        } else {
+            check(sph_collider_register(raw_, b.handle_, sampling.kind, sampling.kind == SPH_SAMPLING_CONTACT ? &sampling.shape : nullptr,
+                                        fp(sampling.points), sampling.points.size(), &c));
+        }
         b.coupled_ = true;
         pull_results();
         return c;
@@ -554,11 +577,17 @@ private:
         c->manager->transmit_forces(*c->world, dt, inv_dt);
     }
     std::vector<ParticleId> shape_query(const Isometry3& pos, sph_shape shape) {
+        return shape_query(pos, [&](const float* t, uint32_t* k, uint32_t* h, uint32_t* i, size_t cap, size_t* n) {
+            return sph_world_particles_in_shape(raw_, &shape, t, pos.rotation, k, h, i, cap, n);
+        });
+    }
+    template <class Query>
+    std::vector<ParticleId> shape_query(const Isometry3& pos, Query query) {
         const float t[3] = {pos.translation.x, pos.translation.y, pos.translation.z};
         std::vector<uint32_t> k(256), h(256), i(256);
         size_t n = 0;
         for (;;) {
-            check(sph_world_particles_in_shape(raw_, &shape, t, pos.rotation, k.data(), h.data(), i.data(), k.size(), &n));
+            check(query(t, k.data(), h.data(), i.data(), k.size(), &n));
             if (n <= k.size()) break;
             k.resize(n); h.resize(n); i.resize(n);
         }
@@ -586,10 +615,6 @@ private:
 // salva3d::sampling (sampling/ray_sampling.rs:9-24).  The world is the one extra argument: its device runs the sampler.
 namespace sampling {
 namespace detail {
-inline sph_heightfield view(const HeightField& s) {
-    if (s.heights.size() != (size_t)s.nrows * s.ncols) throw std::runtime_error("salva_b200: HeightField heights must hold nrows * ncols values");
-    return sph_heightfield{s.nrows, s.ncols, s.heights.data(), {s.scale.x, s.scale.y, s.scale.z}};
-}
 inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Ball& s, Real r) { return w.ray_sample(m, sph_shape{SPH_SHAPE_BALL, {s.radius}}, nullptr, r); }
 inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Cuboid& s, Real r) {
     return w.ray_sample(m, sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}}, nullptr, r);
@@ -598,7 +623,7 @@ inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Capsule& s, Real
     return w.ray_sample(m, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}, nullptr, r);
 }
 inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const HeightField& s, Real r) {
-    const sph_heightfield hf = view(s);
+    const sph_heightfield hf = heightfield_view(s);
     return w.ray_sample(m, sph_shape{SPH_SHAPE_HEIGHTFIELD, {}}, &hf, r);
 }
 }  // namespace detail

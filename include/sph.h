@@ -289,8 +289,9 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
 /* salva3d::sampling::shape_surface_ray_sample / shape_volume_ray_sample  sampling/ray_sampling.rs:9-24 (the 3-D branch of
  * :27-231) on the device.  The shape is in its local frame.  SPH_SHAPE_HEIGHTFIELD is parry's HeightField: rows of the
  * height matrix run along z and columns along x, x and z span [-0.5, 0.5] * scale, heights are multiplied by scale[1], and
- * cell (row i, column j) is split along its (x0, z1)-(x1, z0) diagonal; its triangles are hit from both sides.  Only the
- * sampler takes it: sph_world_particles_in_shape and sph_collider_register refuse it.  The world supplies the device, the
+ * cell (row i, column j) is split along its (x0, z1)-(x1, z0) diagonal; its triangles are hit from both sides.
+ * sph_world_particles_in_shape and sph_collider_register refuse it (they have no sph_heightfield argument): a heightfield
+ * goes to sph_world_particles_in_heightfield and sph_collider_register_heightfield.  The world supplies the device, the
  * stream and the scratch memory; the world's particles are not touched.  Output: *n points (packed xyz) in ascending
  * order of their quantised (x, y, z) keys, where the reference's order is HashSet order; *n may exceed cap, only cap points are
  * written.  SPH_ERR_INVALID (nothing written) for a particle_radius that is not finite and positive, a shape parameter
@@ -306,6 +307,15 @@ typedef struct {
 } sph_heightfield;
 sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape* shape, const sph_heightfield* heightfield,
                                   float particle_radius, float* xyz, size_t cap, size_t* n);
+/* LiquidWorld::particles_intersecting_shape liquid_world.rs:246-281 for a parry HeightField: the cells of compute_aabb(pos)
+ * (the field's local AABB is not centred: centre R c + t, half extents |R| e), every particle in them with
+ * shape.distance_to_point(pos, p, solid = true) <= particle_radius, where parry's heightfield point query has is_inside always
+ * false: the distance is the unsigned distance to the closest point of the triangulated surface.  Heightfield checks as
+ * sph_world_sample_shape (SPH_ERR_INVALID, nothing written); output and pending-edit rules as sph_world_particles_in_shape.
+ * See DESIGN.md section 10. */
+sph_status sph_world_particles_in_heightfield(sph_world* w, const sph_heightfield* heightfield, const float translation[3],
+                                              const float rotation_rowmajor[9], uint32_t* kinds, uint32_t* handles, uint32_t* indices,
+                                              size_t cap, size_t* n);
 
 /* LiquidWorld::step  liquid_world.rs:62-158 */
 sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]);
@@ -336,7 +346,9 @@ enum { SPH_SAMPLING_STATIC = 0,    /* ColliderSampling::StaticSampling(points)  
    pushed out along the projection normal by depth + 0.1 particle_radius and loses its velocity into the shape; the projection
    becomes a boundary particle with the body's velocity at that WORLD point, unless p lies more than 1.5 h outside.  Colliders
    run in slot order; the boundary holds its samples ordered by the sampled particle's fluid slot, then index.  A ball's
-   centre yields no sample; a point on a capsule's axis projects along local +x.  See DESIGN.md section 10. */
+   centre yields no sample; a point on a capsule's axis projects along local +x.  A heightfield (parry's point query has
+   is_inside always false, point_heightfield.rs) never pushes: it only samples its closest surface points.  See DESIGN.md
+   section 10. */
 enum { SPH_BODY_NONE = 0,     /* collider.parent() == None: velocity 0, boundary.forces left as it is (fluids_pipeline.rs:163-171),
                                  no impulse (transmit_forces needs the parent body, :273-276) */
        SPH_BODY_FIXED = 1,    /* !body.is_dynamic(): boundary.forces = None, no impulse */
@@ -357,6 +369,14 @@ typedef struct {
  * is the identity pose with SPH_BODY_NONE.  Handles are slot | generation << 16. */
 sph_status sph_collider_register(sph_world* w, uint32_t boundary, int32_t sampling, const sph_shape* shape, const float* local_points_xyz,
                                  size_t n_points, uint32_t* collider);
+/* register_coupling(boundary, collider, ColliderSampling::DynamicContactSampling) fluids_pipeline.rs:98-114, 192-255 for a
+ * collider whose shape is a parry HeightField (StaticSampling needs no shape: use sph_collider_register).  The heights are
+ * copied into device memory owned by the collider, so the caller's buffer may be freed; sph_collider_unregister and
+ * sph_world_destroy free it.  The heightfield never pushes fluid (is_inside is always false in parry's heightfield point
+ * query): each candidate's closest surface point becomes a sample unless it lies more than 1.5 h away.  All other rules of
+ * sph_collider_register apply.  Heightfield checks as sph_world_sample_shape (SPH_ERR_INVALID, nothing written);
+ * SPH_ERR_OOM when the heights cannot be allocated. */
+sph_status sph_collider_register_heightfield(sph_world* w, uint32_t boundary, const sph_heightfield* heightfield, uint32_t* collider);
 /* The collider's pose and body for the next steps (the reference reads collider.position() and the parent body each
  * update_boundaries, fluids_pipeline.rs:159-186).  A StaticSampling collider whose state is bit-equal to the one of its
  * last step leaves its boundary unchanged, so the boundary's sort and volumes are reused as for a static boundary. */

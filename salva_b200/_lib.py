@@ -142,6 +142,9 @@ SYMBOLS = {
     "sph_boundary_read": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
     "sph_world_sample_shape": (C.c_int, [_vp, C.c_int32, C.POINTER(Shape), C.POINTER(HeightFieldC), C.c_float, _fp, C.c_size_t,
                                          C.POINTER(C.c_size_t)]),
+    "sph_world_particles_in_heightfield": (C.c_int, [_vp, C.POINTER(HeightFieldC), _fp, _fp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
+                                                     C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(C.c_size_t)]),
+    "sph_collider_register_heightfield": (C.c_int, [_vp, C.c_uint32, C.POINTER(HeightFieldC), C.POINTER(C.c_uint32)]),
 }
 
 

@@ -11,15 +11,41 @@ from .liquid_world import BODY_NONE, CouplingManager
 
 F32 = np.float32
 EPS = F32(np.finfo(np.float32).eps)  # Unit::try_new_and_get(dpt, f32::EPSILON)
-BALL, CUBOID, CAPSULE = 1, 2, 3
+BALL, CUBOID, CAPSULE, HEIGHTFIELD = 1, 2, 3, 4
+NO_TRI = 2 ** 32 - 1  # no triangle yet (the device's UINT32_MAX)
 
 
 def _dot(a0, a1, a2, b0, b1, b2):
     return (a0 * b0 + a1 * b1) + a2 * b2
 
 
-def posed_aabb(kind, params, rotation, translation):
-    """The posed shape's AABB (shape.compute_aabb(pos)): translation -/+ the half extents sph_world_particles_in_shape uses."""
+def hf_grid(heights, scale):
+    """The host constants of a heightfield (sph_engine.cu hf_check): half extents, cell sizes, height scale, the scaled
+    height range."""
+    H = np.ascontiguousarray(heights, F32)
+    sx, sy, sz = (F32(x) for x in scale)
+    nr, nc = H.shape
+    g = dict(H=H, nrows=nr, ncols=nc, hx=sx * F32(0.5), hz=sz * F32(0.5), sy=sy, dx=sx / F32(nc - 1), dz=sz / F32(nr - 1))
+    g["dmin"] = min(g["dx"], g["dz"])
+    g["ylo"], g["yhi"] = H.min() * sy, H.max() * sy
+    return g
+
+
+def hf_margin(g, cap):
+    """The search margin M = 2^-10 (sx/2 + sz/2 + max |y| + cap) of hf_set_cap."""
+    return (((g["hx"] + g["hz"]) + max(abs(g["ylo"]), abs(g["yhi"]))) + F32(cap)) * F32(2.0 ** -10)
+
+
+def posed_aabb(kind, params, rotation, translation, hf=None):
+    """The posed shape's AABB (shape.compute_aabb(pos)): translation -/+ the half extents sph_world_particles_in_shape uses;
+    for a heightfield (hf: hf_grid) Aabb::transform_by of its local box, centre R c + t and half extents |R| e."""
+    if kind == HEIGHTFIELD:
+        R = np.asarray(rotation, F32).reshape(3, 3)
+        t = np.asarray(translation, F32)
+        cy, ey = (hf["ylo"] + hf["yhi"]) * F32(0.5), (hf["yhi"] - hf["ylo"]) * F32(0.5)
+        ext = np.array([(abs(R[a, 0]) * hf["hx"] + abs(R[a, 1]) * ey) + abs(R[a, 2]) * hf["hz"] for a in range(3)], F32)
+        c = np.array([R[a, 1] * cy + t[a] for a in range(3)], F32)
+        return c - ext, c + ext
     R = np.asarray(rotation, F32).reshape(3, 3)
     p = np.zeros(4, F32)
     p[:len(params)] = np.asarray(params, F32)
@@ -33,6 +59,108 @@ def posed_aabb(kind, params, rotation, translation):
         else:
             ext[a] = abs(R[a, 1]) * p[0] + p[1]
     return t - ext, t + ext
+
+
+def _grid(j, last, half, d):
+    """smp_grid: vertex coordinate j of a grid of `last` cells of size d from -half (the last one exactly +half)."""
+    return np.where(j == last, half, -half + j.astype(F32) * d).astype(F32)
+
+
+def _cell(c, half, d, cells):
+    """smp_cell: the cell of coordinate c, clamped to the grid."""
+    t = (c + half) / d
+    return np.clip(np.floor(t), 0, cells - 1).astype(np.int64)
+
+
+def _dot3(a, b):
+    return _dot(a[..., 0], a[..., 1], a[..., 2], b[..., 0], b[..., 1], b[..., 2])
+
+
+def hf_tri(p, a, b, c):
+    """hf_tri: the closest point of the closed triangles (a, b, c) to p (Ericson's regions, the device's float32
+    operations) and its squared distance; arrays (..., 3)."""
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        ab, ac, ap, bp, cp = b - a, c - a, p - a, p - b, p - c
+        d1, d2, d3, d4, d5, d6 = _dot3(ab, ap), _dot3(ac, ap), _dot3(ab, bp), _dot3(ac, bp), _dot3(ab, cp), _dot3(ac, cp)
+        vc, vb, va = d1 * d4 - d3 * d2, d5 * d2 - d1 * d6, d3 * d6 - d5 * d4
+        e43, e56 = d4 - d3, d5 - d6
+        regions = [(d1 <= 0) & (d2 <= 0), (d3 >= 0) & (d4 <= d3), (vc <= 0) & (d1 >= 0) & (d3 <= 0), (d6 >= 0) & (d5 <= d6),
+                   (vb <= 0) & (d2 >= 0) & (d6 <= 0), (va <= 0) & (e43 >= 0) & (e56 >= 0)]
+        den = F32(1) / ((va + vb) + vc)
+        face = (a + ab * (vb * den)[..., None]) + ac * (vc * den)[..., None]
+        q = np.select([m[..., None] for m in regions],
+                      [a, b, a + (d1 / (d1 - d3))[..., None] * ab, c, a + (d2 / (d2 - d6))[..., None] * ac,
+                       b + (e43 / (e43 + e56))[..., None] * (c - b)], face).astype(F32)
+        e = p - q
+        return q, _dot3(e, e)
+
+
+def _ring_gap(r, g, margin):
+    """The least horizontal distance of ring r's cells, less the margin: (r - 1) dmin - M."""
+    return F32(r - 1) * g["dmin"] - margin
+
+
+def _beats(d, t, best, bidx):
+    """(d, t) before (best, bidx) in the order (squared distance, parry triangle index)."""
+    return (d < best) | ((d == best) & (t < bidx))
+
+
+def hf_project_local(g, l, cap):
+    """hf_closest for local points l (n, 3) float32: the ring search with the device's stop rule (cap: h + prediction for
+    contact sampling, particle_radius for queries).  Returns (q (n, 3), squared distance (n,), found (n,))."""
+    l = np.asarray(l, F32)
+    n = len(l)
+    ni, nj = g["nrows"] - 1, g["ncols"] - 1
+    ci, cj = _cell(l[:, 2], g["hz"], g["dz"], ni), _cell(l[:, 0], g["hx"], g["dx"], nj)
+    rmax = np.maximum(np.maximum(ci, ni - 1 - ci), np.maximum(cj, nj - 1 - cj))
+    cap2, margin = F32(cap) * F32(cap), hf_margin(g, cap)
+    best = np.full(n, np.inf, F32)
+    bidx = np.full(n, NO_TRI, np.int64)
+    q = np.zeros((n, 3), F32)
+    active = np.ones(n, bool)
+    H, sy = g["H"], g["sy"]
+    for r in range(int(rmax.max(initial=0)) + 1):
+        active &= r <= rmax
+        gap = _ring_gap(r, g, margin)
+        if gap > 0:
+            active &= ~(gap * gap > np.minimum(best, cap2))
+        idx = np.nonzero(active)[0]
+        if not len(idx):
+            break
+        if r == 0:
+            di, dj = np.zeros(1, np.int64), np.zeros(1, np.int64)
+        else:
+            k = np.arange(-r, r + 1)
+            m = np.arange(-r + 1, r)
+            di = np.concatenate([np.full(2 * r + 1, -r), np.full(2 * r + 1, r), m, m])
+            dj = np.concatenate([k, k, np.full(2 * r - 1, -r), np.full(2 * r - 1, r)])
+        I, J = ci[idx, None] + di[None, :], cj[idx, None] + dj[None, :]
+        ok = (I >= 0) & (I < ni) & (J >= 0) & (J < nj)
+        I, J = np.clip(I, 0, ni - 1), np.clip(J, 0, nj - 1)
+        x0, x1 = _grid(J, nj, g["hx"], g["dx"]), _grid(J + 1, nj, g["hx"], g["dx"])
+        z0, z1 = _grid(I, ni, g["hz"], g["dz"]), _grid(I + 1, ni, g["hz"], g["dz"])
+        p00 = np.stack([x0, H[I, J] * sy, z0], -1)
+        p10 = np.stack([x1, H[I, J + 1] * sy, z0], -1)
+        p01 = np.stack([x0, H[I + 1, J] * sy, z1], -1)
+        p11 = np.stack([x1, H[I + 1, J + 1] * sy, z1], -1)
+        p = l[idx, None, :]
+        qa, da = hf_tri(p, p00, p10, p01)
+        qb, db = hf_tri(p, p10, p11, p01)
+        base = 2 * (J * ni + I)
+        D = np.concatenate([da, db], 1)
+        T = np.concatenate([base, base + 1], 1)
+        Q = np.concatenate([qa, qb], 1)
+        bad = ~np.concatenate([ok, ok], 1) | np.isnan(D)  # NaN never wins on the device
+        D = np.where(bad, F32(np.inf), D)
+        T = np.where(bad, 2 ** 40, T)
+        dm = D.min(axis=1)
+        win = np.where(D == dm[:, None], T, 2 ** 41).argmin(axis=1)
+        rows = np.arange(len(idx))
+        rd, rt = D[rows, win], T[rows, win]
+        take = _beats(rd, rt, best[idx], bidx[idx])
+        best[idx[take]], bidx[idx[take]] = rd[take], rt[take]
+        q[idx[take]] = Q[rows, win][take]
+    return q, best, bidx != NO_TRI
 
 
 def project_local(kind, params, l):
@@ -93,8 +221,9 @@ def velocity_at(points, body, linvel, angvel, world_com):
 
 def contact_sample(pos, vel, colliders, dt, h, particle_radius, branches=None):
     """One update_boundaries over every fluid particle (pos, vel: (n, 3) float32 in global original order) and the contact
-    colliders in slot order, each a dict(kind, params, rotation, translation, body, linvel, angvel, world_com); the
-    pose defaults to the identity, the rest to a parentless collider.  `dt` is
+    colliders in slot order, each a dict(kind, params, rotation, translation, body, linvel, angvel, world_com), a heightfield
+    (kind 4) with heights (nrows, ncols) and scale instead of params; the pose defaults to the identity, the rest to a
+    parentless collider.  `dt` is
     the lagging timestep.  Returns (pos, vel, samples) with the pushes applied and samples[k] = (positions, velocities)
     of collider k in original particle order.  `branches` (a dict) counts, over all colliders, the candidates that took each
     branch of the rule: pushed, shell (outside, kept), beyond (outside by more than h + prediction), on_surface (|dpt| <=
@@ -111,7 +240,8 @@ def contact_sample(pos, vel, colliders, dt, h, particle_radius, branches=None):
     for col in colliders:
         R = np.asarray(col.get("rotation", np.eye(3)), F32).reshape(3, 3)  # the identity pose by default, as sph_collider_register
         t = np.asarray(col.get("translation", (0.0, 0.0, 0.0)), F32)
-        mins, maxs = posed_aabb(col["kind"], col["params"], R, t)
+        hf = hf_grid(col["heights"], col["scale"]) if col["kind"] == HEIGHTFIELD else None
+        mins, maxs = posed_aabb(col["kind"], col.get("params", ()), R, t, hf)
         mins, maxs = mins - cut, maxs + cut
         lo, hi = np.floor(mins / h), np.floor(maxs / h)
         in_box = np.all((cells >= lo) & (cells <= hi), axis=1)
@@ -127,7 +257,11 @@ def contact_sample(pos, vel, colliders, dt, h, particle_radius, branches=None):
         idx, p, v, pr = idx[keep], p[keep], v[keep], pr[keep]
         w = pr - t
         l = np.stack([_dot(R[0, a], R[1, a], R[2, a], w[:, 0], w[:, 1], w[:, 2]) for a in range(3)], axis=1).astype(F32)
-        q, inside, valid = project_local(col["kind"], col["params"], l)
+        if hf is not None:  # is_inside is always false: no push
+            q, _, valid = hf_project_local(hf, l, cut)
+            inside = np.zeros(len(l), bool)
+        else:
+            q, inside, valid = project_local(col["kind"], col["params"], l)
         idx, p, v, pr, q, inside = idx[valid], p[valid], v[valid], pr[valid], q[valid], inside[valid]
         qw = np.stack([_dot(R[a, 0], R[a, 1], R[a, 2], q[:, 0], q[:, 1], q[:, 2]) + t[a] for a in range(3)], axis=1).astype(F32)
         d = pr - qw

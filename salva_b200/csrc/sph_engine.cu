@@ -110,6 +110,9 @@ struct ColliderRec {
     sph_shape shape{};              // SPH_SAMPLING_CONTACT: the collider's shape
     size_t n = 0;                   // StaticSampling: sample points
     DBuf<float4> local;             // the points in the collider's frame
+    DBuf<float> hgt;                // a heightfield shape (shape.kind == SPH_SHAPE_HEIGHTFIELD): its heights, owned by the record
+    HfGrid hf{};                    // ... its grid constants (hf.hgt = hgt.p)
+    float hf_ylo = 0.f, hf_yhi = 0.f;  // ... and its scaled height range: the local AABB's y extent
     sph_collider_state state{};     // for the next step
     sph_collider_state applied{};   // what the boundary's particles on the device were posed with
     bool applied_valid = false;
@@ -225,6 +228,7 @@ struct sph_world {
     float* h_imp = nullptr;  // pinned copy, read back with the step's final read-back
     // DynamicContactSampling (colliders_contact): collider table, result ints, growing sample / push records, sort buffers
     DBuf<ContactCollider> d_ccol;
+    DBuf<HfGrid> d_chf;  // per contact collider: a heightfield's grid (ContactParams::hf)
     DBuf<int> d_cres;
     DBuf<float4> cs_s4, cs_p4;
     DBuf<unsigned long long> cs_key[2];
@@ -776,6 +780,57 @@ void posed_aabb_ext(const sph_shape& s, const float R[9], float ext[3]) {
     }
 }
 
+// The heightfield checks of sph_world_sample_shape, shared by every entry point that takes one: 2 x 2 or more, finite
+// heights, a finite positive scale.  Fills the grid constants and the scaled height range [*ylo, *yhi].
+sph_status hf_check(sph_world* w, const sph_heightfield* hf, std::vector<float>& heights, HfGrid& g, float* ylo, float* yhi) {
+    if (!hf || !hf->heights) return w->fail(SPH_ERR_INVALID, "a heightfield shape needs its sph_heightfield");
+    if (hf->nrows < 2 || hf->ncols < 2)
+        return w->fail(SPH_ERR_INVALID, "heightfield needs at least 2 rows and 2 columns (got %u x %u)", hf->nrows, hf->ncols);
+    for (int a = 0; a < 3; ++a)
+        if (!(std::isfinite(hf->scale[a]) && hf->scale[a] > 0.f))
+            return w->fail(SPH_ERR_INVALID, "heightfield scale[%d] must be finite and > 0 (got %g)", a, (double)hf->scale[a]);
+    const size_t cnt = (size_t)hf->nrows * hf->ncols;
+    heights.assign(hf->heights, hf->heights + cnt);
+    float lo = heights[0], hi = heights[0];
+    for (size_t q = 0; q < cnt; ++q) {
+        if (!std::isfinite(heights[q])) return w->fail(SPH_ERR_INVALID, "heightfield height %zu is not finite", q);
+        lo = std::min(lo, heights[q]);
+        hi = std::max(hi, heights[q]);
+    }
+    memset(&g, 0, sizeof g);
+    g.nrows = (int)hf->nrows;
+    g.ncols = (int)hf->ncols;
+    g.hx = hf->scale[0] * 0.5f;
+    g.hz = hf->scale[2] * 0.5f;
+    g.sy = hf->scale[1];
+    g.dx = hf->scale[0] / (float)(hf->ncols - 1);
+    g.dz = hf->scale[2] / (float)(hf->nrows - 1);
+    g.dmin = std::min(g.dx, g.dz);
+    *ylo = lo * g.sy;
+    *yhi = hi * g.sy;
+    if (!std::isfinite(*ylo) || !std::isfinite(*yhi)) return w->fail(SPH_ERR_INVALID, "heightfield heights overflow once scaled");
+    return SPH_OK;
+}
+
+// The search cap of hf_closest and its margin M = 2^-10 (sx/2 + sz/2 + max |y| + cap): far above the float32 error of any
+// distance the routine computes for a point within the cap (DESIGN.md section 10).
+void hf_set_cap(HfGrid& g, float ylo, float yhi, float cap) {
+    g.cap2 = cap * cap;
+    g.margin = (((g.hx + g.hz) + std::max(std::fabs(ylo), std::fabs(yhi))) + cap) * 0.0009765625f;
+}
+
+// compute_aabb(pos) of a heightfield: Aabb::transform_by, centre R c + t and half extents |R| e, where the local box
+// [-sx/2, ylo, -sz/2]-[sx/2, yhi, sz/2] is centred on c = (0, (ylo + yhi) / 2, 0), not on the origin.
+void hf_posed_aabb(const HfGrid& g, float ylo, float yhi, const float R[9], const float t[3], float mins[3], float maxs[3]) {
+    const float cy = (ylo + yhi) * 0.5f, ey = (yhi - ylo) * 0.5f;
+    for (int a = 0; a < 3; ++a) {
+        const float ext = (std::fabs(R[3 * a]) * g.hx + std::fabs(R[3 * a + 1]) * ey) + std::fabs(R[3 * a + 2]) * g.hz;
+        const float c = R[3 * a + 1] * cy + t[a];
+        mins[a] = c - ext;
+        maxs[a] = c + ext;
+    }
+}
+
 sph_status phase_grid(sph_world* w);
 
 bool any_contact(const sph_world* w) {
@@ -798,8 +853,10 @@ sph_status colliders_contact(sph_world* w) {
     const int go[3] = {hc.ox / xs, hc.oy / xs, hc.oz}, gn[3] = {hc.nx / xs, hc.ny / xs, hc.nz};
     const float h = w->h, prediction = h * 0.5f, cut = h + prediction, margin = w->desc.particle_radius * 0.1f;
     std::vector<ContactCollider> cc;
+    std::vector<HfGrid> chf;
     unsigned long long skip = 0;
     size_t bins = 0;
+    bool any_hf = false;
     for (size_t k = 0; k < w->colliders.size(); ++k) {
         const ColliderRec& c = w->colliders[k];
         if (!c.alive || c.sampling != SPH_SAMPLING_CONTACT) continue;
@@ -817,12 +874,24 @@ sph_status colliders_contact(sph_world* w) {
         memcpy(K.angvel, c.state.angvel, sizeof K.angvel);
         memcpy(K.com, c.state.world_com, sizeof K.com);
         K.moving = c.state.body != SPH_BODY_NONE;
-        float ext[3];
-        posed_aabb_ext(c.shape, K.rot, ext);
+        float lo[3], hi[3];  // compute_aabb(pos)
+        chf.push_back(c.hf);
+        if (c.shape.kind == SPH_SHAPE_HEIGHTFIELD) {
+            hf_set_cap(chf.back(), c.hf_ylo, c.hf_yhi, cut);
+            hf_posed_aabb(c.hf, c.hf_ylo, c.hf_yhi, K.rot, K.t, lo, hi);
+            any_hf = true;
+        } else {
+            float ext[3];
+            posed_aabb_ext(c.shape, K.rot, ext);
+            for (int a = 0; a < 3; ++a) {
+                lo[a] = K.t[a] - ext[a];
+                hi[a] = K.t[a] + ext[a];
+            }
+        }
         size_t nbin = 1;
         for (int a = 0; a < 3; ++a) {
-            K.mins[a] = (K.t[a] - ext[a]) - cut;  // compute_aabb(pos).loosened(h + prediction)
-            K.maxs[a] = (K.t[a] + ext[a]) + cut;
+            K.mins[a] = lo[a] - cut;  // .loosened(h + prediction)
+            K.maxs[a] = hi[a] + cut;
             // hgrid.rs:41-52 keys; clamped where no particle can be (k_bounds refuses |cell| >= 1e9)
             const float flo = std::fmin(std::fmax(std::floor(K.mins[a] / h), -1.5e9f), 1.5e9f);
             const float fhi = std::fmin(std::fmax(std::floor(K.maxs[a] / h), -1.5e9f), 1.5e9f);
@@ -842,6 +911,10 @@ sph_status colliders_contact(sph_world* w) {
     const int nc = (int)cc.size();
     CU(w->d_ccol.ensure(nc));
     CU(cudaMemcpyAsync(w->d_ccol.p, cc.data(), nc * sizeof(ContactCollider), cudaMemcpyHostToDevice, w->st));
+    if (any_hf) {
+        CU(w->d_chf.ensure(nc));
+        CU(cudaMemcpyAsync(w->d_chf.p, chf.data(), nc * sizeof(HfGrid), cudaMemcpyHostToDevice, w->st));
+    }
     constexpr int NRES = CS_PER_COLLIDER + MAX_BOUNDARIES;
     int init[NRES] = {};
     for (int base : {CS_FLUID_BOUNDS, CS_BOUND_BOUNDS})
@@ -859,9 +932,13 @@ sph_status colliders_contact(sph_world* w) {
         CU(w->cs_p4.ensure(2 * (size_t)w->cap_p));
         CU(cudaMemcpyAsync(w->d_cres.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
         if (N && bins) {
-            ContactParams P{w->d_ccol.p, nc, (uint32_t)bins, w->dt, cut, margin, w->cap_s, w->cap_p};
-            LAUNCH(k_contact_sample, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p, w->cs_key[0].p,
-                   w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
+            ContactParams P{w->d_ccol.p, nc, (uint32_t)bins, w->dt, cut, margin, w->cap_s, w->cap_p, any_hf ? w->d_chf.p : nullptr};
+            if (any_hf)
+                LAUNCH(k_contact_sample<true>, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p,
+                       w->cs_key[0].p, w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
+            else
+                LAUNCH(k_contact_sample<false>, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p,
+                       w->cs_key[0].p, w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
             k_contact_apply<<<std::min<uint32_t>(cdiv(w->cap_p, 256), 264), 256, 0, w->st>>>(w->cs_p4.p, w->d_cres.p, w->cap_s, w->cap_p, w->pos[c].p,
                                                                                          w->vel[c].p);
             w->launches++;
@@ -2145,11 +2222,15 @@ void sph_world_destroy(sph_world* w) {
         cudaEventDestroy(s.b);
     }
     if (w->h_pinned) cudaFreeHost(w->h_pinned);
-    for (auto& c : w->colliders) c.local.release();
+    for (auto& c : w->colliders) {
+        c.local.release();
+        c.hgt.release();
+    }
     w->smp_f.release(); w->smp_xyz.release(); w->smp_cnt.release(); w->smp_off.release(); w->smp_flag.release();
     w->smp_key[0].release(); w->smp_key[1].release();
     w->d_cb.release();
     w->d_imp.release();
+    w->d_chf.release();
     if (w->h_imp) cudaFreeHost(w->h_imp);
     w->d_ticket.release();
     w->d_nb.release();
@@ -2471,8 +2552,12 @@ static sph_status run_query(sph_world* w, AabbQuery q, const float mins[3], cons
     for (int attempt = 0; attempt < 2; ++attempt) {
         CU(w->q_out.ensure(2 * qcap));
         CU(cudaMemsetAsync(w->q_count.p, 0, sizeof(uint32_t), w->st));
-        LAUNCH(k_aabb_query, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr, w->bstart.p,
-               w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
+        if (q.kind == SPH_SHAPE_HEIGHTFIELD)
+            LAUNCH(k_aabb_query<true>, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr,
+                   w->bstart.p, w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
+        else
+            LAUNCH(k_aabb_query<false>, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr,
+                   w->bstart.p, w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
         CU(cudaMemcpyAsync(&found, w->q_count.p, sizeof found, cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
         if (found <= qcap) break;
@@ -2560,6 +2645,37 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
     return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
 }
 
+// particles_intersecting_shape liquid_world.rs:246-281 for a parry HeightField: the cells of compute_aabb(pos) (centre
+// R c + t), every particle in them whose distance_to_point(pos, p, solid) (is_inside is always false: the unsigned distance
+// to the closest point) is <= particle_radius.  The heights live in the sampler's scratch for the call.
+sph_status sph_world_particles_in_heightfield(sph_world* w, const sph_heightfield* hf, const float translation[3], const float rotation_rowmajor[9],
+                                              uint32_t* kinds, uint32_t* handles, uint32_t* indices, size_t cap, size_t* n) {
+    if (!w || !translation || !n || (cap && (!kinds || !handles || !indices))) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    AabbQuery q;
+    memset(&q, 0, sizeof q);
+    static const float ident[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
+    const float* R = rotation_rowmajor ? rotation_rowmajor : ident;
+    for (int k = 0; k < 9; ++k) q.rot[k] = R[k];
+    for (int a = 0; a < 3; ++a) q.t[a] = translation[a];
+    std::vector<float> heights;
+    float ylo, yhi;
+    TRY(hf_check(w, hf, heights, q.hf, &ylo, &yhi));
+    q.kind = SPH_SHAPE_HEIGHTFIELD;
+    hf_set_cap(q.hf, ylo, yhi, w->desc.particle_radius);
+    float mins[3], maxs[3];
+    hf_posed_aabb(q.hf, ylo, yhi, R, translation, mins, maxs);
+    *n = 0;
+    if (!w->grid_ready) return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);  // empty, or refused while edits are pending
+    TRY(enter(w));
+    CU(w->smp_f.ensure(heights.size()));
+    CU(cudaMemcpyAsync(w->smp_f.p, heights.data(), heights.size() * sizeof(float), cudaMemcpyHostToDevice, w->st));
+    q.hf.hgt = w->smp_f.p;
+    const sph_status st = run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
+    CU(cudaStreamSynchronize(w->st));  // the upload has left `heights` on every path
+    return st;
+}
+
 // salva3d::sampling::shape_{surface,volume}_ray_sample ray_sampling.rs:9-231 (sph_sampling.cuh, DESIGN.md section 11)
 sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape* shape, const sph_heightfield* hf, float particle_radius,
                                   float* xyz, size_t cap, size_t* n) {
@@ -2595,31 +2711,17 @@ sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape*
             maxs[1] = P.p[0] + P.p[1];
             break;
         case SPH_SHAPE_HEIGHTFIELD: {
-            if (!hf || !hf->heights) return w->fail(SPH_ERR_INVALID, "a heightfield shape needs its sph_heightfield");
-            if (hf->nrows < 2 || hf->ncols < 2)
-                return w->fail(SPH_ERR_INVALID, "heightfield needs at least 2 rows and 2 columns (got %u x %u)", hf->nrows, hf->ncols);
-            for (int a = 0; a < 3; ++a)
-                if (!(std::isfinite(hf->scale[a]) && hf->scale[a] > 0.f))
-                    return w->fail(SPH_ERR_INVALID, "heightfield scale[%d] must be finite and > 0 (got %g)", a, (double)hf->scale[a]);
-            const size_t cnt = (size_t)hf->nrows * hf->ncols;
-            heights.assign(hf->heights, hf->heights + cnt);
-            float lo = heights[0], hi = heights[0];
-            for (size_t q = 0; q < cnt; ++q) {
-                if (!std::isfinite(heights[q])) return w->fail(SPH_ERR_INVALID, "heightfield height %zu is not finite", q);
-                lo = std::min(lo, heights[q]);
-                hi = std::max(hi, heights[q]);
-            }
-            P.nrows = (int)hf->nrows;
-            P.ncols = (int)hf->ncols;
-            P.hx = hf->scale[0] * 0.5f;
-            P.hz = hf->scale[2] * 0.5f;
-            P.sy = hf->scale[1];
-            P.dx = hf->scale[0] / (float)(hf->ncols - 1);
-            P.dz = hf->scale[2] / (float)(hf->nrows - 1);
+            HfGrid g;
+            TRY(hf_check(w, hf, heights, g, &mins[1], &maxs[1]));
+            P.nrows = g.nrows;
+            P.ncols = g.ncols;
+            P.hx = g.hx;
+            P.hz = g.hz;
+            P.sy = g.sy;
+            P.dx = g.dx;
+            P.dz = g.dz;
             mins[0] = -P.hx; maxs[0] = P.hx;
-            mins[1] = lo * P.sy; maxs[1] = hi * P.sy;
             mins[2] = -P.hz; maxs[2] = P.hz;
-            if (!std::isfinite(mins[1]) || !std::isfinite(maxs[1])) return w->fail(SPH_ERR_INVALID, "heightfield heights overflow once scaled");
             break;
         }
         default:
@@ -3033,15 +3135,29 @@ sph_status sph_boundary_read(sph_world* w, uint32_t boundary_h, float* pos, floa
     return SPH_OK;
 }
 
+// The rules every registration shares: not from a callback, not in a slab world, a live boundary not coupled yet.
+static sph_status collider_check_boundary(sph_world* w, uint32_t boundary_h) {
+    if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "colliders cannot be registered from inside a coupling callback");
+    if (w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
+    BOUNDARY_OR_FAIL(boundary, boundary_h)
+    if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "boundary %u is already coupled to a collider", (unsigned)boundary_h);
+    return SPH_OK;
+}
+
+// The first free collider slot, or MAX_BOUNDARIES when all are taken.
+static size_t collider_free_slot(const sph_world* w) {
+    for (size_t k = 0; k < w->colliders.size(); ++k)
+        if (!w->colliders[k].alive) return k;
+    return w->colliders.size();
+}
+
 // ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114
 sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t sampling, const sph_shape* shape, const float* pts, size_t n,
                                  uint32_t* collider) {
     if (!w || !collider || (n && !pts)) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
-    if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "colliders cannot be registered from inside a coupling callback");
-    if (w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
+    TRY(collider_check_boundary(w, boundary_h));
     BOUNDARY_OR_FAIL(boundary, boundary_h)
-    if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "boundary %u is already coupled to a collider", (unsigned)boundary_h);
     if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE)) return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
     if (sampling != SPH_SAMPLING_STATIC && sampling != SPH_SAMPLING_CONTACT) return w->fail(SPH_ERR_INVALID, "unknown sampling %d", sampling);
     if (sampling == SPH_SAMPLING_CONTACT) {
@@ -3054,9 +3170,7 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     if (n >= (size_t)UINT32_MAX) return w->fail(SPH_ERR_INVALID, "too many sample points");
     for (size_t k = 0; k < 3 * n; ++k)
         if (!std::isfinite(pts[k])) return w->fail(SPH_ERR_INVALID, "non-finite sample point");
-    size_t slot = w->colliders.size();
-    for (size_t k = 0; k < w->colliders.size(); ++k)
-        if (!w->colliders[k].alive) { slot = k; break; }
+    const size_t slot = collider_free_slot(w);
     if (slot >= (size_t)MAX_BOUNDARIES) return w->fail(SPH_ERR_INVALID, "too many colliders (max %d)", MAX_BOUNDARIES);
     TRY(enter(w));
     if (!w->h_imp) CU(cudaMallocHost(&w->h_imp, 6 * MAX_BOUNDARIES * sizeof(float)));
@@ -3092,6 +3206,43 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     b.n = n;
     recompute_offsets(w);
     w->b_dirty = true;
+    if (slot == w->colliders.size()) w->colliders.push_back(c);
+    else w->colliders[slot] = c;
+    *collider = make_handle(slot, c.gen);
+    return SPH_OK;
+}
+
+// register_coupling(boundary, collider, DynamicContactSampling) for a collider whose shape is a parry HeightField: the
+// heights are copied into device memory the record owns (freed by unregister and by sph_world_destroy).
+sph_status sph_collider_register_heightfield(sph_world* w, uint32_t boundary_h, const sph_heightfield* hf, uint32_t* collider) {
+    if (!w || !collider) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    TRY(collider_check_boundary(w, boundary_h));
+    std::vector<float> heights;
+    ColliderRec c;
+    TRY(hf_check(w, hf, heights, c.hf, &c.hf_ylo, &c.hf_yhi));
+    const size_t slot = collider_free_slot(w);
+    if (slot >= (size_t)MAX_BOUNDARIES) return w->fail(SPH_ERR_INVALID, "too many colliders (max %d)", MAX_BOUNDARIES);
+    TRY(enter(w));
+    if (!w->h_imp) CU(cudaMallocHost(&w->h_imp, 6 * MAX_BOUNDARIES * sizeof(float)));
+    CU(w->d_imp.ensure(6 * MAX_BOUNDARIES));
+    {
+        const cudaError_t e = c.hgt.ensure(heights.size());
+        if (e != cudaSuccess) return w->fail(SPH_ERR_OOM, "heightfield collider: %s", cudaGetErrorString(e));
+    }
+    cudaError_t e = cudaMemcpyAsync(c.hgt.p, heights.data(), heights.size() * sizeof(float), cudaMemcpyHostToDevice, w->st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(w->st);
+    if (e != cudaSuccess) {
+        c.hgt.release();
+        return w->fail(SPH_ERR_CUDA, "heightfield collider upload: %s", cudaGetErrorString(e));
+    }
+    c.hf.hgt = c.hgt.p;
+    if (slot < w->colliders.size()) c.gen = w->colliders[slot].gen + 1;
+    c.boundary = boundary_h;
+    c.sampling = SPH_SAMPLING_CONTACT;
+    c.shape.kind = SPH_SHAPE_HEIGHTFIELD;
+    c.state.rotation_rowmajor[0] = c.state.rotation_rowmajor[4] = c.state.rotation_rowmajor[8] = 1.f;
+    c.state.body = SPH_BODY_NONE;
     if (slot == w->colliders.size()) w->colliders.push_back(c);
     else w->colliders[slot] = c;
     *collider = make_handle(slot, c.gen);
@@ -3138,6 +3289,7 @@ sph_status sph_collider_unregister(sph_world* w, uint32_t collider_h) {
     COLLIDER_OR_FAIL(c, collider_h)
     TRY(enter(w));
     c.local.release();
+    c.hgt.release();
     c.alive = false;
     return SPH_OK;
 }

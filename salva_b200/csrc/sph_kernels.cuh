@@ -1420,6 +1420,120 @@ __global__ void k_p2p_allreduce(float* __restrict__ vals, int n, int rank, int n
     }
 }
 
+__device__ __forceinline__ float dot3_rn(float a0, float a1, float a2, float b0, float b1, float b2) {
+    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
+}
+
+// ---- parry HeightField (DESIGN.md section 11 geometry), shared by the sampler and the point query ----------------------
+// cell index and fraction of coordinate c on a grid of `cells` cells of size d starting at -half
+__device__ __forceinline__ int smp_cell(float c, float half, float d, int cells, float* frac) {
+    const float t = __fdiv_rn(__fadd_rn(c, half), d);
+    const int i = min(max((int)floorf(t), 0), cells - 1);
+    *frac = __fsub_rn(t, (float)i);
+    return i;
+}
+
+__device__ __forceinline__ float smp_grid(int j, int last, float half, float d) {
+    return j == last ? half : __fadd_rn(-half, __fmul_rn((float)j, d));
+}
+
+struct HfGrid {
+    const float* hgt;         // nrows * ncols heights, row-major: rows along z, columns along x
+    int nrows, ncols;
+    float hx, hz, dx, dz, sy; // half extents in x and z, cell sizes, height scale
+    float dmin;               // min(dx, dz)
+    float cap2, margin;       // the search's cap (squared) and its margin M (DESIGN.md section 10)
+};
+
+// Closest point q of the closed triangle (a, b, c) to p and its squared distance: Ericson, Real-Time Collision Detection
+// 5.1.5 (vertex, edge and face regions), every operation an explicit round-to-nearest one.
+__device__ __forceinline__ float hf_tri(const float* p, const float* a, const float* b, const float* c, float* q) {
+    const float ab[3] = {__fsub_rn(b[0], a[0]), __fsub_rn(b[1], a[1]), __fsub_rn(b[2], a[2])};
+    const float ac[3] = {__fsub_rn(c[0], a[0]), __fsub_rn(c[1], a[1]), __fsub_rn(c[2], a[2])};
+    const float ap[3] = {__fsub_rn(p[0], a[0]), __fsub_rn(p[1], a[1]), __fsub_rn(p[2], a[2])};
+    const float d1 = dot3_rn(ab[0], ab[1], ab[2], ap[0], ap[1], ap[2]), d2 = dot3_rn(ac[0], ac[1], ac[2], ap[0], ap[1], ap[2]);
+    const float bp[3] = {__fsub_rn(p[0], b[0]), __fsub_rn(p[1], b[1]), __fsub_rn(p[2], b[2])};
+    const float d3 = dot3_rn(ab[0], ab[1], ab[2], bp[0], bp[1], bp[2]), d4 = dot3_rn(ac[0], ac[1], ac[2], bp[0], bp[1], bp[2]);
+    const float cp[3] = {__fsub_rn(p[0], c[0]), __fsub_rn(p[1], c[1]), __fsub_rn(p[2], c[2])};
+    const float d5 = dot3_rn(ab[0], ab[1], ab[2], cp[0], cp[1], cp[2]), d6 = dot3_rn(ac[0], ac[1], ac[2], cp[0], cp[1], cp[2]);
+    const float vc = __fsub_rn(__fmul_rn(d1, d4), __fmul_rn(d3, d2));
+    const float vb = __fsub_rn(__fmul_rn(d5, d2), __fmul_rn(d1, d6));
+    const float va = __fsub_rn(__fmul_rn(d3, d6), __fmul_rn(d5, d4));
+    const float e43 = __fsub_rn(d4, d3), e56 = __fsub_rn(d5, d6);
+    if (d1 <= 0.f && d2 <= 0.f) {
+        q[0] = a[0]; q[1] = a[1]; q[2] = a[2];
+    } else if (d3 >= 0.f && d4 <= d3) {
+        q[0] = b[0]; q[1] = b[1]; q[2] = b[2];
+    } else if (vc <= 0.f && d1 >= 0.f && d3 <= 0.f) {
+        const float v = __fdiv_rn(d1, __fsub_rn(d1, d3));
+        for (int k = 0; k < 3; ++k) q[k] = __fadd_rn(a[k], __fmul_rn(v, ab[k]));
+    } else if (d6 >= 0.f && d5 <= d6) {
+        q[0] = c[0]; q[1] = c[1]; q[2] = c[2];
+    } else if (vb <= 0.f && d2 >= 0.f && d6 <= 0.f) {
+        const float v = __fdiv_rn(d2, __fsub_rn(d2, d6));
+        for (int k = 0; k < 3; ++k) q[k] = __fadd_rn(a[k], __fmul_rn(v, ac[k]));
+    } else if (va <= 0.f && e43 >= 0.f && e56 >= 0.f) {
+        const float v = __fdiv_rn(e43, __fadd_rn(e43, e56));
+        for (int k = 0; k < 3; ++k) q[k] = __fadd_rn(b[k], __fmul_rn(v, __fsub_rn(c[k], b[k])));
+    } else {
+        const float den = __fdiv_rn(1.f, __fadd_rn(__fadd_rn(va, vb), vc));
+        const float v = __fmul_rn(vb, den), w = __fmul_rn(vc, den);
+        for (int k = 0; k < 3; ++k) q[k] = __fadd_rn(__fadd_rn(a[k], __fmul_rn(ab[k], v)), __fmul_rn(ac[k], w));
+    }
+    const float e[3] = {__fsub_rn(p[0], q[0]), __fsub_rn(p[1], q[1]), __fsub_rn(p[2], q[2])};
+    return dot3_rn(e[0], e[1], e[2], e[0], e[1], e[2]);
+}
+
+// Both triangles of cell (i, j), (p00, p10, p01) and (p10, p11, p01), into the running best: the lexicographic minimum of
+// (squared distance, parry triangle index 2 (j (nrows - 1) + i) + t), so the visit order cannot change a tie.
+__device__ __forceinline__ void hf_cell(const HfGrid& g, int i, int j, const float* p, float& best, uint32_t& bidx, float* q) {
+    const int ni = g.nrows - 1, nj = g.ncols - 1;
+    const float x0 = smp_grid(j, nj, g.hx, g.dx), x1 = smp_grid(j + 1, nj, g.hx, g.dx);
+    const float z0 = smp_grid(i, ni, g.hz, g.dz), z1 = smp_grid(i + 1, ni, g.hz, g.dz);
+    const float* r0 = g.hgt + (size_t)i * g.ncols + j;
+    const float p00[3] = {x0, __fmul_rn(__ldg(r0), g.sy), z0};
+    const float p10[3] = {x1, __fmul_rn(__ldg(r0 + 1), g.sy), z0};
+    const float p01[3] = {x0, __fmul_rn(__ldg(r0 + g.ncols), g.sy), z1};
+    const float p11[3] = {x1, __fmul_rn(__ldg(r0 + g.ncols + 1), g.sy), z1};
+    const uint32_t base = 2u * ((uint32_t)j * (uint32_t)ni + (uint32_t)i);
+    float t[3];
+    float d = hf_tri(p, p00, p10, p01, t);
+    if (d < best || (d == best && base < bidx)) { best = d; bidx = base; q[0] = t[0]; q[1] = t[1]; q[2] = t[2]; }
+    d = hf_tri(p, p10, p11, p01, t);
+    if (d < best || (d == best && base + 1u < bidx)) { best = d; bidx = base + 1u; q[0] = t[0]; q[1] = t[1]; q[2] = t[2]; }
+}
+
+// HeightField::project_local_point (parry query/point/point_heightfield.rs): the closest point q over all triangles of a
+// local point, is_inside always false.  Cells are searched in square rings around the point's (x, z) cell, clipped to the
+// field; ring r lies at least (r - 1) dmin away horizontally, and the search stops once (r - 1) dmin - M exceeds both the
+// best distance and the cap.  M covers the float32 error of every distance, so a triangle within the cap is never missed
+// and the result equals the all-triangle minimum wherever it lies within the cap.  *d2 = |p - q|^2; false: no triangle.
+__device__ __forceinline__ bool hf_closest(const HfGrid& g, float lx, float ly, float lz, float* q, float* d2) {
+    const float p[3] = {lx, ly, lz};
+    const int ni = g.nrows - 1, nj = g.ncols - 1;
+    float fu, fv;
+    const int ci = smp_cell(lz, g.hz, g.dz, ni, &fv), cj = smp_cell(lx, g.hx, g.dx, nj, &fu);
+    const int rmax = max(max(ci, ni - 1 - ci), max(cj, nj - 1 - cj));
+    float best = __int_as_float(0x7f800000);
+    uint32_t bidx = UINT32_MAX;
+    for (int r = 0; r <= rmax; ++r) {
+        const float gap = __fsub_rn(__fmul_rn((float)(r - 1), g.dmin), g.margin);
+        if (gap > 0.f && __fmul_rn(gap, gap) > fminf(best, g.cap2)) break;
+        const int i0 = max(ci - r, 0), i1 = min(ci + r, ni - 1);
+        for (int i = i0; i <= i1; ++i) {
+            if (i == ci - r || i == ci + r) {
+                const int j1 = min(cj + r, nj - 1);
+                for (int j = max(cj - r, 0); j <= j1; ++j) hf_cell(g, i, j, p, best, bidx, q);
+            } else {
+                if (cj - r >= 0) hf_cell(g, i, cj - r, p, best, bidx, q);
+                if (cj + r < nj) hf_cell(g, i, cj + r, p, best, bidx, q);
+            }
+        }
+    }
+    *d2 = best;
+    return bidx != UINT32_MAX;
+}
+
 // LiquidWorld::particles_intersecting_aabb liquid_world.rs:211-243 over HGrid::cells_intersecting_aabb hgrid.rs:122-133.
 // One thread per cell of the (clipped) cell box [key(mins), key(maxs)] of the grid built by the last step; the CURRENT
 // positions are tested (Aabb::distance_to_point, solid: norm of the per-axis excess) against particle_radius.
@@ -1434,9 +1548,11 @@ struct AabbQuery {
     int kind;
     float rot[9], t[3];          // world = rot * local + t (row-major rotation)
     float sp[3];                 // ball: radius; cuboid: half extents; capsule: half height, radius
+    HfGrid hf;                   // kind 4, heightfield (k_aabb_query<true>): cap = radius
 };
+template <bool HF>
 __device__ __forceinline__ bool query_near(const AabbQuery& q, const float4& p) {
-    if (q.kind == 0) {
+    if (!HF && q.kind == 0) {
         float ex = fmaxf(fmaxf(q.mins[0] - p.x, p.x - q.maxs[0]), 0.f);
         float ey = fmaxf(fmaxf(q.mins[1] - p.y, p.y - q.maxs[1]), 0.f);
         float ez = fmaxf(fmaxf(q.mins[2] - p.z, p.z - q.maxs[2]), 0.f);
@@ -1448,7 +1564,10 @@ __device__ __forceinline__ bool query_near(const AabbQuery& q, const float4& p) 
     const float ly = q.rot[1] * wx + q.rot[4] * wy + q.rot[7] * wz;
     const float lz = q.rot[2] * wx + q.rot[5] * wy + q.rot[8] * wz;
     float d;
-    if (q.kind == 1) {
+    if (HF) {  // HeightField::distance_to_point: the unsigned distance to the closest point (is_inside is always false)
+        float c[3], d2;
+        return hf_closest(q.hf, lx, ly, lz, c, &d2) && __fsqrt_rn(d2) <= q.radius;
+    } else if (q.kind == 1) {
         d = fmaxf(__fsqrt_rn(dist2_exact(lx, ly, lz)) - q.sp[0], 0.f);
     } else if (q.kind == 2) {
         float ex = fmaxf(fabsf(lx) - q.sp[0], 0.f), ey = fmaxf(fabsf(ly) - q.sp[1], 0.f), ez = fmaxf(fabsf(lz) - q.sp[2], 0.f);
@@ -1468,9 +1587,6 @@ struct ColliderPose {
     float linvel[3], angvel[3], com[3];
     int moving;  // 0: no parent body, velocity 0 (:184-186)
 };
-__device__ __forceinline__ float dot3_rn(float a0, float a1, float a2, float b0, float b1, float b2) {
-    return __fadd_rn(__fadd_rn(__fmul_rn(a0, b0), __fmul_rn(a1, b1)), __fmul_rn(a2, b2));
-}
 // One thread per SORTED boundary slot; the slots whose original index lies in [first, first + n) belong to the collider.
 __global__ void k_collider_static(uint32_t nb, const uint32_t* __restrict__ borig, uint32_t first, uint32_t n, const float4* __restrict__ local,
                                   ColliderPose P, float4* __restrict__ bpos, float4* __restrict__ bvel) {
@@ -1533,7 +1649,7 @@ __global__ void k_collider_impulse(uint32_t nb, const float4* __restrict__ bpos,
 // re-run with larger buffers when they overflow.  Every operation is an explicit round-to-nearest one, a fixed float32
 // expression a host can restate.
 struct ContactCollider {
-    int kind;                       // 1 ball (sp[0] radius), 2 cuboid (sp half extents), 3 capsule along local y (sp[0] half height, sp[1] radius)
+    int kind;                       // 1 ball (sp[0] radius), 2 cuboid (sp half extents), 3 capsule along local y (sp[0] half height, sp[1] radius), 4 heightfield
     uint32_t slot;                  // collider slot: the samples' sort key
     float rot[9], t[3], sp[3];      // world = rot * local + t
     float mins[3], maxs[3];         // the posed shape's AABB loosened by h + prediction
@@ -1550,6 +1666,7 @@ struct ContactParams {
     uint32_t total_bins;
     float dt, cut, margin;          // lagging dt, h + prediction, 0.1 particle_radius
     uint32_t cap_s, cap_p;
+    const HfGrid* hf;               // k_contact_sample<true>: per collider (same index as col), the grid of a kind-4 heightfield
 };
 __device__ __forceinline__ bool contact_in_box(const ContactCollider& c, int cx, int cy, int cz) {
     return cx >= c.clo[0] && cx <= c.chi[0] && cy >= c.clo[1] && cy <= c.chi[1] && cz >= c.clo[2] && cz <= c.chi[2];
@@ -1633,6 +1750,8 @@ __device__ __forceinline__ void warp_bounds_commit(int* mn, int* mx, int bad, in
 // A particle is processed by the enumeration of the lowest-slot collider whose box holds its cell.  Records:
 // samples  s4[2r] = (proj, orig), s4[2r+1] = (velocity, 0), key[r] = slot << 32 | orig, val[r] = r;
 // pushes   p4[2r] = (new position, sorted slot), p4[2r+1] = (new velocity, 0).
+// HF: the instantiation for worlds with a heightfield collider; the others run k_contact_sample<false>, without its code.
+template <bool HF>
 __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                                  const uint32_t* __restrict__ orig, float4* __restrict__ s4, unsigned long long* __restrict__ key, uint32_t* __restrict__ val,
                                  float4* __restrict__ p4, int* __restrict__ res) {
@@ -1673,8 +1792,14 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
                 bool inside = false;
                 if (emit) {
                     const float wx = __fsub_rn(pr[0], K.t[0]), wy = __fsub_rn(pr[1], K.t[1]), wz = __fsub_rn(pr[2], K.t[2]);
-                    emit = contact_project_local(K, dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
-                                                 dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &inside);
+                    if (HF && K.kind == 4) {  // a heightfield never has the point inside: samples only, no push
+                        float d2;
+                        emit = hf_closest(P.hf[k], dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
+                                          dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &d2);
+                    } else {
+                        emit = contact_project_local(K, dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
+                                                     dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &inside);
+                    }
                 }
                 if (emit) {
 #pragma unroll
@@ -1796,6 +1921,7 @@ __global__ void k_contact_write(uint32_t n, const unsigned long long* __restrict
     oorig[d] = d;
 }
 
+template <bool HF>
 __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const uint32_t* __restrict__ cstart, const uint32_t* __restrict__ orig,
                              const float4* __restrict__ bpos, const uint32_t* __restrict__ bstart, const uint32_t* __restrict__ borig,
                              uint32_t* __restrict__ out, uint32_t cap, uint32_t* __restrict__ count) {
@@ -1808,7 +1934,7 @@ __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const u
     if (pos) {
         uint32_t s = max(cstart[c], q.slot_lo), e = min(cstart[c + 1], q.slot_hi);
         for (uint32_t j = s; j < e; ++j)
-            if (query_near(q, pos[j])) {
+            if (query_near<HF>(q, pos[j])) {
                 uint32_t k = atomicAdd(count, 1u);
                 if (k < cap) {
                     out[2 * (size_t)k] = 0u;
@@ -1818,7 +1944,7 @@ __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const u
     }
     if (bpos) {
         for (uint32_t j = bstart[c]; j < bstart[c + 1]; ++j)
-            if (query_near(q, bpos[j])) {
+            if (query_near<HF>(q, bpos[j])) {
                 uint32_t k = atomicAdd(count, 1u);
                 if (k < cap) {
                     out[2 * (size_t)k] = 1u;

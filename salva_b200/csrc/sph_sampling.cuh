@@ -107,18 +107,6 @@ __device__ __forceinline__ void smp_piece(float xa, float xb, float fa, float fb
     wk.hit(__fadd_rn(xa, __fmul_rn(__fsub_rn(xb, xa), __fdiv_rn(fa, __fsub_rn(fa, fb)))), s);
 }
 
-// cell index and fraction of coordinate c on a grid of `cells` cells of size d starting at -half
-__device__ __forceinline__ int smp_cell(float c, float half, float d, int cells, float* frac) {
-    const float t = __fdiv_rn(__fadd_rn(c, half), d);
-    const int i = min(max((int)floorf(t), 0), cells - 1);
-    *frac = __fsub_rn(t, (float)i);
-    return i;
-}
-
-__device__ __forceinline__ float smp_grid(int j, int last, float half, float d) {
-    return j == last ? half : __fadd_rn(-half, __fmul_rn((float)j, d));
-}
-
 // heightfield, ray along x at (y, z): the profile of cell row i at z fraction v.  In each cell the ray crosses triangle
 // (p00, p10, p01) up to the diagonal at x0 + (1 - v) dx, then (p10, p11, p01).
 __device__ void smp_hf_along_x(const SampleRays& P, float y, float z, SmpWalk& wk, SmpSink& s) {

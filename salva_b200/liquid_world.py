@@ -175,11 +175,24 @@ class StaticSampling:
 
 class DynamicContactSampling:
     """ColliderSampling::DynamicContactSampling (fluids_pipeline.rs:71, 192-255): every step the collider's shape (Ball,
-    Cuboid or Capsule) is sampled where the fluid is about to touch it, and penetrating fluid particles are pushed out."""
+    Cuboid, Capsule or sampling.HeightField) is sampled where the fluid is about to touch it, and penetrating fluid particles
+    are pushed out.  A heightfield never pushes (parry's heightfield point query has is_inside always false): it only samples."""
     kind = 1
 
     def __init__(self, shape):
         self.shape = shape
+
+
+HEIGHTFIELD = 4  # SPH_SHAPE_HEIGHTFIELD: salva_b200.sampling.HeightField
+
+
+def heightfield_c(shape):
+    """The sph_heightfield of a sampling.HeightField; it points into shape.heights, which must outlive the call."""
+    hf = _lib.HeightFieldC()
+    hf.nrows, hf.ncols = shape.heights.shape
+    hf.heights = shape.heights.ctypes.data_as(C.POINTER(C.c_float))
+    hf.scale[:] = shape.scale
+    return hf
 
 
 # the rigid body a collider is attached to (include/sph.h SPH_BODY_*)
@@ -415,6 +428,11 @@ class LiquidWorld:
         """ColliderCouplingSet::register_coupling (fluids_pipeline.rs:98-114): couples `boundary` to a new collider and
         returns the collider's handle.  The engine owns the boundary's particles from then on."""
         pts = getattr(sampling, "points", np.zeros((0, 3), np.float32))
+        if sampling.kind == DynamicContactSampling.kind and getattr(getattr(sampling, "shape", None), "kind", None) == HEIGHTFIELD:
+            h = C.c_uint32()
+            self._ck(self._L.sph_collider_register_heightfield(self._w, boundary, C.byref(heightfield_c(sampling.shape)), C.byref(h)))
+            self._nb.pop(boundary, None)
+            return h.value
         sh = None
         if getattr(sampling, "shape", None) is not None:
             sh = _lib.Shape()
@@ -463,11 +481,17 @@ class LiquidWorld:
         return p, v
 
     def particles_intersecting_shape(self, shape, translation=(0.0, 0.0, 0.0), rotation=None):
-        """liquid_world.rs:246-281 for Ball / Cuboid / Capsule under the isometry (rotation 3x3 row-major, translation)."""
-        sh = _lib.Shape()
-        sh.kind = shape.kind
-        for i, x in enumerate(shape.params):
-            sh.p[i] = x
+        """liquid_world.rs:246-281 for Ball / Cuboid / Capsule / sampling.HeightField under the isometry (rotation 3x3
+        row-major, translation)."""
+        if shape.kind == HEIGHTFIELD:
+            sh = heightfield_c(shape)
+            query = self._L.sph_world_particles_in_heightfield
+        else:
+            sh = _lib.Shape()
+            sh.kind = shape.kind
+            for i, x in enumerate(shape.params):
+                sh.p[i] = x
+            query = self._L.sph_world_particles_in_shape
         t = np.ascontiguousarray(translation, np.float32)
         R = None if rotation is None else np.ascontiguousarray(rotation, np.float32).reshape(9)
         n = C.c_size_t(0)
@@ -477,8 +501,8 @@ class LiquidWorld:
             k = np.empty(cap, np.uint32)
             h = np.empty(cap, np.uint32)
             i = np.empty(cap, np.uint32)
-            self._ck(self._L.sph_world_particles_in_shape(self._w, C.byref(sh), _fp(t), _fp(R), k.ctypes.data_as(u32p), h.ctypes.data_as(u32p),
-                                                          i.ctypes.data_as(u32p), cap, C.byref(n)))
+            self._ck(query(self._w, C.byref(sh), _fp(t), _fp(R), k.ctypes.data_as(u32p), h.ctypes.data_as(u32p), i.ctypes.data_as(u32p), cap,
+                           C.byref(n)))
             if n.value <= cap:
                 return k[:n.value], h[:n.value], i[:n.value]
             cap = n.value

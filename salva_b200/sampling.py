@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .liquid_world import Ball, Capsule, Cuboid  # noqa: F401  (the shapes the sampler takes, with HeightField)
+from .liquid_world import Ball, Capsule, Cuboid, heightfield_c  # noqa: F401  (the shapes the sampler takes, with HeightField)
 
 SURFACE, VOLUME = 0, 1  # SPH_SAMPLE_*
 
@@ -18,7 +18,7 @@ SURFACE, VOLUME = 0, 1  # SPH_SAMPLE_*
 class HeightField:
     """parry HeightField(heights, scale): rows of `heights` run along z and columns along x, the field spans
     [-0.5, 0.5] * scale in x and z, heights are multiplied by scale[1], and each cell is split along its (x0, z1)-(x1, z0)
-    diagonal."""
+    diagonal.  Also a collider shape for DynamicContactSampling and LiquidWorld.particles_intersecting_shape."""
     kind = 4
 
     def __init__(self, heights, scale):
@@ -34,12 +34,7 @@ def _ray_sample(world, shape, particle_rad, method):
     sh.kind = shape.kind
     for a, p in enumerate(shape.params):
         sh.p[a] = p
-    hf = None
-    if shape.kind == HeightField.kind:
-        hf = _lib.HeightFieldC()
-        hf.nrows, hf.ncols = shape.heights.shape
-        hf.heights = shape.heights.ctypes.data_as(C.POINTER(C.c_float))
-        hf.scale[:] = shape.scale
+    hf = heightfield_c(shape) if shape.kind == HeightField.kind else None
     n = C.c_size_t(0)
     cap = getattr(world, "_sample_cap", 1 << 16)
     while True:
