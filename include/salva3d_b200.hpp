@@ -160,6 +160,8 @@ struct Isometry3 {
 struct Ball { Real radius; };
 struct Cuboid { Vector3 half_extents; };
 struct Capsule { Real half_height, radius; };  // segment along local y
+struct Cylinder { Real half_height, radius; };  // axis along local y
+struct Cone { Real half_height, radius; };      // axis along local y, apex at (0, half_height, 0), base disc at y = -half_height
 // parry HeightField(heights, scale) for ray sampling: nrows x ncols row-major heights, rows along z, columns along x,
 // centred on [-0.5, 0.5] * scale in x and z, cells split along their (x0, z1)-(x1, z0) diagonal (DESIGN.md section 11)
 struct HeightField {
@@ -184,6 +186,8 @@ struct ColliderSampling {
         return contact(sph_shape{SPH_SHAPE_CUBOID, {s.half_extents.x, s.half_extents.y, s.half_extents.z}});
     }
     static ColliderSampling DynamicContactSampling(const Capsule& s) { return contact(sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}); }
+    static ColliderSampling DynamicContactSampling(const Cylinder& s) { return contact(sph_shape{SPH_SHAPE_CYLINDER, {s.half_height, s.radius}}); }
+    static ColliderSampling DynamicContactSampling(const Cone& s) { return contact(sph_shape{SPH_SHAPE_CONE, {s.half_height, s.radius}}); }
     // a heightfield only samples, it never pushes fluid (parry's heightfield point query has is_inside always false)
     static ColliderSampling DynamicContactSampling(const HeightField& s) {
         ColliderSampling c = contact(sph_shape{SPH_SHAPE_HEIGHTFIELD, {}});
@@ -481,7 +485,7 @@ public:
         for (size_t t = 0; t < n; ++t) out[t] = ParticleId{k[t] != 0, h[t], i[t]};
         return out;
     }
-    // liquid_world.rs:246-281 for Ball / Cuboid / Capsule / HeightField
+    // liquid_world.rs:246-281 for Ball / Cuboid / Capsule / Cylinder / Cone / HeightField
     // ray_sampling.rs:9-24 on this world's device (salva3d::sampling below): points in ascending quantised-key order
     std::vector<Point3> ray_sample(int32_t method, const sph_shape& shape, const sph_heightfield* hf, Real particle_rad) {
         std::vector<Point3> out(4096);
@@ -500,6 +504,12 @@ public:
     }
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Capsule& s) {
         return shape_query(pos, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}});
+    }
+    std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Cylinder& s) {
+        return shape_query(pos, sph_shape{SPH_SHAPE_CYLINDER, {s.half_height, s.radius}});
+    }
+    std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const Cone& s) {
+        return shape_query(pos, sph_shape{SPH_SHAPE_CONE, {s.half_height, s.radius}});
     }
     std::vector<ParticleId> particles_intersecting_shape(const Isometry3& pos, const HeightField& s) {
         const sph_heightfield hf = heightfield_view(s);
@@ -621,6 +631,12 @@ inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Cuboid& s, Real 
 }
 inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Capsule& s, Real r) {
     return w.ray_sample(m, sph_shape{SPH_SHAPE_CAPSULE, {s.half_height, s.radius}}, nullptr, r);
+}
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Cylinder& s, Real r) {
+    return w.ray_sample(m, sph_shape{SPH_SHAPE_CYLINDER, {s.half_height, s.radius}}, nullptr, r);
+}
+inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const Cone& s, Real r) {
+    return w.ray_sample(m, sph_shape{SPH_SHAPE_CONE, {s.half_height, s.radius}}, nullptr, r);
 }
 inline std::vector<Point3> run(LiquidWorld& w, int32_t m, const HeightField& s, Real r) {
     const sph_heightfield hf = heightfield_view(s);

@@ -279,6 +279,13 @@ sph_status sph_world_particles_in_aabb(sph_world* w, const float mins[3], const 
 enum { SPH_SHAPE_BALL = 1,     /* p[0] = radius */
        SPH_SHAPE_CUBOID = 2,   /* p[0..2] = half extents */
        SPH_SHAPE_CAPSULE = 3   /* p[0] = half height (segment along local y), p[1] = radius */ };
+/* parry Cylinder / Cone, axis along local y, p[0] = half height a, p[1] = (base) radius r, both finite and >= 0 (zero gives a
+ * disc, a segment, a flat or a needle cone).  The cylinder is sqrt(x^2 + z^2) <= r, |y| <= a; the cone's apex is (0, a, 0)
+ * and its base disc lies at y = -a: |y| <= a, sqrt(x^2 + z^2) <= r (a - y) / (2a).  Local AABB [-r, -a, -r]-[r, a, r]; the
+ * posed AABB is parry's tight support-map box, not centred on the translation for the cone.  Projection, inside test and
+ * tie order: DESIGN.md section 10.  Kinds 5 and 6 are accepted by sph_world_particles_in_shape, sph_collider_register and
+ * sph_world_sample_shape. */
+enum { SPH_SHAPE_CYLINDER = 5, SPH_SHAPE_CONE = 6 };
 typedef struct {
     int32_t kind;
     float   p[4];
@@ -346,7 +353,7 @@ enum { SPH_SAMPLING_STATIC = 0,    /* ColliderSampling::StaticSampling(points)  
    pushed out along the projection normal by depth + 0.1 particle_radius and loses its velocity into the shape; the projection
    becomes a boundary particle with the body's velocity at that WORLD point, unless p lies more than 1.5 h outside.  Colliders
    run in slot order; the boundary holds its samples ordered by the sampled particle's fluid slot, then index.  A ball's
-   centre yields no sample; a point on a capsule's axis projects along local +x.  A heightfield (parry's point query has
+   centre yields no sample; a point on a capsule's, cylinder's or cone's axis projects along local +x.  A heightfield (parry's point query has
    is_inside always false, point_heightfield.rs) never pushes: it only samples its closest surface points.  See DESIGN.md
    section 10. */
 enum { SPH_BODY_NONE = 0,     /* collider.parent() == None: velocity 0, boundary.forces left as it is (fluids_pipeline.rs:163-171),
@@ -362,7 +369,7 @@ typedef struct {
 /* ColliderCouplingSet::register_coupling(boundary, collider, sampling)  fluids_pipeline.rs:98-114.  StaticSampling: the n_points
  * local points (packed xyz) become the boundary's particles; every step they are posed by the collider's state, with the
  * velocity velocity_at_point(pt) evaluated at the LOCAL point pt, as fluids_pipeline.rs:183 does (a quirk of the reference,
- * reproduced).  `shape` may be NULL for StaticSampling.  SPH_SAMPLING_CONTACT needs a ball, cuboid or capsule `shape` with
+ * reproduced).  `shape` may be NULL for StaticSampling.  SPH_SAMPLING_CONTACT needs a ball, cuboid, capsule, cylinder or cone `shape` with
  * finite, non-negative parameters and n_points == 0; the boundary keeps its particles until the next step refills it, and its
  * particle count changes every step (sph_boundary_count).  The engine owns the boundary's particle set from then on:
  * sph_boundary_write / _set_particles refuse it.  A boundary can be coupled to one collider at a time.  The initial state

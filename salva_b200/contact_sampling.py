@@ -11,7 +11,7 @@ from .liquid_world import BODY_NONE, CouplingManager
 
 F32 = np.float32
 EPS = F32(np.finfo(np.float32).eps)  # Unit::try_new_and_get(dpt, f32::EPSILON)
-BALL, CUBOID, CAPSULE, HEIGHTFIELD = 1, 2, 3, 4
+BALL, CUBOID, CAPSULE, HEIGHTFIELD, CYLINDER, CONE = 1, 2, 3, 4, 5, 6
 NO_TRI = 2 ** 32 - 1  # no triangle yet (the device's UINT32_MAX)
 
 
@@ -50,6 +50,18 @@ def posed_aabb(kind, params, rotation, translation, hf=None):
     p = np.zeros(4, F32)
     p[:len(params)] = np.asarray(params, F32)
     t = np.asarray(translation, F32)
+    if kind in (CYLINDER, CONE):  # rev_posed_aabb: parry's tight support-map box
+        mins, maxs = np.empty(3, F32), np.empty(3, F32)
+        a, r = p[0], p[1]
+        for i in range(3):
+            si = np.sqrt(R[i, 0] * R[i, 0] + R[i, 2] * R[i, 2])
+            ay, rs = a * R[i, 1], r * si
+            if kind == CYLINDER:
+                ext = abs(R[i, 1]) * a + rs
+                mins[i], maxs[i] = t[i] - ext, t[i] + ext
+            else:
+                mins[i], maxs[i] = t[i] + min(ay, -ay - rs), t[i] + max(ay, -ay + rs)
+        return mins, maxs
     ext = np.empty(3, F32)
     for a in range(3):
         if kind == BALL:
@@ -163,6 +175,34 @@ def hf_project_local(g, l, cap):
     return q, best, bidx != NO_TRI
 
 
+def rev_meridian(kind, a, r, rho, y):
+    """rev_meridian: the meridian foot (qr, qy) of a cylinder or cone (half height a, radius r) for points (rho, y), whether
+    the point is inside (surface included) and whether the foot keeps the point's rho."""
+    a, r = F32(a), F32(r)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        if kind == CYLINDER:
+            inside = (rho <= r) & (np.abs(y) <= a)
+            ds, db, dt = r - rho, y + a, a - y
+            keep_in = ~((ds <= db) & (ds <= dt))
+            qy_in = np.where(~keep_in, y, np.where(db <= dt, -a, a))
+            keep = np.where(inside, keep_in, rho <= r)
+            qr = np.where(keep, rho, r)
+            qy = np.where(inside, qy_in, np.minimum(np.maximum(y, -a), a))
+            return qr.astype(F32), qy.astype(F32), inside, keep
+        a2 = a + a
+        L2 = r * r + a2 * a2
+        num = r * (a - y) - a2 * rho
+        inside = (y >= -a) & (y <= a) & (rho <= r) & (num >= 0)
+        slant = (L2 > 0) & (num / np.sqrt(L2) <= y + a)
+        w = num / L2
+        under = (y < -a) & (rho <= r)
+        s = np.minimum(np.maximum((r * rho + a2 * (a - y)) / L2, F32(0)), F32(1)) if L2 > 0 else np.zeros_like(rho)
+        keep = np.where(inside, ~slant, under)
+        qr = np.where(inside, np.where(slant, rho + w * a2, rho), np.where(under, rho, s * r))
+        qy = np.where(inside, np.where(slant, y + w * r, -a), np.where(under, -a, a - s * a2))
+        return qr.astype(F32), qy.astype(F32), inside, keep
+
+
 def project_local(kind, params, l):
     """project_point_and_get_feature (non-solid) in the shape's local frame, for points l (n, 3) float32.
     Returns (proj (n, 3), inside (n,), valid (n,)); valid is False where the projection is undefined (a ball's centre)."""
@@ -172,7 +212,13 @@ def project_local(kind, params, l):
     lx, ly, lz = l[:, 0], l[:, 1], l[:, 2]
     valid = np.ones(len(l), bool)
     with np.errstate(divide="ignore", invalid="ignore"):
-        if kind == BALL:
+        if kind in (CYLINDER, CONE):  # the meridian foot lifted along (x, z) / rho, along local +x at rho = 0
+            rho = np.sqrt(lx * lx + lz * lz)
+            qr, qy, inside, keep = rev_meridian(kind, p[0], p[1], rho, ly)
+            s = qr / rho
+            axis = rho == 0
+            q = np.stack([np.where(keep, lx, np.where(axis, qr, lx * s)), qy, np.where(keep, lz, np.where(axis, F32(0), lz * s))], axis=1)
+        elif kind == BALL:
             n2 = _dot(lx, ly, lz, lx, ly, lz)
             valid = n2 != 0
             inside = n2 <= p[0] * p[0]

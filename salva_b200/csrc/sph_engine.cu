@@ -780,6 +780,30 @@ void posed_aabb_ext(const sph_shape& s, const float R[9], float ext[3]) {
     }
 }
 
+// compute_aabb(pos) of a cylinder or cone (a = p[0], r = p[1], axis along local y): parry's support-map box, which is tight.
+// With s_i = |(R_i0, R_i2)|, the cylinder's box is centred on t with half extents a |R_i1| + r s_i; the cone's apex
+// t + a R_1 and base rim give max_i = t_i + max(a R_i1, -a R_i1 + r s_i), min_i = t_i + min(a R_i1, -a R_i1 - r s_i).
+void rev_posed_aabb(const sph_shape& s, const float R[9], const float t[3], float mins[3], float maxs[3]) {
+    const float a = s.p[0], r = s.p[1];
+    for (int i = 0; i < 3; ++i) {
+        const float si = std::sqrt(R[3 * i] * R[3 * i] + R[3 * i + 2] * R[3 * i + 2]);
+        const float ay = a * R[3 * i + 1], rs = r * si;
+        if (s.kind == SPH_SHAPE_CYLINDER) {
+            const float ext = std::fabs(R[3 * i + 1]) * a + rs;
+            mins[i] = t[i] - ext;
+            maxs[i] = t[i] + ext;
+        } else {
+            mins[i] = t[i] + std::fmin(ay, -ay - rs);
+            maxs[i] = t[i] + std::fmax(ay, -ay + rs);
+        }
+    }
+}
+bool is_rev(int kind) { return kind == SPH_SHAPE_CYLINDER || kind == SPH_SHAPE_CONE; }
+// parameters a shape kind reads from sph_shape.p (0: unknown kind, or a heightfield)
+int shape_nparams(int kind) {
+    return kind == SPH_SHAPE_BALL ? 1 : kind == SPH_SHAPE_CUBOID ? 3 : kind == SPH_SHAPE_CAPSULE || is_rev(kind) ? 2 : 0;
+}
+
 // The heightfield checks of sph_world_sample_shape, shared by every entry point that takes one: 2 x 2 or more, finite
 // heights, a finite positive scale.  Fills the grid constants and the scaled height range [*ylo, *yhi].
 sph_status hf_check(sph_world* w, const sph_heightfield* hf, std::vector<float>& heights, HfGrid& g, float* ylo, float* yhi) {
@@ -856,7 +880,7 @@ sph_status colliders_contact(sph_world* w) {
     std::vector<HfGrid> chf;
     unsigned long long skip = 0;
     size_t bins = 0;
-    bool any_hf = false;
+    bool any_hf = false, any_rev = false;
     for (size_t k = 0; k < w->colliders.size(); ++k) {
         const ColliderRec& c = w->colliders[k];
         if (!c.alive || c.sampling != SPH_SAMPLING_CONTACT) continue;
@@ -880,6 +904,9 @@ sph_status colliders_contact(sph_world* w) {
             hf_set_cap(chf.back(), c.hf_ylo, c.hf_yhi, cut);
             hf_posed_aabb(c.hf, c.hf_ylo, c.hf_yhi, K.rot, K.t, lo, hi);
             any_hf = true;
+        } else if (is_rev(c.shape.kind)) {
+            rev_posed_aabb(c.shape, K.rot, K.t, lo, hi);
+            any_rev = true;
         } else {
             float ext[3];
             posed_aabb_ext(c.shape, K.rot, ext);
@@ -933,12 +960,10 @@ sph_status colliders_contact(sph_world* w) {
         CU(cudaMemcpyAsync(w->d_cres.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
         if (N && bins) {
             ContactParams P{w->d_ccol.p, nc, (uint32_t)bins, w->dt, cut, margin, w->cap_s, w->cap_p, any_hf ? w->d_chf.p : nullptr};
-            if (any_hf)
-                LAUNCH(k_contact_sample<true>, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p,
-                       w->cs_key[0].p, w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
-            else
-                LAUNCH(k_contact_sample<false>, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p,
-                       w->cs_key[0].p, w->cs_val[0].p, w->cs_p4.p, w->d_cres.p);
+            const auto kern = any_hf ? (any_rev ? k_contact_sample<true, true> : k_contact_sample<true, false>)
+                                     : (any_rev ? k_contact_sample<false, true> : k_contact_sample<false, false>);
+            LAUNCH(kern, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p, w->cs_key[0].p, w->cs_val[0].p,
+                   w->cs_p4.p, w->d_cres.p);
             k_contact_apply<<<std::min<uint32_t>(cdiv(w->cap_p, 256), 264), 256, 0, w->st>>>(w->cs_p4.p, w->d_cres.p, w->cap_s, w->cap_p, w->pos[c].p,
                                                                                          w->vel[c].p);
             w->launches++;
@@ -2552,12 +2577,9 @@ static sph_status run_query(sph_world* w, AabbQuery q, const float mins[3], cons
     for (int attempt = 0; attempt < 2; ++attempt) {
         CU(w->q_out.ensure(2 * qcap));
         CU(cudaMemsetAsync(w->q_count.p, 0, sizeof(uint32_t), w->st));
-        if (q.kind == SPH_SHAPE_HEIGHTFIELD)
-            LAUNCH(k_aabb_query<true>, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr,
-                   w->bstart.p, w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
-        else
-            LAUNCH(k_aabb_query<false>, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr,
-                   w->bstart.p, w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
+        const auto kern = q.kind == SPH_SHAPE_HEIGHTFIELD ? k_aabb_query<true, false> : is_rev(q.kind) ? k_aabb_query<false, true> : k_aabb_query<false, false>;
+        LAUNCH(kern, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr, w->bstart.p,
+               w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
         CU(cudaMemcpyAsync(&found, w->q_count.p, sizeof found, cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
         if (found <= qcap) break;
@@ -2632,15 +2654,27 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
             q.sp[0] = shape->p[0];
             q.sp[1] = shape->p[1];
             break;
+        case SPH_SHAPE_CYLINDER:
+        case SPH_SHAPE_CONE:
+            for (int a = 0; a < 2; ++a)
+                if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f)) return w->fail(SPH_ERR_INVALID, "shape parameters must be finite and >= 0");
+            q.kind = shape->kind;
+            q.sp[0] = shape->p[0];
+            q.sp[1] = shape->p[1];
+            break;
         default:
             return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
     }
-    float ext[3];  // half extents of the posed shape's AABB
-    posed_aabb_ext(*shape, R, ext);
     float mins[3], maxs[3];
-    for (int a = 0; a < 3; ++a) {
-        mins[a] = translation[a] - ext[a];
-        maxs[a] = translation[a] + ext[a];
+    if (is_rev(shape->kind)) {
+        rev_posed_aabb(*shape, R, translation, mins, maxs);
+    } else {
+        float ext[3];  // half extents of the posed shape's AABB
+        posed_aabb_ext(*shape, R, ext);
+        for (int a = 0; a < 3; ++a) {
+            mins[a] = translation[a] - ext[a];
+            maxs[a] = translation[a] + ext[a];
+        }
     }
     return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
 }
@@ -2690,7 +2724,7 @@ sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape*
     P.volume = method == SPH_SAMPLE_VOLUME;
     float mins[3], maxs[3];
     std::vector<float> heights;
-    const int np = shape->kind == SPH_SHAPE_BALL ? 1 : shape->kind == SPH_SHAPE_CUBOID ? 3 : shape->kind == SPH_SHAPE_CAPSULE ? 2 : 0;
+    const int np = shape_nparams(shape->kind);
     for (int a = 0; a < np; ++a) {
         if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f))
             return w->fail(SPH_ERR_INVALID, "shape parameter %d must be finite and >= 0 (got %g)", a, (double)shape->p[a]);
@@ -2709,6 +2743,13 @@ sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape*
             maxs[0] = maxs[2] = 0.f + P.p[1];
             mins[1] = -P.p[0] - P.p[1];
             maxs[1] = P.p[0] + P.p[1];
+            break;
+        case SPH_SHAPE_CYLINDER:  // both: [-r, -a, -r] to [r, a, r]
+        case SPH_SHAPE_CONE:
+            mins[0] = mins[2] = 0.f - P.p[1];
+            maxs[0] = maxs[2] = 0.f + P.p[1];
+            mins[1] = -P.p[0];
+            maxs[1] = P.p[0];
             break;
         case SPH_SHAPE_HEIGHTFIELD: {
             HfGrid g;
@@ -3158,12 +3199,13 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     TRY(collider_check_boundary(w, boundary_h));
     BOUNDARY_OR_FAIL(boundary, boundary_h)
-    if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE)) return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
+    if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE) && !is_rev(shape->kind))
+        return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
     if (sampling != SPH_SAMPLING_STATIC && sampling != SPH_SAMPLING_CONTACT) return w->fail(SPH_ERR_INVALID, "unknown sampling %d", sampling);
     if (sampling == SPH_SAMPLING_CONTACT) {
         if (!shape) return w->fail(SPH_ERR_INVALID, "DynamicContactSampling needs the collider's shape");
         if (n) return w->fail(SPH_ERR_INVALID, "DynamicContactSampling takes no sample points");
-        const int np = shape->kind == SPH_SHAPE_BALL ? 1 : shape->kind == SPH_SHAPE_CUBOID ? 3 : 2;
+        const int np = shape_nparams(shape->kind);
         for (int a = 0; a < np; ++a)
             if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f)) return w->fail(SPH_ERR_INVALID, "shape parameters must be finite and >= 0");
     }

@@ -1534,6 +1534,53 @@ __device__ __forceinline__ bool hf_closest(const HfGrid& g, float lx, float ly, 
     return bidx != UINT32_MAX;
 }
 
+// Solids of revolution about local y: kind 5 cylinder, kind 6 cone, a = half height, r = (base) radius; the cone's apex is
+// at (0, a, 0) and its base disc at y = -a.  Every query is a 2-D one in the meridian half-plane (rho, y), rho = |(x, z)|,
+// on the closed section [0, r] x [-a, a] or the triangle (0, a), (r, -a), (0, -a).  Outside: the closest point of the
+// section.  Inside, surface included: the foot on the nearest surface edge (the axis is no surface); a tie goes to the side
+// (the cone's slant), then to the bottom (base), then to the top.  keep: the foot keeps the point's rho.
+__device__ __forceinline__ void rev_meridian(int kind, float a, float r, float rho, float y, float& qr, float& qy, bool& inside, bool& keep) {
+    if (kind == 5) {
+        inside = rho <= r && fabsf(y) <= a;
+        if (inside) {
+            const float ds = __fsub_rn(r, rho), db = __fadd_rn(y, a), dt = __fsub_rn(a, y);
+            keep = !(ds <= db && ds <= dt);
+            qr = keep ? rho : r;
+            qy = !keep ? y : db <= dt ? -a : a;
+        } else {
+            keep = rho <= r;
+            qr = keep ? rho : r;
+            qy = fminf(fmaxf(y, -a), a);
+        }
+        return;
+    }
+    const float a2 = __fadd_rn(a, a);
+    const float L2 = __fadd_rn(__fmul_rn(r, r), __fmul_rn(a2, a2));
+    const float num = __fsub_rn(__fmul_rn(r, __fsub_rn(a, y)), __fmul_rn(a2, rho));  // |slant| times the depth below the slant
+    inside = y >= -a && y <= a && rho <= r && num >= 0.f;
+    if (inside) {
+        keep = !(L2 > 0.f && __fdiv_rn(num, __fsqrt_rn(L2)) <= __fadd_rn(y, a));
+        if (!keep) {  // the foot on the slant: the point plus depth times the unit normal (2a, r) / |slant|
+            const float w = __fdiv_rn(num, L2);
+            qr = __fadd_rn(rho, __fmul_rn(w, a2));
+            qy = __fadd_rn(y, __fmul_rn(w, r));
+        } else {
+            qr = rho;
+            qy = -a;
+        }
+    } else if (y < -a && rho <= r) {  // under the base disc
+        keep = true;
+        qr = rho;
+        qy = -a;
+    } else {  // the slant from the apex (0, a) to the rim (r, -a), its parameter clamped to the segment
+        keep = false;
+        const float s = L2 > 0.f ? fminf(fmaxf(__fdiv_rn(__fadd_rn(__fmul_rn(r, rho), __fmul_rn(a2, __fsub_rn(a, y))), L2), 0.f), 1.f) : 0.f;
+        qr = __fmul_rn(s, r);
+        qy = __fsub_rn(a, __fmul_rn(s, a2));
+    }
+}
+__device__ __forceinline__ float rev_rho(float lx, float lz) { return __fsqrt_rn(__fadd_rn(__fmul_rn(lx, lx), __fmul_rn(lz, lz))); }
+
 // LiquidWorld::particles_intersecting_aabb liquid_world.rs:211-243 over HGrid::cells_intersecting_aabb hgrid.rs:122-133.
 // One thread per cell of the (clipped) cell box [key(mins), key(maxs)] of the grid built by the last step; the CURRENT
 // positions are tested (Aabb::distance_to_point, solid: norm of the per-axis excess) against particle_radius.
@@ -1547,11 +1594,24 @@ struct AabbQuery {
     // when shape.distance_to_point(pos, p, solid) <= radius (:263)
     int kind;
     float rot[9], t[3];          // world = rot * local + t (row-major rotation)
-    float sp[3];                 // ball: radius; cuboid: half extents; capsule: half height, radius
+    float sp[3];                 // ball: radius; cuboid: half extents; capsule, cylinder, cone: half height, radius
     HfGrid hf;                   // kind 4, heightfield (k_aabb_query<true>): cap = radius
 };
-template <bool HF>
+// HF: kind 4 only; REV: kinds 5 and 6 only (k_aabb_query<false, true>); neither: kinds 0 to 3.
+template <bool HF, bool REV = false>
 __device__ __forceinline__ bool query_near(const AabbQuery& q, const float4& p) {
+    if (REV) {  // distance_to_point(solid): 0 inside, else the meridian distance to the closest point of the section
+        const float wx = __fsub_rn(p.x, q.t[0]), wy = __fsub_rn(p.y, q.t[1]), wz = __fsub_rn(p.z, q.t[2]);
+        const float lx = dot3_rn(q.rot[0], q.rot[3], q.rot[6], wx, wy, wz), ly = dot3_rn(q.rot[1], q.rot[4], q.rot[7], wx, wy, wz);
+        const float lz = dot3_rn(q.rot[2], q.rot[5], q.rot[8], wx, wy, wz);
+        const float rho = rev_rho(lx, lz);
+        float qr, qy;
+        bool in, keep;
+        rev_meridian(q.kind, q.sp[0], q.sp[1], rho, ly, qr, qy, in, keep);
+        if (in) return true;
+        const float dr = __fsub_rn(rho, qr), dy = __fsub_rn(ly, qy);
+        return __fsqrt_rn(__fadd_rn(__fmul_rn(dr, dr), __fmul_rn(dy, dy))) <= q.radius;
+    }
     if (!HF && q.kind == 0) {
         float ex = fmaxf(fmaxf(q.mins[0] - p.x, p.x - q.maxs[0]), 0.f);
         float ey = fmaxf(fmaxf(q.mins[1] - p.y, p.y - q.maxs[1]), 0.f);
@@ -1649,7 +1709,8 @@ __global__ void k_collider_impulse(uint32_t nb, const float4* __restrict__ bpos,
 // re-run with larger buffers when they overflow.  Every operation is an explicit round-to-nearest one, a fixed float32
 // expression a host can restate.
 struct ContactCollider {
-    int kind;                       // 1 ball (sp[0] radius), 2 cuboid (sp half extents), 3 capsule along local y (sp[0] half height, sp[1] radius), 4 heightfield
+    int kind;                       // 1 ball (sp[0] radius), 2 cuboid (sp half extents), 3 capsule along local y (sp[0] half height, sp[1] radius), 4 heightfield,
+                                    // 5 cylinder, 6 cone along local y (sp[0] half height, sp[1] radius)
     uint32_t slot;                  // collider slot: the samples' sort key
     float rot[9], t[3], sp[3];      // world = rot * local + t
     float mins[3], maxs[3];         // the posed shape's AABB loosened by h + prediction
@@ -1672,8 +1733,23 @@ __device__ __forceinline__ bool contact_in_box(const ContactCollider& c, int cx,
     return cx >= c.clo[0] && cx <= c.chi[0] && cy >= c.clo[1] && cy <= c.chi[1] && cz >= c.clo[2] && cz <= c.chi[2];
 }
 // project_point_and_get_feature, non-solid, in the shape's local frame: false when the projection is undefined (ball centre)
+template <bool REV>
 __device__ __forceinline__ bool contact_project_local(const ContactCollider& c, float lx, float ly, float lz, float* q, bool* inside) {
-    if (c.kind == 1) {  // parry Ball::project_local_point
+    if (REV && c.kind >= 5) {  // cylinder, cone: the meridian foot lifted along u = (x, z) / rho, along local +x at rho = 0
+        const float rho = rev_rho(lx, lz);
+        float qr, qy;
+        bool keep;
+        rev_meridian(c.kind, c.sp[0], c.sp[1], rho, ly, qr, qy, *inside, keep);
+        if (keep) {
+            q[0] = lx; q[2] = lz;
+        } else if (rho == 0.f) {
+            q[0] = qr; q[2] = 0.f;
+        } else {
+            const float s = __fdiv_rn(qr, rho);
+            q[0] = __fmul_rn(lx, s); q[2] = __fmul_rn(lz, s);
+        }
+        q[1] = qy;
+    } else if (c.kind == 1) {  // parry Ball::project_local_point
         const float n2 = dot3_rn(lx, ly, lz, lx, ly, lz);
         if (n2 == 0.f) return false;  // parry divides by zero here (NaN): no sample, no push
         *inside = n2 <= __fmul_rn(c.sp[0], c.sp[0]);
@@ -1750,8 +1826,9 @@ __device__ __forceinline__ void warp_bounds_commit(int* mn, int* mx, int bad, in
 // A particle is processed by the enumeration of the lowest-slot collider whose box holds its cell.  Records:
 // samples  s4[2r] = (proj, orig), s4[2r+1] = (velocity, 0), key[r] = slot << 32 | orig, val[r] = r;
 // pushes   p4[2r] = (new position, sorted slot), p4[2r+1] = (new velocity, 0).
-// HF: the instantiation for worlds with a heightfield collider; the others run k_contact_sample<false>, without its code.
-template <bool HF>
+// HF: the instantiations for worlds with a heightfield collider, REV: with a cylinder or cone collider; a world with
+// neither runs k_contact_sample<false, false>, without their code.
+template <bool HF, bool REV>
 __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                                  const uint32_t* __restrict__ orig, float4* __restrict__ s4, unsigned long long* __restrict__ key, uint32_t* __restrict__ val,
                                  float4* __restrict__ p4, int* __restrict__ res) {
@@ -1797,7 +1874,7 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
                         emit = hf_closest(P.hf[k], dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
                                           dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &d2);
                     } else {
-                        emit = contact_project_local(K, dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
+                        emit = contact_project_local<REV>(K,dot3_rn(K.rot[0], K.rot[3], K.rot[6], wx, wy, wz), dot3_rn(K.rot[1], K.rot[4], K.rot[7], wx, wy, wz),
                                                      dot3_rn(K.rot[2], K.rot[5], K.rot[8], wx, wy, wz), lq, &inside);
                     }
                 }
@@ -1921,7 +1998,7 @@ __global__ void k_contact_write(uint32_t n, const unsigned long long* __restrict
     oorig[d] = d;
 }
 
-template <bool HF>
+template <bool HF, bool REV>
 __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const uint32_t* __restrict__ cstart, const uint32_t* __restrict__ orig,
                              const float4* __restrict__ bpos, const uint32_t* __restrict__ bstart, const uint32_t* __restrict__ borig,
                              uint32_t* __restrict__ out, uint32_t cap, uint32_t* __restrict__ count) {
@@ -1934,7 +2011,7 @@ __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const u
     if (pos) {
         uint32_t s = max(cstart[c], q.slot_lo), e = min(cstart[c + 1], q.slot_hi);
         for (uint32_t j = s; j < e; ++j)
-            if (query_near<HF>(q, pos[j])) {
+            if (query_near<HF, REV>(q, pos[j])) {
                 uint32_t k = atomicAdd(count, 1u);
                 if (k < cap) {
                     out[2 * (size_t)k] = 0u;
@@ -1944,7 +2021,7 @@ __global__ void k_aabb_query(AabbQuery q,const float4* __restrict__ pos, const u
     }
     if (bpos) {
         for (uint32_t j = bstart[c]; j < bstart[c + 1]; ++j)
-            if (query_near<HF>(q, bpos[j])) {
+            if (query_near<HF, REV>(q, bpos[j])) {
                 uint32_t k = atomicAdd(count, 1u);
                 if (k < cap) {
                     out[2 * (size_t)k] = 1u;

@@ -6,8 +6,8 @@
 // j = (i + 1) % 3 and its columns along k = (i + 2) % 3; the first row of families 1 and 2 starts one step in, because the
 // reference's traversal does not reset that coordinate before its first row.
 //
-// Every ray is an axis-aligned line, so its crossings with the shape have closed forms: two for a ball, cuboid or capsule,
-// and for a heightfield a walk over the cells of the row (or column) strip the ray lies in, where the surface along the
+// Every ray is an axis-aligned line, so its crossings with the shape have closed forms: two for a ball, cuboid, capsule,
+// cylinder or cone (the cone's vertical pair, base and slant, is not symmetric), and for a heightfield a walk over the cells of the row (or column) strip the ray lies in, where the surface along the
 // ray is a polyline with a break on every cell edge and on every cell diagonal.  Each ray then runs the reference's loop:
 // the first crossing at or after the ray origin is the hit, impact = o + toi, the origin moves to o + (toi + sub / 10) and
 // entry / exit alternate.  k_sample_rays runs twice with the same code: once to count each ray's keys, once (after a scan)
@@ -23,7 +23,7 @@ constexpr unsigned long long SMP_KEY_MASK = SMP_KEY_LIM - 1;
 
 struct SampleRays {
     int kind, volume;
-    float p[4];                    // ball / cuboid / capsule parameters (sph_shape.p)
+    float p[4];                    // ball / cuboid / capsule / cylinder / cone parameters (sph_shape.p)
     float origin[3], sub, sub10;   // volume.mins + sub / 2, 2 * particle_rad, sub / 10
     const float* tab[3];           // ray coordinates along each axis (f32 running sums from origin)
     uint32_t n[3];                 // their counts
@@ -226,6 +226,36 @@ __global__ void __launch_bounds__(256) k_sample_rays(SampleRays P, unsigned long
                     const float dy = fmaxf(__fsub_rn(fabsf(y), P.p[0]), 0.f);
                     const float sq = __fsub_rn(r2, __fadd_rn(__fmul_rn(dy, dy), __fmul_rn(c, c)));
                     if (sq >= 0.f) smp_pair(__fsqrt_rn(sq), wk, s);
+                }
+                break;
+            }
+            case 5: {  // cylinder: |y| <= p0, x^2 + z^2 <= p1^2, closed
+                if (i == 1) {
+                    if (__fsub_rn(r2, __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck))) >= 0.f) smp_pair(P.p[0], wk, s);
+                } else {
+                    const float y = i == 0 ? cj : ck, c = i == 0 ? ck : cj;
+                    const float sq = __fsub_rn(r2, __fmul_rn(c, c));
+                    if (fabsf(y) <= P.p[0] && sq >= 0.f) smp_pair(__fsqrt_rn(sq), wk, s);
+                }
+                break;
+            }
+            case 6: {  // cone: apex (0, p0, 0), base disc of radius p1 at y = -p0; radius R(y) = p1 (p0 - y) / (2 p0)
+                const float a = P.p[0], a2 = __fadd_rn(a, a);
+                if (i == 1) {  // the base, then the slant at y = a - 2a rho / r (a at rho = 0, -a at the rim)
+                    const float c2 = __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck));
+                    if (__fsub_rn(r2, c2) >= 0.f) {
+                        const float rho = __fsqrt_rn(c2);
+                        const float f = rho == 0.f ? 0.f : fminf(__fdiv_rn(rho, P.p[1]), 1.f);
+                        wk.hit(-a, s);
+                        wk.hit(__fsub_rn(a, __fmul_rn(a2, f)), s);
+                    }
+                } else {
+                    const float y = i == 0 ? cj : ck, c = i == 0 ? ck : cj;
+                    if (fabsf(y) <= a) {
+                        const float R = a == 0.f ? P.p[1] : __fdiv_rn(__fmul_rn(P.p[1], __fsub_rn(a, y)), a2);
+                        const float sq = __fsub_rn(__fmul_rn(R, R), __fmul_rn(c, c));
+                        if (sq >= 0.f) smp_pair(__fsqrt_rn(sq), wk, s);
+                    }
                 }
                 break;
             }

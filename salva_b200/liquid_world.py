@@ -164,6 +164,22 @@ class Capsule:
         self.params = [half_height, radius]
 
 
+class Cylinder:
+    """parry Cylinder along local y: half_height, radius (sqrt(x^2 + z^2) <= radius, |y| <= half_height)"""
+    kind = 5
+
+    def __init__(self, half_height, radius):
+        self.params = [half_height, radius]
+
+
+class Cone:
+    """parry Cone along local y: half_height, base radius; the apex at (0, half_height, 0), the base disc at y = -half_height"""
+    kind = 6
+
+    def __init__(self, half_height, radius):
+        self.params = [half_height, radius]
+
+
 class StaticSampling:
     """ColliderSampling::StaticSampling(points) (fluids_pipeline.rs:64-69): the collider approximated by sample points given
     in its local frame."""
@@ -175,7 +191,7 @@ class StaticSampling:
 
 class DynamicContactSampling:
     """ColliderSampling::DynamicContactSampling (fluids_pipeline.rs:71, 192-255): every step the collider's shape (Ball,
-    Cuboid, Capsule or sampling.HeightField) is sampled where the fluid is about to touch it, and penetrating fluid particles
+    Cuboid, Capsule, Cylinder, Cone or sampling.HeightField) is sampled where the fluid is about to touch it, and penetrating fluid particles
     are pushed out.  A heightfield never pushes (parry's heightfield point query has is_inside always false): it only samples."""
     kind = 1
 
@@ -481,7 +497,7 @@ class LiquidWorld:
         return p, v
 
     def particles_intersecting_shape(self, shape, translation=(0.0, 0.0, 0.0), rotation=None):
-        """liquid_world.rs:246-281 for Ball / Cuboid / Capsule / sampling.HeightField under the isometry (rotation 3x3
+        """liquid_world.rs:246-281 for Ball / Cuboid / Capsule / Cylinder / Cone / sampling.HeightField under the isometry (rotation 3x3
         row-major, translation)."""
         if shape.kind == HEIGHTFIELD:
             sh = heightfield_c(shape)

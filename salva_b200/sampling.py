@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 
 from . import _lib
-from .liquid_world import Ball, Capsule, Cuboid, heightfield_c  # noqa: F401  (the shapes the sampler takes, with HeightField)
+from .liquid_world import Ball, Capsule, Cone, Cuboid, Cylinder, heightfield_c  # noqa: F401  (the shapes the sampler takes, with HeightField)
 
 SURFACE, VOLUME = 0, 1  # SPH_SAMPLE_*
 
@@ -48,7 +48,7 @@ def _ray_sample(world, shape, particle_rad, method):
 
 
 def shape_surface_ray_sample(world, shape, particle_rad):
-    """ray_sampling.rs:9-15: points on the surface of `shape` (Ball, Cuboid, Capsule or HeightField)."""
+    """ray_sampling.rs:9-15: points on the surface of `shape` (Ball, Cuboid, Capsule, Cylinder, Cone or HeightField)."""
     return _ray_sample(world, shape, particle_rad, SURFACE)
 
 

@@ -3,6 +3,7 @@ CouplingManager (salva_b200.contact_sampling.ContactSamplingHook through step_wi
 
 C2: the 1M-particle dam break (DFSPH + XSPH) with a 0.6 m cuboid on a dynamic body that moves through the block every step.
 Droplet: examples/contact_sampling3.cpp's scene (surface_tension3.rs, a 7^3 droplet on a fixed cuboid ground).
+C2 again with a moving cylinder and a moving cone, after the two scenes above, whose output does not change.
 The variants of a scene are stepped alternately in one process; the card, its power limit and SM clock are read in the
 same run.  Prints one JSON line per scene: median step ms (CUDA events), median wall ms and kernels per step.
 
@@ -20,7 +21,7 @@ import numpy as np
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from salva_b200 import BODY_DYNAMIC, BODY_FIXED, DFSPHSolver, DynamicContactSampling, LiquidWorld, scenes  # noqa: E402
 from salva_b200.contact_sampling import ContactSamplingHook  # noqa: E402
-from salva_b200.liquid_world import Cuboid  # noqa: E402
+from salva_b200.liquid_world import Cone, Cuboid, Cylinder  # noqa: E402
 
 F32 = np.float32
 
@@ -129,6 +130,9 @@ def main():
     print(json.dumps(dict(scene="contact_sampling3 droplet", gpu=gpu, **run(
         scene_variants(make_drop, Cuboid((0.15, 0.02, 0.15)), drop_state, 1.0 / 200.0, (0.0, -0.981, 0.0)), 1.0 / 200.0, (0.0, -0.981, 0.0),
         a.steps, a.warmup))), flush=True)
+    for shape, label in ((Cylinder(0.3, 0.3), "cylinder"), (Cone(0.3, 0.3), "cone")):  # k_contact_sample<false, true>
+        print(json.dumps(dict(scene="C2-%d moving 0.6 m %s" % (a.c2 ** 3, label), gpu=gpu, **run(
+            scene_variants(make_c2, shape, c2_state, c2["dt"], c2["gravity"]), c2["dt"], c2["gravity"], a.steps, a.warmup))), flush=True)
     print(json.dumps(dict(gpu_after=card())))
 
 

@@ -49,7 +49,9 @@ def main():
     r = 2.0 ** -7
     work = [("heightfield3_ground_surface", S.HeightField(ground(), (12.0, 1.0, 12.0)), 0.1, False),
             ("heightfield_1000x1000_surface", S.HeightField(big, (100.0, 4.0, 100.0)), 0.05, False),
-            ("cuboid_10M_volume", S.Cuboid([215 * r, 216 * r, 217 * r]), r, True)]
+            ("cuboid_10M_volume", S.Cuboid([215 * r, 216 * r, 217 * r]), r, True),
+            ("cylinder_volume", S.Cylinder(1.0, 0.5), 0.005, True),
+            ("cone_surface", S.Cone(1.0, 0.8), 0.002, False)]
     w = LiquidWorld(particle_radius=0.05)
     res = {"card": card(), "workloads": []}
     for name, shape, rad, vol in work:
