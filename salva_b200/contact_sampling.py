@@ -1,6 +1,6 @@
 """DynamicContactSampling (fluids_pipeline.rs:192-255) restated in numpy float32.
 
-Every operation below is one float32 operation in the order k_contact_sample (csrc/sph_kernels.cuh) performs it, so the
+Every operation below is one float32 operation in the order k_contact_sample (csrc/sph_shapes.cuh) performs it, so the
 restatement is bit-identical to the device path.  ContactSamplingHook runs it as a host CouplingManager, through
 LiquidWorld.step_with_coupling: the way to contact-sample without the device path, and the yardstick the device path is
 checked and timed against.
@@ -20,7 +20,7 @@ def _dot(a0, a1, a2, b0, b1, b2):
 
 
 def hf_grid(heights, scale):
-    """The host constants of a heightfield (sph_engine.cu hf_check): half extents, cell sizes, height scale, the scaled
+    """The host constants of a heightfield (csrc/sph_colliders_host.inl hf_check): half extents, cell sizes, height scale, the scaled
     height range."""
     H = np.ascontiguousarray(heights, F32)
     sx, sy, sz = (F32(x) for x in scale)
@@ -50,7 +50,7 @@ def posed_aabb(kind, params, rotation, translation, hf=None):
     p = np.zeros(4, F32)
     p[:len(params)] = np.asarray(params, F32)
     t = np.asarray(translation, F32)
-    if kind in (CYLINDER, CONE):  # rev_posed_aabb: parry's tight support-map box
+    if kind in (CYLINDER, CONE):  # parry's tight support-map box
         mins, maxs = np.empty(3, F32), np.empty(3, F32)
         a, r = p[0], p[1]
         for i in range(3):

@@ -20,6 +20,7 @@
 
 #include "../../include/sph.h"
 #include "sph_kernels.cuh"
+#include "sph_shapes.cuh"
 #include "sph_passes.cuh"
 #include "sph_tile.cuh"
 #include "sph_iisph.cuh"
@@ -143,6 +144,11 @@ void elasticity_release(ForceRec& fr);
 sph_status elasticity_restore(sph_world* w, ForceRec& fr, size_t n, uint32_t cap0, uint32_t stride0, const char* blob);
 sph_status viscosity_solve(sph_world* w, uint32_t fluid, ForceRec& fr);
 void viscosity_release(sph_world* w);
+bool any_collider(const sph_world* w);
+bool any_contact(const sph_world* w);
+sph_status colliders_update(sph_world* w, bool reposed_all);
+sph_status colliders_contact(sph_world* w);
+sph_status colliders_impulse(sph_world* w);
 inline float __uint_as_float_host(uint32_t u) {
     float f;
     memcpy(&f, &u, sizeof f);
@@ -684,368 +690,6 @@ sph_status pull_boundaries(sph_world* w) {
     CU(cudaStreamSynchronize(w->st));
     w->hb_stale = false;
     return SPH_OK;
-}
-
-inline int collider_slot(const sph_world* w, uint32_t handle) {
-    const uint32_t slot = handle & 0xFFFFu;
-    if (slot >= w->colliders.size() || !w->colliders[slot].alive || (w->colliders[slot].gen & 0xFFFFu) != (handle >> 16)) return -1;
-    return (int)slot;
-}
-// a live collider whose boundary exists (a removed boundary leaves its collider inert)
-bool any_collider(const sph_world* w) {
-    for (const ColliderRec& c : w->colliders)
-        if (c.alive && boundary_slot(w, c.boundary) >= 0) return true;
-    return false;
-}
-bool boundary_coupled(const sph_world* w, uint32_t boundary) {
-    for (const ColliderRec& c : w->colliders)
-        if (c.alive && boundary_slot(w, c.boundary) == (int)boundary) return true;
-    return false;
-}
-
-// ColliderCouplingManager::update_boundaries (fluids_pipeline.rs:151-261) for StaticSampling colliders.  Their samples do not
-// depend on the fluid, so they are posed before the step's grid is sized: the grid then covers them.  `reposed_all`: the
-// boundaries were just uploaded from the host copy, which holds the points of registration, not the posed ones.
-sph_status colliders_update(sph_world* w, bool reposed_all) {
-    const size_t B = w->B;
-    bool moved = false;
-    for (ColliderRec& c : w->colliders) {
-        if (!c.alive) continue;
-        const int bs = boundary_slot(w, c.boundary);
-        if (bs < 0) continue;  // boundaries.get_mut finds nothing (:159-162)
-        BoundaryRec& b = w->bounds[bs];
-        if (c.state.body == SPH_BODY_FIXED) b.want_forces = false;  // :163-171
-        else if (c.state.body == SPH_BODY_DYNAMIC) b.want_forces = true;
-        if (!reposed_all && c.applied_valid && memcmp(&c.state, &c.applied, sizeof c.state) == 0) continue;
-        ColliderPose P;
-        memcpy(P.rot, c.state.rotation_rowmajor, sizeof P.rot);
-        memcpy(P.t, c.state.translation, sizeof P.t);
-        memcpy(P.linvel, c.state.linvel, sizeof P.linvel);
-        memcpy(P.angvel, c.state.angvel, sizeof P.angvel);
-        memcpy(P.com, c.state.world_com, sizeof P.com);
-        P.moving = c.state.body != SPH_BODY_NONE;
-        const int bc = w->bcur;
-        if (c.n) LAUNCH(k_collider_static, B, 256, (uint32_t)B, w->borig[bc].p, (uint32_t)b.offset, (uint32_t)c.n, c.local.p, P, w->bpos[bc].p, w->bvel[bc].p);
-        c.applied = c.state;
-        c.applied_valid = true;
-        moved = moved || c.n;
-    }
-    if (!moved) return SPH_OK;
-    // the boundary AABB sizes the grid (phase_grid): recompute it from the device particles, the step's one collider sync
-    static const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
-    CU(w->d_cb.ensure(8));
-    CU(cudaMemcpyAsync(w->d_cb.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
-    k_bounds<<<std::min<uint32_t>(cdiv(B, 256), 296), 256, 0, w->st>>>(w->bpos[w->bcur].p, (uint32_t)B, w->d_cb.p);
-    w->launches++;
-    int hb[7];
-    CU(cudaMemcpyAsync(hb, w->d_cb.p, sizeof hb, cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
-    memcpy(w->b_aabb, hb, sizeof w->b_aabb);
-    w->b_bad = hb[6] != 0;
-    w->b_sorted_valid = false;  // re-sort the boundaries and recompute their volumes
-    w->hb_stale = true;
-    return SPH_OK;
-}
-
-// transmit_forces (fluids_pipeline.rs:263-287): enqueued after the solve; the impulses come back with the step's final read-back
-sph_status colliders_impulse(sph_world* w) {
-    ImpulseTable T;
-    for (int b = 0; b < MAX_BOUNDARIES; ++b) T.collider[b] = -1;
-    bool any = false;
-    for (size_t k = 0; k < w->colliders.size(); ++k) {
-        ColliderRec& c = w->colliders[k];
-        const int bs = c.alive ? boundary_slot(w, c.boundary) : -1;
-        if (bs < 0 || c.state.body != SPH_BODY_DYNAMIC || !w->bounds[bs].want_forces || w->bounds[bs].n == 0) continue;
-        T.collider[bs] = (int)k;
-        memcpy(T.com[k], c.state.world_com, sizeof T.com[k]);
-        c.impulse_pending = any = true;
-    }
-    if (!any) return SPH_OK;
-    const size_t bytes = 6 * w->colliders.size() * sizeof(float);
-    CU(cudaMemsetAsync(w->d_imp.p, 0, bytes, w->st));
-    k_collider_impulse<<<std::min<uint32_t>(cdiv(w->B, 256), 264), 256, 0, w->st>>>((uint32_t)w->B, w->bpos[w->bcur].p, w->bvel[w->bcur].p, w->bforce.p,
-                                                                                   w->dt, T, w->d_imp.p);
-    w->launches++;
-    CU(cudaMemcpyAsync(w->h_imp, w->d_imp.p, bytes, cudaMemcpyDeviceToHost, w->st));
-    return SPH_OK;
-}
-
-// Half extents of the AABB of a ball / cuboid / capsule (segment along local y) under the rotation R: the box parry's
-// compute_aabb(pos) centres on the translation.
-void posed_aabb_ext(const sph_shape& s, const float R[9], float ext[3]) {
-    for (int a = 0; a < 3; ++a) {
-        if (s.kind == SPH_SHAPE_BALL) ext[a] = s.p[0];
-        else if (s.kind == SPH_SHAPE_CUBOID) ext[a] = std::fabs(R[3 * a]) * s.p[0] + std::fabs(R[3 * a + 1]) * s.p[1] + std::fabs(R[3 * a + 2]) * s.p[2];
-        else ext[a] = std::fabs(R[3 * a + 1]) * s.p[0] + s.p[1];  // the segment, swept by the radius
-    }
-}
-
-// compute_aabb(pos) of a cylinder or cone (a = p[0], r = p[1], axis along local y): parry's support-map box, which is tight.
-// With s_i = |(R_i0, R_i2)|, the cylinder's box is centred on t with half extents a |R_i1| + r s_i; the cone's apex
-// t + a R_1 and base rim give max_i = t_i + max(a R_i1, -a R_i1 + r s_i), min_i = t_i + min(a R_i1, -a R_i1 - r s_i).
-void rev_posed_aabb(const sph_shape& s, const float R[9], const float t[3], float mins[3], float maxs[3]) {
-    const float a = s.p[0], r = s.p[1];
-    for (int i = 0; i < 3; ++i) {
-        const float si = std::sqrt(R[3 * i] * R[3 * i] + R[3 * i + 2] * R[3 * i + 2]);
-        const float ay = a * R[3 * i + 1], rs = r * si;
-        if (s.kind == SPH_SHAPE_CYLINDER) {
-            const float ext = std::fabs(R[3 * i + 1]) * a + rs;
-            mins[i] = t[i] - ext;
-            maxs[i] = t[i] + ext;
-        } else {
-            mins[i] = t[i] + std::fmin(ay, -ay - rs);
-            maxs[i] = t[i] + std::fmax(ay, -ay + rs);
-        }
-    }
-}
-bool is_rev(int kind) { return kind == SPH_SHAPE_CYLINDER || kind == SPH_SHAPE_CONE; }
-// parameters a shape kind reads from sph_shape.p (0: unknown kind, or a heightfield)
-int shape_nparams(int kind) {
-    return kind == SPH_SHAPE_BALL ? 1 : kind == SPH_SHAPE_CUBOID ? 3 : kind == SPH_SHAPE_CAPSULE || is_rev(kind) ? 2 : 0;
-}
-
-// The heightfield checks of sph_world_sample_shape, shared by every entry point that takes one: 2 x 2 or more, finite
-// heights, a finite positive scale.  Fills the grid constants and the scaled height range [*ylo, *yhi].
-sph_status hf_check(sph_world* w, const sph_heightfield* hf, std::vector<float>& heights, HfGrid& g, float* ylo, float* yhi) {
-    if (!hf || !hf->heights) return w->fail(SPH_ERR_INVALID, "a heightfield shape needs its sph_heightfield");
-    if (hf->nrows < 2 || hf->ncols < 2)
-        return w->fail(SPH_ERR_INVALID, "heightfield needs at least 2 rows and 2 columns (got %u x %u)", hf->nrows, hf->ncols);
-    for (int a = 0; a < 3; ++a)
-        if (!(std::isfinite(hf->scale[a]) && hf->scale[a] > 0.f))
-            return w->fail(SPH_ERR_INVALID, "heightfield scale[%d] must be finite and > 0 (got %g)", a, (double)hf->scale[a]);
-    const size_t cnt = (size_t)hf->nrows * hf->ncols;
-    heights.assign(hf->heights, hf->heights + cnt);
-    float lo = heights[0], hi = heights[0];
-    for (size_t q = 0; q < cnt; ++q) {
-        if (!std::isfinite(heights[q])) return w->fail(SPH_ERR_INVALID, "heightfield height %zu is not finite", q);
-        lo = std::min(lo, heights[q]);
-        hi = std::max(hi, heights[q]);
-    }
-    memset(&g, 0, sizeof g);
-    g.nrows = (int)hf->nrows;
-    g.ncols = (int)hf->ncols;
-    g.hx = hf->scale[0] * 0.5f;
-    g.hz = hf->scale[2] * 0.5f;
-    g.sy = hf->scale[1];
-    g.dx = hf->scale[0] / (float)(hf->ncols - 1);
-    g.dz = hf->scale[2] / (float)(hf->nrows - 1);
-    g.dmin = std::min(g.dx, g.dz);
-    *ylo = lo * g.sy;
-    *yhi = hi * g.sy;
-    if (!std::isfinite(*ylo) || !std::isfinite(*yhi)) return w->fail(SPH_ERR_INVALID, "heightfield heights overflow once scaled");
-    return SPH_OK;
-}
-
-// The search cap of hf_closest and its margin M = 2^-10 (sx/2 + sz/2 + max |y| + cap): far above the float32 error of any
-// distance the routine computes for a point within the cap (DESIGN.md section 10).
-void hf_set_cap(HfGrid& g, float ylo, float yhi, float cap) {
-    g.cap2 = cap * cap;
-    g.margin = (((g.hx + g.hz) + std::max(std::fabs(ylo), std::fabs(yhi))) + cap) * 0.0009765625f;
-}
-
-// compute_aabb(pos) of a heightfield: Aabb::transform_by, centre R c + t and half extents |R| e, where the local box
-// [-sx/2, ylo, -sz/2]-[sx/2, yhi, sz/2] is centred on c = (0, (ylo + yhi) / 2, 0), not on the origin.
-void hf_posed_aabb(const HfGrid& g, float ylo, float yhi, const float R[9], const float t[3], float mins[3], float maxs[3]) {
-    const float cy = (ylo + yhi) * 0.5f, ey = (yhi - ylo) * 0.5f;
-    for (int a = 0; a < 3; ++a) {
-        const float ext = (std::fabs(R[3 * a]) * g.hx + std::fabs(R[3 * a + 1]) * ey) + std::fabs(R[3 * a + 2]) * g.hz;
-        const float c = R[3 * a + 1] * cy + t[a];
-        mins[a] = c - ext;
-        maxs[a] = c + ext;
-    }
-}
-
-sph_status phase_grid(sph_world* w);
-
-bool any_contact(const sph_world* w) {
-    for (const ColliderRec& c : w->colliders)
-        if (c.alive && c.sampling == SPH_SAMPLING_CONTACT && boundary_slot(w, c.boundary) >= 0) return true;
-    return false;
-}
-
-// ColliderCouplingManager::update_boundaries (fluids_pipeline.rs:192-255) for DynamicContactSampling colliders.  Runs after
-// the fluid sort of phase_grid, where a host CouplingManager runs (liquid_world.rs:90-103): k_contact_sample finds the
-// candidates in each collider's cell box and appends sample and push records; the pushes are applied and the cell bounds of
-// the fluid and of the new boundary set reduced, and ONE read-back brings the counts and bounds to the host.  Then, with
-// nothing more read back, the samples are radix-sorted by (collider slot, original fluid index), the boundary arrays are
-// rebuilt in original order (the other boundaries un-sorted through borig to their new offsets) and the grid is rebuilt
-// from the bounds already read back: the pushes moved particles, and the re-sort also refreshes v* = vel + vc.
-sph_status colliders_contact(sph_world* w) {
-    const size_t N = w->N, B = w->B;
-    const Consts& hc = w->hc;
-    const int xs = hc.xysub > 0 ? hc.xysub : 1;  // the grid counts x and y in bins of h / xysub
-    const int go[3] = {hc.ox / xs, hc.oy / xs, hc.oz}, gn[3] = {hc.nx / xs, hc.ny / xs, hc.nz};
-    const float h = w->h, prediction = h * 0.5f, cut = h + prediction, margin = w->desc.particle_radius * 0.1f;
-    std::vector<ContactCollider> cc;
-    std::vector<HfGrid> chf;
-    unsigned long long skip = 0;
-    size_t bins = 0;
-    bool any_hf = false, any_rev = false;
-    for (size_t k = 0; k < w->colliders.size(); ++k) {
-        const ColliderRec& c = w->colliders[k];
-        if (!c.alive || c.sampling != SPH_SAMPLING_CONTACT) continue;
-        const int bs = boundary_slot(w, c.boundary);
-        if (bs < 0) continue;
-        skip |= 1ull << bs;
-        ContactCollider K;
-        memset(&K, 0, sizeof K);
-        K.kind = c.shape.kind;
-        K.slot = (uint32_t)k;
-        memcpy(K.rot, c.state.rotation_rowmajor, sizeof K.rot);
-        memcpy(K.t, c.state.translation, sizeof K.t);
-        for (int a = 0; a < 3; ++a) K.sp[a] = c.shape.p[a];
-        memcpy(K.linvel, c.state.linvel, sizeof K.linvel);
-        memcpy(K.angvel, c.state.angvel, sizeof K.angvel);
-        memcpy(K.com, c.state.world_com, sizeof K.com);
-        K.moving = c.state.body != SPH_BODY_NONE;
-        float lo[3], hi[3];  // compute_aabb(pos)
-        chf.push_back(c.hf);
-        if (c.shape.kind == SPH_SHAPE_HEIGHTFIELD) {
-            hf_set_cap(chf.back(), c.hf_ylo, c.hf_yhi, cut);
-            hf_posed_aabb(c.hf, c.hf_ylo, c.hf_yhi, K.rot, K.t, lo, hi);
-            any_hf = true;
-        } else if (is_rev(c.shape.kind)) {
-            rev_posed_aabb(c.shape, K.rot, K.t, lo, hi);
-            any_rev = true;
-        } else {
-            float ext[3];
-            posed_aabb_ext(c.shape, K.rot, ext);
-            for (int a = 0; a < 3; ++a) {
-                lo[a] = K.t[a] - ext[a];
-                hi[a] = K.t[a] + ext[a];
-            }
-        }
-        size_t nbin = 1;
-        for (int a = 0; a < 3; ++a) {
-            K.mins[a] = lo[a] - cut;  // .loosened(h + prediction)
-            K.maxs[a] = hi[a] + cut;
-            // hgrid.rs:41-52 keys; clamped where no particle can be (k_bounds refuses |cell| >= 1e9)
-            const float flo = std::fmin(std::fmax(std::floor(K.mins[a] / h), -1.5e9f), 1.5e9f);
-            const float fhi = std::fmin(std::fmax(std::floor(K.maxs[a] / h), -1.5e9f), 1.5e9f);
-            K.clo[a] = (int)flo;
-            K.chi[a] = (int)fhi;
-            const int lo = std::max(K.clo[a], go[a]), hi = std::min(K.chi[a], go[a] + gn[a] - 1);
-            const int sub = a < 2 ? xs : 1;
-            K.bl[a] = lo * sub;
-            K.bd[a] = hi < lo ? 0 : (hi - lo + 1) * sub;
-            nbin *= (size_t)K.bd[a];
-        }
-        K.first_bin = (uint32_t)bins;
-        bins += nbin;
-        if (bins > (size_t)(UINT32_MAX / 64)) return w->fail(SPH_ERR_OOM, "contact sampling: collider cell boxes too large");
-        cc.push_back(K);
-    }
-    const int nc = (int)cc.size();
-    CU(w->d_ccol.ensure(nc));
-    CU(cudaMemcpyAsync(w->d_ccol.p, cc.data(), nc * sizeof(ContactCollider), cudaMemcpyHostToDevice, w->st));
-    if (any_hf) {
-        CU(w->d_chf.ensure(nc));
-        CU(cudaMemcpyAsync(w->d_chf.p, chf.data(), nc * sizeof(HfGrid), cudaMemcpyHostToDevice, w->st));
-    }
-    constexpr int NRES = CS_PER_COLLIDER + MAX_BOUNDARIES;
-    int init[NRES] = {};
-    for (int base : {CS_FLUID_BOUNDS, CS_BOUND_BOUNDS})
-        for (int a = 0; a < 3; ++a) {
-            init[base + a] = INT_MAX;
-            init[base + 3 + a] = INT_MIN;
-        }
-    int res[NRES];
-    CU(w->d_cres.ensure(NRES));
-    const int c = w->cur, bc = w->bcur;
-    for (;;) {
-        CU(w->cs_s4.ensure(2 * (size_t)w->cap_s));
-        CU(w->cs_key[0].ensure(w->cap_s));
-        CU(w->cs_val[0].ensure(w->cap_s));
-        CU(w->cs_p4.ensure(2 * (size_t)w->cap_p));
-        CU(cudaMemcpyAsync(w->d_cres.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
-        if (N && bins) {
-            ContactParams P{w->d_ccol.p, nc, (uint32_t)bins, w->dt, cut, margin, w->cap_s, w->cap_p, any_hf ? w->d_chf.p : nullptr};
-            const auto kern = any_hf ? (any_rev ? k_contact_sample<true, true> : k_contact_sample<true, false>)
-                                     : (any_rev ? k_contact_sample<false, true> : k_contact_sample<false, false>);
-            LAUNCH(kern, 32 * bins, 256, P, w->pos[c].p, w->vel[c].p, w->cstart.p, w->orig[c].p, w->cs_s4.p, w->cs_key[0].p, w->cs_val[0].p,
-                   w->cs_p4.p, w->d_cres.p);
-            k_contact_apply<<<std::min<uint32_t>(cdiv(w->cap_p, 256), 264), 256, 0, w->st>>>(w->cs_p4.p, w->d_cres.p, w->cap_s, w->cap_p, w->pos[c].p,
-                                                                                         w->vel[c].p);
-            w->launches++;
-        }
-        if (N) {
-            k_bounds<<<std::min<uint32_t>(cdiv(N, 256), 296), 256, 0, w->st>>>(w->pos[c].p, (uint32_t)N, w->d_cres.p + CS_FLUID_BOUNDS);
-            w->launches++;
-        }
-        if (B) {
-            k_bounds_kept<<<std::min<uint32_t>(cdiv(B, 256), 296), 256, 0, w->st>>>(w->bpos[bc].p, w->bvel[bc].p, (uint32_t)B, skip,
-                                                                                   w->d_cres.p + CS_BOUND_BOUNDS);
-            w->launches++;
-        }
-        CU(cudaMemcpyAsync(res, w->d_cres.p, sizeof res, cudaMemcpyDeviceToHost, w->st));
-        CU(cudaStreamSynchronize(w->st));  // the step's one contact-sampling round trip
-        const uint32_t ns = (uint32_t)res[CS_SAMPLES], np = (uint32_t)res[CS_PUSHES];
-        if (ns <= w->cap_s && np <= w->cap_p) break;
-        // nothing was written to the fluid: re-run with room for every record
-        w->cap_s = std::max(w->cap_s, ns + ns / 4);
-        w->cap_p = std::max(w->cap_p, np + np / 4);
-    }
-    const uint32_t M = (uint32_t)res[CS_SAMPLES];
-    // the coupled boundaries' new sizes and everyone's new offsets
-    ContactRebuild T;
-    memset(&T, 0, sizeof T);
-    T.skip = skip;
-    for (size_t b = 0; b < w->bounds.size(); ++b) T.old_off[b] = (uint32_t)w->bounds[b].offset;
-    for (size_t k = 0; k < w->colliders.size(); ++k) {
-        const ColliderRec& cr = w->colliders[k];
-        const int bs = cr.alive && cr.sampling == SPH_SAMPLING_CONTACT ? boundary_slot(w, cr.boundary) : -1;
-        if (bs >= 0) w->bounds[bs].n = (size_t)res[CS_PER_COLLIDER + k];
-    }
-    recompute_offsets(w);
-    for (size_t b = 0; b < w->bounds.size(); ++b) T.new_off[b] = (uint32_t)w->bounds[b].offset;
-    uint32_t first = 0;
-    for (size_t k = 0; k < w->colliders.size(); ++k) {
-        const ColliderRec& cr = w->colliders[k];
-        const int bs = cr.alive && cr.sampling == SPH_SAMPLING_CONTACT ? boundary_slot(w, cr.boundary) : -1;
-        if (bs < 0) continue;
-        T.col_first[k] = first;
-        T.col_dst[k] = (uint32_t)w->bounds[bs].offset;
-        T.col_bslot[k] = (uint32_t)bs;
-        first += (uint32_t)res[CS_PER_COLLIDER + k];
-    }
-    const size_t NB = w->B;
-    const int nbc = bc ^ 1;
-    CU(w->bpos[bc].ensure(NB, true, w->st));  // the source of the rebuild, the target of the next boundary sort
-    CU(w->bvel[bc].ensure(NB, true, w->st));
-    CU(w->borig[bc].ensure(NB, true, w->st));
-    CU(w->bpos[nbc].ensure(NB));
-    CU(w->bvel[nbc].ensure(NB));
-    CU(w->borig[nbc].ensure(NB));
-    CU(w->bvol.ensure(NB));
-    CU(w->bcid.ensure(NB));
-    CU(w->brank.ensure(NB));
-    CU(w->bperm.ensure(NB));
-    CU(w->bforce.ensure(3 * NB));
-    if (M) {
-        CU(w->cs_key[1].ensure(M));
-        CU(w->cs_val[1].ensure(M));
-        const int end_bit = 32 + 6;  // collider slots < MAX_BOUNDARIES = 64
-        size_t tmp = 0;
-        CU(cub::DeviceRadixSort::SortPairs(nullptr, tmp, w->cs_key[0].p, w->cs_key[1].p, w->cs_val[0].p, w->cs_val[1].p, (int)M, 0, end_bit, w->st));
-        CU(w->cs_tmp.ensure(tmp));
-        CU(cub::DeviceRadixSort::SortPairs(w->cs_tmp.p, tmp, w->cs_key[0].p, w->cs_key[1].p, w->cs_val[0].p, w->cs_val[1].p, (int)M, 0, end_bit,
-                                           w->st));
-        w->launches++;  // (CUB's passes count as one)
-    }
-    LAUNCH(k_contact_keep, B, 256, (uint32_t)B, w->bpos[bc].p, w->bvel[bc].p, w->borig[bc].p, T, w->bpos[nbc].p, w->bvel[nbc].p, w->borig[nbc].p);
-    LAUNCH(k_contact_write, M, 256, M, w->cs_key[1].p, w->cs_val[1].p, w->cs_s4.p, T, w->bpos[nbc].p, w->bvel[nbc].p, w->borig[nbc].p);
-    w->bcur = nbc;
-    memcpy(w->b_aabb, res + CS_BOUND_BOUNDS, sizeof w->b_aabb);
-    w->b_bad = res[CS_BOUND_BOUNDS + 6] != 0;
-    memcpy(w->nb, res + CS_FLUID_BOUNDS, sizeof w->nb);
-    w->nb_valid = N > 0;  // phase_grid sizes the grid from these bounds, without a bounds pass of its own
-    w->b_sorted_valid = false;
-    w->lists_valid = false;
-    w->hb_pos.resize(3 * NB);
-    w->hb_vel.resize(3 * NB);
-    w->hb_stale = true;
-    w->stats.n_boundary_particles = NB;
-    return phase_grid(w);
 }
 
 // fluid.rs:88-98 apply_particles_removal (+ solver scratch filtering dfsph_solver.rs:550-559)
@@ -2153,6 +1797,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 #include "sph_iisph_host.inl"
 #include "sph_elasticity_host.inl"
 #include "sph_viscosity_host.inl"
+#include "sph_colliders_host.inl"
 
 // ===================================================================================================
 // extern "C" boundary
@@ -2538,82 +2183,6 @@ sph_status sph_boundary_read_volumes(sph_world* w, uint32_t boundary, float* vol
     return boundary_export(w, boundary, volumes, cap, false);
 }
 
-// Shared runner of particles_intersecting_aabb / particles_intersecting_shape: the cells [key(mins), key(maxs)] of the last
-// step's grid (hgrid.rs:122-133), every particle in them tested by query_near().
-static sph_status run_query(sph_world* w, AabbQuery q, const float mins[3], const float maxs[3], uint32_t* kinds, uint32_t* handles, uint32_t* indices,
-                            size_t cap, size_t* n) {
-    *n = 0;
-    if (!w->grid_ready) {
-        if (!w->ever_stepped) return SPH_OK;  // no step yet: the reference's grid is empty
-        return w->fail(SPH_ERR_INVALID, "particle query: host edits are pending; the last step's cell grid no longer describes the particles");
-    }
-    if (w->b_dirty && !w->in_coupling) return w->fail(SPH_ERR_INVALID, "particle query: a boundary rewrite is pending; step first");
-    for (int a = 0; a < 3; ++a)
-        if (std::isnan(mins[a]) || std::isnan(maxs[a])) return w->fail(SPH_ERR_INVALID, "particle query: NaN bounds");
-    TRY(enter(w));
-    const Consts& hc = w->hc;
-    int lo[3], hi[3];
-    const int xs = hc.xysub > 0 ? hc.xysub : 1;  // the grid counts x and y in bins of h / xysub; the query box is in cells
-    const int go[3] = {hc.ox / xs, hc.oy / xs, hc.oz}, gn[3] = {hc.nx / xs, hc.ny / xs, hc.nz};
-    for (int a = 0; a < 3; ++a) {  // hgrid.rs:41-52 keys, clipped IN FLOAT to the dense grid (cells outside hold nothing; +-inf / FLT_MAX bounds are legal)
-        const float flo = std::floor(mins[a] / w->h), fhi = std::floor(maxs[a] / w->h);
-        if (fhi < (float)go[a] || flo > (float)(go[a] + gn[a] - 1)) return SPH_OK;
-        lo[a] = (int)std::fmax(flo, (float)go[a]);
-        hi[a] = (int)std::fmin(fhi, (float)(go[a] + gn[a] - 1));
-        if (hi[a] < lo[a]) return SPH_OK;
-    }
-    q.lx = lo[0] * xs; q.ly = lo[1] * xs; q.lz = lo[2];
-    q.dx = (hi[0] - lo[0] + 1) * xs; q.dy = (hi[1] - lo[1] + 1) * xs; q.dz = hi[2] - lo[2] + 1;
-    for (int a = 0; a < 3; ++a) { q.mins[a] = mins[a]; q.maxs[a] = maxs[a]; }
-    q.radius = w->desc.particle_radius;
-    q.slot_lo = w->own_begin;
-    q.slot_hi = w->own_begin + (uint32_t)w->N;
-    const size_t cells = (size_t)q.dx * q.dy * q.dz;
-    int c = w->cur, bc = w->bcur;
-    const bool with_bounds = w->B && !w->in_coupling;  // during update_boundaries the grid holds fluids only (liquid_world.rs:90-103)
-    CU(w->q_count.ensure(1));
-    size_t qcap = std::max<size_t>(w->q_out.cap / 2, 4096);
-    uint32_t found = 0;
-    for (int attempt = 0; attempt < 2; ++attempt) {
-        CU(w->q_out.ensure(2 * qcap));
-        CU(cudaMemsetAsync(w->q_count.p, 0, sizeof(uint32_t), w->st));
-        const auto kern = q.kind == SPH_SHAPE_HEIGHTFIELD ? k_aabb_query<true, false> : is_rev(q.kind) ? k_aabb_query<false, true> : k_aabb_query<false, false>;
-        LAUNCH(kern, cells, 128, q, w->N ? w->pos[c].p : nullptr, w->cstart.p, w->orig[c].p, with_bounds ? w->bpos[bc].p : nullptr, w->bstart.p,
-               w->borig[bc].p, w->q_out.p, (uint32_t)qcap, w->q_count.p);
-        CU(cudaMemcpyAsync(&found, w->q_count.p, sizeof found, cudaMemcpyDeviceToHost, w->st));
-        CU(cudaStreamSynchronize(w->st));
-        if (found <= qcap) break;
-        qcap = found;
-    }
-    std::vector<uint32_t> raw(2 * (size_t)found);
-    if (found) CU(cudaMemcpy(raw.data(), w->q_out.p, raw.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
-    struct Hit {
-        uint32_t kind, handle, index;
-    };
-    std::vector<Hit> hits(found);
-    for (uint32_t k = 0; k < found; ++k) {
-        uint32_t kind = raw[2 * (size_t)k], g = raw[2 * (size_t)k + 1];
-        Hit h{kind, 0u, g};
-        if (kind == 0) {
-            for (size_t f = 0; f < w->fluids.size(); ++f)
-                if (g >= w->fluids[f].offset && g < w->fluids[f].offset + w->fluids[f].n) { h.handle = make_handle(f, w->fluids[f].gen); h.index = g - (uint32_t)w->fluids[f].offset; }
-        } else {
-            for (size_t b = 0; b < w->bounds.size(); ++b)
-                if (g >= w->bounds[b].offset && g < w->bounds[b].offset + w->bounds[b].n) { h.handle = make_handle(b, w->bounds[b].gen); h.index = g - (uint32_t)w->bounds[b].offset; }
-        }
-        hits[k] = h;
-    }
-    std::sort(hits.begin(), hits.end(), [](const Hit& a, const Hit& b) {
-        return a.kind != b.kind ? a.kind < b.kind : a.handle != b.handle ? a.handle < b.handle : a.index < b.index;
-    });
-    *n = found;
-    for (size_t k = 0; k < hits.size() && k < cap; ++k) {
-        kinds[k] = hits[k].kind;
-        handles[k] = hits[k].handle;
-        indices[k] = hits[k].index;
-    }
-    return SPH_OK;
-}
 
 // LiquidWorld::particles_intersecting_aabb liquid_world.rs:211-243
 sph_status sph_world_particles_in_aabb(sph_world* w, const float mins[3], const float maxs[3], uint32_t* kinds, uint32_t* handles, uint32_t* indices,
@@ -2633,50 +2202,7 @@ sph_status sph_world_particles_in_shape(sph_world* w, const sph_shape* shape, co
                                         uint32_t* handles, uint32_t* indices, size_t cap, size_t* n) {
     if (!w || !shape || !translation || !n || (cap && (!kinds || !handles || !indices))) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
-    AabbQuery q;
-    memset(&q, 0, sizeof q);
-    static const float ident[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    const float* R = rotation_rowmajor ? rotation_rowmajor : ident;
-    for (int k = 0; k < 9; ++k) q.rot[k] = R[k];
-    for (int a = 0; a < 3; ++a) q.t[a] = translation[a];
-    switch (shape->kind) {
-        case SPH_SHAPE_BALL:
-            if (!(shape->p[0] >= 0.f)) return w->fail(SPH_ERR_INVALID, "ball radius must be >= 0");
-            q.kind = 1;
-            q.sp[0] = shape->p[0];
-            break;
-        case SPH_SHAPE_CUBOID:
-            q.kind = 2;
-            for (int a = 0; a < 3; ++a) q.sp[a] = shape->p[a];
-            break;
-        case SPH_SHAPE_CAPSULE:
-            q.kind = 3;
-            q.sp[0] = shape->p[0];
-            q.sp[1] = shape->p[1];
-            break;
-        case SPH_SHAPE_CYLINDER:
-        case SPH_SHAPE_CONE:
-            for (int a = 0; a < 2; ++a)
-                if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f)) return w->fail(SPH_ERR_INVALID, "shape parameters must be finite and >= 0");
-            q.kind = shape->kind;
-            q.sp[0] = shape->p[0];
-            q.sp[1] = shape->p[1];
-            break;
-        default:
-            return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
-    }
-    float mins[3], maxs[3];
-    if (is_rev(shape->kind)) {
-        rev_posed_aabb(*shape, R, translation, mins, maxs);
-    } else {
-        float ext[3];  // half extents of the posed shape's AABB
-        posed_aabb_ext(*shape, R, ext);
-        for (int a = 0; a < 3; ++a) {
-            mins[a] = translation[a] - ext[a];
-            maxs[a] = translation[a] + ext[a];
-        }
-    }
-    return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
+    return particles_in_shape(w, shape, translation, rotation_rowmajor, kinds, handles, indices, cap, n);
 }
 
 // particles_intersecting_shape liquid_world.rs:246-281 for a parry HeightField: the cells of compute_aabb(pos) (centre
@@ -2686,28 +2212,7 @@ sph_status sph_world_particles_in_heightfield(sph_world* w, const sph_heightfiel
                                               uint32_t* kinds, uint32_t* handles, uint32_t* indices, size_t cap, size_t* n) {
     if (!w || !translation || !n || (cap && (!kinds || !handles || !indices))) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
-    AabbQuery q;
-    memset(&q, 0, sizeof q);
-    static const float ident[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-    const float* R = rotation_rowmajor ? rotation_rowmajor : ident;
-    for (int k = 0; k < 9; ++k) q.rot[k] = R[k];
-    for (int a = 0; a < 3; ++a) q.t[a] = translation[a];
-    std::vector<float> heights;
-    float ylo, yhi;
-    TRY(hf_check(w, hf, heights, q.hf, &ylo, &yhi));
-    q.kind = SPH_SHAPE_HEIGHTFIELD;
-    hf_set_cap(q.hf, ylo, yhi, w->desc.particle_radius);
-    float mins[3], maxs[3];
-    hf_posed_aabb(q.hf, ylo, yhi, R, translation, mins, maxs);
-    *n = 0;
-    if (!w->grid_ready) return run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);  // empty, or refused while edits are pending
-    TRY(enter(w));
-    CU(w->smp_f.ensure(heights.size()));
-    CU(cudaMemcpyAsync(w->smp_f.p, heights.data(), heights.size() * sizeof(float), cudaMemcpyHostToDevice, w->st));
-    q.hf.hgt = w->smp_f.p;
-    const sph_status st = run_query(w, q, mins, maxs, kinds, handles, indices, cap, n);
-    CU(cudaStreamSynchronize(w->st));  // the upload has left `heights` on every path
-    return st;
+    return particles_in_heightfield(w, hf, translation, rotation_rowmajor, kinds, handles, indices, cap, n);
 }
 
 // salva3d::sampling::shape_{surface,volume}_ray_sample ray_sampling.rs:9-231 (sph_sampling.cuh, DESIGN.md section 11)
@@ -2715,141 +2220,7 @@ sph_status sph_world_sample_shape(sph_world* w, int32_t method, const sph_shape*
                                   float* xyz, size_t cap, size_t* n) {
     if (!w || !shape || !n || (cap && !xyz)) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
-    if (method != SPH_SAMPLE_SURFACE && method != SPH_SAMPLE_VOLUME) return w->fail(SPH_ERR_INVALID, "unknown sampling method %d", method);
-    if (!(std::isfinite(particle_radius) && particle_radius > 0.f))
-        return w->fail(SPH_ERR_INVALID, "particle radius must be finite and > 0 (got %g)", (double)particle_radius);
-    SampleRays P;
-    memset(&P, 0, sizeof P);
-    P.kind = shape->kind;
-    P.volume = method == SPH_SAMPLE_VOLUME;
-    float mins[3], maxs[3];
-    std::vector<float> heights;
-    const int np = shape_nparams(shape->kind);
-    for (int a = 0; a < np; ++a) {
-        if (!(std::isfinite(shape->p[a]) && shape->p[a] >= 0.f))
-            return w->fail(SPH_ERR_INVALID, "shape parameter %d must be finite and >= 0 (got %g)", a, (double)shape->p[a]);
-        P.p[a] = shape->p[a];
-    }
-    // shape.compute_aabb(&Isometry::identity())
-    switch (shape->kind) {
-        case SPH_SHAPE_BALL:
-            for (int a = 0; a < 3; ++a) { mins[a] = 0.f - P.p[0]; maxs[a] = 0.f + P.p[0]; }
-            break;
-        case SPH_SHAPE_CUBOID:
-            for (int a = 0; a < 3; ++a) { mins[a] = 0.f - P.p[a]; maxs[a] = 0.f + P.p[a]; }
-            break;
-        case SPH_SHAPE_CAPSULE:  // segment a = (0, -hh, 0), b = (0, hh, 0): inf(a, b) - radius, sup(a, b) + radius
-            mins[0] = mins[2] = 0.f - P.p[1];
-            maxs[0] = maxs[2] = 0.f + P.p[1];
-            mins[1] = -P.p[0] - P.p[1];
-            maxs[1] = P.p[0] + P.p[1];
-            break;
-        case SPH_SHAPE_CYLINDER:  // both: [-r, -a, -r] to [r, a, r]
-        case SPH_SHAPE_CONE:
-            mins[0] = mins[2] = 0.f - P.p[1];
-            maxs[0] = maxs[2] = 0.f + P.p[1];
-            mins[1] = -P.p[0];
-            maxs[1] = P.p[0];
-            break;
-        case SPH_SHAPE_HEIGHTFIELD: {
-            HfGrid g;
-            TRY(hf_check(w, hf, heights, g, &mins[1], &maxs[1]));
-            P.nrows = g.nrows;
-            P.ncols = g.ncols;
-            P.hx = g.hx;
-            P.hz = g.hz;
-            P.sy = g.sy;
-            P.dx = g.dx;
-            P.dz = g.dz;
-            mins[0] = -P.hx; maxs[0] = P.hx;
-            mins[2] = -P.hz; maxs[2] = P.hz;
-            break;
-        }
-        default:
-            return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
-    }
-    // surface_ray_sample / volume_ray_sample :32-38 and the running sums of the traversal :55-72
-    const float sub = particle_radius * 2.f;
-    P.sub = sub;
-    P.sub10 = sub / 10.f;
-    std::vector<float> tab[3];
-    for (int a = 0; a < 3; ++a) {
-        const float lo = mins[a] - sub, hi = maxs[a] + sub;  // aabb.loosened(sub)
-        P.origin[a] = lo + sub / 2.f;
-        if (!std::isfinite(P.origin[a]) || !std::isfinite(hi)) return w->fail(SPH_ERR_INVALID, "the shape's AABB is not finite once loosened");
-        for (float c = P.origin[a]; c < hi; c += sub) {
-            if (tab[a].size() > SMP_KEY_LIM)
-                return w->fail(SPH_ERR_INVALID, "axis %d needs more than 2^21 rays of spacing %g: quantised coordinates would reach 2^21", a, (double)sub);
-            tab[a].push_back(c);
-        }
-        P.n[a] = (uint32_t)tab[a].size();
-    }
-    unsigned long long R = 0;
-    for (int i = 0; i < 3; ++i) {
-        R += (unsigned long long)P.n[(i + 1) % 3] * P.n[(i + 2) % 3];
-        P.fam_end[i] = R;
-    }
-    if (R >= (1ull << 31) - 1) return w->fail(SPH_ERR_OOM, "%llu rays exceed the sampler's limit of 2^31 - 2", R);
-    CU(cudaSetDevice(w->desc.device));
-    const size_t nt = (size_t)P.n[0] + P.n[1] + P.n[2];
-    CU(w->smp_f.ensure(nt + heights.size()));
-    std::vector<float> up(nt + heights.size());
-    std::copy(tab[0].begin(), tab[0].end(), up.begin());
-    std::copy(tab[1].begin(), tab[1].end(), up.begin() + P.n[0]);
-    std::copy(tab[2].begin(), tab[2].end(), up.begin() + P.n[0] + P.n[1]);
-    std::copy(heights.begin(), heights.end(), up.begin() + nt);
-    CU(cudaMemcpyAsync(w->smp_f.p, up.data(), up.size() * sizeof(float), cudaMemcpyHostToDevice, w->st));
-    P.tab[0] = w->smp_f.p;
-    P.tab[1] = w->smp_f.p + P.n[0];
-    P.tab[2] = w->smp_f.p + P.n[0] + P.n[1];
-    P.hgt = heights.empty() ? nullptr : w->smp_f.p + nt;
-    // count, scan, fill
-    CU(w->smp_cnt.ensure(R + 1));
-    CU(w->smp_off.ensure(R + 1));
-    CU(w->smp_flag.ensure(1));
-    CU(cudaMemsetAsync(w->smp_flag.p, 0, sizeof(int), w->st));
-    CU(cudaMemsetAsync(w->smp_cnt.p + R, 0, sizeof(unsigned long long), w->st));
-    LAUNCH(k_sample_rays<false>, R, 256, P, w->smp_cnt.p, nullptr, nullptr, w->smp_flag.p);
-    CU(cudaGetLastError());
-    size_t tmp = 0;
-    CU(cub::DeviceScan::ExclusiveSum(nullptr, tmp, w->smp_cnt.p, w->smp_off.p, (int)(R + 1), w->st));
-    CU(w->cs_tmp.ensure(tmp));
-    CU(cub::DeviceScan::ExclusiveSum(w->cs_tmp.p, tmp, w->smp_cnt.p, w->smp_off.p, (int)(R + 1), w->st));
-    unsigned long long total = 0;
-    int overflow = 0;
-    CU(cudaMemcpyAsync(&total, w->smp_off.p + R, sizeof total, cudaMemcpyDeviceToHost, w->st));
-    CU(cudaMemcpyAsync(&overflow, w->smp_flag.p, sizeof overflow, cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
-    if (overflow) return w->fail(SPH_ERR_INVALID, "a quantised coordinate reaches 2^21 (particle radius %g is too small for the shape)", (double)particle_radius);
-    if (total > (1ull << 31) - 1) return w->fail(SPH_ERR_OOM, "%llu candidate keys exceed the sampler's limit of 2^31", total);
-    unsigned long long m = 0;
-    if (total) {
-        CU(w->smp_key[0].ensure(total));
-        CU(w->smp_key[1].ensure(total));
-        LAUNCH(k_sample_rays<true>, R, 256, P, nullptr, w->smp_off.p, w->smp_key[0].p, w->smp_flag.p);
-        CU(cudaGetLastError());
-        // ascending keys, then the unique ones (the reference's HashSet)
-        size_t t1 = 0, t2 = 0;
-        CU(cub::DeviceRadixSort::SortKeys(nullptr, t1, w->smp_key[0].p, w->smp_key[1].p, (int)total, 0, 3 * SMP_KEY_BITS, w->st));
-        CU(cub::DeviceSelect::Unique(nullptr, t2, w->smp_key[1].p, w->smp_key[0].p, w->smp_cnt.p, (int)total, w->st));
-        CU(w->cs_tmp.ensure(std::max(t1, t2)));
-        t1 = t2 = w->cs_tmp.cap;
-        CU(cub::DeviceRadixSort::SortKeys(w->cs_tmp.p, t1, w->smp_key[0].p, w->smp_key[1].p, (int)total, 0, 3 * SMP_KEY_BITS, w->st));
-        CU(cub::DeviceSelect::Unique(w->cs_tmp.p, t2, w->smp_key[1].p, w->smp_key[0].p, w->smp_cnt.p, (int)total, w->st));
-        w->launches += 2;
-        CU(cudaMemcpyAsync(&m, w->smp_cnt.p, sizeof m, cudaMemcpyDeviceToHost, w->st));
-        CU(cudaStreamSynchronize(w->st));
-        const size_t out = std::min<size_t>(m, cap);
-        if (out) {
-            CU(w->smp_xyz.ensure(3 * out));
-            LAUNCH(k_sample_unquantize, out, 256, w->smp_key[0].p, (unsigned long long)out, P.origin[0], P.origin[1], P.origin[2], sub, w->smp_xyz.p);
-            CU(cudaGetLastError());
-            CU(cudaMemcpyAsync(xyz, w->smp_xyz.p, 3 * out * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-            CU(cudaStreamSynchronize(w->st));
-        }
-    }
-    *n = (size_t)m;
-    return SPH_OK;
+    return sample_shape(w, method, shape, hf, particle_radius, xyz, cap, n);
 }
 
 sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]) {
@@ -3185,13 +2556,6 @@ static sph_status collider_check_boundary(sph_world* w, uint32_t boundary_h) {
     return SPH_OK;
 }
 
-// The first free collider slot, or MAX_BOUNDARIES when all are taken.
-static size_t collider_free_slot(const sph_world* w) {
-    for (size_t k = 0; k < w->colliders.size(); ++k)
-        if (!w->colliders[k].alive) return k;
-    return w->colliders.size();
-}
-
 // ColliderCouplingSet::register_coupling fluids_pipeline.rs:98-114
 sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t sampling, const sph_shape* shape, const float* pts, size_t n,
                                  uint32_t* collider) {
@@ -3199,8 +2563,7 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     TRY(collider_check_boundary(w, boundary_h));
     BOUNDARY_OR_FAIL(boundary, boundary_h)
-    if (shape && (shape->kind < SPH_SHAPE_BALL || shape->kind > SPH_SHAPE_CAPSULE) && !is_rev(shape->kind))
-        return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
+    if (shape && !shape_nparams(shape->kind)) return w->fail(SPH_ERR_INVALID, "unknown shape kind %d", shape->kind);
     if (sampling != SPH_SAMPLING_STATIC && sampling != SPH_SAMPLING_CONTACT) return w->fail(SPH_ERR_INVALID, "unknown sampling %d", sampling);
     if (sampling == SPH_SAMPLING_CONTACT) {
         if (!shape) return w->fail(SPH_ERR_INVALID, "DynamicContactSampling needs the collider's shape");
@@ -3212,19 +2575,11 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     if (n >= (size_t)UINT32_MAX) return w->fail(SPH_ERR_INVALID, "too many sample points");
     for (size_t k = 0; k < 3 * n; ++k)
         if (!std::isfinite(pts[k])) return w->fail(SPH_ERR_INVALID, "non-finite sample point");
-    const size_t slot = collider_free_slot(w);
-    if (slot >= (size_t)MAX_BOUNDARIES) return w->fail(SPH_ERR_INVALID, "too many colliders (max %d)", MAX_BOUNDARIES);
-    TRY(enter(w));
-    if (!w->h_imp) CU(cudaMallocHost(&w->h_imp, 6 * MAX_BOUNDARIES * sizeof(float)));
-    CU(w->d_imp.ensure(6 * MAX_BOUNDARIES));
+    size_t slot;
+    TRY(collider_reserve(w, &slot));
     ColliderRec c;
-    if (slot < w->colliders.size()) c.gen = w->colliders[slot].gen + 1;
-    c.boundary = boundary_h;
-    c.sampling = sampling;
     if (shape) c.shape = *shape;
     c.n = n;
-    c.state.rotation_rowmajor[0] = c.state.rotation_rowmajor[4] = c.state.rotation_rowmajor[8] = 1.f;
-    c.state.body = SPH_BODY_NONE;
     if (n) {
         std::vector<float4> l(n);
         for (size_t k = 0; k < n; ++k) l[k] = make_float4(pts[3 * k], pts[3 * k + 1], pts[3 * k + 2], 0.f);
@@ -3232,25 +2587,20 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
         CU(cudaMemcpyAsync(c.local.p, l.data(), n * sizeof(float4), cudaMemcpyHostToDevice, w->st));
         CU(cudaStreamSynchronize(w->st));
     }
-    if (sampling == SPH_SAMPLING_CONTACT) {  // the boundary keeps its particles until the next step samples it
-        if (slot == w->colliders.size()) w->colliders.push_back(c);
-        else w->colliders[slot] = c;
-        *collider = make_handle(slot, c.gen);
-        return SPH_OK;
+    // StaticSampling: the points become the boundary's particle set, and the next step poses them.  DynamicContactSampling:
+    // the boundary keeps its particles until the next step samples it.
+    if (sampling == SPH_SAMPLING_STATIC) {
+        TRY(pull_boundaries(w));
+        BoundaryRec& b = w->bounds[boundary];
+        w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
+        w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
+        w->hb_pos.insert(w->hb_pos.begin() + 3 * b.offset, pts, pts + 3 * n);
+        w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, 3 * n, 0.f);
+        b.n = n;
+        recompute_offsets(w);
+        w->b_dirty = true;
     }
-    // the points become the boundary's particle set; the next step poses them
-    TRY(pull_boundaries(w));
-    BoundaryRec& b = w->bounds[boundary];
-    w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
-    w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
-    w->hb_pos.insert(w->hb_pos.begin() + 3 * b.offset, pts, pts + 3 * n);
-    w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, 3 * n, 0.f);
-    b.n = n;
-    recompute_offsets(w);
-    w->b_dirty = true;
-    if (slot == w->colliders.size()) w->colliders.push_back(c);
-    else w->colliders[slot] = c;
-    *collider = make_handle(slot, c.gen);
+    collider_commit(w, slot, boundary_h, sampling, c, collider);
     return SPH_OK;
 }
 
@@ -3263,11 +2613,8 @@ sph_status sph_collider_register_heightfield(sph_world* w, uint32_t boundary_h, 
     std::vector<float> heights;
     ColliderRec c;
     TRY(hf_check(w, hf, heights, c.hf, &c.hf_ylo, &c.hf_yhi));
-    const size_t slot = collider_free_slot(w);
-    if (slot >= (size_t)MAX_BOUNDARIES) return w->fail(SPH_ERR_INVALID, "too many colliders (max %d)", MAX_BOUNDARIES);
-    TRY(enter(w));
-    if (!w->h_imp) CU(cudaMallocHost(&w->h_imp, 6 * MAX_BOUNDARIES * sizeof(float)));
-    CU(w->d_imp.ensure(6 * MAX_BOUNDARIES));
+    size_t slot;
+    TRY(collider_reserve(w, &slot));
     {
         const cudaError_t e = c.hgt.ensure(heights.size());
         if (e != cudaSuccess) return w->fail(SPH_ERR_OOM, "heightfield collider: %s", cudaGetErrorString(e));
@@ -3279,15 +2626,8 @@ sph_status sph_collider_register_heightfield(sph_world* w, uint32_t boundary_h, 
         return w->fail(SPH_ERR_CUDA, "heightfield collider upload: %s", cudaGetErrorString(e));
     }
     c.hf.hgt = c.hgt.p;
-    if (slot < w->colliders.size()) c.gen = w->colliders[slot].gen + 1;
-    c.boundary = boundary_h;
-    c.sampling = SPH_SAMPLING_CONTACT;
     c.shape.kind = SPH_SHAPE_HEIGHTFIELD;
-    c.state.rotation_rowmajor[0] = c.state.rotation_rowmajor[4] = c.state.rotation_rowmajor[8] = 1.f;
-    c.state.body = SPH_BODY_NONE;
-    if (slot == w->colliders.size()) w->colliders.push_back(c);
-    else w->colliders[slot] = c;
-    *collider = make_handle(slot, c.gen);
+    collider_commit(w, slot, boundary_h, SPH_SAMPLING_CONTACT, c, collider);
     return SPH_OK;
 }
 

@@ -15,6 +15,8 @@
 #pragma once
 #include <cstdint>
 
+#include "sph_shapes.cuh"
+
 namespace sphk {
 
 enum { SMP_KEY_BITS = 21 };
@@ -28,9 +30,7 @@ struct SampleRays {
     const float* tab[3];           // ray coordinates along each axis (f32 running sums from origin)
     uint32_t n[3];                 // their counts
     unsigned long long fam_end[3]; // cumulative ray counts of families 0, 1, 2
-    const float* hgt;              // heightfield: nrows x ncols heights, row-major, rows along z, columns along x
-    int nrows, ncols;
-    float hx, hz, sy, dx, dz;      // half footprint, height scale, cell sizes
+    HfGrid hf;                     // heightfield: heights and grid constants (the closest-point search's cap, margin and dmin unused)
 };
 
 // `f64 as u32` of an integral f32: saturating, NaN -> 0
@@ -110,19 +110,19 @@ __device__ __forceinline__ void smp_piece(float xa, float xb, float fa, float fb
 // heightfield, ray along x at (y, z): the profile of cell row i at z fraction v.  In each cell the ray crosses triangle
 // (p00, p10, p01) up to the diagonal at x0 + (1 - v) dx, then (p10, p11, p01).
 __device__ void smp_hf_along_x(const SampleRays& P, float y, float z, SmpWalk& wk, SmpSink& s) {
-    if (!(z >= -P.hz && z <= P.hz)) return;
+    if (!(z >= -P.hf.hz && z <= P.hf.hz)) return;
     float v;
-    const int i = smp_cell(z, P.hz, P.dz, P.nrows - 1, &v);
+    const int i = smp_cell(z, P.hf.hz, P.hf.dz, P.hf.nrows - 1, &v);
     const float w1 = __fsub_rn(1.f, v);
-    const float* r0 = P.hgt + (size_t)i * P.ncols;
-    const float* r1 = r0 + P.ncols;
-    float xa = -P.hx;
-    float fa = __fsub_rn(__fmul_rn(smp_lerp(r0[0], r1[0], v), P.sy), y);
-    for (int c = 0; c + 1 < P.ncols; ++c) {
-        const float xb = smp_grid(c + 1, P.ncols - 1, P.hx, P.dx);
-        const float xd = __fadd_rn(xa, __fmul_rn(w1, P.dx));
-        const float fd = __fsub_rn(__fmul_rn(smp_lerp(r0[c + 1], r1[c], v), P.sy), y);
-        const float fb = __fsub_rn(__fmul_rn(smp_lerp(r0[c + 1], r1[c + 1], v), P.sy), y);
+    const float* r0 = P.hf.hgt + (size_t)i * P.hf.ncols;
+    const float* r1 = r0 + P.hf.ncols;
+    float xa = -P.hf.hx;
+    float fa = __fsub_rn(__fmul_rn(smp_lerp(r0[0], r1[0], v), P.hf.sy), y);
+    for (int c = 0; c + 1 < P.hf.ncols; ++c) {
+        const float xb = smp_grid(c + 1, P.hf.ncols - 1, P.hf.hx, P.hf.dx);
+        const float xd = __fadd_rn(xa, __fmul_rn(w1, P.hf.dx));
+        const float fd = __fsub_rn(__fmul_rn(smp_lerp(r0[c + 1], r1[c], v), P.hf.sy), y);
+        const float fb = __fsub_rn(__fmul_rn(smp_lerp(r0[c + 1], r1[c + 1], v), P.hf.sy), y);
         smp_piece(xa, xd, fa, fd, wk, s);
         smp_piece(xd, xb, fd, fb, wk, s);
         xa = xb;
@@ -132,21 +132,21 @@ __device__ void smp_hf_along_x(const SampleRays& P, float y, float z, SmpWalk& w
 
 // heightfield, ray along z at (x, y): the profile of cell column j at x fraction u; the diagonal lies at z0 + (1 - u) dz
 __device__ void smp_hf_along_z(const SampleRays& P, float x, float y, SmpWalk& wk, SmpSink& s) {
-    if (!(x >= -P.hx && x <= P.hx)) return;
+    if (!(x >= -P.hf.hx && x <= P.hf.hx)) return;
     float u;
-    const int j = smp_cell(x, P.hx, P.dx, P.ncols - 1, &u);
+    const int j = smp_cell(x, P.hf.hx, P.hf.dx, P.hf.ncols - 1, &u);
     const float w1 = __fsub_rn(1.f, u);
-    const float* H = P.hgt + j;
-    const int nc = P.ncols;
-    float za = -P.hz;
-    float fa = __fsub_rn(__fmul_rn(smp_lerp(H[0], H[1], u), P.sy), y);
-    for (int r = 0; r + 1 < P.nrows; ++r) {
+    const float* H = P.hf.hgt + j;
+    const int nc = P.hf.ncols;
+    float za = -P.hf.hz;
+    float fa = __fsub_rn(__fmul_rn(smp_lerp(H[0], H[1], u), P.hf.sy), y);
+    for (int r = 0; r + 1 < P.hf.nrows; ++r) {
         const float* h0 = H + (size_t)r * nc;
         const float* h1 = h0 + nc;
-        const float zb = smp_grid(r + 1, P.nrows - 1, P.hz, P.dz);
-        const float zd = __fadd_rn(za, __fmul_rn(w1, P.dz));
-        const float fd = __fsub_rn(__fmul_rn(smp_lerp(h1[0], h0[1], u), P.sy), y);
-        const float fb = __fsub_rn(__fmul_rn(smp_lerp(h1[0], h1[1], u), P.sy), y);
+        const float zb = smp_grid(r + 1, P.hf.nrows - 1, P.hf.hz, P.hf.dz);
+        const float zd = __fadd_rn(za, __fmul_rn(w1, P.hf.dz));
+        const float fd = __fsub_rn(__fmul_rn(smp_lerp(h1[0], h0[1], u), P.hf.sy), y);
+        const float fb = __fsub_rn(__fmul_rn(smp_lerp(h1[0], h1[1], u), P.hf.sy), y);
         smp_piece(za, zd, fa, fd, wk, s);
         smp_piece(zd, zb, fd, fb, wk, s);
         za = zb;
@@ -156,19 +156,19 @@ __device__ void smp_hf_along_z(const SampleRays& P, float x, float y, SmpWalk& w
 
 // heightfield, ray along y at (x, z): one crossing at the surface height over the footprint
 __device__ void smp_hf_along_y(const SampleRays& P, float x, float z, SmpWalk& wk, SmpSink& s) {
-    if (!(x >= -P.hx && x <= P.hx && z >= -P.hz && z <= P.hz)) return;
+    if (!(x >= -P.hf.hx && x <= P.hf.hx && z >= -P.hf.hz && z <= P.hf.hz)) return;
     float u, v;
-    const int j = smp_cell(x, P.hx, P.dx, P.ncols - 1, &u);
-    const int i = smp_cell(z, P.hz, P.dz, P.nrows - 1, &v);
-    const float* r0 = P.hgt + (size_t)i * P.ncols + j;
-    const float* r1 = r0 + P.ncols;
+    const int j = smp_cell(x, P.hf.hx, P.hf.dx, P.hf.ncols - 1, &u);
+    const int i = smp_cell(z, P.hf.hz, P.hf.dz, P.hf.nrows - 1, &v);
+    const float* r0 = P.hf.hgt + (size_t)i * P.hf.ncols + j;
+    const float* r1 = r0 + P.hf.ncols;
     const float h00 = r0[0], h10 = r0[1], h01 = r1[0], h11 = r1[1];  // h10: (x1, z0), h01: (x0, z1)
     float h;
     if (__fadd_rn(u, v) <= 1.f)
         h = __fadd_rn(__fadd_rn(h00, __fmul_rn(u, __fsub_rn(h10, h00))), __fmul_rn(v, __fsub_rn(h01, h00)));
     else
         h = __fadd_rn(__fadd_rn(h11, __fmul_rn(__fsub_rn(1.f, u), __fsub_rn(h01, h11))), __fmul_rn(__fsub_rn(1.f, v), __fsub_rn(h10, h11)));
-    wk.hit(__fmul_rn(h, P.sy), s);
+    wk.hit(__fmul_rn(h, P.hf.sy), s);
 }
 
 __device__ __forceinline__ void smp_pair(float t, SmpWalk& wk, SmpSink& s) {
@@ -209,15 +209,15 @@ __global__ void __launch_bounds__(256) k_sample_rays(SampleRays P, unsigned long
         wk.qprev = 0.f;
         const float r2 = __fmul_rn(P.p[1], P.p[1]);
         switch (P.kind) {
-            case 1: {  // ball
+            case SPH_SHAPE_BALL: {
                 const float sq = __fsub_rn(__fmul_rn(P.p[0], P.p[0]), __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck)));
                 if (sq >= 0.f) smp_pair(__fsqrt_rn(sq), wk, s);
                 break;
             }
-            case 2:  // cuboid, closed
+            case SPH_SHAPE_CUBOID:  // closed
                 if (fabsf(cj) <= P.p[j] && fabsf(ck) <= P.p[k]) smp_pair(P.p[i], wk, s);
                 break;
-            case 3: {  // capsule: segment [-p0, p0] along y, radius p1
+            case SPH_SHAPE_CAPSULE: {  // segment [-p0, p0] along y, radius p1
                 if (i == 1) {
                     const float sq = __fsub_rn(r2, __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck)));
                     if (sq >= 0.f) smp_pair(__fadd_rn(P.p[0], __fsqrt_rn(sq)), wk, s);
@@ -229,7 +229,7 @@ __global__ void __launch_bounds__(256) k_sample_rays(SampleRays P, unsigned long
                 }
                 break;
             }
-            case 5: {  // cylinder: |y| <= p0, x^2 + z^2 <= p1^2, closed
+            case SPH_SHAPE_CYLINDER: {  // |y| <= p0, x^2 + z^2 <= p1^2, closed
                 if (i == 1) {
                     if (__fsub_rn(r2, __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck))) >= 0.f) smp_pair(P.p[0], wk, s);
                 } else {
@@ -239,7 +239,7 @@ __global__ void __launch_bounds__(256) k_sample_rays(SampleRays P, unsigned long
                 }
                 break;
             }
-            case 6: {  // cone: apex (0, p0, 0), base disc of radius p1 at y = -p0; radius R(y) = p1 (p0 - y) / (2 p0)
+            case SPH_SHAPE_CONE: {  // apex (0, p0, 0), base disc of radius p1 at y = -p0; radius R(y) = p1 (p0 - y) / (2 p0)
                 const float a = P.p[0], a2 = __fadd_rn(a, a);
                 if (i == 1) {  // the base, then the slant at y = a - 2a rho / r (a at rho = 0, -a at the rim)
                     const float c2 = __fadd_rn(__fmul_rn(cj, cj), __fmul_rn(ck, ck));
