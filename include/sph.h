@@ -93,8 +93,8 @@ typedef struct {
     int32_t  slab_rank;              /* multi-GPU slab decomposition along x: this world's slab index ... */
     int32_t  slab_count;             /* ... of slab_count slabs (1 = single GPU) */
     int32_t  deterministic;          /* 1: stable in-cell ordering => bit-reproducible run to run */
-    int32_t  gather_backend;         /* 0: L1/texture gathers over 32-bit global lists (default, fastest measured);
-                                        1: tile-staged shared memory via TMA bulk copies + 16-bit tile-local lists */
+    int32_t  gather_backend;         /* must be 0; 1 (the tile backend) was removed. Kept so the struct layout does not
+                                        change; sph_world_create refuses any other value with SPH_ERR_INVALID */
     int32_t  kernel_density;         /* SPH_KERNEL_*: KernelDensity  (0 = CubicSplineKernel) */
     int32_t  kernel_gradient;        /* SPH_KERNEL_*: KernelGradient (0 = CubicSplineKernel) */
 } sph_world_desc;

@@ -22,7 +22,6 @@
 #include "sph_kernels.cuh"
 #include "sph_shapes.cuh"
 #include "sph_passes.cuh"
-#include "sph_tile.cuh"
 #include "sph_iisph.cuh"
 #include "sph_elasticity.cuh"
 #include "sph_viscosity.cuh"
@@ -257,11 +256,6 @@ struct sph_world {
     DBuf<float> dens, alpha, kappa, divv, pred, bvol, bforce;
     DBuf<uint32_t> cid, rank, perm, cstart, bcid, brank, bperm, bstart, scan_aux[3], scan_aux_k[3];
     DBuf<uint32_t> nbr_f, nbr_b, cnt_f, cnt_b;
-    // gather_backend 1 (sph_tile.cuh): 16-bit tile-local fluid contact indices
-    DBuf<uint16_t> nbr16;
-    uint32_t tile_slots = 2048;  // widest tile halo seen by the last neighbour build (local index space size)
-    uint32_t n_tiles = 0;
-    bool tile = false;
     // uniform-mass packed gather records (sph_passes.cuh): pvx4 = (x,y,z,v*x), vyz2 = (v*y,v*z), pk4 = (x,y,z,kappa); their
     // gathers are split evenly over the texture and LSU pipes (even / odd contacts)
     bool unimass = false;
@@ -309,7 +303,7 @@ struct sph_world {
     bool nb_valid = false, nb_pending = false;
     int nb[7] = {0, 0, 0, 0, 0, 0, 0};
     DBuf<int> d_nb;
-    int xysub = 1;              // row order (Consts::xysub, SALVA_B200_XYSUB): x / y bins per cell; one GPU, gather backend 0 only
+    int xysub = 1;              // row order (Consts::xysub, SALVA_B200_XYSUB): x / y bins per cell; one GPU only
 
     bool grid_ready = false;    // cstart/bstart + sorted arrays describe the last step's cell grid (AABB queries)
     bool ever_stepped = false;
@@ -405,7 +399,7 @@ void fill_static_consts(sph_world* w) {
     c.h = w->h;
     c.inv_h = 1.0f / w->h;
     c.h2 = w->h * w->h;
-    c.xysub = (w->tile || w->slab.active) ? 1 : w->xysub;  // slab worlds cut x into cell columns of width h: plain cells there
+    c.xysub = w->slab.active ? 1 : w->xysub;  // slab worlds cut x into cell columns of width h: plain cells there
     c.xysub_f = (float)c.xysub;
     c.h_reach = std::nextafter(w->h * 1.00001f, INFINITY);
     c.sigma = 8.0f / (3.14159265358979323846f * w->h * w->h * w->h);
@@ -561,8 +555,7 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     CU(w->cnt_f.ensure(N));
     CU(w->cnt_b.ensure(N));
     w->stride = (uint32_t)((N + 31) / 32 * 32);
-    if (w->tile) CU(w->nbr16.ensure((size_t)w->cap_f * w->stride));
-    else CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
+    CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
     CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
     uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
     CU(w->partial.ensure((size_t)(nblk + 3) * std::max<size_t>(1, w->fluids.size())));  // +3: a slab pass may run as three sub-range launches
@@ -621,7 +614,7 @@ sph_status stage_up(sph_world* w) {
     // a slab world takes the fast path on every rank or on none: volumes default to uniform there, and an empty
     // slab inherits the constant from its first immigrant only through the classic path -> keep it simple: require
     // particles with uniform volumes on this rank, otherwise fall back (all ranks are built by the same host code).
-    w->unimass = !w->tile && w->desc.solver == SPH_SOLVER_DFSPH && w->fluids.size() == 1 && w->fluids[0].uniform_mass > 0.f;
+    w->unimass = w->desc.solver == SPH_SOLVER_DFSPH && w->fluids.size() == 1 && w->fluids[0].uniform_mass > 0.f;
     return SPH_OK;
 }
 
@@ -768,7 +761,7 @@ sph_status phase_grid(sph_world* w) {
     for (int a = 0; a < 3; ++a) dims[a] = (long long)hb[3 + a] - hb[a] + 3;  // one padding cell each side
     double ncell_d = (double)dims[0] * (double)dims[1] * (double)dims[2];
     if (ncell_d > 1.0e9) return w->fail(SPH_ERR_OOM, "dense cell grid too large: %lld x %lld x %lld cells of width h", dims[0], dims[1], dims[2]);
-    const int xys = (w->tile || w->slab.active) ? 1 : w->xysub;  // x / y bins per cell (row order, Consts::xysub)
+    const int xys = w->slab.active ? 1 : w->xysub;  // x / y bins per cell (row order, Consts::xysub)
     if (ncell_d * xys * xys > 2.0e9) return w->fail(SPH_ERR_OOM, "dense cell grid too large: %lld x %lld x %lld cells of width h", dims[0], dims[1], dims[2]);
     size_t ncell = (size_t)dims[0] * dims[1] * dims[2] * xys * xys;
     w->hc.ox = (hb[0] - 1) * xys;
@@ -777,15 +770,10 @@ sph_status phase_grid(sph_world* w) {
     w->hc.nx = (int)dims[0] * xys;
     w->hc.ny = (int)dims[1] * xys;
     w->hc.nz = (int)dims[2];
-    w->hc.ntx = (int)((dims[0] - 2 + TILE_X - 1) / TILE_X);
-    w->hc.nty = (int)((dims[1] - 2 + TILE_Y - 1) / TILE_Y);
-    w->hc.ntz = (int)((dims[2] - 2 + TILE_Z - 1) / TILE_Z);
-    w->n_tiles = (uint32_t)w->hc.ntx * w->hc.nty * w->hc.ntz;
     fill_static_consts(w);
     TRY(upload_consts(w));
     CU(w->cstart.ensure(ncell + 1));
     CU(w->bstart.ensure(ncell + 1));
-    if (w->tile) CU(w->partial.ensure((size_t)std::max<uint32_t>(w->n_tiles, 1) * std::max<size_t>(1, w->fluids.size())));
     w->stats.grid_dims[0] = (uint32_t)dims[0];
     w->stats.grid_dims[1] = (uint32_t)dims[1];
     w->stats.grid_dims[2] = (uint32_t)dims[2];
@@ -854,60 +842,6 @@ sph_status phase_grid(sph_world* w) {
     return SPH_OK;
 }
 
-// ---- tile kernel launches (gather_backend 1, sph_tile.cuh) -------------------------------------------
-constexpr size_t TILE_DYN_SMEM_LIMIT = 200 * 1024;
-// Number of halo slots staged in shared memory for a kernel that needs `slot_bytes` per slot.
-uint32_t tile_cap(const sph_world* w, uint32_t slot_bytes) {
-    uint32_t want = (w->tile_slots + 63u) / 64u * 64u;
-    uint32_t fit = (uint32_t)(TILE_DYN_SMEM_LIMIT / slot_bytes) / 64u * 64u;
-    return std::min(want, fit);
-}
-template <class K>
-cudaError_t tile_prepare(K kern) {
-    static std::mutex m;
-    static std::vector<const void*> done;
-    std::lock_guard<std::mutex> lock(m);
-    const void* key = reinterpret_cast<const void*>(kern);
-    for (const void* d : done)
-        if (d == key) return cudaSuccess;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)TILE_DYN_SMEM_LIMIT);
-    if (e == cudaSuccess) done.push_back(key);
-    return e;
-}
-#define LAUNCH_TILE(kern, slot_bytes, cap, ...)                                                      \
-    do {                                                                                             \
-        if (w->n_tiles > 0) {                                                                        \
-            CU(tile_prepare(kern));                                                                  \
-            kern<<<w->n_tiles, TILE_T, (size_t)(cap) * (slot_bytes), w->st>>>(__VA_ARGS__);          \
-            w->launches++;                                                                           \
-        }                                                                                            \
-    } while (0)
-#define TDISPATCH1(kern, multi, slot_bytes, cap, ...)                               \
-    do {                                                                            \
-        if (multi) LAUNCH_TILE((kern<true>), slot_bytes, cap, __VA_ARGS__);         \
-        else LAUNCH_TILE((kern<false>), slot_bytes, cap, __VA_ARGS__);              \
-    } while (0)
-#define TDISPATCH2(kern, multi, bf, slot_bytes, cap, ...)                                  \
-    do {                                                                                   \
-        if (multi) {                                                                       \
-            if (bf) LAUNCH_TILE((kern<true, true>), slot_bytes, cap, __VA_ARGS__);         \
-            else LAUNCH_TILE((kern<true, false>), slot_bytes, cap, __VA_ARGS__);           \
-        } else {                                                                           \
-            if (bf) LAUNCH_TILE((kern<false, true>), slot_bytes, cap, __VA_ARGS__);        \
-            else LAUNCH_TILE((kern<false, false>), slot_bytes, cap, __VA_ARGS__);          \
-        }                                                                                  \
-    } while (0)
-#define TDISPATCH3(kern, multi, bf, third, slot_bytes, cap, ...)                                          \
-    do {                                                                                                  \
-        if (multi) {                                                                                      \
-            if (bf) LAUNCH_TILE((kern<true, true, third>), slot_bytes, cap, __VA_ARGS__);                 \
-            else LAUNCH_TILE((kern<true, false, third>), slot_bytes, cap, __VA_ARGS__);                   \
-        } else {                                                                                          \
-            if (bf) LAUNCH_TILE((kern<false, true, third>), slot_bytes, cap, __VA_ARGS__);                \
-            else LAUNCH_TILE((kern<false, false, third>), slot_bytes, cap, __VA_ARGS__);                  \
-        }                                                                                                 \
-    } while (0)
-
 template <class T>
 sph_status ensure_tex(sph_world* w, cudaTextureObject_t* tex, const void** cur, const T* ptr, size_t n) {
     if (*cur == ptr && *tex) return SPH_OK;
@@ -944,7 +878,7 @@ sph_status density_args(sph_world* w, DensArgs* D) {
 // `speculative` (optional) enqueues the work that follows the neighbour search and only writes scratch (the density
 // pass): it is launched BEFORE the host learns whether the lists overflowed, so the GPU is busy during that round trip;
 // on overflow the lists are rebuilt with a larger capacity and the speculative work is simply enqueued again.
-// With w->fused_first_div (DFSPH, list backend) the search itself computes rho, alpha and the first divergence evaluation
+// With w->fused_first_div (DFSPH) the search itself computes rho, alpha and the first divergence evaluation
 // (density_alpha_div); on overflow the relaunched search computes them again.
 sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) = nullptr) {
     size_t N = w->N, B = w->B;
@@ -979,32 +913,19 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             }
     }
     for (int attempt = 0; attempt < 8 && N; ++attempt) {
-        CU(cudaMemsetAsync(w->d_scal.p + 8, 0, 3 * sizeof(int), w->st));
+        CU(cudaMemsetAsync(w->d_scal.p + 8, 0, 2 * sizeof(int), w->st));
         uint32_t* maxcnt = reinterpret_cast<uint32_t*>(w->d_scal.p + 8);
-        if (w->tile) {
-            LAUNCH(k_neighbors_boundary, N, 128, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_b.p, w->cnt_b.p, maxcnt);
-            uint32_t sb = multi ? 32u : 16u;
-            uint32_t cap = tile_cap(w, sb);
-            TDISPATCH1(k_tile_neighbors, multi, sb, cap, w->pos[c].p, w->vel[c].p, w->cstart.p, cap, w->nbr16.p, w->cnt_f.p, maxcnt);
-        } else {
-            LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-                   w->cnt_f.p, w->cnt_b.p, maxcnt, D);
-        }
+        LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
+               w->cnt_f.p, w->cnt_b.p, maxcnt, D);
         int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous
-        CU(cudaMemcpyAsync(hs, w->d_scal.p + 7, 4 * sizeof(int), cudaMemcpyDeviceToHost, w->st));
+        CU(cudaMemcpyAsync(hs, w->d_scal.p + 7, 3 * sizeof(int), cudaMemcpyDeviceToHost, w->st));
         CU(cudaEventRecord(w->ev_lists, w->st));
         CU(cudaEventRecord(w->ev[EV_NBR], w->st));
-        const bool early = speculative && !w->tile;  // (tile launches need this read-back's slot count)
-        if (early) TRY(speculative(w));
+        if (speculative) TRY(speculative(w));
         CU(cudaEventSynchronize(w->ev_lists));
         // (a zero density of the search's own density sweep is reported with the other zero densities at the end of the step)
         if (hs[0] & ~ERR_SEARCH_ZERO_DENSITY)
             return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
-        if (w->tile) {
-            if ((uint32_t)hs[3] > 65535u)
-                return w->fail(SPH_ERR_INVALID, "tile halo of %d particles exceeds the 16-bit contact index space", hs[3]);
-            w->tile_slots = std::max<uint32_t>((uint32_t)hs[3], 64u);
-        }
         w->stats.max_neighbors = (uint32_t)hs[1];
         bool grow = false;
         if ((uint32_t)hs[1] > w->cap_f) {
@@ -1015,13 +936,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             w->cap_b = ((uint32_t)hs[2] + 15) / 16 * 16;
             grow = true;
         }
-        if (!grow) {
-            if (speculative && !early) TRY(speculative(w));
-            break;
-        }
-        if (early) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded density pass or sweep
-        if (w->tile) CU(w->nbr16.ensure((size_t)w->cap_f * w->stride));
-        else CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
+        if (!grow) break;
+        if (speculative) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded density pass or sweep
+        CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
         CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
         fill_static_consts(w);
         TRY(upload_consts(w));
@@ -1087,7 +1004,7 @@ bool any_bforce(const sph_world* w) {
         else LAUNCH((kern<false>), n, threads, __VA_ARGS__);            \
     } while (0)
 
-// ---- gather passes: one wrapper per reference function, two backends ------------------------------------
+// ---- gather passes: one wrapper per reference function ------------------------------------
 
 // ghost refresh of v* in whichever representation the evaluations gather (one NCCL group); vs itself is included
 // because the velocity fold reads vel = v* for ghosts too
@@ -1110,15 +1027,8 @@ sph_status launch_density_alpha(sph_world* w) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
-    if (w->tile) {
-        TileLists L{w->nbr16.p, w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-        uint32_t cap = tile_cap(w, 16);
-        TDISPATCH1(k_tile_density_alpha, multi, 16, cap, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->cstart.p, cap, L, w->dens.p, w->alpha.p,
-                   w->d_scal.p + 7);
-    } else {
-        Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-        DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, w->d_scal.p + 7);
-    }
+    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
+    DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, w->d_scal.p + 7);
     return SPH_OK;  // the ghost refresh of rho follows in post_density_refresh(), once the list-capacity check has passed
 }
 // Ghost refresh of what the density pass produced (rho; DFSPH: also kappa of the fused first divergence evaluation).  Kept out
@@ -1203,7 +1113,7 @@ sph_status run_parts(sph_world* w, const SlabArray* arrays, int n_arrays, uint32
 // The fluid term of the FIRST force of a single-fluid DFSPH world can ride with the divergence evaluations when it is an
 // XSPHViscosity without a boundary term (see k_vel_divergence_xsph_u).
 bool xsph_fusable(const sph_world* w) {
-    if (w->desc.solver != SPH_SOLVER_DFSPH || w->tile || !w->unimass || w->slab.active) return false;
+    if (w->desc.solver != SPH_SOLVER_DFSPH || !w->unimass || w->slab.active) return false;
     if (w->fluids.size() != 1 || w->fluids[0].forces.empty()) return false;
     const sph_force_desc& d = w->fluids[0].forces[0].d;
     return d.kind == SPH_FORCE_XSPH_VISCOSITY && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0);
@@ -1212,7 +1122,7 @@ bool xsph_fusable(const sph_world* w) {
 // term with the evaluation after it (k_vel_divergence_xsph_u<2>), when it is the first force of the single uniform-mass fluid
 // and has no boundary term (no adhesion, or no boundaries) and no boundary wants forces.  Otherwise phase_forces computes it.
 bool akinci_fusable_u(const sph_world* w) {
-    if (w->desc.solver != SPH_SOLVER_DFSPH || w->tile || !w->unimass || w->slab.active) return false;
+    if (w->desc.solver != SPH_SOLVER_DFSPH || !w->unimass || w->slab.active) return false;
     if (w->fluids.size() != 1 || w->fluids[0].forces.empty()) return false;
     const sph_force_desc& d = w->fluids[0].forces[0].d;
     return d.kind == SPH_FORCE_AKINCI2013_TENSION && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0) && !any_bforce(w);
@@ -1231,15 +1141,6 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
     const bool xsf = !predict && xsph_fusable(w);
     const bool akf = !predict && w->nr4_valid && !w->akinci_valid;  // the first evaluation after the normals-carrying update
     if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
-    if (w->tile) {
-        TileLists L{w->nbr16.p, w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-        uint32_t cap = tile_cap(w, 32);
-        TDISPATCH2(k_tile_vel_divergence, multi, predict, 32, cap, w->pos[c].p, w->vs.p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, w->cstart.p, cap, L,
-                   w->dens.p, w->alpha.p, predict ? w->pred.p : w->divv.p, w->kappa.p, w->partial.p, w->dt, w->d_scal.p + 7);
-        *nblk = w->n_tiles;
-        w->errsum_ready = false;
-        return SPH_OK;
-    }
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) {
         TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
@@ -1286,17 +1187,6 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
 sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
-    if (w->tile) {
-        TileLists L{w->nbr16.p, w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-        uint32_t cap = tile_cap(w, 20);
-        if (pressure)
-            TDISPATCH3(k_tile_vel_update, multi, bf, true, 20, cap, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->cstart.p, cap, L, w->kappa.p, w->vc[c].p,
-                       w->vs.p, w->bforce.p, w->inv_dt);
-        else
-            TDISPATCH3(k_tile_vel_update, multi, bf, false, 20, cap, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->cstart.p, cap, L, w->kappa.p, w->vc[c].p,
-                       w->vs.p, w->bforce.p, w->inv_dt);
-        return SPH_OK;
-    }
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) TRY(ensure_tex(w, &w->tex_pk, &w->tex_pk_ptr, w->pk4.p, w->pk4.cap));
     if (normals) {
@@ -1376,7 +1266,6 @@ sph_status materialise_contacts(sph_world* w, uint32_t f, int which, HostContact
 
 sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<float>& hp, std::vector<float>& hv, std::vector<float>& hd,
                             std::vector<float>& ha) {
-    if (w->tile) return w->fail(SPH_ERR_INVALID, "host plugins with contacts need gather_backend 0");
     if (w->slab.active && (fr.host_flags & SPH_HOST_FORCE_CONTACTS))
         return w->fail(SPH_ERR_INVALID, "materialised contacts are not available in slab-decomposed worlds");
     const FluidRec& fl = w->fluids[f];
@@ -1438,29 +1327,16 @@ sph_status phase_forces(sph_world* w) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-    TileLists TL{w->nbr16.p, w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     for (size_t f = 0; f < w->fluids.size(); ++f)
         for (ForceRec& fr : w->fluids[f].forces) {
             const float* p = fr.d.p;
             switch (fr.d.kind) {
                 case SPH_FORCE_XSPH_VISCOSITY:
                     if (w->xs_valid && f == 0 && &fr == &w->fluids[0].forces[0]) break;  // already folded in by k_fold_velocities
-                    if (w->tile) {
-                        uint32_t cap = tile_cap(w, 36);
-                        TDISPATCH2(k_tile_xsph, multi, bf, 36, cap, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, w->cstart.p, cap, TL,
-                                   w->dens.p, w->acc.p, w->bforce.p, (uint32_t)f, p[0], p[1], w->inv_dt);
-                        break;
-                    }
                     DISPATCH2(k_force_xsph, multi, bf, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p, w->acc.p,
                               w->bforce.p, (uint32_t)f, p[0], p[1], w->inv_dt);
                     break;
                 case SPH_FORCE_ARTIFICIAL_VISCOSITY:
-                    if (w->tile) {
-                        uint32_t cap = tile_cap(w, 36);
-                        TDISPATCH2(k_tile_artificial, multi, bf, 36, cap, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, w->cstart.p, cap, TL,
-                                   w->dens.p, w->acc.p, w->bforce.p, (uint32_t)f, p[0], p[1], p[2], p[3], p[4]);
-                        break;
-                    }
                     DISPATCH2(k_force_artificial, multi, bf, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p, w->acc.p,
                               w->bforce.p, (uint32_t)f, p[0], p[1], p[2], p[3], p[4]);
                     break;
@@ -1469,15 +1345,6 @@ sph_status phase_forces(sph_world* w) {
                     CU(w->normals.ensure(std::max(w->Ntot, w->N)));
                     const AkinciNorms an = akinci_norms(w->h);
                     const float coh_norm = an.coh_norm, h6_64 = an.h6_64, adh_norm = an.adh_norm;
-                    if (w->tile) {
-                        uint32_t sb1 = multi ? 36u : 20u, sb2 = multi ? 52u : 36u;
-                        uint32_t cap1 = tile_cap(w, sb1), cap2 = tile_cap(w, sb2);
-                        TDISPATCH1(k_tile_akinci_normals, multi, sb1, cap1, w->pos[c].p, w->vel[c].p, w->cstart.p, cap1, TL, w->dens.p, w->normals.p,
-                                   (uint32_t)f);
-                        TDISPATCH2(k_tile_akinci_force, multi, bf, sb2, cap2, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->cstart.p, cap2, TL, w->dens.p,
-                                   w->normals.p, w->acc.p, w->bforce.p, (uint32_t)f, p[0], p[1], coh_norm, h6_64, adh_norm);
-                        break;
-                    }
                     if (w->nr4_valid && f == 0) {  // normals (and rho, in .w) came with the first divergence update
                         TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
                         if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
@@ -1494,7 +1361,6 @@ sph_status phase_forces(sph_world* w) {
                     TRY(elasticity_solve(w, (uint32_t)f, fr));
                     break;
                 case SPH_FORCE_HE2014_TENSION: {
-                    if (w->tile) return w->fail(SPH_ERR_INVALID, "He2014SurfaceTension is not implemented by gather_backend 1");
                     CU(w->he_colors.ensure(std::max(w->Ntot, w->N)));
                     CU(w->he_gradc.ensure(std::max(w->Ntot, w->N)));
                     DISPATCH1(k_he2014_colors, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->he_colors.p, (uint32_t)f);
@@ -1509,7 +1375,6 @@ sph_status phase_forces(sph_world* w) {
                     TRY(viscosity_solve(w, (uint32_t)f, fr));
                     break;
                 case SPH_FORCE_WCSPH_TENSION:
-                    if (w->tile) return w->fail(SPH_ERR_INVALID, "WCSPHSurfaceTension is not implemented by gather_backend 1");
                     if (p[0] != 0.f) DISPATCH1(k_wcsph_force, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->acc.p, (uint32_t)f, p[0]);
                     break;
                 case FORCE_HOST_CALLBACK: {  // user-defined NonPressureForce::solve on the host (nonpressure_force.rs:10-30)
@@ -1722,10 +1587,10 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
         w->lists_valid = false;
     }
     CU(cudaEventRecord(w->ev[EV_GRID], w->st));
-    // evaluate_kernels + compute_densities (liquid_world.rs:123-134) + compute_alphas (dfsph_solver.rs:679-684).  DFSPH with the
-    // list backend: computed by the neighbour search itself, together with the first divergence evaluation; otherwise enqueued
+    // evaluate_kernels + compute_densities (liquid_world.rs:123-134) + compute_alphas (dfsph_solver.rs:679-684).  DFSPH:
+    // computed by the neighbour search itself, together with the first divergence evaluation; otherwise enqueued
     // speculatively by the neighbour phase (EV_NBR is recorded there, between the two)
-    w->fused_first_div = w->N && w->desc.solver == SPH_SOLVER_DFSPH && !w->tile;
+    w->fused_first_div = w->N && w->desc.solver == SPH_SOLVER_DFSPH;
     TRY(phase_neighbors(w, [](sph_world* w) -> sph_status {
         if (w->N && !w->fused_first_div) TRY(launch_density_alpha(w));
         return SPH_OK;
@@ -1830,6 +1695,7 @@ sph_status sph_world_create(const sph_world_desc* desc, sph_world** out) {
     if (desc->solver != SPH_SOLVER_DFSPH && desc->solver != SPH_SOLVER_IISPH) return SPH_ERR_INVALID;
     if (desc->kernel_density < 0 || desc->kernel_density > SPH_KERNEL_VISCOSITY || desc->kernel_gradient < 0 || desc->kernel_gradient > SPH_KERNEL_VISCOSITY)
         return SPH_ERR_INVALID;
+    if (desc->gather_backend != 0) return SPH_ERR_INVALID;  // see sph_world_desc::gather_backend
 #if !SPH_GENERIC_KERNELS
     // this build monomorphises the solver on CubicSplineKernel; libsalva_b200_kernels.so carries the other kernels
     if (desc->kernel_density != SPH_KERNEL_CUBIC_SPLINE || desc->kernel_gradient != SPH_KERNEL_CUBIC_SPLINE) return SPH_ERR_INVALID;
@@ -1841,7 +1707,6 @@ sph_status sph_world_create(const sph_world_desc* desc, sph_world** out) {
     sph_world* w = new sph_world();
     w->desc = *desc;
     w->h = desc->particle_radius * desc->smoothing_factor * 2.0f;  // liquid_world.rs:44
-    w->tile = desc->gather_backend == 1 && desc->solver == SPH_SOLVER_DFSPH;  // the tile backend covers the DFSPH passes only
     if (const char* t = getenv("SALVA_B200_XYSUB")) w->xysub = std::min(4, std::max(1, atoi(t)));
     memset(&w->hc, 0, sizeof w->hc);
     memset(&w->stats, 0, sizeof w->stats);
@@ -1875,7 +1740,7 @@ void sph_world_destroy(sph_world* w) {
     w->bstart.release();
     for (auto& a : w->scan_aux) a.release();
     for (auto& a : w->scan_aux_k) a.release();
-    w->nbr_f.release(); w->nbr16.release(); w->nbr_b.release(); w->cnt_f.release(); w->cnt_b.release();
+    w->nbr_f.release(); w->nbr_b.release(); w->cnt_f.release(); w->cnt_b.release();
     w->partial.release(); w->errsum.release(); w->d_scal.release(); w->d_cnt.release();
     w->o_a.release(); w->o_b.release(); w->o_c.release(); w->o_mass.release(); w->o_fid.release();
     iisph_release(w);

@@ -1,4 +1,4 @@
-// sph_iisph.cuh — IISPH pressure solver kernels (iisph_solver.rs), default gather backend.
+// sph_iisph.cuh — IISPH pressure solver kernels (iisph_solver.rs).
 //
 // Per-contact gathers are minimised by pre-combining per-particle quantities in the producing kernel:
 //   prho_j = p_j / rho_j^2                        (gathered by compute_dij_pjl and compute_velocity_changes)

@@ -43,14 +43,13 @@ struct Consts {
     int ox, oy, oz;              // grid origin in cell coordinates (one padding cell each side)
     int nx, ny, nz;
     float h_reach;               // h * (1 + 1e-5): covers every |dx| the f32 test d^2 <= h^2 can accept (row order, arun())
-    // "row order" (SALVA_B200_XYSUB, one GPU, gather backend 0): x and y are binned `xysub` times finer than h (ox, oy, nx, ny then
+    // "row order" (SALVA_B200_XYSUB, one GPU): x and y are binned `xysub` times finer than h (ox, oy, nx, ny then
     // count BINS), z stays the run direction.  With xysub = 2 and the usual spacing h/2 every (x, y) bin column holds ONE line of
     // particles along z, so the 32 lanes of a warp are 32 consecutive particles of a line and their k-th contacts are consecutive
     // particles of a neighbouring line: a warp-wide gather touches ~4 cache lines instead of ~17 data-pipe wavefronts
     // (tools/sim_gather_order.py models this).  Contact SETS are unchanged (k_neighbors_xy clips its rows, see arun()).
     int xysub;
     float xysub_f;
-    int ntx, nty, ntz;           // tile grid (sph_tile.cuh): 2 x 2 cell columns x TILE_Z cells per tile
     uint32_t n_fluid, n_bound;   // particle totals (n_fluid counts owned + ghost slots of the sorted arrays)
     uint32_t i_begin, n_owned;   // owned slots [i_begin, i_begin + n_owned): everything on one GPU; the slab between the
                                  // two ghost columns in a multi-GPU world (x-major order keeps ghosts at both ends)
@@ -928,8 +927,7 @@ __global__ void k_set_w(uint32_t n, float4* __restrict__ a, const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------
-// Error reduction + elementwise (streaming) kernels.  The neighbour-gather passes live in sph_passes.cuh
-// (default backend) and sph_tile.cuh (tile/TMA backend).
+// Error reduction + elementwise (streaming) kernels.  The neighbour-gather passes live in sph_passes.cuh.
 // ------------------------------------------------------------------------------------------------
 // One block per fluid: fixed-order sum of the per-block partials.
 __global__ void k_reduce_partials(const float* __restrict__ partial, uint32_t nblocks, int n_fluids, float* __restrict__ out) {
@@ -952,7 +950,7 @@ __global__ void k_reduce_partials(const float* __restrict__ partial, uint32_t nb
 #endif
 constexpr int PASS_T = SPH_PASS_T;  // threads per block of the gather passes
 
-// The fluid reorder fused with k_make_vstar: the sorted pos / vel / vc are in registers anyway, so v* = vel + vc and the packed
+// The fluid reorder fused with v* = vel + vc: the sorted pos / vel / vc are in registers anyway, so v* and the packed
 // gather records are written by the same pass (saves re-reading 48 B per particle and a launch).  g.in4 / out4 [0..2] = pos, vel, vc.
 __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, GatherSet g, float4* __restrict__ vs, float4* __restrict__ pvx,
                                float2* __restrict__ vyz) {
@@ -971,21 +969,6 @@ __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, Ga
     if (pvx) {
         pvx[s] = make_float4(p.x, p.y, p.z, sx);
         vyz[s] = make_float2(sy, sz);
-    }
-}
-
-// v* = vel + vc after the reorder (the divergence solve works on vel + vc carried over from the previous step, Appendix A.3.2)
-__global__ void k_make_vstar(const float4* __restrict__ vel, const float4* __restrict__ vc, float4* __restrict__ vs, const float4* __restrict__ pos,
-                             float4* __restrict__ pvx, float2* __restrict__ vyz) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= C.n_fluid) return;
-    float4 v = vel[i], c = vc[i];
-    float sx = v.x + c.x, sy = v.y + c.y, sz = v.z + c.z;
-    vs[i] = make_float4(sx, sy, sz, 0.f);
-    if (pvx) {  // uniform-mass packed records (sph_passes.cuh)
-        float4 p = pos[i];
-        pvx[i] = make_float4(p.x, p.y, p.z, sx);
-        vyz[i] = make_float2(sy, sz);
     }
 }
 
@@ -1219,11 +1202,6 @@ __global__ void k_import_acc(uint32_t n, const uint32_t* __restrict__ orig, cons
     if (g < lo || g >= hi) return;
     acc[s] = make_float4(src[3 * (size_t)g], src[3 * (size_t)g + 1], src[3 * (size_t)g + 2], 0.f);
 }
-__global__ void k_import1(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    dst[s] = src[orig[s]];
-}
 __global__ void k_iota(uint32_t n, uint32_t* __restrict__ a) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) a[s] = s;
@@ -1292,10 +1270,6 @@ __global__ void k_iota_from(uint32_t n, uint32_t start, uint32_t* __restrict__ a
 __global__ void k_export_u32(uint32_t n, const uint32_t* __restrict__ orig, const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) dst[orig[s]] = src[s];
-}
-__global__ void k_import_u32(uint32_t n, const uint32_t* __restrict__ orig, const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) dst[s] = src[orig[s]];
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1,4 +1,4 @@
-// sph_passes.cuh — neighbour-gather passes, default backend: one thread per particle walks its index-only
+// sph_passes.cuh — neighbour-gather passes: one thread per particle walks its index-only
 // contact list and gathers neighbour data from global memory through L1 (and, for some of the per-contact vectors,
 // through the TEXTURE pipe, whose data path is separate from the LSU one: the L1TEX data pipe — two float4
 // gathers per contact — is what bounds these kernels, not DRAM).
@@ -392,7 +392,7 @@ k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, con
 }
 
 // One fluid-fluid contact of Akinci2013SurfaceTension::solve (akinci2013_surface_tension.rs:113-192): the cohesion and
-// curvature terms of neighbour j (mass mj, normal nj, density rho_j) added to a.  Every list-backend Akinci force pass goes
+// curvature terms of neighbour j (mass mj, normal nj, density rho_j) added to a.  Every Akinci force pass goes
 // through it, so the separate passes and the one fused with a divergence evaluation round alike.
 __device__ __forceinline__ void akinci_contact(const Pair& p, const float4& ni, float rho_i, const float4& nj, float rho_j, float mj, float gamma,
                                                float rho0, float coh_norm, float h6_64, float& ax, float& ay, float& az) {

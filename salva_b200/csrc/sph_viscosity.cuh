@@ -1,4 +1,4 @@
-// sph_viscosity.cuh — DFSPHViscosity (viscosity/dfsph_viscosity.rs, SURVEY row a16), default gather backend.
+// sph_viscosity.cuh — DFSPHViscosity (viscosity/dfsph_viscosity.rs, SURVEY row a16).
 //
 // Per solve: betas (one gather pass + a 6x6 LU inverse per particle), strain-rate targets (one pass), then the
 // reference's Jacobi loop: strain-rate errors (one pass + error mean) / accelerations (one pass).  Per-contact gathers are

@@ -304,7 +304,7 @@ class LiquidWorld:
         d.device = device
         d.deterministic = int(deterministic)
         d.slab_rank, d.slab_count = slab_rank, slab_count
-        d.gather_backend = gather_backend
+        d.gather_backend = gather_backend  # must be 0 (the only gather backend); sph_world_create refuses other values
         d.kernel_density = getattr(solver, "kernel_density", 0)
         d.kernel_gradient = getattr(solver, "kernel_gradient", 0)
         self._w = C.c_void_p()

@@ -80,6 +80,15 @@ def test_no_cpu_fallback_without_cuda():
     assert e.value.status == 2  # SPH_ERR_CUDA
 
 
+@pytest.mark.parametrize("solver, backend", [("dfsph", 1), ("iisph", 1), ("dfsph", 2)])
+def test_gather_backend_other_than_0_is_refused(solver, backend):
+    """gather_backend must be 0; the check runs before any device query, so it holds with or without a GPU."""
+    from salva_b200 import DFSPHSolver, IISPHSolver, LiquidWorld, SphError
+    with pytest.raises(SphError) as e:
+        LiquidWorld(solver={"dfsph": DFSPHSolver, "iisph": IISPHSolver}[solver](), particle_radius=0.05, gather_backend=backend)
+    assert e.value.status == 1  # SPH_ERR_INVALID
+
+
 def test_every_entry_point_cites_the_reference_and_is_in_the_integration_guide():
     """include/sph.h declares the drop-in boundary: every entry point must appear in INTEGRATION.md (what it replaces in the
     reference), and the header itself must cite reference files (file.rs:line) next to the declarations."""

@@ -92,7 +92,7 @@ def _make(kind, coupled):
     if kind == "rows":  # the row order of the counting sort (x / y bins of h / 2), read when a world is created
         os.environ["SALVA_B200_XYSUB"] = "2"
     try:
-        w = LiquidWorld(solver, particle_radius=R, gather_backend=1 if kind == "tile" else 0)
+        w = LiquidWorld(solver, particle_radius=R)
     finally:
         os.environ.pop("SALVA_B200_XYSUB", None)
         if old is not None:
@@ -120,7 +120,7 @@ def _advance(w, b, c, locals_, k):
     w.step(DT)
 
 
-@pytest.mark.parametrize("kind", ["dfsph", "rows", "tile", "iisph", "poly6"])
+@pytest.mark.parametrize("kind", ["dfsph", "rows", "iisph", "poly6"])
 def test_static_colliders_match_host_posed_boundaries(kind):
     """Three StaticSampling colliders (fixed tank, dynamic rotating box, parentless ball far below the fluid) against the
     same boundaries posed by numpy and written from the host every step: fluid and boundary state bit for bit, impulses

@@ -17,7 +17,7 @@ from salva_b200.liquid_world import Ball, Capsule, Cuboid
 pytestmark = pytest.mark.gpu
 
 F = np.float32
-KINDS = ["dfsph", "rows", "tile"]
+KINDS = ["dfsph", "rows"]
 
 
 def _world(kind, radius):
@@ -25,7 +25,7 @@ def _world(kind, radius):
     if kind == "rows":  # x / y bins of h / 2, read when a world is created
         os.environ["SALVA_B200_XYSUB"] = "2"
     try:
-        return LiquidWorld(DFSPHSolver(), particle_radius=radius, gather_backend=1 if kind == "tile" else 0)
+        return LiquidWorld(DFSPHSolver(), particle_radius=radius)
     finally:
         os.environ.pop("SALVA_B200_XYSUB", None)
         if old is not None:

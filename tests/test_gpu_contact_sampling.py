@@ -80,7 +80,7 @@ def _world(kind="dfsph"):
     if kind == "rows":
         os.environ["SALVA_B200_XYSUB"] = "2"
     try:
-        return LiquidWorld(solver, particle_radius=R, gather_backend=1 if kind == "tile" else 0)
+        return LiquidWorld(solver, particle_radius=R)
     finally:
         os.environ.pop("SALVA_B200_XYSUB", None)
         if old is not None:
@@ -162,7 +162,7 @@ def test_pushes_and_samples_are_bit_identical_to_numpy():
         assert branches.get(name, 0) > 0, (name, branches)
 
 
-@pytest.mark.parametrize("kind", ["dfsph", "rows", "tile", "iisph", "poly6"])
+@pytest.mark.parametrize("kind", ["dfsph", "rows", "iisph", "poly6"])
 def test_full_physics_against_the_host_hook(kind):
     """Free iterations (both worlds re-sort the fluid after the coupling, so their error sums see the same order), gravity
     and XSPH: the samples exact on each step's lockstep input, the fluid within 1e-5 h / 1e-4,

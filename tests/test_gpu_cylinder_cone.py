@@ -20,7 +20,7 @@ from salva_b200.liquid_world import Capsule, Poly6Kernel, SpikyKernel
 pytestmark = pytest.mark.gpu
 
 F = np.float32
-KINDS = ["dfsph", "rows", "tile", "poly6"]  # grid orders, the tile backend, and the second library (poly6)
+KINDS = ["dfsph", "rows", "poly6"]  # both grid orders, and the second library (poly6)
 DTS = rc.DTS
 
 SHAPES = {
@@ -64,7 +64,7 @@ def _world(kind, radius):
         os.environ["SALVA_B200_XYSUB"] = "2"
     try:
         solver = DFSPHSolver(Poly6Kernel, SpikyKernel) if kind == "poly6" else DFSPHSolver()
-        return LiquidWorld(solver, particle_radius=radius, gather_backend=1 if kind == "tile" else 0)
+        return LiquidWorld(solver, particle_radius=radius)
     finally:
         os.environ.pop("SALVA_B200_XYSUB", None)
         if old is not None:

@@ -23,7 +23,7 @@ pytestmark = pytest.mark.gpu
 F = np.float32
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GXX = "/usr/bin/g++" if os.path.exists("/usr/bin/g++") else "g++"
-KINDS = ["dfsph", "rows", "tile", "poly6"]  # grid orders, the tile backend, and the second library (poly6)
+KINDS = ["dfsph", "rows", "poly6"]  # both grid orders, and the second library (poly6)
 DTS = (0.004, 0.008, 0.004 / 3)
 
 
@@ -75,7 +75,7 @@ def _world(kind, radius):
         os.environ["SALVA_B200_XYSUB"] = "2"
     try:
         solver = DFSPHSolver(Poly6Kernel, SpikyKernel) if kind == "poly6" else DFSPHSolver()
-        return LiquidWorld(solver, particle_radius=radius, gather_backend=1 if kind == "tile" else 0)
+        return LiquidWorld(solver, particle_radius=radius)
     finally:
         os.environ.pop("SALVA_B200_XYSUB", None)
         if old is not None:

@@ -14,9 +14,9 @@ from salva_b200 import DFSPHSolver, IISPHSolver, LiquidWorld, scenes
 pytestmark = pytest.mark.gpu
 
 
-def _pair(scene, solver=0, **kw):
+def _pair(scene, solver=0):
     r = scene["particle_radius"]
-    gpu = LiquidWorld(DFSPHSolver() if solver == 0 else IISPHSolver(), particle_radius=r, smoothing_factor=2.0, **kw)
+    gpu = LiquidWorld(DFSPHSolver() if solver == 0 else IISPHSolver(), particle_radius=r, smoothing_factor=2.0)
     cpu = OracleWorld(r, 2.0, solver=solver)
     fg, bg = scenes.populate(gpu, scene)
     fc, bc = scenes.populate(cpu, scene)
@@ -90,10 +90,9 @@ def test_list_capacity_regrows_behind_speculative_density_pass():
 @pytest.mark.parametrize("forces", [(), (scenes.xsph_viscosity(0.5, 0.3),), (scenes.artificial_viscosity(1.0, 0.5),),
                                     (scenes.akinci2013_surface_tension(1.0, 0.7),)],
                          ids=["none", "xsph", "artificial", "akinci2013"])
-@pytest.mark.parametrize("backend", [0, 1], ids=["l1-gather", "tile-tma"])
-def test_trajectory_forced_iterations(forces, backend):
+def test_trajectory_forced_iterations(forces):
     sc = _small_scene(seed=5, forces=forces)
-    gpu, cpu, fg, fc, _, _ = _pair(sc, gather_backend=backend)
+    gpu, cpu, fg, fc, _, _ = _pair(sc)
     dt = 0.005
     for w in (gpu, cpu):
         w.force_iterations(2, 3)
@@ -257,10 +256,9 @@ def test_particles_intersecting_aabb_matches_oracle():
         gpu.particles_intersecting_aabb(*boxes[0])
 
 
-@pytest.mark.parametrize("backend", [0, 1], ids=["l1-gather", "tile-tma"])
-def test_two_fluids_with_groups_and_free_running_iterations(backend):
+def test_two_fluids_with_groups_and_free_running_iterations():
     sc = _small_scene(seed=9, forces=(scenes.xsph_viscosity(0.5, 0.0),), two_fluids=True)
-    gpu, cpu, fg, fc, _, _ = _pair(sc, gather_backend=backend)
+    gpu, cpu, fg, fc, _, _ = _pair(sc)
     for _ in range(4):
         gpu.step(0.005)
         cpu.step(0.005)
@@ -413,11 +411,10 @@ def test_host_edits_append_delete_roundtrip():
     assert np.abs(pg - pc).max() <= 1e-3 * float(gpu.h)
 
 
-@pytest.mark.parametrize("backend", [0, 1], ids=["l1-gather", "tile-tma"])
-def test_boundary_forces_accumulate_like_reference(backend):
+def test_boundary_forces_accumulate_like_reference():
     """Boundary::apply_force (boundary.rs:62-67) writers: dfsph_solver.rs:269-272,403-405 and the force plugins."""
     sc = _small_scene(seed=17, forces=(scenes.xsph_viscosity(0.5, 0.3),), want_forces=True)
-    gpu, cpu, fg, fc, bg, bc = _pair(sc, gather_backend=backend)
+    gpu, cpu, fg, fc, bg, bc = _pair(sc)
     for w in (gpu, cpu):
         w.force_iterations(2, 3)
     for _ in range(3):

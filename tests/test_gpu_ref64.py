@@ -17,17 +17,17 @@ FORCE_SCENES = ("block", "pairs", "two_fluids")
 K = {1: Poly6Kernel, 2: SpikyKernel, 3: ViscosityKernel}
 
 
-def _gpu(kd=0, kg=0, backend=0):
+def _gpu(kd=0, kg=0):
     def make(max_divergence_iter=None):
         solver = DFSPHSolver(K[kd], K[kg]) if kd else DFSPHSolver()
         if max_divergence_iter is not None:
             solver.max_divergence_iter = max_divergence_iter
-        return LiquidWorld(solver, particle_radius=S.R, smoothing_factor=2.0, gather_backend=backend)
+        return LiquidWorld(solver, particle_radius=S.R, smoothing_factor=2.0)
     return make
 
 
-def _check(name, kd=0, kg=0, backend=0, forces=True):
-    c = S.Checks(_gpu(kd, kg, backend), S.SCENES[name](), kw=kd, kg=kg)
+def _check(name, kd=0, kg=0, forces=True):
+    c = S.Checks(_gpu(kd, kg), S.SCENES[name](), kw=kd, kg=kg)
     c.stages()
     if forces and name in FORCE_SCENES:
         c.akinci(0.0)
@@ -36,7 +36,7 @@ def _check(name, kd=0, kg=0, backend=0, forces=True):
         c.xsph(0.5, 0.3)
         c.artificial(1.0, 0.0)
         c.artificial(1.0, 0.5, beta=0.3)
-    print("\nREF64 %s" % json.dumps(dict(scene=name, kernels=[kd, kg], backend=backend,
+    print("\nREF64 %s" % json.dumps(dict(scene=name, kernels=[kd, kg],
                                          worst={k: round(v, 5) for k, v in c.worst.items()},
                                          excluded={k: v for k, v in c.excluded.items() if v})))
     assert not c.flagged(), c.worst
@@ -58,11 +58,6 @@ def test_every_pass_meets_its_bound_with_generic_kernels(name, kd, kg):
 def test_every_pass_meets_its_bound_in_row_order(name, monkeypatch):
     monkeypatch.setenv("SALVA_B200_XYSUB", "2")  # read when the world is created
     _check(name)
-
-
-@pytest.mark.parametrize("name", ["block", "pairs", "two_fluids", "volumes"])
-def test_every_pass_meets_its_bound_on_the_tile_backend(name):
-    _check(name, backend=1)
 
 
 # ---- IISPH: the density pass, dii, aii, dij_pjl, the pressure update, its density error, the velocity change and the

@@ -19,12 +19,12 @@ K = {1: Poly6Kernel, 2: SpikyKernel}
 LIBS = pytest.mark.parametrize("kd,kg", [(0, 0), (1, 2)], ids=["cubic", "poly6+spiky"])
 
 
-def _gpu(kd=0, kg=0, backend=0, solver=DFSPHSolver):
+def _gpu(kd=0, kg=0, solver=DFSPHSolver):
     def make(**kw):
         s = solver(K[kd], K[kg]) if kd else solver()
         for k, v in kw.items():
             setattr(s, k, v)
-        return LiquidWorld(s, particle_radius=S.R, smoothing_factor=2.0, gather_backend=backend)
+        return LiquidWorld(s, particle_radius=S.R, smoothing_factor=2.0)
     return make
 
 
@@ -34,11 +34,11 @@ def _report(c, **tags):
     assert not c.flagged(), c.worst
 
 
-def _errors(name, kd=0, kg=0, backend=0):
-    c = S.Checks(_gpu(kd, kg, backend), S.LOOP_SCENES[name](), kw=kd, kg=kg)
+def _errors(name, kd=0, kg=0):
+    c = S.Checks(_gpu(kd, kg), S.LOOP_SCENES[name](), kw=kd, kg=kg)
     c.loop_errors()
     c.loop_errors((DT, 2 * DT))
-    _report(c, scene=name, check="loop_errors", kernels=[kd, kg], backend=backend)
+    _report(c, scene=name, check="loop_errors", kernels=[kd, kg])
     for e in ("divergence_error", "density_error"):
         assert {e, e + "_read", e + "_after_dt_change", e + "_read_after_dt_change"} <= set(c.worst)
 
@@ -53,11 +53,6 @@ def test_the_loop_errors_meet_their_bounds(name, kd, kg):
 def test_the_loop_errors_meet_their_bounds_in_row_order(name, monkeypatch):
     monkeypatch.setenv("SALVA_B200_XYSUB", "2")  # read when the world is created
     _errors(name)
-
-
-@pytest.mark.parametrize("name", ["block", "two_fluids", "sixteen"])
-def test_the_loop_errors_meet_their_bounds_on_the_tile_backend(name):
-    _errors(name, backend=1)
 
 
 def _force(kind):
@@ -106,14 +101,6 @@ def test_the_lagging_dt_meets_every_bound_in_row_order(name, monkeypatch):
     _report(c, scene=name, check="lagging_dt_row_order")
 
 
-@pytest.mark.parametrize("name", ["block", "two_fluids", "sixteen"])
-def test_the_lagging_dt_meets_every_bound_on_the_tile_backend(name):
-    """k_tile_vel_update scales the divergence reaction by inv_dt_prev and the pressure update by inv_dt_cur itself."""
-    c = S.Checks(_gpu(backend=1), S.LOOP_SCENES[name]())
-    c.lagging_dt()
-    _report(c, scene=name, check="lagging_dt_tile")
-
-
 EXITS = pytest.mark.parametrize("factor,margin", [(2.0, 0.25), (0.5, -0.25)], ids=["ends", "iterates"])
 
 
@@ -126,13 +113,11 @@ def test_the_loops_end_where_the_reference_does(factor, margin, kd, kg):
 
 
 @EXITS
-@pytest.mark.parametrize("order", ["rows", "tile"])
-def test_the_loops_end_where_the_reference_does_in_row_order_and_on_the_tile_backend(factor, margin, order, monkeypatch):
-    if order == "rows":
-        monkeypatch.setenv("SALVA_B200_XYSUB", "2")
-    c = S.Checks(_gpu(backend=1 if order == "tile" else 0), S.LOOP_SCENES["block"]())
+def test_the_loops_end_where_the_reference_does_in_row_order(factor, margin, monkeypatch):
+    monkeypatch.setenv("SALVA_B200_XYSUB", "2")
+    c = S.Checks(_gpu(), S.LOOP_SCENES["block"]())
     c.loop_exits(factor, margin)
-    _report(c, scene="block", check="loop_exits_" + order, factor=factor, margin=c.exit_margin)
+    _report(c, scene="block", check="loop_exits_rows", factor=factor, margin=c.exit_margin)
 
 
 @pytest.mark.parametrize("name", ["block", "two_fluids", "sixteen"])
