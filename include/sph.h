@@ -146,7 +146,7 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        SPH_DBG_VELOCITY_CHANGE = 4,    /* velocity_changes (3 floats/particle) dfsph_solver.rs:44 */
        SPH_DBG_NUM_FLUID_CONTACTS = 5, /* len(ff list) as float, self included contacts.rs:83-87 */
        SPH_DBG_NUM_BOUNDARY_CONTACTS = 6,
-       SPH_DBG_PRESSURE = 7,           /* IISPH pressures      iisph_solver.rs:37  */
+       SPH_DBG_PRESSURE = 7,           /* IISPH pressures      iisph_solver.rs:37 (after a host edit: the carried ones) */
        SPH_DBG_ACCELERATION = 8,       /* fluid.accelerations (3 floats/particle), after forces, before integrate */
        /* IISPH scratch (SPH_ERR_INVALID for DFSPH, and before the first IISPH step) */
        SPH_DBG_IISPH_DII = 9,          /* dii (3 floats/particle)                      iisph_solver.rs:32 */
@@ -225,7 +225,13 @@ typedef struct {
 } sph_host_force_ctx;
 typedef void (*sph_host_force_fn2)(void* user, const sph_host_force_ctx* ctx);
 sph_status sph_fluid_push_host_force2(sph_world* w, uint32_t fluid, sph_host_force_fn2 fn, void* user, uint32_t flags);
-/* Fluid::add_particles fluid.rs:126-150 */
+/* Fluid::add_particles fluid.rs:126-150.  The new particles go to the end of the fluid's index range with the default volume,
+ * zero velocity_changes and zero IISPH pressure.  Their ids count up from 1 + the largest id among the fluid's current
+ * particles (those marked for deletion included; 0 for an empty fluid), so an id is never held by two live particles of a
+ * fluid, and a fluid nothing was deleted from keeps the ids 0..n-1.  SPH_ERR_INVALID (nothing appended) when the new ids
+ * would pass 0xFFFFFFFF, which only ids given through sph_fluid_set_ids / sph_fluid_replace_particles can bring about.  In a
+ * slab-decomposed world the largest id is taken over this rank's particles only: give appended particles world-wide ids
+ * with sph_fluid_set_ids there. */
 sph_status sph_fluid_append(sph_world* w, uint32_t fluid, const float* pos_xyz, const float* vel_xyz, size_t n);
 /* Fluid::delete_particle_at_next_timestep fluid.rs:71-76; applied at the next step (fluid.rs:88-98). */
 sph_status sph_fluid_delete(sph_world* w, uint32_t fluid, const uint8_t* mask, size_t n);
@@ -416,8 +422,10 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid, int what, float* out, si
 const char* sph_last_error(const sph_world* w);
 const char* sph_version(void);
 
-/* Caller-visible particle ids (default: the index a particle had when it was added).  They follow particles when the
- * sort reorders them and when a particle migrates to another rank's slab. */
+/* Caller-visible particle ids (default: the index a particle had when it was added with sph_fluid_add; for appended
+ * particles see sph_fluid_append).  They follow particles when the sort reorders them, through deletions, and when a particle
+ * migrates to another rank's slab.  The ids of a fluid are the in-cell sort key: they must be unique within the fluid for
+ * a run to be bit-reproducible from a snapshot, which the library's own ids are and ids given here should be. */
 sph_status sph_fluid_set_ids(sph_world* w, uint32_t fluid, const uint32_t* ids, size_t n);
 sph_status sph_fluid_read_ids(sph_world* w, uint32_t fluid, uint32_t* ids, size_t cap);
 

@@ -379,6 +379,21 @@ MUTANTS = ("drop_entries_32_35", "swap_vy_vz_odd", "gate_at_21", "normals_rho_i"
            "positions_previous_dt", "vc_not_carried", "vc_carried_unsorted", "fluid15_rho0_of_fluid0", "iisph_previous_dt")
 
 
+def alpha_ratio(ps, alpha, bvol, rho0_b=None):
+    """|1 / alpha - den| over its bound per particle (0 where excluded) and the excluded particles: those whose denominator
+    lies within its bound of the 1e-5 gate, and those with a pair at the gradient's zero threshold."""
+    ref = ps.den(bvol, rho0_b=rho0_b)
+    b = ref.bound(0)
+    amb = np.abs(ref.value - 1e-5) <= b
+    with np.errstate(divide="ignore", invalid="ignore"):
+        den_gpu = np.where(alpha > 0, 1.0 / alpha.astype(np.float64), 0.0)
+        # alpha = 0 <=> den <= 1e-5; otherwise 1 / alpha is den up to one more rounding of each reciprocal
+        r = np.where(alpha > 0, np.abs(den_gpu - ref.value) / (b + 2 * ref64.U * np.abs(ref.value)),
+                     np.where(ref.value <= 1e-5, 0.0, np.inf))
+    ex = amb | ps.ambiguous()
+    return np.where(ex, 0.0, r), ex
+
+
 class Checks:
     """Runs the stages of one scene on one world kind and keeps the worst |err| / bound per pass.  `mutant` applies one
     plausible kernel bug to the reference instead (a bound that passes the mutant too is too loose)."""
@@ -588,17 +603,9 @@ class Checks:
         side[1] += int((np.nan_to_num(raw) > b).sum())
 
     def _alpha(self, alpha, bvol):
-        ref = self.ps.den(bvol, rho0_b=self.rho0_b)
-        b = ref.bound(0)
-        amb = np.abs(ref.value - 1e-5) <= b
-        with np.errstate(divide="ignore", invalid="ignore"):
-            den_gpu = np.where(alpha > 0, 1.0 / alpha.astype(np.float64), 0.0)
-        # alpha = 0 <=> den <= 1e-5; otherwise 1 / alpha is den up to one more rounding of each reciprocal
-            r = np.where(alpha > 0, np.abs(den_gpu - ref.value) / (b + 2 * ref64.U * np.abs(ref.value)),
-                         np.where(ref.value <= 1e-5, 0.0, np.inf))
-        r = np.where(amb | self.ps.ambiguous(), 0.0, r)
+        r, ex = alpha_ratio(self.ps, alpha, bvol, self.rho0_b)
         self.worst["alpha"] = float(r.max()) if len(r) else 0.0
-        self.excluded["alpha"] = int((amb | self.ps.ambiguous()).sum())
+        self.excluded["alpha"] = int(ex.sum())
 
     def akinci(self, adhesion=0.0, gamma=1.0):
         """Unfused (0, 0); for a single uniform-mass fluid without adhesion, fused (1, 0) (force in the evaluation after the

@@ -1863,6 +1863,13 @@ sph_status sph_fluid_append(sph_world* w, uint32_t fluid_h, const float* pos, co
     TRY(enter(w));
     TRY(stage_down(w));
     FluidRec& f = w->fluids[fluid];
+    // new ids count up from one past the fluid's largest id, pending deletes included: the count f.n would repeat the
+    // id of a survivor once a delete has shrunk the fluid, and the in-cell order (fluid, id) needs ids to be unique
+    uint64_t next = 0;
+    for (size_t i = 0; i < f.n; ++i) next = std::max<uint64_t>(next, (uint64_t)w->h_gid[f.offset + i] + 1u);
+    if (next + n > (uint64_t)UINT32_MAX + 1u)
+        return w->fail(SPH_ERR_INVALID, "sph_fluid_append: ids %llu.. of %zu new particles do not fit 32 bits (renumber with sph_fluid_set_ids)",
+                       (unsigned long long)next, n);
     size_t at = f.offset + f.n;
     float r = w->desc.particle_radius;
     float pv = r * r * r * (float)(8.0 * 0.8);
@@ -1876,7 +1883,7 @@ sph_status sph_fluid_append(sph_world* w, uint32_t fluid_h, const float* pos, co
     w->h_gid.resize(w->h_vol.size() - n);
     {
         std::vector<uint32_t> ids(n);
-        for (size_t i = 0; i < n; ++i) ids[i] = (uint32_t)(f.n + i);
+        for (size_t i = 0; i < n; ++i) ids[i] = (uint32_t)(next + i);
         w->h_gid.insert(w->h_gid.begin() + at, ids.begin(), ids.end());
     }
     f.n += n;
@@ -2151,7 +2158,9 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     }
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
+        // the carried state is on the host between an edit and the next step; the step's scratch reads as zero until then
         if (what == SPH_DBG_VELOCITY_CHANGE) memcpy(out, w->h_vc.data() + 3 * f.offset, 3 * f.n * sizeof(float));
+        else if (what == SPH_DBG_PRESSURE) memcpy(out, w->h_press.data() + f.offset, f.n * sizeof(float));
         else memset(out, 0, width * f.n * sizeof(float));
         return SPH_OK;
     }
