@@ -30,6 +30,7 @@ products, 10.5u) are a relative error of every term and are counted in each pass
 Cites (reference src/): kernel/*.rs, solver/pressure/dfsph_solver.rs, solver/pressure/iisph_solver.rs, solver/viscosity/xsph_viscosity.rs,
 solver/surface_tension/{akinci2013,he2014,wcsph}_surface_tension.rs, solver/elasticity/becker2009_elasticity.rs, as restated in SURVEY.md Appendix A.
 """
+import itertools
 from dataclasses import dataclass
 
 import numpy as np
@@ -263,6 +264,30 @@ def contacts(P, Q, h, allowed, same=False):
     return Pairs(i, j, P[i].astype(np.float64) - Q[j].astype(np.float64))
 
 
+def contacts_rows(P, Q, h, allowed, rows, tree=None):
+    """The contacts of the points P[rows] only, otherwise as `contacts`: candidates within h (1 + 1e-5) from a k-d tree over
+    all of Q (query_ball_point keeps zero distances, so self contacts and coincident points are in), the same float32 test
+    and group mask, and the same (i, j) order, so each row's list is term for term the one `contacts` gives it.  i and j
+    stay global indices.  tree: a cKDTree over Q to reuse."""
+    h32 = F(h)
+    h2 = F(h32 * h32)
+    rows = np.asarray(rows, np.int64)
+    if len(Q) == 0 or len(rows) == 0:
+        z = np.zeros(0, np.int64)
+        return Pairs(z, z, np.zeros((0, 3)))
+    tq = cKDTree(Q.astype(np.float64)) if tree is None else tree
+    hits = tq.query_ball_point(P[rows].astype(np.float64), float(h32) * (1.0 + 1e-5), workers=-1)
+    ln = np.fromiter(map(len, hits), np.int64, len(hits))
+    i = np.repeat(rows, ln)
+    j = np.fromiter(itertools.chain.from_iterable(hits), np.int64, int(ln.sum()))
+    keep = f32_d2(P[i], Q[j]) <= h2
+    keep &= allowed(i, j)
+    i, j = i[keep], j[keep]
+    o = np.lexsort((j, i))
+    i, j = i[o], j[o]
+    return Pairs(i, j, P[i].astype(np.float64) - Q[j].astype(np.float64))
+
+
 def _coincident(P, Q):
     key = {}
     for k, q in enumerate(Q.tolist()):
@@ -306,9 +331,14 @@ def ratio(gpu, ref, c_pass):
 class Passes:
     """The float64 passes of one scene.  P: fluid positions (float32, all fluids concatenated), fid: fluid of each particle,
     rho0: per-particle rest density (float32), mass: per-particle mass (float32, vol * rho0 as the engine forms it),
-    BP / bid: boundary positions and boundary of each, allowed_ff / allowed_fb: interaction-group masks over (i, j)."""
+    BP / bid: boundary positions and boundary of each, allowed_ff / allowed_fb: interaction-group masks over (i, j).
 
-    def __init__(self, h, P, fid, rho0, mass, BP, bid, allowed_ff=None, allowed_fb=None, allowed_bb=None, kw=0, kg=0):
+    rows: build the fluid-fluid and fluid-boundary contacts of these particles only (contacts_rows).  Every pass then runs
+    unchanged over global indices and is exact, term for term, at the rows; elsewhere its sums are partial and meaningless.
+    Boundary-boundary contacts stay complete.  brows: the boundary particles all of whose fluid contacts belong to rows, so
+    that sums onto boundary particles are whole there."""
+
+    def __init__(self, h, P, fid, rho0, mass, BP, bid, allowed_ff=None, allowed_fb=None, allowed_bb=None, kw=0, kg=0, rows=None):
         self.h = float(F(h))
         self.P, self.fid = P, fid
         self.rho0 = np.asarray(rho0, F).astype(np.float64)
@@ -317,11 +347,34 @@ class Passes:
         self.kw, self.kg = kw, kg
         self.N = len(P)
         every = lambda i, j: np.ones(len(i), bool)  # noqa: E731
-        self.ff = contacts(P, P, self.h, allowed_ff or every, same=True)
-        self.fb = contacts(P, BP, self.h, allowed_fb or every)
+        self.allowed_ff = allowed_ff or every
+        self._halo = None
+        if rows is None:
+            self.rows = self.brows = None
+            self.ff = contacts(P, P, self.h, self.allowed_ff, same=True)
+            self.fb = contacts(P, BP, self.h, allowed_fb or every)
+        else:
+            self.rows = np.unique(np.asarray(rows, np.int64))
+            self._tree = cKDTree(P.astype(np.float64))
+            self.ff = contacts_rows(P, P, self.h, self.allowed_ff, self.rows, tree=self._tree)
+            self.fb = contacts_rows(P, BP, self.h, allowed_fb or every, self.rows)
+            # a boundary particle is whole when no fluid particle outside rows lies within reach of it
+            inside = np.zeros(self.N, bool)
+            inside[self.rows] = True
+            near = self._tree.query_ball_point(np.asarray(BP, np.float64), self.h * (1.0 + 1e-5), workers=-1) if len(BP) else []
+            self.brows = np.array([k for k, hit in enumerate(near) if inside[hit].all()], np.int64)
         self.bb = contacts(BP, BP, self.h, allowed_bb or every, same=True)
         self.nf = np.bincount(self.ff.i, minlength=self.N)
         self.nb = np.bincount(self.fb.i, minlength=self.N)
+
+    def halo(self):
+        """Rows mode: the fluid-fluid contacts of the rows and of all their neighbours (for a pass that reads a gathered
+        quantity of its neighbours, such as Akinci's normals).  Full mode: ff."""
+        if self.rows is None:
+            return self.ff
+        if self._halo is None:
+            self._halo = contacts_rows(self.P, self.P, self.h, self.allowed_ff, np.unique(self.ff.j), tree=self._tree)
+        return self._halo
 
     # ambiguous float decisions: the gradient's zero threshold
     def ambiguous(self, pairs=None):
@@ -460,22 +513,24 @@ class Passes:
         K = _sum(N, ff.i, aK) + _sum(N, fb.i, bK)
         return Ref(val, A, K, (self._n(ff) + self._n(fb) + 1).astype(np.float64))
 
-    def akinci(self, dens, gamma, adhesion, bvol, rho_j=None, ff=None, fb=None):
+    def akinci(self, dens, gamma, adhesion, bvol, rho_i_for_j=False, ff=None, fb=None):
         """Akinci2013SurfaceTension (akinci2013_surface_tension.rs:43-192): normals n_i = h sum_j (m_j / rho_j) grad W_ij over
         the same fluid, then the fluid force sum_j kij (-gamma (n_i - n_j) - gamma m_j C(r) x_ij / r), kij = 2 rho0 /
-        (rho_i + rho_j), and the adhesion -adh vol_b rho0 A(r) x_ib / r.  rho_j: per-contact neighbour densities of the
-        normals (default dens[j]).  The normals' own error bound is carried into the force's bound."""
+        (rho_i + rho_j), and the adhesion -adh vol_b rho0 A(r) x_ib / r.  rho_i_for_j: the normals divide by rho_i instead
+        of rho_j.  The normals' own error bound is carried into the force's bound.  In rows mode the normals come from the
+        halo's contacts (the neighbours' normals are sums over their own lists)."""
         ff = self.ff if ff is None else ff
         fb = self.fb if fb is None else fb
         N, h = self.N, self.h
         same = self.fid[ff.i] == self.fid[ff.j]
         sf = ff.subset(same)
         rho = np.asarray(dens, F).astype(np.float64)
-        rj = rho[sf.j] if rho_j is None else np.asarray(rho_j, F).astype(np.float64)[same]
-        a, aA, aK = self._grad_terms(sf, self.mass[sf.j] / rj)
-        nrm = h * _sum(N, sf.i, a)
+        nf_ = sf if self.rows is None else self.halo()
+        nf_ = nf_.subset(self.fid[nf_.i] == self.fid[nf_.j])
+        a, aA, aK = self._grad_terms(nf_, self.mass[nf_.j] / rho[nf_.i if rho_i_for_j else nf_.j])
+        nrm = h * _sum(N, nf_.i, a)
         nn = self._n(sf).astype(np.float64)
-        e_n = h * ((nn + C_PASS["normals"])[:, None] * U * _sum(N, sf.i, aA) + _sum(N, sf.i, aK))
+        e_n = h * ((self._n(nf_) + C_PASS["normals"])[:, None] * U * _sum(N, nf_.i, aA) + _sum(N, nf_.i, aK))
         gamma = float(F(gamma))
         r = np.where(sf.r > 0, sf.r, 1.0)
         coh, coha, cohe = _cohesion(sf.r, h)
@@ -560,6 +615,35 @@ class Passes:
             # the maximum over fluids is 1-Lipschitz in each: the bound of the maximum is the largest bound
             bound = max(bound, ((n + C_ERR) * U * np.abs(e[sel]).sum() + U * a[sel].sum() + b[sel].sum()) / n)
         return val, bound
+
+    def loop_error_structural(self, kind, x, block, second, mutant=None):
+        """loop_error fed the float32 values read back, over all particles, against the bound of the reduction tree the
+        engine runs (structural_depth) instead of the any-order (n + 4) u sum |e|: (D + C_ERR) u sum |e| + u sum a, per
+        fluid over n.  block: threads per block of the pass (PASS_T, or NBR_T for the neighbour search's fused first
+        evaluation); second: threads of the block that sums the partials (PASS_T for a pass's last block, 256 for
+        k_reduce_partials).  mutant: error_drops_blocks_past_65535 (every partial of block >= 65536 lost).  Returns
+        (value, bound, D)."""
+        v = _f64(x)
+        if kind == "divergence":
+            e = np.maximum(v, 0.0) / self.rho0
+            a = e
+        else:
+            q = v / self.rho0
+            on = v >= self.rho0
+            e = np.where(on, q - 1.0, 0.0)
+            a = np.where(on, np.abs(q) + np.abs(e), 0.0)
+        keep = np.ones(self.N, bool)
+        if mutant == "error_drops_blocks_past_65535":
+            keep[65536 * block:] = False
+        D = structural_depth(self.N, block, second)
+        g = D * U / (1.0 - D * U)
+        val, bound = 0.0, 0.0
+        for f in np.unique(self.fid):
+            sel = np.nonzero(self.fid == f)[0]
+            n = len(sel)
+            val = max(val, e[sel[keep[sel]]].sum() / n)
+            bound = max(bound, ((g + C_ERR * U) * np.abs(e[sel]).sum() + U * a[sel].sum()) / n)
+        return val, bound, D
 
     def integrate(self, acc, dt):
         """The velocity change of the integration (dfsph_solver.rs:505-518): vc = acc dt, one float32 rounding."""
@@ -1030,13 +1114,15 @@ class Becker:
     """Becker2009Elasticity's passes (becker2009_elasticity.rs:84-334) over the rest contacts: the same-fluid contacts of
     the rest positions Q (self included), always with the cubic spline.  Particles are in the fluids' original order, fluids
     concatenated; fid: the fluid of each, mass: float32 masses.  rest: other contacts to use (a kernel that recaptures its
-    lists)."""
+    lists).  rows: rest contacts of these particles only (contacts_rows; the passes are exact at the rows)."""
 
-    def __init__(self, h, Q, fid, mass, young, poisson, nonlinear, rest=None):
+    def __init__(self, h, Q, fid, mass, young, poisson, nonlinear, rest=None, rows=None):
         self.h = float(F(h))
         self.N, self.mass, self.nonlinear, self.fid = len(Q), _f64(mass), nonlinear, np.asarray(fid)
         same = lambda i, j: fid[i] == fid[j]  # noqa: E731
-        self.rest = contacts(Q, Q, self.h, same, same=True) if rest is None else rest
+        if rest is None:
+            rest = contacts(Q, Q, self.h, same, same=True) if rows is None else contacts_rows(Q, Q, self.h, same, rows)
+        self.rest = rest
         r = self.rest
         E, nu, one, two = F(young), F(poisson), F(1.0), F(2.0)   # elasticity_coefficients :15-25, in float32 as solved
         self.d0 = float(F((E * (one - nu)) / ((one + nu) * (one - two * nu))))
@@ -1167,6 +1253,73 @@ class Becker:
 
         t, tA, tK = terms(self.g, False), terms(np.abs(self.g), True), terms(self.ge, True)
         return Ref(_sum(N, r.i, t), _sum(N, r.i, tA), _sum(N, r.i, tK), self.n)
+
+
+def _tree_levels(threads):
+    """Additions on the longest path of block_sum (sph_kernels.cuh) over `threads` lanes: warp_sum's five butterfly levels,
+    then warp_sum again over the ceil(threads / 32) warp sums, padded with zeros (adding 0 is exact, so only
+    ceil(log2(warps)) of those five levels round)."""
+    warps = -(-threads // 32)
+    return 5 + int(np.ceil(np.log2(warps))) if warps > 1 else 5
+
+
+def structural_depth(n, block, second):
+    """The depth D of the float32 loop-error reduction of n terms, derived from the kernels:
+      1. each pass block of `block` threads sums one term per thread with block_sum's fixed tree (reduce_error in
+         sph_passes.cuh; the neighbour search's fused first evaluation sums each warp, then the last warp to arrive sums
+         the NBR_T / 32 warp sums, the same shape): _tree_levels(block) roundings on any term's path;
+      2. the block that sums the nblk = ceil(n / block) partials (a pass's last block by ticket, blockDim = PASS_T, or
+         k_reduce_partials with 256 threads) runs thread t over partials t, t + T, t + 2T, ... into s = 0: at most
+         ceil(nblk / T) terms, of which the first is added to 0 exactly, so ceil(nblk / T) - 1 roundings;
+      3. block_sum over those T per-thread sums: _tree_levels(T) roundings.
+    Every term's path through this tree has at most D = (1) + (2) + (3) roundings of relative size u, so the float32
+    result differs from the exact sum by at most gamma_D sum |e|, gamma_D = D u / (1 - D u) (Higham, Accuracy and
+    Stability, 4.2), whatever the values.  At C3 (n = 10 077 696, 78 732 blocks of 128) D = 7 + 615 + 7 = 629 for a
+    pass's last block and 7 + 307 + 8 = 322 for k_reduce_partials, against the n + 4 of the any-order bound.
+    Sensitivity: losing every partial past block 65 535 (16.8 % of the terms at C3) is about 4000 times this bound;
+    losing one block of 128 terms (1.3e-5 of the sum) lies below it (gamma_629 = 3.7e-5), so no honest bound can see that at
+    this size: the small scenes' error_drops_last_block mutant covers it."""
+    nblk = -(-max(n, 1) // block)
+    return _tree_levels(block) + max(-(-nblk // second) - 1, 0) + _tree_levels(second)
+
+
+def emulate_reduction(e, block, second):
+    """The float32 value of the reduction structural_depth describes, emulated in numpy: e (float32, n terms) in blocks
+    of `block`, warp butterflies, the warp-sum tree, the strided per-thread sums of the partials and the final block tree.
+    Returns (float32 result, float32 partials)."""
+    e = np.asarray(e, F)
+    nblk = -(-len(e) // block)
+    x = np.zeros(nblk * block, F)
+    x[:len(e)] = e
+    part = _block_sum(x.reshape(nblk, block))
+    T = second
+    m = -(-nblk // T)
+    y = np.zeros(m * T, F)
+    y[:nblk] = part
+    y = y.reshape(m, T)
+    s = np.zeros(T, F)
+    for k in range(m):
+        s = (s + y[k]).astype(F)
+    return _block_sum(s[None, :])[0], part
+
+
+def _block_sum(x):
+    """block_sum over the last axis (float32): warp_sum per 32 lanes, then warp_sum over the warp sums padded to 32."""
+    rows, t = x.shape
+    w = -(-t // 32)
+    v = np.zeros((rows, w * 32), F)
+    v[:, :t] = x
+    v = _warp_sum(v.reshape(rows, w, 32))
+    pad = np.zeros((rows, 32), F)
+    pad[:, :w] = v[:, :, 0]
+    return _warp_sum(pad)[:, 0]
+
+
+def _warp_sum(v):
+    lane = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        v = (v + v[..., lane ^ o]).astype(F)
+    return v
 
 
 def from_matrix_eps(A, R0, eps=EPS32, max_iter=20):

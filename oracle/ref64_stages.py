@@ -134,15 +134,22 @@ def scene_pairs():
     return dict(fluids=[_fluid(pts, 13)], boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 7))])
 
 
-def _pass_t():
-    """Threads per block of the gather passes: SPH_PASS_T's default in sph_kernels.cuh, so the tail scenes follow it."""
+def _kernels_constant(pattern):
     import os
     import re
     src = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "salva_b200", "csrc", "sph_kernels.cuh")
-    return int(re.search(r"#define SPH_PASS_T (\d+)", open(src).read()).group(1))
+    return int(re.search(pattern, open(src).read()).group(1))
+
+
+def _pass_t():
+    """Threads per block of the gather passes: SPH_PASS_T's default in sph_kernels.cuh, so the tail scenes follow it."""
+    return _kernels_constant(r"#define SPH_PASS_T (\d+)")
 
 
 PASS_T = _pass_t()
+NBR_T = _kernels_constant(r"constexpr int NBR_T = (\d+);")   # threads per block of the neighbour search
+SCAN_B = _kernels_constant(r"SCAN_T = (\d+)") * _kernels_constant(r"SCAN_I = (\d+)")   # entries per block of the cell-table scan
+REDUCE_T = 256                                                 # threads of k_reduce_partials (read_error)
 TAILS = (1, 31, 32, 33, PASS_T - 1, PASS_T + 1)
 
 
@@ -299,14 +306,15 @@ def _read(world, fh, bh, extra=()):
 
 
 def run(make_world, scene, iters=None, forces=(), first=None, extra=(), steps=None, **world_kw):
-    """Step a fresh world once at DT with force_iterations(*iters) (iters None: the solver's own loops), or twice when
+    """Step a fresh world once at the scene's dt with force_iterations(*iters) (iters None: the solver's own loops), or twice when
     `first` gives the first step's iterations; gravity 0.  Returns the observables after the last step and, for two steps,
     those after the first.
     steps: a list of (dt, iters, gravity) instead, one per step (an entry of iters may be None: that loop runs free);
     returns the list of observables after every step.
     extra: further debug selectors to read (IISPH_SCRATCH); world_kw goes to make_world (min / max_divergence_iter,
     max_divergence_error, min / max_pressure_iter, max_density_error)."""
-    seq = steps if steps is not None else ([(DT, first, ZERO_G)] if first is not None else []) + [(DT, iters, ZERO_G)]
+    dt = timestep(scene)
+    seq = steps if steps is not None else ([(dt, first, ZERO_G)] if first is not None else []) + [(dt, iters, ZERO_G)]
     w = make_world(**world_kw)
     fh, bh = populate(w, scene, forces)
     outs = []
@@ -322,12 +330,23 @@ def run(make_world, scene, iters=None, forces=(), first=None, extra=(), steps=No
     return outs[-1], (outs[0] if first is not None else None)
 
 
-def passes_for(scene, P=None, kw=0, kg=0):
-    """ref64.Passes of a scene (on positions P, default the scene's own)."""
+def radius(scene):
+    """The scene's particle radius (R unless it says otherwise)."""
+    return float(scene.get("particle_radius", R))
+
+
+def timestep(scene):
+    """The scene's step length (DT unless it says otherwise)."""
+    return float(scene.get("dt", DT))
+
+
+def passes_for(scene, P=None, kw=0, kg=0, rows=None):
+    """ref64.Passes of a scene (on positions P, default the scene's own), h and the default volume from its particle
+    radius; rows: ref64.Passes' rows mode."""
     fl, bd = scene["fluids"], scene["boundaries"]
     pos = np.concatenate([f["positions"] for f in fl]).astype(F) if P is None else P
     fid = np.concatenate([np.full(len(f["positions"]), k) for k, f in enumerate(fl)])
-    r = F(R)
+    r = F(radius(scene))
     vdef = r * r * r * F(8.0 * 0.8)
     vol = np.concatenate([np.full(len(f["positions"]), vdef, F) if f.get("volumes") is None else np.asarray(f["volumes"], F)
                           for f in fl])
@@ -356,7 +375,71 @@ def passes_for(scene, P=None, kw=0, kg=0):
         return (a == b) | test(bm[a], bf_[a], bm[b], bf_[b])
 
     h = F(r * F(2.0) * F(2.0))
-    return ref64.Passes(h, pos, fid, rho0, mass, bp, bid, allowed_ff, allowed_fb, allowed_bb, kw=kw, kg=kg)
+    return ref64.Passes(h, pos, fid, rho0, mass, bp, bid, allowed_ff, allowed_fb, allowed_bb, kw=kw, kg=kg, rows=rows)
+
+
+# ---- full-size scenes: counts for every particle, the cell table, and the sample the passes are compared on -------------
+def exact_counts(P, Q, h, tree=None):
+    """Per point of P, the number of points of Q the float32 test d^2 <= h^2 accepts (every pair allowed; Q is P: self
+    included).  Points within h (1 - 1e-5) in float64 are accepted and points beyond h (1 + 1e-5) rejected whatever the
+    float32 roundings (a few ulp of d^2), so the k-d tree counts at those two radii settle every particle where they
+    agree; the others get the exact test on their candidates."""
+    h = float(F(h))
+    t = ref64.cKDTree(np.asarray(Q, np.float64)) if tree is None else tree
+    P64 = np.asarray(P, np.float64)
+    lo = t.query_ball_point(P64, h * (1.0 - 1e-5), return_length=True, workers=-1)
+    hi = t.query_ball_point(P64, h * (1.0 + 1e-5), return_length=True, workers=-1)
+    out = np.asarray(hi, np.int64)
+    edge = np.nonzero(lo != hi)[0]
+    if len(edge):
+        pr = ref64.contacts_rows(np.asarray(P, F), np.asarray(Q, F), h, lambda i, j: np.ones(len(i), bool), edge, tree=t)
+        out[edge] = np.bincount(pr.i, minlength=len(P))[edge]
+    return out, len(edge)
+
+
+def cell_table(P, BP, h, xysub):
+    """The engine's dense cell table for these fluid and boundary positions (phase_grid, cell_id, abin): the cell of
+    every fluid particle as its table index, and the grid dims (cells of width h, one padding cell each side).  In row
+    order (xysub > 1) x and y count bins of h / xysub and z runs fastest.  Returns (index, dims, table length)."""
+    h32 = F(h)
+
+    def coords(X):
+        q = (np.asarray(X, F) / h32).astype(F)    # IEEE division, as __fdiv_rn
+        fl = np.floor(q)
+        return q, fl, fl.astype(np.int64)
+
+    _, _, cp = coords(P)
+    lo = cp.min(axis=0)
+    hi = cp.max(axis=0)
+    if len(BP):
+        _, _, cb = coords(BP)
+        lo, hi = np.minimum(lo, cb.min(axis=0)), np.maximum(hi, cb.max(axis=0))
+    dims = hi - lo + 3
+    q, fl, c = coords(P)
+    b = c.copy()
+    if xysub > 1:
+        for a in (0, 1):
+            b[:, a] = c[:, a] * xysub + np.minimum(xysub - 1, ((q[:, a] - fl[:, a]) * F(xysub)).astype(np.int64))
+    ox, oy, oz = (lo[0] - 1) * xysub, (lo[1] - 1) * xysub, lo[2] - 1
+    ny, nz = dims[1] * xysub, dims[2]
+    idx = ((b[:, 0] - ox) * ny + (b[:, 1] - oy)) * nz + (b[:, 2] - oz)
+    return idx, dims, int(dims.prod()) * xysub * xysub + 1
+
+
+def full_size_rows(idx, nb, n_random, seed, near=2):
+    """The particles a full-size run compares pass by pass: n_random seeded random ones; every particle with a boundary
+    contact (nb > 0); those of the first and the last occupied cell; and those of the cells whose table index lies within
+    `near` of a multiple of SCAN_B or of SCAN_B^2 (the scan's block and level seams)."""
+    rng = np.random.default_rng(seed)
+    n = len(idx)
+    pick = [rng.choice(n, size=min(n_random, n), replace=False), np.nonzero(nb > 0)[0]]
+    pick += [np.nonzero(idx == idx.min())[0], np.nonzero(idx == idx.max())[0]]
+    seam = np.zeros(n, bool)
+    for m in (SCAN_B, SCAN_B * SCAN_B):
+        r = idx % m
+        seam |= (r <= near) | (r >= m - near)
+    pick.append(np.nonzero(seam)[0])
+    return np.unique(np.concatenate(pick))
 
 
 # ---- the checks ----------------------------------------------------------------------------------------------------------------
@@ -396,11 +479,14 @@ def alpha_ratio(ps, alpha, bvol, rho0_b=None):
 
 class Checks:
     """Runs the stages of one scene on one world kind and keeps the worst |err| / bound per pass.  `mutant` applies one
-    plausible kernel bug to the reference instead (a bound that passes the mutant too is too loose)."""
+    plausible kernel bug to the reference instead (a bound that passes the mutant too is too loose).  rows: compare at these
+    particles only (ref64.Passes' rows mode; boundary sums at the boundary particles whose contacts are all rows); h, the
+    default volume and dt come from the scene."""
 
-    def __init__(self, make_world, scene, kw=0, kg=0, mutant=None):
+    def __init__(self, make_world, scene, kw=0, kg=0, mutant=None, rows=None):
         self.make_world, self.scene, self.mutant = make_world, scene, mutant
-        self.ps = passes_for(scene, kw=kw, kg=kg)
+        self.r, self.dt = radius(scene), timestep(scene)
+        self.ps = passes_for(scene, kw=kw, kg=kg, rows=rows)
         self.worst, self.excluded, self.clamp, self.errors, self.nonzero = {}, {}, {}, {}, {}
         ps = self.ps
         self.ff, self.fb = ps.ff, ps.fb
@@ -427,7 +513,13 @@ class Checks:
         t = ref64.grad_threshold(ps.kg, ps.h)
         ex = np.zeros(len(self.want), bool)
         ex[ps.fb.j[np.abs(ps.fb.d2 - t) <= 8 * ref64.U * t]] = True
-        r = np.where(ex | ~self.want, 0.0, r)
+        off = ~self.want
+        if ps.brows is not None:
+            off = off.copy()
+            whole = np.zeros(len(off), bool)
+            whole[ps.brows] = True
+            off |= ~whole
+        r = np.where(ex | off, 0.0, r)
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()))
         self.excluded[name] = self.excluded.get(name, 0) + int((ex & self.want).sum())
 
@@ -440,6 +532,8 @@ class Checks:
             r = r.max(axis=1)
         amb = ps.ambiguous() if ambiguous else np.zeros(len(r), bool)
         ex = amb if exclude is None else exclude | amb
+        if ps.rows is not None:
+            r, ex = r[ps.rows], ex[ps.rows]
         r = np.where(ex, 0.0, r)
         self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()) if len(r) else 0.0)
         self.excluded[name] = self.excluded.get(name, 0) + int(ex.sum())
@@ -458,6 +552,8 @@ class Checks:
         nf, nb = o00["num_fluid_contacts"].astype(np.int64), o00["num_boundary_contacts"].astype(np.int64)
         self.nf, self.nb = nf, nb
         cnt = np.where((nf == np.bincount(self.ff.i, minlength=ps.N)) & (nb == np.bincount(self.fb.i, minlength=ps.N)), 0.0, np.inf)
+        if ps.rows is not None:
+            cnt = cnt[ps.rows]
         self.worst["counts"] = float(cnt.max()) if len(cnt) else 0.0
         bvol = o00["bvol"]
         if len(bvol):
@@ -478,9 +574,9 @@ class Checks:
         self.record("divergence_sweep", o00["divergence"],
                     ps.divergence(V0, bvol, vj=self._vj(V0, self.ff), min_neighbors=self.min_nb, **kw), C_PASS["divergence"])
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
-        vs = (o00["V"] + (o00["acceleration"] * F(DT)).astype(F)).astype(F)
+        vs = (o00["V"] + (o00["acceleration"] * F(self.dt)).astype(F)).astype(F)
         self.record("predicted", o00["predicted_density"],
-                    ps.divergence(vs, bvol, predicted=True, bvel=bvel, dens=o00["density"], dt=DT, vj=self._vj(vs, self.ff), **kw),
+                    ps.divergence(vs, bvol, predicted=True, bvel=bvel, dens=o00["density"], dt=self.dt, vj=self._vj(vs, self.ff), **kw),
                     C_PASS["predicted"])
         o10, _ = run(self.make_world, sc, (1, 0))
         kappa = (o00["divergence"] * o00["alpha"]).astype(F)
@@ -492,8 +588,8 @@ class Checks:
         rho0 = ps.rho0.astype(F)
         kraw = ((o10["predicted_density"] - rho0).astype(F) * o10["alpha"]).astype(F)
         kp = np.maximum(kraw, F(0))
-        inv_dt = F(1.0) / F(DT)
-        vc0 = (o11["acceleration"] * F(DT)).astype(F)
+        inv_dt = F(1.0) / F(self.dt)
+        vc0 = (o11["acceleration"] * F(self.dt)).astype(F)
         kb = kraw if self.mutant == "no_kappa_gate" else None
         self.record("pressure_update", o11["velocity_change"],
                     ps.update(kp, bvol, vc0, pressure=True, inv_dt=inv_dt, kappa_b=kb, **kw), C_PASS["update"])
@@ -529,37 +625,38 @@ class Checks:
         dens = o0["density"]
         V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
-        pred = ps.divergence(V0, bvol, predicted=True, bvel=bvel, dens=dens, dt=DT, **kw)
+        pred = ps.divergence(V0, bvol, predicted=True, bvel=bvel, dens=dens, dt=self.dt, **kw)
         self.record("predicted", o0["predicted_density"], pred, C_PASS["predicted"])
-        self.record("dii", o0["dii"], ps.iisph_dii(dens, bvol, DT, **kw), C_PASS["iisph_dii"])
+        self.record("dii", o0["dii"], ps.iisph_dii(dens, bvol, self.dt, **kw), C_PASS["iisph_dii"])
         dji_mass = ps.mass[self.ff.j] if m == "dji_mass_j" else None
-        self.record("aii", o0["aii"], ps.iisph_aii(dens, o0["dii"], bvol, DT, dji_mass=dji_mass, **kw), C_PASS["iisph_aii"])
+        self.record("aii", o0["aii"], ps.iisph_aii(dens, o0["dii"], bvol, self.dt, dji_mass=dji_mass, **kw), C_PASS["iisph_aii"])
         self.worst["pressure_0"] = 0.0 if not o0["pressure"].any() and np.array_equal(o0["V"], V0) else np.inf
 
         pk = dict(dji_mass=dji_mass, s_dii_p=m != "s_without_dii_p", boundary=m != "next_p_no_boundary", **kw)
         relax = m != "no_relaxation"
         o1, _ = run(self.make_world, sc, (0, 1), extra=X)
         ref, raw = ps.iisph_next_pressure(o1["density"], pred.value, o0["pressure"], o1["aii"], o1["dii"], o1["dij_pjl"], bvol,
-                                          DT, omega, pred_err=pred.bound(C_PASS["predicted"]), relax=relax, **pk)
+                                          self.dt, omega, pred_err=pred.bound(C_PASS["predicted"]), relax=relax, **pk)
         self._pressure("pressure_1", o1["pressure"], ref, raw)
         p1 = o1["pressure"]
-        self.record("velocity", o1["V"], ps.iisph_velocity(dens, p1, V0, bvol, DT, prho_i_twice=m == "velocity_prho_i_twice", **kw),
+        self.record("velocity", o1["V"], ps.iisph_velocity(dens, p1, V0, bvol, self.dt, prho_i_twice=m == "velocity_prho_i_twice", **kw),
                     C_PASS["iisph_velocity"])
         self.record_boundary("boundary_force_iisph", o1["bforce"],
                              ps.iisph_boundary_force(dens, p1, bvol, rho0_b=self.rho0_b, with_mass=m != "iisph_bforce_no_mass"))
 
         o2, _ = run(self.make_world, sc, (0, 2), extra=X)
-        self.record("dij_pjl", o2["dij_pjl"], ps.iisph_dij_pjl(dens, p1, DT, prho_i=m == "dij_prho_i", ff=self.ff),
+        self.record("dij_pjl", o2["dij_pjl"], ps.iisph_dij_pjl(dens, p1, self.dt, prho_i=m == "dij_prho_i", ff=self.ff),
                     C_PASS["iisph_dij_pjl"])
-        ref, raw = ps.iisph_next_pressure(dens, o2["predicted_density"], p1, o2["aii"], o2["dii"], o2["dij_pjl"], bvol, DT, omega,
+        ref, raw = ps.iisph_next_pressure(dens, o2["predicted_density"], p1, o2["aii"], o2["dii"], o2["dij_pjl"], bvol, self.dt, omega,
                                           relax=relax, **pk)
         self._pressure("pressure_2", o2["pressure"], ref, raw)
 
-        for k, p_prev in ((1, o0["pressure"]), (2, p1)):
+        # the density error sums over every particle: not in rows mode (a full-size run checks the loop errors on their own)
+        for k, p_prev in ((1, o0["pressure"]), (2, p1)) if ps.rows is None else ():
             o, _ = run(self.make_world, sc, None, extra=X, min_pressure_iter=k, max_pressure_iter=k)
             assert o["stats"]["n_pressure_iter"] == k, o["stats"]
             v, b, amb = ps.iisph_density_error(o["density"], o["predicted_density"], p_prev, o["aii"], o["dii"], o["dij_pjl"],
-                                               o["bvol"], DT, omega, C_PASS["iisph_pressure"],
+                                               o["bvol"], self.dt, omega, C_PASS["iisph_pressure"],
                                                count_clamped=m == "error_counts_clamped", relax=relax, **pk)
             err = abs(float(o["stats"]["last_density_error"]) - v)
             self.worst["density_error"] = max(self.worst.get("density_error", 0.0), err / b if b > 0 else (0.0 if err == 0 else np.inf))
@@ -568,17 +665,19 @@ class Checks:
         self.iisph_warm(omega=omega)
         return o0
 
-    def iisph_warm(self, dts=(DT, DT), omega=0.5):
+    def iisph_warm(self, dts=None, omega=0.5):
         """The warm-started IISPH step: step 1 at dts[0] with (0, 2), step 2 at dts[1] with (0, 1) on contacts re-derived on
         P1.  dii, aii (fed dii read back), dij_pjl and p (fed 0.5 p_2 of each particle, which checks that pressures ride
         the step's counting sort) all use the current step's dt: IISPH advances the timestep before its passes
         (iisph_solver.rs)."""
+        dts = (self.dt, self.dt) if dts is None else dts
         sc, ps, m = self.scene, self.ps, self.mutant
         tag = "" if dts[0] == dts[1] else "_dt_change"
         dt = dts[0] if m == "iisph_previous_dt" else dts[1]
         o1w, o2w = run(self.make_world, sc, steps=[(dts[0], (0, 2), ZERO_G), (dts[1], (0, 1), ZERO_G)], extra=IISPH_SCRATCH)
-        ps1 = passes_for(sc, P=o1w["P"], kw=ps.kw, kg=ps.kg)
-        assert np.array_equal(o2w["num_fluid_contacts"], ps1.nf) and np.array_equal(o2w["num_boundary_contacts"], ps1.nb)
+        ps1 = passes_for(sc, P=o1w["P"], kw=ps.kw, kg=ps.kg, rows=ps.rows)
+        at = slice(None) if ps.rows is None else ps.rows
+        assert np.array_equal(o2w["num_fluid_contacts"][at], ps1.nf[at]) and np.array_equal(o2w["num_boundary_contacts"][at], ps1.nb[at])
         dens, bvol = o2w["density"], o2w["bvol"]
         self.record("dii_warm" + tag, o2w["dii"], ps1.iisph_dii(dens, bvol, dt, rho0_b=self.rho0_b), C_PASS["iisph_dii"], ps=ps1)
         self.record("aii_warm" + tag, o2w["aii"], ps1.iisph_aii(dens, o2w["dii"], bvol, dt, rho0_b=self.rho0_b), C_PASS["iisph_aii"],
@@ -604,6 +703,8 @@ class Checks:
 
     def _alpha(self, alpha, bvol):
         r, ex = alpha_ratio(self.ps, alpha, bvol, self.rho0_b)
+        if self.ps.rows is not None:
+            r, ex = r[self.ps.rows], ex[self.ps.rows]
         self.worst["alpha"] = float(r.max()) if len(r) else 0.0
         self.excluded["alpha"] = int(ex.sum())
 
@@ -622,14 +723,14 @@ class Checks:
                 assert o["stats"]["n_divergence_iter"] == 1 and o["stats"]["n_divergence_eval"] == 1
             if adhesion != 0 and it is not None:   # the free-running pressure loop adds its own boundary forces
                 self.record_boundary("boundary_force_adhesion", o["bforce"], ps.adhesion_boundary_force(adhesion, o["bvol"]))
-            rho_j = o["density"][self.ps.ff.i] if self.mutant == "normals_rho_i" else None
-            ref = ps.akinci(o["density"], gamma, adhesion, o["bvol"], rho_j=rho_j, ff=self.ff, fb=self.fb)
+            ref = ps.akinci(o["density"], gamma, adhesion, o["bvol"], rho_i_for_j=self.mutant == "normals_rho_i", ff=self.ff, fb=self.fb)
             acc = o["acceleration"]
             assert np.isfinite(acc).all(), "%s: non-finite accelerations at %s" % (name, np.nonzero(~np.isfinite(acc).all(1))[0][:8])
             self.record(name, acc, ref, C_PASS["akinci"])
 
-    def xsph(self, cf=0.5, cb=0.0, dts=(DT, DT)):
+    def xsph(self, cf=0.5, cb=0.0, dts=None):
         """dts: the two steps' dt; step 2's XSPH sees the first one's inv_dt."""
+        dts = (self.dt, self.dt) if dts is None else dts
         from salva_b200 import scenes
         sc = self.scene
         forces = [scenes.xsph_viscosity(cf, cb)]
@@ -638,31 +739,37 @@ class Checks:
         inv_dt = F(1.0) / F(dts[1] if self.mutant == "xsph_current_inv_dt" else dts[0])
         for it, name in (((1, 0), "xsph_after_update" + tag), ((0, 0), "xsph_separate" + tag)):
             o1, o2 = run(self.make_world, sc, forces=forces, steps=[(dts[0], (1, 0), ZERO_G), (dts[1], it, ZERO_G)])
-            ps1 = passes_for(sc, P=o1["P"], kw=self.ps.kw, kg=self.ps.kg)
-            assert np.array_equal(o2["num_fluid_contacts"], np.bincount(ps1.ff.i, minlength=ps1.N))
+            ps1 = passes_for(sc, P=o1["P"], kw=self.ps.kw, kg=self.ps.kg, rows=self.ps.rows)
+            at = slice(None) if ps1.rows is None else ps1.rows
+            assert np.array_equal(o2["num_fluid_contacts"][at], np.bincount(ps1.ff.i, minlength=ps1.N)[at])
             ref = ps1.xsph(o2["V"], o2["density"], cf, cb, inv_dt, bvel, o2["bvol"])
-            r = ref64.ratio(o2["acceleration"], ref, C_PASS["xsph"]).max(axis=1)
-            r = np.where(ps1.ambiguous(), 0.0, r)
+            r = ref64.ratio(o2["acceleration"], ref, C_PASS["xsph"]).max(axis=1)[at]
+            amb = ps1.ambiguous()[at]
+            r = np.where(amb, 0.0, r)
             self.worst[name] = max(self.worst.get(name, 0.0), float(r.max()))
-            self.excluded[name] = self.excluded.get(name, 0) + int(ps1.ambiguous().sum())
+            self.excluded[name] = self.excluded.get(name, 0) + int(amb.sum())
             if it == (0, 0) and cb != 0:   # no update on step 2: the forces are XSPH's alone
                 self.record_boundary("boundary_force_xsph" + tag, o2["bforce"],
                                      ps1.xsph_boundary_force(o2["V"], o2["density"], cb, inv_dt, bvel, o2["bvol"]), ps=ps1)
 
-    def artificial(self, cf=1.0, cb=0.0, alpha=1.0, beta=0.0, cs=10.0):
+    def artificial(self, cf=1.0, cb=0.0, alpha=1.0, beta=0.0, cs=10.0, iisph=False):
         """ArtificialViscosity on the first step, with no update (0, 0) and after one (1, 0): it does not depend on dt, so
         the acceleration is its sum over the velocities the loop left and the step's densities.  Its boundary force is the
         running sum of the particle's boundary term (artificial_viscosity.rs:117), which depends on the order of the
-        contact list, so it is not compared here."""
+        contact list, so it is not compared here.  iisph: a world with the IISPH solver, whose forces run before the
+        pressure solve on the velocities the step starts from (iisph_solver.rs:653-660) and whose step ends by adding the
+        velocity change to them, so the reference is fed the scene's velocities, (0, 0) only."""
         from salva_b200 import scenes
         sc = self.scene
         forces = [scenes.artificial_viscosity(cf, cb, alpha, beta, cs)]
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
-        for it, name in (((0, 0), "artificial_no_update"), ((1, 0), "artificial_after_update")):
+        V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
+        for it, name in (((0, 0), "artificial_no_update"),) + ((((1, 0), "artificial_after_update"),) if not iisph else ()):
             o, _ = run(self.make_world, sc, it, forces)
-            ref, amb = self.ps.artificial(o["V"], o["density"], cf, cb, alpha, beta, cs, bvel, o["bvol"],
+            ref, amb = self.ps.artificial(V0 if iisph else o["V"], o["density"], cf, cb, alpha, beta, cs, bvel, o["bvol"],
                                           vr_gate=self.mutant != "artificial_no_vr_gate")
-            assert amb.mean() <= 0.02, "%s: %d of %d particles at the v_r < 0 decision" % (name, amb.sum(), len(amb))
+            at = amb if self.ps.rows is None else amb[self.ps.rows]
+            assert at.mean() <= 0.02, "%s: %d of %d particles at the v_r < 0 decision" % (name, at.sum(), len(at))
             self.record(name, o["acceleration"], ref, C_PASS["artificial"], exclude=amb)
 
     def wcsph(self, cf=0.5):
@@ -695,7 +802,7 @@ class Checks:
             ref = ref64.Ref(np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros((nb, 3)), np.zeros(nb))
         self.record_boundary("boundary_force_he2014", o["bforce"], ref)
 
-    def viscosity(self, visc=0.5, wcsph=0.0, dts=(DT, DT)):
+    def viscosity(self, visc=0.5, wcsph=0.0, dts=None):
         """DFSPHViscosity.  Forces see the previous step's dt, 0 on the first step, so (as for XSPH) step 1 with (1, 0),
         then step 2 with (0, 0) on positions P1, the velocities V2 and the densities of step 2, once with
         max_viscosity_iter = 1 and once with 2 (max_viscosity_error = 0: no early break).  Each pass fed what its kernel
@@ -703,6 +810,7 @@ class Checks:
         beta and target read back) and after two (vv on the acceleration read back from the one-update run).  wcsph: a
         WCSPHSurfaceTension coefficient pushed before the viscosity, so that a != 0 in vv; its acceleration comes from a
         run with WCSPH alone.  dts: the two steps' dt; step 2's viscosity sees the first one's dt and inv_dt."""
+        dts = (self.dt, self.dt) if dts is None else dts
         from salva_b200 import scenes
         sc, m, kw = self.scene, self.mutant, dict(kw=self.ps.kw, kg=self.ps.kg)
         tag = ("_after_wcsph" if wcsph else "") + ("" if dts[0] == dts[1] else "_dt_change")
@@ -756,7 +864,7 @@ class Checks:
         same = lambda fid: (lambda i, j: fid[i] == fid[j])  # noqa: E731
         bk = ref64.Becker(ps.h, Q, ps.fid, ps.mass, young, poisson, nonlinear)
         tag = "nonlinear" if nonlinear else "linear"
-        w.step(DT, ZERO_G)
+        w.step(self.dt, ZERO_G)
         o = _read(w, fh, bh, EL_SCRATCH)
         self.record("el_volume", ps.mass / o["el_volume0"].astype(np.float64), bk.volume_sum(1.0 if m == "el_volume_once" else 2.0),
                     C_PASS["el_volume"], exclude=np.zeros(ps.N, bool), ambiguous=False)
@@ -769,7 +877,7 @@ class Checks:
             P = deform(o["P"], ps.fid, ang, seed=seed)
             for k, f in enumerate(fh):
                 w.write_fluid(f, positions=P[ps.fid == k])
-            w.step(DT, ZERO_G)
+            w.step(self.dt, ZERO_G)
             o = _read(w, fh, bh, EL_SCRATCH)
             self._becker_step(bk, P, o, R_prev, name + tag)
             R_prev = o["el_rotation"].reshape(ps.N, 3, 3).astype(np.float64)
@@ -778,11 +886,11 @@ class Checks:
                 self.rest_differs = int((np.bincount(bk.rest.i, minlength=ps.N) != np.bincount(cur.i, minlength=ps.N)).sum())
         # re-capture: 7 particles appended to every fluid, near particles of it
         P, vol0 = o["P"], o["el_volume0"]
-        vdef = F(R) * F(R) * F(R) * F(8.0 * 0.8)
+        vdef = F(self.r) * F(self.r) * F(self.r) * F(8.0 * 0.8)
         pos, fid, mass, old_vol, old_rot = [], [], [], [], []
         for k, f in enumerate(fh):
             sel = np.nonzero(ps.fid == k)[0]
-            new = (P[sel[5:68:9]] + np.array([0.4, 0.1, 0.2], F) * F(R)).astype(F)
+            new = (P[sel[5:68:9]] + np.array([0.4, 0.1, 0.2], F) * F(self.r)).astype(F)
             w.append_particles(f, new)
             pos += [P[sel], new]
             fid += [np.full(len(sel) + len(new), k)]
@@ -790,7 +898,7 @@ class Checks:
             old_vol += [vol0[sel], np.zeros(len(new))]
             old_rot += [R_prev[sel], np.tile(np.eye(3), (len(new), 1, 1))]
         Q4, fid4, mass4 = np.concatenate(pos).astype(F), np.concatenate(fid), np.concatenate(mass).astype(F)
-        w.step(DT, ZERO_G)
+        w.step(self.dt, ZERO_G)
         o = _read(w, fh, bh, EL_SCRATCH)
         bk4 = ref64.Becker(ps.h, Q4, fid4, mass4, young, poisson, nonlinear)
         old = np.zeros(len(Q4)) if m == "el_recapture_no_old_volumes" else np.concatenate(old_vol)
@@ -800,6 +908,22 @@ class Checks:
         self._becker_step(bk4, Q4, o, np.concatenate(old_rot), "el_recaptured_" + tag)
         if hasattr(w, "close"):
             w.close()
+
+    def becker_capture(self, young=1.0e5, poisson=0.3, nonlinear=True):
+        """Becker2009Elasticity on the step that captures the rest pose, with no update (0, 0): the rest volumes, A_pq and
+        the rotation (within its bound of the polar rotation, I here), grad_tr, stress and force, each fed what its kernel
+        read (the neighbours' rotations, stresses and rest volumes read back).  Works in rows mode (the rest contacts of
+        the rows only)."""
+        from salva_b200 import scenes
+        ps, sc = self.ps, self.scene
+        forces = [scenes.becker2009_elasticity(young, poisson, nonlinear)]
+        o, _ = run(self.make_world, sc, (0, 0), forces, extra=EL_SCRATCH)
+        Q = np.concatenate([f["positions"] for f in sc["fluids"]]).astype(F)
+        bk = ref64.Becker(ps.h, Q, ps.fid, ps.mass, young, poisson, nonlinear, rows=ps.rows)
+        self.record("el_volume", ps.mass / o["el_volume0"].astype(np.float64), bk.volume_sum(), C_PASS["el_volume"],
+                    exclude=np.zeros(ps.N, bool), ambiguous=False)
+        self._becker_step(bk, Q, o, np.tile(np.eye(3), (ps.N, 1, 1)), "el_capture_" + ("nonlinear" if nonlinear else "linear"))
+        return o
 
     def _becker_step(self, bk, P, o, R_prev, name):
         N, m = bk.N, self.mutant
@@ -820,7 +944,8 @@ class Checks:
         gap = np.abs(Rref - bk.polar(bk.apq(P, C_PASS["el_apq"])[0])).max(axis=(1, 2))
         self.el_polar_gap = max(getattr(self, "el_polar_gap", 0.0), float(gap[ok].max()) if ok.any() else 0.0)
         self.worst[name + "_rotation"] = max(self.worst.get(name + "_rotation", 0.0), float(r.max()))
-        self.excluded[name + "_rotation"] = self.excluded.get(name + "_rotation", 0) + int(ex.sum())
+        at = self.ps.rows if self.ps.rows is not None and N == self.ps.N else slice(None)   # rows mode: A_pq is whole there
+        self.excluded[name + "_rotation"] = self.excluded.get(name + "_rotation", 0) + int(ex[at].sum())
         self.worst[name + "_orthonormal"] = max(self.worst.get(name + "_orthonormal", 0.0), float(ortho.max()))
         kw = dict(exclude=none, ambiguous=False)
         self.record(name + "_grad_tr", G.reshape(N, 9), bk.grad_tr(P, R, o["el_volume0"]), C_PASS["el_grad_tr"], **kw)
@@ -847,7 +972,7 @@ class Checks:
             vc = np.zeros_like(vc)
         return (o["V"] + vc).astype(F)
 
-    def loop_errors(self, dts=(DT,), forces=()):
+    def loop_errors(self, dts=None, forces=()):
         """The errors the DFSPH loops break on (stats last_divergence_error, last_density_error), on the last of the steps
         `dts` (the ones before it pinned at (1, 1), so that it starts from a carried vc and a different dt_prev), with the
         loop free-running but held to min = max = k: the engine reads the error back only where the loop may break.
@@ -858,6 +983,7 @@ class Checks:
         fluid (XSPH and Akinci2013 fuse into the divergence evaluations of a single uniform-mass fluid).
         nonzero: on a first step, per loop, the fewest nonzero error terms of any non-empty fluid, so that a dropped
         partial shows (after a step the expanding scenes leave some small fluids with no compressing particle)."""
+        dts = (self.dt,) if dts is None else dts
         sc, m = self.scene, self.mutant
         pre = [(dt, (1, 1), ZERO_G) for dt in dts[:-1]]
         dt = dts[-1]
@@ -897,6 +1023,34 @@ class Checks:
             ref = ps.divergence(vs, p["bvol"], predicted=True, bvel=bvel, dens=p["density"], dt=dt)
             self._error("density_error%s" % tag, gpu, *ps.loop_error("density", ref, C_PASS["predicted"], mutant=m))
 
+    def loop_errors_read(self):
+        """The errors both DFSPH loops break on (stats last_divergence_error, last_density_error), fed the values read back,
+        over every particle, against ref64's structural bound: the loops held to min = max = k for k = 1, 2.  Divergence
+        k = 1 is evaluation 0, which the neighbour search sums per block of NBR_T and read_error's k_reduce_partials over
+        the blocks; every other evaluation is a pass of PASS_T whose last block sums the partials.  Also checks that the
+        bound flags the loss of every partial past block 65 535 (when there are that many).  Returns the depths."""
+        sc, ps = self.scene, self.ps
+        depth = {}
+        for loop, stat, what in (("divergence", "last_divergence_error", "divergence"),
+                                 ("density", "last_density_error", "predicted_density")):
+            for k in (1, 2):
+                it = (None, 0) if loop == "divergence" else (1, None)
+                lim = dict(min_divergence_iter=k, max_divergence_iter=k) if loop == "divergence" else \
+                    dict(min_pressure_iter=k, max_pressure_iter=k)
+                o, _ = run(self.make_world, sc, it, **lim)
+                n_eval = "n_divergence_eval" if loop == "divergence" else "n_pressure_eval"
+                assert o["stats"][n_eval] == k, o["stats"]
+                block, second = (NBR_T, REDUCE_T) if (loop, k) == ("divergence", 1) else (PASS_T, PASS_T)
+                name = "%s_error_read_%d" % (loop, k)
+                v, b, D = ps.loop_error_structural(loop, o[what], block, second)
+                self._error(name, o["stats"][stat], v, b)
+                depth[name] = D
+                if ps.N > 65536 * block:   # losing the partials past block 65 535 must show (when they hold any error)
+                    mv, _, _ = ps.loop_error_structural(loop, o[what], block, second, mutant="error_drops_blocks_past_65535")
+                    if mv != v:
+                        self.worst[name + "_blind_to_lost_blocks"] = 0.0 if abs(float(o["stats"][stat]) - mv) > b else np.inf
+        return depth
+
     def loop_exits(self, factor, margin=0.25):
         """min_divergence_iter = 0, so evaluation 0 may end the divergence loop.  Step 1 at DT pinned (1, 1); step 2 at
         dt = factor DT runs free, with max_divergence_error set so that the threshold max_err * inv_dt * 0.01 (float32, in
@@ -906,14 +1060,14 @@ class Checks:
         threshold under inv_dt_prev lies above e0.  Likewise max_density_error, `margin` off the density error of step
         2's evaluation 0, whose predicted densities use dt_cur."""
         sc, m = self.scene, self.mutant
-        dt = DT * factor
-        first = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G)])[-1]
+        dt = self.dt * factor
+        first = run(self.make_world, sc, steps=[(self.dt, (1, 1), ZERO_G)])[-1]
         ps = passes_for(sc, P=first["P"], kw=self.ps.kw, kg=self.ps.kg)
         e0, b0 = ps.loop_error("divergence", ps.divergence(self._vstar(first), first["bvol"]), C_PASS["divergence"])
-        inv_prev, inv_cur = F(1.0) / F(DT), F(1.0) / F(dt)
+        inv_prev, inv_cur = F(1.0) / F(self.dt), F(1.0) / F(dt)
         mde = F(e0 * (1.0 + margin) / (float(inv_prev) * 0.01))
         thr = lambda inv: float(F(F(mde * inv) * F(0.01)))  # noqa: E731
-        o = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (None, 0), ZERO_G)], min_divergence_iter=0,
+        o = run(self.make_world, sc, steps=[(self.dt, (1, 1), ZERO_G), (dt, (None, 0), ZERO_G)], min_divergence_iter=0,
                 max_divergence_error=float(mde))[-1]["stats"]
         inv = inv_cur if m == "div_threshold_current_inv_dt" else inv_prev
         ends = e0 <= thr(inv)
@@ -922,20 +1076,20 @@ class Checks:
         self.worst["divergence_" + name] = 0.0 if ok else np.inf
         # the pressure loop, the divergence loop pinned to one update: the density error of evaluation 0 with dt_cur (a
         # run pinned to stop there gives its inputs)
-        p = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (1, 0), ZERO_G)])[-1]
+        p = run(self.make_world, sc, steps=[(self.dt, (1, 1), ZERO_G), (dt, (1, 0), ZERO_G)])[-1]
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
         vs = (p["V"] + p["velocity_change"]).astype(F)
         d0, db0 = ps.loop_error("density", ps.divergence(vs, p["bvol"], predicted=True, bvel=bvel, dens=p["density"], dt=dt),
                                 C_PASS["predicted"])
         mxd = F(d0 * (1.0 + margin))
-        q = run(self.make_world, sc, steps=[(DT, (1, 1), ZERO_G), (dt, (1, None), ZERO_G)], min_pressure_iter=0,
+        q = run(self.make_world, sc, steps=[(self.dt, (1, 1), ZERO_G), (dt, (1, None), ZERO_G)], min_pressure_iter=0,
                 max_density_error=float(mxd))[-1]["stats"]
         pok = (q["n_pressure_iter"] == 0) if d0 <= float(mxd) else (q["n_pressure_iter"] >= 1)
         self.worst["density_" + name] = 0.0 if pok else np.inf
         # how far the decisions lie from the rounding: |threshold - e0| in units of e0's bound
         self.exit_margin = min(getattr(self, "exit_margin", np.inf), abs(thr(inv_prev) - e0) / b0, abs(float(mxd) - d0) / db0)
 
-    def lagging_dt(self, dts=(DT, 2 * DT, DT / 3), gravity=(0.0, -9.81, 0.0)):
+    def lagging_dt(self, dts=None, gravity=(0.0, -9.81, 0.0)):
         """Steps of varying length under gravity, each checked step pinned at (0, 0), (1, 0) and (1, 1) after the steps
         before it at (1, 1).  The divergence loop and the forces run before timestep.advance and see the previous step's dt
         (dfsph_solver.rs:686-702); the pressure loop, the integration and the positions see the current one.  Per particle:
@@ -950,6 +1104,7 @@ class Checks:
         checked step's predecessor.  The engine's grid has its own origin and cell order, so this is a proxy for how many
         particles the counting sort moved, not the engine's count; likewise the vc_carried_unsorted mutant permutes vc
         by a lexicographic order of those cells, a stand-in for the engine's previous sort."""
+        dts = (self.dt, 2 * self.dt, self.dt / 3) if dts is None else dts
         sc, m = self.scene, self.mutant
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
         rho0 = self.ps.rho0.astype(F)
@@ -999,7 +1154,7 @@ class Checks:
     def grid_growth(self):
         """Two steps pinned at (0, 0): the second step's per-particle contact counts on the positions the first left.
         grown: how far (in cells) those positions reach beyond the first step's bounding box."""
-        o = run(self.make_world, self.scene, steps=[(DT, (0, 0), ZERO_G)] * 2)
+        o = run(self.make_world, self.scene, steps=[(self.dt, (0, 0), ZERO_G)] * 2)
         ps1 = passes_for(self.scene, P=o[0]["P"], kw=self.ps.kw, kg=self.ps.kg)
         same = np.array_equal(o[1]["num_fluid_contacts"], ps1.nf) and np.array_equal(o[1]["num_boundary_contacts"], ps1.nb)
         self.worst["grown_counts"] = 0.0 if same else np.inf
