@@ -12,15 +12,17 @@ and pressures to refresh(); ids, volumes, marks and the slot table stay the mode
 permutations, filters and splices, so a world and its model agree bit for bit after every edit (mismatches()).
 
 Also here, because the CPU and the GPU tests share them: the seeded edit programs (make_program), their interpreter (apply_op)
-and the comparisons (mismatches, step_mismatches, mass_mismatches).
+and the comparisons (mismatches, step_mismatches, mass_mismatches, snapshot_bytes).
 """
 import copy
+import struct
 
 import numpy as np
 
 from . import ref64
 
 F = np.float32
+SOLVER_DFSPH, SOLVER_IISPH = 0, 1  # include/sph.h
 
 
 def default_volume(particle_radius):
@@ -241,6 +243,31 @@ def mismatches(world, model, pressures=False, dead=(), after_step=False):
             if d:
                 out.append(d)
     return out + stale_handles_refused(world, dead)
+
+
+def snapshot_bytes(model, solver, dt, inv_dt):
+    """The blob sph_world_snapshot_save writes (format version 1) for a single-GPU world holding the model's state, which
+    must be a snapshot's: no marks pending.  Little-endian, in order: the header (magic "SPHS", version, solver, fluid slots,
+    dt, inv_dt as float32, the slab planes INT32_MIN / INT32_MAX of an undivided world, the particle count, the blob's
+    length); per slot its count, whether it is alive, its number of forces; the positions, velocities, velocity_changes,
+    volumes, pressures and ids of every slot one after the other; per force a zero elasticity record (no rest pose)."""
+    cols = (("pos", F), ("vel", F), ("vc", F), ("volume", F), ("pressure", F), ("id", np.uint32))
+    body = b"".join(struct.pack("<QII", s.n, int(s.alive), len(s.forces)) for s in model.slots)
+    body += b"".join(np.ascontiguousarray(getattr(s, name), t).tobytes() for name, t in cols for s in model.slots)
+    body += b"".join(struct.pack("<QII", 0, 0, 0) for s in model.slots for _ in s.forces)
+    head = "<IIIIffiiQQ"
+    n = sum(s.n for s in model.slots)
+    return struct.pack(head, 0x53485053, 1, solver, len(model.slots), dt, inv_dt, -2**31, 2**31 - 1, n,
+                       struct.calcsize(head) + len(body)) + body
+
+
+def snapshot_mismatches(blob, want):
+    if blob == want:
+        return []
+    n = min(len(blob), len(want))
+    differ = np.frombuffer(blob[:n], np.uint8) != np.frombuffer(want[:n], np.uint8)
+    k = int(np.argmax(differ)) if differ.any() else n
+    return ["the snapshot has %d bytes, the model's %d; they differ first at byte %d" % (len(blob), len(want), k)]
 
 
 def refresh_from(world, model, pressures=False):
@@ -465,11 +492,12 @@ def apply_op(world, model, op, state, pressures=False):
     two operations and the handles that died.  A step refreshes the model from the world after comparing what the step must
     not have changed: counts and ids.  What a delete applied INSIDE a step did to positions, velocities, vc and pressures is
     therefore compared only where marks are applied and nothing is computed: at a step of dt = 0 (the step's own path:
-    the marks go, the state is uploaded, the solver does not run) and at a snapshot.  Returns the mismatches after the
+    the marks go, the state is uploaded, the solver does not run) and at a snapshot, whose bytes must be snapshot_bytes of
+    the model.  pressures: the world is an IISPH one, whose pressures are carried.  Returns the mismatches after the
     operation."""
     kind = op[0]
     dead = state.setdefault("dead", [])
-    after_step = False
+    after_step, out = False, []
     if kind == "step":
         model.begin_step()
         if world is not None:
@@ -519,7 +547,10 @@ def apply_op(world, model, op, state, pressures=False):
     elif kind == "snapshot":
         state["model_snapshot"] = model.snapshot()
         if world is not None:
-            state["world_snapshot"] = world.snapshot()
+            blob = state["world_snapshot"] = world.snapshot()
+            if isinstance(blob, bytes):  # an engine's blob; a stand-in world built on a model hands back the model's snapshot
+                dt, inv_dt = struct.unpack_from("<ff", blob, 16)  # the lagging timestep is the world's, not the model's
+                out = snapshot_mismatches(blob, snapshot_bytes(model, SOLVER_IISPH if pressures else SOLVER_DFSPH, dt, inv_dt))
     elif kind == "restore":
         model.restore(state["model_snapshot"])
         if world is not None:
@@ -528,7 +559,7 @@ def apply_op(world, model, op, state, pressures=False):
         raise ValueError(kind)
     if world is None:
         return []
-    out = mismatches(world, model, pressures, dead, after_step)
+    out += mismatches(world, model, pressures, dead, after_step)
     if after_step and not out:
         refresh_from(world, model, pressures)
     return out

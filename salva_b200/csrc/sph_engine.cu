@@ -8,6 +8,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include <algorithm>
+#include <array>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -102,6 +103,83 @@ struct BoundaryRec {
     bool want_forces = false;
     bool alive = true;
     uint32_t gen = 0;
+};
+
+// fluid.rs:110-120: the volume of a particle given none
+inline float default_volume(float r) { return r * r * r * (float)(8.0 * 0.8); }
+
+// Rows [at, at + old) of a column with `width` values per row become n rows copied from src, or n rows of `fill`.
+template <class T>
+void splice_rows(std::vector<T>& c, size_t width, size_t at, size_t old, size_t n, const T* src, T fill) {
+    c.erase(c.begin() + width * at, c.begin() + width * (at + old));
+    if (src) c.insert(c.begin() + width * at, src, src + width * n);
+    else c.insert(c.begin() + width * at, width * n, fill);
+}
+
+// Keeps the rows of a column whose mask entry is set, in order.
+template <class T>
+void keep_rows(std::vector<T>& c, size_t width, const std::vector<uint8_t>& mask) {
+    size_t kept = 0;
+    for (size_t i = 0; i < mask.size(); ++i)
+        if (mask[i]) std::copy_n(c.begin() + width * i, width, c.begin() + width * kept++);
+    c.resize(width * kept);
+}
+
+// What the fluid particles carry across steps, on the host in slot order (the fluids' ranges one after the other): the
+// truth while sph_world::staged.  Every column holds one row per particle; host edits change rows through splice and keep.
+struct FluidRows {
+    std::vector<float> pos, vel, vc;  // xyz per row
+    std::vector<float> vol, press;    // volume, IISPH pressure
+    std::vector<uint32_t> gid;        // caller-visible id
+    float vol0 = 0.f;                 // default_volume of the world's particle radius
+
+    // Rows [at, at + old) become n new ones.  A null vel, vc or volume reads as zero, zero and vol0; pressures start at 0.
+    void splice(size_t at, size_t old, size_t n, const float* p, const float* v, const float* c, const float* volume, const uint32_t* ids) {
+        splice_rows(pos, 3, at, old, n, p, 0.f);
+        splice_rows(vel, 3, at, old, n, v, 0.f);
+        splice_rows(vc, 3, at, old, n, c, 0.f);
+        splice_rows(vol, 1, at, old, n, volume, vol0);
+        splice_rows(press, 1, at, old, n, (const float*)nullptr, 0.f);
+        splice_rows(gid, 1, at, old, n, ids, 0u);
+    }
+    void keep(const std::vector<uint8_t>& mask) {
+        keep_rows(pos, 3, mask);
+        keep_rows(vel, 3, mask);
+        keep_rows(vc, 3, mask);
+        keep_rows(vol, 1, mask);
+        keep_rows(press, 1, mask);
+        keep_rows(gid, 1, mask);
+    }
+    // n rows for a download that writes positions, velocities, vc and ids.  Pressures read 0 until it writes them too;
+    // volumes stay with their rows, and rows past the old size (a slab step's immigrants) take vol0.
+    void resize(size_t n) {
+        pos.resize(3 * n);
+        vel.resize(3 * n);
+        vc.resize(3 * n);
+        vol.resize(n, vol0);
+        press.assign(n, 0.f);
+        gid.resize(n);
+    }
+    struct Column { void* p; size_t row_bytes; };
+    // the columns in the order of a snapshot (format version 1)
+    std::array<Column, 6> columns() {
+        return {{{pos.data(), 3 * sizeof(float)}, {vel.data(), 3 * sizeof(float)}, {vc.data(), 3 * sizeof(float)},
+                 {vol.data(), sizeof(float)}, {press.data(), sizeof(float)}, {gid.data(), sizeof(uint32_t)}}};
+    }
+};
+
+// The boundary particles on the host in slot order; every column has as many rows as the boundaries have particles.
+struct BoundaryRows {
+    std::vector<float> pos, vel;  // xyz per row
+    // rows [at, at + old) become n new ones; a null vel reads as zero
+    void splice(size_t at, size_t old, size_t n, const float* p, const float* v) {
+        splice_rows(pos, 3, at, old, n, p, 0.f);
+        splice_rows(vel, 3, at, old, n, v, 0.f);
+    }
+    void resize(size_t n) {
+        pos.resize(3 * n);
+        vel.resize(3 * n);
+    }
 };
 // ColliderCouplingEntry (fluids_pipeline.rs:76-80)
 struct ColliderRec {
@@ -216,7 +294,7 @@ struct sph_world {
 
     // host truth in ORIGINAL order while `staged` (before the first step / after structural edits)
     bool staged = true;
-    std::vector<float> h_pos, h_vel, h_vc, h_vol, h_press;
+    FluidRows rows;
     // boundaries: host copy is always kept (static data); b_dirty => re-upload
     bool b_dirty = true;
     int b_aabb[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};  // boundary cell-coordinate AABB (host side, static)
@@ -225,8 +303,8 @@ struct sph_world {
     bool b_sorted_valid = false, b_reused = false;
     unsigned long long bb_contacts = 0;
     int b_sorted_grid[6] = {0, 0, 0, 0, 0, 0};
-    std::vector<float> hb_pos, hb_vel;
-    bool hb_stale = false;  // colliders posed boundary particles on the device: hb_pos / hb_vel lag behind (pull_boundaries)
+    BoundaryRows brows;
+    bool hb_stale = false;  // colliders posed boundary particles on the device: brows lags behind (pull_boundaries)
     std::vector<ColliderRec> colliders;
     DBuf<int> d_cb;         // boundary cell AABB + bad flag after colliders moved (as k_bounds writes it)
     DBuf<float> d_imp;      // 6 floats per collider slot: the impulses of the step
@@ -250,7 +328,6 @@ struct sph_world {
     DBuf<float4> pos[2], vel[2], vc[2], bpos[2], bvel[2];
     DBuf<uint32_t> orig[2], borig[2];
     DBuf<uint32_t> gid[2];  // caller-visible particle ids (default: original index); follow particles across ranks
-    std::vector<uint32_t> h_gid;
     DBuf<float> press[2];
     DBuf<float4> vs, acc, normals, dbg_acc;
     DBuf<float> dens, alpha, kappa, divv, pred, bvol, bforce;
@@ -480,28 +557,24 @@ sph_status scan_exclusive_k(sph_world* w, ScanSet<K> arrays, size_t n, int level
 sph_status stage_down(sph_world* w) {
     if (w->staged) return SPH_OK;
     size_t N = w->N;
-    w->h_pos.resize(3 * N);
-    w->h_vel.resize(3 * N);
-    w->h_vc.resize(3 * N);
-    w->h_press.assign(N, 0.f);
-    w->h_gid.resize(N);
+    w->rows.resize(N);
     if (N) {
         int c = w->cur;
         uint32_t ob = w->own_begin;
         CU(w->o_a.ensure(3 * N));
         const float4* srcs[3] = {w->pos[c].p, w->vel[c].p, w->vc[c].p};
-        float* dsts[3] = {w->h_pos.data(), w->h_vel.data(), w->h_vc.data()};
+        float* dsts[3] = {w->rows.pos.data(), w->rows.vel.data(), w->rows.vc.data()};
         for (int a = 0; a < 3; ++a) {
             LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + ob, srcs[a] + ob, w->o_a.p);
             CU(cudaMemcpyAsync(dsts[a], w->o_a.p, 3 * N * sizeof(float), cudaMemcpyDeviceToHost, w->st));
             CU(cudaStreamSynchronize(w->st));
         }
         LAUNCH(k_export_u32, N, 256, (uint32_t)N, w->orig[c].p + ob, w->gid[c].p + ob, reinterpret_cast<uint32_t*>(w->o_a.p));
-        CU(cudaMemcpyAsync(w->h_gid.data(), w->o_a.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
+        CU(cudaMemcpyAsync(w->rows.gid.data(), w->o_a.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
         if (w->desc.solver == SPH_SOLVER_IISPH && w->press[c].p) {
             LAUNCH(k_export1, N, 256, (uint32_t)N, w->orig[c].p + ob, w->press[c].p + ob, w->o_a.p);
-            CU(cudaMemcpyAsync(w->h_press.data(), w->o_a.p, N * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+            CU(cudaMemcpyAsync(w->rows.press.data(), w->o_a.p, N * sizeof(float), cudaMemcpyDeviceToHost, w->st));
             CU(cudaStreamSynchronize(w->st));
         }
     }
@@ -571,17 +644,17 @@ sph_status stage_up(sph_world* w) {
     w->Ntot = N;
     w->own_begin = 0;
     TRY(ensure_fluid_buffers(w));
-    w->h_gid.resize(N);
     if (N) {
+        const std::vector<float>& vol = w->rows.vol;
         std::vector<float> mass(N);
         std::vector<uint32_t> fid(N);
         for (size_t f = 0; f < w->fluids.size(); ++f) {
             bool uniform = w->fluids[f].n > 0;
             for (size_t i = 0; i < w->fluids[f].n; ++i) {
                 size_t g = w->fluids[f].offset + i;
-                mass[g] = w->h_vol[g] * w->fluids[f].density0;  // fluid.rs:183-185
+                mass[g] = vol[g] * w->fluids[f].density0;  // fluid.rs:183-185
                 fid[g] = (uint32_t)f;
-                uniform = uniform && w->h_vol[g] == w->h_vol[w->fluids[f].offset];
+                uniform = uniform && vol[g] == vol[w->fluids[f].offset];
             }
             w->fluids[f].uniform_mass = uniform ? mass[w->fluids[f].offset] : 0.f;
         }
@@ -590,22 +663,20 @@ sph_status stage_up(sph_world* w) {
         CU(w->o_c.ensure(3 * N));
         CU(w->o_mass.ensure(N));
         CU(w->o_fid.ensure(N));
-        CU(cudaMemcpyAsync(w->o_a.p, w->h_pos.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_b.p, w->h_vel.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_c.p, w->h_vc.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
+        CU(cudaMemcpyAsync(w->o_a.p, w->rows.pos.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
+        CU(cudaMemcpyAsync(w->o_b.p, w->rows.vel.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
+        CU(cudaMemcpyAsync(w->o_c.p, w->rows.vc.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
         CU(cudaMemcpyAsync(w->o_mass.p, mass.data(), N * sizeof(float), cudaMemcpyHostToDevice, w->st));
         CU(cudaMemcpyAsync(w->o_fid.p, fid.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
         int c = w->cur;
         LAUNCH(k_iota, N, 256, (uint32_t)N, w->orig[c].p);
-        CU(cudaMemcpyAsync(w->gid[c].p, w->h_gid.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
+        CU(cudaMemcpyAsync(w->gid[c].p, w->rows.gid.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
         CU(cudaMemsetAsync(w->pos[c].p, 0, N * sizeof(float4), w->st));
         CU(cudaMemsetAsync(w->vel[c].p, 0, N * sizeof(float4), w->st));
         LAUNCH(k_import, N, 256, (uint32_t)N, w->orig[c].p, w->o_a.p, w->o_b.p, w->o_c.p, w->o_mass.p, w->o_fid.p, w->pos[c].p, w->vel[c].p,
                w->vc[c].p, 0u, (uint32_t)N);
-        if (w->desc.solver == SPH_SOLVER_IISPH) {
-            w->h_press.resize(N, 0.f);
-            CU(cudaMemcpyAsync(w->press[c].p, w->h_press.data(), N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        }
+        if (w->desc.solver == SPH_SOLVER_IISPH)
+            CU(cudaMemcpyAsync(w->press[c].p, w->rows.press.data(), N * sizeof(float), cudaMemcpyHostToDevice, w->st));
         CU(cudaStreamSynchronize(w->st));  // host temporaries go out of scope
     }
     w->staged = false;
@@ -638,7 +709,7 @@ sph_status upload_boundaries(sph_world* w) {
         bool bad = false;
         for (size_t g = 0; g < B; ++g)
             for (int a = 0; a < 3; ++a) {
-                float cf = floorf(w->hb_pos[3 * g + a] / w->h);  // hgrid.rs:41-43, same IEEE division as the device
+                float cf = floorf(w->brows.pos[3 * g + a] / w->h);  // hgrid.rs:41-43, same IEEE division as the device
                 if (!(fabsf(cf) < 1.0e9f)) { bad = true; continue; }
                 aabb[a] = std::min(aabb[a], (int)cf);
                 aabb[3 + a] = std::max(aabb[3 + a], (int)cf);
@@ -648,8 +719,8 @@ sph_status upload_boundaries(sph_world* w) {
         for (size_t b = 0; b < w->bounds.size(); ++b)
             for (size_t i = 0; i < w->bounds[b].n; ++i) {
                 size_t g = w->bounds[b].offset + i;
-                p[g] = make_float4(w->hb_pos[3 * g], w->hb_pos[3 * g + 1], w->hb_pos[3 * g + 2], 0.f);
-                v[g] = make_float4(w->hb_vel[3 * g], w->hb_vel[3 * g + 1], w->hb_vel[3 * g + 2], __uint_as_float_host((uint32_t)b));
+                p[g] = make_float4(w->brows.pos[3 * g], w->brows.pos[3 * g + 1], w->brows.pos[3 * g + 2], 0.f);
+                v[g] = make_float4(w->brows.vel[3 * g], w->brows.vel[3 * g + 1], w->brows.vel[3 * g + 2], __uint_as_float_host((uint32_t)b));
             }
         int c = w->bcur;
         CU(cudaMemcpyAsync(w->bpos[c].p, p.data(), B * sizeof(float4), cudaMemcpyHostToDevice, w->st));
@@ -678,8 +749,8 @@ sph_status pull_boundaries(sph_world* w) {
     CU(w->o_c.ensure(3 * B));
     LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bpos[bc].p, w->o_b.p);
     LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bvel[bc].p, w->o_c.p);
-    CU(cudaMemcpyAsync(w->hb_pos.data(), w->o_b.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaMemcpyAsync(w->hb_vel.data(), w->o_c.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaMemcpyAsync(w->brows.pos.data(), w->o_b.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaMemcpyAsync(w->brows.vel.data(), w->o_c.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
     CU(cudaStreamSynchronize(w->st));
     w->hb_stale = false;
     return SPH_OK;
@@ -691,36 +762,19 @@ sph_status apply_pending_deletes(sph_world* w) {
     for (auto& f : w->fluids) any |= f.n_pending != 0;
     if (!any) return SPH_OK;
     TRY(stage_down(w));
-    std::vector<float> np, nv, nc, nvol, npr;
-    std::vector<uint32_t> ngid;
-    np.reserve(w->h_pos.size());
-    nv.reserve(w->h_pos.size());
-    nc.reserve(w->h_pos.size());
+    std::vector<uint8_t> keep;
+    keep.reserve(w->N);
     for (auto& f : w->fluids) {
         size_t kept = 0;
         for (size_t i = 0; i < f.n; ++i) {
-            if (f.n_pending && f.pending_delete[i]) continue;
-            size_t g = f.offset + i;
-            for (int a = 0; a < 3; ++a) {
-                np.push_back(w->h_pos[3 * g + a]);
-                nv.push_back(w->h_vel[3 * g + a]);
-                nc.push_back(w->h_vc[3 * g + a]);
-            }
-            nvol.push_back(w->h_vol[g]);
-            ngid.push_back(g < w->h_gid.size() ? w->h_gid[g] : (uint32_t)g);
-            npr.push_back(g < w->h_press.size() ? w->h_press[g] : 0.f);
-            ++kept;
+            keep.push_back(!(f.n_pending && f.pending_delete[i]));
+            kept += keep.back();
         }
         f.n = kept;
         f.pending_delete.assign(kept, 0);
         f.n_pending = 0;
     }
-    w->h_pos.swap(np);
-    w->h_vel.swap(nv);
-    w->h_vc.swap(nc);
-    w->h_vol.swap(nvol);
-    w->h_press.swap(npr);
-    w->h_gid.swap(ngid);
+    w->rows.keep(keep);
     recompute_offsets(w);
     return SPH_OK;
 }
@@ -1283,8 +1337,7 @@ sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<
     ctx.velocities_xyz = hv.data();
     ctx.densities = hd.data();
     ctx.accelerations_xyz = ha.data();
-    std::vector<float> vol;
-    if (!w->slab.active && w->h_vol.size() >= fl.offset + fl.n) ctx.volumes = w->h_vol.data() + fl.offset;
+    if (!w->slab.active) ctx.volumes = w->rows.vol.data() + fl.offset;  // a slab step does not size the host rows
     HostContacts ff, fb;
     if (fr.host_flags & SPH_HOST_FORCE_CONTACTS) {
         TRY(materialise_contacts(w, f, 0, &ff));
@@ -1310,8 +1363,8 @@ sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<
         for (size_t b = 0; b < w->bounds.size(); ++b) {
             const BoundaryRec& br = w->bounds[b];
             views[b].n = br.alive ? br.n : 0;
-            views[b].positions_xyz = w->hb_pos.data() + 3 * br.offset;
-            views[b].velocities_xyz = w->hb_vel.data() + 3 * br.offset;
+            views[b].positions_xyz = w->brows.pos.data() + 3 * br.offset;
+            views[b].velocities_xyz = w->brows.vel.data() + 3 * br.offset;
             views[b].volumes = bvol.data() + br.offset;
         }
         ctx.n_boundaries = views.size();
@@ -1707,6 +1760,7 @@ sph_status sph_world_create(const sph_world_desc* desc, sph_world** out) {
     sph_world* w = new sph_world();
     w->desc = *desc;
     w->h = desc->particle_radius * desc->smoothing_factor * 2.0f;  // liquid_world.rs:44
+    w->rows.vol0 = default_volume(desc->particle_radius);
     if (const char* t = getenv("SALVA_B200_XYSUB")) w->xysub = std::min(4, std::max(1, atoi(t)));
     memset(&w->hc, 0, sizeof w->hc);
     memset(&w->stats, 0, sizeof w->stats);
@@ -1778,6 +1832,21 @@ void sph_world_destroy(sph_world* w) {
     delete w;
 }
 
+// The id rule (DESIGN.md §3) for n new particles: sph_fluid_add and sph_fluid_replace_particles without ids number a fluid
+// 0..n-1 (append_to = null).  sph_fluid_append numbers upwards from 1 + the largest id of the fluid's particles, marked ones
+// included: the count would repeat the id of a survivor once a delete has shrunk the fluid, and the in-cell order (fluid, id)
+// needs ids to be unique.  Ids past 2^32 - 1 are refused.
+static sph_status new_ids(sph_world* w, const FluidRec* append_to, size_t n, std::vector<uint32_t>* ids) {
+    uint64_t next = 0;
+    if (append_to)
+        for (size_t i = 0; i < append_to->n; ++i) next = std::max<uint64_t>(next, (uint64_t)w->rows.gid[append_to->offset + i] + 1u);
+    if (next + n > (uint64_t)UINT32_MAX + 1u)
+        return w->fail(SPH_ERR_INVALID, "ids %llu.. of %zu new particles do not fit 32 bits (renumber with sph_fluid_set_ids)", (unsigned long long)next, n);
+    ids->resize(n);
+    for (size_t i = 0; i < n; ++i) (*ids)[i] = (uint32_t)(next + i);
+    return SPH_OK;
+}
+
 sph_status sph_fluid_add(sph_world* w, const float* pos, const float* vel, const float* volumes, size_t n, float density0, uint32_t memberships,
                          uint32_t filter, uint32_t* handle) {
     if (!w) return SPH_ERR_INVALID;
@@ -1789,6 +1858,8 @@ sph_status sph_fluid_add(sph_world* w, const float* pos, const float* vel, const
     if (slot >= (size_t)MAX_FLUIDS) return w->fail(SPH_ERR_INVALID, "too many fluids (max %d)", MAX_FLUIDS);
     TRY(enter(w));
     TRY(stage_down(w));
+    std::vector<uint32_t> ids;
+    TRY(new_ids(w, nullptr, n, &ids));
     FluidRec f;
     if (slot < w->fluids.size()) f.gen = w->fluids[slot].gen + 1;
     f.n = n;
@@ -1796,27 +1867,11 @@ sph_status sph_fluid_add(sph_world* w, const float* pos, const float* vel, const
     f.memberships = memberships;
     f.filter = filter;
     f.pending_delete.assign(n, 0);
-    float r = w->desc.particle_radius;
-    float pv = r * r * r * (float)(8.0 * 0.8);  // fluid.rs:110-120
-    // the host arrays are ordered by slot: a reused slot's (empty) range sits at its offset
+    // the host rows are ordered by slot: a reused slot's (empty) range sits at its offset
     if (slot == w->fluids.size()) w->fluids.push_back(FluidRec());
     w->fluids[slot].n = 0;
     recompute_offsets(w);
-    const size_t at = w->fluids[slot].offset;
-    w->h_press.resize(w->h_vol.size(), 0.f);
-    w->h_gid.resize(w->h_vol.size());
-    w->h_pos.insert(w->h_pos.begin() + 3 * at, pos, pos + 3 * n);
-    if (vel) w->h_vel.insert(w->h_vel.begin() + 3 * at, vel, vel + 3 * n);
-    else w->h_vel.insert(w->h_vel.begin() + 3 * at, 3 * n, 0.f);
-    w->h_vc.insert(w->h_vc.begin() + 3 * at, 3 * n, 0.f);
-    if (volumes) w->h_vol.insert(w->h_vol.begin() + at, volumes, volumes + n);
-    else w->h_vol.insert(w->h_vol.begin() + at, n, pv);
-    w->h_press.insert(w->h_press.begin() + at, n, 0.f);
-    {
-        std::vector<uint32_t> ids(n);
-        for (size_t i = 0; i < n; ++i) ids[i] = (uint32_t)i;
-        w->h_gid.insert(w->h_gid.begin() + at, ids.begin(), ids.end());
-    }
+    w->rows.splice(w->fluids[slot].offset, 0, n, pos, vel, nullptr, volumes, ids.data());
     w->fluids[slot] = f;
     recompute_offsets(w);
     if (handle) *handle = make_handle(slot, f.gen);
@@ -1863,29 +1918,9 @@ sph_status sph_fluid_append(sph_world* w, uint32_t fluid_h, const float* pos, co
     TRY(enter(w));
     TRY(stage_down(w));
     FluidRec& f = w->fluids[fluid];
-    // new ids count up from one past the fluid's largest id, pending deletes included: the count f.n would repeat the
-    // id of a survivor once a delete has shrunk the fluid, and the in-cell order (fluid, id) needs ids to be unique
-    uint64_t next = 0;
-    for (size_t i = 0; i < f.n; ++i) next = std::max<uint64_t>(next, (uint64_t)w->h_gid[f.offset + i] + 1u);
-    if (next + n > (uint64_t)UINT32_MAX + 1u)
-        return w->fail(SPH_ERR_INVALID, "sph_fluid_append: ids %llu.. of %zu new particles do not fit 32 bits (renumber with sph_fluid_set_ids)",
-                       (unsigned long long)next, n);
-    size_t at = f.offset + f.n;
-    float r = w->desc.particle_radius;
-    float pv = r * r * r * (float)(8.0 * 0.8);
-    w->h_pos.insert(w->h_pos.begin() + 3 * at, pos, pos + 3 * n);
-    if (vel) w->h_vel.insert(w->h_vel.begin() + 3 * at, vel, vel + 3 * n);
-    else w->h_vel.insert(w->h_vel.begin() + 3 * at, 3 * n, 0.f);
-    w->h_vc.insert(w->h_vc.begin() + 3 * at, 3 * n, 0.f);
-    w->h_vol.insert(w->h_vol.begin() + at, n, pv);
-    w->h_press.resize(w->h_vol.size() - n, 0.f);
-    w->h_press.insert(w->h_press.begin() + at, n, 0.f);
-    w->h_gid.resize(w->h_vol.size() - n);
-    {
-        std::vector<uint32_t> ids(n);
-        for (size_t i = 0; i < n; ++i) ids[i] = (uint32_t)(next + i);
-        w->h_gid.insert(w->h_gid.begin() + at, ids.begin(), ids.end());
-    }
+    std::vector<uint32_t> ids;
+    TRY(new_ids(w, &f, n, &ids));
+    w->rows.splice(f.offset + f.n, 0, n, pos, vel, nullptr, nullptr, ids.data());
     f.n += n;
     f.pending_delete.resize(f.n, 0);
     recompute_offsets(w);
@@ -1922,8 +1957,8 @@ sph_status sph_fluid_write(sph_world* w, uint32_t fluid_h, const float* pos, con
     if (n != f.n) return w->fail(SPH_ERR_INVALID, "sph_fluid_write: length %zu != particle count %zu", n, f.n);
     if (n == 0 || (!pos && !vel)) return SPH_OK;
     if (w->staged) {
-        if (pos) memcpy(w->h_pos.data() + 3 * f.offset, pos, 3 * n * sizeof(float));
-        if (vel) memcpy(w->h_vel.data() + 3 * f.offset, vel, 3 * n * sizeof(float));
+        if (pos) memcpy(w->rows.pos.data() + 3 * f.offset, pos, 3 * n * sizeof(float));
+        if (vel) memcpy(w->rows.vel.data() + 3 * f.offset, vel, 3 * n * sizeof(float));
         return SPH_OK;
     }
     TRY(enter(w));
@@ -1954,8 +1989,8 @@ sph_status sph_fluid_read(sph_world* w, uint32_t fluid_h, float* pos, float* vel
     if (cap < f.n) return w->fail(SPH_ERR_INVALID, "sph_fluid_read: capacity %zu < particle count %zu", cap, f.n);
     if (f.n == 0 || (!pos && !vel)) return SPH_OK;
     if (w->staged) {
-        if (pos) memcpy(pos, w->h_pos.data() + 3 * f.offset, 3 * f.n * sizeof(float));
-        if (vel) memcpy(vel, w->h_vel.data() + 3 * f.offset, 3 * f.n * sizeof(float));
+        if (pos) memcpy(pos, w->rows.pos.data() + 3 * f.offset, 3 * f.n * sizeof(float));
+        if (vel) memcpy(vel, w->rows.vel.data() + 3 * f.offset, 3 * f.n * sizeof(float));
         return SPH_OK;
     }
     TRY(enter(w));
@@ -1994,10 +2029,7 @@ sph_status sph_boundary_add(sph_world* w, const float* pos, const float* vel, si
     if (slot == w->bounds.size()) w->bounds.push_back(BoundaryRec());
     w->bounds[slot].n = 0;
     recompute_offsets(w);
-    const size_t at = w->bounds[slot].offset;
-    w->hb_pos.insert(w->hb_pos.begin() + 3 * at, pos, pos + 3 * n);
-    if (vel) w->hb_vel.insert(w->hb_vel.begin() + 3 * at, vel, vel + 3 * n);
-    else w->hb_vel.insert(w->hb_vel.begin() + 3 * at, 3 * n, 0.f);
+    w->brows.splice(w->bounds[slot].offset, 0, n, pos, vel);
     w->bounds[slot] = b;
     recompute_offsets(w);
     w->b_dirty = true;
@@ -2013,8 +2045,8 @@ sph_status sph_boundary_write(sph_world* w, uint32_t boundary_h, const float* po
     if (n != b.n) return w->fail(SPH_ERR_INVALID, "sph_boundary_write: length %zu != particle count %zu", n, b.n);
     if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "sph_boundary_write: the boundary is coupled to a collider");
     TRY(pull_boundaries(w));
-    if (pos) memcpy(w->hb_pos.data() + 3 * b.offset, pos, 3 * n * sizeof(float));
-    if (vel) memcpy(w->hb_vel.data() + 3 * b.offset, vel, 3 * n * sizeof(float));
+    if (pos) memcpy(w->brows.pos.data() + 3 * b.offset, pos, 3 * n * sizeof(float));
+    if (vel) memcpy(w->brows.vel.data() + 3 * b.offset, vel, 3 * n * sizeof(float));
     w->b_dirty = true;
     return SPH_OK;
 }
@@ -2159,8 +2191,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
         // the carried state is on the host between an edit and the next step; the step's scratch reads as zero until then
-        if (what == SPH_DBG_VELOCITY_CHANGE) memcpy(out, w->h_vc.data() + 3 * f.offset, 3 * f.n * sizeof(float));
-        else if (what == SPH_DBG_PRESSURE) memcpy(out, w->h_press.data() + f.offset, f.n * sizeof(float));
+        if (what == SPH_DBG_VELOCITY_CHANGE) memcpy(out, w->rows.vc.data() + 3 * f.offset, 3 * f.n * sizeof(float));
+        else if (what == SPH_DBG_PRESSURE) memcpy(out, w->rows.press.data() + f.offset, f.n * sizeof(float));
         else memset(out, 0, width * f.n * sizeof(float));
         return SPH_OK;
     }
@@ -2290,8 +2322,7 @@ sph_status sph_fluid_set_ids(sph_world* w, uint32_t fluid_h, const uint32_t* ids
     if (n != f.n) return w->fail(SPH_ERR_INVALID, "sph_fluid_set_ids: length %zu != particle count %zu", n, f.n);
     TRY(enter(w));
     TRY(stage_down(w));
-    w->h_gid.resize(w->N);
-    memcpy(w->h_gid.data() + f.offset, ids, n * sizeof(uint32_t));
+    memcpy(w->rows.gid.data() + f.offset, ids, n * sizeof(uint32_t));
     return SPH_OK;
 }
 
@@ -2303,7 +2334,7 @@ sph_status sph_fluid_read_ids(sph_world* w, uint32_t fluid_h, uint32_t* ids, siz
     if (cap < f.n) return w->fail(SPH_ERR_INVALID, "sph_fluid_read_ids: capacity %zu < particle count %zu", cap, f.n);
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
-        memcpy(ids, w->h_gid.data() + f.offset, f.n * sizeof(uint32_t));
+        memcpy(ids, w->rows.gid.data() + f.offset, f.n * sizeof(uint32_t));
         return SPH_OK;
     }
     TRY(enter(w));
@@ -2343,15 +2374,7 @@ sph_status sph_fluid_remove(sph_world* w, uint32_t fluid_h) {
     TRY(enter(w));
     TRY(stage_down(w));
     FluidRec& f = w->fluids[fluid];
-    const size_t at = f.offset, n = f.n;
-    w->h_press.resize(w->h_vol.size(), 0.f);
-    w->h_gid.resize(w->h_vol.size());
-    w->h_pos.erase(w->h_pos.begin() + 3 * at, w->h_pos.begin() + 3 * (at + n));
-    w->h_vel.erase(w->h_vel.begin() + 3 * at, w->h_vel.begin() + 3 * (at + n));
-    w->h_vc.erase(w->h_vc.begin() + 3 * at, w->h_vc.begin() + 3 * (at + n));
-    w->h_vol.erase(w->h_vol.begin() + at, w->h_vol.begin() + at + n);
-    w->h_press.erase(w->h_press.begin() + at, w->h_press.begin() + at + n);
-    w->h_gid.erase(w->h_gid.begin() + at, w->h_gid.begin() + at + n);
+    w->rows.splice(f.offset, f.n, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
     for (auto& fr : f.forces) elasticity_release(fr);
     f.forces.clear();
     f.pending_delete.clear();
@@ -2369,8 +2392,7 @@ sph_status sph_boundary_remove(sph_world* w, uint32_t boundary_h) {
     BOUNDARY_OR_FAIL(boundary, boundary_h)
     TRY(pull_boundaries(w));
     BoundaryRec& b = w->bounds[boundary];
-    w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
-    w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
+    w->brows.splice(b.offset, b.n, 0, nullptr, nullptr);
     b.n = 0;
     b.alive = false;
     b.want_forces = false;
@@ -2388,11 +2410,7 @@ sph_status sph_boundary_set_particles(sph_world* w, uint32_t boundary_h, const f
     if (boundary_coupled(w, boundary)) return w->fail(SPH_ERR_INVALID, "sph_boundary_set_particles: the boundary is coupled to a collider");
     TRY(pull_boundaries(w));
     BoundaryRec& b = w->bounds[boundary];
-    w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
-    w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
-    w->hb_pos.insert(w->hb_pos.begin() + 3 * b.offset, pos, pos + 3 * n);
-    if (vel) w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, vel, vel + 3 * n);
-    else w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, 3 * n, 0.f);
+    w->brows.splice(b.offset, b.n, n, pos, vel);
     b.n = n;
     recompute_offsets(w);
     w->b_dirty = true;
@@ -2416,8 +2434,8 @@ sph_status sph_boundary_read(sph_world* w, uint32_t boundary_h, float* pos, floa
     *n = b.n;
     if ((pos || vel) && cap < b.n) return w->fail(SPH_ERR_INVALID, "sph_boundary_read: capacity %zu < particle count %zu", cap, b.n);
     TRY(pull_boundaries(w));
-    if (pos) memcpy(pos, w->hb_pos.data() + 3 * b.offset, 3 * b.n * sizeof(float));
-    if (vel) memcpy(vel, w->hb_vel.data() + 3 * b.offset, 3 * b.n * sizeof(float));
+    if (pos) memcpy(pos, w->brows.pos.data() + 3 * b.offset, 3 * b.n * sizeof(float));
+    if (vel) memcpy(vel, w->brows.vel.data() + 3 * b.offset, 3 * b.n * sizeof(float));
     return SPH_OK;
 }
 
@@ -2466,10 +2484,7 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
     if (sampling == SPH_SAMPLING_STATIC) {
         TRY(pull_boundaries(w));
         BoundaryRec& b = w->bounds[boundary];
-        w->hb_pos.erase(w->hb_pos.begin() + 3 * b.offset, w->hb_pos.begin() + 3 * (b.offset + b.n));
-        w->hb_vel.erase(w->hb_vel.begin() + 3 * b.offset, w->hb_vel.begin() + 3 * (b.offset + b.n));
-        w->hb_pos.insert(w->hb_pos.begin() + 3 * b.offset, pts, pts + 3 * n);
-        w->hb_vel.insert(w->hb_vel.begin() + 3 * b.offset, 3 * n, 0.f);
+        w->brows.splice(b.offset, b.n, n, pts, nullptr);
         b.n = n;
         recompute_offsets(w);
         w->b_dirty = true;
@@ -2593,28 +2608,12 @@ sph_status sph_fluid_replace_particles(sph_world* w, uint32_t fluid_h, const flo
     TRY(enter(w));
     TRY(stage_down(w));
     FluidRec& f = w->fluids[fluid];
-    const size_t at = f.offset, old = f.n;
-    const float r = w->desc.particle_radius, pv = r * r * r * (float)(8.0 * 0.8);
-    w->h_press.resize(w->h_vol.size(), 0.f);
-    w->h_gid.resize(w->h_vol.size());
-    auto splice3 = [&](std::vector<float>& v, const float* src) {
-        v.erase(v.begin() + 3 * at, v.begin() + 3 * (at + old));
-        if (src) v.insert(v.begin() + 3 * at, src, src + 3 * n);
-        else v.insert(v.begin() + 3 * at, 3 * n, 0.f);
-    };
-    splice3(w->h_pos, pos);
-    splice3(w->h_vel, vel);
-    splice3(w->h_vc, vc);
-    w->h_vol.erase(w->h_vol.begin() + at, w->h_vol.begin() + at + old);
-    w->h_vol.insert(w->h_vol.begin() + at, n, pv);
-    w->h_press.erase(w->h_press.begin() + at, w->h_press.begin() + at + old);
-    w->h_press.insert(w->h_press.begin() + at, n, 0.f);
-    w->h_gid.erase(w->h_gid.begin() + at, w->h_gid.begin() + at + old);
-    {
-        std::vector<uint32_t> g(n);
-        for (size_t i = 0; i < n; ++i) g[i] = ids ? ids[i] : (uint32_t)i;
-        w->h_gid.insert(w->h_gid.begin() + at, g.begin(), g.end());
+    std::vector<uint32_t> numbered;
+    if (!ids) {
+        TRY(new_ids(w, nullptr, n, &numbered));
+        ids = numbered.data();
     }
+    w->rows.splice(f.offset, f.n, n, pos, vel, vc, nullptr, ids);
     f.n = n;
     f.pending_delete.assign(n, 0);
     f.n_pending = 0;
@@ -2672,13 +2671,7 @@ sph_status snapshot_write(sph_world* w, Writer& wr) {
         SnapFluid sf{f.n, f.alive ? 1u : 0u, (uint32_t)f.forces.size()};
         wr.put(&sf, sizeof sf);
     }
-    const size_t N = w->N;
-    wr.put(w->h_pos.data(), 3 * N * sizeof(float));
-    wr.put(w->h_vel.data(), 3 * N * sizeof(float));
-    wr.put(w->h_vc.data(), 3 * N * sizeof(float));
-    wr.put(w->h_vol.data(), N * sizeof(float));
-    wr.put(w->h_press.data(), N * sizeof(float));
-    wr.put(w->h_gid.data(), N * sizeof(uint32_t));
+    for (const auto& c : w->rows.columns()) wr.put(c.p, w->N * c.row_bytes);
     for (auto& f : w->fluids)
         for (auto& fr : f.forces) {
             SnapElastic se{0, 0, 0};
@@ -2770,12 +2763,8 @@ sph_status sph_world_snapshot_load(sph_world* w, const void* buffer, size_t leng
         memcpy(dst, p + off, bytes);
         off += bytes;
     };
-    w->h_pos.resize(3 * N); take(w->h_pos.data(), 3 * N * sizeof(float));
-    w->h_vel.resize(3 * N); take(w->h_vel.data(), 3 * N * sizeof(float));
-    w->h_vc.resize(3 * N);  take(w->h_vc.data(), 3 * N * sizeof(float));
-    w->h_vol.resize(N);     take(w->h_vol.data(), N * sizeof(float));
-    w->h_press.resize(N);   take(w->h_press.data(), N * sizeof(float));
-    w->h_gid.resize(N);     take(w->h_gid.data(), N * sizeof(uint32_t));
+    w->rows.resize(N);
+    for (const auto& c : w->rows.columns()) take(c.p, N * c.row_bytes);
     for (size_t k = 0; k < sf.size(); ++k) {
         w->fluids[k].n = (size_t)sf[k].n;
         w->fluids[k].pending_delete.assign((size_t)sf[k].n, 0);

@@ -2,6 +2,8 @@
 against mutants.  Each mutant is one plausible splice bug of an engine; the programs and the comparison functions are the
 ones tests/test_gpu_edits.py runs, with the unmutated model (and a stand-in step) in the engine's place, so a mutant that is
 not flagged here would not be flagged on the GPU either."""
+import struct
+
 import numpy as np
 import pytest
 
@@ -280,6 +282,30 @@ def test_ids_from_the_count_repeat_a_survivors_id(all_programs):
             em.apply_op(None, model, op, state)
         repeated |= any(len(np.unique(model.slot(h).id)) < model.slot(h).n for h in model.handles())
     assert repeated
+
+
+def test_snapshot_bytes_lay_out_the_model_in_slot_order():
+    """em.snapshot_bytes, which the GPU programs compare every world's snapshot with: the 48-byte header, a 16-byte record
+    per slot (a removed one included), the six columns each over all slots, a 16-byte zero record per force."""
+    scene = ge.make_scene("dfsph3")
+    model = em.EditModel(ge.R)
+    ge.populate(None, model, scene)
+    h0, h1, h2 = model.handles()
+    model.delete(h2, np.arange(model.slot(h2).n) % 3 == 0)
+    model.remove_fluid(h1)
+    model.snapshot()
+    blob = em.snapshot_bytes(model, em.SOLVER_DFSPH, 0.004, 250.0)
+    n = [s.n for s in model.slots]
+    assert n[1] == 0 and 0 < n[2] < len(scene["fluids"][2]["positions"])   # the marks went with the snapshot
+    head = struct.unpack_from("<IIIIffiiQQ", blob)
+    assert head == (0x53485053, 1, em.SOLVER_DFSPH, 3, F(0.004), 250.0, -2**31, 2**31 - 1, sum(n), len(blob))
+    assert [struct.unpack_from("<QII", blob, 48 + 16 * k) for k in range(3)] == [(n[0], 1, 1), (0, 0, 0), (n[2], 1, 1)]
+    at, N = 48 + 16 * 3, sum(n)
+    for name, width, t in (("pos", 3, F), ("vel", 3, F), ("vc", 3, F), ("volume", 1, F), ("pressure", 1, F), ("id", 1, np.uint32)):
+        col = np.frombuffer(blob, t, width * N, at)
+        assert np.array_equal(col, np.concatenate([getattr(s, name).reshape(-1) for s in model.slots])), name
+        at += 4 * width * N
+    assert blob[at:] == bytes(16 * 2)   # the forces of slots 0 and 2; the removed slot has none
 
 
 # ---- the model against the CPU oracle --------------------------------------------------------------------------------------
