@@ -178,7 +178,9 @@ sph_status sph_fluid_push_force(sph_world* w, uint32_t fluid, const sph_force_de
  * arbitrary HOST code that adds to fluid.accelerations.  At the force's slot in push order the library hands the
  * callback the fluid's particles in ORIGINAL index order (host copies) and takes the accelerations back.  `dt` / `inv_dt`
  * are the TimestepManager values the reference passes at that point (the previous step's: dfsph_solver.rs:693-702).
- * Contact lists are not materialised for callbacks (pass-through of ParticlesContacts is a later row). */
+ * Like the reference's predict_advection (dfsph_solver.rs:580-603, iisph_solver.rs alike), every step that runs the solver
+ * (the world holds at least one fluid particle) calls each force once, that of an empty fluid too, with n == 0 (its
+ * pointers may then be NULL).  Contact lists are not materialised for these callbacks: see sph_fluid_push_host_force2. */
 typedef void (*sph_host_force_fn)(void* user, float dt, float inv_dt, float kernel_radius, size_t n, const float* positions_xyz,
                                   const float* velocities_xyz, const float* densities, float* accelerations_xyz);
 sph_status sph_fluid_push_host_force(sph_world* w, uint32_t fluid, sph_host_force_fn fn, void* user);
@@ -189,7 +191,8 @@ sph_status sph_fluid_push_host_force(sph_world* w, uint32_t fluid, sph_host_forc
  * over the fluid's particles in ORIGINAL index order: the contacts of particle i are entries ff_offsets[i] ..
  * ff_offsets[i+1]; `j` is the neighbour's index INSIDE its own fluid / boundary, `j_model` that object's slot
  * (handle & 0xFFFF; == ctx.fluid_index for same-fluid contacts); the self contact (j == i, gradient 0) is included, as
- * in the reference.  All pointers are host memory owned by the library for the duration of the call. */
+ * in the reference.  An empty fluid's force is called too, with n == 0 and ff_offsets == fb_offsets == {0}.  All
+ * pointers are host memory owned by the library for the duration of the call. */
 enum { SPH_HOST_FORCE_CONTACTS = 1u,    /* fill ff_* / fb_* */
        SPH_HOST_FORCE_BOUNDARIES = 2u   /* fill boundaries[] (positions, velocities, volumes) */ };
 typedef struct {

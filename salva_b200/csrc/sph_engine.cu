@@ -1431,8 +1431,8 @@ sph_status phase_forces(sph_world* w) {
                     if (p[0] != 0.f) DISPATCH1(k_wcsph_force, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->acc.p, (uint32_t)f, p[0]);
                     break;
                 case FORCE_HOST_CALLBACK: {  // user-defined NonPressureForce::solve on the host (nonpressure_force.rs:10-30)
+                    // called for an empty fluid too (n = 0, offsets {0}), as predict_advection calls solve for every fluid
                     FluidRec& fl = w->fluids[f];
-                    if (fl.n == 0) break;
                     const uint32_t ob = w->own_begin;
                     const size_t Nf = fl.n;
                     CU(w->o_a.ensure(3 * N));

@@ -274,6 +274,14 @@ def _fp(a):
     return None if a is None else a.ctypes.data_as(C.POINTER(C.c_float))
 
 
+def _view(ptr, shape, dtype=np.float32):
+    """numpy view of a callback's pointer argument; an empty one (an empty fluid's, possibly NULL) as an empty array."""
+    n = int(np.prod(shape))
+    if n == 0 or not ptr:
+        return np.zeros(shape, dtype)
+    return np.ctypeslib.as_array(ptr, (n,)).view(dtype).reshape(shape)
+
+
 def nccl_unique_id():
     """128-byte NCCL unique id (rank 0 creates it, the host's plumbing broadcasts it)."""
     buf = C.create_string_buffer(128)
@@ -368,8 +376,7 @@ class LiquidWorld:
         velocities, densities, accelerations) is called on the host with numpy views in ORIGINAL index order and adds
         to `accelerations` in place (examples3d/custom_forces3.rs:66-90)."""
         def tramp(_user, dt, inv_dt, h, n, pos, vel, dens, acc):
-            solve(dt, inv_dt, h, np.ctypeslib.as_array(pos, (n, 3)), np.ctypeslib.as_array(vel, (n, 3)),
-                  np.ctypeslib.as_array(dens, (n,)), np.ctypeslib.as_array(acc, (n, 3)))
+            solve(dt, inv_dt, h, _view(pos, (n, 3)), _view(vel, (n, 3)), _view(dens, (n,)), _view(acc, (n, 3)))
         cb = _lib.HOST_FORCE_FN(tramp)
         self._callbacks.append(cb)  # keep the trampoline alive as long as the world
         self._ck(self._L.sph_fluid_push_host_force(self._w, fluid, cb, None))
@@ -381,34 +388,28 @@ class LiquidWorld:
         (ContactsView) and boundaries (list of dicts with positions / velocities / volumes)."""
         import types
 
-        def arr(ptr, shape, dtype=np.float32):
-            n = int(np.prod(shape))
-            if n == 0 or not ptr:
-                return np.zeros(shape, dtype)
-            return np.ctypeslib.as_array(ptr, (n,)).view(dtype).reshape(shape)
-
         def tramp(_user, cp):
             c = cp.contents
             n = c.n
             ctx = types.SimpleNamespace(dt=c.dt, inv_dt=c.inv_dt, kernel_radius=c.kernel_radius, particle_radius=c.particle_radius,
                                         fluid=c.fluid, fluid_index=c.fluid_index, density0=c.density0,
-                                        positions=arr(c.positions_xyz, (n, 3)), velocities=arr(c.velocities_xyz, (n, 3)),
-                                        densities=arr(c.densities, (n,)), volumes=arr(c.volumes, (n,)) if c.volumes else None,
-                                        accelerations=arr(c.accelerations_xyz, (n, 3)),
+                                        positions=_view(c.positions_xyz, (n, 3)), velocities=_view(c.velocities_xyz, (n, 3)),
+                                        densities=_view(c.densities, (n,)), volumes=_view(c.volumes, (n,)) if c.volumes else None,
+                                        accelerations=_view(c.accelerations_xyz, (n, 3)),
                                         fluid_fluid_contacts=None, fluid_boundaries_contacts=None, boundaries=None)
             if c.ff_offsets:
-                off = arr(c.ff_offsets, (n + 1,), np.uint32)
+                off = _view(c.ff_offsets, (n + 1,), np.uint32)
                 m = int(off[-1]) if n else 0
-                ctx.fluid_fluid_contacts = ContactsView(off, arr(c.ff_j, (m,), np.uint32), arr(c.ff_j_model, (m,), np.uint32),
-                                                        arr(c.ff_weight, (m,)), arr(c.ff_gradient_xyz, (m, 3)))
-                off = arr(c.fb_offsets, (n + 1,), np.uint32)
+                ctx.fluid_fluid_contacts = ContactsView(off, _view(c.ff_j, (m,), np.uint32), _view(c.ff_j_model, (m,), np.uint32),
+                                                        _view(c.ff_weight, (m,)), _view(c.ff_gradient_xyz, (m, 3)))
+                off = _view(c.fb_offsets, (n + 1,), np.uint32)
                 m = int(off[-1]) if n else 0
-                ctx.fluid_boundaries_contacts = ContactsView(off, arr(c.fb_j, (m,), np.uint32), arr(c.fb_j_model, (m,), np.uint32),
-                                                             arr(c.fb_weight, (m,)), arr(c.fb_gradient_xyz, (m, 3)))
+                ctx.fluid_boundaries_contacts = ContactsView(off, _view(c.fb_j, (m,), np.uint32), _view(c.fb_j_model, (m,), np.uint32),
+                                                             _view(c.fb_weight, (m,)), _view(c.fb_gradient_xyz, (m, 3)))
             if c.boundaries:
-                ctx.boundaries = [dict(positions=arr(c.boundaries[b].positions_xyz, (c.boundaries[b].n, 3)),
-                                       velocities=arr(c.boundaries[b].velocities_xyz, (c.boundaries[b].n, 3)),
-                                       volumes=arr(c.boundaries[b].volumes, (c.boundaries[b].n,))) for b in range(c.n_boundaries)]
+                ctx.boundaries = [dict(positions=_view(c.boundaries[b].positions_xyz, (c.boundaries[b].n, 3)),
+                                       velocities=_view(c.boundaries[b].velocities_xyz, (c.boundaries[b].n, 3)),
+                                       volumes=_view(c.boundaries[b].volumes, (c.boundaries[b].n,))) for b in range(c.n_boundaries)]
             solve(ctx)
 
         cb = _lib.HOST_FORCE_FN2(tramp)
