@@ -369,6 +369,19 @@ public:
     const std::vector<Boundary>& boundaries() const { return boundaries_; }
     Real h() const { return sph_world_h(raw_); }
     Real particle_radius() const { return sph_world_particle_radius(raw_); }
+    // CFL-bounded substeps inside each step (sph_world_set_substepping); the defaults are the reference TimestepManager's
+    // (timestep_manager.rs:21-31), which has no setter: an extension.  cfl_coeff = 0 turns substepping off.
+    void set_substepping(Real cfl_coeff = 0.4f, uint32_t min_substeps = 1, uint32_t max_substeps = 10) {
+        check(sph_world_set_substepping(raw_, cfl_coeff, min_substeps, max_substeps));
+    }
+    // The lengths of the last step's substeps, in order (empty when the step ran no solver).
+    std::vector<Real> substeps() {
+        size_t n = 0;
+        check(sph_world_read_substeps(raw_, nullptr, 0, &n));
+        std::vector<Real> out(n);
+        if (n) check(sph_world_read_substeps(raw_, out.data(), out.size(), &n));
+        return out;
+    }
 
     // Advances the simulation by dt seconds (liquid_world.rs:62-64).
     void step(Real dt, const Vector3& gravity) { step_with_coupling(dt, gravity, nullptr); }

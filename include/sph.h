@@ -135,7 +135,9 @@ typedef struct {
     uint32_t n_ghost_particles;      /* multi-GPU: ghost particles received from the neighbour slabs this step */
     uint32_t n_migrated;             /* multi-GPU: particles handed over to / received from neighbour slabs */
     uint32_t n_exchanges;            /* multi-GPU: ghost-refresh exchanges (ncclSend/Recv groups) this step */
-    uint32_t reserved_;
+    uint32_t n_substeps;             /* counters.nsubsteps (liquid_world.rs:86): substeps the step ran, 0 when no solver ran.
+                                        Over a substepped step the times, iteration / evaluation counts and kernel_launches are
+                                        sums, max_neighbors the maximum, everything else the last substep's */
 } sph_step_stats;
 
 /* sph_debug_read() selectors: solver scratch in ORIGINAL particle order. */
@@ -417,6 +419,20 @@ sph_status sph_world_snapshot_load(sph_world* w, const void* buffer, size_t leng
 /* Parity/bench aid: run exactly this many velocity-change updates in the next steps'
  * divergence / pressure loops instead of the error-driven break (negative = free running). */
 sph_status sph_world_force_iterations(sph_world* w, int32_t n_divergence, int32_t n_pressure);
+/* CFL-bounded substeps: the TimestepManager's cfl_coeff / min_num_substeps / max_num_substeps (timestep_manager.rs:21-46),
+ * whose rule the reference leaves commented out (compute_substep :87-94 returns the whole step).  cfl_coeff == 0 (the
+ * default) turns substepping off: every step is one substep, as in the reference.  Otherwise a step of length T runs
+ * substeps k = 0, 1, ... while the remaining time R_k > FLT_EPSILON (R_0 = T).  Each computes, after the non-pressure forces,
+ * m = max over the fluid particles of |v + a * R_k|^2 and d = (2 r) / sqrt(m) * cfl_coeff (+inf when m == 0), and runs
+ * n_k = clamp(ceil(R_k / d), max(1, min_substeps - k), max(1, max_substeps - k)) even parts of R_k: dt_k = R_k / n_k,
+ * R_{k+1} = R_k - dt_k.  So dt_k <= d unless max_substeps binds, the substeps add up to T (f32 rounding aside), and their
+ * count lies in [min_substeps, max_substeps].  SPH_ERR_INVALID, nothing changed, for a NaN or negative cfl_coeff (+inf is
+ * allowed), min_substeps == 0, min_substeps > max_substeps, and in a slab-decomposed world (slab_count > 1).  Snapshots
+ * do not carry these settings.  See DESIGN.md section 12. */
+sph_status sph_world_set_substepping(sph_world* w, float cfl_coeff, uint32_t min_substeps, uint32_t max_substeps);
+/* The lengths dt_k of the last step's substeps in order (counters.nsubsteps of them, liquid_world.rs:86): min(cap, *n)
+ * are written, and *n (which may exceed cap) is the count; 0 when the step ran no solver. */
+sph_status sph_world_read_substeps(sph_world* w, float* dts, size_t cap, size_t* n);
 sph_status sph_world_stats(sph_world* w, sph_step_stats* out);
 /* LiquidWorld::h / particle_radius  liquid_world.rs:201-208 */
 float      sph_world_h(const sph_world* w);

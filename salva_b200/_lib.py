@@ -39,7 +39,7 @@ class StepStats(C.Structure):
                 ("n_fluid_particles", C.c_uint64), ("n_boundary_particles", C.c_uint64), ("n_contacts", C.c_uint64),
                 ("max_neighbors", C.c_uint32), ("grid_dims", C.c_uint32 * 3), ("kernel_launches", C.c_uint64),
                 ("n_ghost_particles", C.c_uint32), ("n_migrated", C.c_uint32), ("n_exchanges", C.c_uint32),
-                ("reserved_", C.c_uint32)]
+                ("n_substeps", C.c_uint32)]
 
 
 _fp, _u8p, _vp = C.POINTER(C.c_float), C.POINTER(C.c_uint8), C.c_void_p
@@ -109,6 +109,8 @@ SYMBOLS = {
     "sph_boundary_read_volumes": (C.c_int, [_vp, C.c_uint32, _fp, C.c_size_t]),
     "sph_world_step": (C.c_int, [_vp, C.c_float, _fp]),
     "sph_world_force_iterations": (C.c_int, [_vp, C.c_int32, C.c_int32]),
+    "sph_world_set_substepping": (C.c_int, [_vp, C.c_float, C.c_uint32, C.c_uint32]),
+    "sph_world_read_substeps": (C.c_int, [_vp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
     "sph_world_stats": (C.c_int, [_vp, C.POINTER(StepStats)]),
     "sph_world_h": (C.c_float, [_vp]),
     "sph_world_particle_radius": (C.c_float, [_vp]),

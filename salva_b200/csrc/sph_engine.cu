@@ -291,6 +291,10 @@ struct sph_world {
     // timestep_manager.rs:21-31: dt/inv_dt are 0 until the first advance()
     float dt = 0.f, inv_dt = 0.f;
     int force_div = -1, force_press = -1;
+    // CFL-bounded substeps (sph_world_set_substepping, DESIGN.md section 12): off while cfl_coeff == 0
+    float cfl_coeff = 0.f;
+    uint32_t min_substeps = 1, max_substeps = 10;
+    std::vector<float> substeps;  // dt_k of the last step's substeps, in order (its size is the running substep's k)
 
     // host truth in ORIGINAL order while `staged` (before the first step / after structural edits)
     bool staged = true;
@@ -361,7 +365,7 @@ struct sph_world {
     cudaTextureObject_t tex_vs = 0;  // the general evaluations gather v* through the texture pipe
     const void* tex_vs_ptr = nullptr;
     DBuf<float> partial, errsum;
-    DBuf<int> d_scal;  // [0..6] bounds + bad flag, [7] error flag, [8..9] maxcnt
+    DBuf<int> d_scal;  // [0..6] bounds + bad flag, [7] error flag, [8..9] maxcnt, [11] elasticity widest, [12] CFL max |v + a R|^2
     DBuf<unsigned long long> d_cnt;  // [0] bb contacts, [1] ff+fb contacts
     DBuf<float> o_a, o_b, o_c, o_mass;  // staging, original order
     DBuf<uint32_t> o_fid;
@@ -1466,14 +1470,44 @@ sph_status phase_forces(sph_world* w) {
     return SPH_OK;
 }
 
-// timestep_manager.rs:76-88
-void timestep_advance(sph_world* w, float total) {
-    w->dt = total;
-    w->inv_dt = total == 0.f ? 0.f : 1.0f / total;
+// The CFL rule's substep count (DESIGN.md section 12): d = (r * 2) / sqrt(m) * cfl in the order of max_substep
+// (timestep_manager.rs:36-46), +inf for m == 0, and n = clamp(ceil(R / d), max(1, min - k), max(1, max - k)); a non-finite
+// or NaN ratio takes the upper bound
+uint32_t cfl_substeps(float m, float remaining, float r, float cfl, uint32_t min_substeps, uint32_t max_substeps, uint32_t k) {
+    const float d = m == 0.f ? INFINITY : r * 2.0f / sqrtf(m) * cfl;
+    const int64_t lo = std::max<int64_t>(1, (int64_t)min_substeps - k), hi = std::max<int64_t>(1, (int64_t)max_substeps - k);
+    const float q = ceilf(remaining / d);
+    if (!(q <= (float)hi)) return (uint32_t)hi;
+    return (uint32_t)std::max<int64_t>(lo, (int64_t)q);
 }
 
-// DFSPHSolver::step dfsph_solver.rs:667-708
-sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
+// Substepping only: the CFL reduction over the velocities `vel` and this substep's accelerations, enqueued after the forces
+sph_status launch_cfl_max(sph_world* w, const float4* vel, float remaining) {
+    if (w->cfl_coeff == 0.f) return SPH_OK;
+    CU(cudaMemsetAsync(w->d_scal.p + 12, 0, sizeof(int), w->st));
+    LAUNCH(k_cfl_max, w->N, 256, vel, w->acc.p, remaining, reinterpret_cast<unsigned int*>(w->d_scal.p + 12));
+    return SPH_OK;
+}
+
+// TimestepManager::advance timestep_manager.rs:76-88: the substep is the whole remaining time R_k, or with substepping on
+// R_k / n_k of the CFL rule, which reads back launch_cfl_max's result (the substep's one host synchronisation for it)
+sph_status timestep_advance(sph_world* w, float remaining) {
+    float dt = remaining;
+    if (w->cfl_coeff != 0.f) {
+        CU(cudaMemcpyAsync(w->h_pinned + 48, w->d_scal.p + 12, sizeof(float), cudaMemcpyDeviceToHost, w->st));
+        CU(cudaStreamSynchronize(w->st));
+        const uint32_t n = cfl_substeps(w->h_pinned[48], remaining, w->desc.particle_radius, w->cfl_coeff, w->min_substeps,
+                                        w->max_substeps, (uint32_t)w->substeps.size());
+        dt = remaining / (float)n;
+    }
+    w->dt = dt;
+    w->inv_dt = dt == 0.f ? 0.f : 1.0f / dt;
+    w->substeps.push_back(dt);
+    return SPH_OK;
+}
+
+// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k
+sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
@@ -1522,23 +1556,25 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
     const bool folded = w->xs_valid || w->akinci_valid;
     const float4* xs = folded ? w->xs.p : nullptr;
     const float xs_scale = w->akinci_valid ? 1.0f : w->inv_dt;
-    // nothing (else) to launch in the force phase?  Then fold, acceleration and integration are one streaming pass
+    // nothing (else) to launch in the force phase?  Then fold, acceleration and integration are one streaming pass, unless
+    // substepping needs the CFL reduction between the fold and the integration, which takes the new dt
     bool quiet_forces = true;
     for (size_t f = 0; f < w->fluids.size() && quiet_forces; ++f)
         for (const ForceRec& fr : w->fluids[f].forces)
             if (!(folded && f == 0 && &fr == &w->fluids[0].forces[0])) quiet_forces = false;
-    if (quiet_forces) {
+    if (quiet_forces && w->cfl_coeff == 0.f) {
         CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
         CU(cudaEventRecord(w->ev[EV_FORCES], w->st));
-        timestep_advance(w, dt_total);  // :702
+        TRY(timestep_advance(w, remaining));  // :702
         LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale, w->dt,
                w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
     } else {
         LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale);  // ghosts too (vel = v*)
         CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
-        TRY(phase_forces(w));
+        if (!quiet_forces) TRY(phase_forces(w));
         CU(cudaEventRecord(w->ev[EV_FORCES], w->st));
-        timestep_advance(w, dt_total);  // :702
+        TRY(launch_cfl_max(w, w->vel[c].p, remaining));
+        TRY(timestep_advance(w, remaining));  // :702
         LAUNCH(k_integrate_acc, N, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, w->dt, w->unimass ? w->pvx4.p : nullptr,
                w->unimass ? w->vyz2.p : nullptr);
     }
@@ -1581,40 +1617,33 @@ sph_status dfsph_step(sph_world* w, float dt_total, const float g[3]) {
     return SPH_OK;
 }
 
-sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupling_manager* coupling = nullptr) {
-    TRY(enter(w));
-    w->launches = 0;
-    w->stats_exchanges = 0;
-    w->n_spans = 0;
-    w->nb_pending = false;
-    memset(&w->stats, 0, sizeof w->stats);
-    const bool colliders = any_collider(w);  // refused before anything of the step is applied
-    if (colliders && coupling) return w->fail(SPH_ERR_INVALID, "registered colliders and a host coupling manager cannot run in one step");
-    if (colliders && w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
-    TRY(apply_pending_deletes(w));  // liquid_world.rs:79-81
-    TRY(stage_up(w));
-    for (ColliderRec& c : w->colliders) {
-        memset(c.impulse, 0, sizeof c.impulse);
-        c.impulse_pending = false;
-    }
-    const bool b_uploaded = w->b_dirty;
-    TRY(upload_boundaries(w));
-    size_t N = w->N;
-    w->stats.n_fluid_particles = N;
-    w->stats.n_boundary_particles = w->B;
-    if (w->fluids.size() > (size_t)MAX_FLUIDS || w->bounds.size() > (size_t)MAX_BOUNDARIES)
-        return w->fail(SPH_ERR_INVALID, "too many fluids (max %d) or boundaries (max %d)", MAX_FLUIDS, MAX_BOUNDARIES);
-    if (!(dt > F32_EPS)) return SPH_OK;  // timestep_manager.rs:56-58: is_done() before the first substep
-    CU(cudaEventRecord(w->ev[EV_START], w->st));
-    if (w->slab.active) {
-        TRY(slab_begin_step(w));
-        N = w->N;
-        w->stats.n_fluid_particles = N;
-    } else {
-        w->Ntot = N;
-        w->own_begin = 0;
-    }
-    if (w->Ntot + w->B == 0) return SPH_OK;
+// Counters resume and pause across substeps (liquid_world.rs:84-148): `t` holds the substeps so far, `s` the one that just ran.
+// Times and iteration / evaluation counts add up, max_neighbors is the widest of all, everything else is the last substep's.
+void stats_merge(sph_step_stats& t, const sph_step_stats& s) {
+    sph_step_stats m = s;
+    m.step_ms = t.step_ms + s.step_ms;
+    m.grid_ms = t.grid_ms + s.grid_ms;
+    m.neighbors_ms = t.neighbors_ms + s.neighbors_ms;
+    m.density_ms = t.density_ms + s.density_ms;
+    m.divergence_ms = t.divergence_ms + s.divergence_ms;
+    m.nonpressure_ms = t.nonpressure_ms + s.nonpressure_ms;
+    m.pressure_ms = t.pressure_ms + s.pressure_ms;
+    m.integrate_ms = t.integrate_ms + s.integrate_ms;
+    m.n_divergence_iter = t.n_divergence_iter + s.n_divergence_iter;
+    m.n_pressure_iter = t.n_pressure_iter + s.n_pressure_iter;
+    m.n_divergence_eval = t.n_divergence_eval + s.n_divergence_eval;
+    m.n_pressure_eval = t.n_pressure_eval + s.n_pressure_eval;
+    m.max_neighbors = std::max(t.max_neighbors, s.max_neighbors);
+    t = m;
+}
+
+// One substep of LiquidWorld::step (liquid_world.rs:84-148): colliders, grid, coupling, neighbours, the solver with the
+// remaining time R_k, the substep's read-back and transmit_forces.  The solver pushes dt_k to w->substeps; a substep
+// without fluid particles runs no solver and pushes nothing.
+sph_status world_substep(sph_world* w, float remaining, const float g[3], const sph_coupling_manager* coupling, bool colliders,
+                         bool b_uploaded) {
+    const size_t N = w->N, k = w->substeps.size();
+    for (ColliderRec& c : w->colliders) c.impulse_pending = false;
     if (colliders) TRY(colliders_update(w, b_uploaded));
     TRY(phase_grid(w));
     w->grid_ready = true;
@@ -1650,8 +1679,8 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     }));
     CU(cudaEventRecord(w->ev[EV_DENS], w->st));
     if (N) {
-        if (w->desc.solver == SPH_SOLVER_DFSPH) TRY(dfsph_step(w, dt, g));
-        else TRY(iisph_step(w, dt, g));
+        if (w->desc.solver == SPH_SOLVER_DFSPH) TRY(dfsph_step(w, remaining, g));
+        else TRY(iisph_step(w, remaining, g));
     }
     if (colliders && N) TRY(colliders_impulse(w));  // without fluid particles no force reaches a boundary (and dt did not advance)
     CU(cudaEventRecord(w->ev[EV_END], w->st));
@@ -1664,14 +1693,15 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     w->nb_valid = w->nb_pending;
     w->nb_pending = false;
     CU(cudaGetLastError());
-    for (size_t k = 0; k < w->colliders.size(); ++k)
-        if (w->colliders[k].impulse_pending) memcpy(w->colliders[k].impulse, w->h_imp + 6 * k, sizeof w->colliders[k].impulse);
+    for (size_t i = 0; i < w->colliders.size(); ++i) {  // the step's impulse: the f32 sum of its substeps', in substep order
+        ColliderRec& c = w->colliders[i];
+        if (!c.impulse_pending) continue;
+        if (k == 0) memcpy(c.impulse, w->h_imp + 6 * i, sizeof c.impulse);
+        else
+            for (int j = 0; j < 6; ++j) c.impulse[j] += w->h_imp[6 * i + j];
+    }
     if (!w->b_reused) w->bb_contacts = cnts[0];
     w->stats.n_contacts = w->bb_contacts + cnts[1];
-    w->stats.kernel_launches = w->launches;
-    w->stats.n_ghost_particles = (uint32_t)(w->Ntot - w->N);
-    w->stats.n_migrated = w->slab.migrated_in + w->slab.migrated_out;
-    w->stats.n_exchanges = (uint32_t)w->stats_exchanges;
     auto el = [&](int a, int b) {
         float ms = 0.f;
         cudaEventElapsedTime(&ms, w->ev[a], w->ev[b]);
@@ -1691,22 +1721,78 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
         w->stats.pressure_ms = el(EV_INTEG, EV_PRESS);
         w->stats.integrate_ms = el(EV_FORCES, EV_INTEG) + el(EV_PRESS, EV_END);
     }
-    {
-        float acc[SP_COUNT] = {0.f, 0.f, 0.f, 0.f};
-        for (size_t k = 0; k < w->n_spans; ++k) {
-            float ms = 0.f;
-            cudaEventElapsedTime(&ms, w->spans[k].a, w->spans[k].b);
-            acc[w->spans[k].slot] += ms;
-        }
-        w->stats.divergence_eval_ms = acc[SP_DIV_EVAL];
-        w->stats.divergence_update_ms = acc[SP_DIV_UPD];
-        w->stats.predict_density_ms = acc[SP_PRED];
-        w->stats.pressure_update_ms = acc[SP_PUPD];
-    }
     if (flag & 2) return w->fail(SPH_ERR_NCCL, "peer-memory ghost exchange timed out (a neighbour rank never delivered its boundary column)");
     if (flag) return w->fail(SPH_ERR_ZERO_DENSITY, "zero density (reference asserts dfsph_solver.rs:92,145,662)");
     if (coupling && coupling->transmit_forces) coupling->transmit_forces(coupling->user, w, w->dt, w->inv_dt);  // liquid_world.rs:146
     return SPH_OK;
+}
+
+// LiquidWorld::step liquid_world.rs:62-158: the refusals, the pending deletes (:79-81) and the staging run once, then substeps
+// until the remaining time is used up (:84, is_done timestep_manager.rs:56-58)
+sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupling_manager* coupling = nullptr) {
+    TRY(enter(w));
+    w->launches = 0;
+    w->stats_exchanges = 0;
+    w->n_spans = 0;
+    w->nb_pending = false;
+    memset(&w->stats, 0, sizeof w->stats);
+    w->substeps.clear();
+    const bool colliders = any_collider(w);  // refused before anything of the step is applied
+    if (colliders && coupling) return w->fail(SPH_ERR_INVALID, "registered colliders and a host coupling manager cannot run in one step");
+    if (colliders && w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
+    TRY(apply_pending_deletes(w));  // liquid_world.rs:79-81
+    TRY(stage_up(w));
+    for (ColliderRec& c : w->colliders) memset(c.impulse, 0, sizeof c.impulse);
+    const bool b_uploaded = w->b_dirty;
+    TRY(upload_boundaries(w));
+    w->stats.n_fluid_particles = w->N;
+    w->stats.n_boundary_particles = w->B;
+    if (w->fluids.size() > (size_t)MAX_FLUIDS || w->bounds.size() > (size_t)MAX_BOUNDARIES)
+        return w->fail(SPH_ERR_INVALID, "too many fluids (max %d) or boundaries (max %d)", MAX_FLUIDS, MAX_BOUNDARIES);
+    if (!(dt > F32_EPS)) return SPH_OK;  // timestep_manager.rs:56-58: is_done() before the first substep
+    CU(cudaEventRecord(w->ev[EV_START], w->st));
+    if (w->slab.active) {  // one substep: sph_world_set_substepping refuses slab worlds
+        TRY(slab_begin_step(w));
+        w->stats.n_fluid_particles = w->N;
+    } else {
+        w->Ntot = w->N;
+        w->own_begin = 0;
+    }
+    if (w->Ntot + w->B == 0) return SPH_OK;
+    const sph_step_stats start = w->stats;
+    sph_step_stats total = start;
+    sph_status s = SPH_OK;
+    for (float remaining = dt;;) {
+        const size_t k = w->substeps.size();
+        if (k) {
+            w->stats = start;
+            w->stats.n_boundary_particles = w->B;
+            CU(cudaEventRecord(w->ev[EV_START], w->st));
+        }
+        s = world_substep(w, remaining, g, coupling, colliders, b_uploaded && k == 0);
+        if (k == 0) total = w->stats;
+        else stats_merge(total, w->stats);
+        if (s != SPH_OK || w->substeps.size() == k) break;  // failed, or no solver ran: dt did not advance
+        remaining -= w->dt;                                 // R_{k+1} = R_k - dt_k
+        if (!(remaining > F32_EPS)) break;
+    }
+    w->stats = total;
+    w->stats.n_substeps = (uint32_t)w->substeps.size();
+    w->stats.kernel_launches = w->launches;
+    w->stats.n_ghost_particles = (uint32_t)(w->Ntot - w->N);
+    w->stats.n_migrated = w->slab.migrated_in + w->slab.migrated_out;
+    w->stats.n_exchanges = (uint32_t)w->stats_exchanges;
+    float acc[SP_COUNT] = {0.f, 0.f, 0.f, 0.f};
+    for (size_t i = 0; i < w->n_spans; ++i) {
+        float ms = 0.f;
+        cudaEventElapsedTime(&ms, w->spans[i].a, w->spans[i].b);
+        acc[w->spans[i].slot] += ms;
+    }
+    w->stats.divergence_eval_ms = acc[SP_DIV_EVAL];
+    w->stats.divergence_update_ms = acc[SP_DIV_UPD];
+    w->stats.predict_density_ms = acc[SP_PRED];
+    w->stats.pressure_update_ms = acc[SP_PUPD];
+    return s;
 }
 
 }  // namespace
@@ -2152,6 +2238,29 @@ sph_status sph_world_force_iterations(sph_world* w, int32_t n_div, int32_t n_pre
     if (!w) return SPH_ERR_INVALID;
     w->force_div = n_div;
     w->force_press = n_press;
+    return SPH_OK;
+}
+
+// TimestepManager's cfl_coeff / min_num_substeps / max_num_substeps (timestep_manager.rs:21-46), applied with the even split of
+// DESIGN.md section 12 in place of the commented-out clamp of compute_substep (:87-94)
+sph_status sph_world_set_substepping(sph_world* w, float cfl_coeff, uint32_t min_substeps, uint32_t max_substeps) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    if (!(cfl_coeff >= 0.f)) return w->fail(SPH_ERR_INVALID, "cfl_coeff must be 0 (off) or positive, got %g", (double)cfl_coeff);
+    if (min_substeps == 0 || min_substeps > max_substeps)
+        return w->fail(SPH_ERR_INVALID, "substep bounds need 1 <= min_substeps <= max_substeps, got %u, %u", min_substeps, max_substeps);
+    if (w->desc.slab_count > 1 || w->slab.active) return w->fail(SPH_ERR_INVALID, "substepping is not supported in slab-decomposed worlds");
+    w->cfl_coeff = cfl_coeff;
+    w->min_substeps = min_substeps;
+    w->max_substeps = max_substeps;
+    return SPH_OK;
+}
+
+sph_status sph_world_read_substeps(sph_world* w, float* dts, size_t cap, size_t* n) {
+    if (!w || !n || (cap && !dts)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    *n = w->substeps.size();
+    if (*n && cap) memcpy(dts, w->substeps.data(), std::min(cap, *n) * sizeof(float));
     return SPH_OK;
 }
 

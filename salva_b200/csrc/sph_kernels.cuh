@@ -1051,6 +1051,25 @@ __global__ void k_integrate_acc(const float4* __restrict__ vel, float4* __restri
     }
 }
 
+// The CFL bound's reduction (TimestepManager::max_substep timestep_manager.rs:36-46): max over the owned fluid particles of
+// |v + a * remaining|^2, in the reference's operation order (v + a * R, then ((x^2 + y^2) + z^2)).  Non-negative floats
+// order like their bit patterns, so each warp reduces the bits with __reduce_max_sync and one lane atomicMax-es them into
+// *out, which the host zeroes per substep: the result does not depend on the block order.  A NaN (bits above +inf's)
+// wins the reduction, and the host then takes the largest substep count.
+__global__ void k_cfl_max(const float4* __restrict__ vel, const float4* __restrict__ acc, float remaining, unsigned int* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    unsigned int bits = 0u;
+    if (i < C.n_owned) {
+        const float4 v = vel[C.i_begin + i], a = acc[C.i_begin + i];
+        const float x = __fadd_rn(v.x, __fmul_rn(a.x, remaining));
+        const float y = __fadd_rn(v.y, __fmul_rn(a.y, remaining));
+        const float z = __fadd_rn(v.z, __fmul_rn(a.z, remaining));
+        bits = __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
+    }
+    bits = __reduce_max_sync(0xffffffffu, bits);
+    if ((threadIdx.x & 31u) == 0u && bits) atomicMax(out, bits);
+}
+
 // a22: update_positions dfsph_solver.rs:411-420: pos += (vel + vc) * dt.  bounds_out (optional): the cell-coordinate AABB of
 // the NEW positions (what k_bounds computes), so the next step's grid is sized without a bounds pass and its host round trip.
 __global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, float dt, int* __restrict__ bounds_out) {

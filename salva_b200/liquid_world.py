@@ -571,6 +571,19 @@ class LiquidWorld:
         g = np.asarray(gravity, np.float32)
         self._ck(self._L.sph_world_step(self._w, dt, _fp(g)))
 
+    def set_substepping(self, cfl_coeff=0.4, min_substeps=1, max_substeps=10):
+        """CFL-bounded substeps inside each step (include/sph.h sph_world_set_substepping); the defaults are the reference
+        TimestepManager's (timestep_manager.rs:21-31).  cfl_coeff=0 turns substepping off."""
+        self._ck(self._L.sph_world_set_substepping(self._w, cfl_coeff, min_substeps, max_substeps))
+
+    def substeps(self):
+        """The lengths of the last step's substeps, in order, as float32 (empty when the step ran no solver)."""
+        n = C.c_size_t()
+        self._ck(self._L.sph_world_read_substeps(self._w, None, 0, C.byref(n)))
+        out = np.empty(n.value, np.float32)
+        self._ck(self._L.sph_world_read_substeps(self._w, _fp(out), n.value, C.byref(n)))
+        return out
+
     # -- particle access (fluids_mut() edits, fluid.rs / liquid_world.rs:181-198) -------------------
     def num_particles(self, fluid):
         n = C.c_size_t()
