@@ -7,21 +7,6 @@
 #pragma once
 #include "sph_passes.cuh"
 
-struct ElasticityState {
-    size_t n = 0;            // particle count the rest pose was captured for (re-captured when it changes, :87)
-    uint32_t cap0 = 0;       // rest-list capacity (rows)
-    uint32_t stride0 = 0;
-    float4* pos0 = nullptr;  // positions0.xyz, volumes0 in .w
-    uint32_t* nbr0 = nullptr;  // nbr0[k * stride0 + t]: local original index of the k-th rest contact (self included)
-    uint32_t* cnt0 = nullptr;
-    float* rot = nullptr;      // 9 floats per particle, row-major rotation (warm start for the next step, :134-135)
-    float* grad_tr = nullptr;  // 9 floats per particle: deformation_gradient_tr
-    float* stress = nullptr;   // 6 floats per particle: x y z w a b (:27-37)
-    float4* cur = nullptr;     // current positions (xyz) + mass (.w) in original order
-    uint32_t* slot_of = nullptr;  // sorted slot of local original index t
-    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-};
-
 namespace sphk {
 
 struct M3 {

@@ -15,8 +15,11 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/sph.h"
@@ -43,10 +46,24 @@ const void* g_const_owner = nullptr;
 
 inline uint32_t cdiv(size_t a, size_t b) { return (uint32_t)((a + b - 1) / b); }
 
+// A device buffer that owns its allocation: it moves, never copies, and frees the allocation when it dies.
 template <class T>
 struct DBuf {
     T* p = nullptr;
     size_t cap = 0;
+    DBuf() = default;
+    DBuf(const DBuf&) = delete;
+    DBuf& operator=(const DBuf&) = delete;
+    DBuf(DBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), cap(std::exchange(o.cap, 0)) {}
+    DBuf& operator=(DBuf&& o) noexcept {
+        if (this != &o) {
+            release();
+            p = std::exchange(o.p, nullptr);
+            cap = std::exchange(o.cap, 0);
+        }
+        return *this;
+    }
+    ~DBuf() { release(); }
     cudaError_t ensure(size_t n, bool keep = false, cudaStream_t st = 0) {
         if (n <= cap) return cudaSuccess;
         size_t ncap = std::max(n, cap + cap / 4);
@@ -70,6 +87,79 @@ struct DBuf {
     }
 };
 
+// A linear texture object over a DBuf, destroyed with its owner; declare it after the buffer it views.
+struct Tex {
+    cudaTextureObject_t obj = 0;
+    const void* ptr = nullptr;
+    size_t bytes = 0;
+    Tex() = default;
+    Tex(const Tex&) = delete;
+    Tex& operator=(const Tex&) = delete;
+    ~Tex() {
+        if (obj) cudaDestroyTextureObject(obj);
+    }
+    // rebuilds the object only when the buffer's allocation changed
+    template <class T>
+    cudaError_t bind(const DBuf<T>& b) {
+        if (obj && ptr == b.p && bytes == b.cap * sizeof(T)) return cudaSuccess;
+        if (obj) cudaDestroyTextureObject(obj);
+        obj = 0;
+        cudaResourceDesc rd;
+        memset(&rd, 0, sizeof rd);
+        rd.resType = cudaResourceTypeLinear;
+        rd.res.linear.devPtr = b.p;
+        rd.res.linear.desc = cudaCreateChannelDesc<T>();
+        rd.res.linear.sizeInBytes = b.cap * sizeof(T);
+        cudaTextureDesc td;
+        memset(&td, 0, sizeof td);
+        td.readMode = cudaReadModeElementType;
+        cudaError_t e = cudaCreateTextureObject(&obj, &rd, &td, nullptr);
+        if (e != cudaSuccess) {
+            obj = 0;
+            return e;
+        }
+        ptr = b.p;
+        bytes = b.cap * sizeof(T);
+        return cudaSuccess;
+    }
+};
+
+// Solver and plugin scratch.  The kernels take the raw pointers (.p).
+struct IisphState {
+    DBuf<float4> dii;      // iisph_solver.rs:32
+    DBuf<float4> dij_pjl;  // iisph_solver.rs:34
+    DBuf<float4> s;        // dii * p + dij_pjl
+    DBuf<float> aii;       // iisph_solver.rs:33
+    DBuf<float> next_p;    // iisph_solver.rs:38
+    DBuf<float> prho;      // p / rho^2
+    DBuf<float> next_prho;
+    size_t cap = 0;        // rows of every buffer; 0 until all of them are allocated
+    Tex tex_s;             // over s
+};
+struct ViscosityState {
+    DBuf<float> beta;    // beta[(r * 6 + c) * stride + i]
+    DBuf<float> target;  // target[k * stride + i]            dfsph_viscosity.rs:24
+    DBuf<float4> vv;     // vel + acc * dt
+    DBuf<float4> u4;     // u[0..3]
+    DBuf<float2> u2;     // u[4..5]
+    size_t cap = 0;      // rows of every buffer; 0 until all of them are allocated
+};
+// Becker2009 rest pose of one force (sph_elasticity_host.inl)
+struct ElasticityState {
+    size_t n = 0;            // particle count the rest pose was captured for (re-captured when it changes, :87)
+    uint32_t cap0 = 0;       // rest-list capacity (rows)
+    uint32_t stride0 = 0;
+    DBuf<float4> pos0;       // positions0.xyz, volumes0 in .w
+    DBuf<uint32_t> nbr0;     // nbr0[k * stride0 + t]: local original index of the k-th rest contact (self included)
+    DBuf<uint32_t> cnt0;
+    DBuf<float> rot;         // 9 floats per particle, row-major rotation (warm start for the next step, :134-135)
+    DBuf<float> grad_tr;     // 9 floats per particle: deformation_gradient_tr
+    DBuf<float> stress;      // 6 floats per particle: x y z w a b (:27-37)
+    DBuf<float4> cur;        // current positions (xyz) + mass (.w) in original order
+    DBuf<uint32_t> slot_of;  // sorted slot of local original index t
+    float d0 = 0.f, d1 = 0.f, d2 = 0.f;
+};
+
 struct ForceRec;
 }  // namespace
 struct sph_world;
@@ -81,7 +171,7 @@ struct ForceRec {
     sph_host_force_fn2 host_fn2 = nullptr;  // context-style callback (contacts / boundaries on request)
     uint32_t host_flags = 0;
     void* host_user = nullptr;
-    ElasticityState* elastic = nullptr;  // Becker2009 rest-pose state (sph_elasticity.cuh)
+    std::unique_ptr<ElasticityState> elastic;  // Becker2009 rest-pose state
     uint32_t visc_iters = 0;             // DFSPHViscosity: acceleration updates of the last solve
     float visc_err = 0.f;                // ... and its last strain-rate error
     bool solved = false;                 // has run in a step (sph_debug_read's plugin scratch is valid until particles change)
@@ -96,6 +186,10 @@ struct FluidRec {
     float uniform_mass = 0.f;  // common particle mass if all volumes are equal, else 0
     bool alive = true;         // false after LiquidWorld::remove_fluid (liquid_world.rs:171-173); the slot is reused by the next add
     uint32_t gen = 0;          // handle = slot | gen << 16 (the reference's arena handles carry a generation too)
+    // move-only: the forces own device memory, and std::vector<ForceRec> would still declare a copy
+    FluidRec() = default;
+    FluidRec(FluidRec&&) = default;
+    FluidRec& operator=(FluidRec&&) = default;
 };
 struct BoundaryRec {
     size_t n = 0, offset = 0;
@@ -199,6 +293,9 @@ struct ColliderRec {
     bool alive = true;
     uint32_t gen = 0;
 };
+static_assert(!std::is_copy_constructible<DBuf<float>>::value && !std::is_copy_constructible<ForceRec>::value &&
+                  !std::is_copy_constructible<FluidRec>::value && !std::is_copy_constructible<ColliderRec>::value,
+              "records that own device memory move, never copy");
 
 sph_status iisph_step(sph_world* w, float dt_total, const float g[3]);
 sph_status slab_begin_step(sph_world* w);
@@ -213,14 +310,11 @@ sph_status slab_wait(sph_world* w);
 sph_status p2p_setup(sph_world* w);
 sph_status post_density_refresh(sph_world* w);
 sph_status slab_allreduce(sph_world* w, float* buf, size_t n);
-void iisph_release(sph_world* w);
 void slab_release(sph_world* w);
 const float* iisph_pred(sph_world* w);
 sph_status elasticity_solve(sph_world* w, uint32_t fluid, ForceRec& fr);
-void elasticity_release(ForceRec& fr);
 sph_status elasticity_restore(sph_world* w, ForceRec& fr, size_t n, uint32_t cap0, uint32_t stride0, const char* blob);
 sph_status viscosity_solve(sph_world* w, uint32_t fluid, ForceRec& fr);
-void viscosity_release(sph_world* w);
 bool any_collider(const sph_world* w);
 bool any_contact(const sph_world* w);
 sph_status colliders_update(sph_world* w, bool reposed_all);
@@ -344,10 +438,7 @@ struct sph_world {
     DBuf<float2> vyz2;
     bool nr4_valid = false;     // Akinci normals nr4 = (n, rho) rode with the divergence loop's first update (k_vel_update_u<.., NORMALS>)
     bool akinci_valid = false;  // ... and the Akinci fluid force with the evaluation after it (k_vel_divergence_xsph_u<2>), in xs
-    cudaTextureObject_t tex_pvx = 0, tex_vyz = 0, tex_pk = 0;
-    const void* tex_pvx_ptr = nullptr;
-    const void* tex_vyz_ptr = nullptr;
-    const void* tex_pk_ptr = nullptr;
+    Tex tex_pvx, tex_vyz, tex_pk;
     DBuf<float> he_colors, he_gradc;  // He2014 colours / squared colour-gradient norms (he2014_surface_tension.rs:16-17)
     DBuf<uint32_t> q_out, q_count;     // particles_intersecting_aabb results
     DBuf<float> map_pos, map_vel;      // sph_fluid_map_positions / _velocities: ORIGINAL-order device views
@@ -362,8 +453,7 @@ struct sph_world {
     bool xs_valid = false;    // XSPH sums rode with the divergence loop's last evaluation (k_vel_divergence_xsph_u)
     DBuf<float4> xs;
     uint32_t fused_nblk = 0;
-    cudaTextureObject_t tex_vs = 0;  // the general evaluations gather v* through the texture pipe
-    const void* tex_vs_ptr = nullptr;
+    Tex tex_vs;  // the general evaluations gather v* through the texture pipe
     DBuf<float> partial, errsum;
     DBuf<int> d_scal;  // [0..6] bounds + bad flag, [7] error flag, [8..9] maxcnt, [11] elasticity widest, [12] CFL max |v + a R|^2
     DBuf<unsigned long long> d_cnt;  // [0] bb contacts, [1] ff+fb contacts
@@ -390,6 +480,20 @@ struct sph_world {
     bool ever_stepped = false;
     sph_step_stats stats;
     uint64_t launches = 0;
+
+    // Every DBuf, Tex and record frees itself after this body; it destroys what is not device memory.
+    ~sph_world() {
+        for (auto& s : spans) {
+            cudaEventDestroy(s.a);
+            cudaEventDestroy(s.b);
+        }
+        for (auto& e : ev)
+            if (e) cudaEventDestroy(e);
+        if (ev_lists) cudaEventDestroy(ev_lists);
+        if (h_pinned) cudaFreeHost(h_pinned);
+        if (h_imp) cudaFreeHost(h_imp);
+        if (st) cudaStreamDestroy(st);
+    }
 
     sph_status fail(sph_status s, const char* fmt, ...) {
         char buf[512];
@@ -900,36 +1004,17 @@ sph_status phase_grid(sph_world* w) {
     return SPH_OK;
 }
 
-template <class T>
-sph_status ensure_tex(sph_world* w, cudaTextureObject_t* tex, const void** cur, const T* ptr, size_t n) {
-    if (*cur == ptr && *tex) return SPH_OK;
-    if (*tex) cudaDestroyTextureObject(*tex);
-    *tex = 0;
-    cudaResourceDesc rd;
-    memset(&rd, 0, sizeof rd);
-    rd.resType = cudaResourceTypeLinear;
-    rd.res.linear.devPtr = const_cast<T*>(ptr);
-    rd.res.linear.desc = cudaCreateChannelDesc<T>();
-    rd.res.linear.sizeInBytes = n * sizeof(T);
-    cudaTextureDesc td;
-    memset(&td, 0, sizeof td);
-    td.readMode = cudaReadModeElementType;
-    CU(cudaCreateTextureObject(tex, &rd, &td, nullptr));
-    *cur = ptr;
-    return SPH_OK;
-}
-
 // Inputs and outputs of the density sweep that the DFSPH neighbour search runs over its fresh lists (density_alpha_div)
 sph_status density_args(sph_world* w, DensArgs* D) {
     if (w->unimass) {
-        TRY(ensure_tex(w, &w->tex_vyz, &w->tex_vyz_ptr, w->vyz2.p, w->vyz2.cap));
-        TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
+        CU(w->tex_vyz.bind(w->vyz2));
+        CU(w->tex_pvx.bind(w->pvx4));
     } else {
-        TRY(ensure_tex(w, &w->tex_vs, &w->tex_vs_ptr, w->vs.p, w->vs.cap));
+        CU(w->tex_vs.bind(w->vs));
     }
     TRY(slab_wait(w));  // the sweep gathers v* of ghosts
-    *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx : 0, w->vs.p, w->unimass ? 0 : w->tex_vs, w->vyz2.p,
-                  w->unimass ? w->tex_vyz : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, w->d_scal.p + 7};
+    *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx.obj : 0, w->vs.p, w->unimass ? 0 : w->tex_vs.obj, w->vyz2.p,
+                  w->unimass ? w->tex_vyz.obj : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, w->d_scal.p + 7};
     return SPH_OK;
 }
 
@@ -1201,10 +1286,10 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
     if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) {
-        TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
-        TRY(ensure_tex(w, &w->tex_vyz, &w->tex_vyz_ptr, w->vyz2.p, w->vyz2.cap));
+        CU(w->tex_pvx.bind(w->pvx4));
+        CU(w->tex_vyz.bind(w->vyz2));
     } else {
-        TRY(ensure_tex(w, &w->tex_vs, &w->tex_vs_ptr, w->vs.p, w->vs.cap));
+        CU(w->tex_vs.bind(w->vs));
     }
     float* out = predict ? w->pred.p : w->divv.p;
     const size_t nf = std::max<size_t>(1, w->fluids.size());
@@ -1215,24 +1300,24 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
         uint32_t* tk = w->single_launch ? w->d_ticket.p : nullptr;
         if (w->unimass) {
             if (predict) {
-                LAUNCH_R((k_vel_divergence_u<true>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
+                LAUNCH_R((k_vel_divergence_u<true>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
                          w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
             } else if (xsf) {
                 const float cf = w->fluids[0].forces[0].d.p[0];
-                LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
+                LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
                          w->pk4.p, partial, tk, w->errsum.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
                 w->xs_valid = true;
             } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
                 const AkinciNorms an = akinci_norms(w->h);
-                LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
+                LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
                          w->pk4.p, partial, tk, w->errsum.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
                 w->akinci_valid = true;
             } else {
-                LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx, w->vyz2.p, w->tex_vyz, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
+                LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
                          w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
             }
         } else {
-            DISPATCH2(k_vel_divergence, multi, predict, rg.count, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
+            DISPATCH2(k_vel_divergence, multi, predict, rg.count, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
                       w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p, rg);
         }
         return SPH_OK;
@@ -1246,7 +1331,7 @@ sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) 
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
-    if (w->unimass) TRY(ensure_tex(w, &w->tex_pk, &w->tex_pk_ptr, w->pk4.p, w->pk4.cap));
+    if (w->unimass) CU(w->tex_pk.bind(w->pk4));
     if (normals) {
         CU(w->normals.ensure(std::max(w->Ntot, w->N)));
         w->nr4_valid = true;
@@ -1256,10 +1341,10 @@ sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) 
     SlabArray a1[1] = {{w->vs.p, sizeof(float4)}};
     return run_parts(w, w->unimass ? a : a1, w->unimass ? 3 : 1, nullptr, [&](Range rg, uint32_t) -> sph_status {
         if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
-            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
+            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
                      w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
         else if (w->unimass)
-            DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
+            DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
                       w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr, rg);
         else
             BOOL3(k_vel_update, multi, bf, pressure, rg, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p, w->bforce.p, w->inv_dt);
@@ -1403,9 +1488,9 @@ sph_status phase_forces(sph_world* w) {
                     const AkinciNorms an = akinci_norms(w->h);
                     const float coh_norm = an.coh_norm, h6_64 = an.h6_64, adh_norm = an.adh_norm;
                     if (w->nr4_valid && f == 0) {  // normals (and rho, in .w) came with the first divergence update
-                        TRY(ensure_tex(w, &w->tex_pvx, &w->tex_pvx_ptr, w->pvx4.p, w->pvx4.cap));
-                        if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
-                        else LAUNCH((k_akinci_force_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
+                        CU(w->tex_pvx.bind(w->pvx4));
+                        if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
+                        else LAUNCH((k_akinci_force_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
                         break;
                     }
                     DISPATCH1(k_akinci_normals, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->dens.p, w->normals.p, (uint32_t)f);
@@ -1870,50 +1955,7 @@ void sph_world_destroy(sph_world* w) {
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     cudaSetDevice(w->desc.device);
     if (w->st) cudaStreamSynchronize(w->st);
-    for (int k = 0; k < 2; ++k) {
-        w->pos[k].release(); w->vel[k].release(); w->vc[k].release(); w->bpos[k].release(); w->bvel[k].release();
-        w->orig[k].release(); w->borig[k].release(); w->press[k].release(); w->gid[k].release();
-    }
-    w->vs.release(); w->acc.release(); w->normals.release(); w->dbg_acc.release();
-    w->dens.release(); w->alpha.release(); w->kappa.release(); w->divv.release(); w->pred.release(); w->bvol.release(); w->bforce.release();
-    w->cid.release(); w->rank.release(); w->perm.release(); w->cstart.release(); w->bcid.release(); w->brank.release(); w->bperm.release();
-    w->bstart.release();
-    for (auto& a : w->scan_aux) a.release();
-    for (auto& a : w->scan_aux_k) a.release();
-    w->nbr_f.release(); w->nbr_b.release(); w->cnt_f.release(); w->cnt_b.release();
-    w->partial.release(); w->errsum.release(); w->d_scal.release(); w->d_cnt.release();
-    w->o_a.release(); w->o_b.release(); w->o_c.release(); w->o_mass.release(); w->o_fid.release();
-    iisph_release(w);
-    viscosity_release(w);
     slab_release(w);
-    for (auto& f : w->fluids)
-        for (auto& fr : f.forces) elasticity_release(fr);
-    for (cudaTextureObject_t t : {w->tex_pvx, w->tex_vyz, w->tex_pk})
-        if (t) cudaDestroyTextureObject(t);
-    w->pvx4.release(); w->pk4.release(); w->vyz2.release();
-    if (w->tex_vs) cudaDestroyTextureObject(w->tex_vs);
-    for (auto& s : w->spans) {
-        cudaEventDestroy(s.a);
-        cudaEventDestroy(s.b);
-    }
-    if (w->h_pinned) cudaFreeHost(w->h_pinned);
-    for (auto& c : w->colliders) {
-        c.local.release();
-        c.hgt.release();
-    }
-    w->smp_f.release(); w->smp_xyz.release(); w->smp_cnt.release(); w->smp_off.release(); w->smp_flag.release();
-    w->smp_key[0].release(); w->smp_key[1].release();
-    w->d_cb.release();
-    w->d_imp.release();
-    w->d_chf.release();
-    if (w->h_imp) cudaFreeHost(w->h_imp);
-    w->d_ticket.release();
-    w->d_nb.release();
-    w->xs.release(); w->he_colors.release(); w->he_gradc.release(); w->q_out.release(); w->q_count.release();
-    for (auto& e : w->ev)
-        if (e) cudaEventDestroy(e);
-    if (w->ev_lists) cudaEventDestroy(w->ev_lists);
-    if (w->st) cudaStreamDestroy(w->st);
     if (g_const_owner == w) g_const_owner = nullptr;
     delete w;
 }
@@ -1958,9 +2000,9 @@ sph_status sph_fluid_add(sph_world* w, const float* pos, const float* vel, const
     w->fluids[slot].n = 0;
     recompute_offsets(w);
     w->rows.splice(w->fluids[slot].offset, 0, n, pos, vel, nullptr, volumes, ids.data());
-    w->fluids[slot] = f;
+    w->fluids[slot] = std::move(f);
     recompute_offsets(w);
-    if (handle) *handle = make_handle(slot, f.gen);
+    if (handle) *handle = make_handle(slot, w->fluids[slot].gen);
     return SPH_OK;
 }
 
@@ -1977,7 +2019,7 @@ sph_status sph_fluid_push_force(sph_world* w, uint32_t fluid_h, const sph_force_
         return w->fail(SPH_ERR_INVALID, "The viscosity coefficient must be between 0.0 and 1.0. (dfsph_viscosity.rs:106-110)");
     ForceRec fr;
     fr.d = *force;
-    w->fluids[fluid].forces.push_back(fr);
+    w->fluids[fluid].forces.push_back(std::move(fr));
     return SPH_OK;
 }
 
@@ -1990,7 +2032,7 @@ sph_status sph_fluid_push_host_force(sph_world* w, uint32_t fluid_h, sph_host_fo
     fr.d.kind = FORCE_HOST_CALLBACK;
     fr.host_fn = fn;
     fr.host_user = user;
-    w->fluids[fluid].forces.push_back(fr);
+    w->fluids[fluid].forces.push_back(std::move(fr));
     return SPH_OK;
 }
 
@@ -2282,7 +2324,7 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     size_t width = vec ? 3 : 1;
     if (cap < f.n) return w->fail(SPH_ERR_INVALID, "sph_debug_read: capacity %zu < particle count %zu", cap, f.n);
     const bool iisph_sel = what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_AII || what == SPH_DBG_IISPH_DIJ_PJL;
-    if (iisph_sel && (w->desc.solver != SPH_SOLVER_IISPH || !w->iisph.dii || w->own_begin + w->N > w->iisph.cap))
+    if (iisph_sel && (w->desc.solver != SPH_SOLVER_IISPH || !w->iisph.dii.p || w->own_begin + w->N > w->iisph.cap))
         return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs an IISPH world that has stepped with its current particles", what);
     // plugin scratch: that of the fluid's last force of the selector's kind, solved since its particles last changed
     const ForceRec* pf = nullptr;
@@ -2311,9 +2353,9 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     CU(w->o_c.ensure(std::max(width * N, 3 * std::max(N, w->B))));
     if (pf && pf->elastic) {  // the rest pose is kept in the fluid's original order already
         const ElasticityState& E = *pf->elastic;
-        const float* src = what == SPH_DBG_EL_ROTATION ? E.rot : what == SPH_DBG_EL_GRAD_TR ? E.grad_tr : E.stress;
+        const float* src = what == SPH_DBG_EL_ROTATION ? E.rot.p : what == SPH_DBG_EL_GRAD_TR ? E.grad_tr.p : E.stress.p;
         if (what == SPH_DBG_EL_VOLUME0) {
-            LAUNCH(k_export_w_plain, f.n, 256, (uint32_t)f.n, E.pos0, w->o_c.p);
+            LAUNCH(k_export_w_plain, f.n, 256, (uint32_t)f.n, E.pos0.p, w->o_c.p);
             src = w->o_c.p;
         }
         CU(cudaMemcpyAsync(out, src, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
@@ -2327,7 +2369,7 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         case SPH_DBG_DIVERGENCE: s1 = w->divv.p; break;
         case SPH_DBG_PREDICTED_DENSITY: s1 = w->desc.solver == SPH_SOLVER_IISPH ? iisph_pred(w) : w->pred.p; break;
         case SPH_DBG_PRESSURE: s1 = w->press[c].p; break;
-        case SPH_DBG_IISPH_AII: s1 = w->iisph.aii; break;
+        case SPH_DBG_IISPH_AII: s1 = w->iisph.aii.p; break;
         case SPH_DBG_HE2014_COLOR: s1 = w->he_colors.p; break;
         case SPH_DBG_HE2014_GRADC: s1 = w->he_gradc.p; break;
         default: break;
@@ -2337,10 +2379,10 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     if (s1) LAUNCH(k_export1, N, 256, (uint32_t)N, og, s1 + ob, w->o_c.p);
     else if (what == SPH_DBG_VELOCITY_CHANGE) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->vc[c].p + ob, w->o_c.p);
     else if (what == SPH_DBG_ACCELERATION) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->acc.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_IISPH_DII) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dii + ob, w->o_c.p);
-    else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl + ob, w->o_c.p);
-    else if (what == SPH_DBG_VISC_BETA) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 36u, w->stride, og, w->visc.beta + ob, w->o_c.p);
-    else if (what == SPH_DBG_VISC_TARGET) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 6u, w->stride, og, w->visc.target + ob, w->o_c.p);
+    else if (what == SPH_DBG_IISPH_DII) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dii.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_VISC_BETA) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 36u, w->stride, og, w->visc.beta.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_VISC_TARGET) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 6u, w->stride, og, w->visc.target.p + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_f.p + ob, w->o_c.p);
     else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_b.p + ob, w->o_c.p);
     else return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);
@@ -2469,7 +2511,7 @@ sph_status sph_fluid_push_host_force2(sph_world* w, uint32_t fluid_h, sph_host_f
     fr.host_fn2 = fn;
     fr.host_flags = flags;
     fr.host_user = user;
-    w->fluids[fluid].forces.push_back(fr);
+    w->fluids[fluid].forces.push_back(std::move(fr));
     return SPH_OK;
 }
 
@@ -2484,7 +2526,6 @@ sph_status sph_fluid_remove(sph_world* w, uint32_t fluid_h) {
     TRY(stage_down(w));
     FluidRec& f = w->fluids[fluid];
     w->rows.splice(f.offset, f.n, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
-    for (auto& fr : f.forces) elasticity_release(fr);
     f.forces.clear();
     f.pending_delete.clear();
     f.n_pending = 0;
@@ -2598,7 +2639,7 @@ sph_status sph_collider_register(sph_world* w, uint32_t boundary_h, int32_t samp
         recompute_offsets(w);
         w->b_dirty = true;
     }
-    collider_commit(w, slot, boundary_h, sampling, c, collider);
+    collider_commit(w, slot, boundary_h, sampling, std::move(c), collider);
     return SPH_OK;
 }
 
@@ -2619,13 +2660,10 @@ sph_status sph_collider_register_heightfield(sph_world* w, uint32_t boundary_h, 
     }
     cudaError_t e = cudaMemcpyAsync(c.hgt.p, heights.data(), heights.size() * sizeof(float), cudaMemcpyHostToDevice, w->st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(w->st);
-    if (e != cudaSuccess) {
-        c.hgt.release();
-        return w->fail(SPH_ERR_CUDA, "heightfield collider upload: %s", cudaGetErrorString(e));
-    }
+    if (e != cudaSuccess) return w->fail(SPH_ERR_CUDA, "heightfield collider upload: %s", cudaGetErrorString(e));
     c.hf.hgt = c.hgt.p;
     c.shape.kind = SPH_SHAPE_HEIGHTFIELD;
-    collider_commit(w, slot, boundary_h, SPH_SAMPLING_CONTACT, c, collider);
+    collider_commit(w, slot, boundary_h, SPH_SAMPLING_CONTACT, std::move(c), collider);
     return SPH_OK;
 }
 
@@ -2726,7 +2764,7 @@ sph_status sph_fluid_replace_particles(sph_world* w, uint32_t fluid_h, const flo
     f.n = n;
     f.pending_delete.assign(n, 0);
     f.n_pending = 0;
-    for (auto& fr : f.forces) elasticity_release(fr);  // a rest pose belongs to the particle set it was captured from
+    for (auto& fr : f.forces) fr.elastic.reset();  // a rest pose belongs to the particle set it was captured from
     recompute_offsets(w);
     w->slab.global_valid = false;
     return SPH_OK;
@@ -2784,7 +2822,7 @@ sph_status snapshot_write(sph_world* w, Writer& wr) {
     for (auto& f : w->fluids)
         for (auto& fr : f.forces) {
             SnapElastic se{0, 0, 0};
-            const ElasticityState* E = fr.elastic;
+            const ElasticityState* E = fr.elastic.get();
             if (fr.d.kind == SPH_FORCE_BECKER2009_ELASTICITY && E && E->n) se = SnapElastic{E->n, E->cap0, E->stride0};
             wr.put(&se, sizeof se);
             if (!se.n) continue;
@@ -2792,13 +2830,13 @@ sph_status snapshot_write(sph_world* w, Writer& wr) {
             const size_t bytes = n * sizeof(float4) + n * sizeof(uint32_t) + nl * sizeof(uint32_t) + 9 * n * sizeof(float);
             if (wr.p && wr.off + bytes <= wr.cap) {
                 char* dst = wr.p + wr.off;
-                CU(cudaMemcpyAsync(dst, E->pos0, n * sizeof(float4), cudaMemcpyDeviceToHost, w->st));
+                CU(cudaMemcpyAsync(dst, E->pos0.p, n * sizeof(float4), cudaMemcpyDeviceToHost, w->st));
                 dst += n * sizeof(float4);
-                CU(cudaMemcpyAsync(dst, E->cnt0, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
+                CU(cudaMemcpyAsync(dst, E->cnt0.p, n * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
                 dst += n * sizeof(uint32_t);
-                CU(cudaMemcpyAsync(dst, E->nbr0, nl * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
+                CU(cudaMemcpyAsync(dst, E->nbr0.p, nl * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
                 dst += nl * sizeof(uint32_t);
-                CU(cudaMemcpyAsync(dst, E->rot, 9 * n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+                CU(cudaMemcpyAsync(dst, E->rot.p, 9 * n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
                 CU(cudaStreamSynchronize(w->st));
             }
             wr.off += bytes;
@@ -2894,7 +2932,7 @@ sph_status sph_world_snapshot_load(sph_world* w, const void* buffer, size_t leng
             SnapElastic se;
             if (!need(sizeof se)) return w->fail(SPH_ERR_INVALID, "snapshot truncated");
             take(&se, sizeof se);
-            elasticity_release(fr);
+            fr.elastic.reset();
             if (!se.n) continue;
             const size_t n = (size_t)se.n, nl = (size_t)se.cap0 * se.stride0;
             if (!need(n * sizeof(float4) + n * sizeof(uint32_t) + nl * sizeof(uint32_t) + 9 * n * sizeof(float))) return w->fail(SPH_ERR_INVALID, "snapshot truncated");

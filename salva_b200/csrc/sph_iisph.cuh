@@ -7,18 +7,6 @@
 #pragma once
 #include "sph_passes.cuh"
 
-struct IisphState {
-    float4* dii = nullptr;      // iisph_solver.rs:32
-    float4* dij_pjl = nullptr;  // iisph_solver.rs:34
-    float4* s = nullptr;        // dii * p + dij_pjl
-    float* aii = nullptr;       // iisph_solver.rs:33
-    float* next_p = nullptr;    // iisph_solver.rs:38
-    float* prho = nullptr;      // p / rho^2
-    float* next_prho = nullptr;
-    size_t cap = 0;
-    cudaTextureObject_t tex_s = 0;
-};
-
 namespace sphk {
 
 // pressures *= 0.5 (iisph_solver.rs:673-677) and prho = p / rho^2

@@ -9,15 +9,6 @@
 #pragma once
 #include "sph_passes.cuh"
 
-struct ViscosityState {
-    float* beta = nullptr;    // beta[(r * 6 + c) * stride + i]
-    float* target = nullptr;  // target[k * stride + i]            dfsph_viscosity.rs:24
-    float4* vv = nullptr;     // vel + acc * dt
-    float4* u4 = nullptr;     // u[0..3]
-    float2* u2 = nullptr;     // u[4..5]
-    size_t cap = 0;
-};
-
 namespace sphk {
 
 __global__ void k_visc_vv(const float4* __restrict__ vel, const float4* __restrict__ acc, float dt, float4* __restrict__ vv) {
