@@ -385,6 +385,16 @@ public:
 
     // Advances the simulation by dt seconds (liquid_world.rs:62-64).
     void step(Real dt, const Vector3& gravity) { step_with_coupling(dt, gravity, nullptr); }
+    // n steps of step(dt, gravity) in one call, steps 2..n as one CUDA graph (sph_world_step_many); returns the steps done.
+    // On an error it throws as step() does, before the host mirror is pulled.
+    uint32_t step_many(Real dt, const Vector3& gravity, uint32_t n) {
+        push_host_edits();
+        const float g[3] = {gravity.x, gravity.y, gravity.z};
+        uint32_t done = 0;
+        check(sph_world_step_many(raw_, dt, g, n, &done));
+        pull_results();
+        return done;
+    }
     // liquid_world.rs:67-158
     void step_with_coupling(Real dt, const Vector3& gravity, CouplingManager* coupling) {
         push_host_edits();

@@ -338,6 +338,32 @@ sph_status sph_world_particles_in_heightfield(sph_world* w, const sph_heightfiel
 /* LiquidWorld::step  liquid_world.rs:62-158 */
 sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]);
 
+/* n_steps calls of sph_world_step(w, dt, gravity) in one call (LiquidWorld::step liquid_world.rs:62-158, repeated).  Step 1
+ * runs as sph_world_step does; steps 2..n_steps run as one CUDA graph whose Jacobi loops end on the device, with no host round
+ * trip between steps.  The results equal those of the n_steps calls, bit for bit in deterministic mode.  *steps_done is the
+ * number of steps that returned SPH_OK; on an error the failing step is applied as sph_world_step applies it, and its status
+ * is returned.  sph_world_stats afterwards merges the steps as substeps are merged: times and counts summed, max_neighbors the
+ * widest, the rest the last step's, n_substeps the steps run, kernel_launches the host's launches (a graph launch counts
+ * one), phase times 0 for steps run in the graph, step_ms the device time of the call, and grid_dims, when the last step ran in
+ * the graph, the dims of the graph's grid (the fluid and boundary AABB with 4 cells to spare on every side, DESIGN.md
+ * section 13) rather than of the grid that step would have had on its own.  A driver older than CUDA 12.4 runs every step as
+ * sph_world_step does (records with on_device 0).  DFSPH on one GPU only: SPH_ERR_INVALID,
+ * nothing changed, for IISPH, Becker2009 or DFSPHViscosity forces, host forces, registered colliders, substepping on
+ * (cfl_coeff != 0) and slab-decomposed worlds.  n_steps == 0 does nothing.  See DESIGN.md section 13. */
+sph_status sph_world_step_many(sph_world* w, float dt, const float gravity[3], uint32_t n_steps, uint32_t* steps_done);
+
+/* What one step did (sph_step_stats' per-step counts; liquid_world.rs:84-148 counters) */
+typedef struct {
+    uint32_t n_divergence_iter, n_pressure_iter, n_divergence_eval, n_pressure_eval;
+    float    last_divergence_error, last_density_error;
+    uint32_t max_neighbors;
+    uint32_t on_device;            /* 1: this step ran inside the graph, 0: on the per-step path */
+    uint64_t n_contacts;
+} sph_step_record;
+/* One record per step of the last sph_world_step / sph_world_step_many call, in order: min(cap, *n) are written, and *n
+ * (which may exceed cap) is the count. */
+sph_status sph_world_read_step_records(sph_world* w, sph_step_record* out, size_t cap, size_t* n);
+
 /* trait CouplingManager (coupling/coupling_manager.rs:9-28) + LiquidWorld::step_with_coupling (liquid_world.rs:67-158).
  * update_boundaries runs after this substep's FLUID particles are in the cell grid and before the boundaries are
  * (liquid_world.rs:86-103): particle queries issued from it return fluid particles only, and it may rewrite boundaries

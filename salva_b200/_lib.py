@@ -48,6 +48,12 @@ HOST_FORCE_FN = C.CFUNCTYPE(None, C.c_void_p, C.c_float, C.c_float, C.c_float, C
 
 
 
+class StepRecord(C.Structure):
+    _fields_ = [(n, C.c_uint32) for n in ("n_divergence_iter", "n_pressure_iter", "n_divergence_eval", "n_pressure_eval")] + \
+               [("last_divergence_error", C.c_float), ("last_density_error", C.c_float), ("max_neighbors", C.c_uint32),
+                ("on_device", C.c_uint32), ("n_contacts", C.c_uint64)]
+
+
 class BoundaryView(C.Structure):
     _fields_ = [("n", C.c_size_t), ("positions_xyz", C.POINTER(C.c_float)), ("velocities_xyz", C.POINTER(C.c_float)),
                 ("volumes", C.POINTER(C.c_float))]
@@ -108,6 +114,8 @@ SYMBOLS = {
     "sph_boundary_read_forces": (C.c_int, [_vp, C.c_uint32, _fp, C.c_size_t]),
     "sph_boundary_read_volumes": (C.c_int, [_vp, C.c_uint32, _fp, C.c_size_t]),
     "sph_world_step": (C.c_int, [_vp, C.c_float, _fp]),
+    "sph_world_step_many": (C.c_int, [_vp, C.c_float, _fp, C.c_uint32, C.POINTER(C.c_uint32)]),
+    "sph_world_read_step_records": (C.c_int, [_vp, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
     "sph_world_force_iterations": (C.c_int, [_vp, C.c_int32, C.c_int32]),
     "sph_world_set_substepping": (C.c_int, [_vp, C.c_float, C.c_uint32, C.c_uint32]),
     "sph_world_read_substeps": (C.c_int, [_vp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),

@@ -359,6 +359,41 @@ struct SlabState {
     unsigned long long global_n = 0;
 };
 
+// sph_world_step_many's captured steps (sph_graph.inl): instantiated graphs, each with the state it was captured from
+struct StepGraph {
+    std::vector<char> key;
+    cudaGraph_t g = nullptr;
+    cudaGraphExec_t x = nullptr;
+};
+struct StepGraphs {
+    std::vector<StepGraph> cache;       // at most one per parity of the fluid and the boundary buffers
+    std::vector<cudaStream_t> streams;  // conditional bodies are captured on these, one per nesting level
+    int depth = 0;
+    DBuf<GraphCtl> ctl;
+    DBuf<StepRec> rec;
+    GraphCtl* h_ctl = nullptr;          // pinned
+    cudaGraphConditionalHandle h_lists = 0;  // the IF of the step being captured past its neighbour search
+    cudaGraph_t top = nullptr;          // the graph being captured
+    Envelope env{};                     // the fluid cell range the graph's grid covers with ENVELOPE_MARGIN to spare
+    bool env_valid = false;             // env was set up by an earlier call
+    bool driver_checked = false;
+    bool unsupported = false;           // the driver predates CUDA 12.4: step_many runs the per-step path
+    void drop() {
+        for (auto& e : cache) {
+            if (e.x) cudaGraphExecDestroy(e.x);
+            if (e.g) cudaGraphDestroy(e.g);
+        }
+        cache.clear();
+    }
+    void release() {
+        drop();
+        for (auto s : streams) cudaStreamDestroy(s);
+        streams.clear();
+        if (h_ctl) cudaFreeHost(h_ctl);
+        h_ctl = nullptr;
+    }
+};
+
 enum { EV_START = 0, EV_GRID, EV_NBR, EV_DENS, EV_DIV, EV_FOLD, EV_FORCES, EV_INTEG, EV_PRESS, EV_END, EV_COUNT };
 
 }  // namespace
@@ -480,6 +515,10 @@ struct sph_world {
     bool ever_stepped = false;
     sph_step_stats stats;
     uint64_t launches = 0;
+    uint32_t max_nb_b = 0;                 // the widest boundary list of the last neighbour search
+    std::vector<sph_step_record> records;  // one per step of the last sph_world_step / sph_world_step_many call
+    StepGraphs graphs;                     // sph_world_step_many's captured steps (sph_graph.inl)
+    bool cap = false;                      // the launches go into a step graph: no host read-back, sync or event
 
     // Every DBuf, Tex and record frees itself after this body; it destroys what is not device memory.
     ~sph_world() {
@@ -490,6 +529,7 @@ struct sph_world {
         for (auto& e : ev)
             if (e) cudaEventDestroy(e);
         if (ev_lists) cudaEventDestroy(ev_lists);
+        graphs.release();
         if (h_pinned) cudaFreeHost(h_pinned);
         if (h_imp) cudaFreeHost(h_imp);
         if (st) cudaStreamDestroy(st);
@@ -551,6 +591,7 @@ inline int boundary_slot(const sph_world* w, uint32_t handle) {
 
 enum { SP_DIV_EVAL = 0, SP_DIV_UPD, SP_PRED, SP_PUPD, SP_COUNT };
 sph_status span_begin(sph_world* w, int slot) {
+    if (w->cap) return SPH_OK;
     if (w->n_spans == w->spans.size()) {
         sph_world::Span s{slot, nullptr, nullptr};
         CU(cudaEventCreate(&s.a));
@@ -562,8 +603,15 @@ sph_status span_begin(sph_world* w, int slot) {
     return SPH_OK;
 }
 sph_status span_end(sph_world* w) {
+    if (w->cap) return SPH_OK;
     CU(cudaEventRecord(w->spans[w->n_spans].b, w->st));
     w->n_spans++;
+    return SPH_OK;
+}
+
+// a phase boundary's timing event; a step graph records none (its conditional bodies cannot hold event nodes)
+sph_status ev_record(sph_world* w, int e) {
+    if (!w->cap) CU(cudaEventRecord(w->ev[e], w->st));
     return SPH_OK;
 }
 
@@ -888,33 +936,11 @@ sph_status apply_pending_deletes(sph_world* w) {
 }
 
 // ---- step phases ----------------------------------------------------------------------------------
-sph_status phase_grid(sph_world* w) {
-    size_t N = w->Ntot, B = w->B;  // the sort covers owned + ghost slots
-    int c = w->cur, bc = w->bcur;
-    // slab worlds: the prologue appended immigrants / ghosts behind the owned range of the live arrays and flagged the
-    // particles that left; the sort reads [off, off + Nin) and drops the flagged slots.  Elsewhere: all N slots from 0.
-    const uint32_t off = w->slab.active ? w->slab.sort_off : 0u;
-    const size_t Nin = w->slab.active ? w->slab.sort_n : N;
-    const uint32_t* dead = w->slab.active ? w->slab.flag.p : nullptr;
-    const uint32_t n_dead = w->slab.active ? w->slab.sort_dead_n : 0u;
-    int init[11] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0, 0, 0, 0, 0};
-    CU(cudaMemcpyAsync(w->d_scal.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
-    CU(cudaMemsetAsync(w->d_cnt.p, 0, 2 * sizeof(unsigned long long), w->st));
-    int hb[7];
-    if (w->nb_valid && !w->slab.active && N) {
-        // positions are exactly what the last step's k_update_positions wrote (no host edit since): its bounds came back with
-        // that step's final read-back, so this step starts without a bounds pass and without a host round trip
-        memcpy(hb, w->nb, sizeof hb);
-    } else {
-        if (Nin) {
-            k_bounds<<<std::min<uint32_t>(cdiv(Nin, 256), 296), 256, 0, w->st>>>(w->pos[c].p + off, (uint32_t)Nin, w->d_scal.p);
-            w->launches++;
-        }
-        CU(cudaMemcpyAsync(hb, w->d_scal.p, sizeof hb, cudaMemcpyDeviceToHost, w->st));
-        CU(cudaStreamSynchronize(w->st));
-    }
-    w->nb_valid = false;
-    if (hb[6] || w->b_bad) return w->fail(SPH_ERR_INVALID, "non-finite or out-of-range particle coordinates");
+// The dense cell grid over the cell-coordinate AABB hb (lo xyz, hi xyz) of the fluid, with the boundaries' AABB and one padding
+// cell each side: its constants (uploaded) and cell arrays.  *ncell: its cells.
+sph_status grid_size(sph_world* w, const int* hb_fluid, size_t* ncell_out) {
+    int hb[6];
+    memcpy(hb, hb_fluid, sizeof hb);
     for (int a = 0; a < 3; ++a) {  // boundary AABB: static, kept on the host
         hb[a] = std::min(hb[a], w->b_aabb[a]);
         hb[3 + a] = std::max(hb[3 + a], w->b_aabb[3 + a]);
@@ -939,6 +965,82 @@ sph_status phase_grid(sph_world* w) {
     w->stats.grid_dims[0] = (uint32_t)dims[0];
     w->stats.grid_dims[1] = (uint32_t)dims[1];
     w->stats.grid_dims[2] = (uint32_t)dims[2];
+    *ncell_out = ncell;
+    return SPH_OK;
+}
+
+// The boundaries' counting sort on the current grid — reused while neither the boundaries nor the cell mapping changed
+// (static tanks).  ncell: the grid's cells.
+sph_status sort_boundaries(sph_world* w, size_t ncell) {
+    const size_t B = w->B;
+    const int bc = w->bcur;
+    const int xys = w->slab.active ? 1 : w->xysub;
+    const int gridkey[6] = {w->hc.ox, w->hc.oy, w->hc.oz, w->hc.nx, w->hc.ny, w->hc.nz};
+    const bool reuse_b = w->b_sorted_valid && memcmp(gridkey, w->b_sorted_grid, sizeof gridkey) == 0;
+    w->b_reused = reuse_b;
+    if (!reuse_b) CU(cudaMemsetAsync(w->bstart.p, 0, (ncell + 1) * sizeof(uint32_t), w->st));
+    if (B && !reuse_b) {
+        if (xys > 1) LAUNCH(k_cell_hist_xy, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p);
+        else LAUNCH(k_cell_hist, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, (const uint32_t*)nullptr, 0u);
+        TRY(scan_exclusive(w, w->bstart.p, ncell + 1));
+        LAUNCH(k_cell_scatter, B, 256, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, w->bperm.p);
+        // in-cell order by original index: the same whether the input is a fresh upload or the last sort of boundaries that
+        // colliders moved on the device
+        if (w->desc.deterministic)
+            LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, (const uint32_t*)w->borig[bc].p, (const float4*)nullptr);
+        GatherSet g;
+        memset(&g, 0, sizeof g);
+        g.in4[0] = w->bpos[bc].p; g.out4[0] = w->bpos[bc ^ 1].p;
+        g.in4[1] = w->bvel[bc].p; g.out4[1] = w->bvel[bc ^ 1].p;
+        g.n4 = 2;
+        g.in1[0] = w->borig[bc].p; g.out1[0] = w->borig[bc ^ 1].p;
+        g.n1 = 1;
+        LAUNCH(k_gather, B, 256, (uint32_t)B, w->bperm.p, g);
+        w->bcur = bc ^ 1;
+    }
+    if (!reuse_b) {
+        memcpy(w->b_sorted_grid, gridkey, sizeof gridkey);
+        w->b_sorted_valid = true;
+    }
+    return SPH_OK;
+}
+
+sph_status phase_grid(sph_world* w) {
+    size_t N = w->Ntot;  // the sort covers owned + ghost slots
+    int c = w->cur;
+    // slab worlds: the prologue appended immigrants / ghosts behind the owned range of the live arrays and flagged the
+    // particles that left; the sort reads [off, off + Nin) and drops the flagged slots.  Elsewhere: all N slots from 0.
+    const uint32_t off = w->slab.active ? w->slab.sort_off : 0u;
+    const size_t Nin = w->slab.active ? w->slab.sort_n : N;
+    const uint32_t* dead = w->slab.active ? w->slab.flag.p : nullptr;
+    const uint32_t n_dead = w->slab.active ? w->slab.sort_dead_n : 0u;
+    size_t ncell;
+    if (w->cap) {  // a step graph runs on the envelope's grid, which graph_prepare set up
+        CU(cudaMemsetAsync(w->d_scal.p + 6, 0, 5 * sizeof(int), w->st));
+        CU(cudaMemsetAsync(w->d_cnt.p, 0, 2 * sizeof(unsigned long long), w->st));
+        ncell = (size_t)w->hc.nx * w->hc.ny * w->hc.nz;
+    } else {
+        int init[11] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0, 0, 0, 0, 0};
+        CU(cudaMemcpyAsync(w->d_scal.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
+        CU(cudaMemsetAsync(w->d_cnt.p, 0, 2 * sizeof(unsigned long long), w->st));
+        int hb[7];
+        if (w->nb_valid && !w->slab.active && N) {
+            // positions are exactly what the last step's k_update_positions wrote (no host edit since): its bounds came back with
+            // that step's final read-back, so this step starts without a bounds pass and without a host round trip
+            memcpy(hb, w->nb, sizeof hb);
+        } else {
+            if (Nin) {
+                k_bounds<<<std::min<uint32_t>(cdiv(Nin, 256), 296), 256, 0, w->st>>>(w->pos[c].p + off, (uint32_t)Nin, w->d_scal.p);
+                w->launches++;
+            }
+            CU(cudaMemcpyAsync(hb, w->d_scal.p, sizeof hb, cudaMemcpyDeviceToHost, w->st));
+            CU(cudaStreamSynchronize(w->st));
+        }
+        w->nb_valid = false;
+        if (hb[6] || w->b_bad) return w->fail(SPH_ERR_INVALID, "non-finite or out-of-range particle coordinates");
+        TRY(grid_size(w, hb, &ncell));
+    }
+    const int xys = w->slab.active ? 1 : w->xysub;  // x / y bins per cell (row order, Consts::xysub)
     // fluid: counting sort by cell, then reorder every persistent array
     CU(cudaMemsetAsync(w->cstart.p, 0, (ncell + 1) * sizeof(uint32_t), w->st));
     if (xys > 1) LAUNCH(k_cell_hist_xy, Nin, 256, w->pos[c].p + off, (uint32_t)Nin, w->cid.p, w->rank.p, w->cstart.p);  // (never a slab world: no dead slots)
@@ -967,34 +1069,8 @@ sph_status phase_grid(sph_world* w) {
         LAUNCH(k_gather_vstar, N, 256, (uint32_t)N, w->perm.p, g, w->vs.p, w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
         w->cur = c ^ 1;
     }
-    // boundaries: same sort — reused while neither the boundaries nor the cell mapping changed (static tanks)
-    const int gridkey[6] = {w->hc.ox, w->hc.oy, w->hc.oz, w->hc.nx, w->hc.ny, w->hc.nz};
-    const bool reuse_b = w->b_sorted_valid && memcmp(gridkey, w->b_sorted_grid, sizeof gridkey) == 0;
-    w->b_reused = reuse_b;
-    if (!reuse_b) CU(cudaMemsetAsync(w->bstart.p, 0, (ncell + 1) * sizeof(uint32_t), w->st));
-    if (B && !reuse_b) {
-        if (xys > 1) LAUNCH(k_cell_hist_xy, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p);
-        else LAUNCH(k_cell_hist, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, (const uint32_t*)nullptr, 0u);
-        TRY(scan_exclusive(w, w->bstart.p, ncell + 1));
-        LAUNCH(k_cell_scatter, B, 256, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, w->bperm.p);
-        // in-cell order by original index: the same whether the input is a fresh upload or the last sort of boundaries that
-        // colliders moved on the device
-        if (w->desc.deterministic)
-            LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, (const uint32_t*)w->borig[bc].p, (const float4*)nullptr);
-        GatherSet g;
-        memset(&g, 0, sizeof g);
-        g.in4[0] = w->bpos[bc].p; g.out4[0] = w->bpos[bc ^ 1].p;
-        g.in4[1] = w->bvel[bc].p; g.out4[1] = w->bvel[bc ^ 1].p;
-        g.n4 = 2;
-        g.in1[0] = w->borig[bc].p; g.out1[0] = w->borig[bc ^ 1].p;
-        g.n1 = 1;
-        LAUNCH(k_gather, B, 256, (uint32_t)B, w->bperm.p, g);
-        w->bcur = bc ^ 1;
-    }
-    if (!reuse_b) {
-        memcpy(w->b_sorted_grid, gridkey, sizeof gridkey);
-        w->b_sorted_valid = true;
-    }
+    TRY(sort_boundaries(w, ncell));
+    if (w->cap && !w->b_reused) return w->fail(SPH_ERR_INVALID, "step graph: the boundaries are not sorted on the envelope's grid");
     CU(cudaGetLastError());
     if (w->slab.active) {
         TRY(slab_after_sort(w));
@@ -1060,6 +1136,10 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
         uint32_t* maxcnt = reinterpret_cast<uint32_t*>(w->d_scal.p + 8);
         LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
                w->cnt_f.p, w->cnt_b.p, maxcnt, D);
+        if (w->cap) {  // a step graph checks the capacities on the device and skips the rest of the step past them
+            k_lists_check<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_scal.p, w->cap_f, w->cap_b, w->graphs.h_lists);
+            break;
+        }
         int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous
         CU(cudaMemcpyAsync(hs, w->d_scal.p + 7, 3 * sizeof(int), cudaMemcpyDeviceToHost, w->st));
         CU(cudaEventRecord(w->ev_lists, w->st));
@@ -1070,6 +1150,7 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
         if (hs[0] & ~ERR_SEARCH_ZERO_DENSITY)
             return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
         w->stats.max_neighbors = (uint32_t)hs[1];
+        w->max_nb_b = (uint32_t)hs[2];
         bool grow = false;
         if ((uint32_t)hs[1] > w->cap_f) {
             w->cap_f = ((uint32_t)hs[1] + 15) / 16 * 16;
@@ -1087,7 +1168,7 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
         TRY(upload_consts(w));
     }
     if (!N) {  // boundaries only
-        CU(cudaEventRecord(w->ev[EV_NBR], w->st));
+        TRY(ev_record(w, EV_NBR));
         if (speculative) TRY(speculative(w));
     }
     if (N) {
@@ -1105,6 +1186,14 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     return SPH_OK;
 }
 
+// the particle count of every fluid as the loop error divides by it (slab worlds: over all ranks)
+std::array<float, MAX_FLUIDS> loop_sizes(const sph_world* w) {
+    std::array<float, MAX_FLUIDS> n{};
+    for (size_t f = 0; f < w->fluids.size() && f < (size_t)MAX_FLUIDS; ++f)
+        n[f] = (float)(w->slab.active ? (double)w->slab.global_n : (double)w->fluids[f].n);
+    return n;
+}
+
 // mean-per-fluid -> max over fluids (dfsph_solver.rs:153-158, :347-352)
 sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     int nf = (int)w->fluids.size();
@@ -1116,12 +1205,7 @@ sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     TRY(slab_allreduce(w, w->errsum.p, nf));  // multi-GPU: the means are over ALL ranks' particles
     CU(cudaMemcpyAsync(w->h_pinned, w->errsum.p, nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
     CU(cudaStreamSynchronize(w->st));
-    float mx = 0.f;
-    for (int f = 0; f < nf; ++f) {
-        double n = w->slab.active ? (double)w->slab.global_n : (double)w->fluids[f].n;
-        if (n > 0) mx = std::max(mx, w->h_pinned[f] / (float)n);
-    }
-    *out = mx;
+    *out = loop_error(w->h_pinned, loop_sizes(w).data(), nf);
     return SPH_OK;
 }
 
@@ -1587,54 +1671,15 @@ sph_status timestep_advance(sph_world* w, float remaining) {
     }
     w->dt = dt;
     w->inv_dt = dt == 0.f ? 0.f : 1.0f / dt;
-    w->substeps.push_back(dt);
+    if (!w->cap) w->substeps.push_back(dt);
     return SPH_OK;
 }
 
-// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k
-sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
+// update_velocities :422-430, zero vc :689-691, acc += gravity :574-578, the non-pressure forces and the integration, after the
+// divergence loop ended in the state of xs_valid, nr4_valid and akinci_valid
+sph_status dfsph_fold(sph_world* w, float remaining, const float g[3]) {
     size_t N = w->N;
-    int c = w->cur, bc = w->bcur;
-    const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
-    uint32_t nblk = 0;
-    (void)bc; (void)multi; (void)bf;
-    // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step)
-    w->stats.n_divergence_iter = w->stats.n_divergence_eval = 0;
-    w->xs_valid = false;
-    w->nr4_valid = w->akinci_valid = false;
-    const bool akf = akinci_fusable_u(w);
-    uint32_t maxit = w->force_div >= 0 ? (uint32_t)w->force_div + 1 : w->desc.max_divergence_iter;
-    for (uint32_t i = 0; i < maxit; ++i) {
-        if (i == 0 && w->fused_first_div) {
-            nblk = w->fused_nblk;  // evaluation 0 was computed by the neighbour search
-        } else {
-            TRY(span_begin(w, SP_DIV_EVAL));
-            TRY(launch_vel_divergence(w, false, &nblk));
-            TRY(span_end(w));
-        }
-        w->stats.n_divergence_eval++;
-        if (w->force_div >= 0) {
-            if ((int)i >= w->force_div) break;
-        } else if (i < w->desc.min_divergence_iter && i + 1 < maxit) {
-            // the break needs `i >= min_iter` (:486): this evaluation's error cannot end the loop and the next
-            // evaluation reports a fresher one, so neither the read-back (a host sync) nor the allreduce is needed
-            w->errsum_ready = false;
-        } else {
-            float avg;
-            TRY(read_error(w, nblk, &avg));
-            w->stats.last_divergence_error = avg;
-            float max_err = w->desc.max_divergence_error * w->inv_dt * 0.01f;
-            if (avg <= max_err && i >= w->desc.min_divergence_iter) break;
-        }
-        if (!(i == 0 && w->fused_first_div)) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts
-        TRY(span_begin(w, SP_DIV_UPD));
-        TRY(launch_vel_update(w, false, akf && i == 0));
-        TRY(span_end(w));
-        w->xs_valid = false;  // v* moved on: XSPH sums of the evaluation above are stale unless another evaluation follows
-        w->stats.n_divergence_iter++;
-    }
-    CU(cudaEventRecord(w->ev[EV_DIV], w->st));
-    // update_velocities :422-430, zero vc :689-691, acc += gravity :574-578
+    int c = w->cur;
     TRY(slab_wait(w));
     // the first force of fluid 0 may already sit in xs: the XSPH sums of the loop's last evaluation (acc = g + xs * inv_dt) or
     // the Akinci fluid force (acc = g + xs; a scale of 1 leaves the product exact)
@@ -1648,53 +1693,109 @@ sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
         for (const ForceRec& fr : w->fluids[f].forces)
             if (!(folded && f == 0 && &fr == &w->fluids[0].forces[0])) quiet_forces = false;
     if (quiet_forces && w->cfl_coeff == 0.f) {
-        CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
-        CU(cudaEventRecord(w->ev[EV_FORCES], w->st));
+        TRY(ev_record(w, EV_FOLD));
+        TRY(ev_record(w, EV_FORCES));
         TRY(timestep_advance(w, remaining));  // :702
         LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale, w->dt,
                w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
     } else {
         LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale);  // ghosts too (vel = v*)
-        CU(cudaEventRecord(w->ev[EV_FOLD], w->st));
+        TRY(ev_record(w, EV_FOLD));
         if (!quiet_forces) TRY(phase_forces(w));
-        CU(cudaEventRecord(w->ev[EV_FORCES], w->st));
+        TRY(ev_record(w, EV_FORCES));
         TRY(launch_cfl_max(w, w->vel[c].p, remaining));
         TRY(timestep_advance(w, remaining));  // :702
         LAUNCH(k_integrate_acc, N, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, w->dt, w->unimass ? w->pvx4.p : nullptr,
                w->unimass ? w->vyz2.p : nullptr);
     }
     TRY(refresh_vstar(w));
-    CU(cudaEventRecord(w->ev[EV_INTEG], w->st));
+    return ev_record(w, EV_INTEG);
+}
+
+// The Jacobi loops of a step graph (sph_graph.inl): the same launches, ended on the device
+sph_status graph_divergence_loop(sph_world* w, float remaining, const float g[3]);
+sph_status graph_pressure_loop(sph_world* w);
+
+// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k
+sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
+    size_t N = w->N;
+    int c = w->cur;
+    uint32_t nblk = 0;
+    // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step)
+    w->stats.n_divergence_iter = w->stats.n_divergence_eval = 0;
+    w->xs_valid = false;
+    w->nr4_valid = w->akinci_valid = false;
+    const bool akf = akinci_fusable_u(w);
+    uint32_t maxit = w->force_div >= 0 ? (uint32_t)w->force_div + 1 : w->desc.max_divergence_iter;
+    if (w->cap) {
+        TRY(graph_divergence_loop(w, remaining, g));  // with the post-loop fold of every way the loop can end
+    } else {
+        for (uint32_t i = 0; i < maxit; ++i) {
+            if (i == 0 && w->fused_first_div) {
+                nblk = w->fused_nblk;  // evaluation 0 was computed by the neighbour search
+            } else {
+                TRY(span_begin(w, SP_DIV_EVAL));
+                TRY(launch_vel_divergence(w, false, &nblk));
+                TRY(span_end(w));
+            }
+            w->stats.n_divergence_eval++;
+            if (w->force_div >= 0) {
+                if ((int)i >= w->force_div) break;
+            } else if (i < w->desc.min_divergence_iter && i + 1 < maxit) {
+                // the break needs `i >= min_iter` (:486): this evaluation's error cannot end the loop and the next
+                // evaluation reports a fresher one, so neither the read-back (a host sync) nor the allreduce is needed
+                w->errsum_ready = false;
+            } else {
+                float avg;
+                TRY(read_error(w, nblk, &avg));
+                w->stats.last_divergence_error = avg;
+                if (loop_exit(avg, w->desc.max_divergence_error, true, w->inv_dt, i, w->desc.min_divergence_iter)) break;
+            }
+            if (!(i == 0 && w->fused_first_div)) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts
+            TRY(span_begin(w, SP_DIV_UPD));
+            TRY(launch_vel_update(w, false, akf && i == 0));
+            TRY(span_end(w));
+            w->xs_valid = false;  // v* moved on: XSPH sums of the evaluation above are stale unless another evaluation follows
+            w->stats.n_divergence_iter++;
+        }
+        CU(cudaEventRecord(w->ev[EV_DIV], w->st));
+        TRY(dfsph_fold(w, remaining, g));
+    }
     // pressure_solve :432-464
     w->stats.n_pressure_iter = w->stats.n_pressure_eval = 0;
     maxit = w->force_press >= 0 ? (uint32_t)w->force_press + 1 : w->desc.max_pressure_iter;
-    for (uint32_t i = 0; i < maxit; ++i) {
-        TRY(span_begin(w, SP_PRED));
-        TRY(launch_vel_divergence(w, true, &nblk));
-        TRY(span_end(w));
-        w->stats.n_pressure_eval++;
-        if (w->force_press >= 0) {
-            if ((int)i >= w->force_press) break;
-        } else if (i < w->desc.min_pressure_iter && i + 1 < maxit) {
-            w->errsum_ready = false;  // cannot break yet (:450): skip the read-back, as in the divergence loop
-        } else {
-            float avg;
-            TRY(read_error(w, nblk, &avg));
-            w->stats.last_density_error = avg;
-            if (avg <= w->desc.max_density_error && i >= w->desc.min_pressure_iter) break;
+    if (w->cap) {
+        TRY(graph_pressure_loop(w));
+    } else {
+        for (uint32_t i = 0; i < maxit; ++i) {
+            TRY(span_begin(w, SP_PRED));
+            TRY(launch_vel_divergence(w, true, &nblk));
+            TRY(span_end(w));
+            w->stats.n_pressure_eval++;
+            if (w->force_press >= 0) {
+                if ((int)i >= w->force_press) break;
+            } else if (i < w->desc.min_pressure_iter && i + 1 < maxit) {
+                w->errsum_ready = false;  // cannot break yet (:450): skip the read-back, as in the divergence loop
+            } else {
+                float avg;
+                TRY(read_error(w, nblk, &avg));
+                w->stats.last_density_error = avg;
+                if (loop_exit(avg, w->desc.max_density_error, false, w->inv_dt, i, w->desc.min_pressure_iter)) break;
+            }
+            TRY(refresh_kappa(w));
+            TRY(span_begin(w, SP_PUPD));
+            TRY(launch_vel_update(w, true));
+            TRY(span_end(w));
+            w->stats.n_pressure_iter++;
         }
-        TRY(refresh_kappa(w));
-        TRY(span_begin(w, SP_PUPD));
-        TRY(launch_vel_update(w, true));
-        TRY(span_end(w));
-        w->stats.n_pressure_iter++;
     }
-    CU(cudaEventRecord(w->ev[EV_PRESS], w->st));
+    TRY(ev_record(w, EV_PRESS));
     TRY(slab_wait(w));  // a speculative exchange may still be in flight: it must land before the arrays are reused
     {
         static const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
         CU(w->d_nb.ensure(8));
-        CU(cudaMemcpyAsync(w->d_nb.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
+        if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(w->d_nb.p);
+        else CU(cudaMemcpyAsync(w->d_nb.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
         LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->dt, w->slab.active ? (int*)nullptr : w->d_nb.p);  // :411-420
         w->nb_pending = !w->slab.active;
     }
@@ -1887,6 +1988,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 #include "sph_elasticity_host.inl"
 #include "sph_viscosity_host.inl"
 #include "sph_colliders_host.inl"
+#include "sph_graph.inl"
 
 // ===================================================================================================
 // extern "C" boundary
@@ -2260,8 +2362,30 @@ sph_status sph_world_step(sph_world* w, float dt, const float gravity[3]) {
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "sph_world_step called from inside a coupling callback");
     sph_status s = world_step(w, dt, gravity);
+    w->records.assign(1, step_record(w->stats, 0));
     if (s != SPH_OK) cudaStreamSynchronize(w->st);
     return s;
+}
+
+// n_steps calls of sph_world_step, steps 2..n_steps in a CUDA graph (DESIGN.md section 13)
+sph_status sph_world_step_many(sph_world* w, float dt, const float gravity[3], uint32_t n_steps, uint32_t* steps_done) {
+    if (!w || !gravity || !steps_done) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    *steps_done = 0;
+    if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "sph_world_step_many called from inside a coupling callback");
+    if (const char* why = step_many_refusal(w)) return w->fail(SPH_ERR_INVALID, "%s", why);
+    if (n_steps == 0) return SPH_OK;
+    sph_status s = step_many(w, dt, gravity, n_steps, steps_done);
+    if (s != SPH_OK) cudaStreamSynchronize(w->st);
+    return s;
+}
+
+sph_status sph_world_read_step_records(sph_world* w, sph_step_record* out, size_t cap, size_t* n) {
+    if (!w || !n || (cap && !out)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    *n = w->records.size();
+    if (*n && cap) memcpy(out, w->records.data(), std::min(cap, *n) * sizeof(sph_step_record));
+    return SPH_OK;
 }
 
 // LiquidWorld::step_with_coupling liquid_world.rs:67-158
@@ -2271,6 +2395,7 @@ sph_status sph_world_step_with_coupling(sph_world* w, float dt, const float grav
     if (w->in_coupling) return w->fail(SPH_ERR_INVALID, "sph_world_step_with_coupling called from inside a coupling callback");
     if (coupling && w->slab.active) return w->fail(SPH_ERR_INVALID, "coupling callbacks are not supported in slab-decomposed worlds");
     sph_status s = world_step(w, dt, gravity, coupling);
+    w->records.assign(1, step_record(w->stats, 0));
     w->in_coupling = false;
     if (s != SPH_OK) cudaStreamSynchronize(w->st);
     return s;

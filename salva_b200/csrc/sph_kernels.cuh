@@ -1458,4 +1458,134 @@ __global__ void k_sum_u32(uint32_t n, const uint32_t* __restrict__ a, const uint
     if ((threadIdx.x & 31) == 0 && s) atomicAdd(out, s);
 }
 
+// ------------------------------------------------------------------------------------------------
+// Jacobi-loop exits (dfsph_solver.rs:153-158, :347-352, :450, :486), shared by the host loop of dfsph_step and the device
+// decisions of the step graph (sph_graph.inl), so that both end a loop after the same evaluation.
+// ------------------------------------------------------------------------------------------------
+// The largest per-fluid mean errsum[f] / n[f] over the fluids with n[f] > 0 (n as float, from the particle count); 0 without
+// any, and a NaN mean never wins (the comparison of std::max).
+__host__ __device__ inline float loop_error(const float* errsum, const float* n, int nf) {
+    float mx = 0.f;
+    for (int f = 0; f < nf; ++f)
+        if (n[f] > 0.f) {
+            const float e = errsum[f] / n[f];
+            mx = mx < e ? e : mx;
+        }
+    return mx;
+}
+// Whether the loop breaks after evaluation i with error avg: the divergence bound is max_error * inv_dt * 0.01 (products only, so
+// nothing contracts into an FMA), the density bound max_error itself.
+__host__ __device__ inline bool loop_exit(float avg, float max_error, bool divergence, float inv_dt, uint32_t i, uint32_t min_iter) {
+    const float max_err = divergence ? max_error * inv_dt * 0.01f : max_error;
+    return avg <= max_err && i >= min_iter;
+}
+
+// ---- step graph (sph_world_step_many, sph_graph.inl): device-side control ------------------------------------------------
+// One record per step of a call; the layout of sph_step_record.
+struct StepRec {
+    uint32_t n_div_iter, n_press_iter, n_div_eval, n_press_eval;
+    float last_div_err, last_dens_err;
+    uint32_t max_neighbors, on_device;
+    unsigned long long n_contacts;
+};
+enum { GRAPH_STOP_NONE = 0, GRAPH_STOP_REDO = 1, GRAPH_STOP_LEFT = 2, GRAPH_STOP_ERROR = 3 };
+// What the graph carries from kernel to kernel.  REDO: the step found lists longer than their capacity and stopped after its
+// sort; LEFT: the step's new positions left the grid envelope or are not finite; ERROR: the step raised the error flag.
+struct GraphCtl {
+    uint32_t left;  // steps still to run
+    uint32_t step;  // steps completed (index of the running step's record)
+    uint32_t stop;  // GRAPH_STOP_*
+    uint32_t it;    // iteration of the running Jacobi loop
+};
+// One Jacobi loop as dfsph_step runs it: maxit evaluations at most (force + 1 when force >= 0), the exit rule, the fluid sizes.
+struct LoopRule {
+    uint32_t maxit, min_iter;
+    int32_t force;
+    float max_error, inv_dt;
+    int divergence, nf;
+    float n[MAX_FLUIDS];
+};
+// Conditional handles a decision sets: [0] to "an update follows", [1] to "an update and another evaluation follow",
+// [2] to "an update follows and ends the loop", [3] and [4] to 0 (unused entries are 0 and not set).  k_fold_arm: [s] to
+// "the loop ended in state s".
+struct Decide {
+    cudaGraphConditionalHandle h[8];
+};
+
+__global__ void k_graph_arm(const GraphCtl* ctl, cudaGraphConditionalHandle h) {
+    cudaGraphSetConditional(h, (ctl->stop == GRAPH_STOP_NONE && ctl->left > 0) ? 1u : 0u);
+}
+
+// After evaluation i (i0 >= 0: this i, else the running loop's next) of a loop: the host loop's decision, its counts and error
+// read, and the handles of what follows.  The read is skipped where dfsph_step skips its read-back.
+__global__ void k_loop_decide(GraphCtl* ctl, StepRec* rec, const float* errsum, LoopRule r, int i0, Decide d) {
+    const uint32_t i = i0 >= 0 ? (uint32_t)i0 : ctl->it + 1;
+    ctl->it = i;
+    StepRec& R = rec[ctl->step];
+    (r.divergence ? R.n_div_eval : R.n_press_eval)++;
+    bool brk;
+    if (r.force >= 0) {
+        brk = (int)i >= r.force;
+    } else if (i < r.min_iter && i + 1 < r.maxit) {
+        brk = false;
+    } else {
+        const float avg = loop_error(errsum, r.n, r.nf);
+        (r.divergence ? R.last_div_err : R.last_dens_err) = avg;
+        brk = loop_exit(avg, r.max_error, r.divergence != 0, r.inv_dt, i, r.min_iter);
+    }
+    if (!brk) (r.divergence ? R.n_div_iter : R.n_press_iter)++;
+    const bool more = !brk && i + 1 < r.maxit;
+    const unsigned v[5] = {!brk, more, !brk && !more, 0u, 0u};
+    for (int k = 0; k < 5; ++k)
+        if (d.h[k]) cudaGraphSetConditional(d.h[k], v[k]);
+}
+
+// After the divergence loop: which post-loop branch runs, from the step's counts.  The loop's first update carries the
+// Akinci normals (nr4: an update ran), its evaluation 1 the Akinci force (two evaluations ran); the XSPH sums of an
+// evaluation i >= 1 are valid when the loop ended on that evaluation (one update fewer than evaluations).  h[s] is the
+// branch of state s = xs | nr4 << 1 | akinci << 2.
+__global__ void k_fold_arm(const GraphCtl* ctl, const StepRec* rec, int xsf, int akf, Decide d) {
+    const StepRec& R = rec[ctl->step];
+    const uint32_t xs = xsf && R.n_div_eval >= 2 && R.n_div_iter + 1 == R.n_div_eval;
+    const uint32_t nr4 = akf && R.n_div_iter >= 1, ak = akf && R.n_div_eval >= 2;
+    const uint32_t s = xs | nr4 << 1 | ak << 2;
+    for (uint32_t k = 0; k < 8; ++k)
+        if (d.h[k]) cudaGraphSetConditional(d.h[k], k == s ? 1u : 0u);
+}
+
+// After the neighbour search of a graph step: the list capacity check and error word of phase_neighbors' read-back.  A list
+// longer than its capacity (or a boundary-volume error) stops the graph before the solver; the host redoes the step.
+__global__ void k_lists_check(GraphCtl* ctl, StepRec* rec, const int* scal, uint32_t cap_f, uint32_t cap_b, cudaGraphConditionalHandle h) {
+    const int err = scal[7];
+    const uint32_t mf = (uint32_t)scal[8], mb = (uint32_t)scal[9];
+    const bool ok = !(err & ~ERR_SEARCH_ZERO_DENSITY) && mf <= cap_f && mb <= cap_b;
+    rec[ctl->step].max_neighbors = mf;
+    if (!ok) ctl->stop = GRAPH_STOP_REDO;
+    cudaGraphSetConditional(h, ok ? 1u : 0u);
+}
+
+// Initial value of k_update_positions' bounds
+__global__ void k_bounds_init(int* b) {
+    const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+    for (int a = 0; a < 7; ++a) b[a] = init[a];
+}
+
+// End of a graph step: the record's contacts, the count, and the stops of world_substep's read-back: the error flag, and new
+// positions outside the envelope env (cell coordinates lo xyz, hi xyz) or not finite.
+struct Envelope {
+    int lo[3], hi[3];
+};
+__global__ void k_step_end(GraphCtl* ctl, StepRec* rec, const int* scal, const unsigned long long* cnt, const int* nb, Envelope env,
+                           unsigned long long bb_contacts) {
+    StepRec& R = rec[ctl->step];
+    R.on_device = 1;
+    R.n_contacts = bb_contacts + cnt[1];
+    bool inside = nb[6] == 0;
+    for (int a = 0; a < 3; ++a) inside = inside && nb[a] >= env.lo[a] && nb[3 + a] <= env.hi[a];
+    if (scal[7]) ctl->stop = GRAPH_STOP_ERROR;
+    else if (!inside) ctl->stop = GRAPH_STOP_LEFT;
+    ctl->step++;
+    ctl->left--;
+}
+
 }  // namespace sphk

@@ -571,6 +571,27 @@ class LiquidWorld:
         g = np.asarray(gravity, np.float32)
         self._ck(self._L.sph_world_step(self._w, dt, _fp(g)))
 
+    def step_many(self, dt, n_steps, gravity=(0.0, -9.81, 0.0)):
+        """n_steps calls of step(dt, gravity), steps 2..n_steps as one CUDA graph (include/sph.h sph_world_step_many).
+        Returns the number of steps done; raises SphError as step does, with the steps done before the failing one in its
+        steps_done attribute."""
+        g = np.asarray(gravity, np.float32)
+        done = C.c_uint32()
+        st = self._L.sph_world_step_many(self._w, dt, _fp(g), n_steps, C.byref(done))
+        if st != 0:
+            e = SphError(st, self._L.sph_last_error(self._w).decode())
+            e.steps_done = done.value
+            raise e
+        return done.value
+
+    def step_records(self):
+        """One dict per step of the last step / step_many call (include/sph.h sph_step_record)."""
+        n = C.c_size_t()
+        self._ck(self._L.sph_world_read_step_records(self._w, None, 0, C.byref(n)))
+        out = (_lib.StepRecord * max(n.value, 1))()
+        self._ck(self._L.sph_world_read_step_records(self._w, out, n.value, C.byref(n)))
+        return [{f: getattr(out[i], f) for f, _ in _lib.StepRecord._fields_} for i in range(n.value)]
+
     def set_substepping(self, cfl_coeff=0.4, min_substeps=1, max_substeps=10):
         """CFL-bounded substeps inside each step (include/sph.h sph_world_set_substepping); the defaults are the reference
         TimestepManager's (timestep_manager.rs:21-31).  cfl_coeff=0 turns substepping off."""
