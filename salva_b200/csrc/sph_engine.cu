@@ -471,8 +471,6 @@ struct sph_world {
     bool unimass = false;
     DBuf<float4> pvx4, pk4;
     DBuf<float2> vyz2;
-    bool nr4_valid = false;     // Akinci normals nr4 = (n, rho) rode with the divergence loop's first update (k_vel_update_u<.., NORMALS>)
-    bool akinci_valid = false;  // ... and the Akinci fluid force with the evaluation after it (k_vel_divergence_xsph_u<2>), in xs
     Tex tex_pvx, tex_vyz, tex_pk;
     DBuf<float> he_colors, he_gradc;  // He2014 colours / squared colour-gradient norms (he2014_surface_tension.rs:16-17)
     DBuf<uint32_t> q_out, q_count;     // particles_intersecting_aabb results
@@ -484,9 +482,7 @@ struct sph_world {
     DBuf<float> ct_w[2], ct_g[2];
     DBuf<uint32_t> d_ticket;      // last-block ticket of the in-kernel error reduction (kept at 0 between launches)
     bool errsum_ready = false;    // the last evaluation launch already reduced its partials into errsum
-    bool fused_first_div = false;  // the neighbour search computed rho, alpha and the first compute_divergences evaluation
-    bool xs_valid = false;    // XSPH sums rode with the divergence loop's last evaluation (k_vel_divergence_xsph_u)
-    DBuf<float4> xs;
+    DBuf<float4> xs;  // the XSPH sums or the Akinci fluid force of a divergence evaluation (fold_state)
     uint32_t fused_nblk = 0;
     Tex tex_vs;  // the general evaluations gather v* through the texture pipe
     DBuf<float> partial, errsum;
@@ -1097,13 +1093,13 @@ sph_status density_args(sph_world* w, DensArgs* D) {
 // `speculative` (optional) enqueues the work that follows the neighbour search and only writes scratch (the density
 // pass): it is launched BEFORE the host learns whether the lists overflowed, so the GPU is busy during that round trip;
 // on overflow the lists are rebuilt with a larger capacity and the speculative work is simply enqueued again.
-// With w->fused_first_div (DFSPH) the search itself computes rho, alpha and the first divergence evaluation
-// (density_alpha_div); on overflow the relaunched search computes them again.
+// With DFSPH the search itself computes rho, alpha and the first divergence evaluation (density_alpha_div); on overflow the
+// relaunched search computes them again.
 sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) = nullptr) {
     size_t N = w->N, B = w->B;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
-    const bool dens = w->fused_first_div, uni = dens && w->unimass;
+    const bool dens = N && w->desc.solver == SPH_SOLVER_DFSPH, uni = dens && w->unimass;
     DensArgs D{};
     if (dens) TRY(density_args(w, &D));
     using NbrKernel = void (*)(const float4*, const float4*, const uint32_t*, const float4*, const float4*, const uint32_t*, uint32_t*,
@@ -1194,6 +1190,23 @@ std::array<float, MAX_FLUIDS> loop_sizes(const sph_world* w) {
     return n;
 }
 
+// dfsph_step's loop bounds and exit rule for the divergence (true) or the pressure loop
+LoopRule loop_rule(const sph_world* w, bool divergence) {
+    LoopRule r;
+    memset(&r, 0, sizeof r);
+    const int force = divergence ? w->force_div : w->force_press;
+    r.force = force;
+    r.maxit = force >= 0 ? (uint32_t)force + 1 : (divergence ? w->desc.max_divergence_iter : w->desc.max_pressure_iter);
+    r.min_iter = divergence ? w->desc.min_divergence_iter : w->desc.min_pressure_iter;
+    r.max_error = divergence ? w->desc.max_divergence_error : w->desc.max_density_error;
+    r.inv_dt = w->inv_dt;
+    r.divergence = divergence;
+    r.nf = (int)w->fluids.size();
+    const std::array<float, MAX_FLUIDS> n = loop_sizes(w);
+    memcpy(r.n, n.data(), sizeof r.n);
+    return r;
+}
+
 // mean-per-fluid -> max over fluids (dfsph_solver.rs:153-158, :347-352)
 sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     int nf = (int)w->fluids.size();
@@ -1207,6 +1220,17 @@ sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     CU(cudaStreamSynchronize(w->st));
     *out = loop_error(w->h_pinned, loop_sizes(w).data(), nf);
     return SPH_OK;
+}
+
+// A host loop's decision after evaluation i: loop_decision, with read_error (of nblk partials) into *err where it reads
+sph_status host_decision(sph_world* w, const LoopRule& r, uint32_t i, uint32_t nblk, float* err, LoopDecision* d) {
+    sph_status s = SPH_OK;
+    *d = loop_decision(r, i, [&] {
+        s = read_error(w, nblk, err);
+        return *err;
+    });
+    w->errsum_ready = false;  // read, or not needed: the next read follows an evaluation that sets it
+    return s;
 }
 
 bool any_bforce(const sph_world* w) {
@@ -1264,7 +1288,7 @@ sph_status launch_density_alpha(sph_world* w) {
 // leave its neighbours waiting in a collective they entered once and it enters twice.
 sph_status post_density_refresh(sph_world* w) {
     if (!w->slab.active || !w->N) return SPH_OK;
-    if (w->fused_first_div) {
+    if (w->desc.solver == SPH_SOLVER_DFSPH) {
         SlabArray a[2] = {{w->dens.p, sizeof(float)}, {w->unimass ? (void*)w->pk4.p : (void*)w->kappa.p, w->unimass ? sizeof(float4) : sizeof(float)}};
         return slab_refresh_n(w, a, 2);
     }
@@ -1362,11 +1386,11 @@ AkinciNorms akinci_norms(float h) {
     return {32.0f / (3.14159265358979323846f * powf(h, 9.f)), powf(h, 6.f) / 64.0f, 0.007f / powf(h, 3.25f)};
 }
 
-sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
+// akinci: the Akinci fluid force rides along (evaluation 1 of the divergence loop, on the normals update 0 wrote).
+sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, bool akinci = false) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
-    const bool xsf = !predict && xsph_fusable(w);
-    const bool akf = !predict && w->nr4_valid && !w->akinci_valid;  // the first evaluation after the normals-carrying update
+    const bool xsf = !predict && xsph_fusable(w), akf = !predict && akinci;
     if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) {
@@ -1390,12 +1414,10 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk) {
                 const float cf = w->fluids[0].forces[0].d.p[0];
                 LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
                          w->pk4.p, partial, tk, w->errsum.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
-                w->xs_valid = true;
             } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
                 const AkinciNorms an = akinci_norms(w->h);
                 LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
                          w->pk4.p, partial, tk, w->errsum.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
-                w->akinci_valid = true;
             } else {
                 LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
                          w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
@@ -1416,10 +1438,7 @@ sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) 
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
     Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
     if (w->unimass) CU(w->tex_pk.bind(w->pk4));
-    if (normals) {
-        CU(w->normals.ensure(std::max(w->Ntot, w->N)));
-        w->nr4_valid = true;
-    }
+    if (normals) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
     // the following evaluation gathers v*_j of ghosts (vs itself too: the velocity fold reads vel = v* for ghosts)
     SlabArray a[3] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}, {w->vs.p, sizeof(float4)}};
     SlabArray a1[1] = {{w->vs.p, sizeof(float4)}};
@@ -1547,8 +1566,9 @@ sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<
     return SPH_OK;
 }
 
-// predict_advection dfsph_solver.rs:580-603: every fluid's forces in push order
-sph_status phase_forces(sph_world* w) {
+// predict_advection dfsph_solver.rs:580-603: every fluid's forces in push order, less what the divergence loop computed
+// (fold: fold_state)
+sph_status phase_forces(sph_world* w, uint32_t fold) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
@@ -1558,7 +1578,7 @@ sph_status phase_forces(sph_world* w) {
             const float* p = fr.d.p;
             switch (fr.d.kind) {
                 case SPH_FORCE_XSPH_VISCOSITY:
-                    if (w->xs_valid && f == 0 && &fr == &w->fluids[0].forces[0]) break;  // already folded in by k_fold_velocities
+                    if ((fold & FOLD_XS) && f == 0 && &fr == &w->fluids[0].forces[0]) break;  // already folded in by k_fold_velocities
                     DISPATCH2(k_force_xsph, multi, bf, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p, w->acc.p,
                               w->bforce.p, (uint32_t)f, p[0], p[1], w->inv_dt);
                     break;
@@ -1567,11 +1587,11 @@ sph_status phase_forces(sph_world* w) {
                               w->bforce.p, (uint32_t)f, p[0], p[1], p[2], p[3], p[4]);
                     break;
                 case SPH_FORCE_AKINCI2013_TENSION: {
-                    if (w->akinci_valid && &fr == &w->fluids[0].forces[0]) break;  // in xs, folded in by the fold pass
+                    if ((fold & FOLD_AKINCI) && &fr == &w->fluids[0].forces[0]) break;  // in xs, folded in by the fold pass
                     CU(w->normals.ensure(std::max(w->Ntot, w->N)));
                     const AkinciNorms an = akinci_norms(w->h);
                     const float coh_norm = an.coh_norm, h6_64 = an.h6_64, adh_norm = an.adh_norm;
-                    if (w->nr4_valid && f == 0) {  // normals (and rho, in .w) came with the first divergence update
+                    if ((fold & FOLD_NR4) && f == 0) {  // normals (and rho, in .w) came with the first divergence update
                         CU(w->tex_pvx.bind(w->pvx4));
                         if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
                         else LAUNCH((k_akinci_force_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
@@ -1676,16 +1696,16 @@ sph_status timestep_advance(sph_world* w, float remaining) {
 }
 
 // update_velocities :422-430, zero vc :689-691, acc += gravity :574-578, the non-pressure forces and the integration, after the
-// divergence loop ended in the state of xs_valid, nr4_valid and akinci_valid
-sph_status dfsph_fold(sph_world* w, float remaining, const float g[3]) {
+// divergence loop ended in fold state `fold` (fold_state)
+sph_status dfsph_fold(sph_world* w, float remaining, const float g[3], uint32_t fold) {
     size_t N = w->N;
     int c = w->cur;
     TRY(slab_wait(w));
     // the first force of fluid 0 may already sit in xs: the XSPH sums of the loop's last evaluation (acc = g + xs * inv_dt) or
     // the Akinci fluid force (acc = g + xs; a scale of 1 leaves the product exact)
-    const bool folded = w->xs_valid || w->akinci_valid;
+    const bool folded = fold & (FOLD_XS | FOLD_AKINCI);
     const float4* xs = folded ? w->xs.p : nullptr;
-    const float xs_scale = w->akinci_valid ? 1.0f : w->inv_dt;
+    const float xs_scale = (fold & FOLD_AKINCI) ? 1.0f : w->inv_dt;
     // nothing (else) to launch in the force phase?  Then fold, acceleration and integration are one streaming pass, unless
     // substepping needs the CFL reduction between the fold and the integration, which takes the new dt
     bool quiet_forces = true;
@@ -1701,7 +1721,7 @@ sph_status dfsph_fold(sph_world* w, float remaining, const float g[3]) {
     } else {
         LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale);  // ghosts too (vel = v*)
         TRY(ev_record(w, EV_FOLD));
-        if (!quiet_forces) TRY(phase_forces(w));
+        if (!quiet_forces) TRY(phase_forces(w, fold));
         TRY(ev_record(w, EV_FORCES));
         TRY(launch_cfl_max(w, w->vel[c].p, remaining));
         TRY(timestep_advance(w, remaining));  // :702
@@ -1712,82 +1732,135 @@ sph_status dfsph_fold(sph_world* w, float remaining, const float g[3]) {
     return ev_record(w, EV_INTEG);
 }
 
-// The Jacobi loops of a step graph (sph_graph.inl): the same launches, ended on the device
-sph_status graph_divergence_loop(sph_world* w, float remaining, const float g[3]);
-sph_status graph_pressure_loop(sph_world* w);
+// A condition of dfsph_step's loops: out of capture a host bool that decide() sets, in capture a conditional handle
+struct Cond {
+    bool v = false;
+    cudaGraphConditionalHandle h = 0;
+};
+template <class Fn>
+sph_status cap_cond(sph_world* w, cudaGraphConditionalHandle h, cudaGraphConditionalNodeType type, Fn body);  // sph_graph.inl
+sph_status new_handle(sph_world* w, cudaGraphConditionalHandle* h);
 
-// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k
+sph_status cond_new(sph_world* w, Cond* c) { return w->cap ? new_handle(w, &c->h) : SPH_OK; }
+
+// IF (cudaGraphCondTypeIf) or WHILE c { body }: plain control flow out of capture, a conditional node in capture
+template <class Fn>
+sph_status cond(sph_world* w, const Cond& c, cudaGraphConditionalNodeType type, Fn body) {
+    if (w->cap) return cap_cond(w, c.h, type, body);
+    if (type == cudaGraphCondTypeIf) return c.v ? body() : SPH_OK;
+    while (c.v) TRY(body());
+    return SPH_OK;
+}
+
+// The decision after evaluation i of loop r (i < 0: the evaluation after the last decided one), from nblk error partials.
+// It sets c[0] to "an update follows", c[1] to "an update and another evaluation follow", c[2] to "an update follows and
+// ends the loop", c[3] and c[4] to false (a graph's handles keep their values from the last step); null entries are not
+// set.  Out of capture it is host_decision with the step's counts; in capture k_loop_decide, behind read_error's reduction
+// of the search's partials where evaluation 0 is read.
+sph_status decide(sph_world* w, const LoopRule& r, int i, uint32_t nblk, std::array<Cond*, 5> c) {
+    if (w->cap) {
+        if (!w->errsum_ready && i >= 0 && loop_decision(r, (uint32_t)i, [] { return 0.f; }).read) {
+            const int nf = (int)w->fluids.size();
+            k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
+        }
+        w->errsum_ready = false;
+        Decide d{};
+        for (int k = 0; k < 5; ++k)
+            if (c[k]) d.h[k] = c[k]->h;
+        k_loop_decide<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->errsum.p, r, i, d);
+        CU(cudaGetLastError());
+        return SPH_OK;
+    }
+    sph_step_stats& S = w->stats;
+    LoopDecision d;
+    TRY(host_decision(w, r, (r.divergence ? S.n_divergence_eval : S.n_pressure_eval)++, nblk,
+                      r.divergence ? &S.last_divergence_error : &S.last_density_error, &d));
+    if (!d.brk) (r.divergence ? S.n_divergence_iter : S.n_pressure_iter)++;
+    const bool v[5] = {!d.brk, d.more, !d.brk && !d.more, false, false};
+    for (int k = 0; k < 5; ++k)
+        if (c[k]) c[k]->v = v[k];
+    return SPH_OK;
+}
+
+// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k.  sph_world_step and the step graph
+// (sph_graph.inl) run these same loops: out of capture their conditions are host bools, in capture conditional nodes.
 sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
     size_t N = w->N;
     int c = w->cur;
-    uint32_t nblk = 0;
-    // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step)
+    // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step), unrolled where its passes depend on
+    // the iteration: evaluation 0 (the neighbour search's), update 0 (with the Akinci normals), evaluation 1 (with the XSPH
+    // sums or the Akinci force), then a uniform WHILE body and the update that ends a loop running out of iterations
     w->stats.n_divergence_iter = w->stats.n_divergence_eval = 0;
-    w->xs_valid = false;
-    w->nr4_valid = w->akinci_valid = false;
-    const bool akf = akinci_fusable_u(w);
-    uint32_t maxit = w->force_div >= 0 ? (uint32_t)w->force_div + 1 : w->desc.max_divergence_iter;
-    if (w->cap) {
-        TRY(graph_divergence_loop(w, remaining, g));  // with the post-loop fold of every way the loop can end
-    } else {
-        for (uint32_t i = 0; i < maxit; ++i) {
-            if (i == 0 && w->fused_first_div) {
-                nblk = w->fused_nblk;  // evaluation 0 was computed by the neighbour search
-            } else {
-                TRY(span_begin(w, SP_DIV_EVAL));
-                TRY(launch_vel_divergence(w, false, &nblk));
-                TRY(span_end(w));
-            }
-            w->stats.n_divergence_eval++;
-            if (w->force_div >= 0) {
-                if ((int)i >= w->force_div) break;
-            } else if (i < w->desc.min_divergence_iter && i + 1 < maxit) {
-                // the break needs `i >= min_iter` (:486): this evaluation's error cannot end the loop and the next
-                // evaluation reports a fresher one, so neither the read-back (a host sync) nor the allreduce is needed
-                w->errsum_ready = false;
-            } else {
-                float avg;
-                TRY(read_error(w, nblk, &avg));
-                w->stats.last_divergence_error = avg;
-                if (loop_exit(avg, w->desc.max_divergence_error, true, w->inv_dt, i, w->desc.min_divergence_iter)) break;
-            }
-            if (!(i == 0 && w->fused_first_div)) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts
-            TRY(span_begin(w, SP_DIV_UPD));
-            TRY(launch_vel_update(w, false, akf && i == 0));
-            TRY(span_end(w));
-            w->xs_valid = false;  // v* moved on: XSPH sums of the evaluation above are stale unless another evaluation follows
-            w->stats.n_divergence_iter++;
-        }
-        CU(cudaEventRecord(w->ev[EV_DIV], w->st));
-        TRY(dfsph_fold(w, remaining, g));
+    const bool akf = akinci_fusable_u(w), xsf = xsph_fusable(w);
+    const LoopRule rd = loop_rule(w, true);
+    uint32_t nblk = w->fused_nblk;
+    auto div_update = [&](bool first) -> sph_status {
+        if (!first) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts (post_density_refresh sent evaluation 0's)
+        TRY(span_begin(w, SP_DIV_UPD));
+        TRY(launch_vel_update(w, false, first && akf));
+        return span_end(w);
+    };
+    auto div_eval = [&](bool first) -> sph_status {
+        TRY(span_begin(w, SP_DIV_EVAL));
+        TRY(launch_vel_divergence(w, false, &nblk, first && akf));
+        return span_end(w);
+    };
+    if (rd.maxit > 0) {  // max_divergence_iter 0: no pass at all
+        Cond upd0, eval1, more, tail;
+        for (Cond* x : {&upd0, &eval1, &more, &tail}) TRY(cond_new(w, x));
+        TRY(decide(w, rd, 0, nblk, {&upd0, &eval1, nullptr, &more, &tail}));
+        TRY(cond(w, upd0, cudaGraphCondTypeIf, [&] { return div_update(true); }));
+        TRY(cond(w, eval1, cudaGraphCondTypeIf, [&] {
+            TRY(div_eval(true));
+            return decide(w, rd, 1, nblk, {nullptr, &more, &tail});
+        }));
+        TRY(cond(w, more, cudaGraphCondTypeWhile, [&] {
+            TRY(div_update(false));
+            TRY(div_eval(false));
+            return decide(w, rd, -1, nblk, {nullptr, &more, &tail});
+        }));
+        TRY(cond(w, tail, cudaGraphCondTypeIf, [&] { return div_update(false); }));
     }
-    // pressure_solve :432-464
-    w->stats.n_pressure_iter = w->stats.n_pressure_eval = 0;
-    maxit = w->force_press >= 0 ? (uint32_t)w->force_press + 1 : w->desc.max_pressure_iter;
-    if (w->cap) {
-        TRY(graph_pressure_loop(w));
+    TRY(ev_record(w, EV_DIV));
+    // the fold in the state the loop ended in: from the host's counts, or in capture one branch per state it can end in
+    if (!w->cap || !(xsf || akf) || rd.maxit == 0) {
+        TRY(dfsph_fold(w, remaining, g, fold_state(xsf, akf, w->stats.n_divergence_eval, w->stats.n_divergence_iter)));
     } else {
-        for (uint32_t i = 0; i < maxit; ++i) {
-            TRY(span_begin(w, SP_PRED));
-            TRY(launch_vel_divergence(w, true, &nblk));
-            TRY(span_end(w));
-            w->stats.n_pressure_eval++;
-            if (w->force_press >= 0) {
-                if ((int)i >= w->force_press) break;
-            } else if (i < w->desc.min_pressure_iter && i + 1 < maxit) {
-                w->errsum_ready = false;  // cannot break yet (:450): skip the read-back, as in the divergence loop
-            } else {
-                float avg;
-                TRY(read_error(w, nblk, &avg));
-                w->stats.last_density_error = avg;
-                if (loop_exit(avg, w->desc.max_density_error, false, w->inv_dt, i, w->desc.min_pressure_iter)) break;
-            }
-            TRY(refresh_kappa(w));
-            TRY(span_begin(w, SP_PUPD));
-            TRY(launch_vel_update(w, true));
-            TRY(span_end(w));
-            w->stats.n_pressure_iter++;
-        }
+        const uint32_t states[3] = {0u, xsf ? FOLD_XS : FOLD_NR4, FOLD_NR4 | FOLD_AKINCI};
+        const int n_states = xsf ? 2 : 3;
+        Decide d{};
+        for (int k = 0; k < n_states; ++k) TRY(new_handle(w, &d.h[states[k]]));
+        k_fold_arm<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, xsf, akf, d);
+        for (int k = 0; k < n_states; ++k)
+            TRY(cap_cond(w, d.h[states[k]], cudaGraphCondTypeIf, [&] { return dfsph_fold(w, remaining, g, states[k]); }));
+    }
+    // pressure_solve :432-464 (with the new inv_dt): evaluation 0, a uniform WHILE body, and the update that ends a loop
+    // running out of iterations
+    w->stats.n_pressure_iter = w->stats.n_pressure_eval = 0;
+    const LoopRule rp = loop_rule(w, false);
+    auto press_update = [&]() -> sph_status {
+        TRY(refresh_kappa(w));
+        TRY(span_begin(w, SP_PUPD));
+        TRY(launch_vel_update(w, true));
+        return span_end(w);
+    };
+    auto press_eval = [&]() -> sph_status {
+        TRY(span_begin(w, SP_PRED));
+        TRY(launch_vel_divergence(w, true, &nblk));
+        return span_end(w);
+    };
+    if (rp.maxit > 0) {  // max_pressure_iter 0: no pressure pass at all
+        Cond more, tail;
+        TRY(cond_new(w, &more));
+        TRY(cond_new(w, &tail));
+        TRY(press_eval());
+        TRY(decide(w, rp, 0, nblk, {nullptr, &more, &tail}));
+        TRY(cond(w, more, cudaGraphCondTypeWhile, [&] {
+            TRY(press_update());
+            TRY(press_eval());
+            return decide(w, rp, -1, nblk, {nullptr, &more, &tail});
+        }));
+        TRY(cond(w, tail, cudaGraphCondTypeIf, press_update));
     }
     TRY(ev_record(w, EV_PRESS));
     TRY(slab_wait(w));  // a speculative exchange may still be in flight: it must land before the arrays are reused
@@ -1858,9 +1931,8 @@ sph_status world_substep(sph_world* w, float remaining, const float g[3], const 
     // evaluate_kernels + compute_densities (liquid_world.rs:123-134) + compute_alphas (dfsph_solver.rs:679-684).  DFSPH:
     // computed by the neighbour search itself, together with the first divergence evaluation; otherwise enqueued
     // speculatively by the neighbour phase (EV_NBR is recorded there, between the two)
-    w->fused_first_div = w->N && w->desc.solver == SPH_SOLVER_DFSPH;
     TRY(phase_neighbors(w, [](sph_world* w) -> sph_status {
-        if (w->N && !w->fused_first_div) TRY(launch_density_alpha(w));
+        if (w->N && w->desc.solver != SPH_SOLVER_DFSPH) TRY(launch_density_alpha(w));
         return SPH_OK;
     }));
     CU(cudaEventRecord(w->ev[EV_DENS], w->st));

@@ -1459,8 +1459,8 @@ __global__ void k_sum_u32(uint32_t n, const uint32_t* __restrict__ a, const uint
 }
 
 // ------------------------------------------------------------------------------------------------
-// Jacobi-loop exits (dfsph_solver.rs:153-158, :347-352, :450, :486), shared by the host loop of dfsph_step and the device
-// decisions of the step graph (sph_graph.inl), so that both end a loop after the same evaluation.
+// Jacobi-loop exits (dfsph_solver.rs:153-158, :347-352, :450, :486), shared by the host loops and the device decisions of
+// the step graph (sph_graph.inl), so that both end a loop after the same evaluation.
 // ------------------------------------------------------------------------------------------------
 // The largest per-fluid mean errsum[f] / n[f] over the fluids with n[f] > 0 (n as float, from the particle count); 0 without
 // any, and a NaN mean never wins (the comparison of std::max).
@@ -1478,6 +1478,40 @@ __host__ __device__ inline float loop_error(const float* errsum, const float* n,
 __host__ __device__ inline bool loop_exit(float avg, float max_error, bool divergence, float inv_dt, uint32_t i, uint32_t min_iter) {
     const float max_err = divergence ? max_error * inv_dt * 0.01f : max_error;
     return avg <= max_err && i >= min_iter;
+}
+// One Jacobi loop: maxit evaluations at most (DFSPH: force + 1 when force >= 0), the exit rule, the fluid sizes.
+struct LoopRule {
+    uint32_t maxit, min_iter;
+    int32_t force;
+    float max_error, inv_dt;
+    int divergence, nf;
+    float n[MAX_FLUIDS];
+};
+// The decision after evaluation i of loop r: whether its error is read (error() is called then and only then), whether the
+// loop breaks, and whether another evaluation follows.  A pinned count (force >= 0) reads nothing and breaks at i == force.
+// The break needs i >= min_iter (dfsph_solver.rs:450, :486), so an earlier evaluation that is not the last cannot end the
+// loop and the next one reports a fresher error: it reads nothing, which spares the host a read-back.
+struct LoopDecision {
+    bool read, brk, more;
+};
+#pragma nv_exec_check_disable  // error() is a host lambda on the host (read_error) and a device lambda in k_loop_decide
+template <class Error>
+__host__ __device__ inline LoopDecision loop_decision(const LoopRule& r, uint32_t i, Error error) {
+    LoopDecision d;
+    d.read = r.force < 0 && !(i < r.min_iter && i + 1 < r.maxit);
+    d.brk = r.force >= 0 ? (int)i >= r.force : d.read && loop_exit(error(), r.max_error, r.divergence != 0, r.inv_dt, i, r.min_iter);
+    d.more = !d.brk && i + 1 < r.maxit;
+    return d;
+}
+
+// Which fused sums are valid when the divergence loop ends, from its counts (xsf: xsph_fusable, akf: akinci_fusable_u).  The
+// loop's update 0 carries the Akinci normals (an update ran), its evaluation 1 the Akinci force (two evaluations ran); the
+// XSPH sums of an evaluation i >= 1 are valid when the loop ended on that evaluation (one update fewer than evaluations).
+enum : uint32_t { FOLD_XS = 1, FOLD_NR4 = 2, FOLD_AKINCI = 4 };
+__host__ __device__ inline uint32_t fold_state(bool xsf, bool akf, uint32_t n_eval, uint32_t n_iter) {
+    const uint32_t xs = xsf && n_eval >= 2 && n_iter + 1 == n_eval;
+    const uint32_t nr4 = akf && n_iter >= 1, ak = akf && n_eval >= 2;
+    return xs * FOLD_XS | nr4 * FOLD_NR4 | ak * FOLD_AKINCI;
 }
 
 // ---- step graph (sph_world_step_many, sph_graph.inl): device-side control ------------------------------------------------
@@ -1497,14 +1531,6 @@ struct GraphCtl {
     uint32_t stop;  // GRAPH_STOP_*
     uint32_t it;    // iteration of the running Jacobi loop
 };
-// One Jacobi loop as dfsph_step runs it: maxit evaluations at most (force + 1 when force >= 0), the exit rule, the fluid sizes.
-struct LoopRule {
-    uint32_t maxit, min_iter;
-    int32_t force;
-    float max_error, inv_dt;
-    int divergence, nf;
-    float n[MAX_FLUIDS];
-};
 // Conditional handles a decision sets: [0] to "an update follows", [1] to "an update and another evaluation follow",
 // [2] to "an update follows and ends the loop", [3] and [4] to 0 (unused entries are 0 and not set).  k_fold_arm: [s] to
 // "the loop ended in state s".
@@ -1516,39 +1542,28 @@ __global__ void k_graph_arm(const GraphCtl* ctl, cudaGraphConditionalHandle h) {
     cudaGraphSetConditional(h, (ctl->stop == GRAPH_STOP_NONE && ctl->left > 0) ? 1u : 0u);
 }
 
-// After evaluation i (i0 >= 0: this i, else the running loop's next) of a loop: the host loop's decision, its counts and error
-// read, and the handles of what follows.  The read is skipped where dfsph_step skips its read-back.
+// After evaluation i (i0 >= 0: this i, else the running loop's next) of a loop: loop_decision with its counts and error
+// read, and the handles of what follows.
 __global__ void k_loop_decide(GraphCtl* ctl, StepRec* rec, const float* errsum, LoopRule r, int i0, Decide d) {
     const uint32_t i = i0 >= 0 ? (uint32_t)i0 : ctl->it + 1;
     ctl->it = i;
     StepRec& R = rec[ctl->step];
     (r.divergence ? R.n_div_eval : R.n_press_eval)++;
-    bool brk;
-    if (r.force >= 0) {
-        brk = (int)i >= r.force;
-    } else if (i < r.min_iter && i + 1 < r.maxit) {
-        brk = false;
-    } else {
+    const LoopDecision x = loop_decision(r, i, [&] {
         const float avg = loop_error(errsum, r.n, r.nf);
         (r.divergence ? R.last_div_err : R.last_dens_err) = avg;
-        brk = loop_exit(avg, r.max_error, r.divergence != 0, r.inv_dt, i, r.min_iter);
-    }
-    if (!brk) (r.divergence ? R.n_div_iter : R.n_press_iter)++;
-    const bool more = !brk && i + 1 < r.maxit;
-    const unsigned v[5] = {!brk, more, !brk && !more, 0u, 0u};
+        return avg;
+    });
+    if (!x.brk) (r.divergence ? R.n_div_iter : R.n_press_iter)++;
+    const unsigned v[5] = {!x.brk, x.more, !x.brk && !x.more, 0u, 0u};
     for (int k = 0; k < 5; ++k)
         if (d.h[k]) cudaGraphSetConditional(d.h[k], v[k]);
 }
 
-// After the divergence loop: which post-loop branch runs, from the step's counts.  The loop's first update carries the
-// Akinci normals (nr4: an update ran), its evaluation 1 the Akinci force (two evaluations ran); the XSPH sums of an
-// evaluation i >= 1 are valid when the loop ended on that evaluation (one update fewer than evaluations).  h[s] is the
-// branch of state s = xs | nr4 << 1 | akinci << 2.
+// After the divergence loop: h[s] is the post-loop branch of fold state s, set from the step's counts
 __global__ void k_fold_arm(const GraphCtl* ctl, const StepRec* rec, int xsf, int akf, Decide d) {
     const StepRec& R = rec[ctl->step];
-    const uint32_t xs = xsf && R.n_div_eval >= 2 && R.n_div_iter + 1 == R.n_div_eval;
-    const uint32_t nr4 = akf && R.n_div_iter >= 1, ak = akf && R.n_div_eval >= 2;
-    const uint32_t s = xs | nr4 << 1 | ak << 2;
+    const uint32_t s = fold_state(xsf, akf, R.n_div_eval, R.n_div_iter);
     for (uint32_t k = 0; k < 8; ++k)
         if (d.h[k]) cudaGraphSetConditional(d.h[k], k == s ? 1u : 0u);
 }
