@@ -395,6 +395,30 @@ public:
         pull_results();
         return done;
     }
+    // Particle sinks and sources applied on the device at the start of every step (sph_fluid_add_sink / sph_fluid_add_source,
+    // DESIGN.md section 14): what faucet3.rs:69-105 does with delete_particle_at_next_timestep and add_particles before each
+    // step, without reading the fluid.  A sink removes the fluid's particles in [lo, hi) (outside: those not in it); a source
+    // appends its template on the first step and every interval-th step after it.  Both return a handle.
+    uint32_t add_particle_sink(FluidHandle fluid, const Vector3& lo, const Vector3& hi, bool outside = false) {
+        const sph_sink_desc d{{lo.x, lo.y, lo.z}, {hi.x, hi.y, hi.z}, outside ? 1 : 0};
+        uint32_t h = 0;
+        check(sph_fluid_add_sink(raw_, fluids_.at(fluid).handle_, &d, &h));
+        return h;
+    }
+    uint32_t add_particle_source(FluidHandle fluid, const std::vector<Point3>& pos, const std::vector<Vector3>* vel = nullptr, uint32_t interval = 1) {
+        if (vel && vel->size() != pos.size()) throw std::invalid_argument("source positions / velocities differ in length");
+        uint32_t h = 0;
+        check(sph_fluid_add_source(raw_, fluids_.at(fluid).handle_, fp(pos), vel ? fp(*vel) : nullptr, pos.size(), interval, &h));
+        return h;
+    }
+    void remove_particle_sink(uint32_t sink) { check(sph_sink_remove(raw_, sink)); }
+    void remove_particle_source(uint32_t source) { check(sph_source_remove(raw_, source)); }
+    // (removed, emitted): the fluid's particles that the last step's sinks removed and its sources emitted
+    std::pair<uint32_t, uint32_t> step_edits(FluidHandle fluid) {
+        uint32_t r = 0, e = 0;
+        check(sph_fluid_read_step_edits(raw_, fluids_.at(fluid).handle_, &r, &e));
+        return {r, e};
+    }
     // liquid_world.rs:67-158
     void step_with_coupling(Real dt, const Vector3& gravity, CouplingManager* coupling) {
         push_host_edits();

@@ -431,6 +431,43 @@ sph_status sph_collider_set_state(sph_world* w, uint32_t collider, const sph_col
 sph_status sph_collider_read_impulse(sph_world* w, uint32_t collider, float linear[3], float angular[3]);
 /* ColliderCouplingSet::unregister_coupling fluids_pipeline.rs:119-122: the boundary stays, with its last particle set. */
 sph_status sph_collider_unregister(sph_world* w, uint32_t collider);
+/* Particle sinks and sources of a fluid, applied on the device at the start of every step (DESIGN.md section 14).  They do on
+ * the device what faucet3.rs:69-105 does from a host callback before each step: mark the particles below a plane with
+ * delete_particle_at_next_timestep (fluid.rs:100-104) and append a sheet with add_particles (fluid.rs:126-150) every 0.06 s.
+ * Each sph_world_step / sph_world_step_with_coupling call that gets past its refusals counts as one step, a step of
+ * dt <= FLT_EPSILON included.  In it, after the marks of sph_fluid_delete are applied (liquid_world.rs:79-81) and before the
+ * boundaries, colliders, grid and solver:
+ *   1. every particle that a sink of its fluid removes, tested at its position at the start of the step, is deleted; the
+ *      survivors keep their order (fluid.rs:88-98);
+ *   2. every source that fires appends its template to the end of its fluid's index range, in registration order, exactly
+ *      as sph_fluid_append would: default volume, zero velocity_changes and IISPH pressure.  The ids count up from 1 + the
+ *      largest id the fluid held at the start of the step, marked and sunk particles included, continuing from one source
+ *      to the next.
+ * The result equals reading the positions, sph_fluid_delete with the sinks' mask and sph_fluid_append of each firing template
+ * before the step, bit for bit in deterministic mode, without a round trip of the particles through the host.  Up to 64 sinks
+ * and 64 sources per world; handles are slot | generation << 16.  sph_fluid_remove removes its fluid's sinks and sources.
+ * Snapshots store neither, and sph_world_snapshot_load leaves them and their step counts as they are.  Slab-decomposed worlds
+ * refuse them (SPH_ERR_INVALID), and sph_world_step_many refuses to run while any is registered.  A step whose emissions
+ * would number ids past 2^32 - 1 is refused with SPH_ERR_INVALID before it changes anything. */
+typedef struct {
+    float   lo[3], hi[3];  /* a particle is in the box iff lo[a] <= x[a] < hi[a] on every axis (f32 comparisons; +-INFINITY allowed) */
+    int32_t outside;       /* 0: removes the particles in the box (faucet3.rs:77-81: y < -2 is lo = -inf, hi = (inf, -2, inf));
+                              1: removes every particle not in the box (a domain sink; non-finite positions are in no box) */
+} sph_sink_desc;
+/* A sink of `fluid` (faucet3.rs:74-86).  SPH_ERR_INVALID, nothing changed, for a NaN bound, lo > hi on an axis or outside
+ * other than 0 / 1. */
+sph_status sph_fluid_add_sink(sph_world* w, uint32_t fluid, const sph_sink_desc* sink, uint32_t* sink_handle);
+sph_status sph_sink_remove(sph_world* w, uint32_t sink);
+/* A source of `fluid` (faucet3.rs:88-103): the n particles of pos_xyz (packed xyz) with velocities vel_xyz (NULL: zero) are
+ * copied to the device now and appended on the first step after this call and on every interval-th step after it (interval
+ * counts steps: faucet3's 0.06 s at dt = 1 / 200 is 12).  SPH_ERR_INVALID, nothing changed, for n == 0, a NULL template or
+ * interval == 0. */
+sph_status sph_fluid_add_source(sph_world* w, uint32_t fluid, const float* pos_xyz, const float* vel_xyz, size_t n, uint32_t interval,
+                                uint32_t* source_handle);
+sph_status sph_source_remove(sph_world* w, uint32_t source);
+/* How many particles of `fluid` the sinks removed and the sources emitted in the last step (0 before any step).  NULL = skip. */
+sph_status sph_fluid_read_step_edits(sph_world* w, uint32_t fluid, uint32_t* removed, uint32_t* emitted);
+
 /* boundary.positions / velocities (boundary.rs:13-15) in ORIGINAL index order.  NULL = skip; *n = particle count. */
 sph_status sph_boundary_read(sph_world* w, uint32_t boundary, float* pos_xyz, float* vel_xyz, size_t cap, size_t* n);
 

@@ -92,6 +92,10 @@ class CouplingManagerC(C.Structure):
     _fields_ = [("update_boundaries", COUPLING_UPDATE_FN), ("transmit_forces", COUPLING_TRANSMIT_FN), ("user", C.c_void_p)]
 
 
+class SinkDesc(C.Structure):
+    _fields_ = [("lo", C.c_float * 3), ("hi", C.c_float * 3), ("outside", C.c_int32)]
+
+
 # every symbol include/sph.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "sph_world_desc_default": (None, [C.POINTER(WorldDesc)]),
@@ -155,6 +159,11 @@ SYMBOLS = {
     "sph_world_particles_in_heightfield": (C.c_int, [_vp, C.POINTER(HeightFieldC), _fp, _fp, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
                                                      C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(C.c_size_t)]),
     "sph_collider_register_heightfield": (C.c_int, [_vp, C.c_uint32, C.POINTER(HeightFieldC), C.POINTER(C.c_uint32)]),
+    "sph_fluid_add_sink": (C.c_int, [_vp, C.c_uint32, C.POINTER(SinkDesc), C.POINTER(C.c_uint32)]),
+    "sph_sink_remove": (C.c_int, [_vp, C.c_uint32]),
+    "sph_fluid_add_source": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.c_uint32, C.POINTER(C.c_uint32)]),
+    "sph_source_remove": (C.c_int, [_vp, C.c_uint32]),
+    "sph_fluid_read_step_edits": (C.c_int, [_vp, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
 }
 
 

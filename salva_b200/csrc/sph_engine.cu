@@ -30,6 +30,7 @@
 #include "sph_elasticity.cuh"
 #include "sph_viscosity.cuh"
 #include "sph_sampling.cuh"
+#include "sph_edits.cuh"
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -186,6 +187,7 @@ struct FluidRec {
     float uniform_mass = 0.f;  // common particle mass if all volumes are equal, else 0
     bool alive = true;         // false after LiquidWorld::remove_fluid (liquid_world.rs:171-173); the slot is reused by the next add
     uint32_t gen = 0;          // handle = slot | gen << 16 (the reference's arena handles carry a generation too)
+    size_t step_removed = 0, step_emitted = 0;  // what the last step's sinks removed and its sources emitted
     // move-only: the forces own device memory, and std::vector<ForceRec> would still declare a copy
     FluidRec() = default;
     FluidRec(FluidRec&&) = default;
@@ -293,6 +295,23 @@ struct ColliderRec {
     bool alive = true;
     uint32_t gen = 0;
 };
+// A particle sink or source of one fluid (sph_edits_host.inl); handles are slot | gen << 16 like the colliders'.
+struct SinkRec {
+    sph_sink_desc d{};
+    uint32_t fluid = 0;  // fluid slot
+    bool alive = true;
+    uint32_t gen = 0;
+};
+struct SourceRec {
+    uint32_t fluid = 0;
+    size_t n = 0;             // template particles
+    DBuf<float4> pos, vel;    // the template, uploaded at registration
+    bool has_vel = false;
+    uint32_t interval = 1, age = 0;  // fires on the steps with age % interval == 0; age counts the steps since registration
+    int cells[7] = {};        // the template's cell AABB and bad flag, as k_bounds computes them
+    bool alive = true;
+    uint32_t gen = 0;
+};
 static_assert(!std::is_copy_constructible<DBuf<float>>::value && !std::is_copy_constructible<ForceRec>::value &&
                   !std::is_copy_constructible<FluidRec>::value && !std::is_copy_constructible<ColliderRec>::value,
               "records that own device memory move, never copy");
@@ -320,6 +339,9 @@ bool any_contact(const sph_world* w);
 sph_status colliders_update(sph_world* w, bool reposed_all);
 sph_status colliders_contact(sph_world* w);
 sph_status colliders_impulse(sph_world* w);
+bool any_edit(const sph_world* w);
+sph_status edits_before_marks(sph_world* w, uint64_t* next);
+sph_status apply_sources_sinks(sph_world* w, uint64_t* next);
 inline float __uint_as_float_host(uint32_t u) {
     float f;
     memcpy(&f, &u, sizeof f);
@@ -505,6 +527,13 @@ struct sph_world {
     bool nb_valid = false, nb_pending = false;
     int nb[7] = {0, 0, 0, 0, 0, 0, 0};
     DBuf<int> d_nb;
+    // particle sinks and sources (sph_edits_host.inl) and their classification's flags, result and removed original indices
+    std::vector<SinkRec> sinks;
+    std::vector<SourceRec> sources;
+    DBuf<EditScan> d_edit;
+    EditScan* h_edit = nullptr;  // pinned
+    DBuf<uint32_t> ed_keep, ed_rm, ed_list;
+    bool vol_all_default = true;  // every row of rows.vol is rows.vol0 (set by stage_up): edits then only resize the column
     int xysub = 1;              // row order (Consts::xysub, SALVA_B200_XYSUB): x / y bins per cell; one GPU only
 
     bool grid_ready = false;    // cstart/bstart + sorted arrays describe the last step's cell grid (AABB queries)
@@ -528,6 +557,7 @@ struct sph_world {
         graphs.release();
         if (h_pinned) cudaFreeHost(h_pinned);
         if (h_imp) cudaFreeHost(h_imp);
+        if (h_edit) cudaFreeHost(h_edit);
         if (st) cudaStreamDestroy(st);
     }
 
@@ -796,10 +826,14 @@ sph_status stage_up(sph_world* w) {
     w->Ntot = N;
     w->own_begin = 0;
     TRY(ensure_fluid_buffers(w));
+    w->vol_all_default = true;
     if (N) {
         const std::vector<float>& vol = w->rows.vol;
         std::vector<float> mass(N);
         std::vector<uint32_t> fid(N);
+        bool all_default = true;
+        for (size_t g = 0; g < N; ++g) all_default = all_default && vol[g] == w->rows.vol0;
+        w->vol_all_default = all_default;
         for (size_t f = 0; f < w->fluids.size(); ++f) {
             bool uniform = w->fluids[f].n > 0;
             for (size_t i = 0; i < w->fluids[f].n; ++i) {
@@ -1998,8 +2032,11 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
     const bool colliders = any_collider(w);  // refused before anything of the step is applied
     if (colliders && coupling) return w->fail(SPH_ERR_INVALID, "registered colliders and a host coupling manager cannot run in one step");
     if (colliders && w->slab.active) return w->fail(SPH_ERR_INVALID, "colliders are not supported in slab-decomposed worlds");
+    uint64_t next_ids[MAX_FLUIDS];
+    TRY(edits_before_marks(w, next_ids));
     TRY(apply_pending_deletes(w));  // liquid_world.rs:79-81
     TRY(stage_up(w));
+    TRY(apply_sources_sinks(w, next_ids));  // DESIGN.md section 14
     for (ColliderRec& c : w->colliders) memset(c.impulse, 0, sizeof c.impulse);
     const bool b_uploaded = w->b_dirty;
     TRY(upload_boundaries(w));
@@ -2061,6 +2098,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 #include "sph_viscosity_host.inl"
 #include "sph_colliders_host.inl"
 #include "sph_graph.inl"
+#include "sph_edits_host.inl"
 
 // ===================================================================================================
 // extern "C" boundary
@@ -2725,6 +2763,14 @@ sph_status sph_fluid_remove(sph_world* w, uint32_t fluid_h) {
     w->rows.splice(f.offset, f.n, 0, nullptr, nullptr, nullptr, nullptr, nullptr);
     f.forces.clear();
     f.pending_delete.clear();
+    for (SinkRec& s : w->sinks)
+        if (s.fluid == fluid) s.alive = false;
+    for (SourceRec& s : w->sources)
+        if (s.fluid == fluid && s.alive) {
+            s.pos.release();
+            s.vel.release();
+            s.alive = false;
+        }
     f.n_pending = 0;
     f.n = 0;
     f.alive = false;
@@ -2906,6 +2952,101 @@ sph_status sph_collider_unregister(sph_world* w, uint32_t collider_h) {
     c.local.release();
     c.hgt.release();
     c.alive = false;
+    return SPH_OK;
+}
+
+// ---- particle sinks and sources (faucet3.rs:69-105, DESIGN.md section 14) ----------------------------------------------
+// Fluid::delete_particle_at_next_timestep for every particle in (or, outside = 1, not in) a box, every step (faucet3.rs:74-86)
+sph_status sph_fluid_add_sink(sph_world* w, uint32_t fluid_h, const sph_sink_desc* sink, uint32_t* handle) {
+    if (!w || !sink) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    FLUID_OR_FAIL(fluid, fluid_h)
+    for (int a = 0; a < 3; ++a)
+        if (std::isnan(sink->lo[a]) || std::isnan(sink->hi[a]) || sink->lo[a] > sink->hi[a])
+            return w->fail(SPH_ERR_INVALID, "sph_fluid_add_sink: axis %d needs lo <= hi without NaN, got [%g, %g)", a, (double)sink->lo[a], (double)sink->hi[a]);
+    if (sink->outside != 0 && sink->outside != 1) return w->fail(SPH_ERR_INVALID, "sph_fluid_add_sink: outside must be 0 or 1, got %d", sink->outside);
+    TRY(edits_check_world(w));
+    const int slot = edits_slot(w->sinks, MAX_SINKS);
+    if (slot < 0) return w->fail(SPH_ERR_INVALID, "too many particle sinks (max %d)", MAX_SINKS);
+    SinkRec& r = w->sinks[slot];
+    r.d = *sink;
+    r.fluid = fluid;
+    r.alive = true;
+    r.gen++;
+    if (handle) *handle = make_handle(slot, r.gen & 0xFFFFu);
+    return SPH_OK;
+}
+
+sph_status sph_sink_remove(sph_world* w, uint32_t sink_h) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const int slot = edits_lookup(w->sinks, sink_h);
+    if (slot < 0) return w->fail(SPH_ERR_INVALID, "bad sink handle %u", (unsigned)sink_h);
+    w->sinks[slot].alive = false;
+    return SPH_OK;
+}
+
+// Fluid::add_particles of the same template every `interval` steps (faucet3.rs:88-103 adds a 10 x 10 sheet every 0.06 s)
+sph_status sph_fluid_add_source(sph_world* w, uint32_t fluid_h, const float* pos, const float* vel, size_t n, uint32_t interval, uint32_t* handle) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    FLUID_OR_FAIL(fluid, fluid_h)
+    if (!pos || n == 0) return w->fail(SPH_ERR_INVALID, "sph_fluid_add_source: empty template");
+    if (interval == 0) return w->fail(SPH_ERR_INVALID, "sph_fluid_add_source: interval must be at least 1 step");
+    if (n > UINT32_MAX) return w->fail(SPH_ERR_INVALID, "sph_fluid_add_source: template of %zu particles is too large", n);
+    TRY(edits_check_world(w));
+    std::vector<float4> p(n), v(vel ? n : 0);
+    int cells[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+    for (size_t i = 0; i < n; ++i) {
+        p[i] = make_float4(pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], 0.f);
+        if (vel) v[i] = make_float4(vel[3 * i], vel[3 * i + 1], vel[3 * i + 2], 0.f);
+        for (int a = 0; a < 3; ++a) {
+            const float cf = floorf(pos[3 * i + a] / w->h);  // hgrid.rs:41-43, the same IEEE division as k_bounds
+            if (!(fabsf(cf) < 1.0e9f)) { cells[6] = 1; continue; }
+            cells[a] = std::min(cells[a], (int)cf);
+            cells[3 + a] = std::max(cells[3 + a], (int)cf);
+        }
+    }
+    SourceRec r;
+    CU(r.pos.ensure(n));
+    CU(cudaMemcpy(r.pos.p, p.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+    if (vel) {
+        CU(r.vel.ensure(n));
+        CU(cudaMemcpy(r.vel.p, v.data(), n * sizeof(float4), cudaMemcpyHostToDevice));
+    }
+    const int slot = edits_slot(w->sources, MAX_SOURCES);
+    if (slot < 0) return w->fail(SPH_ERR_INVALID, "too many particle sources (max %d)", MAX_SOURCES);
+    r.fluid = fluid;
+    r.n = n;
+    r.has_vel = vel != nullptr;
+    r.interval = interval;
+    r.age = 0;
+    memcpy(r.cells, cells, sizeof cells);
+    r.gen = w->sources[slot].gen + 1;
+    w->sources[slot] = std::move(r);
+    if (handle) *handle = make_handle(slot, w->sources[slot].gen & 0xFFFFu);
+    return SPH_OK;
+}
+
+sph_status sph_source_remove(sph_world* w, uint32_t source_h) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const int slot = edits_lookup(w->sources, source_h);
+    if (slot < 0) return w->fail(SPH_ERR_INVALID, "bad source handle %u", (unsigned)source_h);
+    TRY(enter(w));
+    SourceRec& r = w->sources[slot];
+    r.pos.release();
+    r.vel.release();
+    r.alive = false;
+    return SPH_OK;
+}
+
+sph_status sph_fluid_read_step_edits(sph_world* w, uint32_t fluid_h, uint32_t* removed, uint32_t* emitted) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    FLUID_OR_FAIL(fluid, fluid_h)
+    if (removed) *removed = (uint32_t)w->fluids[fluid].step_removed;
+    if (emitted) *emitted = (uint32_t)w->fluids[fluid].step_emitted;
     return SPH_OK;
 }
 

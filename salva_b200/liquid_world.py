@@ -524,6 +524,41 @@ class LiquidWorld:
                 return k[:n.value], h[:n.value], i[:n.value]
             cap = n.value
 
+    # -- particle sinks and sources (faucet3.rs:69-105, include/sph.h, DESIGN.md section 14) ------------------------
+    def add_sink(self, fluid, lo, hi, outside=False):
+        """Every step, removes the particles of `fluid` in the box lo <= x < hi (outside=True: every particle not in it) at the
+        start of the step, on the device.  Returns the sink's handle."""
+        d = _lib.SinkDesc()
+        d.lo[:] = [float(x) for x in np.asarray(lo, np.float32)]
+        d.hi[:] = [float(x) for x in np.asarray(hi, np.float32)]
+        d.outside = int(outside)
+        h = C.c_uint32()
+        self._ck(self._L.sph_fluid_add_sink(self._w, fluid, C.byref(d), C.byref(h)))
+        return h.value
+
+    def add_source(self, fluid, positions, velocities=None, interval=1):
+        """Appends the template (positions, velocities=None: zero) to `fluid` on the first step and every interval-th step
+        after it, as append_particles would.  Returns the source's handle."""
+        p = _f32(positions, (-1, 3))
+        v = _f32(velocities, (-1, 3))
+        if v is not None and len(v) != len(p):
+            raise ValueError("add_source: %d velocities for %d positions" % (len(v), len(p)))
+        h = C.c_uint32()
+        self._ck(self._L.sph_fluid_add_source(self._w, fluid, _fp(p), _fp(v), 0 if p is None else len(p), int(interval), C.byref(h)))
+        return h.value
+
+    def remove_sink(self, sink):
+        self._ck(self._L.sph_sink_remove(self._w, sink))
+
+    def remove_source(self, source):
+        self._ck(self._L.sph_source_remove(self._w, source))
+
+    def step_edits(self, fluid):
+        """(removed, emitted): the particles of `fluid` the last step's sinks removed and its sources emitted."""
+        r, e = C.c_uint32(), C.c_uint32()
+        self._ck(self._L.sph_fluid_read_step_edits(self._w, fluid, C.byref(r), C.byref(e)))
+        return r.value, e.value
+
     # -- snapshot / restore and zero-copy views (include/sph.h) ---------------------------------------------
     def snapshot(self):
         """Everything the solver carries across steps (vc, dt lag, IISPH pressures, Becker rest pose, ids) as bytes."""
