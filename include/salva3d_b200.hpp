@@ -285,6 +285,12 @@ private:
 };
 
 using FluidHandle = size_t;
+// A fluid surface mesh (LiquidWorld::extract_surface): counter-clockwise triangles seen from outside, vertex normals when asked
+struct SurfaceMesh {
+    std::vector<Point3> vertices;
+    std::vector<Vector3> normals;
+    std::vector<uint32_t> triangles;  // 3 vertex indices per triangle
+};
 using BoundaryHandle = size_t;
 
 class LiquidWorld {  // liquid_world.rs:17-158
@@ -418,6 +424,24 @@ public:
         uint32_t r = 0, e = 0;
         check(sph_fluid_read_step_edits(raw_, fluids_.at(fluid).handle_, &r, &e));
         return {r, e};
+    }
+    // The surface phi = iso of the fluids' smoothed volume fraction (include/sph.h sph_world_extract_surface, DESIGN.md section
+    // 15), sampled on a lattice of `spacing` (<= 0: the particle radius).  fluids empty: every fluid.  lo.x > hi.x (the default)
+    // meshes the fluids' AABB grown by h, where every surface closes; a box clips the lattice and leaves surfaces open there.
+    SurfaceMesh extract_surface(Real iso = 0.6f, Real spacing = 0.f, const std::vector<FluidHandle>& fluids = {}, bool normals = true,
+                                const Vector3& lo = Vector3{1, 1, 1}, const Vector3& hi = Vector3{0, 0, 0}) {
+        std::vector<uint32_t> hs;
+        for (FluidHandle f : fluids) hs.push_back(fluids_.at(f).handle_);
+        const sph_surface_desc d{iso, spacing > 0.f ? spacing : particle_radius(), {lo.x, lo.y, lo.z}, {hi.x, hi.y, hi.z}, normals ? 1 : 0};
+        size_t nv = 0, nt = 0;
+        check(sph_world_extract_surface(raw_, hs.data(), hs.size(), &d, &nv, &nt));
+        SurfaceMesh m;
+        m.vertices.resize(nv);
+        m.normals.resize(normals ? nv : 0);
+        m.triangles.resize(3 * nt);
+        check(sph_world_read_surface(raw_, reinterpret_cast<float*>(m.vertices.data()), normals ? reinterpret_cast<float*>(m.normals.data()) : nullptr, nv,
+                                     m.triangles.data(), nt));
+        return m;
     }
     // liquid_world.rs:67-158
     void step_with_coupling(Real dt, const Vector3& gravity, CouplingManager* coupling) {

@@ -468,6 +468,46 @@ sph_status sph_source_remove(sph_world* w, uint32_t source);
 /* How many particles of `fluid` the sinks removed and the sources emitted in the last step (0 before any step).  NULL = skip. */
 sph_status sph_fluid_read_step_edits(sph_world* w, uint32_t fluid, uint32_t* removed, uint32_t* emitted);
 
+/* Fluid surface meshes on the device (DESIGN.md section 15).  The field phi(x) = sum_j V_j W(|x - x_j|) sums over the particles
+ * of the selected fluids (boundaries are not included), with V_j the particle's volume, W the world's density kernel and h, and
+ * the positions of the last step (before the first step: those given).  Inside settled fluid phi ~ rho / rho0 ~ 1.  It is
+ * sampled on the lattice p_ijk = origin + spacing * (i, j, k), x fastest, with origin[a] = spacing * floor(lo[a] / spacing)
+ * and n[a] = ceil((hi[a] - origin[a]) / spacing) + 1 points per axis (f32 operations; a coordinate is origin[a] + (float)i *
+ * spacing, a product and then a sum), so the lattices of successive frames and of different boxes share their points.  A point
+ * is inside iff phi >= iso.  Every lattice cube is split into the 6 tetrahedra (0, e_a, e_a + e_b, 1) and each is polygonised
+ * by a 16-case table, so the mesh is watertight and no case is ambiguous.  Vertices: one per crossed lattice edge, at
+ * x = p_a + t (p_b - p_a) with t = (iso - phi_a) / (phi_b - phi_a), a the inside end; ordered by the point owning the edge
+ * (x fastest), then by its direction +x, +y, +z, +x+y, +x+z, +y+z, +x+y+z.  Triangles: ordered by cube, tetrahedron
+ * (permutations xyz, xzy, yxz, yzx, zxy, zyx) and table order; counter-clockwise seen from outside (the side of lower phi).
+ * Normals (optional): -grad phi / |grad phi| at the vertex with the world's gradient kernel, 0 where the gradient is 0.  In
+ * deterministic mode field and mesh are bit-identical run to run and do not depend on the fluids' slot order.
+ * The default box (lo[0] > hi[0]) is the selected fluids' AABB grown by h on every side: phi is 0 on its border and every
+ * surface closes.  A caller box clips the lattice, and surfaces are open where the box cuts them. */
+typedef struct {
+    float   iso;           /* finite, > 0 */
+    float   spacing;       /* finite, > 0 */
+    float   lo[3], hi[3];  /* box to mesh; lo[0] > hi[0] = the selected fluids' AABB grown by h */
+    int32_t normals;       /* 1: also compute vertex normals (a second gather), 0: skip */
+} sph_surface_desc;
+/* Extracts the surface of fluids[0..n_fluids) (n_fluids == 0: every fluid).  The field and mesh stay in device buffers of the
+ * world until the next extraction or sph_world_destroy; the step, its grid and its cached graphs are not touched.  No fluid
+ * particles give 0 vertices and 0 triangles.  SPH_ERR_INVALID, nothing changed and the previous mesh kept, for NaN or
+ * out-of-range desc fields, lo > hi on some axes but not all, a non-finite caller box, stale or duplicate fluid handles,
+ * slab-decomposed worlds, calls from inside a coupling or host-force callback, and pending host edits (sph_fluid_write /
+ * _append / _delete after the last step: step first).  SPH_ERR_OOM, nothing changed, when the lattice would exceed 2^31
+ * points, the vertex or triangle count would pass 2^32 - 1, or an allocation fails. */
+sph_status sph_world_extract_surface(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_surface_desc* desc,
+                                     size_t* n_vertices, size_t* n_triangles);
+/* The last extraction's mesh: packed xyz vertices, their normals (NULL = skip) and 3 vertex indices per triangle.
+ * SPH_ERR_INVALID when vcap or tcap is below the counts, or normals_xyz is not NULL and the extraction ran with normals = 0. */
+sph_status sph_world_read_surface(sph_world* w, float* vertices_xyz, float* normals_xyz, size_t vcap, uint32_t* triangles, size_t tcap);
+/* Device pointers to the same arrays (d_normals_xyz NULL when not computed), valid until the next extraction: the zero-copy
+ * path for renderers, like sph_fluid_map_positions.  Any output pointer may be NULL. */
+sph_status sph_world_map_surface(sph_world* w, const float** d_vertices_xyz, const float** d_normals_xyz, const uint32_t** d_triangles);
+/* phi on the last extraction's lattice, x fastest, with its origin and point counts (0 before any extraction and when no
+ * lattice was built).  phi == NULL: only origin and dims are written.  SPH_ERR_INVALID when cap is below the point count. */
+sph_status sph_world_read_surface_field(sph_world* w, float* phi, size_t cap, float origin[3], uint32_t dims[3]);
+
 /* boundary.positions / velocities (boundary.rs:13-15) in ORIGINAL index order.  NULL = skip; *n = particle count. */
 sph_status sph_boundary_read(sph_world* w, uint32_t boundary, float* pos_xyz, float* vel_xyz, size_t cap, size_t* n);
 

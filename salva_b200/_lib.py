@@ -96,6 +96,10 @@ class SinkDesc(C.Structure):
     _fields_ = [("lo", C.c_float * 3), ("hi", C.c_float * 3), ("outside", C.c_int32)]
 
 
+class SurfaceDesc(C.Structure):
+    _fields_ = [("iso", C.c_float), ("spacing", C.c_float), ("lo", C.c_float * 3), ("hi", C.c_float * 3), ("normals", C.c_int32)]
+
+
 # every symbol include/sph.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "sph_world_desc_default": (None, [C.POINTER(WorldDesc)]),
@@ -164,6 +168,11 @@ SYMBOLS = {
     "sph_fluid_add_source": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.c_uint32, C.POINTER(C.c_uint32)]),
     "sph_source_remove": (C.c_int, [_vp, C.c_uint32]),
     "sph_fluid_read_step_edits": (C.c_int, [_vp, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]),
+    "sph_world_extract_surface": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(SurfaceDesc), C.POINTER(C.c_size_t),
+                                            C.POINTER(C.c_size_t)]),
+    "sph_world_read_surface": (C.c_int, [_vp, _fp, _fp, C.c_size_t, C.POINTER(C.c_uint32), C.c_size_t]),
+    "sph_world_map_surface": (C.c_int, [_vp, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(C.POINTER(C.c_uint32))]),
+    "sph_world_read_surface_field": (C.c_int, [_vp, _fp, C.c_size_t, _fp, C.POINTER(C.c_uint32)]),
 }
 
 

@@ -31,6 +31,7 @@
 #include "sph_viscosity.cuh"
 #include "sph_sampling.cuh"
 #include "sph_edits.cuh"
+#include "sph_surface.cuh"
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -159,6 +160,26 @@ struct ElasticityState {
     DBuf<float4> cur;        // current positions (xyz) + mass (.w) in original order
     DBuf<uint32_t> slot_of;  // sorted slot of local original index t
     float d0 = 0.f, d1 = 0.f, d2 = 0.f;
+};
+
+// Fluid surface extraction (sph_surface_host.inl): the collected particles, their cells and the lattice scratch of one
+// extraction, and the field and mesh of the last one.  An extraction builds into the scratch set and swaps it in on success,
+// so a refused one keeps the previous mesh.
+struct SurfaceSet {
+    DBuf<float> phi, verts, nrm;
+    DBuf<uint32_t> tris;
+    SurfLattice L{};
+    size_t nv = 0, nt = 0;
+    bool normals = false;
+};
+struct SurfaceState {
+    DBuf<float4> p4, sp4;                  // (x, y, z, volume): collected, then in cell order
+    DBuf<unsigned long long> key;          // (fluid slot, id)
+    DBuf<float> vol;                       // the host's volume column while it is not all default
+    DBuf<uint32_t> cid, rank, perm, cstart, aabb, vcnt, tcnt, scan_aux[3];
+    DBuf<uint8_t> emask;
+    DBuf<unsigned long long> totals;
+    SurfaceSet cur, next;
 };
 
 struct ForceRec;
@@ -498,6 +519,7 @@ struct sph_world {
     DBuf<uint32_t> q_out, q_count;     // particles_intersecting_aabb results
     DBuf<float> map_pos, map_vel;      // sph_fluid_map_positions / _velocities: ORIGINAL-order device views
     bool in_coupling = false;          // inside CouplingManager::update_boundaries: the grid holds fluids only (liquid_world.rs:90-103)
+    bool in_host_force = false;        // inside a host NonPressureForce callback
     const sph_coupling_manager* coupling = nullptr;
     // ParticlesContacts materialised for host plugins (original order CSR)
     DBuf<uint32_t> ct_cnt[2], ct_j[2], ct_model[2];
@@ -533,6 +555,7 @@ struct sph_world {
     DBuf<EditScan> d_edit;
     EditScan* h_edit = nullptr;  // pinned
     DBuf<uint32_t> ed_keep, ed_rm, ed_list;
+    SurfaceState surf;  // sph_world_extract_surface's scratch and its last mesh
     bool vol_all_default = true;  // every row of rows.vol is rows.vol0 (set by stage_up): edits then only resize the column
     int xysub = 1;              // row order (Consts::xysub, SALVA_B200_XYSUB): x / y bins per cell; one GPU only
 
@@ -711,9 +734,11 @@ sph_status scan_exclusive(sph_world* w, uint32_t* data, size_t n, int level = 0)
     return SPH_OK;
 }
 
-// K arrays of the same length scanned together (in place, exclusive); n <= 2048 * 2048 * 2048
+// K arrays of the same length scanned together (in place, exclusive); n <= 2048 * 2048 * 2048.  aux: three levels of block
+// sums (default: the step's scan_aux_k)
 template <int K>
-sph_status scan_exclusive_k(sph_world* w, ScanSet<K> arrays, size_t n, int level = 0) {
+sph_status scan_exclusive_k(sph_world* w, ScanSet<K> arrays, size_t n, int level = 0, DBuf<uint32_t>* aux = nullptr) {
+    if (!aux) aux = w->scan_aux_k;
     if (n == 0) return SPH_OK;
     uint32_t nb = cdiv(n, SCAN_B);
     ScanSet<K> sums;
@@ -724,11 +749,11 @@ sph_status scan_exclusive_k(sph_world* w, ScanSet<K> arrays, size_t n, int level
         return SPH_OK;
     }
     if (level >= 3) return w->fail(SPH_ERR_INVALID, "scan too deep");
-    CU(w->scan_aux_k[level].ensure((size_t)K * nb));
-    for (int a = 0; a < K; ++a) sums.a[a] = w->scan_aux_k[level].p + (size_t)a * nb;
+    CU(aux[level].ensure((size_t)K * nb));
+    for (int a = 0; a < K; ++a) sums.a[a] = aux[level].p + (size_t)a * nb;
     k_scanK_block<K><<<nb, SCAN_T, 0, w->st>>>(arrays, (uint32_t)n, sums);
     w->launches++;
-    TRY(scan_exclusive_k<K>(w, sums, nb, level + 1));
+    TRY(scan_exclusive_k<K>(w, sums, nb, level + 1, aux));
     k_scanK_add<K><<<nb, SCAN_T, 0, w->st>>>(arrays, (uint32_t)n, sums);
     w->launches++;
     return SPH_OK;
@@ -1676,8 +1701,12 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
                     CU(cudaMemcpyAsync(ha.data(), w->o_c.p + 3 * fl.offset, 3 * Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
                     CU(cudaMemcpyAsync(hd.data(), w->o_mass.p + fl.offset, Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
                     CU(cudaStreamSynchronize(w->st));
-                    if (fr.host_fn2) TRY(call_host_force2(w, (uint32_t)f, fr, hp, hv, hd, ha));
+                    w->in_host_force = true;
+                    sph_status hs = SPH_OK;
+                    if (fr.host_fn2) hs = call_host_force2(w, (uint32_t)f, fr, hp, hv, hd, ha);
                     else fr.host_fn(fr.host_user, w->dt, w->inv_dt, w->h, Nf, hp.data(), hv.data(), hd.data(), ha.data());
+                    w->in_host_force = false;
+                    TRY(hs);
                     TRY(enter(w));  // the callback may have used another world of this process
                     CU(cudaMemcpyAsync(w->o_c.p + 3 * fl.offset, ha.data(), 3 * Nf * sizeof(float), cudaMemcpyHostToDevice, w->st));
                     LAUNCH(k_import_acc, N, 256, (uint32_t)N, w->orig[c].p + ob, w->o_c.p, (uint32_t)fl.offset, (uint32_t)(fl.offset + Nf), w->acc.p + ob);
@@ -2099,6 +2128,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 #include "sph_colliders_host.inl"
 #include "sph_graph.inl"
 #include "sph_edits_host.inl"
+#include "sph_surface_host.inl"
 
 // ===================================================================================================
 // extern "C" boundary
@@ -3047,6 +3077,54 @@ sph_status sph_fluid_read_step_edits(sph_world* w, uint32_t fluid_h, uint32_t* r
     FLUID_OR_FAIL(fluid, fluid_h)
     if (removed) *removed = (uint32_t)w->fluids[fluid].step_removed;
     if (emitted) *emitted = (uint32_t)w->fluids[fluid].step_emitted;
+    return SPH_OK;
+}
+
+// Fluid surface meshes (sph_surface_host.inl, DESIGN.md section 15)
+sph_status sph_world_extract_surface(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_surface_desc* desc, size_t* n_vertices,
+                                     size_t* n_triangles) {
+    if (!w || !desc || !n_vertices || !n_triangles || (n_fluids && !fluids)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    return extract_surface(w, fluids, n_fluids, desc, n_vertices, n_triangles);
+}
+sph_status sph_world_read_surface(sph_world* w, float* vertices_xyz, float* normals_xyz, size_t vcap, uint32_t* triangles, size_t tcap) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const SurfaceSet& R = w->surf.cur;
+    if (vcap < R.nv || tcap < R.nt) return w->fail(SPH_ERR_INVALID, "sph_world_read_surface: caps %zu / %zu below the counts %zu / %zu", vcap, tcap, R.nv, R.nt);
+    if (normals_xyz && !R.normals) return w->fail(SPH_ERR_INVALID, "sph_world_read_surface: the extraction ran without normals");
+    if ((R.nv && !vertices_xyz) || (R.nt && !triangles)) return w->fail(SPH_ERR_INVALID, "sph_world_read_surface: null output");
+    TRY(enter(w));
+    if (R.nv) CU(cudaMemcpyAsync(vertices_xyz, R.verts.p, 3 * R.nv * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    if (R.nv && normals_xyz) CU(cudaMemcpyAsync(normals_xyz, R.nrm.p, 3 * R.nv * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    if (R.nt) CU(cudaMemcpyAsync(triangles, R.tris.p, 3 * R.nt * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaStreamSynchronize(w->st));
+    return SPH_OK;
+}
+sph_status sph_world_map_surface(sph_world* w, const float** d_vertices_xyz, const float** d_normals_xyz, const uint32_t** d_triangles) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const SurfaceSet& R = w->surf.cur;
+    if (d_vertices_xyz) *d_vertices_xyz = R.verts.p;
+    if (d_normals_xyz) *d_normals_xyz = R.normals ? R.nrm.p : nullptr;
+    if (d_triangles) *d_triangles = R.tris.p;
+    return SPH_OK;
+}
+sph_status sph_world_read_surface_field(sph_world* w, float* phi, size_t cap, float origin[3], uint32_t dims[3]) {
+    if (!w || !origin || !dims) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const SurfaceSet& R = w->surf.cur;
+    const size_t npts = (size_t)R.L.n[0] * R.L.n[1] * R.L.n[2];
+    if (phi && cap < npts) return w->fail(SPH_ERR_INVALID, "sph_world_read_surface_field: cap %zu below the %zu lattice points", cap, npts);
+    for (int a = 0; a < 3; ++a) {
+        origin[a] = R.L.o[a];
+        dims[a] = R.L.n[a];
+    }
+    if (phi && npts) {
+        TRY(enter(w));
+        CU(cudaMemcpyAsync(phi, R.phi.p, npts * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+        CU(cudaStreamSynchronize(w->st));
+    }
     return SPH_OK;
 }
 

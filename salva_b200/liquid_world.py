@@ -559,6 +559,74 @@ class LiquidWorld:
         self._ck(self._L.sph_fluid_read_step_edits(self._w, fluid, C.byref(r), C.byref(e)))
         return r.value, e.value
 
+    # -- fluid surface meshes (include/sph.h, DESIGN.md section 15) -------------------------------------------------
+    def extract_surface(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True):
+        """Samples phi = sum_j V_j W(|x - x_j|) of `fluids` (None: all) on a lattice of `spacing` (None: the particle radius)
+        and polygonises phi = iso on the device.  box=None meshes the fluids' AABB grown by h, where every surface closes; a
+        box (lo, hi) clips the lattice, and surfaces are open where it cuts them.  Returns (n_vertices, n_triangles); the mesh
+        stays on the device until the next extraction."""
+        d = _lib.SurfaceDesc()
+        d.iso = float(iso)
+        d.spacing = float(self.particle_radius if spacing is None else spacing)
+        if box is None:
+            d.lo[:], d.hi[:] = [1.0, 1.0, 1.0], [0.0, 0.0, 0.0]
+        else:
+            d.lo[:] = [float(x) for x in np.asarray(box[0], np.float32)]
+            d.hi[:] = [float(x) for x in np.asarray(box[1], np.float32)]
+        d.normals = int(bool(normals))
+        hs = np.ascontiguousarray(np.asarray([] if fluids is None else list(fluids), np.uint32))
+        nv, nt = C.c_size_t(), C.c_size_t()
+        self._ck(self._L.sph_world_extract_surface(self._w, hs.ctypes.data_as(C.POINTER(C.c_uint32)), len(hs), C.byref(d), C.byref(nv),
+                                                   C.byref(nt)))
+        self._surface_normals = bool(normals)
+        self._surface_spacing = np.float32(d.spacing)
+        self._surface_counts = (nv.value, nt.value)
+        return nv.value, nt.value
+
+    def read_surface(self, normals=None):
+        """(vertices[nv, 3], triangles[nt, 3], normals[nv, 3] or None) of the last extraction."""
+        nv, nt = getattr(self, "_surface_counts", (0, 0))
+        if normals is None:
+            normals = getattr(self, "_surface_normals", False)
+        v = np.empty((nv, 3), np.float32)
+        t = np.empty((nt, 3), np.uint32)
+        n = np.empty((nv, 3), np.float32) if normals else None
+        self._ck(self._L.sph_world_read_surface(self._w, _fp(v), _fp(n) if n is not None else None, nv,
+                                                t.ctypes.data_as(C.POINTER(C.c_uint32)), nt))
+        return v, t, n
+
+    def surface_mesh(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True):
+        """extract_surface then read_surface: (vertices[nv, 3] f32, triangles[nt, 3] u32, normals[nv, 3] f32 or None).
+        Triangles wind counter-clockwise seen from outside; see include/sph.h for the lattice and the ordering."""
+        self.extract_surface(iso, spacing, fluids, box, normals)
+        return self.read_surface(normals)
+
+    def surface_field(self):
+        """(phi[nz, ny, nx], origin[3], spacing) of the last extraction's lattice."""
+        o = np.zeros(3, np.float32)
+        dims = (C.c_uint32 * 3)()
+        self._ck(self._L.sph_world_read_surface_field(self._w, None, 0, _fp(o), dims))
+        nx, ny, nz = int(dims[0]), int(dims[1]), int(dims[2])
+        phi = np.empty((nz, ny, nx), np.float32)
+        self._ck(self._L.sph_world_read_surface_field(self._w, _fp(phi), phi.size, _fp(o), dims))
+        return phi, o, getattr(self, "_surface_spacing", np.float32(0.0))
+
+    def map_surface(self):
+        """Device views (no host copy) of the last extraction's (vertices[nv, 3], triangles[nt, 3], normals[nv, 3] or None) as
+        objects with __cuda_array_interface__; valid until the next extraction."""
+        nv, nt = getattr(self, "_surface_counts", (0, 0))
+        vp, np_, tp = C.POINTER(C.c_float)(), C.POINTER(C.c_float)(), C.POINTER(C.c_uint32)()
+        self._ck(self._L.sph_world_map_surface(self._w, C.byref(vp), C.byref(np_), C.byref(tp)))
+
+        def view(ptr, shape, typestr):
+            addr = C.cast(ptr, C.c_void_p).value or 0
+
+            class _View:
+                __cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (addr, False), "version": 2, "strides": None}
+            return _View()
+        normals = view(np_, (nv, 3), "<f4") if C.cast(np_, C.c_void_p).value else None
+        return view(vp, (nv, 3), "<f4"), view(tp, (nt, 3), "<u4"), normals
+
     # -- snapshot / restore and zero-copy views (include/sph.h) ---------------------------------------------
     def snapshot(self):
         """Everything the solver carries across steps (vc, dt lag, IISPH pressures, Becker rest pose, ids) as bytes."""
