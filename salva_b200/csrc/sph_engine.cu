@@ -454,7 +454,6 @@ struct sph_world {
     std::vector<BoundaryRec> bounds;
     size_t N = 0, B = 0;   // N = fluid particles OWNED by this world
     size_t Ntot = 0;       // slots of the sorted arrays during a step: owned + ghost (== N on one GPU)
-    bool single_launch = true;
     int protect_buf = -1;    // double-buffer index ensure_fluid_buffers() must not reallocate (it is being read)
     uint32_t own_begin = 0;  // first owned slot (ghost columns of a slab world sit at both ends of the sorted arrays)
     SlabState slab;
@@ -524,8 +523,6 @@ struct sph_world {
     // ParticlesContacts materialised for host plugins (original order CSR)
     DBuf<uint32_t> ct_cnt[2], ct_j[2], ct_model[2];
     DBuf<float> ct_w[2], ct_g[2];
-    DBuf<uint32_t> d_ticket;      // last-block ticket of the in-kernel error reduction (kept at 0 between launches)
-    bool errsum_ready = false;    // the last evaluation launch already reduced its partials into errsum
     DBuf<float4> xs;  // the XSPH sums or the Akinci fluid force of a divergence evaluation (fold_state)
     uint32_t fused_nblk = 0;
     Tex tex_vs;  // the general evaluations gather v* through the texture pipe
@@ -1231,10 +1228,7 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
                                                                              w->d_cnt.p + 1);
         w->launches++;
     }
-    if (dens) {
-        w->fused_nblk = cdiv(N, NBR_T);  // one error partial per block, summed by read_error()
-        w->errsum_ready = false;
-    }
+    if (dens) w->fused_nblk = cdiv(N, NBR_T);  // one error partial per block, summed by read_error()
     CU(cudaGetLastError());
     w->lists_valid = true;
     if (speculative) TRY(post_density_refresh(w));
@@ -1269,11 +1263,8 @@ LoopRule loop_rule(const sph_world* w, bool divergence) {
 // mean-per-fluid -> max over fluids (dfsph_solver.rs:153-158, :347-352)
 sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     int nf = (int)w->fluids.size();
-    if (!w->errsum_ready) {
-        k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
-        w->launches++;
-    }
-    w->errsum_ready = false;
+    k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
+    w->launches++;
     TRY(slab_allreduce(w, w->errsum.p, nf));  // multi-GPU: the means are over ALL ranks' particles
     CU(cudaMemcpyAsync(w->h_pinned, w->errsum.p, nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
     CU(cudaStreamSynchronize(w->st));
@@ -1288,7 +1279,6 @@ sph_status host_decision(sph_world* w, const LoopRule& r, uint32_t i, uint32_t n
         s = read_error(w, nblk, err);
         return *err;
     });
-    w->errsum_ready = false;  // read, or not needed: the next read follows an evaluation that sets it
     return s;
 }
 
@@ -1391,7 +1381,6 @@ sph_status run_parts(sph_world* w, const SlabArray* arrays, int n_arrays, uint32
     SlabState& S = w->slab;
     TRY(slab_wait(w));
     uint32_t off = 0;
-    w->single_launch = !(S.active && S.overlap && n_arrays != 0);  // one launch covers the pass -> in-kernel final reduction
     auto part = [&](uint32_t b, uint32_t cnt) -> sph_status {
         if (!cnt) return SPH_OK;
         TRY(fn(Range{b, cnt}, off));
@@ -1464,30 +1453,28 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
     const int n_arrays = (w->slab.active && w->slab.overlap) ? 1 : 0;
     sph_status rs = run_parts(w, a, n_arrays, nblk, [&](Range rg, uint32_t blk) -> sph_status {
         float* partial = w->partial.p + (size_t)blk * nf;
-        uint32_t* tk = w->single_launch ? w->d_ticket.p : nullptr;
         if (w->unimass) {
             if (predict) {
                 LAUNCH_R((k_vel_divergence_u<true>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
+                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7);
             } else if (xsf) {
                 const float cf = w->fluids[0].forces[0].d.p[0];
                 LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, tk, w->errsum.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
+                         w->pk4.p, partial, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
             } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
                 const AkinciNorms an = akinci_norms(w->h);
                 LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, tk, w->errsum.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
+                         w->pk4.p, partial, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
             } else {
                 LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p);
+                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7);
             }
         } else {
             DISPATCH2(k_vel_divergence, multi, predict, rg.count, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
-                      w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, w->d_scal.p + 7, tk, w->errsum.p, rg);
+                      w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, w->d_scal.p + 7, rg);
         }
         return SPH_OK;
     });
-    w->errsum_ready = w->single_launch;
     return rs;
 }
 // compute_velocity_changes_for_divergence (pressure = false) / compute_velocity_changes (pressure = true).
@@ -1818,15 +1805,14 @@ sph_status cond(sph_world* w, const Cond& c, cudaGraphConditionalNodeType type, 
 // The decision after evaluation i of loop r (i < 0: the evaluation after the last decided one), from nblk error partials.
 // It sets c[0] to "an update follows", c[1] to "an update and another evaluation follow", c[2] to "an update follows and
 // ends the loop", c[3] and c[4] to false (a graph's handles keep their values from the last step); null entries are not
-// set.  Out of capture it is host_decision with the step's counts; in capture k_loop_decide, behind read_error's reduction
-// of the search's partials where evaluation 0 is read.
+// set.  Out of capture it is host_decision with the step's counts; in capture k_loop_decide, behind a k_reduce_partials of the
+// evaluation's partials wherever its error is read.
 sph_status decide(sph_world* w, const LoopRule& r, int i, uint32_t nblk, std::array<Cond*, 5> c) {
     if (w->cap) {
-        if (!w->errsum_ready && i >= 0 && loop_decision(r, (uint32_t)i, [] { return 0.f; }).read) {
+        if (i < 0 || loop_decision(r, (uint32_t)i, [] { return 0.f; }).read) {  // i < 0: the device decides whether it reads
             const int nf = (int)w->fluids.size();
             k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
         }
-        w->errsum_ready = false;
         Decide d{};
         for (int k = 0; k < 5; ++k)
             if (c[k]) d.h[k] = c[k]->h;
@@ -2182,7 +2168,6 @@ sph_status sph_world_create(const sph_world_desc* desc, sph_world** out) {
     ok = ok && cudaEventCreateWithFlags(&w->ev_lists, cudaEventDisableTiming) == cudaSuccess;
     ok = ok && cudaMallocHost(&w->h_pinned, 64 * sizeof(float)) == cudaSuccess;
     ok = ok && w->d_scal.ensure(16) == cudaSuccess && w->d_cnt.ensure(2) == cudaSuccess;
-    ok = ok && w->d_ticket.ensure(4) == cudaSuccess && cudaMemset(w->d_ticket.p, 0, 4 * sizeof(uint32_t)) == cudaSuccess;
     if (!ok) {
         delete w;
         return SPH_ERR_CUDA;

@@ -140,35 +140,18 @@ __device__ __forceinline__ float4 fetch4(const float4* __restrict__ a, cudaTextu
     return __ldg(&a[j]);
 }
 
-// Per-fluid deterministic error reduction: partial[block * n_fluids + f].
-// With a ticket counter the LAST block to finish also sums the partials of the whole launch in index order into
-// errsum[f] (saves a separate k_reduce_partials launch per evaluation; same fixed summation tree every run).
+// Per-fluid deterministic error reduction: partial[block * n_fluids + f], summed in index order by k_reduce_partials when the
+// error is read.  (A last-block ticket that summed them inside the pass cost every block a memory fence and an atomic on one
+// counter: 0.2-0.5 ms per evaluation at 10M particles, far more than the separate launch.)
 template <bool MULTI>
-__device__ __forceinline__ void reduce_error(float e, uint32_t fi, bool valid, float* __restrict__ partial, float* sm, uint32_t* __restrict__ ticket = nullptr,
-                                             float* __restrict__ errsum = nullptr) {
-    const int nf = MULTI ? C.n_fluids : 1;
+__device__ __forceinline__ void reduce_error(float e, uint32_t fi, bool valid, float* __restrict__ partial, float* sm) {
     if (!MULTI) {
         float s = block_sum(valid ? e : 0.f, sm);
         if (threadIdx.x == 0) partial[blockIdx.x] = s;
     } else {
-        for (int f = 0; f < nf; ++f) {
+        for (int f = 0; f < C.n_fluids; ++f) {
             float s = block_sum((valid && fi == (uint32_t)f) ? e : 0.f, sm);
-            if (threadIdx.x == 0) partial[(size_t)blockIdx.x * nf + f] = s;
-        }
-    }
-    if (ticket) {
-        __shared__ bool s_last;
-        __threadfence();
-        if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == gridDim.x - 1;
-        __syncthreads();
-        if (s_last) {
-            for (int f = 0; f < nf; ++f) {
-                float s = 0.f;
-                for (uint32_t b = threadIdx.x; b < gridDim.x; b += blockDim.x) s += __ldcg(&partial[(size_t)b * nf + f]);
-                s = block_sum(s, sm);
-                if (threadIdx.x == 0) errsum[f] = s;
-            }
-            if (threadIdx.x == 0) *ticket = 0;
+            if (threadIdx.x == 0) partial[(size_t)blockIdx.x * C.n_fluids + f] = s;
         }
     }
 }
@@ -237,7 +220,7 @@ __global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
 k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, cudaTextureObject_t tvs, const float4* __restrict__ vel,
                  const float4* __restrict__ bpos, const float4* __restrict__ bvel, Lists L, const float* __restrict__ dens,
                  const float* __restrict__ alpha, float* __restrict__ out, float* __restrict__ kappa, float* __restrict__ partial, float dt,
-                 int* __restrict__ err, uint32_t* __restrict__ ticket, float* __restrict__ errsum, Range rg) {
+                 int* __restrict__ err, Range rg) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     bool valid = i < rg.count;
@@ -281,7 +264,7 @@ k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, 
             e = d / rho0;
         }
     }
-    reduce_error<MULTI>(e, fi, valid, partial, sm, ticket, errsum);
+    reduce_error<MULTI>(e, fi, valid, partial, sm);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -340,7 +323,7 @@ __global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
 k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float2* __restrict__ vyz, cudaTextureObject_t tvyz,
                    const float4* __restrict__ bpos, const float4* __restrict__ bvel, Lists L, const float* __restrict__ dens,
                    const float* __restrict__ alpha, float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, float dt,
-                   int* __restrict__ err, uint32_t* __restrict__ ticket, float* __restrict__ errsum, Range rg) {
+                   int* __restrict__ err, Range rg) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     bool valid = i < rg.count;
@@ -388,7 +371,7 @@ k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, con
         }
         pk4[i] = make_float4(a.x, a.y, a.z, kap);
     }
-    reduce_error<false>(e, 0u, valid, partial, sm, ticket, errsum);
+    reduce_error<false>(e, 0u, valid, partial, sm);
 }
 
 // One fluid-fluid contact of Akinci2013SurfaceTension::solve (akinci2013_surface_tension.rs:113-192): the cohesion and
@@ -434,8 +417,7 @@ template <int EXTRA>
 __global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)  // 64 registers: the extra sums spill at 56
 k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float2* __restrict__ vyz, cudaTextureObject_t tvyz,
                         const float4* __restrict__ bpos, Lists L, const float* __restrict__ dens, const float* __restrict__ alpha,
-                        float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, uint32_t* __restrict__ ticket,
-                        float* __restrict__ errsum, float4* __restrict__ xs, float cf, const float4* __restrict__ nr4, float coh_norm,
+                        float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, float4* __restrict__ xs, float cf, const float4* __restrict__ nr4, float coh_norm,
                         float h6_64, Range rg) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -484,7 +466,7 @@ k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx
         pk4[i] = make_float4(a.x, a.y, a.z, d * alpha[i]);
         xs[i] = make_float4(fx, fy, fz, 0.f);
     }
-    reduce_error<false>(e, 0u, valid, partial, sm, ticket, errsum);
+    reduce_error<false>(e, 0u, valid, partial, sm);
 }
 
 // a14 pass 2 for a single uniform-mass fluid on the normals record of k_vel_update_u<.., NORMALS>: positions from pvx4

@@ -5,7 +5,9 @@ A jittered lattice at the usual spacing h/2 is sorted (a) by h-cell, z fastest, 
 in z (experiment K), (c) in "row order" (x / y binned at h/2, SALVA_B200_XYSUB=2).  Every particle's contact list is its neighbours within h in
 ascending sorted index, as k_neighbors writes them; for every interior warp of 32 consecutive particles and every list position k the script
 counts the distinct 32-byte sectors / 128-byte lines the k-th contacts of the 32 lanes fall into (records of 16 bytes), and the same per
-quarter-warp (8 lanes), which is what the L1TEX data stage appears to pay for.   usage: sim_gather_order.py [jitter amplitude in r, default 0.05]"""
+quarter-warp (8 lanes), which is what the L1TEX data stage appears to pay for.  The last table splits each list over n lanes (the split
+gather passes measured and not adopted, DESIGN.md 4a.15): a warp holds 32 / n particles, and in gather t lane u of particle p reads entry u + n t of p's list;
+counts are per 32 contacts gathered.   usage: sim_gather_order.py [jitter amplitude in r, default 0.05]"""
 import numpy as np, sys
 from scipy.spatial import cKDTree
 rng=np.random.default_rng(0)
@@ -56,3 +58,19 @@ for mode in ('h','rows'):
             ql.append(sum(len(np.unique(js[q*8:(q+1)*8]//8)) for q in range(4)))
             qs.append(sum(len(np.unique(js[q*8:(q+1)*8]//2)) for q in range(4)))
     print("jitter %.2f r  %-6s quarter-lines %.1f  quarter-sectors %.1f"%(amp,mode,np.mean(ql),np.mean(qs)))
+print("---- lanes per particle (h order): per 32 contacts, distinct 32-byte sectors / 128-byte lines / quarter-warp 128-byte lines")
+o=order('h'); rank=np.empty(len(P),int); rank[o]=np.arange(len(P))
+lists=[np.sort(rank[np.array(nb[i])]) for i in o]
+Q=P[o]; inner=np.all((Q>3*h)&(Q<hi-3*h),axis=1)
+for n in (1,2,4,8):
+    ps=32//n; sect=[];lines=[];ql=[]
+    for w0 in range(0,len(P)-ps+1,ps):
+        if not inner[w0:w0+ps].all(): continue
+        L=[lists[s] for s in range(w0,w0+ps)]
+        M=max(len(x) for x in L)
+        for t in range((M+n-1)//n):
+            js=np.array([L[l//n][l%n+n*t] if l%n+n*t<len(L[l//n]) else -1 for l in range(32)])  # lane l = (particle l // n, u = l % n)
+            on=js>=0; k=on.sum(); a=js[on]
+            sect.append(len(np.unique(a//2))*32/k); lines.append(len(np.unique(a//8))*32/k)
+            ql.append(sum(len(np.unique(js[q*8:(q+1)*8][on[q*8:(q+1)*8]]//8)) for q in range(4))*32/k)
+    print("jitter %.2f r  lanes %d (%2d particles per warp)  sectors %.1f  128-byte lines %.1f  quarter-warp lines %.1f"%(amp,n,ps,np.mean(sect),np.mean(lines),np.mean(ql)))
