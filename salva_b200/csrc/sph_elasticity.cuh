@@ -55,11 +55,10 @@ __global__ void k_el_capture_lists(Lists L, const float4* __restrict__ vel, cons
     uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
     if (t >= n) return;
     uint32_t i = slot_of[t];
-    uint32_t cnt = min(L.cnt_f[i], C.cap_f);
-    const uint32_t* base = reinterpret_cast<const uint32_t*>(L.nbr_f);
+    uint32_t cnt = L.fluid_count(i);
     uint32_t k0 = 0;
     for (uint32_t k = 0; k < cnt; ++k) {
-        uint32_t j = base[((size_t)(k >> 2) * C.stride + i) * 4 + (k & 3)];
+        uint32_t j = L.fluid(i, k);
         if (fid_of(vel[j]) != which) continue;
         if (k0 < cap0) nbr0[(size_t)k0 * stride0 + t] = orig[j] - lo;
         ++k0;

@@ -126,6 +126,23 @@ struct Tex {
     }
 };
 
+// The neighbour lists (layout: sph_lists.cuh) and their capacities in rows.  The constants carry the capacities: grow_lists()
+// raises them.
+struct ListState {
+    DBuf<uint32_t> nbr_f, nbr_b, cnt_f, cnt_b;
+    uint32_t cap_f = 64, cap_b = 32;
+    Lists view() const { return out().view(); }
+    ListsOut out() const { return {nbr_f.p, nbr_b.p, cnt_f.p, cnt_b.p}; }
+    // counts for n particles, and cap_f / cap_b rows of `stride` entries (sph_world::stride)
+    cudaError_t ensure(size_t n, uint32_t stride) {
+        cudaError_t e = cnt_f.ensure(n);
+        if (e == cudaSuccess) e = cnt_b.ensure(n);
+        if (e == cudaSuccess) e = nbr_f.ensure((size_t)cap_f * stride);
+        if (e == cudaSuccess) e = nbr_b.ensure((size_t)cap_b * stride);
+        return e;
+    }
+};
+
 // Solver and plugin scratch.  The kernels take the raw pointers (.p).
 struct IisphState {
     DBuf<float4> dii;      // iisph_solver.rs:32
@@ -507,7 +524,7 @@ struct sph_world {
     DBuf<float4> vs, acc, normals, dbg_acc;
     DBuf<float> dens, alpha, kappa, divv, pred, bvol, bforce;
     DBuf<uint32_t> cid, rank, perm, cstart, bcid, brank, bperm, bstart, scan_aux[3], scan_aux_k[3];
-    DBuf<uint32_t> nbr_f, nbr_b, cnt_f, cnt_b;
+    ListState lists;
     // uniform-mass packed gather records (sph_passes.cuh): pvx4 = (x,y,z,v*x), vyz2 = (v*y,v*z), pk4 = (x,y,z,kappa); their
     // gathers are split evenly over the texture and LSU pipes (even / odd contacts)
     bool unimass = false;
@@ -540,7 +557,7 @@ struct sph_world {
     std::vector<Span> spans;
     size_t n_spans = 0;
 
-    uint32_t cap_f = 64, cap_b = 32, stride = 0;
+    uint32_t stride = 0;  // per-particle plane stride (Consts::stride)
     bool lists_valid = false;
     // cell-coordinate AABB of the positions the last step wrote (k_update_positions): sizes the next grid without a bounds pass
     bool nb_valid = false, nb_pending = false;
@@ -708,8 +725,19 @@ void fill_static_consts(sph_world* w) {
         c.fluids[f] = {w->fluids[f].density0, w->fluids[f].memberships, w->fluids[f].filter, w->fluids[f].uniform_mass};
     for (size_t b = 0; b < w->bounds.size(); ++b) c.bounds[b] = {w->bounds[b].memberships, w->bounds[b].filter};
     c.stride = w->stride;
-    c.cap_f = w->cap_f;
-    c.cap_b = w->cap_b;
+    c.cap_f = w->lists.cap_f;
+    c.cap_b = w->lists.cap_b;
+}
+
+// Raises the list capacities to at least cf / cb rows, grows the lists and refreshes the constants that carry the capacities.
+sph_status grow_lists(sph_world* w, uint32_t cf, uint32_t cb) {
+    ListState& L = w->lists;
+    if (cf <= L.cap_f && cb <= L.cap_b) return SPH_OK;
+    L.cap_f = std::max(L.cap_f, cf);
+    L.cap_b = std::max(L.cap_b, cb);
+    CU(L.ensure(0, w->stride));  // (the counts keep their size)
+    fill_static_consts(w);
+    return upload_consts(w);
 }
 
 // ---- exclusive scan over n u32 (in place) -------------------------------------------------------
@@ -829,11 +857,8 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     CU(w->cid.ensure(N));
     CU(w->rank.ensure(N));
     CU(w->perm.ensure(N));
-    CU(w->cnt_f.ensure(N));
-    CU(w->cnt_b.ensure(N));
     w->stride = (uint32_t)((N + 31) / 32 * 32);
-    CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
-    CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
+    CU(w->lists.ensure(N, w->stride));
     uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
     CU(w->partial.ensure((size_t)(nblk + 3) * std::max<size_t>(1, w->fluids.size())));  // +3: a slab pass may run as three sub-range launches
     CU(w->errsum.ensure(MAX_FLUIDS));
@@ -1158,8 +1183,8 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     const bool dens = N && w->desc.solver == SPH_SOLVER_DFSPH, uni = dens && w->unimass;
     DensArgs D{};
     if (dens) TRY(density_args(w, &D));
-    using NbrKernel = void (*)(const float4*, const float4*, const uint32_t*, const float4*, const float4*, const uint32_t*, uint32_t*,
-                               uint32_t*, uint32_t*, uint32_t*, uint32_t*, DensArgs);
+    using NbrKernel = void (*)(const float4*, const float4*, const uint32_t*, const float4*, const float4*, const uint32_t*, ListsOut,
+                               uint32_t*, DensArgs);
     NbrKernel search;
     if (w->hc.xysub > 1) {  // row order
         if (multi) search = dens ? k_neighbors_xy<true, true, false> : k_neighbors_xy<true, false, false>;
@@ -1186,10 +1211,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     for (int attempt = 0; attempt < 8 && N; ++attempt) {
         CU(cudaMemsetAsync(w->d_scal.p + 8, 0, 2 * sizeof(int), w->st));
         uint32_t* maxcnt = reinterpret_cast<uint32_t*>(w->d_scal.p + 8);
-        LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->nbr_f.p, w->nbr_b.p,
-               w->cnt_f.p, w->cnt_b.p, maxcnt, D);
+        LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->lists.out(), maxcnt, D);
         if (w->cap) {  // a step graph checks the capacities on the device and skips the rest of the step past them
-            k_lists_check<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_scal.p, w->cap_f, w->cap_b, w->graphs.h_lists);
+            k_lists_check<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_scal.p, w->lists.cap_f, w->lists.cap_b, w->graphs.h_lists);
             break;
         }
         int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous
@@ -1203,28 +1227,16 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
         w->stats.max_neighbors = (uint32_t)hs[1];
         w->max_nb_b = (uint32_t)hs[2];
-        bool grow = false;
-        if ((uint32_t)hs[1] > w->cap_f) {
-            w->cap_f = ((uint32_t)hs[1] + 15) / 16 * 16;
-            grow = true;
-        }
-        if ((uint32_t)hs[2] > w->cap_b) {
-            w->cap_b = ((uint32_t)hs[2] + 15) / 16 * 16;
-            grow = true;
-        }
-        if (!grow) break;
+        if ((uint32_t)hs[1] <= w->lists.cap_f && (uint32_t)hs[2] <= w->lists.cap_b) break;
         if (speculative) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded density pass or sweep
-        CU(w->nbr_f.ensure((size_t)w->cap_f * w->stride));
-        CU(w->nbr_b.ensure((size_t)w->cap_b * w->stride));
-        fill_static_consts(w);
-        TRY(upload_consts(w));
+        TRY(grow_lists(w, ((uint32_t)hs[1] + 15) / 16 * 16, ((uint32_t)hs[2] + 15) / 16 * 16));
     }
     if (!N) {  // boundaries only
         TRY(ev_record(w, EV_NBR));
         if (speculative) TRY(speculative(w));
     }
     if (N) {
-        k_sum_u32<<<std::min<uint32_t>(cdiv(N, 256), 1184), 256, 0, w->st>>>((uint32_t)N, w->cnt_f.p + w->own_begin, w->cnt_b.p + w->own_begin,
+        k_sum_u32<<<std::min<uint32_t>(cdiv(N, 256), 1184), 256, 0, w->st>>>((uint32_t)N, w->lists.cnt_f.p + w->own_begin, w->lists.cnt_b.p + w->own_begin,
                                                                              w->d_cnt.p + 1);
         w->launches++;
     }
@@ -1327,7 +1339,7 @@ sph_status launch_density_alpha(sph_world* w) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
-    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
+    const Lists L = w->lists.view();
     DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, w->d_scal.p + 7);
     return SPH_OK;  // the ghost refresh of rho follows in post_density_refresh(), once the list-capacity check has passed
 }
@@ -1440,7 +1452,7 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
     const bool multi = w->fluids.size() > 1;
     const bool xsf = !predict && xsph_fusable(w), akf = !predict && akinci;
     if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
-    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
+    const Lists L = w->lists.view();
     if (w->unimass) {
         CU(w->tex_pvx.bind(w->pvx4));
         CU(w->tex_vyz.bind(w->vyz2));
@@ -1482,7 +1494,7 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
 sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
-    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
+    const Lists L = w->lists.view();
     if (w->unimass) CU(w->tex_pk.bind(w->pk4));
     if (normals) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
     // the following evaluation gathers v*_j of ghosts (vs itself too: the velocity fold reads vel = v* for ghosts)
@@ -1512,8 +1524,8 @@ sph_status materialise_contacts(sph_world* w, uint32_t f, int which, HostContact
     const size_t N = w->N, Nf = fl.n;
     const int c = w->cur, bc = w->bcur;
     const uint32_t ob = w->own_begin;
-    const uint32_t cap = which ? w->cap_b : w->cap_f;
-    const uint32_t* cnt = which ? w->cnt_b.p : w->cnt_f.p;
+    const uint32_t cap = which ? w->lists.cap_b : w->lists.cap_f;
+    const uint32_t* cnt = which ? w->lists.cnt_b.p : w->lists.cnt_f.p;
     CU(w->ct_cnt[which].ensure(N + 1));
     LAUNCH(k_contacts_count, N, 256, (uint32_t)N, w->orig[c].p + ob, cnt + ob, cap, w->ct_cnt[which].p);
     CU(cudaMemsetAsync(w->ct_cnt[which].p + N, 0, sizeof(uint32_t), w->st));
@@ -1532,11 +1544,11 @@ sph_status materialise_contacts(sph_world* w, uint32_t f, int which, HostContact
     if (which) {
         for (size_t b = 0; b < w->bounds.size(); ++b) tab.off[b] = (uint32_t)w->bounds[b].offset;
         if (w->B)
-            LAUNCH((k_contacts_fill<true>), N, 128, (uint32_t)N, w->pos[c].p, w->bpos[bc].p, w->bvel[bc].p, w->orig[c].p, w->borig[bc].p, w->nbr_b.p, cnt, cap,
+            LAUNCH((k_contacts_fill<true>), N, 128, (uint32_t)N, w->pos[c].p, w->bpos[bc].p, w->bvel[bc].p, w->orig[c].p, w->borig[bc].p, w->lists.view(),
                    w->ct_cnt[which].p, tab, w->ct_j[which].p, w->ct_model[which].p, w->ct_w[which].p, w->ct_g[which].p);
     } else {
         for (size_t k = 0; k < w->fluids.size(); ++k) tab.off[k] = (uint32_t)w->fluids[k].offset;
-        LAUNCH((k_contacts_fill<false>), N, 128, (uint32_t)N, w->pos[c].p, w->pos[c].p, w->vel[c].p, w->orig[c].p, w->orig[c].p, w->nbr_f.p, cnt, cap,
+        LAUNCH((k_contacts_fill<false>), N, 128, (uint32_t)N, w->pos[c].p, w->pos[c].p, w->vel[c].p, w->orig[c].p, w->orig[c].p, w->lists.view(),
                w->ct_cnt[which].p, tab, w->ct_j[which].p, w->ct_model[which].p, w->ct_w[which].p, w->ct_g[which].p);
     }
     const uint32_t first = scan[0], nent = scan[Nf] - scan[0];
@@ -1618,7 +1630,7 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
-    Lists L{reinterpret_cast<const uint4*>(w->nbr_f.p), w->nbr_b.p, w->cnt_f.p, w->cnt_b.p};
+    const Lists L = w->lists.view();
     for (size_t f = 0; f < w->fluids.size(); ++f)
         for (ForceRec& fr : w->fluids[f].forces) {
             const float* p = fr.d.p;
@@ -2633,8 +2645,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl.p + ob, w->o_c.p);
     else if (what == SPH_DBG_VISC_BETA) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 36u, w->stride, og, w->visc.beta.p + ob, w->o_c.p);
     else if (what == SPH_DBG_VISC_TARGET) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 6u, w->stride, og, w->visc.target.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_f.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->cnt_b.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->lists.cnt_f.p + ob, w->o_c.p);
+    else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->lists.cnt_b.p + ob, w->o_c.p);
     else return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);
     CU(cudaMemcpyAsync(out, w->o_c.p + width * f.offset, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
     CU(cudaStreamSynchronize(w->st));

@@ -7,11 +7,7 @@
 //   vc4   : velocity_changes       (dfsph_solver.rs:44)
 //   vs4   : v* = vel + vc          (materialised so gather passes read ONE vector per neighbour)
 //   bpos4 : boundary x, y, z, volume (dfsph_solver.rs:72-96);  bvel4: boundary velocity, boundary id
-// Neighbour lists ("contacts", contacts.rs:83-87) are index-only and column-major:
-//   nbr_f[((k / 4) * stride + i) * 4 + k % 4] = sorted index of the k-th fluid neighbour of i (self included,
-//   ascending j): groups of 4 contacts are interleaved so a thread fetches 4 indices with one coalesced LDG.128;
-//   nbr_b[k * stride + i] likewise (scalar) for boundary particles; W and grad W are recomputed from pos4 in
-//   every pass (cheaper than streaming cached 16-byte contacts from HBM: see DESIGN.md).
+// The neighbour lists' layout is sph_lists.cuh's.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -53,14 +49,21 @@ struct Consts {
     uint32_t n_fluid, n_bound;   // particle totals (n_fluid counts owned + ghost slots of the sorted arrays)
     uint32_t i_begin, n_owned;   // owned slots [i_begin, i_begin + n_owned): everything on one GPU; the slab between the
                                  // two ghost columns in a multi-GPU world (x-major order keeps ghosts at both ends)
-    uint32_t stride;             // neighbour-list column stride (>= n_fluid, multiple of 32)
-    uint32_t cap_f, cap_b;       // list capacities (rows)
+    uint32_t stride;             // the world's per-particle plane stride (>= n_fluid, multiple of 32): neighbour-list rows,
+                                 // DFSPHViscosity's beta / target planes
+    uint32_t cap_f, cap_b;       // neighbour-list capacities (rows)
     int n_fluids, n_bounds;      // object counts
     FluidParams fluids[MAX_FLUIDS];
     BoundaryParams bounds[MAX_BOUNDARIES];
 };
 
 __constant__ Consts C;
+
+}  // namespace sphk
+
+#include "sph_lists.cuh"
+
+namespace sphk {
 
 // ------------------------------------------------------------------------------------------------
 // geometry helpers
@@ -625,7 +628,7 @@ __device__ __forceinline__ void density_alpha_div(uint32_t i, bool valid, uint32
             vi = Vel3{s.x, s.y, s.z};
         }
         float rho = 0.f, sq = 0.f, gx = 0.f, gy = 0.f, gz = 0.f, d = 0.f;
-        const uint32_t n = min(nf, C.cap_f);
+        const uint32_t n = fluid_stored(nf);
         const uint32_t nq = (n + 3u) >> 2;
         uint4 J = nq ? group(0u) : make_uint4(i, i, i, i);
         for (uint32_t q = 0; q < nq; ++q) {
@@ -666,7 +669,7 @@ __device__ __forceinline__ void density_alpha_div(uint32_t i, bool valid, uint32
             }
             J = Jn;
         }
-        const uint32_t m = min(nb, C.cap_b);
+        const uint32_t m = boundary_stored(nb);
         for (uint32_t k = 0; k < m; ++k) {
             const float4 pj = __ldg(&bpos[bentry(k)]);
             const Pair p = make_pair<true, true>(pi, pj);
@@ -720,7 +723,7 @@ __device__ __forceinline__ void density_alpha_div(uint32_t i, bool valid, uint32
 // kernel, with the lanes of a warp at different k: the sectors being filled (~29 MB at 10M particles) do not fit H100's L2.
 // Staged, entry k of a lane is one STS at row k, column lane (bank-conflict-free whatever k each lane is at); the write-out
 // then stores group g of 32 consecutive particles as 32 x 16 contiguous bytes, and boundary row k as 32 x 4.
-// Entries past the staging rows go straight to their place in global memory, so any cap_f / cap_b works (list regrow
+// Entries past the staging rows go straight to their place in global memory, so any capacity works (list regrow
 // included) while the shared-memory size stays fixed.  The row counts trade the share of staged entries against occupancy:
 // 32 + 8 rows (20 KB per block) leave 10 blocks per SM, as many as the registers allow; at C3 (~33 contacts on average,
 // up to ~51) 48 + 16 rows (6 blocks) made the search 26 % slower, 40 + 8 (9 blocks) 1 % slower (DESIGN.md §4a.11).
@@ -735,8 +738,7 @@ constexpr uint32_t NBR_SF = 32, NBR_SB = 8;  // staged fluid / boundary rows per
 template <bool MULTI, bool STAGE, bool DENS, bool UNI, class Runs>
 __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                                                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-                                               uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f,
-                                               uint32_t* __restrict__ cnt_b, uint32_t* __restrict__ maxcnt, const DensArgs& D, Runs runs) {
+                                               const ListsOut& out, uint32_t* __restrict__ maxcnt, const DensArgs& D, Runs runs) {
     __shared__ uint32_t stage[NBR_T / 32][NBR_SF + NBR_SB][32];
     __shared__ uint32_t arrived;  // DENS: warps of the block done with their density sweep
     if (DENS) {
@@ -763,7 +765,7 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
                 },
                 [&](uint32_t j) {
                     if (STAGE && nf < NBR_SF) sf[nf][lane] = j;
-                    else if (nf < C.cap_f) nbr_f[((size_t)(nf >> 2) * C.stride + i) * 4 + (nf & 3)] = j;
+                    else out.fluid(i, nf, j);
                     ++nf;
                 });
             if (C.n_bound)
@@ -775,25 +777,22 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
                     },
                     [&](uint32_t j) {
                         if (STAGE && nb < NBR_SB) sb[nb][lane] = j;
-                        else if (nb < C.cap_b) nbr_b[(size_t)nb * C.stride + i] = j;
+                        else out.boundary(i, nb, j);
                         ++nb;
                     });
         });
-        // write-out: the last group is padded with i; cap_f and NBR_SF are multiples of 4, so a staged group is whole
+        // write-out: the last group is padded with i; the capacities and NBR_SF are multiples of 4, so a staged group is whole
         if (STAGE) {
-            const uint32_t sfn = min(nf, min(NBR_SF, C.cap_f));
-            uint4* out = reinterpret_cast<uint4*>(nbr_f) + i;
-            for (uint32_t k = 0; k < sfn; k += 4, out += C.stride) {
+            const uint32_t sfn = min(fluid_stored(nf), NBR_SF);
+            for (uint32_t k = 0; k < sfn; k += 4) {
                 const uint32_t a = sf[k][lane], b = sf[k + 1][lane], c = sf[k + 2][lane], d = sf[k + 3][lane];
-                *out = make_uint4(a, k + 1 < nf ? b : i, k + 2 < nf ? c : i, k + 3 < nf ? d : i);
+                out.group(i, k >> 2, make_uint4(a, k + 1 < nf ? b : i, k + 2 < nf ? c : i, k + 3 < nf ? d : i));
             }
-            const uint32_t sbn = min(nb, min(NBR_SB, C.cap_b));
-            for (uint32_t k = 0; k < sbn; ++k) nbr_b[(size_t)k * C.stride + i] = sb[k][lane];
+            const uint32_t sbn = min(boundary_stored(nb), NBR_SB);
+            for (uint32_t k = 0; k < sbn; ++k) out.boundary(i, k, sb[k][lane]);
         }
-        for (uint32_t t = STAGE ? max(nf, NBR_SF) : nf; t < ((nf + 3u) & ~3u) && t < C.cap_f; ++t)  // pad the last group unless staged
-            nbr_f[((size_t)(t >> 2) * C.stride + i) * 4 + (t & 3)] = i;
-        cnt_f[i] = nf;
-        cnt_b[i] = nb;
+        out.pad(i, STAGE ? max(nf, NBR_SF) : nf, nf);  // pad the last group unless staged
+        out.counts(i, nf, nb);
     }
     uint32_t mf = nf, mb = nb;
     for (int o = 16; o > 0; o >>= 1) {
@@ -805,15 +804,15 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
         if (mb) atomicMax(&maxcnt[1], mb);
     }
     if constexpr (DENS) {
-        const uint4* const col = reinterpret_cast<const uint4*>(nbr_f) + i;
+        const Lists L = out.view();
         density_alpha_div<MULTI, UNI>(
             i, owned, nf, nb, vel, bpos, D, arrived,
             [&](uint32_t q) {
                 const uint32_t k = q * 4u;
                 if (STAGE && k < NBR_SF) return make_uint4(sf[k][lane], sf[k + 1][lane], sf[k + 2][lane], sf[k + 3][lane]);
-                return __ldcs(col + (size_t)q * C.stride);  // this thread's own stores above
+                return L.group(i, q);  // this thread's own stores above
             },
-            [&](uint32_t k) { return STAGE && k < NBR_SB ? sb[k][lane] : nbr_b[(size_t)k * C.stride + i]; });
+            [&](uint32_t k) { return STAGE && k < NBR_SB ? sb[k][lane] : L.boundary(i, k); });
     }
 }
 
@@ -823,9 +822,8 @@ template <bool MULTI, bool DENS = false, bool UNI = false>
 __global__ void __launch_bounds__(NBR_T, !DENS || SPH_GENERIC_KERNELS ? 1 : MULTI ? 8 : 9)
 k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
             const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-            uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
-            uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
-    neighbor_lists<MULTI, true, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, D, [](const float4& pi, auto&& visit) {
+            ListsOut out, uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+    neighbor_lists<MULTI, true, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, out, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         for (int ax = -1; ax <= 1; ++ax)
             for (int ay = -1; ay <= 1; ++ay) visit(cell_id(cx + ax, cy + ay, cz - 1));  // the z-run of cells cz-1..cz+1
@@ -840,9 +838,8 @@ template <bool MULTI, bool DENS = false, bool UNI = false>
 __global__ void
 k_neighbors_xy(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-               uint32_t* __restrict__ nbr_f, uint32_t* __restrict__ nbr_b, uint32_t* __restrict__ cnt_f, uint32_t* __restrict__ cnt_b,
-               uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
-    neighbor_lists<MULTI, false, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, nbr_f, nbr_b, cnt_f, cnt_b, maxcnt, D, [](const float4& pi, auto&& visit) {
+               ListsOut out, uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+    neighbor_lists<MULTI, false, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, out, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         int xlo, xhi, ylo, yhi;
         arun(pi.x, cx, C.xysub, C.xysub_f, xlo, xhi);
@@ -1428,17 +1425,17 @@ __global__ void k_contacts_count(uint32_t n, const uint32_t* __restrict__ orig, 
 // one thread per sorted slot: writes its particle's contacts at scan[orig[s]]..
 template <bool BOUNDARY>
 __global__ void k_contacts_fill(uint32_t n, const float4* __restrict__ pos, const float4* __restrict__ other_pos, const float4* __restrict__ other_vel,
-                                const uint32_t* __restrict__ orig, const uint32_t* __restrict__ other_orig, const uint32_t* __restrict__ nbr,
-                                const uint32_t* __restrict__ cnt, uint32_t cap, const uint32_t* __restrict__ scan, OffsetTable tab, uint32_t* __restrict__ out_j,
+                                const uint32_t* __restrict__ orig, const uint32_t* __restrict__ other_orig, Lists L,
+                                const uint32_t* __restrict__ scan, OffsetTable tab, uint32_t* __restrict__ out_j,
                                 uint32_t* __restrict__ out_model, float* __restrict__ out_w, float* __restrict__ out_g) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     const uint32_t i = s + C.i_begin;
     const float4 pi = pos[i];
-    const uint32_t m = min(cnt[i], cap);
+    const uint32_t m = BOUNDARY ? L.boundary_count(i) : L.fluid_count(i);
     size_t base = scan[orig[i]];
     for (uint32_t k = 0; k < m; ++k) {
-        const uint32_t j = BOUNDARY ? nbr[(size_t)k * C.stride + i] : nbr[((size_t)(k >> 2) * C.stride + i) * 4 + (k & 3)];
+        const uint32_t j = BOUNDARY ? L.boundary(i, k) : L.fluid(i, k);
         const float4 pj = other_pos[j];
         const Pair p = make_pair<true, true>(pi, pj);
         const uint32_t model = fid_of(other_vel[j]);

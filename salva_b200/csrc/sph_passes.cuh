@@ -13,14 +13,6 @@
 
 namespace sphk {
 
-struct Lists {
-    const uint4* nbr_f;     // nbr_f[(k / 4) * stride + i] = contacts 4*(k/4) .. 4*(k/4)+3 of particle i (sorted indices);
-                            // tail slots of the last group hold i itself (a self contact has zero gradient)
-    const uint32_t* nbr_b;  // nbr_b[k * stride + i]
-    const uint32_t* cnt_f;
-    const uint32_t* cnt_b;
-};
-
 struct NoAux {};
 
 // Gather lambdas may take the contact's position u in its group of four as a second argument: kernels use it to send the
@@ -38,21 +30,16 @@ struct Range {
     uint32_t begin, count;
 };
 
-// The contact lists are streamed exactly once per pass: load them with the evict-first policy so they do not push the
-// gathered particle data out of L1/L2.
-__device__ __forceinline__ uint4 ld_list(const uint4* p) { return __ldcs(p); }
-
 // ldpos(j) -> float4 whose xyz is the neighbour position (w = whatever the array packs there); ld(j) -> Aux loads
 // whatever else the pass needs from neighbour j; ff(j, pair, posrec_j, aux) consumes one contact.
 template <bool W, bool G, class LP, class LD, class FF>
 __device__ __forceinline__ void for_fluid_contacts_g(uint32_t i, const float4& pi, const Lists& L, LP ldpos, LD ld, FF ff) {
-    const uint32_t n = min(L.cnt_f[i], C.cap_f);
+    const uint32_t n = L.fluid_count(i);
     const uint32_t nq = (n + 3u) >> 2;
-    const uint4* col = L.nbr_f + i;
-    uint4 J = nq ? ld_list(col) : make_uint4(i, i, i, i);
+    uint4 J = nq ? L.group(i, 0) : make_uint4(i, i, i, i);
     for (uint32_t q = 0; q < nq; ++q) {
         uint4 Jn = J;
-        if (q + 1 < nq) Jn = ld_list(col + (size_t)(q + 1) * C.stride);  // fetch the next group of indices early
+        if (q + 1 < nq) Jn = L.group(i, q + 1);  // fetch the next group of indices early
         uint32_t j[4] = {J.x, J.y, J.z, J.w};
         const uint32_t k0 = q * 4u;
         bool ok[4];
@@ -87,14 +74,13 @@ __device__ __forceinline__ void for_fluid_contacts_g(uint32_t i, const float4& p
 template <bool NEED_W = false, int BATCH = 4, class LP, class LD, class FF>
 __device__ __forceinline__ void for_fluid_grads(uint32_t i, const float4& pi, const Lists& L, LP ldpos, LD ld, FF ff) {
     static_assert(BATCH == 2 || BATCH == 4, "a group of four contacts is split into whole batches");
-    const uint32_t n = min(L.cnt_f[i], C.cap_f);
+    const uint32_t n = L.fluid_count(i);
     const uint32_t nq = (n + 3u) >> 2;
     if (nq == 0) return;
-    const uint4* col = L.nbr_f + i;
-    uint4 J = ld_list(col);
+    uint4 J = L.group(i, 0);
     for (uint32_t q = 0; q < nq; ++q) {
         uint4 Jn = J;
-        if (q + 1 < nq) Jn = ld_list(col + (size_t)(q + 1) * C.stride);  // fetch the next group early
+        if (q + 1 < nq) Jn = L.group(i, q + 1);  // fetch the next group early
         const uint32_t j[4] = {J.x, J.y, J.z, J.w};
 #pragma unroll
         for (int u0 = 0; u0 < 4; u0 += BATCH) {
@@ -124,10 +110,9 @@ __device__ __forceinline__ void for_fluid_contacts(uint32_t i, const float4& pi,
 }
 template <bool W, bool G, class FB>
 __device__ __forceinline__ void for_boundary_contacts(uint32_t i, const float4& pi, const Lists& L, const float4* __restrict__ bpos, FB fb) {
-    uint32_t n = min(L.cnt_b[i], C.cap_b);
-    const uint32_t* col = L.nbr_b + i;
+    uint32_t n = L.boundary_count(i);
     for (uint32_t k = 0; k < n; ++k) {
-        uint32_t j = col[(size_t)k * C.stride];
+        uint32_t j = L.boundary(i, k);
         float4 pj = __ldg(&bpos[j]);
         Pair p = make_pair<W, G>(pi, pj);
         fb(j, p, pj);
@@ -168,13 +153,14 @@ k_density_alpha(const float4* __restrict__ pos, const float4* __restrict__ vel, 
     float rho0 = C.fluids[MULTI ? fid_of(vel[i]) : 0].density0;
     float rho = 0.f, sq = 0.f, gx = 0.f, gy = 0.f, gz = 0.f;
     {
-        const uint32_t n = min(L.cnt_f[i], C.cap_f);
+        // Not for_fluid_contacts: masking the tail slots before the gathers made this pass 1 % slower at C5's 2M particles
+        // (H100 80GB HBM3, 700 W); the slots already hold i itself.
+        const uint32_t n = L.fluid_count(i);
         const uint32_t nq = (n + 3u) >> 2;
-        const uint4* col = L.nbr_f + i;
-        uint4 J = nq ? ld_list(col) : make_uint4(i, i, i, i);
+        uint4 J = nq ? L.group(i, 0) : make_uint4(i, i, i, i);
         for (uint32_t q = 0; q < nq; ++q) {
             uint4 Jn = J;
-            if (q + 1 < nq) Jn = ld_list(col + (size_t)(q + 1) * C.stride);
+            if (q + 1 < nq) Jn = L.group(i, q + 1);
             const uint32_t j[4] = {J.x, J.y, J.z, J.w};
             float4 pj[4];
 #pragma unroll
@@ -233,7 +219,7 @@ k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, 
         fi = MULTI ? fid_of(vel[i]) : 0u;
         float rho0 = C.fluids[fi].density0;
         float d = 0.f;
-        if (PREDICT || L.cnt_f[i] + L.cnt_b[i] >= 20u) {
+        if (PREDICT || L.gate_count(i) >= 20u) {
             for_fluid_grads_pos(
                 i, pi, L, pos, [&](uint32_t j) { return tex1Dfetch<float4>(tvs, (int)j); },
                 [&](uint32_t, const Pair& p, const float4& pj, const float4& vj) {
@@ -336,7 +322,7 @@ k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, con
         const float vix = a.w, viy = b.x, viz = b.y;
         const float rho0 = C.fluids[0].density0, mass = C.fluids[0].mass;
         float d = 0.f;
-        if (PREDICT || L.cnt_f[i] + L.cnt_b[i] >= 20u) {
+        if (PREDICT || L.gate_count(i) >= 20u) {
             // even contacts fetch (pvx via TEX, vyz via LSU), odd ones the other way round, so both pipes carry the same load
             for_fluid_grads(
                 i, pi, L, [&](uint32_t j, int u) { return !(u & 1) ? tex1Dfetch<float4>(tpvx, (int)j) : __ldg(&pvx[j]); },
@@ -430,7 +416,7 @@ k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx
         const float4 pi = make_float4(a.x, a.y, a.z, 0.f);
         const float vix = a.w, viy = b.x, viz = b.y;
         const float rho0 = C.fluids[0].density0, mass = C.fluids[0].mass;
-        const bool gated = L.cnt_f[i] + L.cnt_b[i] < 20u;  // dfsph_solver.rs:301-314
+        const bool gated = L.gate_count(i) < 20u;  // dfsph_solver.rs:301-314
         float4 ni;
         if (EXTRA == 2) ni = nr4[i];
         float d = 0.f, fx = 0.f, fy = 0.f, fz = 0.f;
