@@ -546,8 +546,7 @@ struct sph_world {
     DBuf<float> partial, errsum;
     DBuf<int> d_scal;  // [0..6] bounds + bad flag, [7] error flag, [8..9] maxcnt, [11] elasticity widest, [12] CFL max |v + a R|^2
     DBuf<unsigned long long> d_cnt;  // [0] bb contacts, [1] ff+fb contacts
-    DBuf<float> o_a, o_b, o_c, o_mass;  // staging, original order
-    DBuf<uint32_t> o_fid;
+    DBuf<uint32_t> rows_scratch;  // caller-order rows of export_rows / import_rows, one region per column
     IisphState iisph;
     ViscosityState visc;
     float* h_pinned = nullptr;  // 64 floats of pinned host memory for small read-backs
@@ -784,6 +783,95 @@ sph_status scan_exclusive_k(sph_world* w, ScanSet<K> arrays, size_t n, int level
     return SPH_OK;
 }
 
+// ---- sorted order <-> caller order (layout: sph_order.cuh) --------------------------------------------
+// One column of an export: `src` read over the sorted slots [s0, s0 + n) (a null orig maps slot s to row s).  The caller
+// rows [first, first + count) are copied to `host`; or, with `dev` set, every row is written straight into that device array.
+template <class V>
+struct Col {
+    V src;
+    const uint32_t* orig;
+    uint32_t s0, n;
+    size_t first, count;
+    typename V::T* host;
+    typename V::T* dev = nullptr;
+};
+// fluid rows, from the slots this GPU owns
+template <class V>
+Col<V> fluid_col(const sph_world* w, V src, size_t first, size_t count, typename V::T* host) {
+    return {src, w->orig[w->cur].p, w->own_begin, (uint32_t)w->N, first, count, host};
+}
+// boundary rows, from every boundary slot
+template <class V>
+Col<V> boundary_col(const sph_world* w, V src, size_t first, size_t count, typename V::T* host) {
+    return {src, w->borig[w->bcur].p, 0u, (uint32_t)w->B, first, count, host};
+}
+
+// At least `words` 4-byte words of rows_scratch.  It grows to the request exactly, without DBuf's headroom: a world never
+// holds more of it than the largest single call needed (stage_up's 11 words per particle, or a wide debug read's 36).
+// Every call that uses it is done with it when it returns: export_rows and import_rows end in a stream synchronise.
+sph_status ensure_rows_scratch(sph_world* w, size_t words) {
+    if (words > w->rows_scratch.cap) {
+        w->rows_scratch.release();
+        CU(w->rows_scratch.ensure(words));
+    }
+    return SPH_OK;
+}
+
+// Enqueues every column's export and host copy, each host column in a region of its own, then synchronises if any
+// column went to the host.
+template <class... V>
+sph_status export_rows(sph_world* w, const Col<V>&... cols) {
+    size_t words = 0;
+    ((words += cols.dev ? 0 : cols.src.width * (size_t)cols.n), ...);
+    const bool to_host = (!cols.dev || ...);
+    TRY(ensure_rows_scratch(w, words));
+    size_t at = 0;
+    auto one = [&](const auto& col) -> sph_status {
+        using View = std::decay_t<decltype(col.src)>;
+        using T = typename View::T;
+        static_assert(sizeof(T) == sizeof(uint32_t), "rows_scratch holds 4-byte values");
+        T* dst = col.dev ? col.dev : reinterpret_cast<T*>(w->rows_scratch.p + at);
+        LAUNCH(k_export<View>, col.n, 256, col.n, col.s0, col.orig, col.src, dst);
+        if (col.dev) return SPH_OK;
+        const size_t width = col.src.width;
+        CU(cudaMemcpyAsync(col.host, dst + width * col.first, width * col.count * sizeof(T), cudaMemcpyDeviceToHost, w->st));
+        at += width * col.n;
+        return SPH_OK;
+    };
+    sph_status s = SPH_OK;
+    if (!(((s = one(cols)) == SPH_OK) && ...)) return s;
+    if (to_host) CU(cudaStreamSynchronize(w->st));
+    return SPH_OK;
+}
+
+// The mirror: caller rows [first, first + count) from the host into the slots this GPU owns (k_import), then a stream
+// synchronise.  Any source may be null; the velocity changes land in `vc` (a host force writes accelerations back there).
+struct ImportRows {
+    const float *pos = nullptr, *vel = nullptr, *vc = nullptr, *mass = nullptr;
+    const uint32_t* fid = nullptr;
+};
+sph_status import_rows(sph_world* w, const ImportRows& in, size_t first, size_t count, float4* vc) {
+    const void* src[5] = {in.pos, in.vel, in.vc, in.mass, in.fid};
+    const size_t width[5] = {3, 3, 3, 1, 1};
+    size_t words = 0;
+    for (int a = 0; a < 5; ++a) words += src[a] ? width[a] * count : 0;
+    TRY(ensure_rows_scratch(w, words));
+    const void* dev[5] = {};
+    size_t at = 0;
+    for (int a = 0; a < 5; ++a)
+        if (src[a]) {
+            dev[a] = w->rows_scratch.p + at;
+            CU(cudaMemcpyAsync(w->rows_scratch.p + at, src[a], width[a] * count * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
+            at += width[a] * count;
+        }
+    const int c = w->cur;
+    auto f = [&](int a) { return static_cast<const float*>(dev[a]); };
+    LAUNCH(k_import, w->N, 256, (uint32_t)w->N, w->own_begin, w->orig[c].p, f(0), f(1), f(2), f(3), static_cast<const uint32_t*>(dev[4]), w->pos[c].p,
+           w->vel[c].p, vc, (uint32_t)first, (uint32_t)(first + count));
+    CU(cudaStreamSynchronize(w->st));
+    return SPH_OK;
+}
+
 // ---- host <-> device staging --------------------------------------------------------------------
 // Device holds the truth -> pull everything back into the host vectors (original order).
 sph_status stage_down(sph_world* w) {
@@ -791,24 +879,14 @@ sph_status stage_down(sph_world* w) {
     size_t N = w->N;
     w->rows.resize(N);
     if (N) {
-        int c = w->cur;
-        uint32_t ob = w->own_begin;
-        CU(w->o_a.ensure(3 * N));
-        const float4* srcs[3] = {w->pos[c].p, w->vel[c].p, w->vc[c].p};
-        float* dsts[3] = {w->rows.pos.data(), w->rows.vel.data(), w->rows.vc.data()};
-        for (int a = 0; a < 3; ++a) {
-            LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + ob, srcs[a] + ob, w->o_a.p);
-            CU(cudaMemcpyAsync(dsts[a], w->o_a.p, 3 * N * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-            CU(cudaStreamSynchronize(w->st));
-        }
-        LAUNCH(k_export_u32, N, 256, (uint32_t)N, w->orig[c].p + ob, w->gid[c].p + ob, reinterpret_cast<uint32_t*>(w->o_a.p));
-        CU(cudaMemcpyAsync(w->rows.gid.data(), w->o_a.p, N * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
-        CU(cudaStreamSynchronize(w->st));
-        if (w->desc.solver == SPH_SOLVER_IISPH && w->press[c].p) {
-            LAUNCH(k_export1, N, 256, (uint32_t)N, w->orig[c].p + ob, w->press[c].p + ob, w->o_a.p);
-            CU(cudaMemcpyAsync(w->rows.press.data(), w->o_a.p, N * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-            CU(cudaStreamSynchronize(w->st));
-        }
+        // one column per call: the scratch holds 3 words per particle, not all 11
+        const int c = w->cur;
+        FluidRows& r = w->rows;
+        TRY(export_rows(w, fluid_col(w, Xyz{w->pos[c].p}, 0, N, r.pos.data())));
+        TRY(export_rows(w, fluid_col(w, Xyz{w->vel[c].p}, 0, N, r.vel.data())));
+        TRY(export_rows(w, fluid_col(w, Xyz{w->vc[c].p}, 0, N, r.vc.data())));
+        TRY(export_rows(w, fluid_col(w, U32<uint32_t>{w->gid[c].p}, 0, N, r.gid.data())));
+        if (w->desc.solver == SPH_SOLVER_IISPH && w->press[c].p) TRY(export_rows(w, fluid_col(w, Rows<1>{w->press[c].p}, 0, N, r.press.data())));
     }
     w->staged = true;
     w->lists_valid = false;
@@ -891,26 +969,15 @@ sph_status stage_up(sph_world* w) {
             }
             w->fluids[f].uniform_mass = uniform ? mass[w->fluids[f].offset] : 0.f;
         }
-        CU(w->o_a.ensure(3 * N));
-        CU(w->o_b.ensure(3 * N));
-        CU(w->o_c.ensure(3 * N));
-        CU(w->o_mass.ensure(N));
-        CU(w->o_fid.ensure(N));
-        CU(cudaMemcpyAsync(w->o_a.p, w->rows.pos.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_b.p, w->rows.vel.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_c.p, w->rows.vc.data(), 3 * N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_mass.p, mass.data(), N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemcpyAsync(w->o_fid.p, fid.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
         int c = w->cur;
         LAUNCH(k_iota, N, 256, (uint32_t)N, w->orig[c].p);
         CU(cudaMemcpyAsync(w->gid[c].p, w->rows.gid.data(), N * sizeof(uint32_t), cudaMemcpyHostToDevice, w->st));
         CU(cudaMemsetAsync(w->pos[c].p, 0, N * sizeof(float4), w->st));
         CU(cudaMemsetAsync(w->vel[c].p, 0, N * sizeof(float4), w->st));
-        LAUNCH(k_import, N, 256, (uint32_t)N, w->orig[c].p, w->o_a.p, w->o_b.p, w->o_c.p, w->o_mass.p, w->o_fid.p, w->pos[c].p, w->vel[c].p,
-               w->vc[c].p, 0u, (uint32_t)N);
         if (w->desc.solver == SPH_SOLVER_IISPH)
             CU(cudaMemcpyAsync(w->press[c].p, w->rows.press.data(), N * sizeof(float), cudaMemcpyHostToDevice, w->st));
-        CU(cudaStreamSynchronize(w->st));  // host temporaries go out of scope
+        // synchronises before the host temporaries go out of scope
+        TRY(import_rows(w, {w->rows.pos.data(), w->rows.vel.data(), w->rows.vc.data(), mass.data(), fid.data()}, 0, N, w->vc[c].p));
     }
     w->staged = false;
     w->lists_valid = false;
@@ -978,13 +1045,7 @@ sph_status pull_boundaries(sph_world* w) {
     TRY(enter(w));
     const size_t B = w->B;
     const int bc = w->bcur;
-    CU(w->o_b.ensure(3 * B));
-    CU(w->o_c.ensure(3 * B));
-    LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bpos[bc].p, w->o_b.p);
-    LAUNCH(k_export3, B, 256, (uint32_t)B, w->borig[bc].p, w->bvel[bc].p, w->o_c.p);
-    CU(cudaMemcpyAsync(w->brows.pos.data(), w->o_b.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaMemcpyAsync(w->brows.vel.data(), w->o_c.p, 3 * B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
+    TRY(export_rows(w, boundary_col(w, Xyz{w->bpos[bc].p}, 0, B, w->brows.pos.data()), boundary_col(w, Xyz{w->bvel[bc].p}, 0, B, w->brows.vel.data())));
     w->hb_stale = false;
     return SPH_OK;
 }
@@ -1601,13 +1662,7 @@ sph_status call_host_force2(sph_world* w, uint32_t f, ForceRec& fr, std::vector<
     std::vector<float> bvol;
     if (fr.host_flags & SPH_HOST_FORCE_BOUNDARIES) {
         bvol.resize(w->B);
-        if (w->B) {
-            const int bc = w->bcur;
-            CU(w->o_c.ensure(3 * std::max(w->N, w->B)));
-            LAUNCH(k_export_w, w->B, 256, (uint32_t)w->B, w->borig[bc].p, w->bpos[bc].p, w->o_c.p);
-            CU(cudaMemcpyAsync(bvol.data(), w->o_c.p, w->B * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-            CU(cudaStreamSynchronize(w->st));
-        }
+        if (w->B) TRY(export_rows(w, boundary_col(w, W4{w->bpos[w->bcur].p}, 0, w->B, bvol.data())));
         TRY(pull_boundaries(w));
         views.resize(w->bounds.size());
         for (size_t b = 0; b < w->bounds.size(); ++b) {
@@ -1684,22 +1739,10 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
                 case FORCE_HOST_CALLBACK: {  // user-defined NonPressureForce::solve on the host (nonpressure_force.rs:10-30)
                     // called for an empty fluid too (n = 0, offsets {0}), as predict_advection calls solve for every fluid
                     FluidRec& fl = w->fluids[f];
-                    const uint32_t ob = w->own_begin;
                     const size_t Nf = fl.n;
-                    CU(w->o_a.ensure(3 * N));
-                    CU(w->o_b.ensure(3 * N));
-                    CU(w->o_c.ensure(3 * std::max(N, w->B)));
-                    CU(w->o_mass.ensure(N));
-                    LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + ob, w->pos[c].p + ob, w->o_a.p);
-                    LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + ob, w->vel[c].p + ob, w->o_b.p);
-                    LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + ob, w->acc.p + ob, w->o_c.p);
-                    LAUNCH(k_export1, N, 256, (uint32_t)N, w->orig[c].p + ob, w->dens.p + ob, w->o_mass.p);
                     std::vector<float> hp(3 * Nf), hv(3 * Nf), ha(3 * Nf), hd(Nf);
-                    CU(cudaMemcpyAsync(hp.data(), w->o_a.p + 3 * fl.offset, 3 * Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-                    CU(cudaMemcpyAsync(hv.data(), w->o_b.p + 3 * fl.offset, 3 * Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-                    CU(cudaMemcpyAsync(ha.data(), w->o_c.p + 3 * fl.offset, 3 * Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-                    CU(cudaMemcpyAsync(hd.data(), w->o_mass.p + fl.offset, Nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-                    CU(cudaStreamSynchronize(w->st));
+                    TRY(export_rows(w, fluid_col(w, Xyz{w->pos[c].p}, fl.offset, Nf, hp.data()), fluid_col(w, Xyz{w->vel[c].p}, fl.offset, Nf, hv.data()),
+                                    fluid_col(w, Xyz{w->acc.p}, fl.offset, Nf, ha.data()), fluid_col(w, Rows<1>{w->dens.p}, fl.offset, Nf, hd.data())));
                     w->in_host_force = true;
                     sph_status hs = SPH_OK;
                     if (fr.host_fn2) hs = call_host_force2(w, (uint32_t)f, fr, hp, hv, hd, ha);
@@ -1707,9 +1750,9 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
                     w->in_host_force = false;
                     TRY(hs);
                     TRY(enter(w));  // the callback may have used another world of this process
-                    CU(cudaMemcpyAsync(w->o_c.p + 3 * fl.offset, ha.data(), 3 * Nf * sizeof(float), cudaMemcpyHostToDevice, w->st));
-                    LAUNCH(k_import_acc, N, 256, (uint32_t)N, w->orig[c].p + ob, w->o_c.p, (uint32_t)fl.offset, (uint32_t)(fl.offset + Nf), w->acc.p + ob);
-                    CU(cudaStreamSynchronize(w->st));  // host vectors go out of scope
+                    ImportRows back;
+                    back.vc = ha.data();
+                    TRY(import_rows(w, back, fl.offset, Nf, w->acc.p));
                     break;
                 }
                 default:
@@ -2329,19 +2372,7 @@ sph_status sph_fluid_write(sph_world* w, uint32_t fluid_h, const float* pos, con
         return SPH_OK;
     }
     TRY(enter(w));
-    size_t N = w->N;
-    int c = w->cur;
-    CU(w->o_a.ensure(3 * N));
-    CU(w->o_b.ensure(3 * N));
-    if (pos) CU(cudaMemcpyAsync(w->o_a.p + 3 * f.offset, pos, 3 * n * sizeof(float), cudaMemcpyHostToDevice, w->st));
-    if (vel) CU(cudaMemcpyAsync(w->o_b.p + 3 * f.offset, vel, 3 * n * sizeof(float), cudaMemcpyHostToDevice, w->st));
-    {
-        uint32_t ob = w->own_begin;
-        LAUNCH(k_import, N, 256, (uint32_t)N, w->orig[c].p + ob, pos ? w->o_a.p : nullptr, vel ? w->o_b.p : nullptr, (const float*)nullptr,
-               (const float*)nullptr, (const uint32_t*)nullptr, w->pos[c].p + ob, w->vel[c].p + ob, w->vc[c].p + ob, (uint32_t)f.offset,
-               (uint32_t)(f.offset + n));
-    }
-    CU(cudaStreamSynchronize(w->st));
+    TRY(import_rows(w, {pos, vel}, f.offset, n, w->vc[w->cur].p));
     w->lists_valid = false;
     if (pos) w->nb_valid = false;  // the cached bounds describe the positions the last step wrote
     return SPH_OK;
@@ -2361,20 +2392,10 @@ sph_status sph_fluid_read(sph_world* w, uint32_t fluid_h, float* pos, float* vel
         return SPH_OK;
     }
     TRY(enter(w));
-    size_t N = w->N;
-    int c = w->cur;
-    CU(w->o_a.ensure(3 * N));
-    CU(w->o_b.ensure(3 * N));
-    if (pos) {
-        LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + w->own_begin, w->pos[c].p + w->own_begin, w->o_a.p);
-        CU(cudaMemcpyAsync(pos, w->o_a.p + 3 * f.offset, 3 * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    }
-    if (vel) {
-        LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + w->own_begin, w->vel[c].p + w->own_begin, w->o_b.p);
-        CU(cudaMemcpyAsync(vel, w->o_b.p + 3 * f.offset, 3 * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    }
-    CU(cudaStreamSynchronize(w->st));
-    return SPH_OK;
+    const int c = w->cur;
+    const Col<Xyz> p = fluid_col(w, Xyz{w->pos[c].p}, f.offset, f.n, pos), v = fluid_col(w, Xyz{w->vel[c].p}, f.offset, f.n, vel);
+    if (pos && vel) return export_rows(w, p, v);
+    return export_rows(w, pos ? p : v);
 }
 
 sph_status sph_boundary_add(sph_world* w, const float* pos, const float* vel, size_t n, uint32_t memberships, uint32_t filter, int want_forces,
@@ -2429,18 +2450,8 @@ static sph_status boundary_export(sph_world* w, uint32_t boundary_h, float* out,
         return SPH_OK;
     }
     TRY(enter(w));
-    size_t B = w->B;
-    int bc = w->bcur;
-    CU(w->o_c.ensure(3 * std::max(B, w->N)));
-    if (forces) {
-        // bforce is indexed by SORTED boundary index; reuse k_export3 through a float4 view is not possible -> small loop kernel
-        LAUNCH(k_export_rows3, B, 256, (uint32_t)B, w->borig[bc].p, w->bforce.p, w->o_c.p);
-    } else {
-        LAUNCH(k_export_w, B, 256, (uint32_t)B, w->borig[bc].p, w->bpos[bc].p, w->o_c.p);
-    }
-    CU(cudaMemcpyAsync(out, w->o_c.p + width * b.offset, width * b.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
-    return SPH_OK;
+    if (forces) return export_rows(w, boundary_col(w, Rows<3>{w->bforce.p}, b.offset, b.n, out));  // bforce: 3 floats per sorted slot
+    return export_rows(w, boundary_col(w, W4{w->bpos[w->bcur].p}, b.offset, b.n, out));
 }
 
 sph_status sph_boundary_read_forces(sph_world* w, uint32_t boundary, float* f_xyz, size_t cap) {
@@ -2610,47 +2621,38 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         return SPH_OK;
     }
     TRY(enter(w));
-    size_t N = w->N;
-    int c = w->cur;
-    CU(w->o_c.ensure(std::max(width * N, 3 * std::max(N, w->B))));
     if (pf && pf->elastic) {  // the rest pose is kept in the fluid's original order already
         const ElasticityState& E = *pf->elastic;
+        if (what == SPH_DBG_EL_VOLUME0) return export_rows(w, Col<W4>{{E.pos0.p}, nullptr, 0u, (uint32_t)f.n, 0, f.n, out});
         const float* src = what == SPH_DBG_EL_ROTATION ? E.rot.p : what == SPH_DBG_EL_GRAD_TR ? E.grad_tr.p : E.stress.p;
-        if (what == SPH_DBG_EL_VOLUME0) {
-            LAUNCH(k_export_w_plain, f.n, 256, (uint32_t)f.n, E.pos0.p, w->o_c.p);
-            src = w->o_c.p;
-        }
         CU(cudaMemcpyAsync(out, src, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
         return SPH_OK;
     }
-    const float* s1 = nullptr;
+    const int c = w->cur;
+    // a source that does not exist (the pressures of a DFSPH world) is refused like an unknown selector
+    auto read = [&](auto src) {
+        return src.p ? export_rows(w, fluid_col(w, src, f.offset, f.n, out)) : w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);
+    };
     switch (what) {
-        case SPH_DBG_DENSITY: s1 = w->dens.p; break;
-        case SPH_DBG_ALPHA: s1 = w->alpha.p; break;
-        case SPH_DBG_DIVERGENCE: s1 = w->divv.p; break;
-        case SPH_DBG_PREDICTED_DENSITY: s1 = w->desc.solver == SPH_SOLVER_IISPH ? iisph_pred(w) : w->pred.p; break;
-        case SPH_DBG_PRESSURE: s1 = w->press[c].p; break;
-        case SPH_DBG_IISPH_AII: s1 = w->iisph.aii.p; break;
-        case SPH_DBG_HE2014_COLOR: s1 = w->he_colors.p; break;
-        case SPH_DBG_HE2014_GRADC: s1 = w->he_gradc.p; break;
-        default: break;
+        case SPH_DBG_DENSITY: return read(Rows<1>{w->dens.p});
+        case SPH_DBG_ALPHA: return read(Rows<1>{w->alpha.p});
+        case SPH_DBG_DIVERGENCE: return read(Rows<1>{w->divv.p});
+        case SPH_DBG_PREDICTED_DENSITY: return read(Rows<1>{w->desc.solver == SPH_SOLVER_IISPH ? iisph_pred(w) : w->pred.p});
+        case SPH_DBG_PRESSURE: return read(Rows<1>{w->press[c].p});
+        case SPH_DBG_IISPH_AII: return read(Rows<1>{w->iisph.aii.p});
+        case SPH_DBG_HE2014_COLOR: return read(Rows<1>{w->he_colors.p});
+        case SPH_DBG_HE2014_GRADC: return read(Rows<1>{w->he_gradc.p});
+        case SPH_DBG_VELOCITY_CHANGE: return read(Xyz{w->vc[c].p});
+        case SPH_DBG_ACCELERATION: return read(Xyz{w->acc.p});
+        case SPH_DBG_IISPH_DII: return read(Xyz{w->iisph.dii.p});
+        case SPH_DBG_IISPH_DIJ_PJL: return read(Xyz{w->iisph.dij_pjl.p});
+        case SPH_DBG_VISC_BETA: return read(Planes{36u, w->stride, w->visc.beta.p});
+        case SPH_DBG_VISC_TARGET: return read(Planes{6u, w->stride, w->visc.target.p});
+        case SPH_DBG_NUM_FLUID_CONTACTS: return read(U32<float>{w->lists.cnt_f.p});
+        case SPH_DBG_NUM_BOUNDARY_CONTACTS: return read(U32<float>{w->lists.cnt_b.p});
+        default: return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);
     }
-    const uint32_t ob = w->own_begin;
-    const uint32_t* og = w->orig[c].p + ob;
-    if (s1) LAUNCH(k_export1, N, 256, (uint32_t)N, og, s1 + ob, w->o_c.p);
-    else if (what == SPH_DBG_VELOCITY_CHANGE) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->vc[c].p + ob, w->o_c.p);
-    else if (what == SPH_DBG_ACCELERATION) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->acc.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_IISPH_DII) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dii.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_IISPH_DIJ_PJL) LAUNCH(k_export3, N, 256, (uint32_t)N, og, w->iisph.dij_pjl.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_VISC_BETA) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 36u, w->stride, og, w->visc.beta.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_VISC_TARGET) LAUNCH(k_export_planes, N, 256, (uint32_t)N, 6u, w->stride, og, w->visc.target.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_NUM_FLUID_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->lists.cnt_f.p + ob, w->o_c.p);
-    else if (what == SPH_DBG_NUM_BOUNDARY_CONTACTS) LAUNCH(k_export1u, N, 256, (uint32_t)N, og, w->lists.cnt_b.p + ob, w->o_c.p);
-    else return w->fail(SPH_ERR_INVALID, "sph_debug_read: unknown selector %d", what);
-    CU(cudaMemcpyAsync(out, w->o_c.p + width * f.offset, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
-    return SPH_OK;
 }
 
 const char* sph_last_error(const sph_world* w) { return w ? w->err.c_str() : "null world"; }
@@ -2751,13 +2753,7 @@ sph_status sph_fluid_read_ids(sph_world* w, uint32_t fluid_h, uint32_t* ids, siz
         return SPH_OK;
     }
     TRY(enter(w));
-    size_t N = w->N;
-    int c = w->cur;
-    CU(w->o_c.ensure(3 * std::max(N, w->B)));
-    LAUNCH(k_export_u32, N, 256, (uint32_t)N, w->orig[c].p + w->own_begin, w->gid[c].p + w->own_begin, reinterpret_cast<uint32_t*>(w->o_c.p));
-    CU(cudaMemcpyAsync(ids, reinterpret_cast<uint32_t*>(w->o_c.p) + f.offset, f.n * sizeof(uint32_t), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaStreamSynchronize(w->st));
-    return SPH_OK;
+    return export_rows(w, fluid_col(w, U32<uint32_t>{w->gid[w->cur].p}, f.offset, f.n, ids));
 }
 
 
@@ -3136,10 +3132,10 @@ static sph_status fluid_map(sph_world* w, uint32_t fluid_h, bool velocities, con
     }
     const FluidRec& f = w->fluids[fluid];
     DBuf<float>& buf = velocities ? w->map_vel : w->map_pos;
-    const size_t N = w->N;
-    CU(buf.ensure(3 * std::max<size_t>(N, 1)));
-    const int c = w->cur;
-    LAUNCH(k_export3, N, 256, (uint32_t)N, w->orig[c].p + w->own_begin, (velocities ? w->vel[c].p : w->pos[c].p) + w->own_begin, buf.p);
+    CU(buf.ensure(3 * std::max<size_t>(w->N, 1)));
+    Col<Xyz> col = fluid_col(w, Xyz{(velocities ? w->vel : w->pos)[w->cur].p}, 0, 0, (float*)nullptr);
+    col.dev = buf.p;
+    TRY(export_rows(w, col));
     CU(cudaStreamSynchronize(w->st));
     *dev = buf.p + 3 * f.offset;
     *n = f.n;

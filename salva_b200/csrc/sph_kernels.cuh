@@ -62,6 +62,7 @@ __constant__ Consts C;
 }  // namespace sphk
 
 #include "sph_lists.cuh"
+#include "sph_order.cuh"
 
 namespace sphk {
 
@@ -1143,81 +1144,6 @@ __device__ __forceinline__ float adhesion_kernel(float r, float adh_norm) {
     return 0.f;
 }
 
-// ------------------------------------------------------------------------------------------------
-// Host <-> sorted-order marshalling (Fluid/Boundary host SoA: fluid.rs:12-34, boundary.rs:11-24)
-// ------------------------------------------------------------------------------------------------
-// staging (original order, packed xyz) -> sorted arrays.  Any pointer may be null.
-__global__ void k_import(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ o_pos, const float* __restrict__ o_vel,
-                         const float* __restrict__ o_vc, const float* __restrict__ o_mass, const uint32_t* __restrict__ o_fid, float4* __restrict__ pos,
-                         float4* __restrict__ vel, float4* __restrict__ vc, uint32_t lo, uint32_t hi) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    uint32_t g = orig[s];
-    if (g < lo || g >= hi) return;
-    if (o_pos) {
-        float4 p = pos[s];
-        p.x = o_pos[3 * (size_t)g]; p.y = o_pos[3 * (size_t)g + 1]; p.z = o_pos[3 * (size_t)g + 2];
-        if (o_mass) p.w = o_mass[g];
-        pos[s] = p;
-    }
-    if (o_vel) {
-        float4 v = vel[s];
-        v.x = o_vel[3 * (size_t)g]; v.y = o_vel[3 * (size_t)g + 1]; v.z = o_vel[3 * (size_t)g + 2];
-        if (o_fid) v.w = __uint_as_float(o_fid[g]);
-        vel[s] = v;
-    }
-    if (o_vc) vc[s] = make_float4(o_vc[3 * (size_t)g], o_vc[3 * (size_t)g + 1], o_vc[3 * (size_t)g + 2], 0.f);
-}
-// sorted float4 array -> staging (original order, packed xyz)
-__global__ void k_export3(uint32_t n, const uint32_t* __restrict__ orig, const float4* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    uint32_t g = orig[s];
-    float4 v = src[s];
-    dst[3 * (size_t)g] = v.x; dst[3 * (size_t)g + 1] = v.y; dst[3 * (size_t)g + 2] = v.z;
-}
-// rows of 3 floats indexed by sorted index -> original order
-__global__ void k_export_rows3(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    uint32_t g = orig[s];
-    dst[3 * (size_t)g] = src[3 * (size_t)s]; dst[3 * (size_t)g + 1] = src[3 * (size_t)s + 1]; dst[3 * (size_t)g + 2] = src[3 * (size_t)s + 2];
-}
-__global__ void k_export_w(uint32_t n, const uint32_t* __restrict__ orig, const float4* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    dst[orig[s]] = src[s].w;
-}
-__global__ void k_export_w_plain(uint32_t n, const float4* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) dst[s] = src[s].w;
-}
-__global__ void k_export1(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    dst[orig[s]] = src[s];
-}
-__global__ void k_export1u(uint32_t n, const uint32_t* __restrict__ orig, const uint32_t* __restrict__ src, float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    dst[orig[s]] = (float)src[s];
-}
-// `width` planes src[k * stride + s] indexed by sorted index -> original order, packed width floats per particle
-__global__ void k_export_planes(uint32_t n, uint32_t width, uint32_t stride, const uint32_t* __restrict__ orig, const float* __restrict__ src,
-                                float* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    uint32_t g = orig[s];
-    for (uint32_t k = 0; k < width; ++k) dst[(size_t)width * g + k] = src[(size_t)k * stride + s];
-}
-// accelerations back from a host force callback: acc[s].xyz = src[orig[s]] for the particles of one fluid
-__global__ void k_import_acc(uint32_t n, const uint32_t* __restrict__ orig, const float* __restrict__ src, uint32_t lo, uint32_t hi, float4* __restrict__ acc) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s >= n) return;
-    uint32_t g = orig[s];
-    if (g < lo || g >= hi) return;
-    acc[s] = make_float4(src[3 * (size_t)g], src[3 * (size_t)g + 1], src[3 * (size_t)g + 2], 0.f);
-}
 __global__ void k_iota(uint32_t n, uint32_t* __restrict__ a) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) a[s] = s;
@@ -1282,10 +1208,6 @@ __global__ void k_slab_pack_counts(uint32_t* __restrict__ counts) {
 __global__ void k_iota_from(uint32_t n, uint32_t start, uint32_t* __restrict__ a) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s < n) a[s] = start + s;
-}
-__global__ void k_export_u32(uint32_t n, const uint32_t* __restrict__ orig, const uint32_t* __restrict__ src, uint32_t* __restrict__ dst) {
-    uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
-    if (s < n) dst[orig[s]] = src[s];
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -155,7 +155,7 @@ def test_each_materialisation_bug_is_flagged_by_name(mutant):
 
 
 def test_additions_on_another_fluids_rows_are_flagged():
-    """Accelerations out: the plugin of fluid 1 adds its pattern, written back at fluid 0's offset (k_import_acc's range)
+    """Accelerations out: the plugin of fluid 1 adds its pattern, written back at fluid 0's offset (the import's row range)
     instead of its own; and a correct write-back passes."""
     st = _get("two_fluids")
     rng = np.random.default_rng(3)
