@@ -47,7 +47,8 @@ TANK = scenes.open_tank((-R, -0.6, -R), (1.0, 0.8, 1.0), R)
 
 def scene(name):
     """Fluids (positions, velocities, volumes, density0, memberships, filter, forces), boundaries, solver, sinks
-    (fluid, lo, hi, outside) and sources (fluid, positions, velocities, interval)."""
+    (fluid, lo, hi, outside) and sources (fluid, positions, velocities, interval); make() also takes a particle_radius
+    (default R)."""
     p, v = block(6, 6, 6, (0.1, 0.0, 0.1), 3)
     fl = dict(positions=p, velocities=v, density0=1000.0, forces=[])
     sc = dict(solver=DFSPHSolver(), fluids=[fl], boundaries=[TANK], sinks=[], sources=[], forces_wanted=False)
@@ -97,7 +98,7 @@ def scene(name):
 
 
 def make(sc):
-    w = LiquidWorld(solver=sc["solver"], particle_radius=R, smoothing_factor=2.0)
+    w = LiquidWorld(solver=sc["solver"], particle_radius=sc.get("particle_radius", R), smoothing_factor=2.0)
     fh = []
     for f in sc["fluids"]:
         h = w.add_fluid(f["positions"], density0=f["density0"], velocities=f["velocities"], volumes=f.get("volumes"),
