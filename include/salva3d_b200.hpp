@@ -291,6 +291,13 @@ struct SurfaceMesh {
     std::vector<Vector3> normals;
     std::vector<uint32_t> triangles;  // 3 vertex indices per triangle
 };
+// The diffuse particles of a world (LiquidWorld::diffuse), in order; kinds are SPH_DIFFUSE_SPRAY / _FOAM / _BUBBLE
+struct DiffuseParticles {
+    std::vector<Point3> positions;
+    std::vector<Vector3> velocities;
+    std::vector<uint8_t> kinds;
+    std::vector<Real> lives;
+};
 using BoundaryHandle = size_t;
 
 class LiquidWorld {  // liquid_world.rs:17-158
@@ -442,6 +449,32 @@ public:
         check(sph_world_read_surface(raw_, reinterpret_cast<float*>(m.vertices.data()), normals ? reinterpret_cast<float*>(m.normals.data()) : nullptr, nv,
                                      m.triangles.data(), nt));
         return m;
+    }
+    // Advances the diffuse set (spray, foam, air bubbles: include/sph.h sph_world_update_diffuse, DESIGN.md section 16) by one
+    // frame of length dt from `fluids` (empty: every fluid).  desc: sph_diffuse_desc_default's values when not given.
+    sph_diffuse_stats update_diffuse(Real dt, const Vector3& gravity, const sph_diffuse_desc* desc = nullptr,
+                                     const std::vector<FluidHandle>& fluids = {}) {
+        std::vector<uint32_t> hs;
+        for (FluidHandle f : fluids) hs.push_back(fluids_.at(f).handle_);
+        sph_diffuse_desc d;
+        sph_diffuse_desc_default(&d);
+        if (desc) d = *desc;
+        const float g[3] = {gravity.x, gravity.y, gravity.z};
+        sph_diffuse_stats st;
+        check(sph_world_update_diffuse(raw_, hs.data(), hs.size(), &d, dt, g, &st));
+        return st;
+    }
+    DiffuseParticles diffuse() {
+        size_t n = 0;
+        check(sph_world_read_diffuse(raw_, nullptr, nullptr, nullptr, nullptr, 0, &n));
+        DiffuseParticles p;
+        p.positions.resize(n);
+        p.velocities.resize(n);
+        p.kinds.resize(n);
+        p.lives.resize(n);
+        check(sph_world_read_diffuse(raw_, reinterpret_cast<float*>(p.positions.data()), reinterpret_cast<float*>(p.velocities.data()),
+                                     p.kinds.data(), p.lives.data(), n, &n));
+        return p;
     }
     // liquid_world.rs:67-158
     void step_with_coupling(Real dt, const Vector3& gravity, CouplingManager* coupling) {

@@ -163,7 +163,14 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        SPH_DBG_EL_VOLUME0 = 16,        /* Becker2009 rest volumes                      becker2009_elasticity.rs:48-58 */
        SPH_DBG_EL_ROTATION = 17,       /* Becker2009 rotation (9, row-major)           becker2009_elasticity.rs:48-58 */
        SPH_DBG_EL_GRAD_TR = 18,        /* Becker2009 deformation_gradient_tr (9, row-major) becker2009_elasticity.rs:48-58 */
-       SPH_DBG_EL_STRESS = 19          /* Becker2009 stress (6: x y z w a b)           becker2009_elasticity.rs:48-58 */ };
+       SPH_DBG_EL_STRESS = 19,         /* Becker2009 stress (6: x y z w a b)           becker2009_elasticity.rs:48-58 */
+       /* The last sph_world_update_diffuse's values per fluid particle (SPH_ERR_INVALID unless that update selected the
+        * fluid with its current particle count; 0 for particles with non-finite positions) */
+       SPH_DBG_DIFFUSE_NORMAL = 20,    /* n = -grad phi / |grad phi| (3)                DESIGN.md section 16 */
+       SPH_DBG_DIFFUSE_TRAPPED_AIR = 21, /* I_ta before clamping */
+       SPH_DBG_DIFFUSE_WAVE_CREST = 22,  /* I_wc before clamping (0 where v^ . n < 0.6) */
+       SPH_DBG_DIFFUSE_KINETIC = 23,     /* E_k before clamping */
+       SPH_DBG_DIFFUSE_COUNT = 24        /* n_d, the particles it asked to emit, as float */ };
 
 /* LiquidWorld::new  liquid_world.rs:39-57 */
 void       sph_world_desc_default(sph_world_desc* desc);
@@ -507,6 +514,74 @@ sph_status sph_world_map_surface(sph_world* w, const float** d_vertices_xyz, con
 /* phi on the last extraction's lattice, x fastest, with its origin and point counts (0 before any extraction and when no
  * lattice was built).  phi == NULL: only origin and dims are written.  SPH_ERR_INVALID when cap is below the point count. */
 sph_status sph_world_read_surface_field(sph_world* w, float* phi, size_t cap, float origin[3], uint32_t dims[3]);
+
+/* Diffuse particles on the device: spray, foam and air bubbles (Ihmsen et al. 2012; DESIGN.md section 16).  A one-way
+ * post-process: sph_world_update_diffuse reads the selected fluids at the positions and velocities of the last step (before
+ * the first step: those given) and never writes the fluid.  The step, its grid and its cached graphs are not touched.  One
+ * update, in order:
+ *   1. The selected fluids' particles are binned into cells of width h (in (fluid slot, id) order within a cell in
+ *      deterministic mode); particles with non-finite positions are left out.
+ *   2. n_i = -grad phi(x_i) / |grad phi(x_i)|, phi = sum_j V_j W over the selected fluids within h (the surface extractor's
+ *      field, the world's gradient kernel); 0 where grad phi = 0.
+ *   3. Over the j with |x_ij|^2 <= h^2 (the step's unfused float32 pair test), x_ij = x_i - x_j, v_ij = v_i - v_j,
+ *      W~(r) = 1 - r / h:  I_ta = sum |v_ij| (1 - v^_ij . x^_ij) W~ (terms with |x_ij| = 0 or |v_ij| = 0 are 0);
+ *      kappa = sum over j with x_ij . n_i > 0 of (1 - n_i . n_j) W~, I_wc = kappa if |v_i| > 0 and v_i . n_i / |v_i| >= 0.6,
+ *      else 0;  E_k = 0.5 V_i rho0 |v_i|^2.  Each is clamped as Phi(I, lo, hi) = (min(I, hi) - min(I, lo)) / (hi - lo), and
+ *      n_d = floor(Phi_k (k_ta Phi_ta + k_wc Phi_wc) dt + u), each operation rounded once in float32 in this order (products,
+ *      then the sum, then * Phi_k, * dt, + u), min(a, b) = b < a ? b : a, NaN counting 0.  u = hash(seed, counter, slot, id,
+ *      0, stream 0) mapped to (h >> 8) 2^-24 (salva_b200/csrc/sph_hash.h), so small dt still emits on average.
+ *   4. In binned order, fluid particle i emits particles k = 0 .. n_d - 1, appended behind the survivors of the last update;
+ *      those past `capacity` are dropped.  With X_r, X_theta, X_h the hash's streams 1, 2, 3 for k, r = r_p sqrt(X_r),
+ *      theta = 2 pi X_theta and e1, e2 Duff et al. 2017's orthonormal basis around v^_f:  o = r cos theta e1 + r sin theta e2,
+ *      x = x_f + o + X_h dt v_f, v = v_f + o, life = lifetime.
+ *   5. Every diffuse particle, old and new: n_n = the fluid particles within h, v~ = sum v_j W / sum W (the density
+ *      kernel; 0 when the sum is 0).  Spray (n_n < spray_below): v += dt g, x += dt v.  Bubble (n_n > bubble_above):
+ *      v += -dt k_b g + k_d (v~ - v), x += dt v.  Foam (otherwise): v = v~, x += dt v~, life -= dt; only foam ages.
+ *   6. Foam with life <= 0 and every particle outside lo <= x < hi (non-finite positions included) are removed; the
+ *      survivors keep their order.  The update counter increments.
+ * In deterministic mode the set is bit-identical run to run and does not depend on the fluids' slot order.  The defaults
+ * (sph_diffuse_desc_default) are tuning values for scenes of particle radius about 0.05, not values from the paper. */
+enum { SPH_DIFFUSE_SPRAY = 0, SPH_DIFFUSE_FOAM = 1, SPH_DIFFUSE_BUBBLE = 2 };
+typedef struct {
+    float    ta_min, ta_max;      /* trapped-air clamp, finite, ta_min < ta_max */
+    float    wc_min, wc_max;      /* wave-crest clamp */
+    float    k_min, k_max;        /* kinetic-energy clamp */
+    float    k_ta, k_wc;          /* emission rates per second, finite, >= 0 */
+    float    lifetime;            /* foam lifetime, finite, > 0 */
+    float    k_b;                 /* bubble buoyancy, finite, >= 0 */
+    float    k_d;                 /* bubble drag towards the fluid, in [0, 1] */
+    uint32_t spray_below;         /* spray: fewer fluid neighbours than this */
+    uint32_t bubble_above;        /* bubble: more fluid neighbours than this; spray_below <= bubble_above + 1 */
+    uint32_t capacity;            /* most diffuse particles kept, > 0 */
+    uint32_t seed;
+    float    lo[3], hi[3];        /* particles outside lo <= x < hi are removed; lo <= hi, no NaN (infinities allowed) */
+} sph_diffuse_desc;
+typedef struct {
+    uint64_t emitted;             /* appended by this update */
+    uint64_t dropped;             /* asked for past capacity */
+    uint64_t expired;             /* foam whose life ran out */
+    uint64_t left_box;            /* removed outside the box (non-finite positions included) */
+    uint64_t spray, foam, bubble; /* the set after the update, by kind */
+} sph_diffuse_stats;
+void sph_diffuse_desc_default(sph_diffuse_desc* d);
+/* Advances the world's diffuse set by one frame of length dt under gravity, from fluids[0..n_fluids) (n_fluids == 0: every
+ * fluid).  stats may be NULL.  SPH_ERR_INVALID, nothing changed, for NaN or out-of-range desc fields, ta/wc/k min >= max,
+ * dt not finite and > 0, a non-finite gravity, lo > hi on any axis, capacity 0, stale or duplicate fluid handles,
+ * slab-decomposed worlds, calls from inside a coupling or host-force callback, and pending host edits.  SPH_ERR_OOM,
+ * nothing changed, past 2^31 binning cells or when an allocation fails.  A set larger than capacity (capacity lowered
+ * between updates) emits nothing and is not truncated. */
+sph_status sph_world_update_diffuse(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_diffuse_desc* desc, float dt,
+                                    const float gravity[3], sph_diffuse_stats* stats);
+/* The set in order: packed xyz positions and velocities, kinds (SPH_DIFFUSE_*) and lives; NULL = skip; *n = count.
+ * SPH_ERR_INVALID when cap is below the count and some output is not NULL. */
+sph_status sph_world_read_diffuse(sph_world* w, float* pos_xyz, float* vel_xyz, uint8_t* kind, float* life, size_t cap, size_t* n);
+/* Device pointers to the same arrays, valid until the next update or clear: the zero-copy path for renderers.  Any output
+ * pointer may be NULL. */
+sph_status sph_world_map_diffuse(sph_world* w, const float** d_pos_xyz, const float** d_vel_xyz, const uint8_t** d_kind,
+                                 const float** d_life, size_t* n);
+/* Empties the set; the update counter keeps counting.  Snapshots do not store the set, and sph_world_snapshot_load leaves
+ * it as it is. */
+sph_status sph_world_clear_diffuse(sph_world* w);
 
 /* boundary.positions / velocities (boundary.rs:13-15) in ORIGINAL index order.  NULL = skip; *n = particle count. */
 sph_status sph_boundary_read(sph_world* w, uint32_t boundary, float* pos_xyz, float* vel_xyz, size_t cap, size_t* n);

@@ -100,6 +100,17 @@ class SurfaceDesc(C.Structure):
     _fields_ = [("iso", C.c_float), ("spacing", C.c_float), ("lo", C.c_float * 3), ("hi", C.c_float * 3), ("normals", C.c_int32)]
 
 
+class DiffuseDesc(C.Structure):
+    _fields_ = [("ta_min", C.c_float), ("ta_max", C.c_float), ("wc_min", C.c_float), ("wc_max", C.c_float), ("k_min", C.c_float),
+                ("k_max", C.c_float), ("k_ta", C.c_float), ("k_wc", C.c_float), ("lifetime", C.c_float), ("k_b", C.c_float),
+                ("k_d", C.c_float), ("spray_below", C.c_uint32), ("bubble_above", C.c_uint32), ("capacity", C.c_uint32),
+                ("seed", C.c_uint32), ("lo", C.c_float * 3), ("hi", C.c_float * 3)]
+
+
+class DiffuseStats(C.Structure):
+    _fields_ = [(k, C.c_uint64) for k in ("emitted", "dropped", "expired", "left_box", "spray", "foam", "bubble")]
+
+
 # every symbol include/sph.h declares: name -> (restype, argtypes)
 SYMBOLS = {
     "sph_world_desc_default": (None, [C.POINTER(WorldDesc)]),
@@ -173,6 +184,12 @@ SYMBOLS = {
     "sph_world_read_surface": (C.c_int, [_vp, _fp, _fp, C.c_size_t, C.POINTER(C.c_uint32), C.c_size_t]),
     "sph_world_map_surface": (C.c_int, [_vp, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(C.POINTER(C.c_uint32))]),
     "sph_world_read_surface_field": (C.c_int, [_vp, _fp, C.c_size_t, _fp, C.POINTER(C.c_uint32)]),
+    "sph_diffuse_desc_default": (None, [C.POINTER(DiffuseDesc)]),
+    "sph_world_update_diffuse": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(DiffuseDesc), C.c_float, _fp,
+                                           C.POINTER(DiffuseStats)]),
+    "sph_world_read_diffuse": (C.c_int, [_vp, _fp, _fp, _u8p, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "sph_world_map_diffuse": (C.c_int, [_vp, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(_u8p), C.POINTER(_fp), C.POINTER(C.c_size_t)]),
+    "sph_world_clear_diffuse": (C.c_int, [_vp]),
 }
 
 

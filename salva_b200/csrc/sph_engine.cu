@@ -32,6 +32,7 @@
 #include "sph_sampling.cuh"
 #include "sph_edits.cuh"
 #include "sph_surface.cuh"
+#include "sph_diffuse.cuh"
 #include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 
@@ -190,13 +191,46 @@ struct SurfaceSet {
     bool normals = false;
 };
 struct SurfaceState {
-    DBuf<float4> p4, sp4;                  // (x, y, z, volume): collected, then in cell order
-    DBuf<unsigned long long> key;          // (fluid slot, id)
-    DBuf<float> vol;                       // the host's volume column while it is not all default
-    DBuf<uint32_t> cid, rank, perm, cstart, aabb, vcnt, tcnt, scan_aux[3];
+    DBuf<uint32_t> vcnt, tcnt, scan_aux[3];
     DBuf<uint8_t> emask;
     DBuf<unsigned long long> totals;
     SurfaceSet cur, next;
+};
+// The selected fluids' particles binned into cells of width h for one surface extraction or diffuse update
+// (sph_surface_host.inl bins_collect / bins_sort).  Collected rows follow the fluids' index order, slot by slot (sel.out_off).
+struct FluidBins {
+    DBuf<float4> p4, sp4;          // (x, y, z, volume): collected, then in cell order
+    DBuf<float4> v4, sv4;          // velocities (x, y, z, 0), when asked for: collected, then in cell order
+    DBuf<unsigned long long> key;  // (fluid slot, id), collected order
+    DBuf<float> vol;               // the host's volume column while it is not all default
+    DBuf<uint32_t> cid, rank, perm, cstart, aabb, scan_aux[3];
+    SurfSel sel{};
+    SurfGrid g{};
+    size_t np = 0, ncell = 0, binned = 0;  // collected, cells, binned (finite positions inside the cells)
+    bool have = false;                     // some collected position is finite; then amin / amax is their AABB
+    float amin[3] = {0.f, 0.f, 0.f}, amax[3] = {0.f, 0.f, 0.f};
+};
+// Diffuse particles (sph_diffuse_host.inl, DESIGN.md section 16).  A set in the published layout, with the per-fluid-particle
+// values of the update that made it (collected order, for sph_debug_read); an update builds into `next` and swaps it in on
+// success, so a refused one keeps the last set.
+struct DiffuseSet {
+    DBuf<float> pos, vel, life;  // packed xyz, xyz, life
+    DBuf<uint8_t> kind;
+    size_t n = 0;
+    DBuf<float> nrm, ta, wc, ek;  // per collected fluid particle: normal (xyz), I_ta, I_wc, E_k
+    DBuf<uint32_t> nd;            // ... and its emission count
+    SurfSel sel{};                // the fluids those rows belong to
+    uint32_t sel_n[MAX_FLUIDS] = {};
+};
+struct DiffuseState {
+    DBuf<float4> nrm4;                 // normals of the binned fluid, cell order
+    DBuf<unsigned long long> cnt, off;  // emission counts in cell order and their exclusive scan
+    DBuf<char> scan_tmp;               // the offsets scan's scratch
+    DBuf<float4> wx, wv;               // the advected set before compaction: (x, life), (v, kind bits)
+    DBuf<uint32_t> keep, scan_aux[3];  // keep flags, scanned in place into output rows
+    DBuf<unsigned long long> totals;   // expired, left the box, spray, foam, bubble
+    uint32_t counter = 0;              // successful updates: the hash's update counter
+    DiffuseSet cur, next;
 };
 
 struct ForceRec;
@@ -569,6 +603,8 @@ struct sph_world {
     EditScan* h_edit = nullptr;  // pinned
     DBuf<uint32_t> ed_keep, ed_rm, ed_list;
     SurfaceState surf;  // sph_world_extract_surface's scratch and its last mesh
+    FluidBins bins;     // the fluid binned for the last surface extraction or diffuse update
+    DiffuseState diffuse;  // sph_world_update_diffuse's scratch and its set
     bool vol_all_default = true;  // every row of rows.vol is rows.vol0 (set by stage_up): edits then only resize the column
     int xysub = 1;              // row order (Consts::xysub, SALVA_B200_XYSUB): x / y bins per cell; one GPU only
 
@@ -2170,6 +2206,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 #include "sph_graph.inl"
 #include "sph_edits_host.inl"
 #include "sph_surface_host.inl"
+#include "sph_diffuse_host.inl"
 
 // ===================================================================================================
 // extern "C" boundary
@@ -2596,6 +2633,7 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
     bool vec = what == SPH_DBG_VELOCITY_CHANGE || what == SPH_DBG_ACCELERATION || what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_DIJ_PJL;
     size_t width = vec ? 3 : 1;
     if (cap < f.n) return w->fail(SPH_ERR_INVALID, "sph_debug_read: capacity %zu < particle count %zu", cap, f.n);
+    if (what >= SPH_DBG_DIFFUSE_NORMAL && what <= SPH_DBG_DIFFUSE_COUNT) return diffuse_debug_read(w, fluid, what, out);
     const bool iisph_sel = what == SPH_DBG_IISPH_DII || what == SPH_DBG_IISPH_AII || what == SPH_DBG_IISPH_DIJ_PJL;
     if (iisph_sel && (w->desc.solver != SPH_SOLVER_IISPH || !w->iisph.dii.p || w->own_begin + w->N > w->iisph.cap))
         return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs an IISPH world that has stepped with its current particles", what);
@@ -3118,6 +3156,62 @@ sph_status sph_world_read_surface_field(sph_world* w, float* phi, size_t cap, fl
         CU(cudaMemcpyAsync(phi, R.phi.p, npts * sizeof(float), cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
     }
+    return SPH_OK;
+}
+
+// Diffuse particles (sph_diffuse_host.inl, DESIGN.md section 16)
+void sph_diffuse_desc_default(sph_diffuse_desc* d) {
+    if (!d) return;
+    memset(d, 0, sizeof *d);
+    d->ta_min = 2.f, d->ta_max = 8.f;
+    d->wc_min = 0.5f, d->wc_max = 4.f;
+    d->k_min = 0.1f, d->k_max = 2.f;
+    d->k_ta = 50.f, d->k_wc = 50.f;
+    d->lifetime = 2.f;
+    d->k_b = 0.8f, d->k_d = 0.5f;
+    d->spray_below = 6, d->bubble_above = 20;
+    d->capacity = 1u << 20;
+    d->seed = 0;
+    for (int a = 0; a < 3; ++a) d->lo[a] = -INFINITY, d->hi[a] = INFINITY;
+}
+sph_status sph_world_update_diffuse(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_diffuse_desc* desc, float dt,
+                                    const float gravity[3], sph_diffuse_stats* stats) {
+    if (!w || !desc || !gravity || (n_fluids && !fluids)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    return update_diffuse(w, fluids, n_fluids, desc, dt, gravity, stats);
+}
+sph_status sph_world_read_diffuse(sph_world* w, float* pos_xyz, float* vel_xyz, uint8_t* kind, float* life, size_t cap, size_t* n) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const DiffuseSet& R = w->diffuse.cur;
+    if (n) *n = R.n;
+    if (!pos_xyz && !vel_xyz && !kind && !life) return SPH_OK;
+    if (cap < R.n) return w->fail(SPH_ERR_INVALID, "sph_world_read_diffuse: cap %zu below the count %zu", cap, R.n);
+    if (!R.n) return SPH_OK;
+    TRY(enter(w));
+    if (pos_xyz) CU(cudaMemcpyAsync(pos_xyz, R.pos.p, 3 * R.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    if (vel_xyz) CU(cudaMemcpyAsync(vel_xyz, R.vel.p, 3 * R.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    if (kind) CU(cudaMemcpyAsync(kind, R.kind.p, R.n, cudaMemcpyDeviceToHost, w->st));
+    if (life) CU(cudaMemcpyAsync(life, R.life.p, R.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    CU(cudaStreamSynchronize(w->st));
+    return SPH_OK;
+}
+sph_status sph_world_map_diffuse(sph_world* w, const float** d_pos_xyz, const float** d_vel_xyz, const uint8_t** d_kind, const float** d_life,
+                                 size_t* n) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    const DiffuseSet& R = w->diffuse.cur;
+    if (d_pos_xyz) *d_pos_xyz = R.pos.p;
+    if (d_vel_xyz) *d_vel_xyz = R.vel.p;
+    if (d_kind) *d_kind = R.kind.p;
+    if (d_life) *d_life = R.life.p;
+    if (n) *n = R.n;
+    return SPH_OK;
+}
+sph_status sph_world_clear_diffuse(sph_world* w) {
+    if (!w) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    w->diffuse.cur.n = 0;
     return SPH_OK;
 }
 

@@ -55,10 +55,11 @@ __device__ __forceinline__ uint32_t surf_fkey(float f) {
     return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 
-// The selected fluids' particles of the device state, as (x, y, z, volume) and the in-cell sort key (fluid slot, id).
+// The selected fluids' particles of the device state, as (x, y, z, volume), the in-cell sort key (fluid slot, id) and, when
+// vout is not null, the velocities (x, y, z, 0).
 __global__ void k_surf_collect(uint32_t n, const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ orig,
                                const uint32_t* __restrict__ gid, SurfSel sel, const float* __restrict__ vol, float vol0, float4* __restrict__ out,
-                               unsigned long long* __restrict__ key) {
+                               unsigned long long* __restrict__ key, float4* __restrict__ vout) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t f = fid_of(vel[i]);
@@ -68,6 +69,10 @@ __global__ void k_surf_collect(uint32_t n, const float4* __restrict__ pos, const
     const float4 p = pos[i];
     out[k] = make_float4(p.x, p.y, p.z, vol ? vol[g] : vol0);
     key[k] = ((unsigned long long)f << 32) | gid[i];
+    if (vout) {
+        const float4 v = vel[i];
+        vout[k] = make_float4(v.x, v.y, v.z, 0.f);
+    }
 }
 
 // AABB of the finite positions: out[0..2] min keys, out[3..5] max keys (surf_fkey)
@@ -136,39 +141,45 @@ __global__ void k_surf_cell_sort(uint32_t ncell, const uint32_t* __restrict__ st
     }
 }
 
-// The 27 cells around x in a fixed order (x, then y, then the z-run of three cells): sum over their particles of
-// V_j W(r) (G = false) or of V_j W'(r) / r (x - x_j) (G = true).  Returns false when every cell is empty.
-template <bool G>
-__device__ __forceinline__ bool surf_gather(float x, float y, float z, const SurfGrid& g, const uint32_t* __restrict__ cstart,
-                                            const float4* __restrict__ sp, float4& acc) {
+// The particles of the 27 cells around x in a fixed order (x, then y, then the z-run of three cells): fn(j) for each
+// sorted index j.  Returns false when every cell is empty.
+template <class Fn>
+__device__ __forceinline__ bool surf_for_cells(float x, float y, float z, const SurfGrid& g, const uint32_t* __restrict__ cstart, Fn&& fn) {
     const int cx = (int)floorf(__fdiv_rn(x, C.h)) - g.ox, cy = (int)floorf(__fdiv_rn(y, C.h)) - g.oy, cz = (int)floorf(__fdiv_rn(z, C.h)) - g.oz;
     const int z0 = max(cz - 1, 0), z1 = min(cz + 1, g.nz - 1);
     bool any = false;
-    acc = make_float4(0.f, 0.f, 0.f, 0.f);
     if (z0 > z1) return false;
     for (int ix = max(cx - 1, 0); ix <= min(cx + 1, g.nx - 1); ++ix)
         for (int iy = max(cy - 1, 0); iy <= min(cy + 1, g.ny - 1); ++iy) {
             const uint32_t base = ((uint32_t)ix * (uint32_t)g.ny + (uint32_t)iy) * (uint32_t)g.nz;
             const uint32_t s = cstart[base + z0], e = cstart[base + z1 + 1];
             any |= s < e;
-            for (uint32_t j = s; j < e; ++j) {
-                const float4 pj = sp[j];
-                const float dx = __fsub_rn(x, pj.x), dy = __fsub_rn(y, pj.y), dz = __fsub_rn(z, pj.z);
-                const float d2 = dist2_exact(dx, dy, dz);
-                if (!(d2 <= C.h2)) continue;
-                const float r = __fsqrt_rn(d2);
-                if (G) {
-                    if (!(d2 > F32_EPS * F32_EPS)) continue;
-                    const float gf = __fmul_rn(pj.w, __fdiv_rn(kernel_dw_kind(C.kg, r), r));
-                    acc.x = __fmaf_rn(gf, dx, acc.x);
-                    acc.y = __fmaf_rn(gf, dy, acc.y);
-                    acc.z = __fmaf_rn(gf, dz, acc.z);
-                } else {
-                    acc.w = __fmaf_rn(pj.w, kernel_w_kind(C.kw, r), acc.w);
-                }
-            }
+            for (uint32_t j = s; j < e; ++j) fn(j);
         }
     return any;
+}
+
+// Sum over the particles of the 27 cells around x of V_j W(r) (G = false) or of V_j W'(r) / r (x - x_j) (G = true).
+template <bool G>
+__device__ __forceinline__ bool surf_gather(float x, float y, float z, const SurfGrid& g, const uint32_t* __restrict__ cstart,
+                                            const float4* __restrict__ sp, float4& acc) {
+    acc = make_float4(0.f, 0.f, 0.f, 0.f);
+    return surf_for_cells(x, y, z, g, cstart, [&](uint32_t j) {
+        const float4 pj = sp[j];
+        const float dx = __fsub_rn(x, pj.x), dy = __fsub_rn(y, pj.y), dz = __fsub_rn(z, pj.z);
+        const float d2 = dist2_exact(dx, dy, dz);
+        if (!(d2 <= C.h2)) return;
+        const float r = __fsqrt_rn(d2);
+        if (G) {
+            if (!(d2 > F32_EPS * F32_EPS)) return;
+            const float gf = __fmul_rn(pj.w, __fdiv_rn(kernel_dw_kind(C.kg, r), r));
+            acc.x = __fmaf_rn(gf, dx, acc.x);
+            acc.y = __fmaf_rn(gf, dy, acc.y);
+            acc.z = __fmaf_rn(gf, dz, acc.z);
+        } else {
+            acc.w = __fmaf_rn(pj.w, kernel_w_kind(C.kw, r), acc.w);
+        }
+    });
 }
 
 // Field pass: one thread per lattice point, x fastest.

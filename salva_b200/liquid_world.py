@@ -19,9 +19,11 @@ from ._lib import ForceDesc, StepStats, WorldDesc
 
 DBG = dict(density=0, alpha=1, divergence=2, predicted_density=3, velocity_change=4, num_fluid_contacts=5,
            num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11, he2014_color=12, he2014_gradc=13,
-           visc_beta=14, visc_target=15, el_volume0=16, el_rotation=17, el_grad_tr=18, el_stress=19)
+           visc_beta=14, visc_target=15, el_volume0=16, el_rotation=17, el_grad_tr=18, el_stress=19, diffuse_normal=20,
+           diffuse_trapped_air=21, diffuse_wave_crest=22, diffuse_kinetic=23, diffuse_count=24)
 # floats per particle of the selectors that are not scalars (include/sph.h)
-WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6}
+WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6, 20: 3}
+DIFFUSE_KINDS = ("spray", "foam", "bubble")  # SPH_DIFFUSE_SPRAY / _FOAM / _BUBBLE
 
 
 class SphError(RuntimeError):
@@ -626,6 +628,60 @@ class LiquidWorld:
             return _View()
         normals = view(np_, (nv, 3), "<f4") if C.cast(np_, C.c_void_p).value else None
         return view(vp, (nv, 3), "<f4"), view(tp, (nt, 3), "<u4"), normals
+
+    # -- diffuse particles: spray, foam and air bubbles (include/sph.h, DESIGN.md section 16) -------------------------
+    def diffuse_desc(self, **desc):
+        """sph_diffuse_desc_default with `desc`'s fields replaced (lo / hi as 3-sequences)."""
+        d = _lib.DiffuseDesc()
+        self._L.sph_diffuse_desc_default(C.byref(d))
+        for k, v in desc.items():
+            if k in ("lo", "hi"):
+                getattr(d, k)[:] = [float(x) for x in np.asarray(v, np.float32)]
+            elif not hasattr(d, k):
+                raise TypeError("unknown diffuse field %r" % k)
+            else:
+                setattr(d, k, v)
+        return d
+
+    def update_diffuse(self, dt, gravity=(0.0, -9.81, 0.0), fluids=None, **desc):
+        """Advances the world's diffuse set by one frame of length dt from `fluids` (None: all), on the device.  desc fields
+        (include/sph.h sph_diffuse_desc) override the defaults.  Returns the update's stats as a dict."""
+        d = self.diffuse_desc(**desc)
+        hs = np.ascontiguousarray(np.asarray([] if fluids is None else list(fluids), np.uint32))
+        g = np.ascontiguousarray(np.asarray(gravity, np.float32).reshape(3))
+        st = _lib.DiffuseStats()
+        self._ck(self._L.sph_world_update_diffuse(self._w, hs.ctypes.data_as(C.POINTER(C.c_uint32)), len(hs), C.byref(d), float(dt), _fp(g),
+                                                  C.byref(st)))
+        return {k: int(getattr(st, k)) for k, _ in _lib.DiffuseStats._fields_}
+
+    def diffuse_particles(self):
+        """(positions[n, 3] f32, velocities[n, 3] f32, kinds[n] u8 (0 spray, 1 foam, 2 bubble), lives[n] f32) in order."""
+        n = C.c_size_t()
+        self._ck(self._L.sph_world_read_diffuse(self._w, None, None, None, None, 0, C.byref(n)))
+        p, v = np.empty((n.value, 3), np.float32), np.empty((n.value, 3), np.float32)
+        k, life = np.empty(n.value, np.uint8), np.empty(n.value, np.float32)
+        self._ck(self._L.sph_world_read_diffuse(self._w, _fp(p), _fp(v), k.ctypes.data_as(C.POINTER(C.c_uint8)), _fp(life), n.value, C.byref(n)))
+        return p, v, k, life
+
+    def map_diffuse(self):
+        """Device views (no host copy) of (positions[n, 3], velocities[n, 3], kinds[n], lives[n]) as objects with
+        __cuda_array_interface__; valid until the next update or clear."""
+        ptrs = [C.POINTER(C.c_float)(), C.POINTER(C.c_float)(), C.POINTER(C.c_uint8)(), C.POINTER(C.c_float)()]
+        n = C.c_size_t()
+        self._ck(self._L.sph_world_map_diffuse(self._w, *[C.byref(x) for x in ptrs], C.byref(n)))
+
+        def view(ptr, shape, typestr):
+            addr = C.cast(ptr, C.c_void_p).value or 0
+
+            class _View:
+                __cuda_array_interface__ = {"shape": shape, "typestr": typestr, "data": (addr, False), "version": 2, "strides": None}
+            return _View()
+        m = n.value
+        return view(ptrs[0], (m, 3), "<f4"), view(ptrs[1], (m, 3), "<f4"), view(ptrs[2], (m,), "|u1"), view(ptrs[3], (m,), "<f4")
+
+    def clear_diffuse(self):
+        """Empties the diffuse set."""
+        self._ck(self._L.sph_world_clear_diffuse(self._w))
 
     # -- snapshot / restore and zero-copy views (include/sph.h) ---------------------------------------------
     def snapshot(self):
