@@ -27,7 +27,7 @@ struct SinkSet {
 struct EditScan {
     unsigned long long next_id[MAX_FLUIDS];  // 1 + the largest id per fluid, 0 for an empty fluid
     uint32_t removed[MAX_FLUIDS];
-    int bounds[7];  // the survivors' cell-coordinate AABB (lo xyz, hi xyz) and bad flag, as k_bounds writes them
+    CellBox bounds;  // the survivors' cell box
 };
 
 // In the box iff lo <= x < hi on every axis: plain f32 comparisons, so NaN is in no box.
@@ -42,19 +42,16 @@ __global__ void k_edit_classify(uint32_t n, const float4* __restrict__ pos, cons
                                 uint32_t* __restrict__ removed, EditScan* __restrict__ out) {
     __shared__ unsigned long long s_next[MAX_FLUIDS];
     __shared__ uint32_t s_rm[MAX_FLUIDS];
-    __shared__ int s_b[7];
     if (threadIdx.x < MAX_FLUIDS) {
         s_next[threadIdx.x] = 0ull;
         s_rm[threadIdx.x] = 0u;
     }
-    if (threadIdx.x < 7) s_b[threadIdx.x] = threadIdx.x < 3 ? INT_MAX : threadIdx.x < 6 ? INT_MIN : 0;
     __syncthreads();
     const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = s < n;
     bool rm = false;
     uint32_t f = 0u, g = 0u;
-    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
-    int bad = 0;
+    CellBox b = CELL_BOX_EMPTY;
     if (valid) {
         const float4 p = pos[s];
         f = fid_of(vel[s]);
@@ -62,14 +59,7 @@ __global__ void k_edit_classify(uint32_t n, const float4* __restrict__ pos, cons
         for (int k = 0; k < sinks.n && !rm; ++k) rm = sinks.b[k].fluid == f && sink_removes(sinks.b[k], p);
         keep[s] = rm ? 0u : 1u;
         removed[orig[s]] = rm ? 1u : 0u;
-        if (!rm) {
-            const float c[3] = {floorf(__fdiv_rn(p.x, C.h)), floorf(__fdiv_rn(p.y, C.h)), floorf(__fdiv_rn(p.z, C.h))};
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                if (!(fabsf(c[a]) < 1.0e9f)) { bad = 1; continue; }  // NaN / inf / absurd coordinates
-                mn[a] = mx[a] = (int)c[a];
-            }
-        }
+        if (!rm) cell_box_add(b, p.x, p.y, p.z, C.h);
     }
     // per fluid present in the warp: one shared atomic for its removals and one for its largest id
     const int lane = threadIdx.x & 31;
@@ -86,31 +76,11 @@ __global__ void k_edit_classify(uint32_t n, const float4* __restrict__ pos, cons
         }
         pending &= ~grp;
     }
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = min(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = max(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    bad = __any_sync(0xffffffffu, bad);
-    if (lane == 0) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            atomicMin(&s_b[a], mn[a]);
-            atomicMax(&s_b[3 + a], mx[a]);
-        }
-        if (bad) atomicOr(&s_b[6], 1);
-    }
-    __syncthreads();
+    cell_box_commit_block(b, &out->bounds);  // (its barrier also ends the shared atomics above)
     if (threadIdx.x < MAX_FLUIDS) {
         if (s_next[threadIdx.x]) atomicMax(&out->next_id[threadIdx.x], s_next[threadIdx.x]);
         if (s_rm[threadIdx.x]) atomicAdd(&out->removed[threadIdx.x], s_rm[threadIdx.x]);
     }
-    if (threadIdx.x < 3 && s_b[threadIdx.x] <= s_b[3 + threadIdx.x]) {
-        atomicMin(&out->bounds[threadIdx.x], s_b[threadIdx.x]);
-        atomicMax(&out->bounds[3 + threadIdx.x], s_b[3 + threadIdx.x]);
-    }
-    if (threadIdx.x == 0 && s_b[6]) atomicOr(&out->bounds[6], 1);
 }
 
 // After the exclusive scans of keep (slot order) and removed (original order), both n + 1 long: a survivor in slot s goes to

@@ -12,6 +12,7 @@
 #include <climits>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -380,7 +381,7 @@ struct SourceRec {
     DBuf<float4> pos, vel;    // the template, uploaded at registration
     bool has_vel = false;
     uint32_t interval = 1, age = 0;  // fires on the steps with age % interval == 0; age counts the steps since registration
-    int cells[7] = {};        // the template's cell AABB and bad flag, as k_bounds computes them
+    CellBox cells = CELL_BOX_EMPTY;  // the template's cell box
     bool alive = true;
     uint32_t gen = 0;
 };
@@ -468,7 +469,7 @@ struct StepGraphs {
     GraphCtl* h_ctl = nullptr;          // pinned
     cudaGraphConditionalHandle h_lists = 0;  // the IF of the step being captured past its neighbour search
     cudaGraph_t top = nullptr;          // the graph being captured
-    Envelope env{};                     // the fluid cell range the graph's grid covers with ENVELOPE_MARGIN to spare
+    CellBox env{};                      // the fluid cell range the graph's grid covers with ENVELOPE_MARGIN to spare
     bool env_valid = false;             // env was set up by an earlier call
     bool driver_checked = false;
     bool unsupported = false;           // the driver predates CUDA 12.4: step_many runs the per-step path
@@ -523,8 +524,7 @@ struct sph_world {
     FluidRows rows;
     // boundaries: host copy is always kept (static data); b_dirty => re-upload
     bool b_dirty = true;
-    int b_aabb[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};  // boundary cell-coordinate AABB (host side, static)
-    bool b_bad = false;
+    CellBox b_box = CELL_BOX_EMPTY;  // the boundaries' cell box (host side, static)
     // the boundary sort / volumes are reused while the boundaries and the grid mapping are unchanged
     bool b_sorted_valid = false, b_reused = false;
     unsigned long long bb_contacts = 0;
@@ -532,13 +532,13 @@ struct sph_world {
     BoundaryRows brows;
     bool hb_stale = false;  // colliders posed boundary particles on the device: brows lags behind (pull_boundaries)
     std::vector<ColliderRec> colliders;
-    DBuf<int> d_cb;         // boundary cell AABB + bad flag after colliders moved (as k_bounds writes it)
+    DBuf<CellBox> d_cb;     // the boundaries' cell box after colliders moved
     DBuf<float> d_imp;      // 6 floats per collider slot: the impulses of the step
     float* h_imp = nullptr;  // pinned copy, read back with the step's final read-back
     // DynamicContactSampling (colliders_contact): collider table, result ints, growing sample / push records, sort buffers
     DBuf<ContactCollider> d_ccol;
     DBuf<HfGrid> d_chf;  // per contact collider: a heightfield's grid (ContactParams::hf)
-    DBuf<int> d_cres;
+    DBuf<ContactResults> d_cres;
     DBuf<float4> cs_s4, cs_p4;
     DBuf<unsigned long long> cs_key[2];
     DBuf<uint32_t> cs_val[2];
@@ -577,13 +577,12 @@ struct sph_world {
     DBuf<float4> xs;  // the XSPH sums or the Akinci fluid force of a divergence evaluation (fold_state)
     uint32_t fused_nblk = 0;
     Tex tex_vs;  // the general evaluations gather v* through the texture pipe
-    DBuf<float> partial, errsum;
-    DBuf<int> d_scal;  // [0..6] bounds + bad flag, [7] error flag, [8..9] maxcnt, [11] elasticity widest, [12] CFL max |v + a R|^2
-    DBuf<unsigned long long> d_cnt;  // [0] bb contacts, [1] ff+fb contacts
+    DBuf<float> partial;
+    DBuf<StepScalars> d_ss;
+    StepScalars* h_ss = nullptr;  // pinned mirror of d_ss: every read-back lands in its own fields
     DBuf<uint32_t> rows_scratch;  // caller-order rows of export_rows / import_rows, one region per column
     IisphState iisph;
     ViscosityState visc;
-    float* h_pinned = nullptr;  // 64 floats of pinned host memory for small read-backs
 
     // fine-grained kernel timers: (slot, begin, end) event pairs accumulated into stats at step end
     struct Span { int slot; cudaEvent_t a, b; };
@@ -594,8 +593,7 @@ struct sph_world {
     bool lists_valid = false;
     // cell-coordinate AABB of the positions the last step wrote (k_update_positions): sizes the next grid without a bounds pass
     bool nb_valid = false, nb_pending = false;
-    int nb[7] = {0, 0, 0, 0, 0, 0, 0};
-    DBuf<int> d_nb;
+    CellBox nb = CELL_BOX_EMPTY;
     // particle sinks and sources (sph_edits_host.inl) and their classification's flags, result and removed original indices
     std::vector<SinkRec> sinks;
     std::vector<SourceRec> sources;
@@ -627,7 +625,7 @@ struct sph_world {
             if (e) cudaEventDestroy(e);
         if (ev_lists) cudaEventDestroy(ev_lists);
         graphs.release();
-        if (h_pinned) cudaFreeHost(h_pinned);
+        if (h_ss) cudaFreeHost(h_ss);
         if (h_imp) cudaFreeHost(h_imp);
         if (h_edit) cudaFreeHost(h_edit);
         if (st) cudaStreamDestroy(st);
@@ -975,7 +973,6 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     CU(w->lists.ensure(N, w->stride));
     uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
     CU(w->partial.ensure((size_t)(nblk + 3) * std::max<size_t>(1, w->fluids.size())));  // +3: a slab pass may run as three sub-range launches
-    CU(w->errsum.ensure(MAX_FLUIDS));
     return SPH_OK;
 }
 
@@ -1039,19 +1036,10 @@ sph_status upload_boundaries(sph_world* w) {
     CU(w->brank.ensure(B));
     CU(w->bperm.ensure(B));
     CU(w->bforce.ensure(3 * B));
+    w->b_box = CELL_BOX_EMPTY;
+    for (size_t g = 0; g < B; ++g) cell_box_add(w->b_box, w->brows.pos[3 * g], w->brows.pos[3 * g + 1], w->brows.pos[3 * g + 2], w->h);
     if (B) {
         std::vector<float4> p(B), v(B);
-        int aabb[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-        bool bad = false;
-        for (size_t g = 0; g < B; ++g)
-            for (int a = 0; a < 3; ++a) {
-                float cf = floorf(w->brows.pos[3 * g + a] / w->h);  // hgrid.rs:41-43, same IEEE division as the device
-                if (!(fabsf(cf) < 1.0e9f)) { bad = true; continue; }
-                aabb[a] = std::min(aabb[a], (int)cf);
-                aabb[3 + a] = std::max(aabb[3 + a], (int)cf);
-            }
-        memcpy(w->b_aabb, aabb, sizeof aabb);
-        w->b_bad = bad;
         for (size_t b = 0; b < w->bounds.size(); ++b)
             for (size_t i = 0; i < w->bounds[b].n; ++i) {
                 size_t g = w->bounds[b].offset + i;
@@ -1063,11 +1051,6 @@ sph_status upload_boundaries(sph_world* w) {
         CU(cudaMemcpyAsync(w->bvel[c].p, v.data(), B * sizeof(float4), cudaMemcpyHostToDevice, w->st));
         LAUNCH(k_iota, B, 256, (uint32_t)B, w->borig[c].p);
         CU(cudaStreamSynchronize(w->st));
-    }
-    if (!B) {
-        int none[6] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN};
-        memcpy(w->b_aabb, none, sizeof none);
-        w->b_bad = false;
     }
     w->b_dirty = false;
     w->b_sorted_valid = false;
@@ -1110,25 +1093,32 @@ sph_status apply_pending_deletes(sph_world* w) {
 }
 
 // ---- step phases ----------------------------------------------------------------------------------
-// The dense cell grid over the cell-coordinate AABB hb (lo xyz, hi xyz) of the fluid, with the boundaries' AABB and one padding
-// cell each side: its constants (uploaded) and cell arrays.  *ncell: its cells.
-sph_status grid_size(sph_world* w, const int* hb_fluid, size_t* ncell_out) {
-    int hb[6];
-    memcpy(hb, hb_fluid, sizeof hb);
-    for (int a = 0; a < 3; ++a) {  // boundary AABB: static, kept on the host
-        hb[a] = std::min(hb[a], w->b_aabb[a]);
-        hb[3 + a] = std::max(hb[3 + a], w->b_aabb[3 + a]);
-    }
+// Where a StepScalars field begins and ends, in bytes: the bounds of a reset or a read-back
+#define SS_BEGIN(f) offsetof(StepScalars, f)
+#define SS_END(f) (offsetof(StepScalars, f) + sizeof(StepScalars::f))
+
+// Enqueues the copy of the StepScalars bytes [from, to) into the pinned mirror; the caller synchronises before reading it
+sph_status read_scalars(sph_world* w, size_t from, size_t to) {
+    CU(cudaMemcpyAsync(reinterpret_cast<char*>(w->h_ss) + from, reinterpret_cast<const char*>(w->d_ss.p) + from, to - from,
+                       cudaMemcpyDeviceToHost, w->st));
+    return SPH_OK;
+}
+
+// The dense cell grid over the fluid's cell box, with the boundaries' box and one padding cell each side: its constants
+// (uploaded) and cell arrays.  *ncell: its cells.
+sph_status grid_size(sph_world* w, const CellBox& fluid, size_t* ncell_out) {
+    CellBox hb = fluid;
+    merge(hb, w->b_box);  // boundary box: static, kept on the host
     long long dims[3];
-    for (int a = 0; a < 3; ++a) dims[a] = (long long)hb[3 + a] - hb[a] + 3;  // one padding cell each side
+    for (int a = 0; a < 3; ++a) dims[a] = (long long)hb.hi[a] - hb.lo[a] + 3;  // one padding cell each side
     double ncell_d = (double)dims[0] * (double)dims[1] * (double)dims[2];
     if (ncell_d > 1.0e9) return w->fail(SPH_ERR_OOM, "dense cell grid too large: %lld x %lld x %lld cells of width h", dims[0], dims[1], dims[2]);
     const int xys = w->slab.active ? 1 : w->xysub;  // x / y bins per cell (row order, Consts::xysub)
     if (ncell_d * xys * xys > 2.0e9) return w->fail(SPH_ERR_OOM, "dense cell grid too large: %lld x %lld x %lld cells of width h", dims[0], dims[1], dims[2]);
     size_t ncell = (size_t)dims[0] * dims[1] * dims[2] * xys * xys;
-    w->hc.ox = (hb[0] - 1) * xys;
-    w->hc.oy = (hb[1] - 1) * xys;
-    w->hc.oz = hb[2] - 1;
+    w->hc.ox = (hb.lo[0] - 1) * xys;
+    w->hc.oy = (hb.lo[1] - 1) * xys;
+    w->hc.oz = hb.lo[2] - 1;
     w->hc.nx = (int)dims[0] * xys;
     w->hc.ny = (int)dims[1] * xys;
     w->hc.nz = (int)dims[2];
@@ -1190,28 +1180,28 @@ sph_status phase_grid(sph_world* w) {
     const uint32_t n_dead = w->slab.active ? w->slab.sort_dead_n : 0u;
     size_t ncell;
     if (w->cap) {  // a step graph runs on the envelope's grid, which graph_prepare set up
-        CU(cudaMemsetAsync(w->d_scal.p + 6, 0, 5 * sizeof(int), w->st));
-        CU(cudaMemsetAsync(w->d_cnt.p, 0, 2 * sizeof(unsigned long long), w->st));
+        CU(cudaMemsetAsync(reinterpret_cast<char*>(w->d_ss.p) + SS_BEGIN(err), 0, SS_END(contacts_f) - SS_BEGIN(err), w->st));
         ncell = (size_t)w->hc.nx * w->hc.ny * w->hc.nz;
     } else {
-        int init[11] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0, 0, 0, 0, 0};
-        CU(cudaMemcpyAsync(w->d_scal.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
-        CU(cudaMemsetAsync(w->d_cnt.p, 0, 2 * sizeof(unsigned long long), w->st));
-        int hb[7];
+        StepScalars init{};
+        init.grid = CELL_BOX_EMPTY;
+        CU(cudaMemcpyAsync(w->d_ss.p, &init, SS_END(contacts_f), cudaMemcpyHostToDevice, w->st));
+        CellBox hb;
         if (w->nb_valid && !w->slab.active && N) {
             // positions are exactly what the last step's k_update_positions wrote (no host edit since): its bounds came back with
             // that step's final read-back, so this step starts without a bounds pass and without a host round trip
-            memcpy(hb, w->nb, sizeof hb);
+            hb = w->nb;
         } else {
             if (Nin) {
-                k_bounds<<<std::min<uint32_t>(cdiv(Nin, 256), 296), 256, 0, w->st>>>(w->pos[c].p + off, (uint32_t)Nin, w->d_scal.p);
+                k_bounds<<<std::min<uint32_t>(cdiv(Nin, 256), 296), 256, 0, w->st>>>(w->pos[c].p + off, (uint32_t)Nin, &w->d_ss.p->grid);
                 w->launches++;
             }
-            CU(cudaMemcpyAsync(hb, w->d_scal.p, sizeof hb, cudaMemcpyDeviceToHost, w->st));
+            TRY(read_scalars(w, SS_BEGIN(grid), SS_END(grid)));
             CU(cudaStreamSynchronize(w->st));
+            hb = w->h_ss->grid;
         }
         w->nb_valid = false;
-        if (hb[6] || w->b_bad) return w->fail(SPH_ERR_INVALID, "non-finite or out-of-range particle coordinates");
+        if (hb.bad || w->b_box.bad) return w->fail(SPH_ERR_INVALID, "non-finite or out-of-range particle coordinates");
         TRY(grid_size(w, hb, &ncell));
     }
     const int xys = w->slab.active ? 1 : w->xysub;  // x / y bins per cell (row order, Consts::xysub)
@@ -1264,7 +1254,7 @@ sph_status density_args(sph_world* w, DensArgs* D) {
     }
     TRY(slab_wait(w));  // the sweep gathers v* of ghosts
     *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx.obj : 0, w->vs.p, w->unimass ? 0 : w->tex_vs.obj, w->vyz2.p,
-                  w->unimass ? w->tex_vyz.obj : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, w->d_scal.p + 7};
+                  w->unimass ? w->tex_vyz.obj : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, &w->d_ss.p->err};
     return SPH_OK;
 }
 
@@ -1295,8 +1285,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     if (B) {  // compute_boundary_volumes dfsph_solver.rs:72-96: the reference recomputes them every substep; they only
               // depend on the boundary positions, so they are reused while the boundaries are unchanged
         if (!w->b_reused) {
-            if (w->hc.xysub > 1) LAUNCH(k_boundary_volumes_xy, B, 128, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->bvol.p, w->d_cnt.p, w->d_scal.p + 7);
-            else LAUNCH(k_boundary_volumes, B, 128, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->bvol.p, w->d_cnt.p, w->d_scal.p + 7);
+            StepScalars* ss = w->d_ss.p;
+            if (w->hc.xysub > 1) LAUNCH(k_boundary_volumes_xy, B, 128, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->bvol.p, &ss->contacts_bb, &ss->err);
+            else LAUNCH(k_boundary_volumes, B, 128, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->bvol.p, &ss->contacts_bb, &ss->err);
             LAUNCH(k_set_w, B, 256, (uint32_t)B, w->bpos[bc].p, w->bvol.p);
         }
         for (auto& b : w->bounds)
@@ -1306,27 +1297,26 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             }
     }
     for (int attempt = 0; attempt < 8 && N; ++attempt) {
-        CU(cudaMemsetAsync(w->d_scal.p + 8, 0, 2 * sizeof(int), w->st));
-        uint32_t* maxcnt = reinterpret_cast<uint32_t*>(w->d_scal.p + 8);
-        LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->lists.out(), maxcnt, D);
+        CU(cudaMemsetAsync(w->d_ss.p->max_nb, 0, sizeof(StepScalars::max_nb), w->st));
+        LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->lists.out(), w->d_ss.p->max_nb, D);
         if (w->cap) {  // a step graph checks the capacities on the device and skips the rest of the step past them
-            k_lists_check<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_scal.p, w->lists.cap_f, w->lists.cap_b, w->graphs.h_lists);
+            k_lists_check<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_ss.p, w->lists.cap_f, w->lists.cap_b, w->graphs.h_lists);
             break;
         }
-        int* hs = reinterpret_cast<int*>(w->h_pinned + 32);  // pinned: the copy is truly asynchronous
-        CU(cudaMemcpyAsync(hs, w->d_scal.p + 7, 3 * sizeof(int), cudaMemcpyDeviceToHost, w->st));
+        TRY(read_scalars(w, SS_BEGIN(err), SS_END(max_nb)));  // pinned: the copy is truly asynchronous
         CU(cudaEventRecord(w->ev_lists, w->st));
         CU(cudaEventRecord(w->ev[EV_NBR], w->st));
         if (speculative) TRY(speculative(w));
         CU(cudaEventSynchronize(w->ev_lists));
+        const StepScalars& S = *w->h_ss;
         // (a zero density of the search's own density sweep is reported with the other zero densities at the end of the step)
-        if (hs[0] & ~ERR_SEARCH_ZERO_DENSITY)
+        if (S.err & ~ERR_SEARCH_ZERO_DENSITY)
             return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
-        w->stats.max_neighbors = (uint32_t)hs[1];
-        w->max_nb_b = (uint32_t)hs[2];
-        if ((uint32_t)hs[1] <= w->lists.cap_f && (uint32_t)hs[2] <= w->lists.cap_b) break;
-        if (speculative) CU(cudaMemsetAsync(w->d_scal.p + 7, 0, sizeof(int), w->st));  // error flag of the discarded density pass or sweep
-        TRY(grow_lists(w, ((uint32_t)hs[1] + 15) / 16 * 16, ((uint32_t)hs[2] + 15) / 16 * 16));
+        w->stats.max_neighbors = S.max_nb[0];
+        w->max_nb_b = S.max_nb[1];
+        if (S.max_nb[0] <= w->lists.cap_f && S.max_nb[1] <= w->lists.cap_b) break;
+        if (speculative) CU(cudaMemsetAsync(&w->d_ss.p->err, 0, sizeof(int), w->st));  // error word of the discarded density pass or sweep
+        TRY(grow_lists(w, (S.max_nb[0] + 15) / 16 * 16, (S.max_nb[1] + 15) / 16 * 16));
     }
     if (!N) {  // boundaries only
         TRY(ev_record(w, EV_NBR));
@@ -1334,7 +1324,7 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     }
     if (N) {
         k_sum_u32<<<std::min<uint32_t>(cdiv(N, 256), 1184), 256, 0, w->st>>>((uint32_t)N, w->lists.cnt_f.p + w->own_begin, w->lists.cnt_b.p + w->own_begin,
-                                                                             w->d_cnt.p + 1);
+                                                                             &w->d_ss.p->contacts_f);
         w->launches++;
     }
     if (dens) w->fused_nblk = cdiv(N, NBR_T);  // one error partial per block, summed by read_error()
@@ -1372,12 +1362,12 @@ LoopRule loop_rule(const sph_world* w, bool divergence) {
 // mean-per-fluid -> max over fluids (dfsph_solver.rs:153-158, :347-352)
 sph_status read_error(sph_world* w, uint32_t nblk, float* out) {
     int nf = (int)w->fluids.size();
-    k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
+    k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->d_ss.p->loop_err);
     w->launches++;
-    TRY(slab_allreduce(w, w->errsum.p, nf));  // multi-GPU: the means are over ALL ranks' particles
-    CU(cudaMemcpyAsync(w->h_pinned, w->errsum.p, nf * sizeof(float), cudaMemcpyDeviceToHost, w->st));
+    TRY(slab_allreduce(w, w->d_ss.p->loop_err, nf));  // multi-GPU: the means are over ALL ranks' particles
+    TRY(read_scalars(w, SS_BEGIN(loop_err), SS_BEGIN(loop_err) + nf * sizeof(float)));
     CU(cudaStreamSynchronize(w->st));
-    *out = loop_error(w->h_pinned, loop_sizes(w).data(), nf);
+    *out = loop_error(w->h_ss->loop_err, loop_sizes(w).data(), nf);
     return SPH_OK;
 }
 
@@ -1437,7 +1427,7 @@ sph_status launch_density_alpha(sph_world* w) {
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
     const Lists L = w->lists.view();
-    DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, w->d_scal.p + 7);
+    DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, &w->d_ss.p->err);
     return SPH_OK;  // the ghost refresh of rho follows in post_density_refresh(), once the list-capacity check has passed
 }
 // Ghost refresh of what the density pass produced (rho; DFSPH: also kappa of the fused first divergence evaluation).  Kept out
@@ -1565,7 +1555,7 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
         if (w->unimass) {
             if (predict) {
                 LAUNCH_R((k_vel_divergence_u<true>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7);
+                         w->alpha.p, out, w->pk4.p, partial, w->dt, &w->d_ss.p->err);
             } else if (xsf) {
                 const float cf = w->fluids[0].forces[0].d.p[0];
                 LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
@@ -1576,11 +1566,11 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
                          w->pk4.p, partial, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
             } else {
                 LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, w->d_scal.p + 7);
+                         w->alpha.p, out, w->pk4.p, partial, w->dt, &w->d_ss.p->err);
             }
         } else {
             DISPATCH2(k_vel_divergence, multi, predict, rg.count, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
-                      w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, w->d_scal.p + 7, rg);
+                      w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, &w->d_ss.p->err, rg);
         }
         return SPH_OK;
     });
@@ -1814,8 +1804,8 @@ uint32_t cfl_substeps(float m, float remaining, float r, float cfl, uint32_t min
 // Substepping only: the CFL reduction over the velocities `vel` and this substep's accelerations, enqueued after the forces
 sph_status launch_cfl_max(sph_world* w, const float4* vel, float remaining) {
     if (w->cfl_coeff == 0.f) return SPH_OK;
-    CU(cudaMemsetAsync(w->d_scal.p + 12, 0, sizeof(int), w->st));
-    LAUNCH(k_cfl_max, w->N, 256, vel, w->acc.p, remaining, reinterpret_cast<unsigned int*>(w->d_scal.p + 12));
+    CU(cudaMemsetAsync(&w->d_ss.p->cfl_bits, 0, sizeof(uint32_t), w->st));
+    LAUNCH(k_cfl_max, w->N, 256, vel, w->acc.p, remaining, &w->d_ss.p->cfl_bits);
     return SPH_OK;
 }
 
@@ -1824,9 +1814,9 @@ sph_status launch_cfl_max(sph_world* w, const float4* vel, float remaining) {
 sph_status timestep_advance(sph_world* w, float remaining) {
     float dt = remaining;
     if (w->cfl_coeff != 0.f) {
-        CU(cudaMemcpyAsync(w->h_pinned + 48, w->d_scal.p + 12, sizeof(float), cudaMemcpyDeviceToHost, w->st));
+        TRY(read_scalars(w, SS_BEGIN(cfl_bits), SS_END(cfl_bits)));
         CU(cudaStreamSynchronize(w->st));
-        const uint32_t n = cfl_substeps(w->h_pinned[48], remaining, w->desc.particle_radius, w->cfl_coeff, w->min_substeps,
+        const uint32_t n = cfl_substeps(__uint_as_float_host(w->h_ss->cfl_bits), remaining, w->desc.particle_radius, w->cfl_coeff, w->min_substeps,
                                         w->max_substeps, (uint32_t)w->substeps.size());
         dt = remaining / (float)n;
     }
@@ -1902,12 +1892,12 @@ sph_status decide(sph_world* w, const LoopRule& r, int i, uint32_t nblk, std::ar
     if (w->cap) {
         if (i < 0 || loop_decision(r, (uint32_t)i, [] { return 0.f; }).read) {  // i < 0: the device decides whether it reads
             const int nf = (int)w->fluids.size();
-            k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->errsum.p);
+            k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->d_ss.p->loop_err);
         }
         Decide d{};
         for (int k = 0; k < 5; ++k)
             if (c[k]) d.h[k] = c[k]->h;
-        k_loop_decide<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->errsum.p, r, i, d);
+        k_loop_decide<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_ss.p->loop_err, r, i, d);
         CU(cudaGetLastError());
         return SPH_OK;
     }
@@ -2005,11 +1995,10 @@ sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
     TRY(ev_record(w, EV_PRESS));
     TRY(slab_wait(w));  // a speculative exchange may still be in flight: it must land before the arrays are reused
     {
-        static const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
-        CU(w->d_nb.ensure(8));
-        if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(w->d_nb.p);
-        else CU(cudaMemcpyAsync(w->d_nb.p, init, sizeof init, cudaMemcpyHostToDevice, w->st));
-        LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->dt, w->slab.active ? (int*)nullptr : w->d_nb.p);  // :411-420
+        CellBox* next = &w->d_ss.p->next;
+        if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(next);
+        else CU(cudaMemcpyAsync(next, &CELL_BOX_EMPTY, sizeof(CellBox), cudaMemcpyHostToDevice, w->st));
+        LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->dt, w->slab.active ? nullptr : next);  // :411-420
         w->nb_pending = !w->slab.active;
     }
     CU(cudaGetLastError());
@@ -2082,12 +2071,10 @@ sph_status world_substep(sph_world* w, float remaining, const float g[3], const 
     }
     if (colliders && N) TRY(colliders_impulse(w));  // without fluid particles no force reaches a boundary (and dt did not advance)
     CU(cudaEventRecord(w->ev[EV_END], w->st));
-    int flag = 0;
-    unsigned long long cnts[2] = {0, 0};
-    CU(cudaMemcpyAsync(&flag, w->d_scal.p + 7, sizeof(int), cudaMemcpyDeviceToHost, w->st));
-    CU(cudaMemcpyAsync(cnts, w->d_cnt.p, sizeof cnts, cudaMemcpyDeviceToHost, w->st));
-    if (w->nb_pending) CU(cudaMemcpyAsync(w->nb, w->d_nb.p, sizeof w->nb, cudaMemcpyDeviceToHost, w->st));
+    TRY(read_scalars(w, SS_BEGIN(err), SS_END(next)));
     CU(cudaStreamSynchronize(w->st));
+    const StepScalars& S = *w->h_ss;
+    if (w->nb_pending) w->nb = S.next;
     w->nb_valid = w->nb_pending;
     w->nb_pending = false;
     CU(cudaGetLastError());
@@ -2098,8 +2085,8 @@ sph_status world_substep(sph_world* w, float remaining, const float g[3], const 
         else
             for (int j = 0; j < 6; ++j) c.impulse[j] += w->h_imp[6 * i + j];
     }
-    if (!w->b_reused) w->bb_contacts = cnts[0];
-    w->stats.n_contacts = w->bb_contacts + cnts[1];
+    if (!w->b_reused) w->bb_contacts = S.contacts_bb;
+    w->stats.n_contacts = w->bb_contacts + S.contacts_f;
     auto el = [&](int a, int b) {
         float ms = 0.f;
         cudaEventElapsedTime(&ms, w->ev[a], w->ev[b]);
@@ -2119,8 +2106,8 @@ sph_status world_substep(sph_world* w, float remaining, const float g[3], const 
         w->stats.pressure_ms = el(EV_INTEG, EV_PRESS);
         w->stats.integrate_ms = el(EV_FORCES, EV_INTEG) + el(EV_PRESS, EV_END);
     }
-    if (flag & 2) return w->fail(SPH_ERR_NCCL, "peer-memory ghost exchange timed out (a neighbour rank never delivered its boundary column)");
-    if (flag) return w->fail(SPH_ERR_ZERO_DENSITY, "zero density (reference asserts dfsph_solver.rs:92,145,662)");
+    if (S.err & ERR_PEER_TIMEOUT) return w->fail(SPH_ERR_NCCL, "peer-memory ghost exchange timed out (a neighbour rank never delivered its boundary column)");
+    if (S.err) return w->fail(SPH_ERR_ZERO_DENSITY, "zero density (reference asserts dfsph_solver.rs:92,145,662)");
     if (coupling && coupling->transmit_forces) coupling->transmit_forces(coupling->user, w, w->dt, w->inv_dt);  // liquid_world.rs:146
     return SPH_OK;
 }
@@ -2258,8 +2245,8 @@ sph_status sph_world_create(const sph_world_desc* desc, sph_world** out) {
     bool ok = cudaStreamCreateWithFlags(&w->st, cudaStreamNonBlocking) == cudaSuccess;
     for (int i = 0; ok && i < EV_COUNT; ++i) ok = cudaEventCreate(&w->ev[i]) == cudaSuccess;
     ok = ok && cudaEventCreateWithFlags(&w->ev_lists, cudaEventDisableTiming) == cudaSuccess;
-    ok = ok && cudaMallocHost(&w->h_pinned, 64 * sizeof(float)) == cudaSuccess;
-    ok = ok && w->d_scal.ensure(16) == cudaSuccess && w->d_cnt.ensure(2) == cudaSuccess;
+    ok = ok && cudaMallocHost(&w->h_ss, sizeof(StepScalars)) == cudaSuccess;
+    ok = ok && w->d_ss.ensure(1) == cudaSuccess;
     if (!ok) {
         delete w;
         return SPH_ERR_CUDA;
@@ -3057,16 +3044,11 @@ sph_status sph_fluid_add_source(sph_world* w, uint32_t fluid_h, const float* pos
     if (n > UINT32_MAX) return w->fail(SPH_ERR_INVALID, "sph_fluid_add_source: template of %zu particles is too large", n);
     TRY(edits_check_world(w));
     std::vector<float4> p(n), v(vel ? n : 0);
-    int cells[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
+    CellBox cells = CELL_BOX_EMPTY;
     for (size_t i = 0; i < n; ++i) {
         p[i] = make_float4(pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], 0.f);
         if (vel) v[i] = make_float4(vel[3 * i], vel[3 * i + 1], vel[3 * i + 2], 0.f);
-        for (int a = 0; a < 3; ++a) {
-            const float cf = floorf(pos[3 * i + a] / w->h);  // hgrid.rs:41-43, the same IEEE division as k_bounds
-            if (!(fabsf(cf) < 1.0e9f)) { cells[6] = 1; continue; }
-            cells[a] = std::min(cells[a], (int)cf);
-            cells[3 + a] = std::max(cells[3 + a], (int)cf);
-        }
+        cell_box_add(cells, pos[3 * i], pos[3 * i + 1], pos[3 * i + 2], w->h);
     }
     SourceRec r;
     CU(r.pos.ensure(n));
@@ -3082,7 +3064,7 @@ sph_status sph_fluid_add_source(sph_world* w, uint32_t fluid_h, const float* pos
     r.has_vel = vel != nullptr;
     r.interval = interval;
     r.age = 0;
-    memcpy(r.cells, cells, sizeof cells);
+    r.cells = cells;
     r.gen = w->sources[slot].gen + 1;
     w->sources[slot] = std::move(r);
     if (handle) *handle = make_handle(slot, w->sources[slot].gen & 0xFFFFu);

@@ -11,6 +11,8 @@
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <algorithm>
+#include <climits>
 
 namespace sphk {
 
@@ -71,6 +73,116 @@ namespace sphk {
 // ------------------------------------------------------------------------------------------------
 // hgrid.rs:41-52: cell = floor(x / h), IEEE division exactly as the reference.
 __device__ __forceinline__ int cell_coord(float x) { return (int)floorf(__fdiv_rn(x, C.h)); }
+
+// A cell-coordinate AABB (lo, hi inclusive; lo > hi on an axis without a point) and whether a point had a coordinate without
+// a cell.  The dense grid covers the fluid's and the boundaries' boxes.
+struct CellBox {
+    int lo[3], hi[3];
+    int bad;
+};
+constexpr CellBox CELL_BOX_EMPTY{{INT_MAX, INT_MAX, INT_MAX}, {INT_MIN, INT_MIN, INT_MIN}, 0};
+
+// Adds the point (x, y, z) to b: its cell is floor(x / h) with IEEE division (cell_coord) on the device and on the host alike;
+// a coordinate whose cell is NaN, infinite or absurd (|cell| >= 1e9) sets bad instead.
+__host__ __device__ __forceinline__ void cell_box_add(CellBox& b, float x, float y, float z, float h) {
+#ifdef __CUDA_ARCH__
+    const float c[3] = {floorf(__fdiv_rn(x, h)), floorf(__fdiv_rn(y, h)), floorf(__fdiv_rn(z, h))};
+#else
+    const float c[3] = {floorf(x / h), floorf(y / h), floorf(z / h)};
+#endif
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        if (!(fabsf(c[a]) < 1.0e9f)) { b.bad = 1; continue; }
+        b.lo[a] = (int)c[a] < b.lo[a] ? (int)c[a] : b.lo[a];
+        b.hi[a] = (int)c[a] > b.hi[a] ? (int)c[a] : b.hi[a];
+    }
+}
+inline void merge(CellBox& b, const CellBox& o) {
+    for (int a = 0; a < 3; ++a) {
+        b.lo[a] = std::min(b.lo[a], o.lo[a]);
+        b.hi[a] = std::max(b.hi[a], o.hi[a]);
+    }
+    b.bad |= o.bad;
+}
+
+// The warp's boxes merged into every lane's b
+__device__ __forceinline__ void cell_box_warp_reduce(CellBox& b) {
+#pragma unroll
+    for (int a = 0; a < 3; ++a)
+        for (int o = 16; o > 0; o >>= 1) {
+            b.lo[a] = min(b.lo[a], __shfl_xor_sync(0xffffffffu, b.lo[a], o));
+            b.hi[a] = max(b.hi[a], __shfl_xor_sync(0xffffffffu, b.hi[a], o));
+        }
+    b.bad = __any_sync(0xffffffffu, b.bad);
+}
+// Merges the warp's boxes into *out with one global atomic per axis and bound from lane 0.  Every lane of the warp calls it.
+__device__ __forceinline__ void cell_box_commit_warp(CellBox b, CellBox* out) {
+    cell_box_warp_reduce(b);
+    if ((threadIdx.x & 31) == 0) {
+#pragma unroll
+        for (int a = 0; a < 3; ++a)
+            if (b.lo[a] <= b.hi[a]) {
+                atomicMin(&out->lo[a], b.lo[a]);
+                atomicMax(&out->hi[a], b.hi[a]);
+            }
+        if (b.bad) atomicOr(&out->bad, 1);
+    }
+}
+// Merges the block's boxes into *out: warp shuffles, then shared memory, then one global atomic per axis and bound per block
+// (a kernel with one thread per particle would otherwise issue eight times as many).  Every thread of the block (at most 256)
+// calls it; it contains a block barrier.
+__device__ __forceinline__ void cell_box_commit_block(CellBox b, CellBox* out) {
+    cell_box_warp_reduce(b);
+    __shared__ int s_lo[3][8], s_hi[3][8], s_bad[8];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    if (lane == 0) {
+#pragma unroll
+        for (int a = 0; a < 3; ++a) {
+            s_lo[a][wid] = b.lo[a];
+            s_hi[a][wid] = b.hi[a];
+        }
+        s_bad[wid] = b.bad;
+    }
+    __syncthreads();
+    if (threadIdx.x < 3) {
+        const int a = threadIdx.x, nw = (blockDim.x + 31) >> 5;
+        int m0 = INT_MAX, m1 = INT_MIN;
+#pragma unroll 4  // unrolled 8 times, the loads of all warps' entries lift k_edit_classify from 28 to 31 registers
+        for (int k = 0; k < nw; ++k) {
+            m0 = min(m0, s_lo[a][k]);
+            m1 = max(m1, s_hi[a][k]);
+        }
+        if (m0 <= m1) {
+            atomicMin(&out->lo[a], m0);
+            atomicMax(&out->hi[a], m1);
+        }
+        if (a == 0) {
+            int bad = 0;
+            for (int k = 0; k < nw; ++k) bad |= s_bad[k];
+            if (bad) atomicOr(&out->bad, 1);
+        }
+    }
+}
+
+// The bits of StepScalars::err.  The host tells them apart: a zero density or boundary-volume denominator (the boundary
+// volumes are checked right after the search, the passes at the end of the step), a ghost exchange that timed out, and a zero
+// density found by the search's density sweep (reported with the passes' zero densities).
+enum : int { ERR_ZERO_DENSITY = 1, ERR_PEER_TIMEOUT = 2, ERR_SEARCH_ZERO_DENSITY = 4 };
+
+// What the step reads back from the device: one block (sph_world::d_ss) and its pinned host mirror (sph_world::h_ss).  The
+// fields are ordered so that each reset is one range: a substep of the host path sets grid .. contacts_f (phase_grid), a
+// graph step zeroes err .. contacts_f; the host path reads err .. next back with one copy at the end of a substep.
+struct StepScalars {
+    CellBox grid;                    // the fluid's cell box that sizes the grid (k_bounds)
+    int err;                         // error word: ERR_* bits
+    uint32_t max_nb[2];              // the widest fluid [0] and boundary [1] contact list of the search
+    unsigned long long contacts_bb;  // boundary-boundary contacts (k_boundary_volumes)
+    unsigned long long contacts_f;   // fluid-fluid + fluid-boundary contacts (k_sum_u32)
+    uint32_t elast_width;            // the widest Becker2009 rest list (k_el_capture_lists)
+    uint32_t cfl_bits;               // the CFL maximum |v + a R|^2 as float bits (k_cfl_max)
+    CellBox next;                    // the cell box of the positions the step wrote (k_update_positions)
+    float loop_err[MAX_FLUIDS];      // per-fluid error sums of a Jacobi evaluation (k_reduce_partials)
+};
 
 __device__ __forceinline__ int cell_id(int cx, int cy, int cz) { return ((cx - C.ox) * C.ny + (cy - C.oy)) * C.nz + (cz - C.oz); }
 // Row order bins x / y `sub` times finer than h.  abin: reference cell floor(v / h) (same IEEE division) times sub plus the
@@ -278,54 +390,13 @@ __device__ __forceinline__ float block_sum(float v, float* sm /* >= 32 floats */
 // K0: bounds (cell-coordinate AABB) — replaces the unbounded HashMap of hgrid.rs:22-25 by a dense
 // grid over the occupied region.
 // ------------------------------------------------------------------------------------------------
-__global__ void k_bounds(const float4* __restrict__ pos, uint32_t n, int* __restrict__ out /* minx,miny,minz,maxx,maxy,maxz,bad */) {
-    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
-    int bad = 0;
+__global__ void k_bounds(const float4* __restrict__ pos, uint32_t n, CellBox* __restrict__ out) {
+    CellBox b = CELL_BOX_EMPTY;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        float4 p = pos[i];
-        float c[3] = {floorf(__fdiv_rn(p.x, C.h)), floorf(__fdiv_rn(p.y, C.h)), floorf(__fdiv_rn(p.z, C.h))};
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            if (!(fabsf(c[a]) < 1.0e9f)) { bad = 1; continue; }  // NaN / inf / absurd coordinates
-            int v = (int)c[a];
-            mn[a] = min(mn[a], v);
-            mx[a] = max(mx[a], v);
-        }
+        const float4 p = pos[i];
+        cell_box_add(b, p.x, p.y, p.z, C.h);
     }
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = min(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = max(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    }
-    bad = __any_sync(0xffffffffu, bad);
-    __shared__ int s_mn[3][8], s_mx[3][8], s_bad[8];
-    int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            s_mn[a][wid] = mn[a];
-            s_mx[a][wid] = mx[a];
-        }
-        s_bad[wid] = bad;
-    }
-    __syncthreads();
-    if (threadIdx.x < 3) {  // one atomic pair per axis per block
-        int a = threadIdx.x, nw = (blockDim.x + 31) >> 5;
-        int m0 = INT_MAX, m1 = INT_MIN;
-        for (int k = 0; k < nw; ++k) {
-            m0 = min(m0, s_mn[a][k]);
-            m1 = max(m1, s_mx[a][k]);
-        }
-        atomicMin(&out[a], m0);
-        atomicMax(&out[3 + a], m1);
-        if (a == 0) {
-            int b = 0;
-            for (int k = 0; k < nw; ++k) b |= s_bad[k];
-            if (b) atomicOr(&out[6], 1);
-        }
-    }
+    cell_box_commit_block(b, out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -597,11 +668,8 @@ struct DensArgs {
     float *dens, *alpha, *divv, *kappa;
     float4* pk4;                                 // UNI: (position, kappa)
     float* partial;                              // per-block error partials: partial[block * n_fluids + f]
-    int* err;                                    // error word: ERR_SEARCH_ZERO_DENSITY
+    int* err;                                    // StepScalars::err: ERR_SEARCH_ZERO_DENSITY
 };
-// The bit a zero density found by the search's density sweep sets in the error word; the other bits come from the boundary
-// volumes (1, checked right after the search) and the ghost exchange (2), so the host can tell the three apart.
-constexpr int ERR_SEARCH_ZERO_DENSITY = 4;
 struct Vel3 {
     float x, y, z;
 };
@@ -877,7 +945,7 @@ k_boundary_volumes_xy(const float4* __restrict__ bpos, const float4* __restrict_
                     }
                 }
             }
-        if (den == 0.f) atomicOr(err, 1);
+        if (den == 0.f) atomicOr(err, ERR_ZERO_DENSITY);
         bvol[i] = 1.0f / den;
     }
     for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
@@ -913,7 +981,7 @@ k_boundary_volumes(const float4* __restrict__ bpos, const float4* __restrict__ b
                     }
                 }
             }
-        if (den == 0.f) atomicOr(err, 1);  // assert!(!denominator.is_zero()) dfsph_solver.rs:92
+        if (den == 0.f) atomicOr(err, ERR_ZERO_DENSITY);  // assert!(!denominator.is_zero()) dfsph_solver.rs:92
         bvol[i] = 1.0f / den;
     }
     for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
@@ -1070,61 +1138,19 @@ __global__ void k_cfl_max(const float4* __restrict__ vel, const float4* __restri
 
 // a22: update_positions dfsph_solver.rs:411-420: pos += (vel + vc) * dt.  bounds_out (optional): the cell-coordinate AABB of
 // the NEW positions (what k_bounds computes), so the next step's grid is sized without a bounds pass and its host round trip.
-__global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, float dt, int* __restrict__ bounds_out) {
+__global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, float dt, CellBox* __restrict__ bounds_out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = i < C.n_owned;
     i += C.i_begin;
-    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN};
-    int bad = 0;
+    CellBox b = CELL_BOX_EMPTY;
     if (valid) {
         float4 p = pos[i], v = vs[i];
         p.x += v.x * dt; p.y += v.y * dt; p.z += v.z * dt;
         pos[i] = p;
-        if (bounds_out) {
-            const float c[3] = {floorf(__fdiv_rn(p.x, C.h)), floorf(__fdiv_rn(p.y, C.h)), floorf(__fdiv_rn(p.z, C.h))};
-#pragma unroll
-            for (int a = 0; a < 3; ++a) {
-                if (!(fabsf(c[a]) < 1.0e9f)) { bad = 1; continue; }  // NaN / inf / absurd coordinates
-                mn[a] = mx[a] = (int)c[a];
-            }
-        }
+        if (bounds_out) cell_box_add(b, p.x, p.y, p.z, C.h);
     }
     if (!bounds_out) return;
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = min(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = max(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    bad = __any_sync(0xffffffffu, bad);
-    __shared__ int s_mn[3][8], s_mx[3][8], s_bad[8];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    if (lane == 0) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            s_mn[a][wid] = mn[a];
-            s_mx[a][wid] = mx[a];
-        }
-        s_bad[wid] = bad;
-    }
-    __syncthreads();
-    if (threadIdx.x < 3) {  // one atomic pair per axis per block
-        const int a = threadIdx.x, nw = (blockDim.x + 31) >> 5;
-        int m0 = INT_MAX, m1 = INT_MIN;
-        for (int k = 0; k < nw; ++k) {
-            m0 = min(m0, s_mn[a][k]);
-            m1 = max(m1, s_mx[a][k]);
-        }
-        if (m0 <= m1) {
-            atomicMin(&bounds_out[a], m0);
-            atomicMax(&bounds_out[3 + a], m1);
-        }
-        if (a == 0) {
-            int b = 0;
-            for (int k = 0; k < nw; ++k) b |= s_bad[k];
-            if (b) atomicOr(&bounds_out[6], 1);
-        }
-    }
+    cell_box_commit_block(b, bounds_out);
 }
 
 __device__ __forceinline__ float powi3(float x) { return x * x * x; }
@@ -1237,11 +1263,11 @@ __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t* p) {
 __device__ __forceinline__ void st_release_sys(uint32_t* p, uint32_t v) { asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory"); }
 // bounded spin (a peer that never arrives must not hang the GPU): ~2 s of SM clock, then the (sticky) error flag
 __device__ __forceinline__ bool p2p_wait(const uint32_t* flag, uint32_t seq, int* err) {
-    if (*reinterpret_cast<volatile int*>(err) & 2) return false;  // an earlier exchange of this step already timed out: do not wait again
+    if (*reinterpret_cast<volatile int*>(err) & ERR_PEER_TIMEOUT) return false;  // an earlier exchange of this step already timed out: do not wait again
     const long long t0 = clock64();
     while ((int)(ld_acquire_sys(flag) - seq) < 0) {
         if (clock64() - t0 > 4000000000LL) {
-            atomicOr(err, 2);
+            atomicOr(err, ERR_PEER_TIMEOUT);
             return false;
         }
         __nanosleep(64);
@@ -1381,13 +1407,13 @@ __global__ void k_sum_u32(uint32_t n, const uint32_t* __restrict__ a, const uint
 // Jacobi-loop exits (dfsph_solver.rs:153-158, :347-352, :450, :486), shared by the host loops and the device decisions of
 // the step graph (sph_graph.inl), so that both end a loop after the same evaluation.
 // ------------------------------------------------------------------------------------------------
-// The largest per-fluid mean errsum[f] / n[f] over the fluids with n[f] > 0 (n as float, from the particle count); 0 without
+// The largest per-fluid mean sums[f] / n[f] over the fluids with n[f] > 0 (n as float, from the particle count); 0 without
 // any, and a NaN mean never wins (the comparison of std::max).
-__host__ __device__ inline float loop_error(const float* errsum, const float* n, int nf) {
+__host__ __device__ inline float loop_error(const float* sums, const float* n, int nf) {
     float mx = 0.f;
     for (int f = 0; f < nf; ++f)
         if (n[f] > 0.f) {
-            const float e = errsum[f] / n[f];
+            const float e = sums[f] / n[f];
             mx = mx < e ? e : mx;
         }
     return mx;
@@ -1463,13 +1489,13 @@ __global__ void k_graph_arm(const GraphCtl* ctl, cudaGraphConditionalHandle h) {
 
 // After evaluation i (i0 >= 0: this i, else the running loop's next) of a loop: loop_decision with its counts and error
 // read, and the handles of what follows.
-__global__ void k_loop_decide(GraphCtl* ctl, StepRec* rec, const float* errsum, LoopRule r, int i0, Decide d) {
+__global__ void k_loop_decide(GraphCtl* ctl, StepRec* rec, const float* loop_err, LoopRule r, int i0, Decide d) {
     const uint32_t i = i0 >= 0 ? (uint32_t)i0 : ctl->it + 1;
     ctl->it = i;
     StepRec& R = rec[ctl->step];
     (r.divergence ? R.n_div_eval : R.n_press_eval)++;
     const LoopDecision x = loop_decision(r, i, [&] {
-        const float avg = loop_error(errsum, r.n, r.nf);
+        const float avg = loop_error(loop_err, r.n, r.nf);
         (r.divergence ? R.last_div_err : R.last_dens_err) = avg;
         return avg;
     });
@@ -1489,34 +1515,27 @@ __global__ void k_fold_arm(const GraphCtl* ctl, const StepRec* rec, int xsf, int
 
 // After the neighbour search of a graph step: the list capacity check and error word of phase_neighbors' read-back.  A list
 // longer than its capacity (or a boundary-volume error) stops the graph before the solver; the host redoes the step.
-__global__ void k_lists_check(GraphCtl* ctl, StepRec* rec, const int* scal, uint32_t cap_f, uint32_t cap_b, cudaGraphConditionalHandle h) {
-    const int err = scal[7];
-    const uint32_t mf = (uint32_t)scal[8], mb = (uint32_t)scal[9];
-    const bool ok = !(err & ~ERR_SEARCH_ZERO_DENSITY) && mf <= cap_f && mb <= cap_b;
+__global__ void k_lists_check(GraphCtl* ctl, StepRec* rec, const StepScalars* ss, uint32_t cap_f, uint32_t cap_b, cudaGraphConditionalHandle h) {
+    const uint32_t mf = ss->max_nb[0], mb = ss->max_nb[1];
+    const bool ok = !(ss->err & ~ERR_SEARCH_ZERO_DENSITY) && mf <= cap_f && mb <= cap_b;
     rec[ctl->step].max_neighbors = mf;
     if (!ok) ctl->stop = GRAPH_STOP_REDO;
     cudaGraphSetConditional(h, ok ? 1u : 0u);
 }
 
 // Initial value of k_update_positions' bounds
-__global__ void k_bounds_init(int* b) {
-    const int init[7] = {INT_MAX, INT_MAX, INT_MAX, INT_MIN, INT_MIN, INT_MIN, 0};
-    for (int a = 0; a < 7; ++a) b[a] = init[a];
-}
+__global__ void k_bounds_init(CellBox* b) { *b = CELL_BOX_EMPTY; }
 
-// End of a graph step: the record's contacts, the count, and the stops of world_substep's read-back: the error flag, and new
-// positions outside the envelope env (cell coordinates lo xyz, hi xyz) or not finite.
-struct Envelope {
-    int lo[3], hi[3];
-};
-__global__ void k_step_end(GraphCtl* ctl, StepRec* rec, const int* scal, const unsigned long long* cnt, const int* nb, Envelope env,
-                           unsigned long long bb_contacts) {
+// End of a graph step: the record's contacts, the count, and the stops of world_substep's read-back: the error word, and new
+// positions outside the envelope env (the bad flag unused) or not finite.
+__global__ void k_step_end(GraphCtl* ctl, StepRec* rec, const StepScalars* ss, CellBox env, unsigned long long bb_contacts) {
     StepRec& R = rec[ctl->step];
     R.on_device = 1;
-    R.n_contacts = bb_contacts + cnt[1];
-    bool inside = nb[6] == 0;
-    for (int a = 0; a < 3; ++a) inside = inside && nb[a] >= env.lo[a] && nb[3 + a] <= env.hi[a];
-    if (scal[7]) ctl->stop = GRAPH_STOP_ERROR;
+    R.n_contacts = bb_contacts + ss->contacts_f;
+    const CellBox& nb = ss->next;
+    bool inside = nb.bad == 0;
+    for (int a = 0; a < 3; ++a) inside = inside && nb.lo[a] >= env.lo[a] && nb.hi[a] <= env.hi[a];
+    if (ss->err) ctl->stop = GRAPH_STOP_ERROR;
     else if (!inside) ctl->stop = GRAPH_STOP_LEFT;
     ctl->step++;
     ctl->left--;

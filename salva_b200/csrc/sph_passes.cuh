@@ -188,7 +188,7 @@ k_density_alpha(const float4* __restrict__ pos, const float4* __restrict__ vel, 
         sq += ax * ax + ay * ay + az * az;
         gx += ax; gy += ay; gz += az;
     });
-    if (rho == 0.f) atomicOr(err, 1);  // assert!(!density.is_zero()) dfsph_solver.rs:662
+    if (rho == 0.f) atomicOr(err, ERR_ZERO_DENSITY);  // assert!(!density.is_zero()) dfsph_solver.rs:662
     float den = sq + (gx * gx + gy * gy + gz * gz);
     dens[i] = rho;
     alpha[i] = den <= 1.0e-5f ? 0.f : 1.0f / den;  // dfsph_solver.rs:209-213
@@ -239,7 +239,7 @@ k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, 
         }
         if (PREDICT) {
             float pd = fmaf(d, dt, dens[i]);
-            if (pd == 0.f) atomicOr(err, 1);  // assert dfsph_solver.rs:145
+            if (pd == 0.f) atomicOr(err, ERR_ZERO_DENSITY);  // assert dfsph_solver.rs:145
             out[i] = pd;
             kappa[i] = fmaxf((pd - rho0) * alpha[i], 0.f);
             e = pd < rho0 ? 0.f : pd / rho0 - 1.0f;
@@ -345,7 +345,7 @@ k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, con
         float kap;
         if (PREDICT) {
             float pd = fmaf(d, dt, dens[i]);
-            if (pd == 0.f) atomicOr(err, 1);
+            if (pd == 0.f) atomicOr(err, ERR_ZERO_DENSITY);
             out[i] = pd;
             kap = fmaxf((pd - rho0) * alpha[i], 0.f);
             e = pd < rho0 ? 0.f : pd / rho0 - 1.0f;

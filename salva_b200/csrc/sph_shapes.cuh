@@ -326,7 +326,11 @@ struct ContactCollider {
     uint32_t first_bin;             // first enumeration index of this collider's (grid-clipped) bin box
     int bl[3], bd[3];               // that bin box: first bin and extent per axis
 };
-constexpr int CS_SAMPLES = 0, CS_PUSHES = 1, CS_FLUID_BOUNDS = 2, CS_BOUND_BOUNDS = 9, CS_PER_COLLIDER = 16;  // layout of the result ints
+struct ContactResults {                     // what contact sampling reduces, read back with one copy
+    uint32_t samples, pushes;                  // records k_contact_sample made (past the capacities too: the pass is re-run)
+    CellBox fluid, bound;                      // the cell boxes of the fluid after the pushes and of the rebuilt boundaries
+    uint32_t per_collider[MAX_BOUNDARIES];     // samples per collider slot
+};
 struct ContactParams {
     const ContactCollider* col;
     int nc;                         // contact colliders, ascending slot
@@ -402,32 +406,6 @@ __device__ __forceinline__ bool contact_project_local(const ContactCollider& c, 
     }
     return true;
 }
-__device__ __forceinline__ void cell_bounds_add(float x, float y, float z, int* mn, int* mx, int* bad) {
-    const float c[3] = {floorf(__fdiv_rn(x, C.h)), floorf(__fdiv_rn(y, C.h)), floorf(__fdiv_rn(z, C.h))};
-#pragma unroll
-    for (int a = 0; a < 3; ++a) {
-        if (!(fabsf(c[a]) < 1.0e9f)) { *bad = 1; continue; }
-        mn[a] = min(mn[a], (int)c[a]);
-        mx[a] = max(mx[a], (int)c[a]);
-    }
-}
-__device__ __forceinline__ void warp_bounds_commit(int* mn, int* mx, int bad, int* out) {
-#pragma unroll
-    for (int a = 0; a < 3; ++a)
-        for (int o = 16; o > 0; o >>= 1) {
-            mn[a] = min(mn[a], __shfl_xor_sync(0xffffffffu, mn[a], o));
-            mx[a] = max(mx[a], __shfl_xor_sync(0xffffffffu, mx[a], o));
-        }
-    bad = __any_sync(0xffffffffu, bad);
-    if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            if (mn[a] != INT_MAX) atomicMin(&out[a], mn[a]);
-            if (mx[a] != INT_MIN) atomicMax(&out[3 + a], mx[a]);
-        }
-        if (bad) atomicOr(&out[6], 1);
-    }
-}
 // One warp per enumerated bin (the bins of each collider's cell box, clipped to the grid); its lanes take the bin's particles.
 // A particle is processed by the enumeration of the lowest-slot collider whose box holds its cell.  Records:
 // samples  s4[2r] = (proj, orig), s4[2r+1] = (velocity, 0), key[r] = slot << 32 | orig, val[r] = r;
@@ -437,7 +415,7 @@ __device__ __forceinline__ void warp_bounds_commit(int* mn, int* mx, int bad, in
 template <bool HF, bool REV>
 __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                                  const uint32_t* __restrict__ orig, float4* __restrict__ s4, unsigned long long* __restrict__ key, uint32_t* __restrict__ val,
-                                 float4* __restrict__ p4, int* __restrict__ res) {
+                                 float4* __restrict__ p4, ContactResults* __restrict__ res) {
     const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     if (warp >= P.total_bins) return;  // warp-uniform
     int e = 0;
@@ -449,7 +427,7 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
     const int bx = E.bl[0] + (int)(t / (uint32_t)(E.bd[2] * E.bd[1]));
     const int cell = cell_id(bx, by, bz);
     const uint32_t start = cstart[cell], end = cstart[cell + 1];
-    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN}, bad = 0;
+    CellBox box = CELL_BOX_EMPTY;
     for (uint32_t base = start; base < end; base += 32) {
         const uint32_t j = base + lane;
         bool mine = j < end;
@@ -514,14 +492,14 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
             if (!m) continue;
             uint32_t r0 = 0;
             if (lane == 0) {
-                r0 = atomicAdd((uint32_t*)&res[CS_SAMPLES], (uint32_t)__popc(m));
-                atomicAdd(&res[CS_PER_COLLIDER + K.slot], __popc(m));
+                r0 = atomicAdd(&res->samples, (uint32_t)__popc(m));
+                atomicAdd(&res->per_collider[K.slot], (uint32_t)__popc(m));
             }
             r0 = __shfl_sync(0xffffffffu, r0, 0);
             if (emit) {
                 const uint32_t r = r0 + __popc(m & ((1u << lane) - 1u));
                 const uint32_t o = orig[j];
-                cell_bounds_add(q[0], q[1], q[2], mn, mx, &bad);
+                cell_box_add(box, q[0], q[1], q[2], C.h);
                 if (r < P.cap_s) {
                     s4[2 * (size_t)r] = make_float4(q[0], q[1], q[2], __uint_as_float(o));
                     s4[2 * (size_t)r + 1] = make_float4(sv[0], sv[1], sv[2], 0.f);
@@ -533,7 +511,7 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
         const unsigned m = __ballot_sync(0xffffffffu, pushed);
         if (m) {
             uint32_t r0 = 0;
-            if (lane == 0) r0 = atomicAdd((uint32_t*)&res[CS_PUSHES], (uint32_t)__popc(m));
+            if (lane == 0) r0 = atomicAdd(&res->pushes, (uint32_t)__popc(m));
             r0 = __shfl_sync(0xffffffffu, r0, 0);
             const uint32_t r = r0 + __popc(m & ((1u << lane) - 1u));
             if (pushed && r < P.cap_p) {
@@ -542,12 +520,12 @@ __global__ void k_contact_sample(ContactParams P, const float4* __restrict__ pos
             }
         }
     }
-    warp_bounds_commit(mn, mx, bad, res + CS_BOUND_BOUNDS);
+    cell_box_commit_warp(box, &res->bound);
 }
 // The pushes of k_contact_sample, written only when neither record buffer overflowed (the pass is then re-run unchanged).
-__global__ void k_contact_apply(const float4* __restrict__ p4, const int* __restrict__ res, uint32_t cap_s, uint32_t cap_p, float4* __restrict__ pos,
+__global__ void k_contact_apply(const float4* __restrict__ p4, const ContactResults* __restrict__ res, uint32_t cap_s, uint32_t cap_p, float4* __restrict__ pos,
                                 float4* __restrict__ vel) {
-    const uint32_t ns = (uint32_t)res[CS_SAMPLES], np = (uint32_t)res[CS_PUSHES];
+    const uint32_t ns = res->samples, np = res->pushes;
     if (ns > cap_s || np > cap_p) return;
     for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < np; r += gridDim.x * blockDim.x) {
         const float4 a = p4[2 * (size_t)r], b = p4[2 * (size_t)r + 1];
@@ -557,14 +535,14 @@ __global__ void k_contact_apply(const float4* __restrict__ p4, const int* __rest
     }
 }
 // Cell bounds of the boundary particles that stay (boundaries not coupled by contact sampling: skip bit set).
-__global__ void k_bounds_kept(const float4* __restrict__ bpos, const float4* __restrict__ bvel, uint32_t n, unsigned long long skip, int* __restrict__ out) {
-    int mn[3] = {INT_MAX, INT_MAX, INT_MAX}, mx[3] = {INT_MIN, INT_MIN, INT_MIN}, bad = 0;
+__global__ void k_bounds_kept(const float4* __restrict__ bpos, const float4* __restrict__ bvel, uint32_t n, unsigned long long skip, CellBox* __restrict__ out) {
+    CellBox box = CELL_BOX_EMPTY;
     for (uint32_t s = blockIdx.x * blockDim.x + threadIdx.x; s < n; s += gridDim.x * blockDim.x) {
         if ((skip >> fid_of(bvel[s])) & 1ull) continue;
         const float4 p = bpos[s];
-        cell_bounds_add(p.x, p.y, p.z, mn, mx, &bad);
+        cell_box_add(box, p.x, p.y, p.z, C.h);
     }
-    warp_bounds_commit(mn, mx, bad, out);
+    cell_box_commit_warp(box, out);
 }
 // Rebuild of the boundary arrays in ORIGINAL order: the boundaries that stay move to their new offsets...
 struct ContactRebuild {
