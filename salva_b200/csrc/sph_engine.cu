@@ -558,6 +558,7 @@ struct sph_world {
     DBuf<float4> vs, acc, normals, dbg_acc;
     DBuf<float> dens, alpha, kappa, divv, pred, bvol, bforce;
     DBuf<uint32_t> cid, rank, perm, cstart, bcid, brank, bperm, bstart, scan_aux[3], scan_aux_k[3];
+    DBuf<unsigned long long> skey;  // deterministic mode: the in-cell sort keys beside perm / bperm (k_cell_scatter)
     ListState lists;
     // uniform-mass packed gather records (sph_passes.cuh): pvx4 = (x,y,z,v*x), vyz2 = (v*y,v*z), pk4 = (x,y,z,kappa); their
     // gathers are split evenly over the texture and LSU pipes (even / odd contacts)
@@ -969,6 +970,7 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     CU(w->cid.ensure(N));
     CU(w->rank.ensure(N));
     CU(w->perm.ensure(N));
+    if (w->desc.deterministic) CU(w->skey.ensure(N));
     w->stride = (uint32_t)((N + 31) / 32 * 32);
     CU(w->lists.ensure(N, w->stride));
     uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
@@ -1147,11 +1149,13 @@ sph_status sort_boundaries(sph_world* w, size_t ncell) {
         if (xys > 1) LAUNCH(k_cell_hist_xy, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p);
         else LAUNCH(k_cell_hist, B, 256, w->bpos[bc].p, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, (const uint32_t*)nullptr, 0u);
         TRY(scan_exclusive(w, w->bstart.p, ncell + 1));
-        LAUNCH(k_cell_scatter, B, 256, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, w->bperm.p);
         // in-cell order by original index: the same whether the input is a fresh upload or the last sort of boundaries that
         // colliders moved on the device
-        if (w->desc.deterministic)
-            LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, (const uint32_t*)w->borig[bc].p, (const float4*)nullptr);
+        const bool det = w->desc.deterministic;
+        if (det) CU(w->skey.ensure(B));
+        LAUNCH(k_cell_scatter, B, 256, (uint32_t)B, w->bcid.p, w->brank.p, w->bstart.p, w->bperm.p, (const uint32_t*)w->borig[bc].p,
+               (const float4*)nullptr, det ? w->skey.p : nullptr);
+        if (det) LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->bstart.p, w->bperm.p, w->skey.p);
         GatherSet g;
         memset(&g, 0, sizeof g);
         g.in4[0] = w->bpos[bc].p; g.out4[0] = w->bpos[bc ^ 1].p;
@@ -1210,10 +1214,11 @@ sph_status phase_grid(sph_world* w) {
     if (xys > 1) LAUNCH(k_cell_hist_xy, Nin, 256, w->pos[c].p + off, (uint32_t)Nin, w->cid.p, w->rank.p, w->cstart.p);  // (never a slab world: no dead slots)
     else LAUNCH(k_cell_hist, Nin, 256, w->pos[c].p + off, (uint32_t)Nin, w->cid.p, w->rank.p, w->cstart.p, dead, n_dead);
     TRY(scan_exclusive(w, w->cstart.p, ncell + 1));
-    LAUNCH(k_cell_scatter, Nin, 256, (uint32_t)Nin, w->cid.p, w->rank.p, w->cstart.p, w->perm.p);
-    if (w->desc.deterministic)
-        LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->cstart.p, w->perm.p, (const uint32_t*)w->gid[c].p + off,
-               w->fluids.size() > 1 ? (const float4*)w->vel[c].p + off : (const float4*)nullptr);
+    const bool det = w->desc.deterministic;
+    if (det) CU(w->skey.ensure(Nin));  // (a step graph's envelope allocated it: no allocation in capture)
+    LAUNCH(k_cell_scatter, Nin, 256, (uint32_t)Nin, w->cid.p, w->rank.p, w->cstart.p, w->perm.p, (const uint32_t*)w->gid[c].p + off,
+           w->fluids.size() > 1 ? (const float4*)w->vel[c].p + off : (const float4*)nullptr, det ? w->skey.p : nullptr);
+    if (det) LAUNCH(k_cell_sort, ncell, 256, (uint32_t)ncell, w->cstart.p, w->perm.p, w->skey.p);
     if (N) {
         GatherSet g;
         memset(&g, 0, sizeof g);
@@ -1405,13 +1410,13 @@ bool any_bforce(const sph_world* w) {
 
 // ---- gather passes: one wrapper per reference function ------------------------------------
 
-// ghost refresh of v* in whichever representation the evaluations gather (one NCCL group); vs itself is included
-// because the velocity fold reads vel = v* for ghosts too
+// ghost refresh of v* in whichever representation the evaluations and the velocity fold (vel = v* for ghosts too) read:
+// the packed records on the uniform-mass path (one NCCL group), else vs
 sph_status refresh_vstar(sph_world* w) {
     if (!w->slab.active) return SPH_OK;
     if (w->unimass) {
-        SlabArray a[3] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}, {w->vs.p, sizeof(float4)}};
-        return slab_refresh_n(w, a, 3);
+        SlabArray a[2] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}};
+        return slab_refresh_n(w, a, 2);
     }
     return slab_refresh(w, w->vs.p, sizeof(float4));
 }
@@ -1584,15 +1589,15 @@ sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) 
     const Lists L = w->lists.view();
     if (w->unimass) CU(w->tex_pk.bind(w->pk4));
     if (normals) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
-    // the following evaluation gathers v*_j of ghosts (vs itself too: the velocity fold reads vel = v* for ghosts)
-    SlabArray a[3] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}, {w->vs.p, sizeof(float4)}};
+    // the following evaluation gathers v*_j of ghosts (and the velocity fold reads vel = v* for ghosts)
+    SlabArray a[2] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}};
     SlabArray a1[1] = {{w->vs.p, sizeof(float4)}};
-    return run_parts(w, w->unimass ? a : a1, w->unimass ? 3 : 1, nullptr, [&](Range rg, uint32_t) -> sph_status {
+    return run_parts(w, w->unimass ? a : a1, w->unimass ? 2 : 1, nullptr, [&](Range rg, uint32_t) -> sph_status {
         if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
-            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
+            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
                      w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
         else if (w->unimass)
-            DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->vs.p, w->pvx4.p,
+            DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
                       w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr, rg);
         else
             BOOL3(k_vel_update, multi, bf, pressure, rg, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p, w->bforce.p, w->inv_dt);
@@ -1850,7 +1855,8 @@ sph_status dfsph_fold(sph_world* w, float remaining, const float g[3], uint32_t 
         LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale, w->dt,
                w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
     } else {
-        LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale);  // ghosts too (vel = v*)
+        LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale,  // ghosts too (vel = v*)
+               w->unimass ? (const float4*)w->pvx4.p : nullptr, w->unimass ? (const float2*)w->vyz2.p : nullptr);
         TRY(ev_record(w, EV_FOLD));
         if (!quiet_forces) TRY(phase_forces(w, fold));
         TRY(ev_record(w, EV_FORCES));
@@ -1998,7 +2004,8 @@ sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
         CellBox* next = &w->d_ss.p->next;
         if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(next);
         else CU(cudaMemcpyAsync(next, &CELL_BOX_EMPTY, sizeof(CellBox), cudaMemcpyHostToDevice, w->st));
-        LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->dt, w->slab.active ? nullptr : next);  // :411-420
+        LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->unimass ? (const float4*)w->pvx4.p : nullptr,
+               w->unimass ? (const float2*)w->vyz2.p : nullptr, w->dt, w->slab.active ? nullptr : next);  // :411-420
         w->nb_pending = !w->slab.active;
     }
     CU(cudaGetLastError());

@@ -403,71 +403,108 @@ __global__ void k_bounds(const float4* __restrict__ pos, uint32_t n, CellBox* __
 // K1: counting sort by cell (replaces HGrid::insert hgrid.rs:60-63 / insert_*_to_grid contacts.rs:133-151
 // and the dead z_order.rs sort).
 // ------------------------------------------------------------------------------------------------
+// In-cell ranks take one atomic per distinct cell of a warp (__match_any_sync), and follow input order within the warp.  The
+// input is usually the previous step's sorted order, so most cells leave the scatter already in canonical order and the
+// sort below only fixes what the order of the warps' atomics shuffled.  live == false (a tail lane or a dead slot) takes no rank.
+__device__ __forceinline__ uint32_t warp_cell_rank(uint32_t id, bool live, uint32_t* __restrict__ count) {
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t peers = __match_any_sync(0xffffffffu, live ? id : 0xFFFFFFFFu);
+    const uint32_t leader = __ffs(peers) - 1u;
+    uint32_t base = 0u;
+    if (live && lane == leader) base = atomicAdd(&count[id], (uint32_t)__popc(peers));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    return base + __popc(peers & ((1u << lane) - 1u));
+}
+
 // dead (optional): dead[i] != 0 for i < n_dead marks an input slot that must not enter the sorted arrays (a particle that left
 // this rank's slab, sph_slab.inl); such slots get cid = 0xFFFFFFFF and are skipped by the scatter.
+// Every lane of a warp runs to the rank (no early return): __match_any_sync takes the whole warp.
 __global__ void k_cell_hist(const float4* __restrict__ pos, uint32_t n, uint32_t* __restrict__ cid, uint32_t* __restrict__ rank,
                             uint32_t* __restrict__ count, const uint32_t* __restrict__ dead, uint32_t n_dead) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    if (dead && i < n_dead && dead[i]) {
-        cid[i] = 0xFFFFFFFFu;
-        return;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool in = i < n;
+    const bool live = in && !(dead && i < n_dead && dead[i]);
+    uint32_t id = 0xFFFFFFFFu;
+    if (live) {
+        const float4 p = pos[i];
+        id = (uint32_t)cell_id(cell_coord(p.x), cell_coord(p.y), cell_coord(p.z));
     }
-    float4 p = pos[i];
-    uint32_t id = (uint32_t)cell_id(cell_coord(p.x), cell_coord(p.y), cell_coord(p.z));
+    const uint32_t r = warp_cell_rank(id, live, count);
+    if (!in) return;
     cid[i] = id;
-    rank[i] = atomicAdd(&count[id], 1u);
+    if (live) rank[i] = r;
 }
 
 // row order (Consts::xysub > 1): x and y binned finer than h
 __global__ void k_cell_hist_xy(const float4* __restrict__ pos, uint32_t n, uint32_t* __restrict__ cid, uint32_t* __restrict__ rank,
                                uint32_t* __restrict__ count) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    float4 p = pos[i];
-    uint32_t id = (uint32_t)cell_id(abin(p.x, C.xysub, C.xysub_f), abin(p.y, C.xysub, C.xysub_f), cell_coord(p.z));
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    const bool live = i < n;
+    uint32_t id = 0xFFFFFFFFu;
+    if (live) {
+        const float4 p = pos[i];
+        id = (uint32_t)cell_id(abin(p.x, C.xysub, C.xysub_f), abin(p.y, C.xysub, C.xysub_f), cell_coord(p.z));
+    }
+    const uint32_t r = warp_cell_rank(id, live, count);
+    if (!live) return;
     cid[i] = id;
-    rank[i] = atomicAdd(&count[id], 1u);
+    rank[i] = r;
 }
 
+// Deterministic mode: atomics hand out in-cell ranks in arbitrary order; k_cell_sort sorts each cell's slice of perm so the
+// sorted order (and every f32 summation order downstream) is reproducible.  The in-cell order is CANONICAL — ascending
+// (fluid, particle id), ties by source slot, a pure function of the particle set — so a world restored from a snapshot, a
+// world whose state went through the host, and the ranks of a slab decomposition (ghost columns!) all see the same order and
+// produce bit-identical sums.  Boundaries pass their original indices (borig) as the key, so their in-cell order is insertion
+// order whether the input is a fresh upload or a sort of boundaries that colliders moved on the device.
+__device__ __forceinline__ unsigned long long sort_key(uint32_t src, const uint32_t* __restrict__ gid, const float4* __restrict__ vel) {
+    const uint32_t f = vel ? fid_of(vel[src]) : 0u;
+    return ((unsigned long long)f << 32) | gid[src];
+}
+// key (optional, deterministic mode): each entry's sort key beside perm, so the in-cell sort reads keys contiguously instead of
+// through gid[perm[.]].  gid / vel as for sort_key.
 __global__ void k_cell_scatter(uint32_t n, const uint32_t* __restrict__ cid, const uint32_t* __restrict__ rank,
-                               const uint32_t* __restrict__ start, uint32_t* __restrict__ perm) {
+                               const uint32_t* __restrict__ start, uint32_t* __restrict__ perm, const uint32_t* __restrict__ gid = nullptr,
+                               const float4* __restrict__ vel = nullptr, unsigned long long* __restrict__ key = nullptr) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t c = cid[i];
     if (c == 0xFFFFFFFFu) return;
-    perm[start[c] + rank[i]] = i;
+    const uint32_t d = start[c] + rank[i];
+    perm[d] = i;
+    if (key) key[d] = sort_key(i, gid, vel);
 }
 
-// Deterministic mode: atomics hand out in-cell ranks in arbitrary order; sort each cell's slice of perm so the sorted
-// order (and every f32 summation order downstream) is reproducible.  The in-cell order is CANONICAL — ascending
-// (fluid, particle id), a pure function of the particle set — so a world restored from a snapshot, a world whose state
-// went through the host, and the ranks of a slab decomposition (ghost columns!) all see the same order and produce
-// bit-identical sums.  Boundaries pass their original indices (borig) as the key, so their in-cell order is insertion
-// order whether the input is a fresh upload or a sort of boundaries that colliders moved on the device.  key == nullptr:
-// ascending previous slot.
-__device__ __forceinline__ unsigned long long sort_key(uint32_t src, const uint32_t* __restrict__ gid, const float4* __restrict__ vel) {
-    if (!gid) return src;
-    const uint32_t f = vel ? fid_of(vel[src]) : 0u;
-    return ((unsigned long long)f << 32) | gid[src];
-}
-__global__ void k_cell_sort(uint32_t ncell, const uint32_t* __restrict__ start, uint32_t* __restrict__ perm, const uint32_t* __restrict__ gid,
-                            const float4* __restrict__ vel) {
+// Insertion sort of each cell's slice by (key, source slot).  The largest entry so far stays in registers, so an entry already
+// in place costs one load of its key and slot and one compare; keys move with their slots.
+__global__ void k_cell_sort(uint32_t ncell, const uint32_t* __restrict__ start, uint32_t* __restrict__ perm, unsigned long long* __restrict__ key) {
     uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= ncell) return;
-    uint32_t s = start[c], e = start[c + 1];
+    const uint32_t s = start[c], e = start[c + 1];
+    if (e - s < 2u) return;
+    unsigned long long kt = key[s];
+    uint32_t ut = perm[s];
     for (uint32_t a = s + 1; a < e; ++a) {
         const uint32_t v = perm[a];
-        const unsigned long long kv = sort_key(v, gid, vel);
-        uint32_t b = a;
+        const unsigned long long kv = key[a];
+        if (kt < kv || (kt == kv && ut < v)) {
+            kt = kv;
+            ut = v;
+            continue;
+        }
+        perm[a] = ut;
+        key[a] = kt;
+        uint32_t b = a - 1;
         while (b > s) {
             const uint32_t u = perm[b - 1];
-            const unsigned long long ku = sort_key(u, gid, vel);
+            const unsigned long long ku = key[b - 1];
             if (ku < kv || (ku == kv && u < v)) break;
             perm[b] = u;
+            key[b] = ku;
             --b;
         }
         perm[b] = v;
+        key[b] = kv;
     }
 }
 
@@ -1018,6 +1055,7 @@ constexpr int PASS_T = SPH_PASS_T;  // threads per block of the gather passes
 
 // The fluid reorder fused with v* = vel + vc: the sorted pos / vel / vc are in registers anyway, so v* and the packed
 // gather records are written by the same pass (saves re-reading 48 B per particle and a launch).  g.in4 / out4 [0..2] = pos, vel, vc.
+// Uniform mass (pvx != nullptr): v* lives only in the packed records pvx.w and vyz, and vs is not written.
 __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, GatherSet g, float4* __restrict__ vs, float4* __restrict__ pvx,
                                float2* __restrict__ vyz) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1031,11 +1069,19 @@ __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, Ga
     for (int a = 0; a < 4; ++a)
         if (a < g.n1) g.out1[a][s] = g.in1[a][src];
     const float sx = v.x + c.x, sy = v.y + c.y, sz = v.z + c.z;
-    vs[s] = make_float4(sx, sy, sz, 0.f);
     if (pvx) {
         pvx[s] = make_float4(p.x, p.y, p.z, sx);
         vyz[s] = make_float2(sy, sz);
+    } else {
+        vs[s] = make_float4(sx, sy, sz, 0.f);
     }
+}
+
+// v* of slot i: from the packed records on the uniform-mass path (pvx != nullptr), else from vs
+__device__ __forceinline__ float4 load_vstar(uint32_t i, const float4* __restrict__ vs, const float4* __restrict__ pvx, const float2* __restrict__ vyz) {
+    if (!pvx) return vs[i];
+    const float2 b = vyz[i];
+    return make_float4(pvx[i].w, b.x, b.y, 0.f);
 }
 
 // a10: update_velocities dfsph_solver.rs:422-430 + zero vc :689-691 + acc = gravity (predict_advection :574-578).
@@ -1043,12 +1089,12 @@ __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, Ga
 // same for owned particles, and ghost particles (multi-GPU) only carry an up-to-date v*.
 // xs (optional): a force sum of the divergence loop (k_vel_divergence_xsph_u): acc = g + xs * scale, rounded like the force
 // pass's `acc += f * scale` on top of the gravity written here.  XSPH sums: scale = inv_dt; the Akinci force: scale = 1, so
-// acc = g + f exactly as `acc = g; acc += f`.
+// acc = g + f exactly as `acc = g; acc += f`.  pvx / vyz: as for load_vstar.
 __global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__ vc, const float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
-                                  float gz, const float4* __restrict__ xs, float scale) {
+                                  float gz, const float4* __restrict__ xs, float scale, const float4* __restrict__ pvx, const float2* __restrict__ vyz) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
-    float4 v = vel[i], s = vs[i];
+    const float4 v = vel[i], s = load_vstar(i, vs, pvx, vyz);
     vel[i] = make_float4(s.x, s.y, s.z, v.w);
     vc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     float ax = gx, ay = gy, az = gz;
@@ -1063,11 +1109,21 @@ __global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__
 // update_velocities + the gravity / folded-force acceleration + integrate_and_clear_accelerations in ONE pass, for steps whose force
 // phase launches nothing (no plugin, or only the force whose sum rode with the divergence loop): same arithmetic, in the same
 // order, as k_fold_velocities followed by k_integrate_acc.  Ghost slots (multi-GPU) only take the fold part.
+// Uniform mass (pvx != nullptr): v* is read from and written to the packed records only; the whole of pvx[i] is loaded anyway,
+// so it is stored whole (xyz unchanged) rather than as a partial .w store.
 __global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ vc, float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
                                  float gz, const float4* __restrict__ xs, float scale, float dt_new, float4* __restrict__ pvx, float2* __restrict__ vyz) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
-    const float4 v = vel[i], s = vs[i];
+    const float4 v = vel[i];
+    float4 s, r;  // v*, and (uniform mass) the packed record
+    if (pvx) {
+        r = pvx[i];
+        const float2 b = vyz[i];
+        s = make_float4(r.w, b.x, b.y, 0.f);
+    } else {
+        s = vs[i];
+    }
     const float4 nv = make_float4(s.x, s.y, s.z, v.w);
     vel[i] = nv;
     const bool owned = i >= C.i_begin && i < C.i_begin + C.n_owned;
@@ -1086,10 +1142,11 @@ __global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ 
     const float cx = __fmul_rn(ax, dt_new), cy = __fmul_rn(ay, dt_new), cz = __fmul_rn(az, dt_new);  // vc = 0 + acc * dt
     vc[i] = make_float4(cx, cy, cz, 0.f);
     const float sx = nv.x + cx, sy = nv.y + cy, sz = nv.z + cz;
-    vs[i] = make_float4(sx, sy, sz, 0.f);
     if (pvx) {
-        pvx[i].w = sx;
+        pvx[i] = make_float4(r.x, r.y, r.z, sx);
         vyz[i] = make_float2(sy, sz);
+    } else {
+        vs[i] = make_float4(sx, sy, sz, 0.f);
     }
 }
 // IISPH variant: accelerations += gravity only (vc is already zero, velocities untouched).
@@ -1110,10 +1167,11 @@ __global__ void k_integrate_acc(const float4* __restrict__ vel, float4* __restri
     c.x += a.x * dt; c.y += a.y * dt; c.z += a.z * dt;
     vc[i] = c;
     float sx = v.x + c.x, sy = v.y + c.y, sz = v.z + c.z;
-    vs[i] = make_float4(sx, sy, sz, 0.f);
-    if (pvx) {
+    if (pvx) {  // uniform mass: v* only in the packed records
         pvx[i].w = sx;  // xyz already hold the position
         vyz[i] = make_float2(sy, sz);
+    } else {
+        vs[i] = make_float4(sx, sy, sz, 0.f);
     }
 }
 
@@ -1138,13 +1196,16 @@ __global__ void k_cfl_max(const float4* __restrict__ vel, const float4* __restri
 
 // a22: update_positions dfsph_solver.rs:411-420: pos += (vel + vc) * dt.  bounds_out (optional): the cell-coordinate AABB of
 // the NEW positions (what k_bounds computes), so the next step's grid is sized without a bounds pass and its host round trip.
-__global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, float dt, CellBox* __restrict__ bounds_out) {
+// pvx / vyz: as for load_vstar.
+__global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, const float4* __restrict__ pvx, const float2* __restrict__ vyz,
+                                   float dt, CellBox* __restrict__ bounds_out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = i < C.n_owned;
     i += C.i_begin;
     CellBox b = CELL_BOX_EMPTY;
     if (valid) {
-        float4 p = pos[i], v = vs[i];
+        float4 p = pos[i];
+        const float4 v = load_vstar(i, vs, pvx, vyz);
         p.x += v.x * dt; p.y += v.y * dt; p.z += v.z * dt;
         pos[i] = p;
         if (bounds_out) cell_box_add(b, p.x, p.y, p.z, C.h);

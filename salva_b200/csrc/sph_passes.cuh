@@ -501,7 +501,7 @@ k_akinci_force_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const
 template <bool BFORCE, bool PRESSURE, bool NORMALS = false>
 __global__ void __launch_bounds__(PASS_T, NORMALS && SPH_GENERIC_KERNELS ? SPH_FORCE_MINB : SPH_PASS_MINB)  // generic kernels: spills at 56
 k_vel_update_u(const float4* __restrict__ pk4, cudaTextureObject_t tpk, const float4* __restrict__ vel, const float4* __restrict__ bpos, Lists L,
-               float4* __restrict__ vc, float4* __restrict__ vs, float4* __restrict__ pvx, float2* __restrict__ vyz, float* __restrict__ bforce,
+               float4* __restrict__ vc, float4* __restrict__ pvx, float2* __restrict__ vyz, float* __restrict__ bforce,
                float inv_dt, const float* __restrict__ dens, float4* __restrict__ nr4, Range rg) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= rg.count) return;
@@ -544,8 +544,7 @@ k_vel_update_u(const float4* __restrict__ pk4, cudaTextureObject_t tpk, const fl
     float4 c4 = vc[i];
     c4.x -= ax; c4.y -= ay; c4.z -= az;
     vc[i] = c4;
-    const float sx = v.x + c4.x, sy = v.y + c4.y, sz = v.z + c4.z;
-    vs[i] = make_float4(sx, sy, sz, 0.f);
+    const float sx = v.x + c4.x, sy = v.y + c4.y, sz = v.z + c4.z;  // v*: only in the packed records on this path
     pvx[i] = make_float4(a.x, a.y, a.z, sx);
     vyz[i] = make_float2(sy, sz);
 }
