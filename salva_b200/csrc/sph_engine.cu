@@ -397,8 +397,7 @@ struct SlabArray {
     void* p;
     size_t elem;
 };
-sph_status slab_refresh_n(sph_world* w, const SlabArray* arrays, int n_arrays, cudaStream_t st = nullptr);
-sph_status slab_wait(sph_world* w);
+sph_status slab_refresh_n(sph_world* w, const SlabArray* arrays, int n_arrays);
 sph_status p2p_setup(sph_world* w);
 sph_status post_density_refresh(sph_world* w);
 sph_status slab_allreduce(sph_world* w, float* buf, size_t n);
@@ -443,10 +442,6 @@ struct SlabState {
     DBuf<unsigned long long> d_cnt64;
     DBuf<float4> out_l[3], out_r[3], col_l[3], col_r[3];
     bool global_valid = false;
-    // exchange / compute overlap: boundary columns first, their exchange on comm_st behind the interior launch
-    bool overlap = false, pending = false;  // off by default: the step of a 4M-particle slab is host-launch bound, the overlap did not pay
-    cudaStream_t comm_st = nullptr;
-    cudaEvent_t ev_ready = nullptr, ev_done = nullptr;
     // slot ranges of the current step (after the sort)
     uint32_t gl_count = 0, sl_begin = 0, sl_count = 0, sr_begin = 0, sr_count = 0, gr_begin = 0, gr_count = 0;
     uint32_t exp_ghost_l = 0, exp_ghost_r = 0, exp_send_l = 0, exp_send_r = 0;
@@ -974,7 +969,7 @@ sph_status ensure_fluid_buffers(sph_world* w) {
     w->stride = (uint32_t)((N + 31) / 32 * 32);
     CU(w->lists.ensure(N, w->stride));
     uint32_t nblk = cdiv(std::max<size_t>(N, 1), std::min(PASS_T, NBR_T));
-    CU(w->partial.ensure((size_t)(nblk + 3) * std::max<size_t>(1, w->fluids.size())));  // +3: a slab pass may run as three sub-range launches
+    CU(w->partial.ensure((size_t)nblk * std::max<size_t>(1, w->fluids.size())));
     return SPH_OK;
 }
 
@@ -1257,7 +1252,6 @@ sph_status density_args(sph_world* w, DensArgs* D) {
     } else {
         CU(w->tex_vs.bind(w->vs));
     }
-    TRY(slab_wait(w));  // the sweep gathers v* of ghosts
     *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx.obj : 0, w->vs.p, w->unimass ? 0 : w->tex_vs.obj, w->vyz2.p,
                   w->unimass ? w->tex_vyz.obj : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, &w->d_ss.p->err};
     return SPH_OK;
@@ -1402,6 +1396,16 @@ bool any_bforce(const sph_world* w) {
             else LAUNCH((kern<false, false>), n, threads, __VA_ARGS__);               \
         }                                                                             \
     } while (0)
+#define DISPATCH3(kern, b0, b1, b2, n, threads, ...)                                                                    \
+    do {                                                                                                                 \
+        if (b0) {                                                                                                        \
+            if (b1) { if (b2) LAUNCH((kern<true, true, true>), n, threads, __VA_ARGS__); else LAUNCH((kern<true, true, false>), n, threads, __VA_ARGS__); } \
+            else    { if (b2) LAUNCH((kern<true, false, true>), n, threads, __VA_ARGS__); else LAUNCH((kern<true, false, false>), n, threads, __VA_ARGS__); } \
+        } else {                                                                                                         \
+            if (b1) { if (b2) LAUNCH((kern<false, true, true>), n, threads, __VA_ARGS__); else LAUNCH((kern<false, true, false>), n, threads, __VA_ARGS__); } \
+            else    { if (b2) LAUNCH((kern<false, false, true>), n, threads, __VA_ARGS__); else LAUNCH((kern<false, false, false>), n, threads, __VA_ARGS__); } \
+        }                                                                                                                \
+    } while (0)
 #define DISPATCH1(kern, multi, n, threads, ...)                         \
     do {                                                                \
         if (multi) LAUNCH((kern<true>), n, threads, __VA_ARGS__);       \
@@ -1422,7 +1426,7 @@ sph_status refresh_vstar(sph_world* w) {
 }
 // ghost refresh of the evaluation's output (kappa) — only needed when an update follows
 sph_status refresh_kappa(sph_world* w) {
-    if (!w->slab.active || w->slab.overlap) return SPH_OK;  // overlap mode: the evaluation exchanged kappa speculatively
+    if (!w->slab.active) return SPH_OK;
     if (w->unimass) return slab_refresh(w, w->pk4.p, sizeof(float4));
     return slab_refresh(w, w->kappa.p, sizeof(float));
 }
@@ -1447,72 +1451,7 @@ sph_status post_density_refresh(sph_world* w) {
     }
     return slab_refresh(w, w->dens.p, sizeof(float));  // XSPH / artificial viscosity / Akinci gather rho_j of ghosts
 }
-// Launch over a slot range with n = range count (kernels index rg.begin + thread)
-#define LAUNCH_R(kern, rg, ...)                                                                   \
-    do {                                                                                          \
-        if ((rg).count > 0) {                                                                     \
-            kern<<<cdiv((rg).count, PASS_T), PASS_T, 0, w->st>>>(__VA_ARGS__, (rg));              \
-            w->launches++;                                                                        \
-        }                                                                                         \
-    } while (0)
-
-#define BOOL3(kern, b0, b1, b2, n, ...)                                                   \
-    do {                                                                                           \
-        if (b0) {                                                                                  \
-            if (b1) { if (b2) LAUNCH_R((kern<true, true, true>), n, __VA_ARGS__); else LAUNCH_R((kern<true, true, false>), n, __VA_ARGS__); } \
-            else    { if (b2) LAUNCH_R((kern<true, false, true>), n, __VA_ARGS__); else LAUNCH_R((kern<true, false, false>), n, __VA_ARGS__); } \
-        } else {                                                                                   \
-            if (b1) { if (b2) LAUNCH_R((kern<false, true, true>), n, __VA_ARGS__); else LAUNCH_R((kern<false, true, false>), n, __VA_ARGS__); } \
-            else    { if (b2) LAUNCH_R((kern<false, false, true>), n, __VA_ARGS__); else LAUNCH_R((kern<false, false, false>), n, __VA_ARGS__); } \
-        }                                                                                          \
-    } while (0)
-
-
-// ---- slot ranges of a launch and the producer/exchange overlap of a slab world ---------------------------------------
-// A pass that PRODUCES data its neighbours' ghosts need (kappa after an evaluation, v* after an update) is launched on
-// the two boundary columns first; their exchange then runs on the communication stream while the interior launch
-// proceeds on the main stream.  Every pass waits for the previous exchange before it reads ghost slots.
-sph_status slab_wait(sph_world* w) {
-    SlabState& S = w->slab;
-    if (S.pending) {
-        CU(cudaStreamWaitEvent(w->st, S.ev_done, 0));
-        S.pending = false;
-    }
-    return SPH_OK;
-}
-template <class Fn>  // fn(Range rg, uint32_t first_partial_block) -> sph_status
-sph_status run_parts(sph_world* w, const SlabArray* arrays, int n_arrays, uint32_t* nblk_total, Fn fn) {
-    SlabState& S = w->slab;
-    TRY(slab_wait(w));
-    uint32_t off = 0;
-    auto part = [&](uint32_t b, uint32_t cnt) -> sph_status {
-        if (!cnt) return SPH_OK;
-        TRY(fn(Range{b, cnt}, off));
-        off += cdiv(cnt, PASS_T);
-        return SPH_OK;
-    };
-    const uint32_t N = (uint32_t)w->N;
-    if (!S.active || !S.overlap || n_arrays == 0) {
-        TRY(part(w->own_begin, N));
-        if (S.active && n_arrays) TRY(slab_refresh_n(w, arrays, n_arrays));
-    } else {
-        TRY(part(S.sl_begin, S.sl_count));
-        TRY(part(S.sr_begin, S.sr_count));
-        CU(cudaEventRecord(S.ev_ready, w->st));
-        CU(cudaStreamWaitEvent(S.comm_st, S.ev_ready, 0));
-        TRY(slab_refresh_n(w, arrays, n_arrays, S.comm_st));
-        CU(cudaEventRecord(S.ev_done, S.comm_st));
-        S.pending = true;
-        const uint32_t ib = S.sl_begin + S.sl_count, ie = S.has_right ? S.sr_begin : w->own_begin + N;
-        TRY(part(ib, ie > ib ? ie - ib : 0));
-    }
-    if (nblk_total) *nblk_total = off;
-    return SPH_OK;
-}
-
 // compute_divergences (predict = false) / compute_predicted_densities (predict = true); returns #partials.
-// In a slab world with overlap the kappa ghosts are exchanged speculatively (the evaluation may turn out to be the
-// loop's last one) behind the interior launch; otherwise refresh_kappa() does it only when an update follows.
 // The fluid term of the FIRST force of a single-fluid DFSPH world can ride with the divergence evaluations when it is an
 // XSPHViscosity without a boundary term (see k_vel_divergence_xsph_u).
 bool xsph_fusable(const sph_world* w) {
@@ -1552,34 +1491,29 @@ sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, boo
         CU(w->tex_vs.bind(w->vs));
     }
     float* out = predict ? w->pred.p : w->divv.p;
-    const size_t nf = std::max<size_t>(1, w->fluids.size());
-    SlabArray a[1] = {{w->unimass ? (void*)w->pk4.p : (void*)w->kappa.p, w->unimass ? sizeof(float4) : sizeof(float)}};
-    const int n_arrays = (w->slab.active && w->slab.overlap) ? 1 : 0;
-    sph_status rs = run_parts(w, a, n_arrays, nblk, [&](Range rg, uint32_t blk) -> sph_status {
-        float* partial = w->partial.p + (size_t)blk * nf;
-        if (w->unimass) {
-            if (predict) {
-                LAUNCH_R((k_vel_divergence_u<true>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, &w->d_ss.p->err);
-            } else if (xsf) {
-                const float cf = w->fluids[0].forces[0].d.p[0];
-                LAUNCH_R((k_vel_divergence_xsph_u<1>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
-            } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
-                const AkinciNorms an = akinci_norms(w->h);
-                LAUNCH_R((k_vel_divergence_xsph_u<2>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p, w->alpha.p, out,
-                         w->pk4.p, partial, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
-            } else {
-                LAUNCH_R((k_vel_divergence_u<false>), rg, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L, w->dens.p,
-                         w->alpha.p, out, w->pk4.p, partial, w->dt, &w->d_ss.p->err);
-            }
+    const size_t N = w->N;
+    if (w->unimass) {
+        if (predict) {
+            LAUNCH((k_vel_divergence_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L,
+                   w->dens.p, w->alpha.p, out, w->pk4.p, w->partial.p, w->dt, &w->d_ss.p->err);
+        } else if (xsf) {
+            const float cf = w->fluids[0].forces[0].d.p[0];
+            LAUNCH((k_vel_divergence_xsph_u<1>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p,
+                   w->alpha.p, out, w->pk4.p, w->partial.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
+        } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
+            const AkinciNorms an = akinci_norms(w->h);
+            LAUNCH((k_vel_divergence_xsph_u<2>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p,
+                   w->alpha.p, out, w->pk4.p, w->partial.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
         } else {
-            DISPATCH2(k_vel_divergence, multi, predict, rg.count, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
-                      w->dens.p, w->alpha.p, out, w->kappa.p, partial, w->dt, &w->d_ss.p->err, rg);
+            LAUNCH((k_vel_divergence_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L,
+                   w->dens.p, w->alpha.p, out, w->pk4.p, w->partial.p, w->dt, &w->d_ss.p->err);
         }
-        return SPH_OK;
-    });
-    return rs;
+    } else {
+        DISPATCH2(k_vel_divergence, multi, predict, N, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
+                  w->dens.p, w->alpha.p, out, w->kappa.p, w->partial.p, w->dt, &w->d_ss.p->err);
+    }
+    *nblk = cdiv(N, PASS_T);
+    return SPH_OK;
 }
 // compute_velocity_changes_for_divergence (pressure = false) / compute_velocity_changes (pressure = true).
 // normals: the Akinci normals ride along (see akinci_fusable_u).
@@ -1589,20 +1523,17 @@ sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) 
     const Lists L = w->lists.view();
     if (w->unimass) CU(w->tex_pk.bind(w->pk4));
     if (normals) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
-    // the following evaluation gathers v*_j of ghosts (and the velocity fold reads vel = v* for ghosts)
-    SlabArray a[2] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}};
-    SlabArray a1[1] = {{w->vs.p, sizeof(float4)}};
-    return run_parts(w, w->unimass ? a : a1, w->unimass ? 2 : 1, nullptr, [&](Range rg, uint32_t) -> sph_status {
-        if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
-            LAUNCH_R((k_vel_update_u<false, false, true>), rg, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
-                     w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
-        else if (w->unimass)
-            DISPATCH2(k_vel_update_u, bf, pressure, rg.count, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
-                      w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr, rg);
-        else
-            BOOL3(k_vel_update, multi, bf, pressure, rg, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p, w->bforce.p, w->inv_dt);
-        return SPH_OK;
-    });
+    const size_t N = w->N;
+    if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
+        LAUNCH((k_vel_update_u<false, false, true>), N, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
+               w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
+    else if (w->unimass)
+        DISPATCH2(k_vel_update_u, bf, pressure, N, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
+                  w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr);
+    else
+        DISPATCH3(k_vel_update, multi, bf, pressure, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p,
+                  w->bforce.p, w->inv_dt);
+    return refresh_vstar(w);  // the following evaluation gathers v*_j of ghosts (and the velocity fold reads vel = v* for ghosts)
 }
 
 // ---- ParticlesContacts materialisation + the context-style host plugin call (nonpressure_force.rs:15-27) ---------------
@@ -1836,7 +1767,6 @@ sph_status timestep_advance(sph_world* w, float remaining) {
 sph_status dfsph_fold(sph_world* w, float remaining, const float g[3], uint32_t fold) {
     size_t N = w->N;
     int c = w->cur;
-    TRY(slab_wait(w));
     // the first force of fluid 0 may already sit in xs: the XSPH sums of the loop's last evaluation (acc = g + xs * inv_dt) or
     // the Akinci fluid force (acc = g + xs; a scale of 1 leaves the product exact)
     const bool folded = fold & (FOLD_XS | FOLD_AKINCI);
@@ -1999,7 +1929,6 @@ sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
         TRY(cond(w, tail, cudaGraphCondTypeIf, press_update));
     }
     TRY(ev_record(w, EV_PRESS));
-    TRY(slab_wait(w));  // a speculative exchange may still be in flight: it must land before the arrays are reused
     {
         CellBox* next = &w->d_ss.p->next;
         if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(next);
@@ -2720,14 +2649,6 @@ static sph_status slab_attach(sph_world* w, void* comm, bool own, int rank, int 
     w->desc.deterministic = 1;  // ghost-column order agreement relies on the stable in-cell order
     CU(S.d_cnt.ensure(32));
     CU(S.d_cnt64.ensure(1));
-    if (!S.comm_st) {
-        int lo_pri = 0, hi_pri = 0;
-        CU(cudaDeviceGetStreamPriorityRange(&lo_pri, &hi_pri));
-        CU(cudaStreamCreateWithPriority(&S.comm_st, cudaStreamNonBlocking, hi_pri));
-        CU(cudaEventCreateWithFlags(&S.ev_ready, cudaEventDisableTiming));
-        CU(cudaEventCreateWithFlags(&S.ev_done, cudaEventDisableTiming));
-    }
-    if (const char* t = getenv("SALVA_B200_SLAB_OVERLAP")) S.overlap = atoi(t) != 0;
     if (S.active) TRY(p2p_setup(w));
     return SPH_OK;
 }

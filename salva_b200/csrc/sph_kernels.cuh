@@ -216,21 +216,6 @@ __device__ __forceinline__ float kernel_w(float r) {
     float rhs = q <= 0.5f ? a : (q <= 1.0f ? b : 0.0f);
     return C.sigma * rhs;
 }
-// cubic_spline_kernel.rs:55-80 + kernel.rs:18-24: returns g with grad W_ij = g * (x_i - x_j);
-// zero if |x_ij|^2 <= eps^2, q <= 1e-5 or q > 1.
-__device__ __forceinline__ float kernel_gfac(float d2, float r, float inv_r) {
-    float q = r * C.inv_h;
-    float t = 1.0f - q;
-    float a = (q * 3.0f - 2.0f) * q * 6.0f;
-    float b = -t * t * 6.0f;
-    float rhs = q <= 0.5f ? a : b;
-    bool zero = (q > 1.0f) | (q <= 1.0e-5f) | !(d2 > F32_EPS * F32_EPS);
-    return zero ? 0.0f : C.dsigma * rhs * inv_r;
-}
-
-#ifndef SPH_FAST_PAIR
-#define SPH_FAST_PAIR 1
-#endif
 // MUFU.RSQ without the denormal-rescue sequence rsqrtf() compiles to (3 extra instructions per contact): operands
 // here are squared distances floored at 1e-30, far above the denormals.
 __device__ __forceinline__ float rsqrt_ftz(float x) {
@@ -316,13 +301,11 @@ __device__ __forceinline__ Pair make_pair(const float4& pi, const float4& pj) {
         p.g = o.y;
         return p;
     }
-#if SPH_FAST_PAIR
-    // Lean evaluation (about half the instructions of the guarded one below): contacts come from lists built with
-    // d^2 <= h^2, so q <= 1 up to rounding (where (1 - q)^2 ~ 1e-14 anyway), and the two "zero gradient" guards of the
-    // reference (|x_ij|^2 > eps^2, q > 1e-5) collapse into one select on d2.  r itself is the distance down to d2 = 0
-    // (the floor keeps rsqrt finite, so 0 * inv_r = 0): Akinci2013's cohesion and adhesion act on every pair with
-    // |x_ij|^2 > eps^2, below the gradient's threshold too, and divide by r.  W takes the true r as well; at q <= 1e-5,
-    // 1 - 6 q^2 rounds to 1 as it did with r = 0.
+    // Contacts come from lists built with d^2 <= h^2, so q <= 1 up to rounding (where (1 - q)^2 ~ 1e-14 anyway), and the
+    // two "zero gradient" guards of the reference (|x_ij|^2 > eps^2, q > 1e-5) collapse into one select on d2.  r itself
+    // is the distance down to d2 = 0 (the floor keeps rsqrt finite, so 0 * inv_r = 0): Akinci2013's cohesion and adhesion
+    // act on every pair with |x_ij|^2 > eps^2, below the gradient's threshold too, and divide by r.  W takes the true r as
+    // well; at q <= 1e-5, 1 - 6 q^2 rounds to 1 as it did with r = 0.
     const float inv_r = rsqrt_ftz(fmaxf(p.d2, 1.0e-30f));
     const bool nz = p.d2 > C.g_t2;
     p.r = p.d2 * inv_r;
@@ -344,12 +327,6 @@ __device__ __forceinline__ Pair make_pair(const float4& pi, const float4& pj) {
     } else {
         p.g = 0.f;
     }
-#else
-    float inv_r = rsqrtf(fmaxf(p.d2, 1.0e-30f));
-    p.r = p.d2 * inv_r;
-    p.w = NEED_W ? kernel_w(p.r) : 0.f;
-    p.g = NEED_G ? kernel_gfac(p.d2, p.r, inv_r) : 0.f;
-#endif
     return p;
 }
 

@@ -24,12 +24,6 @@ __device__ __forceinline__ auto call_gather(F& f, uint32_t j, int u) {
     else return f(j);
 }
 
-// Slot range a launch covers.  One launch normally covers all owned slots; a slab world splits the Jacobi-loop kernels
-// into [boundary columns] + [interior] so the ghost exchange of the boundary columns overlaps the interior launch.
-struct Range {
-    uint32_t begin, count;
-};
-
 // ldpos(j) -> float4 whose xyz is the neighbour position (w = whatever the array packs there); ld(j) -> Aux loads
 // whatever else the pass needs from neighbour j; ff(j, pair, posrec_j, aux) consumes one contact.
 template <bool W, bool G, class LP, class LD, class FF>
@@ -206,11 +200,11 @@ __global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
 k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, cudaTextureObject_t tvs, const float4* __restrict__ vel,
                  const float4* __restrict__ bpos, const float4* __restrict__ bvel, Lists L, const float* __restrict__ dens,
                  const float* __restrict__ alpha, float* __restrict__ out, float* __restrict__ kappa, float* __restrict__ partial, float dt,
-                 int* __restrict__ err, Range rg) {
+                 int* __restrict__ err) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    bool valid = i < rg.count;
-    i += rg.begin;
+    bool valid = i < C.n_owned;
+    i += C.i_begin;
     float e = 0.f;
     uint32_t fi = 0;
     if (valid) {
@@ -262,10 +256,8 @@ k_vel_divergence(const float4* __restrict__ pos, const float4* __restrict__ vs, 
 template <bool MULTI, bool BFORCE, bool PRESSURE>
 __global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
 k_vel_update(const float4* __restrict__ pos, const float4* __restrict__ vel, const float4* __restrict__ bpos, Lists L, const float* __restrict__ kappa,
-             float4* __restrict__ vc, float4* __restrict__ vs, float* __restrict__ bforce, float inv_dt, Range rg) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= rg.count) return;
-    i += rg.begin;
+             float4* __restrict__ vc, float4* __restrict__ vs, float* __restrict__ bforce, float inv_dt) {
+    SPH_OWNED_INDEX(i)
     float4 pi = pos[i];
     float4 v = vel[i];
     float rho0 = C.fluids[MULTI ? fid_of(v) : 0].density0;
@@ -309,11 +301,11 @@ __global__ void __launch_bounds__(PASS_T, SPH_PASS_MINB)
 k_vel_divergence_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float2* __restrict__ vyz, cudaTextureObject_t tvyz,
                    const float4* __restrict__ bpos, const float4* __restrict__ bvel, Lists L, const float* __restrict__ dens,
                    const float* __restrict__ alpha, float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, float dt,
-                   int* __restrict__ err, Range rg) {
+                   int* __restrict__ err) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    bool valid = i < rg.count;
-    i += rg.begin;
+    bool valid = i < C.n_owned;
+    i += C.i_begin;
     float e = 0.f;
     if (valid) {
         const float4 a = pvx[i];
@@ -404,11 +396,11 @@ __global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)  // 64 registers: the 
 k_vel_divergence_xsph_u(const float4* __restrict__ pvx, cudaTextureObject_t tpvx, const float2* __restrict__ vyz, cudaTextureObject_t tvyz,
                         const float4* __restrict__ bpos, Lists L, const float* __restrict__ dens, const float* __restrict__ alpha,
                         float* __restrict__ out, float4* __restrict__ pk4, float* __restrict__ partial, float4* __restrict__ xs, float cf, const float4* __restrict__ nr4, float coh_norm,
-                        float h6_64, Range rg) {
+                        float h6_64) {
     __shared__ float sm[32];
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    bool valid = i < rg.count;
-    i += rg.begin;
+    bool valid = i < C.n_owned;
+    i += C.i_begin;
     float e = 0.f;
     if (valid) {
         const float4 a = pvx[i];
@@ -502,10 +494,8 @@ template <bool BFORCE, bool PRESSURE, bool NORMALS = false>
 __global__ void __launch_bounds__(PASS_T, NORMALS && SPH_GENERIC_KERNELS ? SPH_FORCE_MINB : SPH_PASS_MINB)  // generic kernels: spills at 56
 k_vel_update_u(const float4* __restrict__ pk4, cudaTextureObject_t tpk, const float4* __restrict__ vel, const float4* __restrict__ bpos, Lists L,
                float4* __restrict__ vc, float4* __restrict__ pvx, float2* __restrict__ vyz, float* __restrict__ bforce,
-               float inv_dt, const float* __restrict__ dens, float4* __restrict__ nr4, Range rg) {
-    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= rg.count) return;
-    i += rg.begin;
+               float inv_dt, const float* __restrict__ dens, float4* __restrict__ nr4) {
+    SPH_OWNED_INDEX(i)
     const float4 a = pk4[i];
     const float4 pi = make_float4(a.x, a.y, a.z, 0.f);
     const float ki = a.w;
