@@ -291,6 +291,20 @@ struct SurfaceMesh {
     std::vector<Vector3> normals;
     std::vector<uint32_t> triangles;  // 3 vertex indices per triangle
 };
+// The anisotropic surface kernels (include/sph.h sph_surface_anisotropy, DESIGN.md section 17); the defaults are
+// sph_surface_anisotropy_default's: smoothed centres with round kernels
+struct SurfaceAnisotropy {
+    Real smoothing = 0.9f;        // lambda in [0, 1]
+    Real max_ratio = 1.f;         // k_r in [1, 1000]
+    Real isolated_radius = 1.f;   // k_n in [0.001, 1], in units of h
+    uint32_t min_neighbours = 6;  // N_eps
+};
+// One fluid's ellipsoids of the last extraction (LiquidWorld::surface_ellipsoids), in its particle order: per particle the
+// centre and 12 floats (e1, a1, e2, a2, e3, a3), a1 >= a2 >= a3
+struct SurfaceEllipsoids {
+    std::vector<Point3> centres;
+    std::vector<Real> axes;
+};
 // The diffuse particles of a world (LiquidWorld::diffuse), in order; kinds are SPH_DIFFUSE_SPRAY / _FOAM / _BUBBLE
 struct DiffuseParticles {
     std::vector<Point3> positions;
@@ -437,11 +451,37 @@ public:
     // meshes the fluids' AABB grown by h, where every surface closes; a box clips the lattice and leaves surfaces open there.
     SurfaceMesh extract_surface(Real iso = 0.6f, Real spacing = 0.f, const std::vector<FluidHandle>& fluids = {}, bool normals = true,
                                 const Vector3& lo = Vector3{1, 1, 1}, const Vector3& hi = Vector3{0, 0, 0}) {
+        return extract_surface_with(nullptr, iso, spacing, fluids, normals, lo, hi);
+    }
+    // The same surface with the anisotropic field (include/sph.h sph_world_extract_surface_anisotropic, DESIGN.md section 17):
+    // smoothed centres and per-particle ellipsoidal kernels, whose rows surface_ellipsoids reads.
+    SurfaceMesh extract_surface(const SurfaceAnisotropy& aniso, Real iso = 0.6f, Real spacing = 0.f, const std::vector<FluidHandle>& fluids = {},
+                                bool normals = true, const Vector3& lo = Vector3{1, 1, 1}, const Vector3& hi = Vector3{0, 0, 0}) {
+        return extract_surface_with(&aniso, iso, spacing, fluids, normals, lo, hi);
+    }
+    // The last extraction's ellipsoids of `fluid` (empty after an isotropic extraction or when the fluid was not selected).
+    SurfaceEllipsoids surface_ellipsoids(FluidHandle fluid) {
+        const uint32_t h = fluids_.at(fluid).handle_;
+        size_t n = 0;
+        check(sph_world_read_surface_ellipsoids(raw_, h, nullptr, nullptr, 0, &n));
+        SurfaceEllipsoids e;
+        e.centres.resize(n);
+        e.axes.resize(12 * n);
+        check(sph_world_read_surface_ellipsoids(raw_, h, reinterpret_cast<float*>(e.centres.data()), e.axes.data(), n, &n));
+        return e;
+    }
+    SurfaceMesh extract_surface_with(const SurfaceAnisotropy* aniso, Real iso, Real spacing, const std::vector<FluidHandle>& fluids, bool normals,
+                                     const Vector3& lo, const Vector3& hi) {
         std::vector<uint32_t> hs;
         for (FluidHandle f : fluids) hs.push_back(fluids_.at(f).handle_);
         const sph_surface_desc d{iso, spacing > 0.f ? spacing : particle_radius(), {lo.x, lo.y, lo.z}, {hi.x, hi.y, hi.z}, normals ? 1 : 0};
         size_t nv = 0, nt = 0;
-        check(sph_world_extract_surface(raw_, hs.data(), hs.size(), &d, &nv, &nt));
+        if (aniso) {
+            const sph_surface_anisotropy a{aniso->smoothing, aniso->max_ratio, aniso->isolated_radius, aniso->min_neighbours};
+            check(sph_world_extract_surface_anisotropic(raw_, hs.data(), hs.size(), &d, &a, &nv, &nt));
+        } else {
+            check(sph_world_extract_surface(raw_, hs.data(), hs.size(), &d, &nv, &nt));
+        }
         SurfaceMesh m;
         m.vertices.resize(nv);
         m.normals.resize(normals ? nv : 0);

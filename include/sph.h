@@ -515,6 +515,58 @@ sph_status sph_world_map_surface(sph_world* w, const float** d_vertices_xyz, con
  * lattice was built).  phi == NULL: only origin and dims are written.  SPH_ERR_INVALID when cap is below the point count. */
 sph_status sph_world_read_surface_field(sph_world* w, float* phi, size_t cap, float origin[3], uint32_t dims[3]);
 
+/* Anisotropic fluid surfaces (Yu & Turk 2013, "Reconstructing surfaces of particle-based fluids using anisotropic kernels";
+ * DESIGN.md section 17).  The same lattice, inside rule, polygonisation, orderings and sph_world_read_surface_field as
+ * sph_world_extract_surface; only phi and the normals differ.  Over the selected fluids' particles with finite positions x_i
+ * (the positions of the last step; before the first step: those given), with volumes V_i, the world's h and its kernels:
+ *   1. Neighbours of i: the j != i with |x_ij|^2 <= h^2 under the step's unfused float32 pair test (the test of
+ *      sph_world_update_diffuse step 3); N_i their count.  Weights w_ij = 1 - (|x_ij| / h)^3; i itself enters the sums below
+ *      with w_ii = 1 but is not counted in N_i.
+ *   2. Weighted mean x^w_i = sum w_ij x_j / sum w_ij; centre x_bar_i = (1 - lambda) x_i + lambda x^w_i.
+ *   3. Covariance C_i = sum w_ij (x_j - x^w_i)(x_j - x^w_i)^T / sum w_ij, eigenvalues s1 >= s2 >= s3 >= 0, orthonormal
+ *      eigenvectors e1, e2, e3 (cyclic Jacobi in float32, at most 8 sweeps).
+ *   4. Radii: if N_i >= N_eps and s1 > 0, a_k = h max(s_k, s1 / k_r) / s1, so a1 = h and every a_k lies in [h / k_r, h];
+ *      otherwise a1 = a2 = a3 = k_n h with the axes x, y, z.
+ *   5. Kernel: G_i = sum_k e_k e_k^T / a_k, W_i(x) = (h^3 / (a1 a2 a3)) W(h |G_i (x - x_bar_i)|) with W the world's density
+ *      kernel.  W_i integrates to 1 and vanishes outside the ellipsoid of semi-axes a_k <= h around x_bar_i.
+ *   6. Field phi(x) = sum_i V_i W_i(x); normals -grad phi / |grad phi| with grad W_i(x) = (h^3 / (a1 a2 a3)) h G_i grad W(u),
+ *      u = h G_i (x - x_bar_i), the world's gradient kernel, grad W(u) = 0 for |u|^2 <= eps^2, and 0 where grad phi = 0.
+ * Two deliberate departures from the paper: (a) the neighbourhood radius is h, not 2h, so the ellipsoid pass is the same
+ * 27-cell gather as every other pass; (b) the paper's global scale k_s is replaced by per-particle normalisation, the longest
+ * semi-axis being exactly h: every ellipsoid then lies inside the sphere of radius h around its centre, so the field pass
+ * keeps the 27-cell gather around the centre's cell, where a global k_s could stretch an axis past h and silently lose
+ * contributions.  With lambda = 0, k_r = 1 and k_n = 1 every kernel is the isotropic one and phi is section 15's phi (in
+ * exact arithmetic).  Radii: a_k = h max(s_k / s1, 1 / k_r) in float32, the ratio first.  Defaults
+ * (sph_surface_anisotropy_default): lambda = 0.9, k_r = 1, k_n = 1, N_eps = 6, project values, not the paper's: smoothed
+ * centres with round kernels.  That is the setting found to mesh a jittered slab flatter than sph_world_extract_surface
+ * without inner shells (DESIGN.md section 17).  k_r > 1 stretches the kernels along the surface, but with the longest axis
+ * held at h their volume shrinks, so in jittered fluid the field can dip below iso under the surface layer and the mesh gains
+ * closed inner shells; DESIGN.md section 17 has the measurements.  Every centre lies in the convex hull of the positions,
+ * so the default box still closes every surface.  Ellipsoids are computed for every selected particle: a caller box clips
+ * only the lattice, so a small box over a large fluid pays for the whole fluid's ellipsoids.  In deterministic mode field,
+ * mesh and ellipsoids are bit-identical run to run and do not depend on the fluids' slot order. */
+typedef struct {
+    float    smoothing;        /* lambda in [0, 1] */
+    float    max_ratio;        /* k_r in [1, 1000] (every semi-axis >= h / 1000) */
+    float    isolated_radius;  /* k_n in [0.001, 1], in units of h */
+    uint32_t min_neighbours;   /* N_eps */
+} sph_surface_anisotropy;
+void sph_surface_anisotropy_default(sph_surface_anisotropy* a);
+/* sph_world_extract_surface with the anisotropic field.  SPH_ERR_INVALID, nothing changed and the previous mesh, field and
+ * ellipsoids kept, for everything sph_world_extract_surface refuses and for NaN or out-of-range anisotropy fields.  Besides
+ * its SPH_ERR_OOM cases, SPH_ERR_OOM when the selected fluids' AABB spans more than 2^31 cells of width h (the ellipsoid pass
+ * bins every particle, where the isotropic field bins only those the lattice reaches). */
+sph_status sph_world_extract_surface_anisotropic(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_surface_desc* desc,
+                                                 const sph_surface_anisotropy* aniso, size_t* n_vertices, size_t* n_triangles);
+/* The last extraction's ellipsoids of one fluid, in that fluid's particle order (sph_fluid_read's): the centre x_bar and
+ * 12 floats per particle, (e1, a1, e2, a2, e3, a3), with a1 >= a2 >= a3.  n = 0 after an isotropic extraction or when the
+ * fluid was not selected.  A non-finite position gives its position as the centre and zero axes.  centres_xyz and axes
+ * NULL: only n is written; SPH_ERR_INVALID when cap is below n. */
+sph_status sph_world_read_surface_ellipsoids(sph_world* w, uint32_t fluid, float* centres_xyz, float* axes, size_t cap, size_t* n);
+/* Device pointers to the same rows (NULL when n = 0), valid until the next extraction: the zero-copy input of a splatting
+ * renderer.  Either output pointer may be NULL. */
+sph_status sph_world_map_surface_ellipsoids(sph_world* w, uint32_t fluid, const float** d_centres_xyz, const float** d_axes, size_t* n);
+
 /* Diffuse particles on the device: spray, foam and air bubbles (Ihmsen et al. 2012; DESIGN.md section 16).  A one-way
  * post-process: sph_world_update_diffuse reads the selected fluids at the positions and velocities of the last step (before
  * the first step: those given) and never writes the fluid.  The step, its grid and its cached graphs are not touched.  One

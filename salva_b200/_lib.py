@@ -100,6 +100,10 @@ class SurfaceDesc(C.Structure):
     _fields_ = [("iso", C.c_float), ("spacing", C.c_float), ("lo", C.c_float * 3), ("hi", C.c_float * 3), ("normals", C.c_int32)]
 
 
+class SurfaceAnisotropy(C.Structure):
+    _fields_ = [("smoothing", C.c_float), ("max_ratio", C.c_float), ("isolated_radius", C.c_float), ("min_neighbours", C.c_uint32)]
+
+
 class DiffuseDesc(C.Structure):
     _fields_ = [("ta_min", C.c_float), ("ta_max", C.c_float), ("wc_min", C.c_float), ("wc_max", C.c_float), ("k_min", C.c_float),
                 ("k_max", C.c_float), ("k_ta", C.c_float), ("k_wc", C.c_float), ("lifetime", C.c_float), ("k_b", C.c_float),
@@ -184,6 +188,11 @@ SYMBOLS = {
     "sph_world_read_surface": (C.c_int, [_vp, _fp, _fp, C.c_size_t, C.POINTER(C.c_uint32), C.c_size_t]),
     "sph_world_map_surface": (C.c_int, [_vp, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(C.POINTER(C.c_uint32))]),
     "sph_world_read_surface_field": (C.c_int, [_vp, _fp, C.c_size_t, _fp, C.POINTER(C.c_uint32)]),
+    "sph_surface_anisotropy_default": (None, [C.POINTER(SurfaceAnisotropy)]),
+    "sph_world_extract_surface_anisotropic": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(SurfaceDesc),
+                                                        C.POINTER(SurfaceAnisotropy), C.POINTER(C.c_size_t), C.POINTER(C.c_size_t)]),
+    "sph_world_read_surface_ellipsoids": (C.c_int, [_vp, C.c_uint32, _fp, _fp, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "sph_world_map_surface_ellipsoids": (C.c_int, [_vp, C.c_uint32, C.POINTER(_fp), C.POINTER(_fp), C.POINTER(C.c_size_t)]),
     "sph_diffuse_desc_default": (None, [C.POINTER(DiffuseDesc)]),
     "sph_world_update_diffuse": (C.c_int, [_vp, C.POINTER(C.c_uint32), C.c_size_t, C.POINTER(DiffuseDesc), C.c_float, _fp,
                                            C.POINTER(DiffuseStats)]),

@@ -190,11 +190,18 @@ struct SurfaceSet {
     SurfLattice L{};
     size_t nv = 0, nt = 0;
     bool normals = false;
+    // an anisotropic extraction's ellipsoids (section 17), collected order: centre xyz, and (e1, a1, e2, a2, e3, a3)
+    bool aniso = false;
+    DBuf<float> ecen, eaxes;
+    SurfSel esel{};
+    uint32_t ehandle[MAX_FLUIDS] = {};  // the selected fluids' handles at the extraction (~0: not selected)
+    uint32_t en[MAX_FLUIDS] = {};       // ... and their particle counts
 };
 struct SurfaceState {
     DBuf<uint32_t> vcnt, tcnt, scan_aux[3];
     DBuf<uint8_t> emask;
     DBuf<unsigned long long> totals;
+    DBuf<float4> e4[3], se4[3];  // anisotropic: (x_bar, V h^3 / (a1 a2 a3)) and h G's six entries, collected, then in cell order
     SurfaceSet cur, next;
 };
 // The selected fluids' particles binned into cells of width h for one surface extraction or diffuse update
@@ -3026,7 +3033,30 @@ sph_status sph_world_extract_surface(sph_world* w, const uint32_t* fluids, size_
                                      size_t* n_triangles) {
     if (!w || !desc || !n_vertices || !n_triangles || (n_fluids && !fluids)) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
-    return extract_surface(w, fluids, n_fluids, desc, n_vertices, n_triangles);
+    return extract_surface(w, fluids, n_fluids, desc, nullptr, n_vertices, n_triangles);
+}
+void sph_surface_anisotropy_default(sph_surface_anisotropy* a) {
+    if (!a) return;
+    a->smoothing = 0.9f;
+    a->max_ratio = 1.f;
+    a->isolated_radius = 1.f;
+    a->min_neighbours = 6;
+}
+sph_status sph_world_extract_surface_anisotropic(sph_world* w, const uint32_t* fluids, size_t n_fluids, const sph_surface_desc* desc,
+                                                 const sph_surface_anisotropy* aniso, size_t* n_vertices, size_t* n_triangles) {
+    if (!w || !desc || !aniso || !n_vertices || !n_triangles || (n_fluids && !fluids)) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    return extract_surface(w, fluids, n_fluids, desc, aniso, n_vertices, n_triangles);
+}
+sph_status sph_world_read_surface_ellipsoids(sph_world* w, uint32_t fluid, float* centres_xyz, float* axes, size_t cap, size_t* n) {
+    if (!w || !n) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    return surface_ellipsoids(w, fluid, centres_xyz, axes, cap, nullptr, nullptr, n);
+}
+sph_status sph_world_map_surface_ellipsoids(sph_world* w, uint32_t fluid, const float** d_centres_xyz, const float** d_axes, size_t* n) {
+    if (!w || !n) return SPH_ERR_INVALID;
+    std::lock_guard<std::recursive_mutex> lock(g_mutex);
+    return surface_ellipsoids(w, fluid, nullptr, nullptr, 0, d_centres_xyz, d_axes, n);
 }
 sph_status sph_world_read_surface(sph_world* w, float* vertices_xyz, float* normals_xyz, size_t vcap, uint32_t* triangles, size_t tcap) {
     if (!w) return SPH_ERR_INVALID;

@@ -318,4 +318,215 @@ __global__ void k_surf_normals(uint32_t nv, const float* __restrict__ verts, Sur
     nrm[3 * (size_t)v + 2] = acc.z * s;
 }
 
+// ---- anisotropic kernels (Yu & Turk 2013; include/sph.h sph_world_extract_surface_anisotropic, DESIGN.md section 17) -------
+struct SurfAniso {
+    float lambda, kr, kn;
+    uint32_t n_eps;
+};
+
+// Cyclic Jacobi rotation of the symmetric 3x3 a in the (p, q) plane; the columns of v collect the rotations.
+__device__ __forceinline__ void surf_jacobi_rot(float (&a)[3][3], float (&v)[3][3], int p, int q) {
+    const float apq = a[p][q];
+    if (apq == 0.f) return;
+    const float theta = __fdiv_rn(__fsub_rn(a[q][q], a[p][p]), __fmul_rn(2.f, apq));
+    const float at = fabsf(theta);
+    // t = sign(theta) / (|theta| + sqrt(theta^2 + 1)), the smaller root; 1 / (2 theta) once theta^2 would overflow
+    const float t = copysignf(at > 1e18f ? __fdiv_rn(0.5f, at) : __fdiv_rn(1.f, __fadd_rn(at, __fsqrt_rn(__fmaf_rn(at, at, 1.f)))), theta);
+    const float c = __frsqrt_rn(__fmaf_rn(t, t, 1.f)), s = __fmul_rn(t, c);
+    const int r = 3 - p - q;  // the third index
+    const float arp = a[r][p], arq = a[r][q];
+    a[p][p] = __fmaf_rn(-t, apq, a[p][p]);
+    a[q][q] = __fmaf_rn(t, apq, a[q][q]);
+    a[p][q] = a[q][p] = 0.f;
+    a[r][p] = a[p][r] = __fsub_rn(__fmul_rn(c, arp), __fmul_rn(s, arq));
+    a[r][q] = a[q][r] = __fadd_rn(__fmul_rn(s, arp), __fmul_rn(c, arq));
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float vp = v[k][p], vq = v[k][q];
+        v[k][p] = __fsub_rn(__fmul_rn(c, vp), __fmul_rn(s, vq));
+        v[k][q] = __fadd_rn(__fmul_rn(s, vp), __fmul_rn(c, vq));
+    }
+}
+
+// The ellipsoids of the collected particles.  Thread s < n handles the binned particle s: the weighted sums over the
+// particles of its 27 cells within h (itself included, with weight 1), taken relative to x_s; the centre x_bar; the
+// covariance's eigen-decomposition by cyclic Jacobi (at most 8 sweeps); the radii.  In collected order (row perm[s]) it
+// writes (x_bar, V h^3 / (a1 a2 a3)) to c4, h G as (xx, yy, zz, xy) to g4a and (xz, yz, 0, 0) to g4b, and the public rows:
+// centre xyz and (e1, a1, e2, a2, e3, a3).  Thread k < np also writes the rows of collected particle k when its position is
+// not finite (it was not binned): its position as centre, zero axes and a non-finite c4 that the re-binning leaves out.
+__global__ void k_surf_ellipsoids(uint32_t n, uint32_t np, SurfGrid g, const uint32_t* __restrict__ cstart, const float4* __restrict__ sp,
+                                  const uint32_t* __restrict__ perm, const float4* __restrict__ p4, SurfAniso P, float4* __restrict__ c4,
+                                  float4* __restrict__ g4a, float4* __restrict__ g4b, float* __restrict__ o_centre, float* __restrict__ o_axes) {
+    const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < np) {
+        const float4 p = p4[s];
+        if (!(isfinite(p.x) && isfinite(p.y) && isfinite(p.z))) {
+            c4[s] = make_float4(p.x, p.y, p.z, 0.f);
+            o_centre[3 * (size_t)s] = p.x;
+            o_centre[3 * (size_t)s + 1] = p.y;
+            o_centre[3 * (size_t)s + 2] = p.z;
+#pragma unroll
+            for (int k = 0; k < 12; ++k) o_axes[12 * (size_t)s + k] = 0.f;
+        }
+    }
+    if (s >= n) return;
+    const float4 pi = sp[s];
+    float sw = 0.f, m[3] = {0.f, 0.f, 0.f}, q2[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};  // q2: xx yy zz xy xz yz
+    uint32_t cnt = 0;
+    surf_for_cells(pi.x, pi.y, pi.z, g, cstart, [&](uint32_t j) {
+        const float4 pj = sp[j];
+        const float dx = __fsub_rn(pi.x, pj.x), dy = __fsub_rn(pi.y, pj.y), dz = __fsub_rn(pi.z, pj.z);
+        const float d2 = dist2_exact(dx, dy, dz);  // the step's unfused pair test
+        if (!(d2 <= C.h2)) return;
+        const float q = __fdiv_rn(__fsqrt_rn(d2), C.h);
+        const float wt = __fsub_rn(1.f, __fmul_rn(__fmul_rn(q, q), q));  // 1 - (r / h)^3
+        const float ox = -dx, oy = -dy, oz = -dz;                          // x_j - x_i, exactly
+        ++cnt;
+        sw = __fadd_rn(sw, wt);
+        const float wx = __fmul_rn(wt, ox), wy = __fmul_rn(wt, oy), wz = __fmul_rn(wt, oz);
+        m[0] = __fadd_rn(m[0], wx);
+        m[1] = __fadd_rn(m[1], wy);
+        m[2] = __fadd_rn(m[2], wz);
+        q2[0] = __fmaf_rn(wx, ox, q2[0]);
+        q2[1] = __fmaf_rn(wy, oy, q2[1]);
+        q2[2] = __fmaf_rn(wz, oz, q2[2]);
+        q2[3] = __fmaf_rn(wx, oy, q2[3]);
+        q2[4] = __fmaf_rn(wx, oz, q2[4]);
+        q2[5] = __fmaf_rn(wy, oz, q2[5]);
+    });
+    const uint32_t nn = cnt - 1;  // the particle itself is among the binned ones, at distance 0
+#pragma unroll
+    for (int a = 0; a < 3; ++a) m[a] = __fdiv_rn(m[a], sw);  // x^w - x_i
+    const float c[3] = {__fmaf_rn(P.lambda, m[0], pi.x), __fmaf_rn(P.lambda, m[1], pi.y), __fmaf_rn(P.lambda, m[2], pi.z)};
+    // C = sum w d d^T / sum w - m m^T, d = x_j - x_i
+    float A[3][3], V[3][3] = {{1.f, 0.f, 0.f}, {0.f, 1.f, 0.f}, {0.f, 0.f, 1.f}};
+    A[0][0] = __fmaf_rn(-m[0], m[0], __fdiv_rn(q2[0], sw));
+    A[1][1] = __fmaf_rn(-m[1], m[1], __fdiv_rn(q2[1], sw));
+    A[2][2] = __fmaf_rn(-m[2], m[2], __fdiv_rn(q2[2], sw));
+    A[0][1] = A[1][0] = __fmaf_rn(-m[0], m[1], __fdiv_rn(q2[3], sw));
+    A[0][2] = A[2][0] = __fmaf_rn(-m[0], m[2], __fdiv_rn(q2[4], sw));
+    A[1][2] = A[2][1] = __fmaf_rn(-m[1], m[2], __fdiv_rn(q2[5], sw));
+    for (int sweep = 0; sweep < 8; ++sweep) {
+        const float off = fabsf(A[0][1]) + fabsf(A[0][2]) + fabsf(A[1][2]);
+        const float diag = fabsf(A[0][0]) + fabsf(A[1][1]) + fabsf(A[2][2]);
+        if (!(off > 1e-7f * diag)) break;  // converged (or the matrix is 0)
+        surf_jacobi_rot(A, V, 0, 1);
+        surf_jacobi_rot(A, V, 0, 2);
+        surf_jacobi_rot(A, V, 1, 2);
+    }
+    float sg[3] = {fmaxf(A[0][0], 0.f), fmaxf(A[1][1], 0.f), fmaxf(A[2][2], 0.f)};
+    // descending, columns of V with them (three compare-exchanges)
+    auto cx = [&](int i, int j) {
+        if (sg[j] > sg[i]) {
+            const float t = sg[i];
+            sg[i] = sg[j];
+            sg[j] = t;
+#pragma unroll
+            for (int k = 0; k < 3; ++k) {
+                const float u = V[k][i];
+                V[k][i] = V[k][j];
+                V[k][j] = u;
+            }
+        }
+    };
+    cx(0, 1);
+    cx(1, 2);
+    cx(0, 1);
+    float ax[3];
+    if (nn >= P.n_eps && sg[0] > 0.f) {
+        // h max(s_k / s1, 1 / k_r): the ratio first, so a denormal s1 / k_r cannot flatten an axis to 0
+        const float lo = __fdiv_rn(1.f, P.kr);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) ax[k] = k == 0 ? C.h : __fmul_rn(C.h, fmaxf(__fdiv_rn(sg[k], sg[0]), lo));
+    } else {
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            ax[k] = __fmul_rn(P.kn, C.h);
+#pragma unroll
+            for (int r = 0; r < 3; ++r) V[r][k] = r == k ? 1.f : 0.f;
+        }
+    }
+    // h G = sum_k e_k e_k^T (h / a_k); the kernel's scale V h^3 / (a1 a2 a3)
+    const float ih[3] = {__fdiv_rn(C.h, ax[0]), __fdiv_rn(C.h, ax[1]), __fdiv_rn(C.h, ax[2])};
+    float G[6];
+    const int gi[6] = {0, 1, 2, 0, 0, 1}, gj[6] = {0, 1, 2, 1, 2, 2};
+#pragma unroll
+    for (int e = 0; e < 6; ++e) {
+        float acc = 0.f;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) acc = __fmaf_rn(__fmul_rn(V[gi[e]][k], V[gj[e]][k]), ih[k], acc);
+        G[e] = acc;
+    }
+    const float scale = __fmul_rn(__fmul_rn(__fmul_rn(pi.w, ih[0]), ih[1]), ih[2]);
+    const uint32_t o = perm[s];
+    c4[o] = make_float4(c[0], c[1], c[2], scale);
+    g4a[o] = make_float4(G[0], G[1], G[2], G[3]);
+    g4b[o] = make_float4(G[4], G[5], 0.f, 0.f);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) o_centre[3 * (size_t)o + a] = c[a];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+#pragma unroll
+        for (int r = 0; r < 3; ++r) o_axes[12 * (size_t)o + 4 * k + r] = V[r][k];
+        o_axes[12 * (size_t)o + 4 * k + 3] = ax[k];
+    }
+}
+
+// u = (h G) (x - x_bar) of the binned ellipsoid j at x; |u|^2 unfused
+__device__ __forceinline__ float surf_aniso_u(float x, float y, float z, float4 c, float4 ga, float4 gb, float (&u)[3]) {
+    const float dx = __fsub_rn(x, c.x), dy = __fsub_rn(y, c.y), dz = __fsub_rn(z, c.z);
+    u[0] = __fmaf_rn(gb.x, dz, __fmaf_rn(ga.w, dy, __fmul_rn(ga.x, dx)));
+    u[1] = __fmaf_rn(gb.y, dz, __fmaf_rn(ga.y, dy, __fmul_rn(ga.w, dx)));
+    u[2] = __fmaf_rn(ga.z, dz, __fmaf_rn(gb.y, dy, __fmul_rn(gb.x, dx)));
+    return dist2_exact(u[0], u[1], u[2]);
+}
+
+// Anisotropic field pass: one thread per lattice point, x fastest; phi = sum_j s_j W(|u_j|) over the binned centres of the 27
+// cells around the point, s_j = V_j h^3 / (a1 a2 a3).
+__global__ void k_surf_field_aniso(SurfLattice L, SurfGrid g, const uint32_t* __restrict__ cstart, const float4* __restrict__ sc,
+                                   const float4* __restrict__ sga, const float4* __restrict__ sgb, float* __restrict__ phi) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t np = L.n[0] * L.n[1] * L.n[2];
+    if (p >= np) return;
+    const uint32_t i = p % L.n[0], j = (p / L.n[0]) % L.n[1], k = p / (L.n[0] * L.n[1]);
+    const float x = surf_coord(L, 0, i), y = surf_coord(L, 1, j), z = surf_coord(L, 2, k);
+    float acc = 0.f;
+    surf_for_cells(x, y, z, g, cstart, [&](uint32_t e) {
+        const float4 c = sc[e];
+        float u[3];
+        const float u2 = surf_aniso_u(x, y, z, c, sga[e], sgb[e], u);
+        if (!(u2 <= C.h2)) return;
+        acc = __fmaf_rn(c.w, kernel_w_kind(C.kw, __fsqrt_rn(u2)), acc);
+    });
+    phi[p] = acc;
+}
+
+// Anisotropic normals: n = -grad phi / |grad phi|, grad W_j = s_j (h G_j) W'(|u|) / |u| u (0 for |u|^2 <= eps^2), 0 where the
+// gradient is 0 (k_surf_normals' rule).
+__global__ void k_surf_normals_aniso(uint32_t nv, const float* __restrict__ verts, SurfGrid g, const uint32_t* __restrict__ cstart,
+                                     const float4* __restrict__ sc, const float4* __restrict__ sga, const float4* __restrict__ sgb,
+                                     float* __restrict__ nrm) {
+    const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+    if (v >= nv) return;
+    const float x = verts[3 * (size_t)v], y = verts[3 * (size_t)v + 1], z = verts[3 * (size_t)v + 2];
+    float acc[3] = {0.f, 0.f, 0.f};
+    surf_for_cells(x, y, z, g, cstart, [&](uint32_t e) {
+        const float4 c = sc[e], ga = sga[e], gb = sgb[e];
+        float u[3];
+        const float u2 = surf_aniso_u(x, y, z, c, ga, gb, u);
+        if (!(u2 <= C.h2) || !(u2 > F32_EPS * F32_EPS)) return;
+        const float r = __fsqrt_rn(u2);
+        const float gf = __fmul_rn(c.w, __fdiv_rn(kernel_dw_kind(C.kg, r), r));
+        const float t[3] = {__fmul_rn(gf, u[0]), __fmul_rn(gf, u[1]), __fmul_rn(gf, u[2])};
+        acc[0] = __fadd_rn(acc[0], __fmaf_rn(gb.x, t[2], __fmaf_rn(ga.w, t[1], __fmul_rn(ga.x, t[0]))));
+        acc[1] = __fadd_rn(acc[1], __fmaf_rn(gb.y, t[2], __fmaf_rn(ga.y, t[1], __fmul_rn(ga.w, t[0]))));
+        acc[2] = __fadd_rn(acc[2], __fmaf_rn(ga.z, t[2], __fmaf_rn(gb.y, t[1], __fmul_rn(gb.x, t[0]))));
+    });
+    const float n2 = dist2_exact(acc[0], acc[1], acc[2]);
+    const float s = n2 > 0.f ? -__frsqrt_rn(n2) : 0.f;
+    nrm[3 * (size_t)v] = acc[0] * s;
+    nrm[3 * (size_t)v + 1] = acc[1] * s;
+    nrm[3 * (size_t)v + 2] = acc[2] * s;
+}
+
 }  // namespace sphk

@@ -34,6 +34,20 @@ class SphError(RuntimeError):
         self.status = status
 
 
+class SurfaceAnisotropy:
+    """include/sph.h sph_surface_anisotropy (Yu & Turk 2013 kernels, DESIGN.md section 17): centre smoothing lambda in [0, 1],
+    largest semi-axis ratio k_r in [1, 1000], radius of a particle with too few neighbours k_n in [0.001, 1] (units of h),
+    and the fewest neighbours N_eps for an anisotropic kernel.  The defaults are sph_surface_anisotropy_default's: smoothed
+    centres with round kernels (k_r = k_n = 1); k_r > 1 stretches the kernels, see DESIGN.md section 17 for its cost."""
+
+    def __init__(self, smoothing=0.9, max_ratio=1.0, isolated_radius=1.0, min_neighbours=6):
+        self.smoothing, self.max_ratio = smoothing, max_ratio
+        self.isolated_radius, self.min_neighbours = isolated_radius, min_neighbours
+
+    def _c(self):
+        return _lib.SurfaceAnisotropy(float(self.smoothing), float(self.max_ratio), float(self.isolated_radius), int(self.min_neighbours))
+
+
 class InteractionGroups:
     """interaction_groups.rs:20-79; default = (GROUP_1, ALL)."""
 
@@ -562,11 +576,13 @@ class LiquidWorld:
         return r.value, e.value
 
     # -- fluid surface meshes (include/sph.h, DESIGN.md section 15) -------------------------------------------------
-    def extract_surface(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True):
+    def extract_surface(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True, anisotropy=None):
         """Samples phi = sum_j V_j W(|x - x_j|) of `fluids` (None: all) on a lattice of `spacing` (None: the particle radius)
         and polygonises phi = iso on the device.  box=None meshes the fluids' AABB grown by h, where every surface closes; a
-        box (lo, hi) clips the lattice, and surfaces are open where it cuts them.  Returns (n_vertices, n_triangles); the mesh
-        stays on the device until the next extraction."""
+        box (lo, hi) clips the lattice, and surfaces are open where it cuts them.  anisotropy=None keeps the spherical
+        kernels; a SurfaceAnisotropy gives every particle a smoothed centre and an ellipsoidal kernel (include/sph.h
+        sph_world_extract_surface_anisotropic), whose rows surface_ellipsoids reads.  Returns (n_vertices, n_triangles); the
+        mesh stays on the device until the next extraction."""
         d = _lib.SurfaceDesc()
         d.iso = float(iso)
         d.spacing = float(self.particle_radius if spacing is None else spacing)
@@ -578,8 +594,12 @@ class LiquidWorld:
         d.normals = int(bool(normals))
         hs = np.ascontiguousarray(np.asarray([] if fluids is None else list(fluids), np.uint32))
         nv, nt = C.c_size_t(), C.c_size_t()
-        self._ck(self._L.sph_world_extract_surface(self._w, hs.ctypes.data_as(C.POINTER(C.c_uint32)), len(hs), C.byref(d), C.byref(nv),
-                                                   C.byref(nt)))
+        hp = hs.ctypes.data_as(C.POINTER(C.c_uint32))
+        if anisotropy is None:
+            self._ck(self._L.sph_world_extract_surface(self._w, hp, len(hs), C.byref(d), C.byref(nv), C.byref(nt)))
+        else:
+            a = anisotropy._c()
+            self._ck(self._L.sph_world_extract_surface_anisotropic(self._w, hp, len(hs), C.byref(d), C.byref(a), C.byref(nv), C.byref(nt)))
         self._surface_normals = bool(normals)
         self._surface_spacing = np.float32(d.spacing)
         self._surface_counts = (nv.value, nt.value)
@@ -597,11 +617,34 @@ class LiquidWorld:
                                                 t.ctypes.data_as(C.POINTER(C.c_uint32)), nt))
         return v, t, n
 
-    def surface_mesh(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True):
+    def surface_mesh(self, iso=0.6, spacing=None, fluids=None, box=None, normals=True, anisotropy=None):
         """extract_surface then read_surface: (vertices[nv, 3] f32, triangles[nt, 3] u32, normals[nv, 3] f32 or None).
         Triangles wind counter-clockwise seen from outside; see include/sph.h for the lattice and the ordering."""
-        self.extract_surface(iso, spacing, fluids, box, normals)
+        self.extract_surface(iso, spacing, fluids, box, normals, anisotropy)
         return self.read_surface(normals)
+
+    def surface_ellipsoids(self, fluid):
+        """(centres[n, 3] f32, axes[n, 3, 4] f32) of the last extraction for `fluid`, in its particle order: axes[i, k] =
+        (e_k, a_k), a_1 >= a_2 >= a_3.  n = 0 after an isotropic extraction or when the fluid was not selected."""
+        n = C.c_size_t()
+        self._ck(self._L.sph_world_read_surface_ellipsoids(self._w, fluid, None, None, 0, C.byref(n)))
+        c, a = np.empty((n.value, 3), np.float32), np.empty((n.value, 3, 4), np.float32)
+        self._ck(self._L.sph_world_read_surface_ellipsoids(self._w, fluid, _fp(c), _fp(a), n.value, C.byref(n)))
+        return c, a
+
+    def map_surface_ellipsoids(self, fluid):
+        """Device views (no host copy) of surface_ellipsoids(fluid)'s (centres[n, 3], axes[n, 3, 4]) as objects with
+        __cuda_array_interface__; valid until the next extraction."""
+        cp, ap, n = C.POINTER(C.c_float)(), C.POINTER(C.c_float)(), C.c_size_t()
+        self._ck(self._L.sph_world_map_surface_ellipsoids(self._w, fluid, C.byref(cp), C.byref(ap), C.byref(n)))
+
+        def view(ptr, shape):
+            addr = C.cast(ptr, C.c_void_p).value or 0
+
+            class _View:
+                __cuda_array_interface__ = {"shape": shape, "typestr": "<f4", "data": (addr, False), "version": 2, "strides": None}
+            return _View()
+        return view(cp, (n.value, 3)), view(ap, (n.value, 3, 4))
 
     def surface_field(self):
         """(phi[nz, ny, nx], origin[3], spacing) of the last extraction's lattice."""

@@ -7,7 +7,11 @@ per configuration under torch.profiler gives the field pass's kernel time; its c
 point, each binned particle read once) over that time is reported as a rate.  The card's name, power limit and SM clocks
 are read in the same run.  Prints one JSON line per configuration.
 
-    python tools/bench_surface.py --out DIR [--profile]
+With --anisotropic (sph_world_extract_surface_anisotropic, DESIGN.md section 17) it times instead the isotropic and the
+anisotropic extraction of the same world, alternating, at C2 spacing r and r / 2 and at C3 spacing r, with normals; with
+--profile also the anisotropic extraction's kernel times per pass (ellipsoids, the two binnings, field, normals).
+
+    python tools/bench_surface.py --out DIR [--profile] [--anisotropic]
 """
 import argparse
 import json
@@ -20,7 +24,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-from salva_b200 import LiquidWorld, scenes  # noqa: E402
+from salva_b200 import LiquidWorld, SurfaceAnisotropy, scenes  # noqa: E402
 
 
 def card():
@@ -74,6 +78,48 @@ def run(name, sc, settle, rounds, profile, out):
         json.dump(lines, f, indent=1)
 
 
+PASSES = {"ellipsoids": ("k_surf_ellipsoids",), "binning_and_scans": ("k_surf_hist", "k_cell_scatter", "k_surf_cell_sort", "k_gather", "k_scan"),
+          "field": ("k_surf_field_aniso",), "normals": ("k_surf_normals_aniso",), "polygonise": ("k_surf_count", "k_surf_emit")}
+
+
+def run_aniso(name, sc, spacings, settle, rounds, profile, out):
+    """Isotropic and anisotropic extraction of one settled world, alternating round by round."""
+    w = LiquidWorld(particle_radius=sc["particle_radius"], smoothing_factor=sc["smoothing_factor"])
+    fh, _ = scenes.populate(w, sc)
+    for _ in range(settle):
+        w.step(sc["dt"])
+    r = float(sc["particle_radius"])
+    an = SurfaceAnisotropy()
+    lines = []
+    for sp_name in spacings:
+        sp = r if sp_name == "r" else 0.5 * r
+        iso = lambda: w.extract_surface(iso=0.6, spacing=sp)  # noqa: E731
+        ani = lambda: w.extract_surface(iso=0.6, spacing=sp, anisotropy=an)  # noqa: E731
+        iso()
+        ani()  # warm-up: allocations and module loads
+        t_iso, t_ani = [], []
+        for _ in range(rounds):
+            t_iso.append(timed(iso, 1)[0])
+            t_ani.append(timed(ani, 1)[0])
+        nv, nt = ani()
+        rec = dict(scene=name, particles=w.num_particles(fh[0]), spacing=sp_name, vertices_aniso=nv, triangles_aniso=nt,
+                   iso_ms=round(float(np.median(t_iso)), 3), aniso_ms=round(float(np.median(t_ani)), 3),
+                   iso_ms_rounds=[round(x, 3) for x in t_iso], aniso_ms_rounds=[round(x, 3) for x in t_ani], card=card())
+        if profile:
+            from torch.profiler import ProfilerActivity, profile as tprof
+            with tprof(activities=[ProfilerActivity.CUDA]) as prof:
+                ani()
+                torch.cuda.synchronize()
+            ev = prof.key_averages()
+            rec["aniso_pass_ms"] = {k: round(sum(e.device_time_total for e in ev if any(n in e.key for n in names)) / 1000.0, 3)
+                                    for k, names in PASSES.items()}
+        print(json.dumps(rec), flush=True)
+        lines.append(rec)
+    w.close()
+    with open(os.path.join(out, "bench_surface_aniso_%s.json" % name), "w") as f:
+        json.dump(lines, f, indent=1)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--out", default=None, help="directory for bench_surface_*.json (default: a temporary one)")
@@ -82,6 +128,7 @@ def main():
     ap.add_argument("--settle", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--profile", action="store_true")
+    ap.add_argument("--anisotropic", action="store_true", help="isotropic against anisotropic extraction, alternating")
     a = ap.parse_args()
     if a.out is None:
         import tempfile
@@ -89,6 +136,10 @@ def main():
     os.makedirs(a.out, exist_ok=True)
     if not torch.cuda.is_available():
         raise SystemExit("bench_surface needs a CUDA device")
+    if a.anisotropic:
+        run_aniso("C2", scenes.scene_c2(a.c2_n), ("r", "r/2"), a.settle, a.rounds, a.profile, a.out)
+        run_aniso("C3", scenes.scene_c3(a.c3_n), ("r",), a.settle, a.rounds, a.profile, a.out)
+        return
     run("C2", scenes.scene_c2(a.c2_n), a.settle, a.rounds, a.profile, a.out)
     run("C3", scenes.scene_c3(a.c3_n), a.settle, a.rounds, a.profile, a.out)
 
