@@ -170,7 +170,9 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        SPH_DBG_DIFFUSE_TRAPPED_AIR = 21, /* I_ta before clamping */
        SPH_DBG_DIFFUSE_WAVE_CREST = 22,  /* I_wc before clamping (0 where v^ . n < 0.6) */
        SPH_DBG_DIFFUSE_KINETIC = 23,     /* E_k before clamping */
-       SPH_DBG_DIFFUSE_COUNT = 24        /* n_d, the particles it asked to emit, as float */ };
+       SPH_DBG_DIFFUSE_COUNT = 24,       /* n_d, the particles it asked to emit, as float */
+       SPH_DBG_FLUID_LIST_BITS = 25      /* the width in bits (16 or 32) of the fluid list entries the last neighbour search
+                                          * stored, the same for every particle (DESIGN.md section 4a.18) */ };
 
 /* LiquidWorld::new  liquid_world.rs:39-57 */
 void       sph_world_desc_default(sph_world_desc* desc);

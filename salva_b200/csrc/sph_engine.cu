@@ -130,11 +130,13 @@ struct Tex {
 
 // The neighbour lists (layout: sph_lists.cuh) and their capacities in rows.  The constants carry the capacities: grow_lists()
 // raises them.
+// wide: the width the lists are stored in, set by each search (phase_neighbors).
 struct ListState {
     DBuf<uint32_t> nbr_f, nbr_b, cnt_f, cnt_b;
     uint32_t cap_f = 64, cap_b = 32;
+    bool wide = true;
     Lists view() const { return out().view(); }
-    ListsOut out() const { return {nbr_f.p, nbr_b.p, cnt_f.p, cnt_b.p}; }
+    ListsOut out() const { return {nbr_f.p, nbr_b.p, cnt_f.p, cnt_b.p, wide}; }
     // counts for n particles, and cap_f / cap_b rows of `stride` entries (sph_world::stride)
     cudaError_t ensure(size_t n, uint32_t stride) {
         cudaError_t e = cnt_f.ensure(n);
@@ -1302,6 +1304,10 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
                 break;
             }
     }
+    // Each search of a one-GPU, one-fluid h-cell world starts with narrow (16-bit) lists and is repeated wide if a stencil window does not
+    // fit them (sph_lists.cuh).  A step graph captures the width the last search of the host path settled on.
+    // Row order, slab worlds (whose windows would add ghost ranges) and several fluids keep wide lists.
+    if (!w->cap) w->lists.wide = !NARROW_LISTS || w->hc.xysub > 1 || w->slab.active || w->fluids.size() > 1;
     for (int attempt = 0; attempt < 8 && N; ++attempt) {
         CU(cudaMemsetAsync(w->d_ss.p->max_nb, 0, sizeof(StepScalars::max_nb), w->st));
         LAUNCH(search, N, NBR_T, w->pos[c].p, w->vel[c].p, w->cstart.p, w->bpos[bc].p, w->bvel[bc].p, w->bstart.p, w->lists.out(), w->d_ss.p->max_nb, D);
@@ -1320,8 +1326,10 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
             return w->fail(SPH_ERR_ZERO_DENSITY, "zero boundary-volume denominator (reference assert dfsph_solver.rs:92)");
         w->stats.max_neighbors = S.max_nb[0];
         w->max_nb_b = S.max_nb[1];
-        if (S.max_nb[0] <= w->lists.cap_f && S.max_nb[1] <= w->lists.cap_b) break;
-        if (speculative) CU(cudaMemsetAsync(&w->d_ss.p->err, 0, sizeof(int), w->st));  // error word of the discarded density pass or sweep
+        if (S.max_nb[0] <= w->lists.cap_f && S.max_nb[1] <= w->lists.cap_b && !S.max_nb[2]) break;
+        // error word of the discarded density pass or sweep (a sweep over narrow lists that did not fit reads wrong contacts)
+        if (speculative || S.max_nb[2]) CU(cudaMemsetAsync(&w->d_ss.p->err, 0, sizeof(int), w->st));
+        if (S.max_nb[2]) w->lists.wide = true;
         TRY(grow_lists(w, (S.max_nb[0] + 15) / 16 * 16, (S.max_nb[1] + 15) / 16 * 16));
     }
     if (!N) {  // boundaries only
@@ -2595,6 +2603,10 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         const float* src = what == SPH_DBG_EL_ROTATION ? E.rot.p : what == SPH_DBG_EL_GRAD_TR ? E.grad_tr.p : E.stress.p;
         CU(cudaMemcpyAsync(out, src, width * f.n * sizeof(float), cudaMemcpyDeviceToHost, w->st));
         CU(cudaStreamSynchronize(w->st));
+        return SPH_OK;
+    }
+    if (what == SPH_DBG_FLUID_LIST_BITS) {
+        std::fill(out, out + f.n, w->lists.wide ? 32.f : 16.f);
         return SPH_OK;
     }
     const int c = w->cur;

@@ -175,7 +175,8 @@ enum : int { ERR_ZERO_DENSITY = 1, ERR_PEER_TIMEOUT = 2, ERR_SEARCH_ZERO_DENSITY
 struct StepScalars {
     CellBox grid;                    // the fluid's cell box that sizes the grid (k_bounds)
     int err;                         // error word: ERR_* bits
-    uint32_t max_nb[2];              // the widest fluid [0] and boundary [1] contact list of the search
+    uint32_t max_nb[3];              // the widest fluid [0] and boundary [1] contact list of the search; [2] != 0: a narrow
+                                     // search met a stencil window of more than WINDOW_SLOTS slots (sph_lists.cuh)
     unsigned long long contacts_bb;  // boundary-boundary contacts (k_boundary_volumes)
     unsigned long long contacts_f;   // fluid-fluid + fluid-boundary contacts (k_sum_u32)
     uint32_t elast_width;            // the widest Becker2009 rest list (k_el_capture_lists)
@@ -814,8 +815,10 @@ __device__ __forceinline__ void density_alpha_div(uint32_t i, bool valid, uint32
 // together, so the per-hit stores already coalesce and staging only added cost (C2 rows: 0.300 vs 0.289 ms per search).
 constexpr uint32_t NBR_SF = 32, NBR_SB = 8;  // staged fluid / boundary rows per lane (multiples of 4)
 
-// The search shared by k_neighbors and k_neighbors_xy; `runs(pi, visit)` calls visit(lo) for every z-run of cells the particle
-// has to scan, lo being the cell id (cstart / bstart index) of the run's first cell; a run is always 3 cells.  STAGE (the
+// The search shared by k_neighbors and k_neighbors_xy; `runs(pi, visit)` calls visit(lo, plane_start) for every z-run of cells the
+// particle has to scan, lo being the cell id (cstart / bstart index) of the run's first cell; a run is always 3 cells.  The
+// h-cell search visits the runs in sorted order and sets plane_start on the first run of each x-plane: it writes narrow lists
+// unless out.wide (sph_lists.cuh), and raises maxcnt[2] if a window does not fit them.  Row order writes wide lists only.  STAGE (the
 // h-cell search) also batches the candidate loads: both pay on h-cell runs only.  DENS: each particle then sweeps its own
 // list with density_alpha_div, reading the staged entries from shared memory and the later ones back from global memory.
 template <bool MULTI, bool STAGE, bool DENS, bool UNI, class Runs>
@@ -833,12 +836,21 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
     const uint32_t lane = threadIdx.x & 31u;
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     uint32_t nf = 0, nb = 0;
+    // narrow lists (sph_lists.cuh; the h-cell search only): the first run of the x-plane being walked, and its window
+    int lo_plane = 0;
+    uint32_t plane = ~0u;
+    Window win{};
+    bool over = false;  // a window of this particle spans more than WINDOW_SLOTS slots
     const bool owned = i < C.n_owned;
     i += C.i_begin;
     if (owned) {
         const float4 pi = pos[i];
         const uint32_t fi = MULTI ? fid_of(vel[i]) : 0u;
-        runs(pi, [&](int lo) {
+        runs(pi, [&](int lo, bool plane_start) {
+            if (STAGE && plane_start) {
+                lo_plane = lo;
+                ++plane;
+            }
             scan_run<STAGE>(
                 pi, pos, cstart[lo], cstart[lo + 3],
                 [&](uint32_t j) {
@@ -848,7 +860,7 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
                 },
                 [&](uint32_t j) {
                     if (STAGE && nf < NBR_SF) sf[nf][lane] = j;
-                    else out.fluid(i, nf, j);
+                    else out.fluid(i, nf, j, plane, out.wide ? 0u : cstart[lo_plane]);
                     ++nf;
                 });
             if (C.n_bound)
@@ -864,17 +876,27 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
                         ++nb;
                     });
         });
-        // write-out: the last group is padded with i; the capacities and NBR_SF are multiples of 4, so a staged group is whole
+        if (STAGE && NARROW_LISTS && !out.wide) {  // the windows: lo_plane is the first run of plane +1, planes are ny * nz cells apart
+            const int P = C.ny * C.nz;
+#pragma unroll
+            for (int d = 0; d < 3; ++d) {
+                const int lo = lo_plane - (2 - d) * P;
+                win.base[d] = cstart[lo];
+                over |= cstart[lo + 2 * C.nz + 3] - win.base[d] > WINDOW_SLOTS;
+            }
+            // lists that do not fit are redone wide; until then every entry decodes to a slot below WINDOW_SLOTS < n_fluid
+            if (over) win = Window{};
+            out.bases(i, win);
+        }
+        // write-out: the last group is padded; the capacities and NBR_SF are multiples of 4, so a staged group is whole
         if (STAGE) {
             const uint32_t sfn = min(fluid_stored(nf), NBR_SF);
-            for (uint32_t k = 0; k < sfn; k += 4) {
-                const uint32_t a = sf[k][lane], b = sf[k + 1][lane], c = sf[k + 2][lane], d = sf[k + 3][lane];
-                out.group(i, k >> 2, make_uint4(a, k + 1 < nf ? b : i, k + 2 < nf ? c : i, k + 3 < nf ? d : i));
-            }
+            for (uint32_t k = 0; k < sfn; k += 4)
+                out.group(i, k >> 2, make_uint4(sf[k][lane], sf[k + 1][lane], sf[k + 2][lane], sf[k + 3][lane]), nf, win);
             const uint32_t sbn = min(boundary_stored(nb), NBR_SB);
             for (uint32_t k = 0; k < sbn; ++k) out.boundary(i, k, sb[k][lane]);
         }
-        out.pad(i, STAGE ? max(nf, NBR_SF) : nf, nf);  // pad the last group unless staged
+        out.pad(i, STAGE ? max(nf, NBR_SF) : nf, nf, win);  // pad the last group unless staged
         out.counts(i, nf, nb);
     }
     uint32_t mf = nf, mb = nb;
@@ -882,9 +904,11 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
         mf = max(mf, __shfl_xor_sync(0xffffffffu, mf, o));
         mb = max(mb, __shfl_xor_sync(0xffffffffu, mb, o));
     }
+    const bool any_over = __any_sync(0xffffffffu, over);
     if (lane == 0) {
         if (mf) atomicMax(&maxcnt[0], mf);
         if (mb) atomicMax(&maxcnt[1], mb);
+        if (any_over) atomicOr(&maxcnt[2], 1u);
     }
     if constexpr (DENS) {
         const Lists L = out.view();
@@ -893,7 +917,7 @@ __device__ __forceinline__ void neighbor_lists(const float4* __restrict__ pos, c
             [&](uint32_t q) {
                 const uint32_t k = q * 4u;
                 if (STAGE && k < NBR_SF) return make_uint4(sf[k][lane], sf[k + 1][lane], sf[k + 2][lane], sf[k + 3][lane]);
-                return L.group(i, q);  // this thread's own stores above
+                return out.group_ids(i, q);  // this thread's own stores above
             },
             [&](uint32_t k) { return STAGE && k < NBR_SB ? sb[k][lane] : L.boundary(i, k); });
     }
@@ -905,11 +929,11 @@ template <bool MULTI, bool DENS = false, bool UNI = false>
 __global__ void __launch_bounds__(NBR_T, !DENS || SPH_GENERIC_KERNELS ? 1 : MULTI ? 8 : 9)
 k_neighbors(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
             const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-            ListsOut out, uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+            ListsOut out, uint32_t* __restrict__ maxcnt /* StepScalars::max_nb */, DensArgs D) {
     neighbor_lists<MULTI, true, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, out, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         for (int ax = -1; ax <= 1; ++ax)
-            for (int ay = -1; ay <= 1; ++ay) visit(cell_id(cx + ax, cy + ay, cz - 1));  // the z-run of cells cz-1..cz+1
+            for (int ay = -1; ay <= 1; ++ay) visit(cell_id(cx + ax, cy + ay, cz - 1), ay == -1);  // the z-run of cells cz-1..cz+1
     });
 }
 
@@ -921,14 +945,14 @@ template <bool MULTI, bool DENS = false, bool UNI = false>
 __global__ void
 k_neighbors_xy(const float4* __restrict__ pos, const float4* __restrict__ vel, const uint32_t* __restrict__ cstart,
                const float4* __restrict__ bpos, const float4* __restrict__ bvel, const uint32_t* __restrict__ bstart,
-               ListsOut out, uint32_t* __restrict__ maxcnt /* [0]=fluid,[1]=boundary */, DensArgs D) {
+               ListsOut out, uint32_t* __restrict__ maxcnt /* StepScalars::max_nb */, DensArgs D) {
     neighbor_lists<MULTI, false, DENS, UNI>(pos, vel, cstart, bpos, bvel, bstart, out, maxcnt, D, [](const float4& pi, auto&& visit) {
         const int cx = cell_coord(pi.x), cy = cell_coord(pi.y), cz = cell_coord(pi.z);
         int xlo, xhi, ylo, yhi;
         arun(pi.x, cx, C.xysub, C.xysub_f, xlo, xhi);
         arun(pi.y, cy, C.xysub, C.xysub_f, ylo, yhi);
         for (int bx = xlo; bx <= xhi; ++bx)
-            for (int by = ylo; by <= yhi; ++by) visit(cell_id(bx, by, cz - 1));
+            for (int by = ylo; by <= yhi; ++by) visit(cell_id(bx, by, cz - 1), false);
     });
 }
 // boundary volumes in row order: every bin of the 3 x 3 x 3 reference cells around the particle
@@ -1551,11 +1575,12 @@ __global__ void k_fold_arm(const GraphCtl* ctl, const StepRec* rec, int xsf, int
         if (d.h[k]) cudaGraphSetConditional(d.h[k], k == s ? 1u : 0u);
 }
 
-// After the neighbour search of a graph step: the list capacity check and error word of phase_neighbors' read-back.  A list
-// longer than its capacity (or a boundary-volume error) stops the graph before the solver; the host redoes the step.
+// After the neighbour search of a graph step: the list capacity and width checks and error word of phase_neighbors' read-back.
+// A list longer than its capacity, narrow lists a window does not fit (or a boundary-volume error) stop the graph before the
+// solver; the host redoes the step.
 __global__ void k_lists_check(GraphCtl* ctl, StepRec* rec, const StepScalars* ss, uint32_t cap_f, uint32_t cap_b, cudaGraphConditionalHandle h) {
     const uint32_t mf = ss->max_nb[0], mb = ss->max_nb[1];
-    const bool ok = !(ss->err & ~ERR_SEARCH_ZERO_DENSITY) && mf <= cap_f && mb <= cap_b;
+    const bool ok = !(ss->err & ~ERR_SEARCH_ZERO_DENSITY) && mf <= cap_f && mb <= cap_b && !ss->max_nb[2];
     rec[ctl->step].max_neighbors = mf;
     if (!ok) ctl->stop = GRAPH_STOP_REDO;
     cudaGraphSetConditional(h, ok ? 1u : 0u);

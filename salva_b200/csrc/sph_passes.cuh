@@ -3,8 +3,8 @@
 // through the TEXTURE pipe, whose data path is separate from the LSU one: the L1TEX data pipe — two float4
 // gathers per contact — is what bounds these kernels, not DRAM).
 //
-// Contacts are consumed in groups of four: one coalesced LDG.128 brings 4 list indices per thread (the next group is
-// prefetched before the current one is used), then 4 position gathers + 4 auxiliary gathers are issued back to back
+// Contacts are consumed in groups of four: one coalesced load brings 4 list entries per thread (the next group is
+// prefetched before the current one is used; sph_lists.cuh decodes them), then 4 position gathers + 4 auxiliary gathers are issued back to back
 // and only then the 4 pair evaluations run, so 8+ independent loads are in flight per thread.
 #pragma once
 #include <type_traits>
@@ -28,35 +28,38 @@ __device__ __forceinline__ auto call_gather(F& f, uint32_t j, int u) {
 // whatever else the pass needs from neighbour j; ff(j, pair, posrec_j, aux) consumes one contact.
 template <bool W, bool G, class LP, class LD, class FF>
 __device__ __forceinline__ void for_fluid_contacts_g(uint32_t i, const float4& pi, const Lists& L, LP ldpos, LD ld, FF ff) {
-    const uint32_t n = L.fluid_count(i);
-    const uint32_t nq = (n + 3u) >> 2;
-    uint4 J = nq ? L.group(i, 0) : make_uint4(i, i, i, i);
-    for (uint32_t q = 0; q < nq; ++q) {
-        uint4 Jn = J;
-        if (q + 1 < nq) Jn = L.group(i, q + 1);  // fetch the next group of indices early
-        uint32_t j[4] = {J.x, J.y, J.z, J.w};
-        const uint32_t k0 = q * 4u;
-        bool ok[4];
+    L.fluid_row(i, [&](const auto& R) {
+        const uint32_t n = R.n;
+        const uint32_t nq = (n + 3u) >> 2;
+        auto J = nq ? R.raw(0) : decltype(R.raw(0)){};
+        for (uint32_t q = 0; q < nq; ++q) {
+            auto Jn = J;
+            if (q + 1 < nq) Jn = R.raw(q + 1);  // fetch the next group of indices early
+            const uint4 D = R.ids(J);
+            uint32_t j[4] = {D.x, D.y, D.z, D.w};
+            const uint32_t k0 = q * 4u;
+            bool ok[4];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            ok[u] = k0 + u < n;
-            if (!ok[u]) j[u] = i;  // unwritten tail slots of the last group: point at self, masked below
-        }
-        float4 pj[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) pj[u] = call_gather(ldpos, j[u], u);
-        decltype(call_gather(ld, 0u, 0)) aux[4];
-#pragma unroll
-        for (int u = 0; u < 4; ++u) aux[u] = call_gather(ld, j[u], u);
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-            if (ok[u]) {
-                Pair p = make_pair<W, G>(pi, pj[u]);
-                ff(j[u], p, pj[u], aux[u]);
+            for (int u = 0; u < 4; ++u) {
+                ok[u] = k0 + u < n;
+                if (!ok[u]) j[u] = i;  // tail slots of the last group: point at self, masked below
             }
+            float4 pj[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) pj[u] = call_gather(ldpos, j[u], u);
+            decltype(call_gather(ld, 0u, 0)) aux[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) aux[u] = call_gather(ld, j[u], u);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+                if (ok[u]) {
+                    Pair p = make_pair<W, G>(pi, pj[u]);
+                    ff(j[u], p, pj[u], aux[u]);
+                }
+            }
+            J = Jn;
         }
-        J = Jn;
-    }
+    });
 }
 // Gradient-only passes.  Contacts are consumed in groups of four: the group's 4 position gathers and 4 auxiliary
 // gathers are issued back to back before any arithmetic, and the next group's list indices are prefetched.
@@ -68,30 +71,32 @@ __device__ __forceinline__ void for_fluid_contacts_g(uint32_t i, const float4& p
 template <bool NEED_W = false, int BATCH = 4, class LP, class LD, class FF>
 __device__ __forceinline__ void for_fluid_grads(uint32_t i, const float4& pi, const Lists& L, LP ldpos, LD ld, FF ff) {
     static_assert(BATCH == 2 || BATCH == 4, "a group of four contacts is split into whole batches");
-    const uint32_t n = L.fluid_count(i);
-    const uint32_t nq = (n + 3u) >> 2;
-    if (nq == 0) return;
-    uint4 J = L.group(i, 0);
-    for (uint32_t q = 0; q < nq; ++q) {
-        uint4 Jn = J;
-        if (q + 1 < nq) Jn = L.group(i, q + 1);  // fetch the next group early
-        const uint32_t j[4] = {J.x, J.y, J.z, J.w};
+    L.fluid_row(i, [&](const auto& R) {
+        const uint32_t nq = (R.n + 3u) >> 2;
+        if (nq == 0) return;
+        auto J = R.raw(0);
+        for (uint32_t q = 0; q < nq; ++q) {
+            auto Jn = J;
+            if (q + 1 < nq) Jn = R.raw(q + 1);  // fetch the next group early
+            const uint4 D = R.ids(J);
+            const uint32_t j[4] = {D.x, D.y, D.z, D.w};
 #pragma unroll
-        for (int u0 = 0; u0 < 4; u0 += BATCH) {
-            float4 pj[BATCH];
+            for (int u0 = 0; u0 < 4; u0 += BATCH) {
+                float4 pj[BATCH];
 #pragma unroll
-            for (int u = 0; u < BATCH; ++u) pj[u] = call_gather(ldpos, j[u0 + u], u0 + u);
-            decltype(call_gather(ld, 0u, 0)) aux[BATCH];
+                for (int u = 0; u < BATCH; ++u) pj[u] = call_gather(ldpos, j[u0 + u], u0 + u);
+                decltype(call_gather(ld, 0u, 0)) aux[BATCH];
 #pragma unroll
-            for (int u = 0; u < BATCH; ++u) aux[u] = call_gather(ld, j[u0 + u], u0 + u);
+                for (int u = 0; u < BATCH; ++u) aux[u] = call_gather(ld, j[u0 + u], u0 + u);
 #pragma unroll
-            for (int u = 0; u < BATCH; ++u) {
-                Pair p = make_pair<NEED_W, true>(pi, pj[u]);
-                ff(j[u0 + u], p, pj[u], aux[u]);
+                for (int u = 0; u < BATCH; ++u) {
+                    Pair p = make_pair<NEED_W, true>(pi, pj[u]);
+                    ff(j[u0 + u], p, pj[u], aux[u]);
+                }
             }
+            J = Jn;
         }
-        J = Jn;
-    }
+    });
 }
 template <class LD, class FF>
 __device__ __forceinline__ void for_fluid_grads_pos(uint32_t i, const float4& pi, const Lists& L, const float4* __restrict__ pos, LD ld, FF ff) {
@@ -149,30 +154,33 @@ k_density_alpha(const float4* __restrict__ pos, const float4* __restrict__ vel, 
     {
         // Not for_fluid_contacts: masking the tail slots before the gathers made this pass 1 % slower at C5's 2M particles
         // (H100 80GB HBM3, 700 W); the slots already hold i itself.
-        const uint32_t n = L.fluid_count(i);
-        const uint32_t nq = (n + 3u) >> 2;
-        uint4 J = nq ? L.group(i, 0) : make_uint4(i, i, i, i);
-        for (uint32_t q = 0; q < nq; ++q) {
-            uint4 Jn = J;
-            if (q + 1 < nq) Jn = L.group(i, q + 1);
-            const uint32_t j[4] = {J.x, J.y, J.z, J.w};
-            float4 pj[4];
+        L.fluid_row(i, [&](const auto& R) {
+            const uint32_t n = R.n;
+            const uint32_t nq = (n + 3u) >> 2;
+            auto J = nq ? R.raw(0) : decltype(R.raw(0)){};
+            for (uint32_t q = 0; q < nq; ++q) {
+                auto Jn = J;
+                if (q + 1 < nq) Jn = R.raw(q + 1);
+                const uint4 D = R.ids(J);
+                const uint32_t j[4] = {D.x, D.y, D.z, D.w};
+                float4 pj[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) pj[u] = __ldg(&pos[j[u]]);  // tail slots point at i itself
+                for (int u = 0; u < 4; ++u) pj[u] = __ldg(&pos[j[u]]);  // tail slots point at i itself
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-                const bool ok = q * 4u + u < n;
-                Pair p = make_pair<true, true>(pi, pj[u]);
-                if (ok) {
-                    rho = fmaf(pj[u].w, p.w, rho);
-                    float s = p.g * pj[u].w;  // m_j * gradient
-                    float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
-                    sq += ax * ax + ay * ay + az * az;
-                    gx += ax; gy += ay; gz += az;
+                for (int u = 0; u < 4; ++u) {
+                    const bool ok = q * 4u + u < n;
+                    Pair p = make_pair<true, true>(pi, pj[u]);
+                    if (ok) {
+                        rho = fmaf(pj[u].w, p.w, rho);
+                        float s = p.g * pj[u].w;  // m_j * gradient
+                        float ax = s * p.dx, ay = s * p.dy, az = s * p.dz;
+                        sq += ax * ax + ay * ay + az * az;
+                        gx += ax; gy += ay; gz += az;
+                    }
                 }
+                J = Jn;
             }
-            J = Jn;
-        }
+        });
     }
     for_boundary_contacts<true, true>(i, pi, L, bpos, [&](uint32_t, const Pair& p, const float4& pj) {
         float mb = pj.w * rho0;  // boundary pseudo mass: vol_b * rho0_i

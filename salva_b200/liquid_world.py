@@ -20,7 +20,8 @@ from ._lib import ForceDesc, StepStats, WorldDesc
 DBG = dict(density=0, alpha=1, divergence=2, predicted_density=3, velocity_change=4, num_fluid_contacts=5,
            num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11, he2014_color=12, he2014_gradc=13,
            visc_beta=14, visc_target=15, el_volume0=16, el_rotation=17, el_grad_tr=18, el_stress=19, diffuse_normal=20,
-           diffuse_trapped_air=21, diffuse_wave_crest=22, diffuse_kinetic=23, diffuse_count=24)
+           diffuse_trapped_air=21, diffuse_wave_crest=22, diffuse_kinetic=23, diffuse_count=24,
+           fluid_list_bits=25)
 # floats per particle of the selectors that are not scalars (include/sph.h)
 WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6, 20: 3}
 DIFFUSE_KINDS = ("spray", "foam", "bubble")  # SPH_DIFFUSE_SPRAY / _FOAM / _BUBBLE

@@ -8,8 +8,10 @@ achieved GB/s.  The card name and power limit (read-only nvidia-smi query) are p
 number in it.  The trace goes under --out (default: a temporary directory).
 
 BYTES is the per-particle traffic of one launch of each streaming kernel as the code stores and loads it, for a single
-uniform-mass fluid (C2, C3): reads + writes, with sector-wide loads of a float4 counted whole.  Gather passes and scans have no
-entry: their traffic depends on the contact lists and the grid, so only their time is printed.
+uniform-mass fluid (C2, C3): reads + writes, with sector-wide loads of a float4 counted whole.  The uniform-mass Jacobi gather
+passes (GATHER_OWN) count their own records plus the fluid lists they stream once (list_bytes: the counts and every stored
+group, in the width the last search chose, sph_lists.cuh); the neighbour records they gather are served by L1/L2 and are not
+counted.  Scans and the other passes have no entry: their traffic depends on the grid, so only their time is printed.
 """
 import argparse
 import json
@@ -33,6 +35,21 @@ BYTES = {
     "k_integrate_acc": 48 + 16 + 8 + 4,                  # acc, vc, vel; vc, vyz2, pvx4.w
     "k_update_positions": 16 + 16 + 8 + 16,              # pos, pvx4, vyz2; pos
 }
+
+# own records of the uniform-mass Jacobi passes per particle and launch (reads; writes)
+GATHER_OWN = {
+    "k_vel_update_u": 16 + 16 + 16 + 16 + 16 + 8,         # pk4, vel, vc; vc, pvx4, vyz2
+    "k_vel_divergence_u": 16 + 8 + 4 + 4 + 4 + 16,        # pvx4, vyz2, alpha, dens (predicted); out, pk4
+    "k_vel_divergence_xsph_u": 16 + 8 + 4 + 16 + 4 + 16 + 16,  # pvx4, vyz2, alpha, nr4; divv, pk4, xs
+}
+
+
+def list_bytes(counts, bits):
+    """Bytes one pass streams from the fluid lists: the two counts per particle, and per stored group of four entries 16 B
+    (32-bit entries) or 8 B plus 12 B of window bases per particle (16-bit entries)."""
+    groups = int(((counts + 3) // 4).sum())
+    return 8 * len(counts) + (16 * groups if bits == 32 else 8 * groups + 12 * len(counts))
+
 
 PHASES = [
     ("grid", ("k_bounds", "k_cell_hist", "k_cell_hist_xy", "k_scan_block", "k_scan_add", "k_scanK_block", "k_scanK_add",
@@ -112,6 +129,10 @@ def main():
             world.step(sc["dt"], sc["gravity"])
             step_ms.append(world.stats()["step_ms"])
         torch.cuda.synchronize()
+    import numpy as np
+    counts = np.concatenate([world.debug(f, "num_fluid_contacts").astype(np.int64) for f in fh])
+    bits = int(world.debug(fh[0], "fluid_list_bits")[0]) if n else 32
+    lbytes = list_bytes(counts, bits)
     out = args.out or tempfile.mkdtemp(prefix="profile_step_")
     os.makedirs(out, exist_ok=True)
     prof.export_chrome_trace(os.path.join(out, "profile_step_%s.pt.trace.json" % args.config))
@@ -133,8 +154,11 @@ def main():
         base = k.split("@")[0].split("<")[0]
         nbytes = BYTES.get(base)
         gbs = None
-        if nbytes is not None and ms > 0:
+        if base in GATHER_OWN:
+            nbytes = (GATHER_OWN[base] * n + lbytes) * launches
+        elif nbytes is not None:
             nbytes = nbytes * n * launches
+        if nbytes is not None and ms > 0:
             gbs = nbytes / (ms * 1e-3) / 1e9
         table.append({"phase": phase_of(k), "kernel": k, "launches_per_step": launches, "ms_per_step": ms,
                       "bytes_per_step": nbytes, "gb_per_s": gbs})
@@ -147,6 +171,8 @@ def main():
           (args.config.upper(), n, args.steps, info.get("name"), info.get("power_limit_w")))
     print("step_ms (CUDA events, under the profiler): %s; iterations (div, press) last step: %d, %d" %
           (", ".join("%.3f" % s for s in step_ms), st["n_divergence_iter"], st["n_pressure_iter"]))
+    print("fluid lists: %d-bit entries, %.1f contacts per particle, %.1f B per particle per pass" %
+          (bits, counts.mean() if n else 0.0, lbytes / max(n, 1)))
     print("%-22s %-34s %8s %10s %10s %8s" % ("phase", "kernel", "launch/s", "ms/step", "MB/step", "GB/s"))
     tot = {}
     for t in table:
@@ -158,7 +184,8 @@ def main():
     print("kernel total: %.3f ms/step" % sum(tot.values()))
     if args.json:
         with open(args.json, "w") as fh_:
-            json.dump({"config": args.config, "particles": n, "gpu": info, "step_ms": step_ms, "kernels": table}, fh_, indent=1)
+            json.dump({"config": args.config, "particles": n, "gpu": info, "step_ms": step_ms, "list_bits": bits,
+                       "list_bytes_per_pass": lbytes, "kernels": table}, fh_, indent=1)
 
 
 if __name__ == "__main__":
