@@ -398,14 +398,67 @@ static_assert(!std::is_copy_constructible<DBuf<float>>::value && !std::is_copy_c
                   !std::is_copy_constructible<FluidRec>::value && !std::is_copy_constructible<ColliderRec>::value,
               "records that own device memory move, never copy");
 
-sph_status iisph_step(sph_world* w, float dt_total, const float g[3]);
-sph_status slab_begin_step(sph_world* w);
-sph_status slab_after_sort(sph_world* w);
-sph_status slab_refresh(sph_world* w, void* array, size_t elem);
 struct SlabArray {
     void* p;
     size_t elem;
 };
+
+// Where v* (vel + vc) and kappa live.  Packed (the uniform-mass path): v* in the gather records pvx4 = (x, y, z, v*x) and
+// vyz2 = (v*y, v*z), kappa in pk4 = (x, y, z, kappa); their gathers are split evenly over the texture and LSU pipes
+// (sph_passes.cuh).  Otherwise v* in vs and kappa in kappa.  IISPH reads v* from vs.
+struct VStarRecords {
+    bool packed = false;
+    DBuf<float4> vs, pvx4, pk4;
+    DBuf<float2> vyz2;
+    DBuf<float> kappa;
+    Tex tex_vs, tex_pvx, tex_vyz, tex_pk;  // bound by ensure() over whatever it (re)allocated
+    // n rows (kappa: n + 8, like the other per-particle scalars) and the textures over them
+    cudaError_t ensure(size_t n) {
+        if (!n) return cudaSuccess;  // (a texture needs an allocation)
+        cudaError_t e = vs.ensure(n);
+        if (e == cudaSuccess) e = pvx4.ensure(n);
+        if (e == cudaSuccess) e = pk4.ensure(n);
+        if (e == cudaSuccess) e = vyz2.ensure(n);
+        if (e == cudaSuccess) e = kappa.ensure(n + 8);
+        if (e == cudaSuccess) e = tex_vs.bind(vs);
+        if (e == cudaSuccess) e = tex_pvx.bind(pvx4);
+        if (e == cudaSuccess) e = tex_vyz.bind(vyz2);
+        if (e == cudaSuccess) e = tex_pk.bind(pk4);
+        return e;
+    }
+    // Packed: one DFSPH fluid whose particles all have the same volume.  A slab world takes the packed path on every rank
+    // or on none: volumes default to uniform there, and an empty slab inherits the constant from its first immigrant only
+    // through the general path -> keep it simple: require particles with uniform volumes on this rank, otherwise fall back
+    // (all ranks are built by the same host code).
+    void choose(int32_t solver, const std::vector<FluidRec>& fluids) {
+        packed = solver == SPH_SOLVER_DFSPH && fluids.size() == 1 && fluids[0].uniform_mass > 0.f;
+    }
+    // the streaming passes' v*, and the v* of vs alone (IISPH)
+    VStar view() const { return {vs.p, packed ? pvx4.p : nullptr, packed ? vyz2.p : nullptr}; }
+    VStar plain() const { return {vs.p, nullptr, nullptr}; }
+    // what a ghost refresh of v* sends (returns the count), and of kappa
+    int vstar_arrays(SlabArray a[2]) const {
+        a[0] = {packed ? pvx4.p : vs.p, sizeof(float4)};
+        a[1] = {vyz2.p, sizeof(float2)};
+        return packed ? 2 : 1;
+    }
+    SlabArray kappa_array() const { return packed ? SlabArray{pk4.p, sizeof(float4)} : SlabArray{kappa.p, sizeof(float)}; }
+    // a step graph's dependence on the layout, the buffers and the textures (graph_key)
+    template <class Put>
+    void key(Put put) const {
+        put(&packed, sizeof packed);
+        for (const void* p : {(const void*)vs.p, (const void*)pvx4.p, (const void*)pk4.p, (const void*)vyz2.p, (const void*)kappa.p}) put(&p, sizeof p);
+        for (cudaTextureObject_t t : {tex_vs.obj, tex_pvx.obj, tex_vyz.obj, tex_pk.obj}) put(&t, sizeof t);
+    }
+};
+
+sph_status dfsph_step(sph_world* w, float remaining, const float g[3]);
+DensArgs density_args(sph_world* w);
+sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, bool akinci = false);
+sph_status iisph_step(sph_world* w, float dt_total, const float g[3]);
+sph_status slab_begin_step(sph_world* w);
+sph_status slab_after_sort(sph_world* w);
+sph_status slab_refresh(sph_world* w, void* array, size_t elem);
 sph_status slab_refresh_n(sph_world* w, const SlabArray* arrays, int n_arrays);
 sph_status p2p_setup(sph_world* w);
 sph_status post_density_refresh(sph_world* w);
@@ -559,17 +612,12 @@ struct sph_world {
     DBuf<uint32_t> orig[2], borig[2];
     DBuf<uint32_t> gid[2];  // caller-visible particle ids (default: original index); follow particles across ranks
     DBuf<float> press[2];
-    DBuf<float4> vs, acc, normals, dbg_acc;
-    DBuf<float> dens, alpha, kappa, divv, pred, bvol, bforce;
+    DBuf<float4> acc, normals, dbg_acc;
+    DBuf<float> dens, alpha, divv, pred, bvol, bforce;
     DBuf<uint32_t> cid, rank, perm, cstart, bcid, brank, bperm, bstart, scan_aux[3], scan_aux_k[3];
     DBuf<unsigned long long> skey;  // deterministic mode: the in-cell sort keys beside perm / bperm (k_cell_scatter)
     ListState lists;
-    // uniform-mass packed gather records (sph_passes.cuh): pvx4 = (x,y,z,v*x), vyz2 = (v*y,v*z), pk4 = (x,y,z,kappa); their
-    // gathers are split evenly over the texture and LSU pipes (even / odd contacts)
-    bool unimass = false;
-    DBuf<float4> pvx4, pk4;
-    DBuf<float2> vyz2;
-    Tex tex_pvx, tex_vyz, tex_pk;
+    VStarRecords vstar;
     DBuf<float> he_colors, he_gradc;  // He2014 colours / squared colour-gradient norms (he2014_surface_tension.rs:16-17)
     DBuf<uint32_t> q_out, q_count;     // particles_intersecting_aabb results
     DBuf<float> map_pos, map_vel;      // sph_fluid_map_positions / _velocities: ORIGINAL-order device views
@@ -581,7 +629,6 @@ struct sph_world {
     DBuf<float> ct_w[2], ct_g[2];
     DBuf<float4> xs;  // the XSPH sums or the Akinci fluid force of a divergence evaluation (fold_state)
     uint32_t fused_nblk = 0;
-    Tex tex_vs;  // the general evaluations gather v* through the texture pipe
     DBuf<float> partial;
     DBuf<StepScalars> d_ss;
     StepScalars* h_ss = nullptr;  // pinned mirror of d_ss: every read-back lands in its own fields
@@ -961,14 +1008,10 @@ sph_status ensure_fluid_buffers(sph_world* w) {
         CU(w->gid[k].ensure(N, keep, w->st));
         if (w->desc.solver == SPH_SOLVER_IISPH) CU(w->press[k].ensure(N, keep, w->st));
     }
-    CU(w->vs.ensure(N));
-    CU(w->pvx4.ensure(N));
-    CU(w->pk4.ensure(N));
-    CU(w->vyz2.ensure(N));
+    CU(w->vstar.ensure(N));
     CU(w->acc.ensure(N));
     CU(w->dens.ensure(N + 8));
     CU(w->alpha.ensure(N + 8));
-    CU(w->kappa.ensure(N + 8));
     CU(w->divv.ensure(N + 8));
     CU(w->pred.ensure(N + 8));
     CU(w->cid.ensure(N));
@@ -1021,10 +1064,7 @@ sph_status stage_up(sph_world* w) {
     w->staged = false;
     w->lists_valid = false;
     w->slab.global_valid = false;
-    // a slab world takes the fast path on every rank or on none: volumes default to uniform there, and an empty
-    // slab inherits the constant from its first immigrant only through the classic path -> keep it simple: require
-    // particles with uniform volumes on this rank, otherwise fall back (all ranks are built by the same host code).
-    w->unimass = w->desc.solver == SPH_SOLVER_DFSPH && w->fluids.size() == 1 && w->fluids[0].uniform_mass > 0.f;
+    w->vstar.choose(w->desc.solver, w->fluids);
     return SPH_OK;
 }
 
@@ -1239,7 +1279,7 @@ sph_status phase_grid(sph_world* w) {
             g.n1 = 3;
         }
         // reorder + v* = vel + vc (the divergence solve works on vel + vc carried over from the previous step, Appendix A.3.2) in one pass
-        LAUNCH(k_gather_vstar, N, 256, (uint32_t)N, w->perm.p, g, w->vs.p, w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
+        LAUNCH(k_gather_vstar, N, 256, (uint32_t)N, w->perm.p, g, w->vstar.view());
         w->cur = c ^ 1;
     }
     TRY(sort_boundaries(w, ncell));
@@ -1253,19 +1293,6 @@ sph_status phase_grid(sph_world* w) {
     return SPH_OK;
 }
 
-// Inputs and outputs of the density sweep that the DFSPH neighbour search runs over its fresh lists (density_alpha_div)
-sph_status density_args(sph_world* w, DensArgs* D) {
-    if (w->unimass) {
-        CU(w->tex_vyz.bind(w->vyz2));
-        CU(w->tex_pvx.bind(w->pvx4));
-    } else {
-        CU(w->tex_vs.bind(w->vs));
-    }
-    *D = DensArgs{w->unimass ? w->pvx4.p : w->pos[w->cur].p, w->unimass ? w->tex_pvx.obj : 0, w->vs.p, w->unimass ? 0 : w->tex_vs.obj, w->vyz2.p,
-                  w->unimass ? w->tex_vyz.obj : 0, w->dens.p, w->alpha.p, w->divv.p, w->kappa.p, w->pk4.p, w->partial.p, &w->d_ss.p->err};
-    return SPH_OK;
-}
-
 // `speculative` (optional) enqueues the work that follows the neighbour search and only writes scratch (the density
 // pass): it is launched BEFORE the host learns whether the lists overflowed, so the GPU is busy during that round trip;
 // on overflow the lists are rebuilt with a larger capacity and the speculative work is simply enqueued again.
@@ -1275,9 +1302,9 @@ sph_status phase_neighbors(sph_world* w, sph_status (*speculative)(sph_world*) =
     size_t N = w->N, B = w->B;
     int c = w->cur, bc = w->bcur;
     const bool multi = w->fluids.size() > 1;
-    const bool dens = N && w->desc.solver == SPH_SOLVER_DFSPH, uni = dens && w->unimass;
+    const bool dens = N && w->desc.solver == SPH_SOLVER_DFSPH, uni = dens && w->vstar.packed;
     DensArgs D{};
-    if (dens) TRY(density_args(w, &D));
+    if (dens) D = density_args(w);
     using NbrKernel = void (*)(const float4*, const float4*, const uint32_t*, const float4*, const float4*, const uint32_t*, ListsOut,
                                uint32_t*, DensArgs);
     NbrKernel search;
@@ -1429,23 +1456,6 @@ bool any_bforce(const sph_world* w) {
 
 // ---- gather passes: one wrapper per reference function ------------------------------------
 
-// ghost refresh of v* in whichever representation the evaluations and the velocity fold (vel = v* for ghosts too) read:
-// the packed records on the uniform-mass path (one NCCL group), else vs
-sph_status refresh_vstar(sph_world* w) {
-    if (!w->slab.active) return SPH_OK;
-    if (w->unimass) {
-        SlabArray a[2] = {{w->pvx4.p, sizeof(float4)}, {w->vyz2.p, sizeof(float2)}};
-        return slab_refresh_n(w, a, 2);
-    }
-    return slab_refresh(w, w->vs.p, sizeof(float4));
-}
-// ghost refresh of the evaluation's output (kappa) — only needed when an update follows
-sph_status refresh_kappa(sph_world* w) {
-    if (!w->slab.active) return SPH_OK;
-    if (w->unimass) return slab_refresh(w, w->pk4.p, sizeof(float4));
-    return slab_refresh(w, w->kappa.p, sizeof(float));
-}
-
 sph_status launch_density_alpha(sph_world* w) {
     size_t N = w->N;
     int c = w->cur, bc = w->bcur;
@@ -1454,101 +1464,12 @@ sph_status launch_density_alpha(sph_world* w) {
     DISPATCH1(k_density_alpha, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->dens.p, w->alpha.p, &w->d_ss.p->err);
     return SPH_OK;  // the ghost refresh of rho follows in post_density_refresh(), once the list-capacity check has passed
 }
-// Ghost refresh of what the density pass produced (rho; DFSPH: also kappa of the fused first divergence evaluation).  Kept out
-// of the density launch itself so that the launch stays purely local: it is enqueued SPECULATIVELY behind the neighbour
-// search (before the host knows whether the lists overflowed), and a rank that has to regrow its lists and repeat it must not
-// leave its neighbours waiting in a collective they entered once and it enters twice.
-sph_status post_density_refresh(sph_world* w) {
-    if (!w->slab.active || !w->N) return SPH_OK;
-    if (w->desc.solver == SPH_SOLVER_DFSPH) {
-        SlabArray a[2] = {{w->dens.p, sizeof(float)}, {w->unimass ? (void*)w->pk4.p : (void*)w->kappa.p, w->unimass ? sizeof(float4) : sizeof(float)}};
-        return slab_refresh_n(w, a, 2);
-    }
-    return slab_refresh(w, w->dens.p, sizeof(float));  // XSPH / artificial viscosity / Akinci gather rho_j of ghosts
-}
-// compute_divergences (predict = false) / compute_predicted_densities (predict = true); returns #partials.
-// The fluid term of the FIRST force of a single-fluid DFSPH world can ride with the divergence evaluations when it is an
-// XSPHViscosity without a boundary term (see k_vel_divergence_xsph_u).
-bool xsph_fusable(const sph_world* w) {
-    if (w->desc.solver != SPH_SOLVER_DFSPH || !w->unimass || w->slab.active) return false;
-    if (w->fluids.size() != 1 || w->fluids[0].forces.empty()) return false;
-    const sph_force_desc& d = w->fluids[0].forces[0].d;
-    return d.kind == SPH_FORCE_XSPH_VISCOSITY && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0);
-}
-// ... and an Akinci2013SurfaceTension: its normals ride with the loop's first update (k_vel_update_u<.., NORMALS>) and its fluid
-// term with the evaluation after it (k_vel_divergence_xsph_u<2>), when it is the first force of the single uniform-mass fluid
-// and has no boundary term (no adhesion, or no boundaries) and no boundary wants forces.  Otherwise phase_forces computes it.
-bool akinci_fusable_u(const sph_world* w) {
-    if (w->desc.solver != SPH_SOLVER_DFSPH || !w->unimass || w->slab.active) return false;
-    if (w->fluids.size() != 1 || w->fluids[0].forces.empty()) return false;
-    const sph_force_desc& d = w->fluids[0].forces[0].d;
-    return d.kind == SPH_FORCE_AKINCI2013_TENSION && d.p[0] != 0.f && (d.p[1] == 0.f || w->B == 0) && !any_bforce(w);
-}
 // Akinci2013 kernel-normalisation constants of `h` (akinci2013_surface_tension.rs): cohesion, its h^6 / 64 offset, adhesion
 struct AkinciNorms {
     float coh_norm, h6_64, adh_norm;
 };
 AkinciNorms akinci_norms(float h) {
     return {32.0f / (3.14159265358979323846f * powf(h, 9.f)), powf(h, 6.f) / 64.0f, 0.007f / powf(h, 3.25f)};
-}
-
-// akinci: the Akinci fluid force rides along (evaluation 1 of the divergence loop, on the normals update 0 wrote).
-sph_status launch_vel_divergence(sph_world* w, bool predict, uint32_t* nblk, bool akinci = false) {
-    int c = w->cur, bc = w->bcur;
-    const bool multi = w->fluids.size() > 1;
-    const bool xsf = !predict && xsph_fusable(w), akf = !predict && akinci;
-    if (xsf || akf) CU(w->xs.ensure(std::max(w->Ntot, w->N)));
-    const Lists L = w->lists.view();
-    if (w->unimass) {
-        CU(w->tex_pvx.bind(w->pvx4));
-        CU(w->tex_vyz.bind(w->vyz2));
-    } else {
-        CU(w->tex_vs.bind(w->vs));
-    }
-    float* out = predict ? w->pred.p : w->divv.p;
-    const size_t N = w->N;
-    if (w->unimass) {
-        if (predict) {
-            LAUNCH((k_vel_divergence_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L,
-                   w->dens.p, w->alpha.p, out, w->pk4.p, w->partial.p, w->dt, &w->d_ss.p->err);
-        } else if (xsf) {
-            const float cf = w->fluids[0].forces[0].d.p[0];
-            LAUNCH((k_vel_divergence_xsph_u<1>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p,
-                   w->alpha.p, out, w->pk4.p, w->partial.p, w->xs.p, cf, (const float4*)nullptr, 0.f, 0.f);
-        } else if (akf) {  // the Akinci fluid force rides along: xs = its sum, on the normals the update wrote
-            const AkinciNorms an = akinci_norms(w->h);
-            LAUNCH((k_vel_divergence_xsph_u<2>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, L, w->dens.p,
-                   w->alpha.p, out, w->pk4.p, w->partial.p, w->xs.p, w->fluids[0].forces[0].d.p[0], w->normals.p, an.coh_norm, an.h6_64);
-        } else {
-            LAUNCH((k_vel_divergence_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->vyz2.p, w->tex_vyz.obj, w->bpos[bc].p, w->bvel[bc].p, L,
-                   w->dens.p, w->alpha.p, out, w->pk4.p, w->partial.p, w->dt, &w->d_ss.p->err);
-        }
-    } else {
-        DISPATCH2(k_vel_divergence, multi, predict, N, PASS_T, w->pos[c].p, w->vs.p, w->tex_vs.obj, w->vel[c].p, w->bpos[bc].p, w->bvel[bc].p, L,
-                  w->dens.p, w->alpha.p, out, w->kappa.p, w->partial.p, w->dt, &w->d_ss.p->err);
-    }
-    *nblk = cdiv(N, PASS_T);
-    return SPH_OK;
-}
-// compute_velocity_changes_for_divergence (pressure = false) / compute_velocity_changes (pressure = true).
-// normals: the Akinci normals ride along (see akinci_fusable_u).
-sph_status launch_vel_update(sph_world* w, bool pressure, bool normals = false) {
-    int c = w->cur, bc = w->bcur;
-    const bool multi = w->fluids.size() > 1, bf = any_bforce(w);
-    const Lists L = w->lists.view();
-    if (w->unimass) CU(w->tex_pk.bind(w->pk4));
-    if (normals) CU(w->normals.ensure(std::max(w->Ntot, w->N)));
-    const size_t N = w->N;
-    if (normals)  // akinci_fusable_u: uniform mass, no boundary forces
-        LAUNCH((k_vel_update_u<false, false, true>), N, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
-               w->vyz2.p, w->bforce.p, w->inv_dt, w->dens.p, w->normals.p);
-    else if (w->unimass)
-        DISPATCH2(k_vel_update_u, bf, pressure, N, PASS_T, w->pk4.p, w->tex_pk.obj, w->vel[c].p, w->bpos[bc].p, L, w->vc[c].p, w->pvx4.p,
-                  w->vyz2.p, w->bforce.p, w->inv_dt, (const float*)nullptr, (float4*)nullptr);
-    else
-        DISPATCH3(k_vel_update, multi, bf, pressure, N, PASS_T, w->pos[c].p, w->vel[c].p, w->bpos[bc].p, L, w->kappa.p, w->vc[c].p, w->vs.p,
-                  w->bforce.p, w->inv_dt);
-    return refresh_vstar(w);  // the following evaluation gathers v*_j of ghosts (and the velocity fold reads vel = v* for ghosts)
 }
 
 // ---- ParticlesContacts materialisation + the context-style host plugin call (nonpressure_force.rs:15-27) ---------------
@@ -1682,9 +1603,9 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
                     const AkinciNorms an = akinci_norms(w->h);
                     const float coh_norm = an.coh_norm, h6_64 = an.h6_64, adh_norm = an.adh_norm;
                     if ((fold & FOLD_NR4) && f == 0) {  // normals (and rho, in .w) came with the first divergence update
-                        CU(w->tex_pvx.bind(w->pvx4));
-                        if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
-                        else LAUNCH((k_akinci_force_u<false>), N, PASS_T, w->pvx4.p, w->tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
+                        const VStarRecords& R = w->vstar;
+                        if (bf) LAUNCH((k_akinci_force_u<true>), N, PASS_T, R.pvx4.p, R.tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
+                        else LAUNCH((k_akinci_force_u<false>), N, PASS_T, R.pvx4.p, R.tex_pvx.obj, w->normals.p, w->bpos[bc].p, L, w->acc.p, w->bforce.p, p[0], p[1], coh_norm, h6_64, adh_norm);
                         break;
                     }
                     DISPATCH1(k_akinci_normals, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->dens.p, w->normals.p, (uint32_t)f);
@@ -1774,185 +1695,6 @@ sph_status timestep_advance(sph_world* w, float remaining) {
     w->dt = dt;
     w->inv_dt = dt == 0.f ? 0.f : 1.0f / dt;
     if (!w->cap) w->substeps.push_back(dt);
-    return SPH_OK;
-}
-
-// update_velocities :422-430, zero vc :689-691, acc += gravity :574-578, the non-pressure forces and the integration, after the
-// divergence loop ended in fold state `fold` (fold_state)
-sph_status dfsph_fold(sph_world* w, float remaining, const float g[3], uint32_t fold) {
-    size_t N = w->N;
-    int c = w->cur;
-    // the first force of fluid 0 may already sit in xs: the XSPH sums of the loop's last evaluation (acc = g + xs * inv_dt) or
-    // the Akinci fluid force (acc = g + xs; a scale of 1 leaves the product exact)
-    const bool folded = fold & (FOLD_XS | FOLD_AKINCI);
-    const float4* xs = folded ? w->xs.p : nullptr;
-    const float xs_scale = (fold & FOLD_AKINCI) ? 1.0f : w->inv_dt;
-    // nothing (else) to launch in the force phase?  Then fold, acceleration and integration are one streaming pass, unless
-    // substepping needs the CFL reduction between the fold and the integration, which takes the new dt
-    bool quiet_forces = true;
-    for (size_t f = 0; f < w->fluids.size() && quiet_forces; ++f)
-        for (const ForceRec& fr : w->fluids[f].forces)
-            if (!(folded && f == 0 && &fr == &w->fluids[0].forces[0])) quiet_forces = false;
-    if (quiet_forces && w->cfl_coeff == 0.f) {
-        TRY(ev_record(w, EV_FOLD));
-        TRY(ev_record(w, EV_FORCES));
-        TRY(timestep_advance(w, remaining));  // :702
-        LAUNCH(k_fold_integrate, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale, w->dt,
-               w->unimass ? w->pvx4.p : nullptr, w->unimass ? w->vyz2.p : nullptr);
-    } else {
-        LAUNCH(k_fold_velocities, w->Ntot, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, g[0], g[1], g[2], xs, xs_scale,  // ghosts too (vel = v*)
-               w->unimass ? (const float4*)w->pvx4.p : nullptr, w->unimass ? (const float2*)w->vyz2.p : nullptr);
-        TRY(ev_record(w, EV_FOLD));
-        if (!quiet_forces) TRY(phase_forces(w, fold));
-        TRY(ev_record(w, EV_FORCES));
-        TRY(launch_cfl_max(w, w->vel[c].p, remaining));
-        TRY(timestep_advance(w, remaining));  // :702
-        LAUNCH(k_integrate_acc, N, 256, w->vel[c].p, w->vc[c].p, w->vs.p, w->acc.p, w->dt, w->unimass ? w->pvx4.p : nullptr,
-               w->unimass ? w->vyz2.p : nullptr);
-    }
-    TRY(refresh_vstar(w));
-    return ev_record(w, EV_INTEG);
-}
-
-// A condition of dfsph_step's loops: out of capture a host bool that decide() sets, in capture a conditional handle
-struct Cond {
-    bool v = false;
-    cudaGraphConditionalHandle h = 0;
-};
-template <class Fn>
-sph_status cap_cond(sph_world* w, cudaGraphConditionalHandle h, cudaGraphConditionalNodeType type, Fn body);  // sph_graph.inl
-sph_status new_handle(sph_world* w, cudaGraphConditionalHandle* h);
-
-sph_status cond_new(sph_world* w, Cond* c) { return w->cap ? new_handle(w, &c->h) : SPH_OK; }
-
-// IF (cudaGraphCondTypeIf) or WHILE c { body }: plain control flow out of capture, a conditional node in capture
-template <class Fn>
-sph_status cond(sph_world* w, const Cond& c, cudaGraphConditionalNodeType type, Fn body) {
-    if (w->cap) return cap_cond(w, c.h, type, body);
-    if (type == cudaGraphCondTypeIf) return c.v ? body() : SPH_OK;
-    while (c.v) TRY(body());
-    return SPH_OK;
-}
-
-// The decision after evaluation i of loop r (i < 0: the evaluation after the last decided one), from nblk error partials.
-// It sets c[0] to "an update follows", c[1] to "an update and another evaluation follow", c[2] to "an update follows and
-// ends the loop", c[3] and c[4] to false (a graph's handles keep their values from the last step); null entries are not
-// set.  Out of capture it is host_decision with the step's counts; in capture k_loop_decide, behind a k_reduce_partials of the
-// evaluation's partials wherever its error is read.
-sph_status decide(sph_world* w, const LoopRule& r, int i, uint32_t nblk, std::array<Cond*, 5> c) {
-    if (w->cap) {
-        if (i < 0 || loop_decision(r, (uint32_t)i, [] { return 0.f; }).read) {  // i < 0: the device decides whether it reads
-            const int nf = (int)w->fluids.size();
-            k_reduce_partials<<<nf, 256, 0, w->st>>>(w->partial.p, nblk, nf, w->d_ss.p->loop_err);
-        }
-        Decide d{};
-        for (int k = 0; k < 5; ++k)
-            if (c[k]) d.h[k] = c[k]->h;
-        k_loop_decide<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, w->d_ss.p->loop_err, r, i, d);
-        CU(cudaGetLastError());
-        return SPH_OK;
-    }
-    sph_step_stats& S = w->stats;
-    LoopDecision d;
-    TRY(host_decision(w, r, (r.divergence ? S.n_divergence_eval : S.n_pressure_eval)++, nblk,
-                      r.divergence ? &S.last_divergence_error : &S.last_density_error, &d));
-    if (!d.brk) (r.divergence ? S.n_divergence_iter : S.n_pressure_iter)++;
-    const bool v[5] = {!d.brk, d.more, !d.brk && !d.more, false, false};
-    for (int k = 0; k < 5; ++k)
-        if (c[k]) c[k]->v = v[k];
-    return SPH_OK;
-}
-
-// DFSPHSolver::step dfsph_solver.rs:667-708 for the substep with remaining time R_k.  sph_world_step and the step graph
-// (sph_graph.inl) run these same loops: out of capture their conditions are host bools, in capture conditional nodes.
-sph_status dfsph_step(sph_world* w, float remaining, const float g[3]) {
-    size_t N = w->N;
-    int c = w->cur;
-    // divergence_solve :466-503 (uses the PREVIOUS step's inv_dt; 0 on the first step), unrolled where its passes depend on
-    // the iteration: evaluation 0 (the neighbour search's), update 0 (with the Akinci normals), evaluation 1 (with the XSPH
-    // sums or the Akinci force), then a uniform WHILE body and the update that ends a loop running out of iterations
-    w->stats.n_divergence_iter = w->stats.n_divergence_eval = 0;
-    const bool akf = akinci_fusable_u(w), xsf = xsph_fusable(w);
-    const LoopRule rd = loop_rule(w, true);
-    uint32_t nblk = w->fused_nblk;
-    auto div_update = [&](bool first) -> sph_status {
-        if (!first) TRY(refresh_kappa(w));  // the update gathers kappa_j of ghosts (post_density_refresh sent evaluation 0's)
-        TRY(span_begin(w, SP_DIV_UPD));
-        TRY(launch_vel_update(w, false, first && akf));
-        return span_end(w);
-    };
-    auto div_eval = [&](bool first) -> sph_status {
-        TRY(span_begin(w, SP_DIV_EVAL));
-        TRY(launch_vel_divergence(w, false, &nblk, first && akf));
-        return span_end(w);
-    };
-    if (rd.maxit > 0) {  // max_divergence_iter 0: no pass at all
-        Cond upd0, eval1, more, tail;
-        for (Cond* x : {&upd0, &eval1, &more, &tail}) TRY(cond_new(w, x));
-        TRY(decide(w, rd, 0, nblk, {&upd0, &eval1, nullptr, &more, &tail}));
-        TRY(cond(w, upd0, cudaGraphCondTypeIf, [&] { return div_update(true); }));
-        TRY(cond(w, eval1, cudaGraphCondTypeIf, [&] {
-            TRY(div_eval(true));
-            return decide(w, rd, 1, nblk, {nullptr, &more, &tail});
-        }));
-        TRY(cond(w, more, cudaGraphCondTypeWhile, [&] {
-            TRY(div_update(false));
-            TRY(div_eval(false));
-            return decide(w, rd, -1, nblk, {nullptr, &more, &tail});
-        }));
-        TRY(cond(w, tail, cudaGraphCondTypeIf, [&] { return div_update(false); }));
-    }
-    TRY(ev_record(w, EV_DIV));
-    // the fold in the state the loop ended in: from the host's counts, or in capture one branch per state it can end in
-    if (!w->cap || !(xsf || akf) || rd.maxit == 0) {
-        TRY(dfsph_fold(w, remaining, g, fold_state(xsf, akf, w->stats.n_divergence_eval, w->stats.n_divergence_iter)));
-    } else {
-        const uint32_t states[3] = {0u, xsf ? FOLD_XS : FOLD_NR4, FOLD_NR4 | FOLD_AKINCI};
-        const int n_states = xsf ? 2 : 3;
-        Decide d{};
-        for (int k = 0; k < n_states; ++k) TRY(new_handle(w, &d.h[states[k]]));
-        k_fold_arm<<<1, 1, 0, w->st>>>(w->graphs.ctl.p, w->graphs.rec.p, xsf, akf, d);
-        for (int k = 0; k < n_states; ++k)
-            TRY(cap_cond(w, d.h[states[k]], cudaGraphCondTypeIf, [&] { return dfsph_fold(w, remaining, g, states[k]); }));
-    }
-    // pressure_solve :432-464 (with the new inv_dt): evaluation 0, a uniform WHILE body, and the update that ends a loop
-    // running out of iterations
-    w->stats.n_pressure_iter = w->stats.n_pressure_eval = 0;
-    const LoopRule rp = loop_rule(w, false);
-    auto press_update = [&]() -> sph_status {
-        TRY(refresh_kappa(w));
-        TRY(span_begin(w, SP_PUPD));
-        TRY(launch_vel_update(w, true));
-        return span_end(w);
-    };
-    auto press_eval = [&]() -> sph_status {
-        TRY(span_begin(w, SP_PRED));
-        TRY(launch_vel_divergence(w, true, &nblk));
-        return span_end(w);
-    };
-    if (rp.maxit > 0) {  // max_pressure_iter 0: no pressure pass at all
-        Cond more, tail;
-        TRY(cond_new(w, &more));
-        TRY(cond_new(w, &tail));
-        TRY(press_eval());
-        TRY(decide(w, rp, 0, nblk, {nullptr, &more, &tail}));
-        TRY(cond(w, more, cudaGraphCondTypeWhile, [&] {
-            TRY(press_update());
-            TRY(press_eval());
-            return decide(w, rp, -1, nblk, {nullptr, &more, &tail});
-        }));
-        TRY(cond(w, tail, cudaGraphCondTypeIf, press_update));
-    }
-    TRY(ev_record(w, EV_PRESS));
-    {
-        CellBox* next = &w->d_ss.p->next;
-        if (w->cap) k_bounds_init<<<1, 1, 0, w->st>>>(next);
-        else CU(cudaMemcpyAsync(next, &CELL_BOX_EMPTY, sizeof(CellBox), cudaMemcpyHostToDevice, w->st));
-        LAUNCH(k_update_positions, N, 256, w->pos[c].p, w->vs.p, w->unimass ? (const float4*)w->pvx4.p : nullptr,
-               w->unimass ? (const float2*)w->vyz2.p : nullptr, w->dt, w->slab.active ? nullptr : next);  // :411-420
-        w->nb_pending = !w->slab.active;
-    }
-    CU(cudaGetLastError());
     return SPH_OK;
 }
 
@@ -2137,6 +1879,7 @@ sph_status world_step(sph_world* w, float dt, const float g[3], const sph_coupli
 }  // namespace
 
 #include "sph_slab.inl"
+#include "sph_dfsph_host.inl"
 #include "sph_iisph_host.inl"
 #include "sph_elasticity_host.inl"
 #include "sph_viscosity_host.inl"

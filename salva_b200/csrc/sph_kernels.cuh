@@ -1054,11 +1054,33 @@ __global__ void k_reduce_partials(const float* __restrict__ partial, uint32_t nb
 #endif
 constexpr int PASS_T = SPH_PASS_T;  // threads per block of the gather passes
 
+// Where v* lives, as the streaming passes see it (VStarRecords on the host): on the uniform-mass path (pvx != nullptr) only in
+// the packed records pvx.w and vyz, and vs is not written; else in vs.  The passes take it as a __grid_constant__ parameter
+// and read its pointers from the parameter bank, as they would plain pointer parameters.
+struct VStar {
+    float4* vs;
+    float4* pvx;
+    float2* vyz;
+    // for passes that do not write v*: reads through the read-only data cache
+    __device__ __forceinline__ float4 load(uint32_t i) const {
+        if (!pvx) return __ldg(&vs[i]);
+        const float2 b = __ldg(&vyz[i]);
+        return make_float4(__ldg(&pvx[i].w), b.x, b.y, 0.f);
+    }
+    // v* of slot i, and (packed) the position p that shares its record
+    __device__ __forceinline__ void store(uint32_t i, const float4& p, float sx, float sy, float sz) const {
+        if (pvx) {
+            pvx[i] = make_float4(p.x, p.y, p.z, sx);
+            vyz[i] = make_float2(sy, sz);
+        } else {
+            vs[i] = make_float4(sx, sy, sz, 0.f);
+        }
+    }
+};
+
 // The fluid reorder fused with v* = vel + vc: the sorted pos / vel / vc are in registers anyway, so v* and the packed
 // gather records are written by the same pass (saves re-reading 48 B per particle and a launch).  g.in4 / out4 [0..2] = pos, vel, vc.
-// Uniform mass (pvx != nullptr): v* lives only in the packed records pvx.w and vyz, and vs is not written.
-__global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, GatherSet g, float4* __restrict__ vs, float4* __restrict__ pvx,
-                               float2* __restrict__ vyz) {
+__global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, GatherSet g, const __grid_constant__ VStar vst) {
     uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
     if (s >= n) return;
     const uint32_t src = perm[s];
@@ -1069,20 +1091,7 @@ __global__ void k_gather_vstar(uint32_t n, const uint32_t* __restrict__ perm, Ga
 #pragma unroll
     for (int a = 0; a < 4; ++a)
         if (a < g.n1) g.out1[a][s] = g.in1[a][src];
-    const float sx = v.x + c.x, sy = v.y + c.y, sz = v.z + c.z;
-    if (pvx) {
-        pvx[s] = make_float4(p.x, p.y, p.z, sx);
-        vyz[s] = make_float2(sy, sz);
-    } else {
-        vs[s] = make_float4(sx, sy, sz, 0.f);
-    }
-}
-
-// v* of slot i: from the packed records on the uniform-mass path (pvx != nullptr), else from vs
-__device__ __forceinline__ float4 load_vstar(uint32_t i, const float4* __restrict__ vs, const float4* __restrict__ pvx, const float2* __restrict__ vyz) {
-    if (!pvx) return vs[i];
-    const float2 b = vyz[i];
-    return make_float4(pvx[i].w, b.x, b.y, 0.f);
+    vst.store(s, p, v.x + c.x, v.y + c.y, v.z + c.z);
 }
 
 // a10: update_velocities dfsph_solver.rs:422-430 + zero vc :689-691 + acc = gravity (predict_advection :574-578).
@@ -1090,12 +1099,12 @@ __device__ __forceinline__ float4 load_vstar(uint32_t i, const float4* __restric
 // same for owned particles, and ghost particles (multi-GPU) only carry an up-to-date v*.
 // xs (optional): a force sum of the divergence loop (k_vel_divergence_xsph_u): acc = g + xs * scale, rounded like the force
 // pass's `acc += f * scale` on top of the gravity written here.  XSPH sums: scale = inv_dt; the Akinci force: scale = 1, so
-// acc = g + f exactly as `acc = g; acc += f`.  pvx / vyz: as for load_vstar.
-__global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__ vc, const float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
-                                  float gz, const float4* __restrict__ xs, float scale, const float4* __restrict__ pvx, const float2* __restrict__ vyz) {
+// acc = g + f exactly as `acc = g; acc += f`.
+__global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__ vc, const __grid_constant__ VStar vst, float4* __restrict__ acc, float gx, float gy,
+                                  float gz, const float4* __restrict__ xs, float scale) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
-    const float4 v = vel[i], s = load_vstar(i, vs, pvx, vyz);
+    const float4 v = vel[i], s = vst.load(i);
     vel[i] = make_float4(s.x, s.y, s.z, v.w);
     vc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
     float ax = gx, ay = gy, az = gz;
@@ -1110,12 +1119,14 @@ __global__ void k_fold_velocities(float4* __restrict__ vel, float4* __restrict__
 // update_velocities + the gravity / folded-force acceleration + integrate_and_clear_accelerations in ONE pass, for steps whose force
 // phase launches nothing (no plugin, or only the force whose sum rode with the divergence loop): same arithmetic, in the same
 // order, as k_fold_velocities followed by k_integrate_acc.  Ghost slots (multi-GPU) only take the fold part.
-// Uniform mass (pvx != nullptr): v* is read from and written to the packed records only; the whole of pvx[i] is loaded anyway,
-// so it is stored whole (xyz unchanged) rather than as a partial .w store.
-__global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ vc, float4* __restrict__ vs, float4* __restrict__ acc, float gx, float gy,
-                                 float gz, const float4* __restrict__ xs, float scale, float dt_new, float4* __restrict__ pvx, float2* __restrict__ vyz) {
+// Uniform mass (vst.pvx != nullptr): the whole of pvx[i] is loaded anyway, so it is stored whole (xyz unchanged) rather than
+// as a partial .w store.
+__global__ void k_fold_integrate(float4* __restrict__ vel, float4* __restrict__ vc, const __grid_constant__ VStar vst, float4* __restrict__ acc, float gx, float gy,
+                                 float gz, const float4* __restrict__ xs, float scale, float dt_new) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= C.n_fluid) return;
+    float4 *const vs = vst.vs, *const pvx = vst.pvx;
+    float2* const vyz = vst.vyz;
     const float4 v = vel[i];
     float4 s, r;  // v*, and (uniform mass) the packed record
     if (pvx) {
@@ -1161,18 +1172,17 @@ __global__ void k_set_gravity(const float4* __restrict__ vel, float4* __restrict
 // a18: integrate_and_clear_accelerations dfsph_solver.rs:505-518 (+ v* = vel + vc).  The accelerations are NOT cleared here:
 // the next step's k_fold_velocities / k_set_gravity overwrites them with gravity before any force adds to them, so the
 // array doubles as the SPH_DBG_ACCELERATION view and the pass saves 32 B per particle of stores.
-__global__ void k_integrate_acc(const float4* __restrict__ vel, float4* __restrict__ vc, float4* __restrict__ vs, const float4* __restrict__ acc, float dt,
-                                float4* __restrict__ pvx, float2* __restrict__ vyz) {
+__global__ void k_integrate_acc(const float4* __restrict__ vel, float4* __restrict__ vc, const __grid_constant__ VStar vst, const float4* __restrict__ acc, float dt) {
     SPH_OWNED_INDEX(i)
     float4 a = acc[i], c = vc[i], v = vel[i];
     c.x += a.x * dt; c.y += a.y * dt; c.z += a.z * dt;
     vc[i] = c;
     float sx = v.x + c.x, sy = v.y + c.y, sz = v.z + c.z;
-    if (pvx) {  // uniform mass: v* only in the packed records
-        pvx[i].w = sx;  // xyz already hold the position
-        vyz[i] = make_float2(sy, sz);
+    if (vst.pvx) {  // uniform mass: v* only in the packed records
+        vst.pvx[i].w = sx;  // xyz already hold the position
+        vst.vyz[i] = make_float2(sy, sz);
     } else {
-        vs[i] = make_float4(sx, sy, sz, 0.f);
+        vst.vs[i] = make_float4(sx, sy, sz, 0.f);
     }
 }
 
@@ -1197,16 +1207,14 @@ __global__ void k_cfl_max(const float4* __restrict__ vel, const float4* __restri
 
 // a22: update_positions dfsph_solver.rs:411-420: pos += (vel + vc) * dt.  bounds_out (optional): the cell-coordinate AABB of
 // the NEW positions (what k_bounds computes), so the next step's grid is sized without a bounds pass and its host round trip.
-// pvx / vyz: as for load_vstar.
-__global__ void k_update_positions(float4* __restrict__ pos, const float4* __restrict__ vs, const float4* __restrict__ pvx, const float2* __restrict__ vyz,
-                                   float dt, CellBox* __restrict__ bounds_out) {
+__global__ void k_update_positions(float4* __restrict__ pos, const __grid_constant__ VStar vst, float dt, CellBox* __restrict__ bounds_out) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     const bool valid = i < C.n_owned;
     i += C.i_begin;
     CellBox b = CELL_BOX_EMPTY;
     if (valid) {
         float4 p = pos[i];
-        const float4 v = load_vstar(i, vs, pvx, vyz);
+        const float4 v = vst.load(i);
         p.x += v.x * dt; p.y += v.y * dt; p.z += v.z * dt;
         pos[i] = p;
         if (bounds_out) cell_box_add(b, p.x, p.y, p.z, C.h);
