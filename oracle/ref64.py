@@ -345,6 +345,7 @@ class Passes:
         self.mass = np.asarray(mass, F).astype(np.float64)
         self.BP, self.bid = BP, bid
         self.kw, self.kg = kw, kg
+        self.grad_t = grad_threshold(kg, self.h)   # the gradient's zero threshold on d^2
         self.N = len(P)
         every = lambda i, j: np.ones(len(i), bool)  # noqa: E731
         self.allowed_ff = allowed_ff or every
@@ -380,7 +381,7 @@ class Passes:
     def ambiguous(self, pairs=None):
         """Particles with a contact whose squared distance lies within the float32 d2's rounding of the gradient's zero
         threshold: there the kernel may take either side."""
-        t = grad_threshold(self.kg, self.h)
+        t = self.grad_t
         out = np.zeros(self.N, bool)
         for pr in ([self.ff, self.fb] if pairs is None else pairs):
             near = np.abs(pr.d2 - t) <= 8 * U * t
@@ -389,7 +390,7 @@ class Passes:
 
     def _g(self, pr):
         g, ga, ge = kernel(self.kg, "g", pr.r, self.h)
-        z = pr.d2 <= grad_threshold(self.kg, self.h)
+        z = pr.d2 <= self.grad_t
         return np.where(z, 0.0, g), np.where(z, 0.0, ga), np.where(z, 0.0, ge)
 
     def _w(self, pr):

@@ -29,26 +29,26 @@ ZERO_G = (0.0, 0.0, 0.0)
 
 
 # ---- scenes ------------------------------------------------------------------------------------------------------------------
-def _lattice(nx, ny, nz, compress, seed, amplitude, origin=(0.0, 0.0, 0.0)):
+def _lattice(nx, ny, nz, compress, seed, amplitude, origin=(0.0, 0.0, 0.0), r=R):
     from salva_b200 import scenes
-    return scenes.jitter(scenes.block_lattice(nx, ny, nz, R * compress, origin=origin), R, seed, amplitude=amplitude)
+    return scenes.jitter(scenes.block_lattice(nx, ny, nz, r * compress, origin=origin), r, seed, amplitude=amplitude)
 
 
-def _tank(nx, nz, compress, shift=(0.0, 0.0, 0.0), top=1.0):
+def _tank(nx, nz, compress, shift=(0.0, 0.0, 0.0), top=1.0, r=R):
     from salva_b200 import scenes
     s = np.asarray(shift, np.float64)
-    t = scenes.open_tank(tuple(np.array([-R, -R, -R]) + s), tuple(np.array([nx * 2 * R * compress + R, top, nz * 2 * R * compress + R]) + s), R)
+    t = scenes.open_tank(tuple(np.array([-r, -r, -r]) + s), tuple(np.array([nx * 2 * r * compress + r, top, nz * 2 * r * compress + r]) + s), r)
     return t.astype(F)
 
 
-def _bvel(n, seed):
+def _bvel(n, seed, scale=1.0):
     rng = np.random.default_rng(seed)
-    return (np.array([0.05, -0.1, 0.02], F) + rng.normal(0, 0.02, (n, 3))).astype(F)
+    return ((np.array([0.05, -0.1, 0.02]) + rng.normal(0, 0.02, (n, 3))) * scale).astype(F)
 
 
-def _fluid(pts, seed, density0=1000.0, **kw):
+def _fluid(pts, seed, density0=1000.0, vscale=1.0, **kw):
     rng = np.random.default_rng(seed)
-    return dict(positions=pts.astype(F), velocities=rng.normal(0, 0.2, pts.shape).astype(F), density0=density0, **kw)
+    return dict(positions=pts.astype(F), velocities=(rng.normal(0, 0.2, pts.shape) * vscale).astype(F), density0=density0, **kw)
 
 
 def scene_block(shift=(0.0, 0.0, 0.0)):
@@ -76,24 +76,27 @@ def scene_gate():
     return dict(fluids=[_fluid(pts, 11)], boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 5))])
 
 
-def _exact_h_offset(h):
-    """An x at which f32(x + h) - x == h exactly, so the pair (x, x + h) sits at d^2 = h^2 in float32."""
-    for k in range(1, 4096):   # x in [1/8, 1/4): its ulp is h's, so x + h can be exact
-        x = F(0.13 + k * 2.0 ** -26)
+def _exact_h_offset(h, x0=0.13):
+    """An x at which f32(x + h) - x == h exactly, so the pair (x, x + h) sits at d^2 = h^2 in float32: searched upwards
+    from x0 in steps of x0's ulp (x0 in h's binade or the one above it, so x + h can be exact)."""
+    step = float(np.spacing(F(x0)))
+    for k in range(1, 4096):
+        x = F(x0 + k * step)
         y = F(x + F(h))
         if F(y - x) == F(h):
             return x, y
     raise AssertionError("no exact offset found")
 
 
-def fma_flips(h, n, seed):
-    """Pairs of float32 points whose unfused squared distance passes d^2 <= h^2 while the fused one (as the CUDA pair
-    evaluation forms it) does not, found by search with an exact FMA emulation."""
+def fma_flips(h, n, seed, box=(0.3, 0.6)):
+    """Pairs of float32 points (the first of each inside `box` on every axis) whose unfused squared distance passes
+    d^2 <= h^2 while the fused one (as the CUDA pair evaluation forms it) does not, found by search with an exact FMA
+    emulation."""
     rng = np.random.default_rng(seed)
     h2 = F(F(h) * F(h))
     out = []
     while len(out) < n:
-        a = (rng.uniform(0.3, 0.6, (4096, 3))).astype(F)
+        a = (rng.uniform(box[0], box[1], (4096, 3))).astype(F)
         u = rng.normal(size=(4096, 3))
         u /= np.linalg.norm(u, axis=1)[:, None]
         b = (a + u * float(h) * (1 + rng.uniform(-3e-7, 3e-7, (4096, 1)))).astype(F)
@@ -113,7 +116,7 @@ def scene_pairs():
     unfused test accepts while the fused d^2 lies above h^2; and fluid particles nearly on a boundary particle."""
     nx, ny, nz, c = 8, 7, 8, 0.76
     pts = _lattice(nx, ny, nz, c, 41, 0.2)
-    h = F(F(R) * F(2.0) * F(2.0))
+    h = kernel_h(R, 2.0)
     extra = [pts[5], pts[77] + F(0)]                                   # coincident with particles 5 and 77
     extra += [(pts[100] + np.array([5e-8, 0, 0], F)).astype(F)]        # d^2 ~ 2.5e-15 < eps^2
     extra += [(pts[150] + np.array([0, 6e-7, 0], F)).astype(F)]        # eps^2 < d^2 ~ 3.6e-13 < (1e-5 h)^2
@@ -195,6 +198,106 @@ def light(scene):
 SCENES = dict(block=scene_block, far=scene_far, gate=scene_gate, pairs=scene_pairs, volumes=scene_volumes,
               two_fluids=scene_two_fluids, **{"tail%d" % n: (lambda n=n: scene_tail(n)) for n in TAILS})
 
+# ---- other particle radii and smoothing factors ------------------------------------------------------------------------------
+def _scaled(r):
+    """dt and the velocity scale of a scene of particle radius r: both scale as sqrt(r / R), as a gravity-driven flow does, so
+    that one step moves a particle the same fraction of its radius as the scenes at R do."""
+    s = float(np.sqrt(r / R))
+    return DT * s, s
+
+
+def scene_sf1_lattice():
+    """r = 2^-4, smoothing factor 1: h = 2r is the lattice spacing.  An unjittered 7 x 6 x 7 block at exactly representable
+    coordinates, so every axis pair sits at d^2 = h^2 in float32 (a contact: the test is d^2 <= h^2) and an interior particle
+    has six such ties and no other contact: far below the 20-contact gate.  Beside it, a jittered sub-block at 0.6 spacing,
+    whose face diagonals lie inside h and body diagonals just outside, so that n_f + n_b runs through 19, 20 and 21; and the
+    tank, whose walls sit at d^2 = h^2 from the block's outer layer."""
+    r, sf = 2.0 ** -4, 1.0
+    dt, vs = _scaled(r)
+    from salva_b200 import scenes
+    lat = scenes.block_lattice(*SF1_LATTICE, r)
+    sub = _lattice(8, 8, 8, 0.6, 53, 0.1, origin=(SF1_LATTICE[0] * 2 * r + 0.4 * r, 0.0, 0.0), r=r)
+    pts = np.concatenate([lat, sub]).astype(F)
+    n_x = (SF1_LATTICE[0] * 2 * r + 0.4 * r + 8 * 2 * r * 0.6) / (2 * r)   # the tank's extent in lattice spacings
+    tank = _tank(n_x, SF1_LATTICE[2], 1.0, top=1.0, r=r)
+    return dict(particle_radius=r, smoothing_factor=sf, dt=dt, lattice=len(lat),
+                fluids=[_fluid(pts, 67, vscale=vs)], boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 11, vs))])
+
+
+SF1_LATTICE = (7, 6, 7)
+
+
+def lattice_ties(n):
+    """The ordered axis pairs of an nx x ny x nz lattice: its d^2 = h^2 contacts at smoothing factor 1."""
+    nx, ny, nz = n
+    return 2 * ((nx - 1) * ny * nz + nx * (ny - 1) * nz + nx * ny * (nz - 1))
+
+
+def scene_sf3():
+    """r = 0.05, smoothing factor 3 (h = 0.3): the block's geometry (0.75 spacing, jittered, the floor row, the tank)
+    enlarged to 16 x 12 x 14, so that interior particles have about 270 fluid contacts, lists regrow from the initial
+    capacity of 64 past 256, hundreds of entries per particle lie beyond the 32 staged rows, and the boundary lists hold
+    dozens of entries."""
+    nx, ny, nz, c = 16, 12, 14, 0.75
+    pts = _lattice(nx, ny, nz, c, 71, 0.4)
+    row = np.stack([np.linspace(0.05, nx * 2 * R * c - 0.05, 12), np.full(12, 0.01), np.full(12, nz * 2 * R * c + 0.12)], 1)
+    pts = np.concatenate([pts, row.astype(F)])
+    tank = _tank(nx, nz, c + 0.2 / nz, top=1.2)
+    return dict(smoothing_factor=3.0, fluids=[_fluid(pts.astype(F), 73)],
+                boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 13))])
+
+
+def scene_sf_odd():
+    """r = 0.05, smoothing factor 1.37 (h = 0.137), no exact relation to the 0.8 spacing: cell faces fall at irregular
+    offsets between the lattice lines; strongly jittered, about 25 contacts per particle, so the 20-contact gate splits the
+    block."""
+    nx, ny, nz, c = 13, 10, 12, 0.8
+    pts = _lattice(nx, ny, nz, c, 79, 0.5)
+    tank = _tank(nx, nz, c)
+    return dict(smoothing_factor=1.37, fluids=[_fluid(pts, 83)], boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 17))])
+
+
+SMALL_R = 0.002
+
+
+def scene_small():
+    """r = 0.002, smoothing factor 2 (h = 0.008): the gradient's zero threshold is eps^2, above (1e-5 h)^2, the only scale at
+    which the engine's max(eps^2, (1e-5 h)^2) takes its first branch.  The pair scene's edges built for this h inside a 0.76
+    compressed block: coincident particles; pairs at d^2 < (1e-5 h)^2 and at (1e-5 h)^2 < d^2 <= eps^2 (no gradient, because
+    of the eps^2 gate alone), fluid particles at that distance above two floor particles; a pair at exactly d^2 = h^2; pairs
+    the unfused test accepts while the fused d^2 lies above h^2.  And an isolated pair at (1e-5 h)^2 < d^2 <= eps^2, more than
+    h from everything else: with no other contact its gradient is zero only through the eps^2 gate, so a wrong gate shows as
+    an unbounded ratio, not a rounding-sized one (scene["isolated"]: its two indices)."""
+    r = SMALL_R
+    dt, vs = _scaled(r)
+    nx, ny, nz, c = 8, 7, 8, 0.76
+    pts = _lattice(nx, ny, nz, c, 41, 0.2, r=r)
+    h = kernel_h(r, 2.0)
+    band = 1.0e-7   # (1e-5 h) = 8e-8 < band < eps = 1.19e-7
+    extra = [pts[5], pts[77] + F(0)]                                           # coincident with particles 5 and 77
+    extra += [(pts[100] + np.array([5e-8, 0, 0], F)).astype(F)]                # d^2 ~ 2.5e-15 < (1e-5 h)^2 < eps^2
+    extra += [(pts[150] + np.array([0, band, 0], F)).astype(F)]                # (1e-5 h)^2 < d^2 <= eps^2
+    extra += [(pts[200] + np.array([0, 0, -band], F)).astype(F)]
+    x0, x1 = _exact_h_offset(h, x0=0.01)
+    p = pts[250].copy()
+    p[0] = x0
+    q = p.copy()
+    q[0] = x1
+    extra += [p, q]
+    for a, b in fma_flips(h, 3, 5, box=(3 * r, nx * 2 * r * c - 3 * r)):
+        extra += [a, b]
+    tank = _tank(nx, nz, c, top=20 * r, r=r)
+    extra += [(tank[k] + np.array([0, band, 0], F)).astype(F) for k in (40, 60)]   # just above two floor particles
+    a = np.array([0.045, 0.01, 0.01], F)
+    b = a.copy()
+    b[0] = F(a[0] + F(27 * np.spacing(a[0])))
+    pts = np.concatenate([pts, np.asarray(extra, F), a[None], b[None]]).astype(F)
+    return dict(particle_radius=r, dt=dt, isolated=(len(pts) - 2, len(pts) - 1),
+                fluids=[_fluid(pts, 13, vscale=vs)], boundaries=[dict(positions=tank, velocities=_bvel(len(tank), 7, vs))])
+
+
+SCALE_SCENES = dict(sf1_lattice=scene_sf1_lattice, sf3=scene_sf3, sf_odd=scene_sf_odd, small=scene_small)
+
 SIXTEEN_SIZES = (1, 2, 7, 31, 33, 64, 96, 127, 128, 129, 290, 0, 100, 120, 90)   # the sixteenth takes the rest (41)
 SIXTEEN_EMPTIED = 11
 
@@ -274,9 +377,9 @@ VISC_SCRATCH = ("visc_beta", "visc_target")
 EL_SCRATCH = ("el_volume0", "el_rotation", "el_grad_tr", "el_stress")
 
 
-def deform(P, fid, angle, seed):
+def deform(P, fid, angle, seed, r=R):
     """Each fluid's positions rotated by `angle` degrees about a tilted axis through its centre, stretched by a few percent
-    along x and compressed along y, plus jitter of 0.2 % of the particle radius."""
+    along x and compressed along y, plus jitter of 0.2 % of the particle radius r."""
     rng = np.random.default_rng(seed)
     ax = np.array([0.3, 1.0, 0.2]) / np.linalg.norm([0.3, 1.0, 0.2])
     t = np.radians(angle)
@@ -288,7 +391,7 @@ def deform(P, fid, angle, seed):
         sel = fid == k
         c = out[sel].mean(axis=0)
         out[sel] = c + (out[sel] - c) @ M.T
-    return (out + rng.normal(0, 0.002 * R, out.shape)).astype(F)
+    return (out + rng.normal(0, 0.002 * r, out.shape)).astype(F)
 
 
 def _read(world, fh, bh, extra=()):
@@ -335,6 +438,17 @@ def radius(scene):
     return float(scene.get("particle_radius", R))
 
 
+def smoothing(scene):
+    """The scene's smoothing factor (2 unless it says otherwise)."""
+    return float(scene.get("smoothing_factor", 2.0))
+
+
+def kernel_h(r, sf):
+    """The kernel radius a world of particle radius r and smoothing factor sf uses: f32(f32(r sf) * 2), formed as the
+    engine forms it (liquid_world.rs:44-46)."""
+    return F(F(F(r) * F(sf)) * F(2.0))
+
+
 def timestep(scene):
     """The scene's step length (DT unless it says otherwise)."""
     return float(scene.get("dt", DT))
@@ -374,7 +488,7 @@ def passes_for(scene, P=None, kw=0, kg=0, rows=None):
         a, b = bid[i], bid[j]
         return (a == b) | test(bm[a], bf_[a], bm[b], bf_[b])
 
-    h = F(r * F(2.0) * F(2.0))
+    h = kernel_h(r, smoothing(scene))
     return ref64.Passes(h, pos, fid, rho0, mass, bp, bid, allowed_ff, allowed_fb, allowed_bb, kw=kw, kg=kg, rows=rows)
 
 
@@ -459,7 +573,9 @@ MUTANTS = ("drop_entries_32_35", "swap_vy_vz_odd", "gate_at_21", "normals_rho_i"
            # the loop errors, the lagging dt and the carried state
            "error_mean_over_all_fluids", "error_drops_last_block", "error_counts_gated", "error_unclamped",
            "div_threshold_current_inv_dt", "div_bforce_current_inv_dt", "xsph_current_inv_dt", "visc_current_dt",
-           "positions_previous_dt", "vc_not_carried", "vc_carried_unsorted", "fluid15_rho0_of_fluid0", "iisph_previous_dt")
+           "positions_previous_dt", "vc_not_carried", "vc_carried_unsorted", "fluid15_rho0_of_fluid0", "iisph_previous_dt",
+           # other radii and smoothing factors
+           "grad_threshold_h_only", "drop_entries_256_259", "ties_excluded")
 
 
 def alpha_ratio(ps, alpha, bvol, rho0_b=None):
@@ -490,9 +606,16 @@ class Checks:
         self.worst, self.excluded, self.clamp, self.errors, self.nonzero = {}, {}, {}, {}, {}
         ps = self.ps
         self.ff, self.fb = ps.ff, ps.fb
-        if mutant == "drop_entries_32_35":
+        if mutant in ("drop_entries_32_35", "drop_entries_256_259"):
+            lo = 32 if mutant == "drop_entries_32_35" else 256
             rk = ps.ff.rank()
-            self.ff = ps.ff.subset(~((rk >= 32) & (rk < 36)))
+            self.ff = ps.ff.subset(~((rk >= lo) & (rk < lo + 4)))
+        elif mutant == "ties_excluded":   # the search tests d^2 < h^2
+            h2 = F(F(ps.h) * F(ps.h))
+            self.ff = ps.ff.subset(ref64.f32_d2(ps.P[ps.ff.i], ps.P[ps.ff.j]) != h2)
+            self.fb = ps.fb.subset(ref64.f32_d2(ps.P[ps.fb.i], ps.BP[ps.fb.j]) != h2)
+        elif mutant == "grad_threshold_h_only":   # (1e-5 h)^2 without the eps^2 floor
+            ps.grad_t = float(F((1e-5 * ps.h) ** 2))
         elif mutant == "drop_last_boundary":
             last = np.r_[ps.fb.i[1:] != ps.fb.i[:-1], True] if len(ps.fb.i) else np.zeros(0, bool)
             self.fb = ps.fb.subset(~last)
@@ -510,7 +633,7 @@ class Checks:
         if not self.want.any():
             return
         r = ref64.ratio(gpu, ref, C_PASS["boundary_force"]).max(axis=1)
-        t = ref64.grad_threshold(ps.kg, ps.h)
+        t = ps.grad_t
         ex = np.zeros(len(self.want), bool)
         ex[ps.fb.j[np.abs(ps.fb.d2 - t) <= 8 * ref64.U * t]] = True
         off = ~self.want
@@ -566,13 +689,21 @@ class Checks:
             self._alpha(o00["alpha"], bvol)
         return bvol, kw
 
-    def stages(self):
+    def search(self):
+        """The neighbour search's outputs, (0, 0): counts, boundary volumes, rho, alpha and the divergence sweep (v* = V0).
+        Returns the observables, the boundary volumes and the contact keywords of the reference's passes."""
         ps, sc = self.ps, self.scene
         o00, _ = run(self.make_world, sc, (0, 0))
         bvol, kw = self._first_step_lists(o00)
         V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
         self.record("divergence_sweep", o00["divergence"],
                     ps.divergence(V0, bvol, vj=self._vj(V0, self.ff), min_neighbors=self.min_nb, **kw), C_PASS["divergence"])
+        return o00, bvol, kw
+
+    def stages(self):
+        ps, sc = self.ps, self.scene
+        o00, bvol, kw = self.search()
+        V0 = np.concatenate([f["velocities"] for f in sc["fluids"]]).astype(F)
         bvel = np.concatenate([b["velocities"] for b in sc["boundaries"]]).astype(F)
         vs = (o00["V"] + (o00["acceleration"] * F(self.dt)).astype(F)).astype(F)
         self.record("predicted", o00["predicted_density"],
@@ -871,10 +1002,10 @@ class Checks:
         self._becker_step(bk, Q, o, np.tile(np.eye(3), (ps.N, 1, 1)), "el_rest_" + tag)
         R_prev = o["el_rotation"].reshape(ps.N, 3, 3).astype(np.float64)
         if m == "el_rest_lists_recaptured":
-            P2 = deform(o["P"], ps.fid, angle, seed=29)
+            P2 = deform(o["P"], ps.fid, angle, seed=29, r=self.r)
             bk = ref64.Becker(ps.h, Q, ps.fid, ps.mass, young, poisson, nonlinear, rest=ref64.contacts(P2, P2, ps.h, same(ps.fid), same=True))
         for name, ang, seed in (("el_deformed_", angle, 29), ("el_warm_", 25.0, 31)):
-            P = deform(o["P"], ps.fid, ang, seed=seed)
+            P = deform(o["P"], ps.fid, ang, seed=seed, r=self.r)
             for k, f in enumerate(fh):
                 w.write_fluid(f, positions=P[ps.fid == k])
             w.step(self.dt, ZERO_G)
