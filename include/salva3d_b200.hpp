@@ -111,6 +111,14 @@ struct He2014SurfaceTension : NonPressureForce {  // he2014_surface_tension.rs:1
         return d;
     }
 };
+struct VorticityConfinement : NonPressureForce {  // no reference counterpart: include/sph.h SPH_FORCE_VORTICITY_CONFINEMENT
+    Real eps;  // > 0 and finite, in m/s
+    explicit VorticityConfinement(Real eps_) : eps(eps_) {}
+    sph_force_desc descriptor() const override {
+        sph_force_desc d{SPH_FORCE_VORTICITY_CONFINEMENT, {eps}};
+        return d;
+    }
+};
 struct WCSPHSurfaceTension : NonPressureForce {  // wcsph_surface_tension.rs:15-27 (boundary coefficient must be 0, see sph.h)
     Real fluid_tension_coefficient, boundary_tension_coefficient;
     WCSPHSurfaceTension(Real fluid_tension_coefficient_, Real boundary_tension_coefficient_)

@@ -64,9 +64,22 @@ enum { SPH_FORCE_XSPH_VISCOSITY = 0,        /* p[0]=fluid coeff, p[1]=boundary c
                                                reference's boundary loop walks the FLUID contact list and indexes
                                                boundaries with it, wcsph_surface_tension.rs:66-83)
                                                wcsph_surface_tension.rs:21-27 */
-       SPH_FORCE_DFSPH_VISCOSITY = 6        /* p[0]=viscosity coeff in [0,1], p[1]=min_viscosity_iter (1),
+       SPH_FORCE_DFSPH_VISCOSITY = 6,       /* p[0]=viscosity coeff in [0,1], p[1]=min_viscosity_iter (1),
                                                p[2]=max_viscosity_iter (50), p[3]=max_viscosity_error (0.01)
-                                               dfsph_viscosity.rs:86-124 */ };
+                                               dfsph_viscosity.rs:86-124 */
+       SPH_FORCE_VORTICITY_CONFINEMENT = 7  /* p[0]=eps > 0 and finite, in m/s; p[1..7] unused.  No reference counterpart
+                                               (Fedkiw, Stam & Jensen 2001; Macklin & Mueller 2013 section 6; DESIGN.md
+                                               section 18).  For a particle i of the force's fluid f, with sums over i's
+                                               fluid contacts j of fluid f (self included, contributing 0; boundaries
+                                               contribute nothing and receive no reaction), V_j = m_j / rho_j of this
+                                               step's densities and grad W_ij the solver's contact gradient at x_i - x_j,
+                                               over the positions, velocities and densities the other forces read:
+                                                 omega_i = sum_j V_j grad W_ij x (v_j - v_i)
+                                                 eta_i   = sum_j V_j (|omega_j| - |omega_i|) grad W_ij
+                                                 N_i     = eta_i / |eta_i| if |eta_i| > 0, else 0
+                                                 a_i    += eps (N_i x omega_i)
+                                               Refused (SPH_ERR_INVALID) for a NaN, infinite or non-positive eps and in
+                                               slab-decomposed worlds. */ };
 
 /* Kernel type parameters of the solver, DFSPHSolver<KernelDensity, KernelGradient> dfsph_solver.rs:17-20 /
  * IISPHSolver<..> iisph_solver.rs:17-20: contact.weight uses the density kernel, contact.gradient the gradient kernel
@@ -171,8 +184,11 @@ enum { SPH_DBG_DENSITY = 0,            /* densities            dfsph_solver.rs:4
        SPH_DBG_DIFFUSE_WAVE_CREST = 22,  /* I_wc before clamping (0 where v^ . n < 0.6) */
        SPH_DBG_DIFFUSE_KINETIC = 23,     /* E_k before clamping */
        SPH_DBG_DIFFUSE_COUNT = 24,       /* n_d, the particles it asked to emit, as float */
-       SPH_DBG_FLUID_LIST_BITS = 25      /* the width in bits (16 or 32) of the fluid list entries the last neighbour search
-                                          * stored, the same for every particle (DESIGN.md section 4a.18) */ };
+       SPH_DBG_FLUID_LIST_BITS = 25,     /* the width in bits (16 or 32) of the fluid list entries the last neighbour search
+                                          * stored, the same for every particle (DESIGN.md section 4a.18) */
+       /* Plugin scratch of the fluid's last SPH_FORCE_VORTICITY_CONFINEMENT, under the rule of selectors 12-19 */
+       SPH_DBG_VORTICITY = 26,           /* omega (3) */
+       SPH_DBG_VORTICITY_ETA = 27        /* eta (3), the unnormalised gradient of |omega| */ };
 
 /* LiquidWorld::new  liquid_world.rs:39-57 */
 void       sph_world_desc_default(sph_world_desc* desc);

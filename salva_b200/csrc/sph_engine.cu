@@ -9,6 +9,7 @@
 
 #include <algorithm>
 #include <array>
+#include <cfloat>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -619,6 +620,7 @@ struct sph_world {
     ListState lists;
     VStarRecords vstar;
     DBuf<float> he_colors, he_gradc;  // He2014 colours / squared colour-gradient norms (he2014_surface_tension.rs:16-17)
+    DBuf<float4> vort_omega, vort_eta;  // vorticity confinement: omega with |omega| in .w, eta with |eta| in .w
     DBuf<uint32_t> q_out, q_count;     // particles_intersecting_aabb results
     DBuf<float> map_pos, map_vel;      // sph_fluid_map_positions / _velocities: ORIGINAL-order device views
     bool in_coupling = false;          // inside CouplingManager::update_boundaries: the grid holds fluids only (liquid_world.rs:90-103)
@@ -1631,6 +1633,13 @@ sph_status phase_forces(sph_world* w, uint32_t fold) {
                 case SPH_FORCE_DFSPH_VISCOSITY:
                     TRY(viscosity_solve(w, (uint32_t)f, fr));
                     break;
+                case SPH_FORCE_VORTICITY_CONFINEMENT:
+                    CU(w->vort_omega.ensure(std::max(w->Ntot, w->N)));
+                    CU(w->vort_eta.ensure(std::max(w->Ntot, w->N)));
+                    DISPATCH1(k_vorticity_omega, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->dens.p, w->vort_omega.p, (uint32_t)f);
+                    DISPATCH1(k_vorticity_force, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->dens.p, w->vort_omega.p, w->vort_eta.p, w->acc.p,
+                              (uint32_t)f, p[0]);
+                    break;
                 case SPH_FORCE_WCSPH_TENSION:
                     if (p[0] != 0.f) DISPATCH1(k_wcsph_force, multi, N, PASS_T, w->pos[c].p, w->vel[c].p, L, w->acc.p, (uint32_t)f, p[0]);
                     break;
@@ -2010,13 +2019,19 @@ sph_status sph_fluid_push_force(sph_world* w, uint32_t fluid_h, const sph_force_
     if (!w || !force) return SPH_ERR_INVALID;
     std::lock_guard<std::recursive_mutex> lock(g_mutex);
     FLUID_OR_FAIL(fluid, fluid_h)
-    if (force->kind < 0 || force->kind > SPH_FORCE_DFSPH_VISCOSITY) return w->fail(SPH_ERR_INVALID, "unknown force kind %d", force->kind);
+    if (force->kind < 0 || force->kind > SPH_FORCE_VORTICITY_CONFINEMENT) return w->fail(SPH_ERR_INVALID, "unknown force kind %d", force->kind);
     if (force->kind == SPH_FORCE_WCSPH_TENSION && force->p[1] != 0.f)
         return w->fail(SPH_ERR_INVALID,
                        "WCSPHSurfaceTension: boundary coefficient must be 0 (the reference's boundary loop indexes boundaries with fluid "
                        "contacts, wcsph_surface_tension.rs:66-83)");
     if (force->kind == SPH_FORCE_DFSPH_VISCOSITY && !(force->p[0] >= 0.f && force->p[0] <= 1.f))
         return w->fail(SPH_ERR_INVALID, "The viscosity coefficient must be between 0.0 and 1.0. (dfsph_viscosity.rs:106-110)");
+    if (force->kind == SPH_FORCE_VORTICITY_CONFINEMENT) {
+        if (!(force->p[0] > 0.f && force->p[0] <= FLT_MAX))
+            return w->fail(SPH_ERR_INVALID, "vorticity confinement: eps must be finite and > 0 (got %g)", (double)force->p[0]);
+        if (w->desc.slab_count > 1 || w->slab.active)
+            return w->fail(SPH_ERR_INVALID, "vorticity confinement is not supported in slab-decomposed worlds");
+    }
     ForceRec fr;
     fr.d = *force;
     w->fluids[fluid].forces.push_back(std::move(fr));
@@ -2331,6 +2346,14 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         if (!pf || w->staged || !pf->solved || (el && (!pf->elastic || pf->elastic->n != f.n)))
             return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs a force of kind %d solved with the fluid's current particles", what, kind);
     }
+    if (what == SPH_DBG_VORTICITY || what == SPH_DBG_VORTICITY_ETA) {  // plugin scratch, under the rule of selectors 12-19
+        width = 3;
+        for (const ForceRec& fr : f.forces)
+            if (fr.d.kind == SPH_FORCE_VORTICITY_CONFINEMENT) pf = &fr;
+        if (!pf || w->staged || !pf->solved)
+            return w->fail(SPH_ERR_INVALID, "sph_debug_read: selector %d needs a force of kind %d solved with the fluid's current particles", what,
+                           (int)SPH_FORCE_VORTICITY_CONFINEMENT);
+    }
     if (f.n == 0) return SPH_OK;
     if (w->staged) {
         // the carried state is on the host between an edit and the next step; the step's scratch reads as zero until then
@@ -2366,6 +2389,8 @@ sph_status sph_debug_read(sph_world* w, uint32_t fluid_h, int what, float* out, 
         case SPH_DBG_IISPH_AII: return read(Rows<1>{w->iisph.aii.p});
         case SPH_DBG_HE2014_COLOR: return read(Rows<1>{w->he_colors.p});
         case SPH_DBG_HE2014_GRADC: return read(Rows<1>{w->he_gradc.p});
+        case SPH_DBG_VORTICITY: return read(Xyz{w->vort_omega.p});
+        case SPH_DBG_VORTICITY_ETA: return read(Xyz{w->vort_eta.p});
         case SPH_DBG_VELOCITY_CHANGE: return read(Xyz{w->vc[c].p});
         case SPH_DBG_ACCELERATION: return read(Xyz{w->acc.p});
         case SPH_DBG_IISPH_DII: return read(Xyz{w->iisph.dii.p});

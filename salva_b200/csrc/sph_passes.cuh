@@ -790,6 +790,66 @@ k_he2014_force(const float4* __restrict__ pos, const float4* __restrict__ vel, c
     acc[i] = a;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Vorticity confinement (include/sph.h SPH_FORCE_VORTICITY_CONFINEMENT, DESIGN.md section 18): vorticity -> its gradient
+// direction -> a_i += eps (N_i x omega_i).  Neighbours of the force's fluid only; boundaries take no part.
+// ------------------------------------------------------------------------------------------------
+// pass 1: omega_i = sum_j V_j grad W_ij x (v_j - v_i), written with |omega_i| in .w so that pass 2 gathers one word per neighbour
+template <bool MULTI>
+__global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)
+k_vorticity_omega(const float4* __restrict__ pos, const float4* __restrict__ vel, Lists L, const float* __restrict__ dens,
+                  float4* __restrict__ omega, uint32_t which) {
+    SPH_OWNED_INDEX(i)
+    const float4 vi = vel[i];
+    if (MULTI && fid_of(vi) != which) return;
+    float4 pi = pos[i];
+    float wx = 0.f, wy = 0.f, wz = 0.f;
+    for_fluid_grads_pos(
+        i, pi, L, pos, [&](uint32_t j) { return VelRho{__ldg(&vel[j]), __ldg(&dens[j])}; },
+        [&](uint32_t, const Pair& p, const float4& pj, const VelRho& a) {
+            if (MULTI && fid_of(a.v) != which) return;
+            const float c = p.g * (pj.w / a.rho);  // grad W_ij = g x_ij, V_j = m_j / rho_j
+            const float ux = a.v.x - vi.x, uy = a.v.y - vi.y, uz = a.v.z - vi.z;
+            wx = fmaf(c, p.dy * uz - p.dz * uy, wx);
+            wy = fmaf(c, p.dz * ux - p.dx * uz, wy);
+            wz = fmaf(c, p.dx * uy - p.dy * ux, wz);
+        });
+    omega[i] = make_float4(wx, wy, wz, sqrtf((wx * wx + wy * wy) + wz * wz));
+}
+
+struct FidRhoW {
+    uint32_t fid;
+    float rho, w;
+};
+// pass 2: eta_i = sum_j V_j (|omega_j| - |omega_i|) grad W_ij, N_i = eta_i / |eta_i| (0 where |eta_i| = 0), a_i += eps N_i x omega_i
+template <bool MULTI>
+__global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)
+k_vorticity_force(const float4* __restrict__ pos, const float4* __restrict__ vel, Lists L, const float* __restrict__ dens,
+                  const float4* __restrict__ omega, float4* __restrict__ eta, float4* __restrict__ acc, uint32_t which, float eps) {
+    SPH_OWNED_INDEX(i)
+    if (MULTI && fid_of(vel[i]) != which) return;
+    float4 pi = pos[i];
+    const float4 oi = omega[i];
+    float ex = 0.f, ey = 0.f, ez = 0.f;
+    for_fluid_grads_pos(
+        i, pi, L, pos, [&](uint32_t j) { return FidRhoW{MULTI ? fid_of(__ldg(&vel[j])) : 0u, __ldg(&dens[j]), __ldg(&omega[j].w)}; },
+        [&](uint32_t, const Pair& p, const float4& pj, const FidRhoW& a) {
+            if (MULTI && a.fid != which) return;
+            const float c = p.g * (pj.w / a.rho) * (a.w - oi.w);
+            ex = fmaf(c, p.dx, ex); ey = fmaf(c, p.dy, ey); ez = fmaf(c, p.dz, ez);
+        });
+    const float en = sqrtf((ex * ex + ey * ey) + ez * ez);
+    eta[i] = make_float4(ex, ey, ez, en);
+    if (en > 0.f) {
+        const float nx = ex / en, ny = ey / en, nz = ez / en;
+        float4 a = acc[i];
+        a.x += eps * (ny * oi.z - nz * oi.y);
+        a.y += eps * (nz * oi.x - nx * oi.z);
+        a.z += eps * (nx * oi.y - ny * oi.x);
+        acc[i] = a;
+    }
+}
+
 // WCSPHSurfaceTension fluid term (surface_tension/wcsph_surface_tension.rs:45-63): a_i -= k W_ij m_j / m_i x_ij
 template <bool MULTI>
 __global__ void __launch_bounds__(PASS_T, SPH_FORCE_MINB)

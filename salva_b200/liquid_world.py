@@ -21,9 +21,9 @@ DBG = dict(density=0, alpha=1, divergence=2, predicted_density=3, velocity_chang
            num_boundary_contacts=6, pressure=7, acceleration=8, dii=9, aii=10, dij_pjl=11, he2014_color=12, he2014_gradc=13,
            visc_beta=14, visc_target=15, el_volume0=16, el_rotation=17, el_grad_tr=18, el_stress=19, diffuse_normal=20,
            diffuse_trapped_air=21, diffuse_wave_crest=22, diffuse_kinetic=23, diffuse_count=24,
-           fluid_list_bits=25)
+           fluid_list_bits=25, vorticity=26, vorticity_eta=27)
 # floats per particle of the selectors that are not scalars (include/sph.h)
-WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6, 20: 3}
+WIDTH = {4: 3, 8: 3, 9: 3, 11: 3, 14: 36, 15: 6, 17: 9, 18: 9, 19: 6, 20: 3, 26: 3, 27: 3}
 DIFFUSE_KINDS = ("spray", "foam", "bubble")  # SPH_DIFFUSE_SPRAY / _FOAM / _BUBBLE
 
 
@@ -147,6 +147,15 @@ class He2014SurfaceTension:
 
     def __init__(self, fluid_tension_coefficient, boundary_tension_coefficient):
         self.params = [fluid_tension_coefficient, boundary_tension_coefficient]
+
+
+class VorticityConfinement:
+    """Vorticity confinement, a_i += eps (N_i x omega_i) with eps > 0 in m/s (include/sph.h SPH_FORCE_VORTICITY_CONFINEMENT,
+    DESIGN.md section 18); no reference counterpart"""
+    kind = 7
+
+    def __init__(self, eps):
+        self.params = [eps]
 
 
 class WCSPHSurfaceTension:

@@ -16,7 +16,7 @@ F32 = np.float32
 GRAVITY = (0.0, -9.81, 0.0)
 
 # force kinds (include/sph.h SPH_FORCE_*)
-XSPH, ARTIFICIAL, AKINCI2013, BECKER2009, HE2014, WCSPH, DFSPH_VISCOSITY = 0, 1, 2, 3, 4, 5, 6
+XSPH, ARTIFICIAL, AKINCI2013, BECKER2009, HE2014, WCSPH, DFSPH_VISCOSITY, VORTICITY = 0, 1, 2, 3, 4, 5, 6, 7
 DFSPH, IISPH = 0, 1
 
 
@@ -53,6 +53,11 @@ def wcsph_surface_tension(fluid_tension, boundary_tension=0.0):
 def dfsph_viscosity(viscosity_coefficient, min_viscosity_iter=1, max_viscosity_iter=50, max_viscosity_error=0.01):
     """DFSPHViscosity::new(coefficient) + public tunables  dfsph_viscosity.rs:86-124"""
     return (DFSPH_VISCOSITY, [viscosity_coefficient, float(min_viscosity_iter), float(max_viscosity_iter), max_viscosity_error])
+
+
+def vorticity_confinement(eps):
+    """Vorticity confinement with strength eps > 0 in m/s (include/sph.h SPH_FORCE_VORTICITY_CONFINEMENT; no reference counterpart)"""
+    return (VORTICITY, [eps])
 
 
 def cube_fluid(ni, nj, nk, particle_rad):
